@@ -147,11 +147,11 @@ SELFTEST_LIB_PATH = os.path.join(HERE, "libg4d_selftest.so")
 
 
 def load_selftest():
-    """The tcgen05 building-block self test lives in its own tiny library (tests / tools only; not in libg4d.so)."""
+    """The wgmma building-block self test lives in its own tiny library (tests only; not in libg4d.so)."""
     if not os.path.isfile(SELFTEST_LIB_PATH):
         raise G4DError("libg4d_selftest.so is not built (run __graft_entry__.build())")
     lib = C.CDLL(SELFTEST_LIB_PATH)
-    lib.g4d_selftest_umma.argtypes = [C.POINTER(C.c_int), fp, fp, fp, C.c_void_p]
+    lib.g4d_selftest_wgmma.argtypes = [C.POINTER(C.c_int), fp, fp, fp, C.c_void_p]
     return lib
 
 

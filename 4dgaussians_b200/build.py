@@ -1,9 +1,9 @@
-"""Build recipe for libg4d.so (hand-written sm_100a kernels behind the C-ABI of include/g4d.h).
+"""Build recipe for libg4d.so (hand-written sm_90a kernels behind the C-ABI of include/g4d.h).
 
 In-tree build with plain nvcc (no torch dependency): the .so travels to the GPU box with the snapshot.
-``g4d_geom.cu``, ``g4d_deform_tc.cu`` and ``g4d_deform_f16.cu`` -- the translation units that contain the projection maths
-(and ``g4d_knn.cu``: exact distances) -- are compiled with -fmad=false (bit-exact index stages, see g4d_math.cuh); the others use the default FMA contraction.  The tcgen05
-building-block self test (``g4d_tc_selftest.cu``) goes into its own ``libg4d_selftest.so`` (tests / tools only).
+``g4d_geom.cu`` and ``g4d_deform_tc.cu`` -- the translation units that contain the projection maths (and ``g4d_knn.cu``:
+exact distances) -- are compiled with -fmad=false (bit-exact index stages, see g4d_math.cuh); the others use the default FMA
+contraction.  The wgmma building-block self test (``g4d_tc_selftest.cu``) goes into its own ``libg4d_selftest.so`` (tests only).
 """
 from __future__ import annotations
 
@@ -16,10 +16,10 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libg4d.so")
-SELFTEST_OUT = os.path.join(HERE, "libg4d_selftest.so")     # tcgen05 building-block self test: tests / tools only
+SELFTEST_OUT = os.path.join(HERE, "libg4d_selftest.so")     # wgmma building-block self test: tests only
 OBJ = os.path.join(HERE, "build")
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "--expt-extended-lambda",
           "-Xptxas", "-v"]
 UNITS = {
@@ -32,7 +32,6 @@ UNITS = {
     "g4d_backward.cu": [],
     "g4d_api.cu": [],
     "g4d_deform_tc.cu": ["-fmad=false"],
-    "g4d_deform_f16.cu": ["-fmad=false"],
     "g4d_deform_tc_bwd.cu": [],
 }
 

@@ -5,7 +5,7 @@
 //   /root/reference/scene/deformation.py:67-83               hidden = Linear(F->Wd)(feat)      (no activation)
 //   /root/reference/scene/deformation.py:97-148              heads ReLU-Linear-ReLU-Linear, residual add
 //
-// B200 layout decisions (DESIGN.md §3):
+// Layout decisions (DESIGN.md §3):
 //   * planes are channel-last [H][W][C] so one bilinear tap is one contiguous 64/128-byte line (L2 resident);
 //   * the three time planes are collapsed once per view to 1-D rows (every Gaussian shares t), halving taps;
 //   * a CTA of 256 threads owns TG Gaussians; activations live in shared memory row-major [TG][K+4];

@@ -52,12 +52,12 @@ struct DevBuf {
 
 struct G4DWorkspace {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     int sync_mode = 1;
     int64_t min_capacity = 0;
     int tight_cull = 0;
     int stage_timing = 0;
-    int tensor_cores = 2;      // 0: FP32 FFMA kernels, 1: tcgen05 3xTF32, 2 (default): tcgen05 FP16x2, two tiles in flight
+    int tensor_cores = 2;      // 0: FP32 FFMA kernels, 1: wgmma 3xTF32, 2 (default): wgmma FP16x2
     int warp_cull = 1;
     int keep_deformed = 0;
     DevBuf tc_packed;
@@ -221,7 +221,7 @@ int refresh_packed(G4DWorkspace* ws, const G4DDeformParams* p, cudaStream_t st) 
 }
 
 bool forward_on_tensor_cores(const G4DWorkspace* ws, const DeformDesc& d) {
-    return ws->tensor_cores == 2 ? f16_deform_supported(d) : (ws->tensor_cores == 1 && tc_deform_supported(d));
+    return ws->tensor_cores != 0 && tc_deform_supported(d, ws->tensor_cores);
 }
 
 // tensor-core weight images, same caching rule as refresh_packed
@@ -230,13 +230,13 @@ int refresh_tc(G4DWorkspace* ws, const G4DDeformParams* p, cudaStream_t st) {
     ws->tcw.status = ws->h_pinned + 8;
     if (arith == 2 && ws->h_pinned[8]) {
         ws->h_pinned[8] = 0;
+        ws->tc_version = ~0ull;      // re-pack (and re-check) the weights on the next call: they may be the out-of-range values
         return fail(G4D_ERR_OVERFLOW, "an earlier FP16x2 tensor-core launch met a value outside the f16 operand range (activation >= 8188, "
                                       "feature >= 1023 or weight >= 255): its results were saturated; set G4D_OPT_TENSOR_CORES = 1 (3xTF32)");
     }
     if (ws->tc_version == p->version && ws->tc_key == (const void*)p->w0 && ws->tc_packed.p && ws->tcw.arith == arith) return G4D_OK;
     G4D_CUDA(ws->tc_packed.ensure(tc_packed_floats(*p) * 4));
-    if (arith == 2) G4D_CUDA(launch_f16_pack_weights(*p, ws->tc_packed.as<float>(), &ws->tcw, st));
-    else G4D_CUDA(launch_tc_pack_weights(*p, ws->tc_packed.as<float>(), &ws->tcw, st));
+    G4D_CUDA(launch_tc_pack_weights(*p, arith, ws->tc_packed.as<float>(), &ws->tcw, st));
     ws->tcw.arith = arith;
     ws->tc_version = p->version;
     ws->tc_key = (const void*)p->w0;
@@ -257,12 +257,11 @@ int deform_backward_dispatch(G4DWorkspace* ws, const DeformDesc& d, const G4DDef
                              float time, int64_t n, const float* xyz, const float* const go[G4D_NUM_HEADS],
                              float* const gi[G4D_NUM_HEADS], const uint32_t* relu_bits, const float* saved_feat, cudaStream_t st) {
     int rc;
-    if (ws->tensor_cores && tc_deform_supported(d)) {
+    if (ws->tensor_cores && tc_backward_supported(d)) {
         if ((rc = refresh_tc_bwd(ws, prm, st)) != G4D_OK) return rc;
-        if (ws->tc_debug) G4D_CUDA(ws->tc_dbg.ensure((size_t)ws->sm_count * 12 * 8));
         G4D_CUDA(ws->scratch.ensure(tc_deform_backward_scratch_bytes(d, n)));
-        G4D_CUDA(launch_deform_backward_tc(d, *prm, *grads, ws->tcbw, time, n, xyz, go, gi, relu_bits, saved_feat, ws->tc_debug ? ws->tc_dbg.as<long long>() : nullptr,
-                                           ws->scratch.as<uint8_t>(), ws->sm_count, st));
+        G4D_CUDA(launch_deform_backward_tc(d, *prm, *grads, ws->tcbw, time, n, xyz, go, gi, relu_bits, saved_feat, ws->scratch.as<uint8_t>(),
+                                           ws->sm_count, st));
         return G4D_OK;
     }
     if ((rc = refresh_packed(ws, prm, st)) != G4D_OK) return rc;

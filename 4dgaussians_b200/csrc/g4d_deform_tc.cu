@@ -1,71 +1,81 @@
 // g4d_deform_tc.cu -- tensor-core version of the fused deform + activate + project forward (net_width 128).
 //
-// The deformation MLP (scene/deformation.py:67-148: 93.6 kMAC per Gaussian at the DyNeRF config) runs on the 5th-gen
-// tensor cores with hand-written tcgen05 PTX:
-//   * a CTA owns a tile of 128 Gaussians = the 128 TMEM lanes; every activation matrix lives in TMEM and is the
-//     A operand of the next GEMM (tcgen05.mma A-from-TMEM), so activations never touch shared memory or HBM;
-//   * weights are the B operand: pre-packed once per parameter version into the canonical K-major smem image
-//     (hi | lo TF32 parts) and streamed head by head with TMA bulk copies + mbarriers;
-//   * fp32 accuracy through 3xTF32 (lo*hi + hi*lo + hi*hi, fp32 accumulate in TMEM): measured error below a plain
-//     fp32 SGEMM's (DESIGN.md §4), which the 1e-4 image tolerance needs -- single-pass TF32 is 1000x worse;
-//   * epilogues (bias, ReLU, sign bits for the backward, hi/lo split) are tcgen05.ld -> registers -> tcgen05.st, one
-//     thread per TMEM lane, two warps per lane quadrant splitting the hidden columns;
-//   * the HexPlane gather runs BEFORE this kernel at full occupancy (deform_features_kernel, feat [N][F] stays in L2):
-//     inside a 1-CTA/SM persistent kernel four gather warps were latency-bound and slowed the epilogue warps;
-//   * the tile's 128 result rows stay in registers of their owner threads, which finish the Gaussian
-//     (activations, EWA projection, SH colour) exactly like the SIMT path (geom_finish.cuh).
+// The deformation MLP (scene/deformation.py:67-148: 93.6 kMAC per Gaussian at the DyNeRF config) runs on the Hopper tensor
+// cores with hand-written wgmma PTX (tc_wgmma.cuh), in one of two arithmetics (G4D_OPT_TENSOR_CORES):
+//   2 (default) FP16x2: x = hi + lo with hi = rn_f16(s x), lo = rn_f16(s x - hi), s a fixed power of two per operand class
+//     (features 2^6, activations 2^3, weights 2^8; undone exactly by the epilogue's FMA).  |x - (hi + lo)/s| <= max(2^-22 |x|,
+//     2^-25 / s): the 3xTF32 relative error, with an absolute floor far below the fp32 accumulation noise of a K = 128 dot
+//     product.  s |x| must stay below 65504 (activations < 8188, features < 1023, weights < 255): conversions saturate and the
+//     kernel raises a flag in host-mapped memory that the next call reports (G4D_ERR_OVERFLOW).
+//   1 3xTF32: hi = rna_tf32(x), lo = rna_tf32(x - hi), no range limit.
+// Both form the three products lo*hi + hi*lo + hi*hi with fp32 accumulation: fp32-level accuracy (single-pass TF32 or F16 is
+// ~1000x worse than the 1e-4 image tolerance allows).
 //
-// TMEM map (512 columns): [0,128) A1 hi, [128,256) A1 lo, [256,384) D0, [384,512) D1 = X.
-//   D0 / D1: the layer-1 accumulators of consecutive heads ALTERNATE between the two, so that the GEMM of head k+1 runs on
-//            the tensor pipe while the 256 epilogue threads drain head k (the SH head always gets D0; its layer-2 output D2
-//            reuses D0[0,48));
-//   X (= D1): feature operand of layer 0 (hi [384,384+F), lo [448,448+F)) at the start of a tile, the SH head's hidden half
-//            (hi [384,448), lo [448,512)) at its end -- both at times when no head GEMM owns D1.
-// W1 streaming: the 128 KB (hi | lo) image of a head is split into two K-halves of 64 KB, each with its own "landed" and
-// "consumed" mbarrier: while the MMAs of K-half 1 of head k run, the TMA of K-half 0 of head k+1 is already in flight, so
-// the tensor pipe never waits for a whole-image copy (measured before: 960 cycles of exposed TMA wait per head + the whole
-// epilogue serialised behind every GEMM).
-// Roles (288 threads): warps 0-7 = the two epilogue groups (below); warp 8, one lane = the MMA issuer.  tcgen05.mma issue is
-// NOT free for the issuing thread -- it blocks while the pipe's queue is full (measured: an epilogue thread that also issued
-// the next head's 48 MMAs tripled every epilogue) -- so it gets its own warp and plain blocking waits on mbarriers:
-// features staged / A1 written / accumulator drained / hidden half written are signalled by the epilogue threads with
-// mbarrier.arrive, weights-landed by the TMA transaction count.  The TMA copies themselves are issued by thread 128, which
-// polls "K-half consumed" between the chunks of its own epilogue work (a copy is one non-blocking instruction).
-// Compiled with -fmad=false (it contains the projection, see g4d_math.cuh).
+// Structure: a warpgroup (128 threads) owns 64 Gaussians (the M = 64 of wgmma) and carries them through every layer:
+//   * the A operand of every GEMM lives in registers: the features are loaded straight into fragment layout, and each
+//     epilogue (bias, ReLU, sign bits for the backward, hi / lo split) turns the fp32 accumulator fragment into the next
+//     layer's A fragment in place (tc_wgmma.cuh) -- activations never touch shared memory or HBM;
+//   * weights are the B operand in shared memory: packed once per parameter version into the no-swizzle canonical K-major
+//     image (hi | lo), W0 and the SH head's W2 resident, W1 streamed head by head through a two-slot ring with TMA bulk
+//     copies and mbarriers (full: transaction count; empty: one arrival per consumer warp), one load ahead;
+//   * FP16x2 runs two warpgroups per CTA (128 Gaussians per W1 image load), 3xTF32 one (its A fragments take 128 registers);
+//   * layer 2 of the <= 4-wide heads runs in exact fp32 in the epilogue (each lane sums its 32 hidden units, a quad shuffle
+//     completes the row); the SH head's layer 2 (N = 48) is a fourth GEMM;
+//   * the per-Gaussian tail (residual adds, activations, EWA projection, SH colour -- geom_finish.cuh) runs after a hand-over
+//     through shared memory: threads 0-63 of the warpgroup finish the geometry, 64-127 the colour of one Gaussian each.
+// The HexPlane gather runs BEFORE this kernel at full occupancy (deform_features_kernel, feat [N][F] stays in L2).
+// Compiled with -fmad=false (it contains the projection, see g4d_math.cuh); the FMAs of the epilogues are explicit.
 #include "geom_finish.cuh"
-#include "tc_umma.cuh"
+#include "tc_wgmma.cuh"
 
 namespace g4d {
 
-constexpr int kW1Parts = 4;                       // K-quarters of a head's W1 image: 4 x (hi 16 KB | lo 16 KB)
-constexpr uint32_t kW1PartBytes = 2u * 128u * (128u / kW1Parts) * 4u;
-constexpr uint32_t kColA1Hi = 0, kColA1Lo = 128, kColD = 256, kColD1 = 384, kColX = 384, kColXLo = 448;
+template <int ARITH> struct TcArith;
+template <> struct TcArith<2> {               // FP16x2
+    static constexpr int KS = 16, ES = 2, EPC = 8, NWG = 2, PH = 1;
+    static constexpr float SF = 64.f, SA = 8.f, SW = 256.f;
+};
+template <> struct TcArith<1> {               // 3xTF32
+    static constexpr int KS = 8, ES = 4, EPC = 4, NWG = 1, PH = 4;
+    static constexpr float SF = 1.f, SA = 1.f, SW = 1.f;
+};
+constexpr float kF16Max = 65504.f;
+constexpr int kStageCols = 60;
+// shared memory of one block: the dynamic layout below + the static camera copy (padded to the 128 B alignment of the dynamic
+// array) must fit the 227 KB a block may use on sm_90
+constexpr uint32_t kMaxSmemPerBlock = 227u * 1024u;
+constexpr uint32_t kTcStaticSmem = (uint32_t)((sizeof(CameraDev) + 127) & ~(size_t)127);                 // per Gaussian: 11 geometry deltas | 48 SH deltas | pad
 
-struct TcSmem { uint32_t w1, w2, w0, bias, w2s, bars, acc, total; };
+struct TcSmem { uint32_t w1, w0, w2, bias, w2s, stage, bars, part_bytes, total; };
 
-inline TcSmem tc_smem_layout(int F, int max_kp16) {
+// part_bytes: one ring slot = one K-range of one head's W1 image, (hi | lo)
+inline TcSmem tc_smem_layout(int arith, int F, bool sh) {
+    const uint32_t es = arith == 2 ? 2u : 4u, ph = arith == 2 ? 1u : 4u, nwg = arith == 2 ? 2u : 1u;
     TcSmem s{};
     uint32_t off = 0;
     auto take = [&](uint32_t bytes) { uint32_t o = off; off += (bytes + 127u) & ~127u; return o; };
-    s.w1 = take(2u * 128 * 128 * 4);
-    s.w2 = take(max_kp16 == 48 ? 2u * 48 * 128 * 4 : 128u);
-    s.w0 = take(2u * 128 * F * 4);
+    s.part_bytes = 2u * 128u * (128u / ph) * es;
+    s.w1 = take(2u * s.part_bytes);
+    s.w0 = take(2u * 128u * F * es);
+    s.w2 = take(sh ? 2u * 48u * 128u * es : 128u);
     s.bias = take((128 + G4D_NUM_HEADS * 128 + 64) * 4);
     s.w2s = take(4 * 128 * 16);
-    s.bars = take(256);     // 18 mbarriers
-    s.acc = take(2 * 128 * 16);
+    s.stage = take(nwg * 64u * kStageCols * 4u);
+    s.bars = take(64);
     s.total = off;
     return s;
 }
 
 // ---- weight packing (once per parameter version) --------------------------------------------------------------
+// Every matrix [rows][K] (torch Linear layout) becomes (hi | lo) canonical K-major images, split into `parts` K-ranges
+// (part p = hi | lo of columns [p K/parts, (p+1) K/parts)); `kperm`: TF32 K order of an accumulator-fed A operand.
 struct TcPackDesc {
-    const float* src[1 + 2 * G4D_NUM_HEADS];
-    float* dst[1 + 2 * G4D_NUM_HEADS];
-    int rows_src[1 + 2 * G4D_NUM_HEADS], rows_dst[1 + 2 * G4D_NUM_HEADS], K[1 + 2 * G4D_NUM_HEADS];
-    int khalves[1 + 2 * G4D_NUM_HEADS];   // P > 0: image = P K-parts (hi_k0 | lo_k0 | hi_k1 | lo_k1 | ...), each canonical with K / P columns
-    int start[2 + 2 * G4D_NUM_HEADS];
-    int count;
+    const float* src[1 + G4D_NUM_HEADS + 1];
+    uint8_t* dst[1 + G4D_NUM_HEADS + 1];
+    int rows[1 + G4D_NUM_HEADS + 1], K[1 + G4D_NUM_HEADS + 1], parts[1 + G4D_NUM_HEADS + 1], kperm[1 + G4D_NUM_HEADS + 1];
+    int start[2 + G4D_NUM_HEADS + 1];
+    int count, arith;
+    uint32_t* status;                 // FP16x2: set to 1 when a scaled weight leaves the f16 range (TcWeights::status)
 };
 
 __global__ void tc_pack_weights_kernel(TcPackDesc p) {
@@ -74,74 +84,61 @@ __global__ void tc_pack_weights_kernel(TcPackDesc p) {
     int m = 0;
     while (i >= p.start[m + 1]) ++m;
     const int e = i - p.start[m];
-    const int K = p.K[m];
-    const uint32_t n = e / K, k = e % K;
-    const float v = (int)n < p.rows_src[m] ? __ldg(p.src[m] + n * K + k) : 0.f;
-    uint32_t hi, lo;
-    tc::tf32_split(v, hi, lo);
-    if (p.khalves[m]) {
-        const uint32_t Kh = K / p.khalves[m], j = k / Kh, blk = p.rows_dst[m] * Kh;   // words per (hi or lo, K-part) block
-        const uint32_t off = tc::canon_off(n, k - j * Kh, Kh) >> 2;
-        reinterpret_cast<uint32_t*>(p.dst[m])[(2 * j) * blk + off] = hi;
-        reinterpret_cast<uint32_t*>(p.dst[m])[(2 * j + 1) * blk + off] = lo;
-        return;
+    const uint32_t K = (uint32_t)p.K[m], n = (uint32_t)e / K, k = (uint32_t)e % K, rows = (uint32_t)p.rows[m];
+    const uint32_t kd = p.kperm[m] ? wg::tf32_kperm(k) : k;
+    const uint32_t KP = K / (uint32_t)p.parts[m], part = kd / KP, kk = kd % KP;
+    const float v = __ldg(p.src[m] + e);
+    if (p.arith == 2) {
+        uint32_t hi, lo;
+        if (fabsf(v * TcArith<2>::SW) >= kF16Max && p.status) *reinterpret_cast<volatile uint32_t*>(p.status) = 1u;   // saturates
+        wg::f16_split2(v * TcArith<2>::SW, 0.f, hi, lo);
+        uint8_t* base = p.dst[m] + (size_t)part * 2u * rows * KP * 2u + wg::img16_off(n, kk, KP);
+        *reinterpret_cast<uint16_t*>(base) = (uint16_t)hi;
+        *reinterpret_cast<uint16_t*>(base + rows * KP * 2u) = (uint16_t)lo;
+    } else {
+        uint32_t hi, lo;
+        wg::tf32_split(v, hi, lo);
+        uint8_t* base = p.dst[m] + (size_t)part * 2u * rows * KP * 4u + wg::img32_off(n, kk, KP);
+        *reinterpret_cast<uint32_t*>(base) = hi;
+        *reinterpret_cast<uint32_t*>(base + rows * KP * 4u) = lo;
     }
-    const uint32_t off = tc::canon_off(n, k, K) >> 2;
-    reinterpret_cast<uint32_t*>(p.dst[m])[off] = hi;
-    reinterpret_cast<uint32_t*>(p.dst[m])[p.rows_dst[m] * K + off] = lo;
 }
 
 size_t tc_packed_floats(const G4DDeformParams& prm) {
     const int F = prm.levels * prm.channels;
     size_t f = 2 * (size_t)128 * F;
-    for (int h = 0; h < G4D_NUM_HEADS; ++h) f += 2 * (size_t)128 * 128 + 2 * (size_t)(h == 4 ? 48 : 16) * 128;
+    for (int h = 0; h < G4D_NUM_HEADS; ++h) f += 2 * (size_t)128 * 128 + (h == 4 ? 2 * (size_t)48 * 128 : 0);
     return f + 64;
 }
 
-cudaError_t launch_tc_pack_weights(const G4DDeformParams& prm, float* blob, TcWeights* out, cudaStream_t st) {
+cudaError_t launch_tc_pack_weights(const G4DDeformParams& prm, int arith, float* blob, TcWeights* out, cudaStream_t st) {
     TcPackDesc p{};
+    p.arith = arith;
+    p.status = out->status;
     const int F = prm.levels * prm.channels;
+    const size_t es = arith == 2 ? 2 : 4;
     int m = 0, total = 0;
-    float* q = blob;
-    auto add = [&](const float* src, int rows_src, int rows_dst, int K, int khalves = 0) {
-        p.src[m] = src; p.dst[m] = q; p.rows_src[m] = rows_src; p.rows_dst[m] = rows_dst; p.K[m] = K; p.khalves[m] = khalves;
+    uint8_t* q = reinterpret_cast<uint8_t*>(blob);
+    auto add = [&](const float* src, int rows, int K, int parts, int kperm) {
+        p.src[m] = src; p.dst[m] = q; p.rows[m] = rows; p.K[m] = K; p.parts[m] = parts; p.kperm[m] = kperm && arith == 1;
         p.start[m] = total;
-        total += rows_dst * K; float* r = q; q += 2 * (size_t)rows_dst * K; ++m; return r;
+        total += rows * K;
+        uint8_t* r = q;
+        q += 2 * (size_t)rows * K * es;
+        ++m;
+        return reinterpret_cast<const float*>(r);
     };
-    out->w0 = add(prm.w0, 128, 128, F);
+    out->w0 = add(prm.w0, 128, F, 1, 0);
     for (int h = 0; h < G4D_NUM_HEADS; ++h) {
-        out->kp16[h] = h == 4 ? 48 : 16;
         out->w1[h] = nullptr; out->w2[h] = nullptr;
         if (!(prm.head_mask & (1 << h))) continue;
-        out->w1[h] = add(prm.w1[h], 128, 128, 128, kW1Parts);
-        out->w2[h] = add(prm.w2[h], head_out(h), out->kp16[h], 128);
+        out->w1[h] = add(prm.w1[h], 128, 128, arith == 2 ? TcArith<2>::PH : TcArith<1>::PH, 1);
+        if (h == 4) out->w2[h] = add(prm.w2[h], 48, 128, 1, 1);   // the small heads' layer 2 runs in fp32 from the caller's tensors
     }
     p.start[m] = total; p.count = m;
     tc_pack_weights_kernel<<<(total + 255) / 256, 256, 0, st>>>(p);
     return cudaGetLastError();
 }
-
-// ---- the kernel -------------------------------------------------------------------------------------------------
-// Thread groups (256 threads; thread 128+m and thread m both own TMEM lane m = Gaussian m of the tile):
-//   M = warps 4-7: MMA issue + TMA weight streaming (thread 128), hidden columns [64,128) of every epilogue, head outputs,
-//       activations + projection of the Gaussian.  (The hardware scheduler favours the higher warp ids of a sub-partition.)
-//   G = warps 0-3: stages the next tile's features into TMEM, hidden columns [0,64) of every epilogue (its partial layer-2
-//       sums of the small heads go to M through shared memory), and the SH colour of the current tile.
-// Hand-offs use named barriers (ids 1-4 and 6, 256 threads) + tcgen05 fences; the M group syncs internally on id 5.
-// Each MMA kind has its own mbarrier (layer 0 / layer 1 / layer-2 partials) so that a thread that only waits for some of
-// them can never fall a full phase behind.
-__device__ __forceinline__ void bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
-__device__ __forceinline__ void bar_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
-
-__device__ __forceinline__ int b2off_of(int mask, int h) {
-    int o = 0;
-    for (int i = 0; i < h; ++i)
-        if (mask & (1 << i)) o += head_out(i);
-    return o;
-}
-
-constexpr int kBarScratch = 3, kBarScratchFree = 4, kBarE = 6;   // named barriers between the two epilogue groups
-constexpr uint32_t kColScratch = kColA1Hi;   // p(3) + dsh(48) handed from M to G after the last head (A1 is dead then)
 
 // One channel vector (4 channels) of one level: product over the 6 planes of the bilinear samples.
 __device__ __forceinline__ float4 sample_vector(const DeformDesc* __restrict__ dp, int l, int v, int C4, float px, float py, float pz) {
@@ -178,527 +175,359 @@ __device__ __forceinline__ float4 sample_vector(const DeformDesc* __restrict__ d
     return prod;
 }
 
-template <int C, int L>
-__device__ __forceinline__ void sample_features_regs(const DeformDesc* d, const float pcs[3], float (&feat)[C * L]) {
-    constexpr int C4 = C / 4;
-#pragma unroll
-    for (int l = 0; l < L; ++l) {
-#pragma unroll
-        for (int v = 0; v < C4; ++v) {
-            const float4 prod = sample_vector(d, l, v, C4, pcs[0], pcs[1], pcs[2]);
-            feat[l * C + 4 * v + 0] = prod.x; feat[l * C + 4 * v + 1] = prod.y;
-            feat[l * C + 4 * v + 2] = prod.z; feat[l * C + 4 * v + 3] = prod.w;
-        }
+
+// ---- fragments ----------------------------------------------------------------------------------------------------------
+using wg::Frags;
+
+// two values of row g (x0, x1 = columns c, c + 1) and the same columns of row g + 8 (y0, y1), in accumulator block j,
+// -> the A fragment slots they occupy
+template <int ARITH, int NS>
+__device__ __forceinline__ void put_block(Frags<NS>& a, int j, float x0, float x1, float y0, float y1) {
+    if constexpr (ARITH == 2) {
+        const int s = j >> 1, o = (j & 1) * 2;
+        wg::f16_split2(x0, x1, a.hi[s][o], a.lo[s][o]);
+        wg::f16_split2(y0, y1, a.hi[s][o + 1], a.lo[s][o + 1]);
+    } else {
+        wg::tf32_split(x0, a.hi[j][0], a.lo[j][0]);
+        wg::tf32_split(y0, a.hi[j][1], a.lo[j][1]);
+        wg::tf32_split(x1, a.hi[j][2], a.lo[j][2]);
+        wg::tf32_split(y1, a.hi[j][3], a.lo[j][3]);
     }
 }
 
-// ReLU sign bits of one Gaussian for one layer (slot 0 = hidden, 1 + h = head h): [slot][N] x 128 bits
-__device__ __forceinline__ void store_relu_bits(uint32_t* base, int slot, int64_t n, int64_t gi, uint64_t lo, uint64_t hi) {
-    *reinterpret_cast<uint4*>(base + ((size_t)slot * (size_t)n + (size_t)gi) * 4) =
-        make_uint4((uint32_t)lo, (uint32_t)(lo >> 32), (uint32_t)hi, (uint32_t)(hi >> 32));
+// D[64 x N] = A * B^T, three products; B = (hi | lo) K-major image with `bcols` columns, K-slices [s0, s0 + NSP) of A
+// against the image's slices [0, NSP)
+template <int ARITH, int N, int NS, int NSP>
+__device__ __forceinline__ void gemm3(float (&d)[N / 2], const Frags<NS>& a, int s0, uint32_t b_hi, uint32_t b_lo, uint32_t bcols,
+                                      bool accumulate) {
+    using A = TcArith<ARITH>;
+    const uint64_t dh = wg::desc_kmajor(b_hi, bcols, A::EPC), dl = wg::desc_kmajor(b_lo, bcols, A::EPC);
+    wg::fence_regs(d);
+    wg::fence();
+#pragma unroll
+    for (int p = 0; p < 3; ++p) {
+#pragma unroll
+        for (int s = 0; s < NSP; ++s) {
+            const uint64_t bd = ((p == 1) ? dl : dh) + (uint64_t)(16 * s);      // + 256 bytes per slice
+            const uint32_t acc = (accumulate || p > 0 || s > 0) ? 1u : 0u;
+            if constexpr (ARITH == 2) wg::mma_f16_rs<N, 0>(d, p == 0 ? a.lo[s0 + s] : a.hi[s0 + s], bd, acc);
+            else wg::mma_tf32_rs<N>(d, p == 0 ? a.lo[s0 + s] : a.hi[s0 + s], bd, acc);
+        }
+    }
+    wg::commit();
+    wg::wait_all();
+    wg::fence_regs(d);
 }
 
-// one 64-bit half of a row's sign bits (word0 = 0 for hidden units 0..63, 2 for 64..127)
-__device__ __forceinline__ void store_relu_half(uint32_t* base, int slot, int64_t n, int64_t gi, int word0, uint32_t lo, uint32_t hi) {
-    *reinterpret_cast<uint2*>(base + ((size_t)slot * (size_t)n + (size_t)gi) * 4 + word0) = make_uint2(lo, hi);
+// bias + ReLU of a 64 x 128 accumulator -> next A operand; sign bits of rows g / g + 8 (4 words each, complete for every lane
+// of the quad); running maximum of the converted values
+template <int ARITH>
+__device__ __forceinline__ void relu_to_frags(const float (&d)[64], float inv, const float* __restrict__ bias, int t, Frags<128 / TcArith<ARITH>::KS>& a,
+                                              uint32_t (&b0)[4], uint32_t (&b1)[4], float& mx) {
+#pragma unroll
+    for (int w = 0; w < 4; ++w) { b0[w] = 0u; b1[w] = 0u; }
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+        const int c = 8 * j + 2 * t;
+        const float2 bb = *reinterpret_cast<const float2*>(bias + c);
+        const float x0 = fmaf(d[4 * j], inv, bb.x), x1 = fmaf(d[4 * j + 1], inv, bb.y);
+        const float y0 = fmaf(d[4 * j + 2], inv, bb.x), y1 = fmaf(d[4 * j + 3], inv, bb.y);
+        const int sh = 8 * (j & 3) + 2 * t;
+        b0[j >> 2] |= ((x0 > 0.f ? 1u : 0u) | (x1 > 0.f ? 2u : 0u)) << sh;
+        b1[j >> 2] |= ((y0 > 0.f ? 1u : 0u) | (y1 > 0.f ? 2u : 0u)) << sh;
+        const float r0 = fmaxf(x0, 0.f), r1 = fmaxf(x1, 0.f), r2 = fmaxf(y0, 0.f), r3 = fmaxf(y1, 0.f);
+        mx = fmaxf(mx, fmaxf(fmaxf(r0, r1), fmaxf(r2, r3)));
+        put_block<ARITH>(a, j, r0, r1, r2, r3);
+    }
+#pragma unroll
+    for (int w = 0; w < 4; ++w) {
+        b0[w] |= __shfl_xor_sync(0xffffffffu, b0[w], 1); b0[w] |= __shfl_xor_sync(0xffffffffu, b0[w], 2);
+        b1[w] |= __shfl_xor_sync(0xffffffffu, b1[w], 1); b1[w] |= __shfl_xor_sync(0xffffffffu, b1[w], 2);
+    }
 }
 
-// non-blocking probe of an mbarrier phase (mbar_wait spins on the blocking form)
-__device__ __forceinline__ bool mbar_test(void* bar, uint32_t parity) {
-    uint32_t done;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    return done != 0;
+// lane t of the quad stores word t of both rows' 128 sign bits: [slot][N][4 words], word w = hidden units [32w, 32w + 32)
+__device__ __forceinline__ void store_bits(uint32_t* base, int slot, int64_t n, int64_t g0, int64_t g1, int t, const uint32_t (&b0)[4],
+                                           const uint32_t (&b1)[4]) {
+    const uint32_t w0 = t == 0 ? b0[0] : t == 1 ? b0[1] : t == 2 ? b0[2] : b0[3];
+    const uint32_t w1 = t == 0 ? b1[0] : t == 1 ? b1[1] : t == 2 ? b1[2] : b1[3];
+    if (g0 < n) base[((size_t)slot * (size_t)n + (size_t)g0) * 4 + t] = w0;
+    if (g1 < n) base[((size_t)slot * (size_t)n + (size_t)g1) * 4 + t] = w1;
 }
 
 __device__ __forceinline__ void mbar_arrive(void* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+__device__ __forceinline__ void bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 
-constexpr int kTcThreads = 288;   // 8 epilogue warps + the MMA warp
-
-template <int MODE, int C, int L, bool SAVE>
-__global__ void __launch_bounds__(kTcThreads, 1)
-deform_tc_kernel(DeformDesc d, TcWeights tw, TcSmem Ls, const CameraDev* __restrict__ camp, float time_arg, int use_cam_time,
-                 int64_t n, DeformIO io) {
-    constexpr int F = C * L;
-    extern __shared__ __align__(1024) uint8_t smem[];
+template <int ARITH, int MODE, int C, int L, bool SAVE>
+__global__ void __launch_bounds__(TcArith<ARITH>::NWG * 128, 1)
+deform_tc_kernel(DeformDesc d, TcWeights tw, TcSmem Ls, const CameraDev* __restrict__ camp, int use_cam, int64_t n, DeformIO io) {
+    using A = TcArith<ARITH>;
+    constexpr int F = C * L, NS0 = F / A::KS, NS1 = 128 / A::KS, NSP = NS1 / A::PH, TM = 64 * A::NWG, NT = 128 * A::NWG;
+    static_assert(F % 16 == 0 && F <= 64, "feature width must be 32, 48 or 64");
+    constexpr float kInvL0 = A::SA / (A::SF * A::SW), kInvH = 1.f / (A::SA * A::SW), kInvHS = 1.f / A::SW;
+    extern __shared__ __align__(128) uint8_t smem[];   // (every operand image and barrier is placed at a multiple of 128 B)
     __shared__ CameraDev cam;
-    __shared__ DeformDesc sd;
-    __shared__ uint32_t tmem_base_s;
-    const int tid = threadIdx.x, warp = tid >> 5;
-    const int row = tid & 127;
-    for (int i = tid; i < (int)(sizeof(DeformDesc) / 4); i += kTcThreads)
-        reinterpret_cast<uint32_t*>(&sd)[i] = reinterpret_cast<const uint32_t*>(&d)[i];
-    // the hardware scheduler favours the higher warp ids of an SM sub-partition: the latency-critical M group takes them
-    const bool is_mma_warp = warp == 8;
-    const bool is_m = tid >= 128 && !is_mma_warp;
-    const bool tma_thread = tid == 128;
-    const int64_t ntiles = (n + 127) / 128;
-    if (MODE == 1 || use_cam_time) {
-        for (int i = tid; i < (int)(sizeof(CameraDev) / 4); i += kTcThreads)
-            reinterpret_cast<uint32_t*>(&cam)[i] = reinterpret_cast<const uint32_t*>(camp)[i];
-    }
-    float* sBias = reinterpret_cast<float*>(smem + Ls.bias);     // b0[128] | b1[5][128] | b2[64]
+    const int tid = threadIdx.x, wgi = tid >> 7, t128 = tid & 127, lane = tid & 31, g = lane >> 2, t = lane & 3;
+    const int r0 = ((t128 >> 5) << 4) + g, r1 = r0 + 8;          // rows of this lane inside the warpgroup's 64
+    float* sBias = reinterpret_cast<float*>(smem + Ls.bias);     // b0 * SA [128] | b1[5][128] (SH head * SA) | b2s[4][4] | b2sh[48]
     float4* sW2s = reinterpret_cast<float4*>(smem + Ls.w2s);     // [4 small heads][128 hidden]: (W2[0][j], W2[1][j], W2[2][j], W2[3][j])
+    float* stage = reinterpret_cast<float*>(smem + Ls.stage) + wgi * 64 * kStageCols;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Ls.bars);
-    // mbarriers: 0 w0 | 1-4 full[j] (W1 K-quarter j landed, tx count) | 5-8 hfree[j] (its MMAs retired) | 9,10 dfull[b] (head
-    // GEMM into D[b] complete) | 11 l0 | 12 l2 | 13 featready (128 G threads) | 14 a1ready (256) | 15,16 dfree[b] (256:
-    // accumulator drained by its epilogue) | 17 xready (256: SH hidden half written)
-    uint64_t *bar_w0 = bars, *bar_full = bars + 1, *bar_hfree = bars + 5, *bar_dfull = bars + 9, *bar_l0 = bars + 11, *bar_l2 = bars + 12;
-    uint64_t *bar_feat = bars + 13, *bar_a1 = bars + 14, *bar_dfree = bars + 15, *bar_x = bars + 17;
-    int b2off[G4D_NUM_HEADS];
-    {
-        int o = 0;
-#pragma unroll
-        for (int h = 0; h < G4D_NUM_HEADS; ++h) { b2off[h] = o; if (d.head_mask & (1 << h)) o += head_out(h); }
-    }
-    for (int i = tid; i < 128; i += kTcThreads) sBias[i] = __ldg(d.b0 + i);
+    uint64_t *bar_w0 = bars, *bar_full = bars + 1, *bar_empty = bars + 3;
+    for (int i = tid; i < 128; i += NT) sBias[i] = __ldg(d.b0 + i) * A::SA;
+    for (int i = tid; i < 64; i += NT) sBias[128 + G4D_NUM_HEADS * 128 + i] = 0.f;
     for (int h = 0; h < G4D_NUM_HEADS; ++h) {
         if (!(d.head_mask & (1 << h))) continue;
-        for (int i = tid; i < 128; i += kTcThreads) sBias[128 + h * 128 + i] = __ldg(d.b1[h] + i);
-        for (int i = tid; i < head_out(h); i += kTcThreads) sBias[128 + G4D_NUM_HEADS * 128 + b2off[h] + i] = __ldg(d.b2[h] + i);
+        for (int i = tid; i < 128; i += NT) sBias[128 + h * 128 + i] = __ldg(d.b1[h] + i) * (h == 4 ? A::SA : 1.f);
         if (h < 4) {
             const int ko = head_out(h);
-            for (int j = tid; j < 128; j += kTcThreads)
+            for (int j = tid; j < 128; j += NT)
                 sW2s[h * 128 + j] = make_float4(__ldg(d.w2[h] + j), ko > 1 ? __ldg(d.w2[h] + 128 + j) : 0.f,
                                                ko > 2 ? __ldg(d.w2[h] + 256 + j) : 0.f, ko > 3 ? __ldg(d.w2[h] + 384 + j) : 0.f);
         }
     }
-    if (warp == 0) tc::tmem_alloc(&tmem_base_s, tc::kTmemCols);
+    __syncthreads();      // (the zero fill of the b2 block above must land before the per-head values)
+    for (int h = 0; h < G4D_NUM_HEADS; ++h) {
+        if (!(d.head_mask & (1 << h))) continue;
+        for (int i = tid; i < head_out(h); i += NT) sBias[128 + G4D_NUM_HEADS * 128 + (h < 4 ? 4 * h : 16) + i] = __ldg(d.b2[h] + i);
+    }
     if (tid == 0) {
-        for (int i = 0; i < 13; ++i) mbar_init(bars + i, 1);
-        mbar_init(bar_feat, 128); mbar_init(bar_a1, 256); mbar_init(bar_dfree, 256); mbar_init(bar_dfree + 1, 256); mbar_init(bar_x, 256);
+        mbar_init(bar_w0, 1);
+        mbar_init(bar_full, 1); mbar_init(bar_full + 1, 1);
+        mbar_init(bar_empty, 4 * A::NWG); mbar_init(bar_empty + 1, 4 * A::NWG);
         fence_barrier_init();
     }
-    tc::fence_before_sync();
+    pdl_wait();           // from here on: the camera, the staged features
+    pdl_trigger();
+    if (use_cam) {
+        for (int i = tid; i < (int)(sizeof(CameraDev) / 4); i += NT)
+            reinterpret_cast<uint32_t*>(&cam)[i] = reinterpret_cast<const uint32_t*>(camp)[i];
+    }
     __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t tbase = __shfl_sync(0xffffffffu, tmem_base_s, 0);    // warp-uniform for the compiler (MMA operands are uniform registers)
-    const uint32_t lane_base = tbase + ((uint32_t)((warp & 3) * 32) << 16);
-    const uint32_t sW1 = tc::smem_addr(smem + Ls.w1), sW2 = tc::smem_addr(smem + Ls.w2), sW0 = tc::smem_addr(smem + Ls.w0);
+
     const bool hsh = d.head_mask & G4D_HEAD_SHS;
-
-    // ---- the W1 stream of this CTA: loads / GEMMs are numbered q = 0, 1, ... over (tile, active head) in program order,
-    //      each made of two K-halves j
-    const uint32_t m_heads = (uint32_t)__popc(d.head_mask & 31);
-    const uint32_t par0 = hsh ? ((m_heads - 1u) & 1u) : 0u;      // accumulator of head k of a tile = (k + par0) & 1: SH gets D0
-    const int64_t my_tiles = (int64_t)blockIdx.x < ntiles ? (ntiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
-    const uint32_t total_q = (uint32_t)my_tiles * m_heads;
-    // head id of the k-th head this CTA processes: the small heads in an order ROTATED by the CTA index (at any moment the
-    // 148 CTAs then stream four different W1 images instead of hammering the L2 slices of one), the SH head always last
-    uint32_t hseq_pack = 0;               // 3 bits per position
+    const int m_heads = __popc(d.head_mask & 31);
+    uint32_t hseq = 0;                         // head of position k (3 bits each): the small heads in order, the SH head last
     {
-        const int ns = __popc(d.head_mask & 15);
-        const int rot = ns ? (int)(blockIdx.x % (unsigned)ns) : 0;
-        int pos = 0;
-        for (int h = 0; h < 4; ++h) {
-            if (!(d.head_mask & (1 << h))) continue;
-            const int k = pos >= rot ? pos - rot : pos - rot + ns;      // active small head #pos runs at position k
-            hseq_pack |= (uint32_t)h << (3 * k);
-            ++pos;
-        }
-        if (hsh) hseq_pack |= 4u << (3 * ns);
+        int k = 0;
+        for (int h = 0; h < G4D_NUM_HEADS; ++h)
+            if (d.head_mask & (1 << h)) hseq |= (uint32_t)h << (3 * k++);
     }
-    auto head_at = [&](uint32_t k) { return (int)((hseq_pack >> (3u * k)) & 7u); };
-
-    // ================================================================================================================
-    // MMA warp: one lane issues every tcgen05.mma of the CTA, in order, with blocking waits
-    // ================================================================================================================
-    if (is_mma_warp) {
-        // the warp walks the loop converged, one elected lane issues (uniform-register operands, tc_umma.cuh)
-        const bool leader = tc::elect_one_sync();
-        {
-            mbar_wait(bar_w0, 0);
-            uint32_t used[2] = {0u, 0u}, seen[2] = {0u, 0u};       // GEMMs issued into / epilogues observed on D[b]
-            uint32_t ph_feat = 0, ph_a1 = 0, ph_x = 0, q = 0;
-            auto drain = [&](uint32_t b) {                          // every earlier user of D[b] has been read out
-                while (seen[b] < used[b]) { mbar_wait(bar_dfree + b, seen[b] & 1u); ++seen[b]; }
-            };
-            for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-                // ---- layer 0: D0 = feat * W0^T
-                mbar_wait(bar_feat, ph_feat); ph_feat ^= 1u;
-                drain(0); drain(1);
-                tc::fence_after_sync();
-                if (leader) {
-                    tc::gemm_3xtf32<F>(tbase + kColD, tbase + kColX, tbase + kColXLo, sW0, sW0 + 128u * F * 4, 128, F, 0, false);
-                    tc::umma_commit(bar_l0);
-                }
-                __syncwarp();
-                mbar_wait(bar_a1, ph_a1); ph_a1 ^= 1u;              // epilogue 0 has written A1 and drained D0
-                for (uint32_t k = 0; k < m_heads; ++k, ++q) {
-                    const uint32_t b = (k + par0) & 1u;
-                    drain(b);
-#pragma unroll 1
-                    for (uint32_t j = 0; j < (uint32_t)kW1Parts; ++j) {
-                        constexpr uint32_t KP = 128 / kW1Parts;
-                        mbar_wait(bar_full + j, q & 1u);
-                        tc::fence_after_sync();
-                        if (leader) {
-                            tc::gemm_3xtf32<(int)KP>(tbase + (b ? kColD1 : kColD), tbase + kColA1Hi + j * KP, tbase + kColA1Lo + j * KP,
-                                                     sW1 + j * kW1PartBytes, sW1 + j * kW1PartBytes + kW1PartBytes / 2, 128, KP, 0, j != 0);
-                            tc::umma_commit(bar_hfree + j);
-                        }
-                        __syncwarp();
-                    }
-                    if (leader) tc::umma_commit(bar_dfull + b);
-                    __syncwarp();
-                    ++used[b];
-                    if (hsh && k + 1 == m_heads) {
-                        // SH head: two layer-2 partials D2 (+)= a2_half * W2[:, 64hh : 64hh+64]^T (D2 = D0 columns [0, 48))
-                        for (int hh = 0; hh < 2; ++hh) {
-                            mbar_wait(bar_x, ph_x); ph_x ^= 1u;
-                            tc::fence_after_sync();
-                            if (leader) {
-                                tc::gemm_3xtf32<64>(tbase + kColD, tbase + kColX, tbase + kColXLo, sW2, sW2 + 48u * 128 * 4, 48, 128,
-                                                    (uint32_t)(hh * 16), hh == 1);
-                                tc::umma_commit(bar_l2);
-                            }
-                            __syncwarp();
-                        }
-                    }
-                }
-            }
-        }
-    } else {
-    // ================================================================================================================
-    // epilogue groups
-    // ================================================================================================================
-    // next W1 K-half copy (thread 128 only): its buffer must have been consumed by the previous GEMM; never blocks
-    uint32_t tq = 0, tj = 0, tk = 0;      // next copy: GEMM index, K-part, head position inside the tile
-    auto pump_tma = [&]() {
-        for (;;) {
-            if (tq >= total_q || (tq != 0 && !mbar_test(bar_hfree + tj, (tq - 1u) & 1u))) break;
-            const int h = head_at(tk);
-            mbar_expect_tx(bar_full + tj, kW1PartBytes);
-            tma_bulk_g2s(smem + Ls.w1 + tj * kW1PartBytes, tw.w1[h] + tj * (kW1PartBytes / 4u), kW1PartBytes, bar_full + tj);
-            if (++tj == (uint32_t)kW1Parts) { tj = 0; ++tq; if (++tk == m_heads) tk = 0; }
-        }
+    const int64_t ntiles = (n + TM - 1) / TM;
+    const int64_t my_tiles = (int64_t)blockIdx.x < ntiles ? (ntiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
+    const uint32_t per_tile = (uint32_t)(m_heads * A::PH), total_items = (uint32_t)my_tiles * per_tile;
+    // W1 ring: item u = (tile, head position, K-part) in consumption order, slot u & 1; thread 0 loads one item ahead
+    auto issue = [&](uint32_t u) {
+        const uint32_t s = u & 1u, r = u % per_tile;
+        if (u >= 2) mbar_wait(bar_empty + s, ((u >> 1) - 1u) & 1u);
+        const int h = (int)((hseq >> (3 * (r / A::PH))) & 7u);
+        mbar_expect_tx(bar_full + s, Ls.part_bytes);
+        tma_bulk_g2s(smem + Ls.w1 + s * Ls.part_bytes, reinterpret_cast<const uint8_t*>(tw.w1[h]) + (r % A::PH) * Ls.part_bytes,
+                     Ls.part_bytes, bar_full + s);
     };
-    // wait for an mbarrier phase; thread 128 keeps the weight stream moving meanwhile
-    auto wait_pumping = [&](uint64_t* bar, uint32_t parity) {
-        if (tma_thread) {
-            while (!mbar_test(bar, parity)) pump_tma();
-        } else {
-            mbar_wait(bar, parity);
-        }
-    };
-
-    // ---- resident operands: W0 and (when active) the SH head's W2 image; the first two W1 K-halves
-    if (tma_thread) {
-        const uint32_t w2b = hsh ? 2u * 48 * 128 * 4 : 0u;
-        mbar_expect_tx(bar_w0, 2u * 128 * F * 4 + w2b);
-        tma_bulk_g2s(smem + Ls.w0, tw.w0, 2u * 128 * F * 4, bar_w0);
+    if (tid == 0) {
+        const uint32_t w0b = 2u * 128u * F * A::ES, w2b = hsh ? 2u * 48u * 128u * A::ES : 0u;
+        mbar_expect_tx(bar_w0, w0b + w2b);
+        tma_bulk_g2s(smem + Ls.w0, tw.w0, w0b, bar_w0);
         if (hsh) tma_bulk_g2s(smem + Ls.w2, tw.w2[4], w2b, bar_w0);
-        pump_tma();
+        if (total_items) issue(0);
     }
-    uint32_t ph_l0 = 0, ph_l2 = 0, ph_d0 = 0, ph_d1 = 0;
-    // column chunks (16 hidden units each) of every epilogue are split between the two thread groups
-    const int ch_lo = is_m ? 4 : 0, ch_hi = is_m ? 8 : 4;        // full-width epilogues (8 chunks)
-    const int hc_lo = is_m ? 2 : 0, hc_hi = is_m ? 4 : 2;        // half-width epilogues of the SH head (4 chunks)
-    float4* sAcc = reinterpret_cast<float4*>(smem + Ls.acc);     // [2][128]: G group's partial layer-2 sums of a small head
+    __syncwarp();
+    mbar_wait(bar_w0, 0);
+    const uint32_t sW0 = wg::smem_addr(smem + Ls.w0), sW1 = wg::smem_addr(smem + Ls.w1), sW2 = wg::smem_addr(smem + Ls.w2);
+    const float* b2s = sBias + 128 + G4D_NUM_HEADS * 128;
+    float mx = 0.f;        // running maximum of every value converted to f16 (range check), in operand units
+    uint32_t u = 0;
+    const bool dbg = tw.dbg && tid == 0;      // G4D_OPT_TC_DEBUG: cycles of the whole kernel / spent waiting for W1 images
+    const long long t_start = dbg ? clock64() : 0;
+    long long t_wait = 0;
 
-    // features of a tile ([N][F] fp32, written by deform_features_kernel at full occupancy) -> A operand X (hi | lo).
-    // X (= D1) is free here: every GEMM that wrote or read it has been waited for by this thread.
-    auto stage_features = [&](int64_t tl) {
-        const int64_t gs = tl * 128 + row;
-        float feat[F];
-        if (gs < n) {
-            const float4* src = reinterpret_cast<const float4*>(tw.feat + gs * F);
+    for (int64_t it = 0; it < my_tiles; ++it) {
+        const int64_t tile = (int64_t)blockIdx.x + it * gridDim.x;
+        const int64_t row0 = tile * TM + wgi * 64, g0 = row0 + r0, g1 = row0 + r1;
+        // ---- layer 0: D = feat W0^T, the features ([N][F] fp32 from deform_features_kernel) loaded as A fragments
+        float acc[64];
+        {
+            Frags<NS0> x;
+            const float* f0 = tw.feat + g0 * F;
+            const float* f1 = tw.feat + g1 * F;
 #pragma unroll
-            for (int c = 0; c < F; c += 4) {
-                const float4 t4 = __ldg(src + (c >> 2));
-                feat[c] = t4.x; feat[c + 1] = t4.y; feat[c + 2] = t4.z; feat[c + 3] = t4.w;
+            for (int s = 0; s < NS0; ++s) {
+                float v[8];   // (row g: c, c + 1 | row g + 8: c, c + 1) for the two column pairs of the slice
+#pragma unroll
+                for (int hlf = 0; hlf < 2; ++hlf) {
+                    const int c = ARITH == 2 ? 16 * s + 8 * hlf + 2 * t : 8 * s + 4 * hlf + t;
+                    if (ARITH == 2) {
+                        const float2 p0 = g0 < n ? __ldg(reinterpret_cast<const float2*>(f0 + c)) : make_float2(0.f, 0.f);
+                        const float2 p1 = g1 < n ? __ldg(reinterpret_cast<const float2*>(f1 + c)) : make_float2(0.f, 0.f);
+                        v[4 * hlf] = p0.x * A::SF; v[4 * hlf + 1] = p0.y * A::SF; v[4 * hlf + 2] = p1.x * A::SF; v[4 * hlf + 3] = p1.y * A::SF;
+                    } else {
+                        v[4 * hlf] = g0 < n ? __ldg(f0 + c) : 0.f;
+                        v[4 * hlf + 2] = g1 < n ? __ldg(f1 + c) : 0.f;
+                    }
+                }
+                if (ARITH == 2) {
+#pragma unroll
+                    for (int e = 0; e < 8; ++e) mx = fmaxf(mx, fabsf(v[e]));
+                    wg::f16_split2(v[0], v[1], x.hi[s][0], x.lo[s][0]);
+                    wg::f16_split2(v[2], v[3], x.hi[s][1], x.lo[s][1]);
+                    wg::f16_split2(v[4], v[5], x.hi[s][2], x.lo[s][2]);
+                    wg::f16_split2(v[6], v[7], x.hi[s][3], x.lo[s][3]);
+                } else {
+                    wg::tf32_split(v[0], x.hi[s][0], x.lo[s][0]);
+                    wg::tf32_split(v[2], x.hi[s][1], x.lo[s][1]);
+                    wg::tf32_split(v[4], x.hi[s][2], x.lo[s][2]);
+                    wg::tf32_split(v[6], x.hi[s][3], x.lo[s][3]);
+                }
             }
-        } else {
-#pragma unroll
-            for (int c = 0; c < F; ++c) feat[c] = 0.f;
+            gemm3<ARITH, 128, NS0, NS0>(acc, x, 0, sW0, sW0 + 128u * F * A::ES, F, false);
         }
-#pragma unroll
-        for (int c0 = 0; c0 < F; c0 += 8) {
-            uint32_t hi[8], lo[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) tc::tf32_split(feat[c0 + j], hi[j], lo[j]);
-            tc::tmem_st8(lane_base + kColX + c0, hi);
-            tc::tmem_st8(lane_base + kColXLo + c0, lo);
+        // ---- epilogue 0: a1 = relu(D / s + b0) -> A fragments (pre-scaled by SA); sign bits for the backward
+        Frags<NS1> a1;
+        {
+            uint32_t bw0[4], bw1[4];
+            relu_to_frags<ARITH>(acc, kInvL0, sBias, t, a1, bw0, bw1, mx);
+            if (SAVE) store_bits(tw.relu_bits, 0, n, g0, g1, t, bw0, bw1);
         }
-        tc::wait_st();
-        tc::fence_before_sync();
-        mbar_arrive(bar_feat);
-    };
-    if (!is_m && blockIdx.x < ntiles) stage_features(blockIdx.x);
-
-    // optional per-phase cycle accounting (thread 128; G4D debug only)
-    long long cyc[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-    long long tprev = clock64();
-#define G4D_CYC(i) do { if (tw.dbg && tma_thread) { const long long tn_ = clock64(); cyc[i] += tn_ - tprev; tprev = tn_; } } while (0)
-    bool first = true;
-    int hseq = 0;   // running small-head counter -> sAcc buffer
-    for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x, first = false) {
-        const int64_t gi = tile * 128 + row;
-        const bool valid = gi < n;
-        const bool has_next = tile + gridDim.x < ntiles;
-        Vec3 p{0.f, 0.f, 0.f};
-        float sl[3] = {0.f, 0.f, 0.f}, q[4] = {0.f, 0.f, 0.f, 0.f}, ol = 0.f;
-        if (is_m && valid) {
-            p = Vec3{io.xyz[3 * gi], io.xyz[3 * gi + 1], io.xyz[3 * gi + 2]};
-            if (io.scaling) { sl[0] = io.scaling[3 * gi]; sl[1] = io.scaling[3 * gi + 1]; sl[2] = io.scaling[3 * gi + 2]; }
-            if (io.rotation) { const float4 r4 = *reinterpret_cast<const float4*>(io.rotation + 4 * gi); q[0] = r4.x; q[1] = r4.y; q[2] = r4.z; q[3] = r4.w; }
-            if (io.opacity) ol = io.opacity[gi];
+        if (t == 0) {
+#pragma unroll
+            for (int j = 0; j < 11; ++j) { stage[r0 * kStageCols + j] = 0.f; stage[r1 * kStageCols + j] = 0.f; }
         }
-        G4D_CYC(0);   // input loads
-        // ---- layer 0 (MMA warp): D0 = feat * W0^T
-        wait_pumping(bar_l0, ph_l0); ph_l0 ^= 1u;
-        tc::fence_after_sync();
-        G4D_CYC(2);   // features + layer-0 MMA
-        if (is_m && !first) { bar_sync(kBarScratchFree, 256); tc::fence_after_sync(); }   // G has read the previous tile's scratch (A1 region)
-        G4D_CYC(3);   // wait scratch free
-        // ---- epilogue 0: a1 = relu(D0 + b0) -> A1 (hi | lo); ReLU sign bits saved for the backward
-        uint32_t rb[4] = {0u, 0u, 0u, 0u};   // my chunks' sign bits: 2 chunks per word
 #pragma unroll 1
-        for (int ch = ch_lo; ch < ch_hi; ++ch) {
-            const uint32_t c0 = (uint32_t)(ch * 16);
-            uint32_t v[16], hi[16], lo[16];
-            tc::tmem_ld16(lane_base + kColD + c0, v);
-            if (tma_thread) pump_tma();
-            tc::wait_ld();
-            float bb[16];
-#pragma unroll
-            for (int j = 0; j < 16; j += 4) {
-                const float4 b4 = *reinterpret_cast<const float4*>(sBias + c0 + j);
-                bb[j] = b4.x; bb[j + 1] = b4.y; bb[j + 2] = b4.z; bb[j + 3] = b4.w;
-            }
-            uint32_t bits = 0;
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-                const float x = __uint_as_float(v[j]) + bb[j];
-                if (SAVE && x > 0.f) bits |= 1u << j;
-                tc::tf32_split(fmaxf(x, 0.f), hi[j], lo[j]);
-            }
-            if (SAVE) { const int k = ch - ch_lo; if (k < 2) rb[0] |= bits << (k * 16); else rb[1] |= bits << ((k - 2) * 16); }
-            tc::tmem_st16(lane_base + kColA1Hi + c0, hi);
-            tc::tmem_st16(lane_base + kColA1Lo + c0, lo);
-        }
-        if (SAVE && valid) store_relu_half(tw.relu_bits, 0, n, gi, is_m ? 2 : 0, rb[0], rb[1]);
-        tc::wait_st();
-        tc::fence_before_sync();
-        mbar_arrive(bar_a1);          // A1 complete, D0 drained: the MMA warp may start the head GEMMs of this tile
-        G4D_CYC(4);   // epilogue 0
-
-        float dl[11];
-#pragma unroll
-        for (int j = 0; j < 11; ++j) dl[j] = 0.f;
-        float dsh[48];
-#pragma unroll
-        for (int j = 0; j < 48; ++j) dsh[j] = 0.f;
-
+        for (int k = 0; k < m_heads; ++k) {
+            const int h = (int)((hseq >> (3 * k)) & 7u);
+            // ---- layer 1: D = a1 W1^T, K-part by K-part out of the ring
 #pragma unroll 1
-        for (uint32_t kact = 0; kact < m_heads; ++kact) {     // heads in this CTA's (rotated) order
-            const int h = head_at(kact);
-            const float* b1 = sBias + 128 + h * 128;
-            const float* b2 = sBias + 128 + G4D_NUM_HEADS * 128 + b2off_of(d.head_mask, h);
-            const uint32_t db = (kact + par0) & 1u;                     // accumulator of this head
-            const uint32_t dcol = db ? kColD1 : kColD;
-            // ---- layer 1 (issued ahead by the MMA warp): wait for D[db] = a1 * W1^T
-            wait_pumping(bar_dfull + db, db ? ph_d1 : ph_d0);
-            if (db) ph_d1 ^= 1u; else ph_d0 ^= 1u;
-            tc::fence_after_sync();
-            G4D_CYC(6);   // layer-1 MMA not hidden behind the previous epilogue
-            rb[0] = rb[1] = rb[2] = rb[3] = 0u;
+            for (int p = 0; p < A::PH; ++p, ++u) {
+                if (tid == 0 && u + 1 < total_items) issue(u + 1);
+                __syncwarp();
+                const uint32_t s = u & 1u;
+                const long long t0 = dbg ? clock64() : 0;
+                mbar_wait(bar_full + s, (u >> 1) & 1u);
+                if (dbg) t_wait += clock64() - t0;
+                const uint32_t b = sW1 + s * Ls.part_bytes;
+                if constexpr (A::PH == 1) {
+                    gemm3<ARITH, 128, NS1, NSP>(acc, a1, 0, b, b + Ls.part_bytes / 2, 128 / A::PH, false);
+                } else {
+                    // (runtime part index into a register array: unrolled over the parts)
+#pragma unroll
+                    for (int pp = 0; pp < A::PH; ++pp)
+                        if (pp == p) gemm3<ARITH, 128, NS1, NSP>(acc, a1, pp * NSP, b, b + Ls.part_bytes / 2, 128 / A::PH, pp != 0);
+                }
+                if (lane == 0) mbar_arrive(bar_empty + s);      // this warp's MMAs have retired: the slot may be refilled
+            }
+            uint32_t bw0[4], bw1[4];
             if (h < 4) {
-                // ---- small head: layer 2 (k <= 4 outputs) fused into the epilogue in exact fp32 -- cheaper than two
-                //      tensor-core round trips for a 128 x 4 x 128 GEMM.  Each group sums its own hidden units.
-                float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+                // ---- small head: a2 = relu(D / s + b1), layer 2 (<= 4 outputs) in exact fp32; each lane sums its 32 hidden
+                //      units, the quad completes the row
+                const float* b1 = sBias + 128 + h * 128;
                 const float4* w2 = sW2s + h * 128;
-#pragma unroll 1
-                for (int ch = ch_lo; ch < ch_hi; ++ch) {
-                    uint32_t v[16];
-                    tc::tmem_ld16(lane_base + dcol + ch * 16, v);
-                    if (tma_thread) pump_tma();
-                    tc::wait_ld();
-                    float bb[16];
+                float o0[4] = {0.f, 0.f, 0.f, 0.f}, o1[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
-                    for (int j = 0; j < 16; j += 4) {
-                        const float4 b4 = *reinterpret_cast<const float4*>(b1 + ch * 16 + j);
-                        bb[j] = b4.x; bb[j + 1] = b4.y; bb[j + 2] = b4.z; bb[j + 3] = b4.w;
-                    }
-                    uint32_t bits = 0;
+                for (int w = 0; w < 4; ++w) { bw0[w] = 0u; bw1[w] = 0u; }
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const float x = __uint_as_float(v[j]) + bb[j];
-                        if (SAVE && x > 0.f) bits |= 1u << j;
-                        const float a2 = fmaxf(x, 0.f);
-                        const float4 w = w2[ch * 16 + j];
-                        acc.x = fmaf(a2, w.x, acc.x); acc.y = fmaf(a2, w.y, acc.y);
-                        acc.z = fmaf(a2, w.z, acc.z); acc.w = fmaf(a2, w.w, acc.w);
+                for (int j = 0; j < 16; ++j) {
+                    const int c = 8 * j + 2 * t;
+                    const float2 bb = *reinterpret_cast<const float2*>(b1 + c);
+                    const float x0 = fmaf(acc[4 * j], kInvH, bb.x), x1 = fmaf(acc[4 * j + 1], kInvH, bb.y);
+                    const float y0 = fmaf(acc[4 * j + 2], kInvH, bb.x), y1 = fmaf(acc[4 * j + 3], kInvH, bb.y);
+                    const int sh = 8 * (j & 3) + 2 * t;
+                    bw0[j >> 2] |= ((x0 > 0.f ? 1u : 0u) | (x1 > 0.f ? 2u : 0u)) << sh;
+                    bw1[j >> 2] |= ((y0 > 0.f ? 1u : 0u) | (y1 > 0.f ? 2u : 0u)) << sh;
+                    const float4 wa = w2[c], wb = w2[c + 1];
+                    const float ax = fmaxf(x0, 0.f), ay = fmaxf(x1, 0.f), bx = fmaxf(y0, 0.f), by = fmaxf(y1, 0.f);
+                    o0[0] = fmaf(ay, wb.x, fmaf(ax, wa.x, o0[0])); o0[1] = fmaf(ay, wb.y, fmaf(ax, wa.y, o0[1]));
+                    o0[2] = fmaf(ay, wb.z, fmaf(ax, wa.z, o0[2])); o0[3] = fmaf(ay, wb.w, fmaf(ax, wa.w, o0[3]));
+                    o1[0] = fmaf(by, wb.x, fmaf(bx, wa.x, o1[0])); o1[1] = fmaf(by, wb.y, fmaf(bx, wa.y, o1[1]));
+                    o1[2] = fmaf(by, wb.z, fmaf(bx, wa.z, o1[2])); o1[3] = fmaf(by, wb.w, fmaf(bx, wa.w, o1[3]));
+                }
+#pragma unroll
+                for (int o = 0; o < 4; ++o) {
+                    o0[o] += __shfl_xor_sync(0xffffffffu, o0[o], 1); o0[o] += __shfl_xor_sync(0xffffffffu, o0[o], 2);
+                    o1[o] += __shfl_xor_sync(0xffffffffu, o1[o], 1); o1[o] += __shfl_xor_sync(0xffffffffu, o1[o], 2);
+                }
+#pragma unroll
+                for (int w = 0; w < 4; ++w) {
+                    bw0[w] |= __shfl_xor_sync(0xffffffffu, bw0[w], 1); bw0[w] |= __shfl_xor_sync(0xffffffffu, bw0[w], 2);
+                    bw1[w] |= __shfl_xor_sync(0xffffffffu, bw1[w], 1); bw1[w] |= __shfl_xor_sync(0xffffffffu, bw1[w], 2);
+                }
+                if (t == 0) {
+                    const int ko = head_out(h), col = head_col(h);
+#pragma unroll
+                    for (int o = 0; o < 4; ++o) {
+                        if (o < ko) {
+                            stage[r0 * kStageCols + col + o] = o0[o] + b2s[4 * h + o];
+                            stage[r1 * kStageCols + col + o] = o1[o] + b2s[4 * h + o];
+                        }
                     }
-                    if (SAVE) { const int k = ch - ch_lo; if (k < 2) rb[0] |= bits << (k * 16); else rb[1] |= bits << ((k - 2) * 16); }
                 }
-                tc::fence_before_sync();
-                mbar_arrive(bar_dfree + db);   // my part of D[db] is read: once all 256 have arrived the MMA warp may reuse it
-                if (SAVE && valid) store_relu_half(tw.relu_bits, 1 + h, n, gi, is_m ? 2 : 0, rb[0], rb[1]);
-                float4* slot = sAcc + (hseq & 1) * 128 + row;
-                if (!is_m) *slot = acc;
-                bar_sync(kBarE, 256);   // G's partial sums are visible to M
-                if (is_m) {
-                    // fixed summation order: (G's hidden units 0..63) + (M's hidden units 64..127)
-                    const float4 ga = *slot;
-                    acc = make_float4(ga.x + acc.x, ga.y + acc.y, ga.z + acc.z, ga.w + acc.w);
-                    if (h == 0) { dl[0] = acc.x + b2[0]; dl[1] = acc.y + b2[1]; dl[2] = acc.z + b2[2]; }
-                    else if (h == 1) { dl[3] = acc.x + b2[0]; dl[4] = acc.y + b2[1]; dl[5] = acc.z + b2[2]; }
-                    else if (h == 2) { dl[6] = acc.x + b2[0]; dl[7] = acc.y + b2[1]; dl[8] = acc.z + b2[2]; dl[9] = acc.w + b2[3]; }
-                    else { dl[10] = acc.x + b2[0]; }
-                }
-                ++hseq;
-                G4D_CYC(8);   // small-head epilogue + fp32 layer 2
             } else {
-                // the SH head is the last one and owns D0; D1 (= X) was drained by the previous head's epilogue
-#pragma unroll 1
-                for (int hh = 0; hh < 2; ++hh) {
-                    // hidden half hh: a2 = relu(D0[:, 64hh : 64hh+64] + b1) -> X (hi | lo)
-#pragma unroll 1
-                    for (int ch = hc_lo; ch < hc_hi; ++ch) {
-                        const uint32_t cl = (uint32_t)(ch * 16);
-                        const uint32_t cg = (uint32_t)(hh * 64) + cl;
-                        uint32_t v[16], hi[16], lo[16];
-                        tc::tmem_ld16(lane_base + kColD + cg, v);
-                        if (tma_thread) pump_tma();
-                        tc::wait_ld();
-                        float bb[16];
+                // ---- SH head (always last: a1 is dead once its layer-1 GEMM has retired): hidden layer -> A fragments,
+                //      layer 2 as a GEMM with N = 48, SH deltas to the stage
+                relu_to_frags<ARITH>(acc, kInvHS, sBias + 128 + 4 * 128, t, a1, bw0, bw1, mx);
+                float acc2[24];
+                gemm3<ARITH, 48, NS1, NS1>(acc2, a1, 0, sW2, sW2 + 48u * 128u * A::ES, 128, false);
+                const float* b2sh = b2s + 16;
 #pragma unroll
-                        for (int j = 0; j < 16; j += 4) {
-                            const float4 b4 = *reinterpret_cast<const float4*>(b1 + cg + j);
-                            bb[j] = b4.x; bb[j + 1] = b4.y; bb[j + 2] = b4.z; bb[j + 3] = b4.w;
-                        }
-                        uint32_t bits = 0;
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) {
-                            const float x = __uint_as_float(v[j]) + bb[j];
-                            if (SAVE && x > 0.f) bits |= 1u << j;
-                            tc::tf32_split(fmaxf(x, 0.f), hi[j], lo[j]);
-                        }
-                        if (SAVE) { if (hh == 0) rb[0] |= bits << ((ch - hc_lo) * 16); else rb[1] |= bits << ((ch - hc_lo) * 16); }
-                        tc::tmem_st16(lane_base + kColX + cl, hi);
-                        tc::tmem_st16(lane_base + kColXLo + cl, lo);
-                    }
-                    tc::wait_st();
-                    tc::fence_before_sync();
-                    mbar_arrive(bar_x);        // hidden half written: the MMA warp issues the layer-2 partial
-                    G4D_CYC(8);   // hidden-half epilogue
-                    wait_pumping(bar_l2, ph_l2); ph_l2 ^= 1u;
-                    tc::fence_after_sync();
-                    G4D_CYC(9);   // layer-2 partial MMA
+                for (int j = 0; j < 6; ++j) {
+                    const int c = 8 * j + 2 * t;
+                    stage[r0 * kStageCols + 11 + c] = fmaf(acc2[4 * j], kInvH, b2sh[c]);
+                    stage[r0 * kStageCols + 12 + c] = fmaf(acc2[4 * j + 1], kInvH, b2sh[c + 1]);
+                    stage[r1 * kStageCols + 11 + c] = fmaf(acc2[4 * j + 2], kInvH, b2sh[c]);
+                    stage[r1 * kStageCols + 12 + c] = fmaf(acc2[4 * j + 3], kInvH, b2sh[c + 1]);
                 }
-                // sign bits of the SH head: word w of the 128-bit row = hidden units [32w, 32w+32); G owns words 0 and 2
-                if (SAVE && valid) {
-                    uint32_t* dst = tw.relu_bits + ((size_t)(1 + h) * (size_t)n + (size_t)gi) * 4 + (is_m ? 1 : 0);
-                    dst[0] = rb[0]; dst[2] = rb[1];
-                }
-                if (is_m) {
-#pragma unroll
-                    for (int ch = 0; ch < 3; ++ch) {
-                        uint32_t v[16];
-                        tc::tmem_ld16(lane_base + kColD + ch * 16, v);
-                        tc::wait_ld();
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) dsh[ch * 16 + j] = __uint_as_float(v[j]) + b2[ch * 16 + j];
-                    }
-                }
-                tc::fence_before_sync();
-                mbar_arrive(bar_dfree + db);   // D0 (and D2 inside it) read out: the next tile's layer-0 GEMM may overwrite it
             }
-            G4D_CYC(10);  // head output / hand-over
+            if (SAVE) store_bits(tw.relu_bits, 1 + h, n, g0, g1, t, bw0, bw1);
         }
-        if (is_m) {
-            p.x += dl[0]; p.y += dl[1]; p.z += dl[2];
-            // ---- hand the deformed position and the SH deltas to the G thread of this lane (A1 is dead now)
-            {
-                uint32_t s8[8] = {__float_as_uint(p.x), __float_as_uint(p.y), __float_as_uint(p.z), 0u, 0u, 0u, 0u, 0u};
-                tc::tmem_st8(lane_base + kColScratch, s8);
-                if (hsh) {
-#pragma unroll
-                    for (int ch = 0; ch < 3; ++ch) {
-                        uint32_t v[16];
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) v[j] = __float_as_uint(dsh[ch * 16 + j]);
-                        tc::tmem_st16(lane_base + kColScratch + 8 + ch * 16, v);
+        // ---- per-Gaussian tail: threads 0-63 the geometry, 64-127 the colour of Gaussian (t128 & 63) of the warpgroup
+        bar_sync(1 + wgi, 128);
+        {
+            const int row = t128 & 63;
+            const int64_t gi = row0 + row;
+            const float* o = stage + row * kStageCols;
+            if (gi < n) {
+                const Vec3 p{io.xyz[3 * gi] + o[0], io.xyz[3 * gi + 1] + o[1], io.xyz[3 * gi + 2] + o[2]};
+                if (t128 < 64) {
+                    float sl[3] = {0.f, 0.f, 0.f}, q[4] = {0.f, 0.f, 0.f, 0.f}, ol = 0.f;
+                    if (io.scaling) { sl[0] = io.scaling[3 * gi]; sl[1] = io.scaling[3 * gi + 1]; sl[2] = io.scaling[3 * gi + 2]; }
+                    if (io.rotation) { const float4 r4 = *reinterpret_cast<const float4*>(io.rotation + 4 * gi); q[0] = r4.x; q[1] = r4.y; q[2] = r4.z; q[3] = r4.w; }
+                    if (io.opacity) ol = io.opacity[gi];
+                    sl[0] += o[3]; sl[1] += o[4]; sl[2] += o[5];
+                    q[0] += o[6]; q[1] += o[7]; q[2] += o[8]; q[3] += o[9];
+                    ol += o[10];
+                    if (MODE == 0) {
+                        io.out_xyz[3 * gi] = p.x; io.out_xyz[3 * gi + 1] = p.y; io.out_xyz[3 * gi + 2] = p.z;
+                        if (io.out_scaling) { io.out_scaling[3 * gi] = sl[0]; io.out_scaling[3 * gi + 1] = sl[1]; io.out_scaling[3 * gi + 2] = sl[2]; }
+                        if (io.out_rotation) *reinterpret_cast<float4*>(io.out_rotation + 4 * gi) = make_float4(q[0], q[1], q[2], q[3]);
+                        if (io.out_opacity) io.out_opacity[gi] = ol;
+                    } else {
+                        fused_finish_geometry(cam, io, gi, p, sl, q, ol);
                     }
-                }
-                tc::wait_st();
-                tc::fence_before_sync();
-                bar_arrive(kBarScratch, 256);
-            }
-            if (tma_thread) pump_tma();   // (prefetch of the next tile's first W1 halves once the last GEMM has retired)
-            // ---- finish the geometric half of my Gaussian
-            if (valid) {
-                sl[0] += dl[3]; sl[1] += dl[4]; sl[2] += dl[5];
-                q[0] += dl[6]; q[1] += dl[7]; q[2] += dl[8]; q[3] += dl[9];
-                ol += dl[10];
-                if (MODE == 0) {
-                    io.out_xyz[3 * gi] = p.x; io.out_xyz[3 * gi + 1] = p.y; io.out_xyz[3 * gi + 2] = p.z;
-                    if (io.out_scaling) { io.out_scaling[3 * gi] = sl[0]; io.out_scaling[3 * gi + 1] = sl[1]; io.out_scaling[3 * gi + 2] = sl[2]; }
-                    if (io.out_rotation) *reinterpret_cast<float4*>(io.out_rotation + 4 * gi) = make_float4(q[0], q[1], q[2], q[3]);
-                    if (io.out_opacity) io.out_opacity[gi] = ol;
                 } else {
-                    fused_finish_geometry(cam, io, gi, p, sl, q, ol);
-                }
-            }
-            if (tma_thread) pump_tma();
-            G4D_CYC(11);  // scratch hand-off + geometry tail
-        } else {
-            // ---- G tail: next tile's features, then the SH colour of my Gaussian once M has published p and the SH deltas
-            if (has_next) stage_features(tile + gridDim.x);
-            bar_sync(kBarScratch, 256);
-            tc::fence_after_sync();
-            uint32_t s8[8];
-            tc::tmem_ld8(lane_base + kColScratch, s8);
-            float gsh[48];
-            if (hsh) {
+                    float dsh[48];
 #pragma unroll
-                for (int ch = 0; ch < 3; ++ch) {
-                    uint32_t v[16];
-                    tc::tmem_ld16(lane_base + kColScratch + 8 + ch * 16, v);
-                    tc::wait_ld();
+                    for (int j = 0; j < 48; ++j) dsh[j] = hsh ? o[11 + j] : 0.f;
+                    if (MODE == 0) {
+                        if (io.out_shs && hsh) {
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) gsh[ch * 16 + j] = __uint_as_float(v[j]);
-                }
-            } else {
-#pragma unroll
-                for (int j = 0; j < 48; ++j) gsh[j] = 0.f;
-            }
-            tc::wait_ld();
-            tc::fence_before_sync();
-            bar_arrive(kBarScratchFree, 256);
-            if (valid) {
-                const Vec3 pg{__uint_as_float(s8[0]), __uint_as_float(s8[1]), __uint_as_float(s8[2])};
-                if (MODE == 0) {
-                    if (io.out_shs && hsh) {
-#pragma unroll
-                        for (int j = 0; j < 48; j += 4) {
-                            const float4 b = *reinterpret_cast<const float4*>(io.shs + gi * 48 + j);
-                            *reinterpret_cast<float4*>(io.out_shs + gi * 48 + j) = make_float4(b.x + gsh[j], b.y + gsh[j + 1], b.z + gsh[j + 2], b.w + gsh[j + 3]);
+                            for (int j = 0; j < 48; j += 4) {
+                                const float4 b = *reinterpret_cast<const float4*>(io.shs + gi * 48 + j);
+                                *reinterpret_cast<float4*>(io.out_shs + gi * 48 + j) = make_float4(b.x + dsh[j], b.y + dsh[j + 1], b.z + dsh[j + 2], b.w + dsh[j + 3]);
+                            }
                         }
+                    } else {
+                        fused_finish_colour(cam, io, gi, p, hsh, dsh);
                     }
-                } else {
-                    fused_finish_colour(cam, io, gi, pg, hsh, gsh);
                 }
             }
         }
+        bar_sync(1 + wgi, 128);   // the stage is read before the next tile's deltas overwrite it
     }
-    if (is_m && !first) { bar_sync(kBarScratchFree, 256); }   // pair the G group's last arrive
-    if (tw.dbg && tma_thread) {
-        for (int i = 0; i < 12; ++i) tw.dbg[blockIdx.x * 12 + i] = cyc[i];
-    }
-#undef G4D_CYC
-    }   // epilogue groups
-    tc::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc(tbase, tc::kTmemCols);
+    // range check of everything that went through an f16 conversion (already in operand units)
+    if (ARITH == 2 && mx >= kF16Max && tw.status) *reinterpret_cast<volatile uint32_t*>(tw.status) = 1u;
+    if (dbg) { tw.dbg[blockIdx.x * 12] = clock64() - t_start; tw.dbg[blockIdx.x * 12 + 1] = t_wait; }
 }
 
 // ---- HexPlane gather at full occupancy: C/4 threads per Gaussian, one channel vector each -> feat [N][F] fp32 -----------
@@ -729,50 +558,50 @@ cudaError_t launch_deform_features(const DeformDesc& d, int64_t n, const float* 
     return cudaErrorInvalidValue;
 }
 
-bool tc_deform_supported(const DeformDesc& d) {
+bool tc_deform_supported(const DeformDesc& d, int arith) {
     if (d.WD != 128) return false;
     if (!((d.C == 16 && (d.levels == 2 || d.levels == 3)) || (d.C == 32 && d.levels == 2))) return false;
-    const int max_kp = (d.head_mask & G4D_HEAD_SHS) ? 48 : 16;
-    return tc_smem_layout(d.F, max_kp).total + 1024 <= 227 * 1024;
+    return tc_smem_layout(arith, d.F, (d.head_mask & G4D_HEAD_SHS) != 0).total + kTcStaticSmem <= kMaxSmemPerBlock;
 }
 
-template <int MODE, int C, int L>
+template <int ARITH, int MODE, int C, int L>
 static cudaError_t launch_deform_tc_t(const DeformDesc& d, const TcWeights& tw, const TcSmem& Ls, size_t bytes, int grid,
-                                      const CameraDev* cam, float time, bool use_cam_time, int64_t n, const DeformIO& io,
-                                      cudaStream_t st) {
+                                      const CameraDev* cam, bool use_cam, int64_t n, const DeformIO& io, cudaStream_t st) {
+    constexpr int threads = TcArith<ARITH>::NWG * 128;
     cudaError_t e;
     if (tw.relu_bits) {
-        e = cudaFuncSetAttribute(deform_tc_kernel<MODE, C, L, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+        e = cudaFuncSetAttribute(deform_tc_kernel<ARITH, MODE, C, L, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
         if (e != cudaSuccess) return e;
-        deform_tc_kernel<MODE, C, L, true><<<grid, kTcThreads, bytes, st>>>(d, tw, Ls, cam, time, use_cam_time ? 1 : 0, n, io);
-    } else {
-        e = cudaFuncSetAttribute(deform_tc_kernel<MODE, C, L, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-        if (e != cudaSuccess) return e;
-        deform_tc_kernel<MODE, C, L, false><<<grid, kTcThreads, bytes, st>>>(d, tw, Ls, cam, time, use_cam_time ? 1 : 0, n, io);
+        return launch_k(deform_tc_kernel<ARITH, MODE, C, L, true>, dim3(grid), dim3(threads), bytes, st, true, d, tw, Ls, cam, use_cam ? 1 : 0, n, io);
     }
-    return cudaGetLastError();
+    e = cudaFuncSetAttribute(deform_tc_kernel<ARITH, MODE, C, L, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e != cudaSuccess) return e;
+    return launch_k(deform_tc_kernel<ARITH, MODE, C, L, false>, dim3(grid), dim3(threads), bytes, st, true, d, tw, Ls, cam, use_cam ? 1 : 0, n, io);
 }
 
-cudaError_t launch_deform_tc(const DeformDesc& d, const TcWeights& tw, int mode, const CameraDev* cam, float time,
-                             bool use_cam_time, int64_t n, const DeformIO& io, int sm_count, cudaStream_t st) {
+cudaError_t launch_deform_tc(const DeformDesc& d, const TcWeights& tw, int mode, const CameraDev* cam, bool use_cam_time,
+                             int64_t n, const DeformIO& io, int sm_count, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
     if (!tw.feat) return cudaErrorInvalidValue;
     {
         cudaError_t e = launch_deform_features(d, n, io.xyz, tw.feat, st);
         if (e != cudaSuccess) return e;
     }
-    const int max_kp = (d.head_mask & G4D_HEAD_SHS) ? 48 : 16;
-    const TcSmem Ls = tc_smem_layout(d.F, max_kp);
-    const size_t bytes = Ls.total + 1024;
-    const int64_t ntiles = (n + 127) / 128;
+    const TcSmem Ls = tc_smem_layout(tw.arith, d.F, (d.head_mask & G4D_HEAD_SHS) != 0);
+    const size_t bytes = Ls.total;
+    const int64_t ntiles = (n + 64 * (tw.arith == 2 ? 2 : 1) - 1) / (64 * (tw.arith == 2 ? 2 : 1));
     const int grid = (int)(ntiles < sm_count ? ntiles : sm_count);
-#define G4D_TC_CASE(CC, LL)                                                                                                   \
-    if (d.C == CC && d.levels == LL)                                                                                          \
-        return mode == 0 ? launch_deform_tc_t<0, CC, LL>(d, tw, Ls, bytes, grid, cam, time, use_cam_time, n, io, st)          \
-                         : launch_deform_tc_t<1, CC, LL>(d, tw, Ls, bytes, grid, cam, time, use_cam_time, n, io, st);
-    G4D_TC_CASE(16, 2)
-    G4D_TC_CASE(16, 3)
-    G4D_TC_CASE(32, 2)
+    const bool use_cam = mode == 1 || use_cam_time;
+#define G4D_TC_CASE(AR, CC, LL)                                                                                        \
+    if (tw.arith == AR && d.C == CC && d.levels == LL)                                                                 \
+        return mode == 0 ? launch_deform_tc_t<AR, 0, CC, LL>(d, tw, Ls, bytes, grid, cam, use_cam, n, io, st)          \
+                         : launch_deform_tc_t<AR, 1, CC, LL>(d, tw, Ls, bytes, grid, cam, use_cam, n, io, st);
+    G4D_TC_CASE(2, 16, 2)
+    G4D_TC_CASE(2, 16, 3)
+    G4D_TC_CASE(2, 32, 2)
+    G4D_TC_CASE(1, 16, 2)
+    G4D_TC_CASE(1, 16, 3)
+    G4D_TC_CASE(1, 32, 2)
 #undef G4D_TC_CASE
     return cudaErrorInvalidValue;
 }

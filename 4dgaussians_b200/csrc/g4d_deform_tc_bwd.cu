@@ -1,119 +1,95 @@
-// g4d_deform_tc_bwd.cu -- tensor-core backward of the deformation network (net_width 128), two kernels:
+// g4d_deform_tc_bwd.cu -- tensor-core backward of the deformation network (net_width 128), two wgmma kernels (tc_wgmma.cuh):
 //
-//  A  "dgrad":  tile of 128 Gaussians per pass (TMEM lanes).  Recomputes the forward activations with BF16x2 tcgen05
-//               MMAs (hi + lo parts, 3 products, fp32 accumulate: ~16 mantissa bits, measured gradient error 1.5e-5),
-//               forms dz per head in the epilogue (layer 2 is tiny: its dgrad is done in fp32 by the epilogue threads),
-//               accumulates d(a1) over the heads IN TMEM with one MMA chain per head, then d(feat) = dh W0 -> [N][F] fp32.
-//               Both 128-thread groups own half of the hidden columns of every epilogue.  The ReLU signs come from the
-//               bits the forward saved (G4D_RELU_BITS_WORDS), so this is the gradient of the forward that ran.
-//               Everything the weight gradients need is written ONCE as ready-to-use MMA operand images
-//               (8x8 bf16 core-matrix layout, tc_umma.cuh) so that kernel B is pure TMA + MMA.
+//  A  "dgrad":  a CTA owns a tile of 128 Gaussians per pass, one warpgroup per 64 of them, persistent over tiles.
+//               Recomputes the forward activations with BF16x2 MMAs (hi + lo parts, 3 products, fp32 accumulate: ~16
+//               mantissa bits), forms dz per head in the epilogue (the <= 4-wide heads' layer-2 dgrad in fp32, the SH head's
+//               as a GEMM with K = 48), accumulates d(a1) over the heads in registers with one GEMM per head (W1 read
+//               MN-major), then d(feat) = dh W0 -> [N][F] fp32.  Every A operand is a register fragment built from the
+//               previous accumulator (tc_wgmma.cuh); W1 images stream through a two-slot TMA ring, one head ahead.  The ReLU
+//               signs come from the bits the forward saved (G4D_RELU_BITS_WORDS), so this is the gradient of the forward
+//               that ran.  Everything the weight gradients need is written ONCE to global memory as ready-to-use MMA operand
+//               images (8x8 bf16 core-matrix layout) so that kernel B is pure TMA + MMA.
 //               HexPlane gather (bwd_features_kernel, skipped when the forward's staging buffer was kept) and scatter
 //               (bwd_scatter_kernel: plane REDs, d(xyz), residual paths) run around it at full occupancy.
-//  B  "wgrad":  dW1_h = DZ_h^T A1, dW2_h^T = A2_h^T DOUT_h, db1_h = DZ_h^T 1, dW0 = DH^T FEAT, db0 = DH^T 1 as split-K
-//               tcgen05 GEMMs over the Gaussian index (both operands MN-major straight from the images), accumulators
-//               persistent in TMEM across the CTA's tiles, one atomic flush per CTA; two half-tile smem stages pipeline
-//               the TMA loads against the MMAs.
+//  B  "wgrad":  dW1_h = DZ_h^T A1, dW2_h^T = A2_h^T DOUT_h, db1_h = DZ_h^T 1, db2_h = 1^T DOUT_h, dW0 = DH^T FEAT, db0 = DH^T 1
+//               as split-K GEMMs over the Gaussian index (operands MN-major straight from the images), accumulators in
+//               registers across the CTA's tiles (warpgroup w: output rows [64 w, 64 w + 64)), one atomic flush per CTA;
+//               two half-tile smem stages pipeline the TMA loads against the MMAs.
 //
 // Replaces the autograd backward of scene/deformation.py:67-148 + scene/hexplane.py:73-106 (loss.backward(), train.py:219).
 // Compiled with the default FMA contraction (no index-producing math here).
 #include "deform_bwd_common.cuh"
-#include "tc_umma.cuh"
+#include "tc_wgmma.cuh"
 
 namespace g4d {
 
 namespace {
 
-constexpr uint32_t kA1 = 0, kA1Lo = 64, kD = 128, kDZ = 256, kDZLo = 320, kDA1 = 384;   // TMEM columns (kernel A)
-constexpr int kBarFeat = 1, kBarXFree = 2, kBarScratch = 3, kBarScratchFree = 4, kBarM = 5, kBarE = 6;
 constexpr uint32_t kImg128 = 128u * 128u * 2u;   // bytes of one 128x128 bf16 part (hi or lo)
 
-__device__ __forceinline__ void bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
-__device__ __forceinline__ void bar_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
-
-// ---- MMA issue helpers (one thread) -----------------------------------------------------------------------------
-// D[128 x N] (+)= A[128 x K] * B^T with A = (hi, lo) bf16 packed two-per-column in TMEM, B = (hi, lo) images in smem.
-//   b_mn = false: B image rows = N, cols = K (K-major);  b_mn = true: B image rows = K, cols = N (MN-major)
-template <int K>
-__device__ __forceinline__ void gemm_bf16x2_ts(uint32_t d_tmem, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo, uint32_t N,
-                                               uint32_t b_ncols, bool b_mn, bool accumulate) {
-    const uint32_t idesc = tc::make_idesc_bf16(128, N, false, b_mn);
-    const uint32_t rowgrp = (b_ncols >> 3) * 128u;
-    const uint32_t lbo = b_mn ? rowgrp : 128u, sbo = b_mn ? 128u : rowgrp;
-    const uint32_t step16 = (b_mn ? 2u * rowgrp : 256u) >> 4;   // one K = 16 step, in 16-byte units
-    const uint64_t bd_hi = tc::make_smem_desc(b_hi, lbo, sbo), bd_lo = tc::make_smem_desc(b_lo, lbo, sbo);
+// D[64 x N] (+)= A * B with A = (hi, lo) bf16 register fragments (NS K-slices) and B = (hi, lo) images described by bh / bl,
+// `step` = descriptor advance (16-byte units) per K = 16; TB = 1: B is MN-major
+template <int N, int NS, int TB>
+__device__ __forceinline__ void gemm3_rs(float (&d)[N / 2], const wg::Frags<NS>& a, uint64_t bh, uint64_t bl, uint32_t step, bool accumulate) {
+    wg::fence_regs(d);
+    wg::fence();
 #pragma unroll
     for (int p = 0; p < 3; ++p) {
-        const uint32_t a = (p == 0) ? a_lo : a_hi;
-        const uint64_t bd = (p == 1) ? bd_lo : bd_hi;
 #pragma unroll
-        for (int ks = 0; ks < K; ks += 16)
-            tc::umma_bf16_ts(d_tmem, a + (ks >> 1), bd + (uint64_t)((ks >> 4) * step16), idesc, accumulate || p > 0 || ks > 0);
+        for (int s = 0; s < NS; ++s)
+            wg::mma_bf16_rs<N, TB>(d, p == 0 ? a.lo[s] : a.hi[s], ((p == 1) ? bl : bh) + (uint64_t)(s * step),
+                                   (accumulate || p > 0 || s > 0) ? 1u : 0u);
     }
+    wg::commit();
+    wg::wait_all();
+    wg::fence_regs(d);
 }
 
-// D[128 x N] (+)= A^T B with both operands MN-major images (rows = K = Gaussian, cols = M resp. N), K rows
-template <int K>
-__device__ __forceinline__ void gemm_bf16x2_ss_mn(uint32_t d_tmem, uint32_t a_hi, uint32_t a_lo, uint32_t a_ncols, uint32_t b_hi,
-                                                  uint32_t b_lo, uint32_t b_ncols, uint32_t N, bool accumulate, bool b_single) {
-    const uint32_t idesc = tc::make_idesc_bf16(128, N, true, true);
-    const uint32_t a_grp = (a_ncols >> 3) * 128u, b_grp = (b_ncols >> 3) * 128u;
-    const uint64_t ad_hi = tc::make_smem_desc(a_hi, a_grp, 128u), ad_lo = tc::make_smem_desc(a_lo, a_grp, 128u);
-    const uint64_t bd_hi = tc::make_smem_desc(b_hi, b_grp, 128u), bd_lo = tc::make_smem_desc(b_lo, b_grp, 128u);
-    const uint32_t a_step = (2u * a_grp) >> 4, b_step = (2u * b_grp) >> 4;
+// D[64 x N] (+)= A * B, both operands from shared memory, K = 64 (4 steps); b_single: B has no lo part (all-ones operand)
+template <int N, int TA, int TB>
+__device__ __forceinline__ void gemm3_ss(float (&d)[N / 2], uint64_t ah, uint64_t al, uint32_t astep, uint64_t bh, uint64_t bl,
+                                         uint32_t bstep, bool accumulate, bool a_single, bool b_single) {
+    wg::fence_regs(d);
+    wg::fence();
 #pragma unroll
     for (int p = 0; p < 3; ++p) {
-        if (b_single && p == 1) continue;   // B has no lo part (e.g. the all-ones operand)
-        const uint64_t ad = (p == 0) ? ad_lo : ad_hi;
-        const uint64_t bd = (p == 1) ? bd_lo : bd_hi;
+        if ((p == 0 && a_single) || (p == 1 && b_single)) continue;
 #pragma unroll
-        for (int ks = 0; ks < K; ks += 16)
-            tc::umma_bf16_ss(d_tmem, ad + (uint64_t)((ks >> 4) * a_step), bd + (uint64_t)((ks >> 4) * b_step), idesc,
-                             accumulate || p > 0 || ks > 0);
+        for (int s = 0; s < 4; ++s)
+            wg::mma_bf16_ss<N, TA, TB>(d, ((p == 0) ? al : ah) + (uint64_t)(s * astep), ((p == 1) ? bl : bh) + (uint64_t)(s * bstep),
+                                       (accumulate || s > 0 || p > (a_single || b_single ? 1 : 0)) ? 1u : 0u);
     }
+    wg::commit();
+    wg::wait_all();
+    wg::fence_regs(d);
 }
 
-// one stage of a transposing butterfly: N values per lane -> N/2 (lanes with `hi` keep the upper half), summed with the partner lane
-template <int N, int CAP>
-__device__ __forceinline__ void halve(float (&v)[CAP], bool hi, int lane_mask) {
-#pragma unroll
-    for (int k = 0; k < N / 2; ++k) {
-        const float send = hi ? v[k] : v[k + N / 2];
-        const float keep = hi ? v[k + N / 2] : v[k];
-        v[k] = keep + __shfl_xor_sync(0xffffffffu, send, lane_mask);
-    }
+// accumulator block j of rows (g, g + 8), columns (c, c + 1) -> bf16 (hi, lo) A fragment slots + the rows' image words
+__device__ __forceinline__ void put16(wg::Frags<8>& a, int j, float x0, float x1, float y0, float y1, uint32_t (&w)[4]) {
+    const int s = j >> 1, o = (j & 1) * 2;
+    wg::bf16_split2(x0, x1, a.hi[s][o], a.lo[s][o]);
+    wg::bf16_split2(y0, y1, a.hi[s][o + 1], a.lo[s][o + 1]);
+    w[0] = a.hi[s][o]; w[1] = a.lo[s][o]; w[2] = a.hi[s][o + 1]; w[3] = a.lo[s][o + 1];
 }
-
-__device__ __forceinline__ uint32_t pack2(uint16_t even_k, uint16_t odd_k) { return (uint32_t)even_k | ((uint32_t)odd_k << 16); }
-
-// 16 consecutive values of row `g` -> (hi | lo) bf16: packed TMEM words (8 + 8) and two 16-byte image core rows each
-struct Split16 {
-    uint32_t hi[8], lo[8];
-};
-__device__ __forceinline__ void split16(const float (&x)[16], Split16& o) {
-    // two elements per cvt: cvt.rn.bf16x2.f32 d, a, b packs a into the upper and b into the lower half (lower = even k)
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-        uint32_t hi, lo;
-        asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(x[2 * j + 1]), "f"(x[2 * j]));
-        const float he = __uint_as_float(hi << 16), ho = __uint_as_float(hi & 0xffff0000u);
-        asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(x[2 * j + 1] - ho), "f"(x[2 * j] - he));
-        o.hi[j] = hi;
-        o.lo[j] = lo;
-    }
+// (hi, lo) words of rows ra / rb at column c of a (hi | lo) image with `ncols` columns (lo part at +part_bytes)
+__device__ __forceinline__ void store_words(uint8_t* img, uint32_t part_bytes, uint32_t ncols, uint32_t ra, uint32_t rb, uint32_t c,
+                                            const uint32_t (&w)[4]) {
+    *reinterpret_cast<uint32_t*>(img + wg::img16_off(ra, c, ncols)) = w[0];
+    *reinterpret_cast<uint32_t*>(img + part_bytes + wg::img16_off(ra, c, ncols)) = w[1];
+    *reinterpret_cast<uint32_t*>(img + wg::img16_off(rb, c, ncols)) = w[2];
+    *reinterpret_cast<uint32_t*>(img + part_bytes + wg::img16_off(rb, c, ncols)) = w[3];
 }
-// write 16 columns [c0, c0+16) of row g of a (hi | lo) image with `ncols` columns (lo part at +part_bytes)
-__device__ __forceinline__ void store_img16(uint8_t* img, uint32_t part_bytes, uint32_t ncols, uint32_t g, uint32_t c0, const Split16& s) {
-    uint8_t* p = img + tc::img16_off(g, c0, ncols);
-    *reinterpret_cast<uint4*>(p) = make_uint4(s.hi[0], s.hi[1], s.hi[2], s.hi[3]);
-    *reinterpret_cast<uint4*>(p + 128) = make_uint4(s.hi[4], s.hi[5], s.hi[6], s.hi[7]);
-    *reinterpret_cast<uint4*>(p + part_bytes) = make_uint4(s.lo[0], s.lo[1], s.lo[2], s.lo[3]);
-    *reinterpret_cast<uint4*>(p + part_bytes + 128) = make_uint4(s.lo[4], s.lo[5], s.lo[6], s.lo[7]);
+__device__ __forceinline__ bool bit_of(const uint32_t (&m)[4], int c) {
+    const uint32_t w = (c >> 5) == 0 ? m[0] : (c >> 5) == 1 ? m[1] : (c >> 5) == 2 ? m[2] : m[3];
+    return (w >> (c & 31)) & 1u;
+}
+__device__ __forceinline__ void mbar_arrive1(void* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
 }  // namespace
 
-// ---- global-memory layout of the operand images ------------------------------------------------------------------
+// ---- global-memory layout of the operand images (per tile of 128 Gaussians, (hi | lo), row = Gaussian) ---------------------
 struct BwdImages {
     uint8_t* a1;                    // [ntiles][2 * kImg128]
     uint8_t* dh;                    // [ntiles][2 * kImg128]
@@ -124,27 +100,28 @@ struct BwdImages {
     uint32_t feat_bytes;            // bytes of one (hi | lo) feature image
 };
 
-struct BwdSmemA { uint32_t w0, w1, w2s, w2sh, bias, bars, total; };
+struct BwdSmemA { uint32_t w0, w1, w2t, bias, w2s, bars, total; };
 static BwdSmemA bwd_smem_a(int F, bool sh) {
     BwdSmemA s{};
     uint32_t off = 0;
     auto take = [&](uint32_t b) { uint32_t o = off; off += (b + 127u) & ~127u; return o; };
     s.w0 = take(2u * 128 * F * 2);
-    s.w1 = take(2u * 2u * kImg128);          // two buffers of (hi | lo)
-    s.w2s = take(4 * 128 * 16);
-    s.w2sh = take(sh ? 48 * 128 * 4 : 128);
+    s.w1 = take(2u * 2u * kImg128);          // ring of two (hi | lo) head images
+    s.w2t = take(sh ? 2u * 128 * 48 * 2 : 128);
     s.bias = take((128 + G4D_NUM_HEADS * 128) * 4);
+    s.w2s = take(4 * 128 * 16);
     s.bars = take(64);
     s.total = off;
     return s;
 }
 
 // ---- weight images (bf16 hi | lo), rebuilt when the parameter version changes --------------------------------------
+// matrix m: [rows][K] source; trans: image of the transpose ([K][rows], the SH head's W2 as the K-major B of d(a2) = dout W2)
 struct BwdPackDesc {
-    const float* src[1 + G4D_NUM_HEADS];
-    uint8_t* dst[1 + G4D_NUM_HEADS];
-    int K[1 + G4D_NUM_HEADS];
-    int start[2 + G4D_NUM_HEADS];
+    const float* src[2 + G4D_NUM_HEADS];
+    uint8_t* dst[2 + G4D_NUM_HEADS];
+    int K[2 + G4D_NUM_HEADS], rows[2 + G4D_NUM_HEADS], trans[2 + G4D_NUM_HEADS];
+    int start[3 + G4D_NUM_HEADS];
     int count;
 };
 __global__ void bwd_pack_weights_kernel(BwdPackDesc p) {
@@ -155,14 +132,14 @@ __global__ void bwd_pack_weights_kernel(BwdPackDesc p) {
     const int e = i - p.start[m], K = p.K[m];
     const uint32_t n = e / K, k = e % K;
     uint16_t hi, lo;
-    tc::bf16_split(__ldg(p.src[m] + e), hi, lo);
-    const uint32_t off = tc::img16_off(n, k, K);
+    wg::bf16_split(__ldg(p.src[m] + e), hi, lo);
+    const uint32_t off = p.trans[m] ? wg::img16_off(k, n, (uint32_t)p.rows[m]) : wg::img16_off(n, k, (uint32_t)K);
     *reinterpret_cast<uint16_t*>(p.dst[m] + off) = hi;
-    *reinterpret_cast<uint16_t*>(p.dst[m] + 128u * K * 2u + off) = lo;
+    *reinterpret_cast<uint16_t*>(p.dst[m] + (size_t)p.rows[m] * K * 2u + off) = lo;
 }
 
 size_t tc_bwd_weight_bytes(const G4DDeformParams& prm) {
-    return (size_t)2 * 128 * (prm.levels * prm.channels) * 2 + (size_t)G4D_NUM_HEADS * 2 * kImg128 + 256;
+    return (size_t)2 * 128 * (prm.levels * prm.channels) * 2 + (size_t)G4D_NUM_HEADS * 2 * kImg128 + (size_t)2 * 48 * 128 * 2 + 512;
 }
 
 cudaError_t launch_tc_bwd_pack_weights(const G4DDeformParams& prm, uint8_t* blob, TcBwdWeights* out, cudaStream_t st) {
@@ -170,15 +147,31 @@ cudaError_t launch_tc_bwd_pack_weights(const G4DDeformParams& prm, uint8_t* blob
     const int F = prm.levels * prm.channels;
     int m = 0, total = 0;
     uint8_t* q = blob;
-    p.src[m] = prm.w0; p.dst[m] = q; p.K[m] = F; p.start[m] = total; total += 128 * F; out->w0 = q; q += (size_t)2 * 128 * F * 2; ++m;
+    auto add = [&](const float* src, int rows, int K, int trans) {
+        p.src[m] = src; p.dst[m] = q; p.rows[m] = rows; p.K[m] = K; p.trans[m] = trans; p.start[m] = total;
+        total += rows * K;
+        uint8_t* r = q;
+        q += (size_t)2 * rows * K * 2;
+        ++m;
+        return r;
+    };
+    out->w0 = add(prm.w0, 128, F, 0);
+    out->w2sh = nullptr;
     for (int h = 0; h < G4D_NUM_HEADS; ++h) {
         out->w1[h] = nullptr;
         if (!(prm.head_mask & (1 << h))) continue;
-        p.src[m] = prm.w1[h]; p.dst[m] = q; p.K[m] = 128; p.start[m] = total; total += 128 * 128; out->w1[h] = q; q += 2 * kImg128; ++m;
+        out->w1[h] = add(prm.w1[h], 128, 128, 0);
     }
+    if (prm.head_mask & G4D_HEAD_SHS) out->w2sh = add(prm.w2[4], 48, 128, 1);
     p.start[m] = total; p.count = m;
     bwd_pack_weights_kernel<<<(total + 255) / 256, 256, 0, st>>>(p);
     return cudaGetLastError();
+}
+
+bool tc_backward_supported(const DeformDesc& d) {
+    if (d.WD != 128) return false;
+    if (!((d.C == 16 && (d.levels == 2 || d.levels == 3)) || (d.C == 32 && d.levels == 2))) return false;
+    return bwd_smem_a(d.F, (d.head_mask & G4D_HEAD_SHS) != 0).total + 1024 <= 227 * 1024;
 }
 
 // ======================================================================================================
@@ -189,36 +182,24 @@ struct BwdADesc {
     TcBwdWeights w;
     BwdImages img;
     const float* go[G4D_NUM_HEADS];
-    float* gi[G4D_NUM_HEADS];
-    float* g_b2[G4D_NUM_HEADS];
     const float* feat;           // [N][F] fp32 (bwd_features_kernel)
     float* dfeat;                // [N][F] fp32 -> bwd_scatter_kernel
     const uint32_t* relu_bits;   // [6][N][4] + tag (g4d.h G4D_RELU_BITS_WORDS) or NULL
-    long long* dbg;              // optional [grid][12] per-phase cycle counters (G4D_OPT_TC_DEBUG)
 };
 
 template <int C, int L>
 __global__ void __launch_bounds__(256, 1)
-deform_tc_bwd_dgrad_kernel(BwdADesc bd, BwdSmemA Ls, float time, int64_t n, const float* __restrict__ xyz) {
-    constexpr int F = C * L;
-    constexpr int C4 = C / 4;
+deform_tc_bwd_dgrad_kernel(BwdADesc bd, BwdSmemA Ls, int64_t n) {
+    constexpr int F = C * L, NS0 = F / 16;
     extern __shared__ __align__(1024) uint8_t smem[];
-    __shared__ DeformDesc sd;
-    __shared__ uint32_t tmem_base_s;
     const DeformDesc& d = bd.d;
-    const int tid = threadIdx.x, warp = tid >> 5;
-    const int row = tid & 127;
-    const bool is_m = tid >= 128;
-    const bool issuer = tid == 128;          // TMA copies
-    const bool issue_warp = warp == 4;       // tcgen05.mma: the whole warp arrives converged, one elected lane issues (tc_umma.cuh)
-    const int64_t ntiles = (n + 127) / 128;
-    for (int i = tid; i < (int)(sizeof(DeformDesc) / 4); i += 256)
-        reinterpret_cast<uint32_t*>(&sd)[i] = reinterpret_cast<const uint32_t*>(&d)[i];
+    const int tid = threadIdx.x, wgi = tid >> 7, t128 = tid & 127, lane = tid & 31, g = lane >> 2, t = lane & 3;
+    const int r0 = ((t128 >> 5) << 4) + g, r1 = r0 + 8;          // rows of this lane inside the warpgroup's 64
+    const uint32_t ra = (uint32_t)(wgi * 64 + r0), rb = (uint32_t)(wgi * 64 + r1);   // ... inside the tile's 128
     float* sBias = reinterpret_cast<float*>(smem + Ls.bias);           // b0[128] | b1[5][128]
     float4* sW2s = reinterpret_cast<float4*>(smem + Ls.w2s);           // small heads: (W2[0][j], W2[1][j], W2[2][j], W2[3][j])
-    float* sW2sh = reinterpret_cast<float*>(smem + Ls.w2sh);           // SH head: W2 [48][128] fp32
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Ls.bars);
-    uint64_t *bar_w0 = bars, *bar_w1 = bars + 1 /* [2] */, *bar_l0 = bars + 3, *bar_da1 = bars + 4, *bar_l1 = bars + 5, *bar_g6 = bars + 6;
+    uint64_t *bar_w = bars, *bar_full = bars + 1, *bar_empty = bars + 3;
     const bool hsh = d.head_mask & G4D_HEAD_SHS;
     for (int i = tid; i < 128; i += 256) sBias[i] = __ldg(d.b0 + i);
     for (int h = 0; h < G4D_NUM_HEADS; ++h) {
@@ -229,429 +210,235 @@ deform_tc_bwd_dgrad_kernel(BwdADesc bd, BwdSmemA Ls, float time, int64_t n, cons
             for (int j = tid; j < 128; j += 256)
                 sW2s[h * 128 + j] = make_float4(__ldg(d.w2[h] + j), ko > 1 ? __ldg(d.w2[h] + 128 + j) : 0.f,
                                                ko > 2 ? __ldg(d.w2[h] + 256 + j) : 0.f, ko > 3 ? __ldg(d.w2[h] + 384 + j) : 0.f);
-        } else {
-            for (int i = tid; i < 48 * 128; i += 256) sW2sh[i] = __ldg(d.w2[4] + i);
         }
     }
-    if (warp == 0) tc::tmem_alloc(&tmem_base_s, tc::kTmemCols);
     if (tid == 0) {
-        mbar_init(bar_w0, 1); mbar_init(bar_w1, 1); mbar_init(bar_w1 + 1, 1); mbar_init(bar_l0, 1); mbar_init(bar_da1, 1); mbar_init(bar_l1, 1); mbar_init(bar_g6, 1);
+        mbar_init(bar_w, 1); mbar_init(bar_full, 1); mbar_init(bar_full + 1, 1); mbar_init(bar_empty, 8); mbar_init(bar_empty + 1, 8);
         fence_barrier_init();
     }
-    tc::fence_before_sync();
     __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t tbase = __shfl_sync(0xffffffffu, tmem_base_s, 0);    // warp-uniform for the compiler (MMA operands are uniform registers)
-    const uint32_t lane_base = tbase + ((uint32_t)((warp & 3) * 32) << 16);
-    const uint32_t sW0 = tc::smem_addr(smem + Ls.w0), sW1 = tc::smem_addr(smem + Ls.w1);
-    float amax[3], ascale[3];
-#pragma unroll
-    for (int a = 0; a < 3; ++a) { amax[a] = __ldg(d.aabb + a); ascale[a] = 2.0f / (__ldg(d.aabb + 3 + a) - amax[a]); }
-    int nheads = 0;
-    for (int h = 0; h < G4D_NUM_HEADS; ++h) nheads += (d.head_mask >> h) & 1;
+    const int nheads = __popc(d.head_mask & 31);
+    uint32_t hseq = 0;
+    {
+        int k = 0;
+        for (int h = 0; h < G4D_NUM_HEADS; ++h)
+            if (d.head_mask & (1 << h)) hseq |= (uint32_t)h << (3 * k++);
+    }
     // saved ReLU signs are used when the forward that produced them says so (tag word behind the bits)
     const bool use_bits = bd.relu_bits && __ldg(bd.relu_bits + (size_t)24 * (size_t)n) == 0x5A5A5A5Au;
-    auto load_bits = [&](int slot, int64_t gi, bool valid, uint64_t& lo, uint64_t& hi) {
-        uint4 m = make_uint4(0u, 0u, 0u, 0u);
-        if (valid) m = __ldg(reinterpret_cast<const uint4*>(bd.relu_bits + ((size_t)slot * (size_t)n + (size_t)gi) * 4));
-        lo = (uint64_t)m.x | ((uint64_t)m.y << 32);
-        hi = (uint64_t)m.z | ((uint64_t)m.w << 32);
+    const int64_t ntiles = (n + 127) / 128;
+    const int64_t my_tiles = (int64_t)blockIdx.x < ntiles ? (ntiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
+    const uint32_t total_items = (uint32_t)(my_tiles * nheads);
+    // W1 ring: item u = (tile, head) in consumption order, slot u & 1; thread 0 loads one item ahead
+    auto issue = [&](uint32_t u) {
+        const uint32_t s = u & 1u;
+        if (u >= 2) mbar_wait(bar_empty + s, ((u >> 1) - 1u) & 1u);
+        const int h = (int)((hseq >> (3 * (u % (uint32_t)nheads))) & 7u);
+        mbar_expect_tx(bar_full + s, 2u * kImg128);
+        tma_bulk_g2s(smem + Ls.w1 + s * 2u * kImg128, bd.w.w1[h], 2u * kImg128, bar_full + s);
     };
-
-    // W1 images are double-buffered: the k-th (tile, head) pair this CTA processes uses buffer k & 1; pair k + 2 is loaded
-    // when pair k retires
-    auto load_w1 = [&](int h, int buf) {
-        mbar_expect_tx(bar_w1 + buf, 2u * kImg128);
-        tma_bulk_g2s(smem + Ls.w1 + buf * 2u * kImg128, bd.w.w1[h], 2u * kImg128, bar_w1 + buf);
-    };
-    auto nth_head = [&](int idx) {
-        int m = d.head_mask;
-        for (int i = 0; i < idx; ++i) m &= m - 1;
-        return __ffs(m) - 1;
-    };
-    const int first_h = __ffs(d.head_mask) - 1;
-    const int64_t my_tiles = (ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x;
-    const int64_t total_uses = my_tiles * nheads;
-    if (issuer) {
-        mbar_expect_tx(bar_w0, 2u * 128 * F * 2);
-        tma_bulk_g2s(smem + Ls.w0, bd.w.w0, 2u * 128 * F * 2, bar_w0);
-        load_w1(first_h, 0);
-        if (total_uses > 1) load_w1(nth_head(1 % nheads), 1);
+    if (tid == 0) {
+        const uint32_t w0b = 2u * 128 * F * 2, w2b = hsh ? 2u * 128 * 48 * 2 : 0u;
+        mbar_expect_tx(bar_w, w0b + w2b);
+        tma_bulk_g2s(smem + Ls.w0, bd.w.w0, w0b, bar_w);
+        if (hsh) tma_bulk_g2s(smem + Ls.w2t, bd.w.w2sh, w2b, bar_w);
+        if (total_items) issue(0);
     }
-    if (is_m) mbar_wait(bar_w0, 0);
-    uint32_t ph_w1_0 = 0, ph_w1_1 = 0, ph_l0 = 0, ph_g6 = 0, ph_l1 = 0, ph_da1 = 0;
-    int64_t seq = 0;      // running (tile, head) counter -> W1 buffer
-    // head epilogues are shared: the G group takes column chunks [0, kGChunks), the M group the rest
-    constexpr int kGChunks = 4;
-    const int ch_lo = is_m ? kGChunks : 0, ch_hi = is_m ? 8 : kGChunks;
-
-    // ---- features of a tile: [N][F] fp32 from bwd_features_kernel -> A operand of layer 0 (DZ region) + FEAT image
-    float feat[F];
-    auto load_features = [&](int64_t tl) {
-        const int64_t gs = tl * 128 + row;
-        if (gs < n) {
-            const float4* src = reinterpret_cast<const float4*>(bd.feat + gs * F);
-#pragma unroll
-            for (int c = 0; c < F; c += 4) {
-                const float4 t4 = __ldg(src + (c >> 2));
-                feat[c] = t4.x; feat[c + 1] = t4.y; feat[c + 2] = t4.z; feat[c + 3] = t4.w;
-            }
-        } else {
-#pragma unroll
-            for (int c = 0; c < F; ++c) feat[c] = 0.f;
-        }
+    __syncwarp();
+    mbar_wait(bar_w, 0);
+    const uint32_t sW0 = wg::smem_addr(smem + Ls.w0), sW1 = wg::smem_addr(smem + Ls.w1), sW2t = wg::smem_addr(smem + Ls.w2t);
+    auto load_bits = [&](int slot, int64_t gi, uint32_t (&m)[4]) {
+        uint4 v = make_uint4(0u, 0u, 0u, 0u);
+        if (gi < n) v = __ldg(reinterpret_cast<const uint4*>(bd.relu_bits + ((size_t)slot * (size_t)n + (size_t)gi) * 4));
+        m[0] = v.x; m[1] = v.y; m[2] = v.z; m[3] = v.w;
     };
-    auto write_features = [&](int64_t tl) {
-        uint8_t* img_f = bd.img.feat + (size_t)tl * bd.img.feat_bytes;
-#pragma unroll
-        for (int c0 = 0; c0 < F; c0 += 16) {
-            float x[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) x[j] = feat[c0 + j];
-            Split16 s;
-            split16(x, s);
-            tc::tmem_st8(lane_base + kDZ + (c0 >> 1), s.hi);
-            tc::tmem_st8(lane_base + kDZLo + (c0 >> 1), s.lo);
-            store_img16(img_f, 128u * F * 2u, (uint32_t)F, (uint32_t)row, (uint32_t)c0, s);
-        }
-        tc::wait_st();
-        tc::fence_before_sync();
-        bar_arrive(kBarFeat, 256);
-    };
-    if (!is_m && blockIdx.x < ntiles) {
-        load_features(blockIdx.x);
-        write_features(blockIdx.x);
-    }
+    uint32_t u = 0;
 
-    float acc_b2s[4] = {0.f, 0.f, 0.f, 0.f};   // (M) db2 partial sums of the small heads (butterfly-distributed over lanes)
-    float acc_b2sh[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    const int lane = tid & 31;
-    long long cyc[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-    long long tprev = clock64();
-    const bool prober = bd.dbg && (tid == 128 || tid == 0);
-#define G4D_CYC(i) do { if (prober) { const long long tn_ = clock64(); cyc[(i) + (is_m ? 0 : 6)] += tn_ - tprev; tprev = tn_; } } while (0)
-    for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-        const int64_t gi = tile * 128 + row;
-        const bool valid = gi < n;
-        const bool has_next = tile + gridDim.x < ntiles;
-        auto load_dout = [&](int hh, float (&dst)[48]) {
-#pragma unroll
-            for (int o = 0; o < 48; ++o) dst[o] = 0.f;
-            if (valid && bd.go[hh]) {
-                const int kk = head_out(hh);
-                const float* gp = bd.go[hh] + gi * kk;
-                if (hh == 4) {
-#pragma unroll
-                    for (int o = 0; o < 48; o += 4) {
-                        const float4 t4 = __ldg(reinterpret_cast<const float4*>(gp + o));
-                        dst[o] = t4.x; dst[o + 1] = t4.y; dst[o + 2] = t4.z; dst[o + 3] = t4.w;
-                    }
-                } else {
-#pragma unroll
-                    for (int o = 0; o < 4; ++o)
-                        if (o < kk) dst[o] = __ldg(gp + o);
-                }
-            }
-        };
-        float dn[48];
-        load_dout(first_h, dn);
-        uint64_t hm0 = 0ull, hm1 = 0ull;   // bit j set <=> hidden[j] > 0 (only this thread's own chunks when recomputed)
-        if (use_bits) load_bits(0, gi, valid, hm0, hm1);
-        // ---- layer 0 recompute: D = feat W0^T
-        if (is_m) {
-            bar_sync(kBarFeat, 256);
-            if (issue_warp) {
-                const bool leader = tc::elect_one_sync();
-                tc::fence_after_sync();
-                if (leader) {
-                    gemm_bf16x2_ts<F>(tbase + kD, tbase + kDZ, tbase + kDZLo, sW0, sW0 + 128u * F * 2, 128, F, false, false);
-                    tc::umma_commit(bar_l0);
-                }
-                __syncwarp();
-            }
-        }
-        mbar_wait(bar_l0, ph_l0); ph_l0 ^= 1u;
-        tc::fence_after_sync();
-        G4D_CYC(0);   // wait features + layer 0
+    for (int64_t it = 0; it < my_tiles; ++it) {
+        const int64_t tile = (int64_t)blockIdx.x + it * gridDim.x;
+        const int64_t g0 = tile * 128 + ra, g1 = tile * 128 + rb;
+        float acc[64];
+        // ---- features -> A fragments + FEAT image; layer 0 recompute: D = feat W0^T
         {
-            uint8_t* img_a1 = bd.img.a1 + (size_t)tile * 2 * kImg128;
+            wg::Frags<NS0> x;
+            uint8_t* img = bd.img.feat + (size_t)tile * bd.img.feat_bytes;
+#pragma unroll
+            for (int s = 0; s < NS0; ++s) {
+#pragma unroll
+                for (int hlf = 0; hlf < 2; ++hlf) {
+                    const int c = 16 * s + 8 * hlf + 2 * t;
+                    const float2 p0 = g0 < n ? __ldg(reinterpret_cast<const float2*>(bd.feat + g0 * F + c)) : make_float2(0.f, 0.f);
+                    const float2 p1 = g1 < n ? __ldg(reinterpret_cast<const float2*>(bd.feat + g1 * F + c)) : make_float2(0.f, 0.f);
+                    wg::bf16_split2(p0.x, p0.y, x.hi[s][2 * hlf], x.lo[s][2 * hlf]);
+                    wg::bf16_split2(p1.x, p1.y, x.hi[s][2 * hlf + 1], x.lo[s][2 * hlf + 1]);
+                    const uint32_t w[4] = {x.hi[s][2 * hlf], x.lo[s][2 * hlf], x.hi[s][2 * hlf + 1], x.lo[s][2 * hlf + 1]};
+                    store_words(img, 128u * F * 2u, F, ra, rb, (uint32_t)c, w);
+                }
+            }
+            const uint64_t bh = wg::desc_kmajor(sW0, F, 8), bl = wg::desc_kmajor(sW0 + 128u * F * 2u, F, 8);
+            gemm3_rs<128, NS0, 0>(acc, x, bh, bl, 16, false);
+        }
+        // ---- a1 = relu(h0) -> A fragments + A1 image; hm = sign bits of h0
+        uint32_t hm0[4], hm1[4];
+        wg::Frags<8> a1;
+        {
+            if (use_bits) { load_bits(0, g0, hm0); load_bits(0, g1, hm1); }
+            else {
+#pragma unroll
+                for (int w = 0; w < 4; ++w) { hm0[w] = 0u; hm1[w] = 0u; }
+            }
+            uint8_t* img = bd.img.a1 + (size_t)tile * 2 * kImg128;
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+                const int c = 8 * j + 2 * t;
+                const float x0 = acc[4 * j] + sBias[c], x1 = acc[4 * j + 1] + sBias[c + 1];
+                const float y0 = acc[4 * j + 2] + sBias[c], y1 = acc[4 * j + 3] + sBias[c + 1];
+                bool on[4];
+                if (use_bits) {
+                    on[0] = bit_of(hm0, c); on[1] = bit_of(hm0, c + 1); on[2] = bit_of(hm1, c); on[3] = bit_of(hm1, c + 1);
+                } else {
+                    on[0] = x0 > 0.f; on[1] = x1 > 0.f; on[2] = y0 > 0.f; on[3] = y1 > 0.f;
+                    const int sh = c & 31;
+                    hm0[j >> 2] |= ((on[0] ? 1u : 0u) | (on[1] ? 2u : 0u)) << sh;
+                    hm1[j >> 2] |= ((on[2] ? 1u : 0u) | (on[3] ? 2u : 0u)) << sh;
+                }
+                uint32_t w[4];
+                put16(a1, j, on[0] ? fmaxf(x0, 0.f) : 0.f, on[1] ? fmaxf(x1, 0.f) : 0.f, on[2] ? fmaxf(y0, 0.f) : 0.f,
+                      on[3] ? fmaxf(y1, 0.f) : 0.f, w);
+                store_words(img, kImg128, 128, ra, rb, (uint32_t)c, w);
+            }
+        }
+        float da1[64];
 #pragma unroll 1
-            for (int ch = ch_lo; ch < ch_hi; ++ch) {
-                uint32_t v[16];
-                tc::tmem_ld16(lane_base + kD + ch * 16, v);
-                tc::wait_ld();
-                float a1v[16];
-                uint32_t bits = 0;
+        for (int k = 0; k < nheads; ++k, ++u) {
+            const int h = (int)((hseq >> (3 * k)) & 7u);
+            const float* b1 = sBias + 128 + h * 128;
+            if (tid == 0 && u + 1 < total_items) issue(u + 1);
+            __syncwarp();
+            const uint32_t slot = u & 1u;
+            mbar_wait(bar_full + slot, (u >> 1) & 1u);
+            const uint32_t w1 = sW1 + slot * 2u * kImg128;
+            // ---- z = a1 W1^T
+            gemm3_rs<128, 8, 0>(acc, a1, wg::desc_kmajor(w1, 128, 8), wg::desc_kmajor(w1 + kImg128, 128, 8), 16, false);
+            uint32_t zm0[4], zm1[4];
+            if (use_bits) { load_bits(1 + h, g0, zm0); load_bits(1 + h, g1, zm1); }
+            // ---- a2 = relu(z) (A2 image); masks; dL/d(out) rows (DOUT image)
+            uint8_t* img_a2 = bd.img.a2[h] + (size_t)tile * 2 * kImg128;
+            const float* go = bd.go[h];
+            float dn0[4] = {0.f, 0.f, 0.f, 0.f}, dn1[4] = {0.f, 0.f, 0.f, 0.f};
+            uint64_t onm = 0ull;   // bit 4 j + q: ReLU of value q (x0, x1, y0, y1) of accumulator block j is on
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+                const int c = 8 * j + 2 * t;
+                const float x0 = acc[4 * j] + b1[c], x1 = acc[4 * j + 1] + b1[c + 1];
+                const float y0 = acc[4 * j + 2] + b1[c], y1 = acc[4 * j + 3] + b1[c + 1];
+                bool on[4];
+                if (use_bits) {
+                    on[0] = bit_of(zm0, c); on[1] = bit_of(zm0, c + 1); on[2] = bit_of(zm1, c); on[3] = bit_of(zm1, c + 1);
+                } else {
+                    on[0] = x0 > 0.f; on[1] = x1 > 0.f; on[2] = y0 > 0.f; on[3] = y1 > 0.f;
+                }
+                onm |= (uint64_t)((on[0] ? 1u : 0u) | (on[1] ? 2u : 0u) | (on[2] ? 4u : 0u) | (on[3] ? 8u : 0u)) << (4 * j);
+                uint32_t w[4];
+                wg::bf16_split2(on[0] ? fmaxf(x0, 0.f) : 0.f, on[1] ? fmaxf(x1, 0.f) : 0.f, w[0], w[1]);
+                wg::bf16_split2(on[2] ? fmaxf(y0, 0.f) : 0.f, on[3] ? fmaxf(y1, 0.f) : 0.f, w[2], w[3]);
+                store_words(img_a2, kImg128, 128, ra, rb, (uint32_t)c, w);
+            }
+            auto on_bit = [&](int j, int q) { return ((onm >> (4 * j + q)) & 1ull) != 0ull; };
+            uint8_t* img_do = bd.img.dout[h] + (size_t)tile * 2 * 128 * (h == 4 ? 48 : 16) * 2;
+            if (h < 4) {
+                const int ko = head_out(h);
+#pragma unroll
+                for (int o = 0; o < 4; ++o) {
+                    if (o < ko && go) {
+                        if (g0 < n) dn0[o] = __ldg(go + g0 * ko + o);
+                        if (g1 < n) dn1[o] = __ldg(go + g1 * ko + o);
+                    }
+                }
+                // DOUT image [128][16]: lane t writes columns 2t, 2t + 1 and 8 + 2t, 9 + 2t (zero beyond the head's outputs)
+                {
+                    uint32_t w[4];
+                    const float e0 = t == 0 ? dn0[0] : t == 1 ? dn0[2] : 0.f, e1 = t == 0 ? dn0[1] : t == 1 ? dn0[3] : 0.f;
+                    const float f0 = t == 0 ? dn1[0] : t == 1 ? dn1[2] : 0.f, f1 = t == 0 ? dn1[1] : t == 1 ? dn1[3] : 0.f;
+                    wg::bf16_split2(e0, e1, w[0], w[1]);
+                    wg::bf16_split2(f0, f1, w[2], w[3]);
+                    store_words(img_do, 128u * 16u * 2u, 16, ra, rb, (uint32_t)(2 * t), w);
+                    const uint32_t z[4] = {0u, 0u, 0u, 0u};
+                    store_words(img_do, 128u * 16u * 2u, 16, ra, rb, (uint32_t)(8 + 2 * t), z);
+                }
+                // dz = (dout W2) * [z > 0], in place of z
 #pragma unroll
                 for (int j = 0; j < 16; ++j) {
-                    const float hpre = __uint_as_float(v[j]) + sBias[ch * 16 + j];
-                    if (hpre > 0.f) bits |= 1u << j;
-                    a1v[j] = fmaxf(hpre, 0.f);
+                    const int c = 8 * j + 2 * t;
+                    const float4 wa = sW2s[h * 128 + c], wb = sW2s[h * 128 + c + 1];
+                    const float da_x0 = dn0[0] * wa.x + dn0[1] * wa.y + dn0[2] * wa.z + dn0[3] * wa.w;
+                    const float da_x1 = dn0[0] * wb.x + dn0[1] * wb.y + dn0[2] * wb.z + dn0[3] * wb.w;
+                    const float da_y0 = dn1[0] * wa.x + dn1[1] * wa.y + dn1[2] * wa.z + dn1[3] * wa.w;
+                    const float da_y1 = dn1[0] * wb.x + dn1[1] * wb.y + dn1[2] * wb.z + dn1[3] * wb.w;
+                    acc[4 * j] = on_bit(j, 0) ? da_x0 : 0.f; acc[4 * j + 1] = on_bit(j, 1) ? da_x1 : 0.f;
+                    acc[4 * j + 2] = on_bit(j, 2) ? da_y0 : 0.f; acc[4 * j + 3] = on_bit(j, 3) ? da_y1 : 0.f;
                 }
-                if (use_bits) {
-                    const uint32_t sb = (uint32_t)((ch < 4 ? hm0 : hm1) >> ((ch & 3) * 16)) & 0xffffu;
+            } else {
+                // SH head: d(a2) = dout W2 as a GEMM (K = 48: dout rows as A fragments, W2^T image as B), DOUT image on the way
+                wg::Frags<3> x;
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) a1v[j] = ((sb >> j) & 1u) ? a1v[j] : 0.f;
-                } else if (ch < 4) hm0 |= (uint64_t)bits << (ch * 16);
-                else hm1 |= (uint64_t)bits << ((ch - 4) * 16);
-                Split16 s;
-                split16(a1v, s);
-                tc::tmem_st8(lane_base + kA1 + ch * 8, s.hi);
-                tc::tmem_st8(lane_base + kA1Lo + ch * 8, s.lo);
-                store_img16(img_a1, kImg128, 128, (uint32_t)row, (uint32_t)(ch * 16), s);
-            }
-            tc::wait_st();
-            tc::fence_before_sync();
-            G4D_CYC(1);   // epilogue 0 (+ dh epilogue below)
-            bar_sync(kBarE, 256);
-            G4D_CYC(4);   // wait for the other group
-        }
-        if (is_m) {
-            // ---- first layer-1 GEMM of the tile
-            const int buf = (int)(seq & 1);
-            if (buf == 0) { mbar_wait(bar_w1, ph_w1_0); ph_w1_0 ^= 1u; } else { mbar_wait(bar_w1 + 1, ph_w1_1); ph_w1_1 ^= 1u; }
-            if (issue_warp) {
-                const bool leader = tc::elect_one_sync();
-                tc::fence_after_sync();
-                const uint32_t w = sW1 + buf * 2u * kImg128;
-                if (leader) {
-                    gemm_bf16x2_ts<128>(tbase + kD, tbase + kA1, tbase + kA1Lo, w, w + kImg128, 128, 128, false, false);
-                    tc::umma_commit(bar_l1);
+                for (int s = 0; s < 3; ++s) {
+#pragma unroll
+                    for (int hlf = 0; hlf < 2; ++hlf) {
+                        const int c = 16 * s + 8 * hlf + 2 * t;
+                        float2 p0 = make_float2(0.f, 0.f), p1 = p0;
+                        if (go && g0 < n) p0 = __ldg(reinterpret_cast<const float2*>(go + g0 * 48 + c));
+                        if (go && g1 < n) p1 = __ldg(reinterpret_cast<const float2*>(go + g1 * 48 + c));
+                        wg::bf16_split2(p0.x, p0.y, x.hi[s][2 * hlf], x.lo[s][2 * hlf]);
+                        wg::bf16_split2(p1.x, p1.y, x.hi[s][2 * hlf + 1], x.lo[s][2 * hlf + 1]);
+                        const uint32_t w[4] = {x.hi[s][2 * hlf], x.lo[s][2 * hlf], x.hi[s][2 * hlf + 1], x.lo[s][2 * hlf + 1]};
+                        store_words(img_do, 128u * 48u * 2u, 48, ra, rb, (uint32_t)c, w);
+                    }
                 }
-                __syncwarp();
+                gemm3_rs<128, 3, 0>(acc, x, wg::desc_kmajor(sW2t, 48, 8), wg::desc_kmajor(sW2t + 128u * 48u * 2u, 48, 8), 16, false);
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+                    acc[4 * j] = on_bit(j, 0) ? acc[4 * j] : 0.f; acc[4 * j + 1] = on_bit(j, 1) ? acc[4 * j + 1] : 0.f;
+                    acc[4 * j + 2] = on_bit(j, 2) ? acc[4 * j + 2] : 0.f; acc[4 * j + 3] = on_bit(j, 3) ? acc[4 * j + 3] : 0.f;
+                }
             }
-        }
-
-        // ================= heads: both groups, column chunks split =================
-        bool da1_started = false;
-        int h = first_h;
-#pragma unroll 1
-        for (int hc = 0; hc < nheads; ++hc) {
-            const int buf = (int)(seq & 1);
-            const float* b1 = sBias + 128 + h * 128;
-            int next_h = -1;
+            // ---- DZ image + A fragments; d(a1) += dz W1 (W1 image read MN-major)
             {
-                const int later = d.head_mask >> (h + 1);
-                if (later) next_h = h + 1 + (__ffs(later) - 1);
-            }
-            // my row of dL/d(out_h): fetched one head ahead (the loads fly during the previous head's epilogue)
-            float dout[48];
+                wg::Frags<8> dz;
+                uint8_t* img = bd.img.dz[h] + (size_t)tile * 2 * kImg128;
 #pragma unroll
-            for (int o = 0; o < 48; ++o) dout[o] = dn[o];
-            if (next_h >= 0) load_dout(next_h, dn);
-            if (is_m) {
-                // DOUT image (operand of dW2)
-                const uint32_t kp16 = (h == 4) ? 48u : 16u;
-                uint8_t* img = bd.img.dout[h] + (size_t)tile * 2 * 128 * kp16 * 2;
-#pragma unroll
-                for (int c0 = 0; c0 < 48; c0 += 16) {
-                    if (c0 > 0 && h != 4) break;
-                    float x[16];
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) x[j] = dout[c0 + j];
-                    Split16 s;
-                    split16(x, s);
-                    store_img16(img, 128u * kp16 * 2u, kp16, (uint32_t)row, (uint32_t)c0, s);
+                for (int j = 0; j < 16; ++j) {
+                    uint32_t w[4];
+                    put16(dz, j, acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3], w);
+                    store_words(img, kImg128, 128, ra, rb, (uint32_t)(8 * j + 2 * t), w);
                 }
-                // db2: transposing butterfly over the warp, partial sums stay distributed over the lanes until the end
-                if (h == 4) {
-                    float t[48];
-#pragma unroll
-                    for (int o = 0; o < 48; ++o) t[o] = dout[o];
-                    halve<48>(t, lane & 16, 16); halve<24>(t, lane & 8, 8); halve<12>(t, lane & 4, 4);
-#pragma unroll
-                    for (int k = 0; k < 6; ++k) acc_b2sh[k] += t[k];
-                } else {
-                    float t[4] = {dout[0], dout[1], dout[2], dout[3]};
-                    halve<4>(t, lane & 16, 16); halve<2>(t, lane & 8, 8);
-                    if (h == 0) acc_b2s[0] += t[0]; else if (h == 1) acc_b2s[1] += t[0];
-                    else if (h == 2) acc_b2s[2] += t[0]; else acc_b2s[3] += t[0];
-                }
+                gemm3_rs<128, 8, 1>(da1, dz, wg::desc_mnmajor(w1, 128), wg::desc_mnmajor(w1 + kImg128, 128), (2u * 16u * 128u) >> 4, k > 0);
             }
-            uint64_t zm0 = 0ull, zm1 = 0ull;
-            if (use_bits) load_bits(1 + h, gi, valid, zm0, zm1);
-            G4D_CYC(2);   // dout / DOUT image / db2
-            // ---- wait for z = a1 W1^T
-            mbar_wait(bar_l1, ph_l1); ph_l1 ^= 1u;
-            tc::fence_after_sync();
-            G4D_CYC(5);   // MMA waits
-            uint8_t* img_a2 = bd.img.a2[h] + (size_t)tile * 2 * kImg128;
-            uint8_t* img_dz = bd.img.dz[h] + (size_t)tile * 2 * kImg128;
-#pragma unroll 1
-            for (int ch = ch_lo; ch < ch_hi; ++ch) {
-                uint32_t v[16];
-                tc::tmem_ld16(lane_base + kD + ch * 16, v);
-                tc::wait_ld();
-                float a2v[16], dzv[16];
-                const uint32_t sb = (uint32_t)((ch < 4 ? zm0 : zm1) >> ((ch & 3) * 16)) & 0xffffu;
-                if (h < 4) {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const float zc = __uint_as_float(v[j]) + b1[ch * 16 + j];
-                        const float4 w = sW2s[h * 128 + ch * 16 + j];
-                        const float da2 = dout[0] * w.x + dout[1] * w.y + dout[2] * w.z + dout[3] * w.w;
-                        const bool on = use_bits ? ((sb >> j) & 1u) != 0u : zc > 0.f;
-                        a2v[j] = on ? fmaxf(zc, 0.f) : 0.f;
-                        dzv[j] = on ? da2 : 0.f;
-                    }
-                } else {
-                    float da2[16];
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) da2[j] = 0.f;
-#pragma unroll 4
-                    for (int o = 0; o < 48; ++o) {
-                        const float* wr = sW2sh + o * 128 + ch * 16;
-#pragma unroll
-                        for (int j = 0; j < 16; j += 4) {
-                            const float4 w = *reinterpret_cast<const float4*>(wr + j);
-                            da2[j] = fmaf(dout[o], w.x, da2[j]); da2[j + 1] = fmaf(dout[o], w.y, da2[j + 1]);
-                            da2[j + 2] = fmaf(dout[o], w.z, da2[j + 2]); da2[j + 3] = fmaf(dout[o], w.w, da2[j + 3]);
-                        }
-                    }
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const float zc = __uint_as_float(v[j]) + b1[ch * 16 + j];
-                        const bool on = use_bits ? ((sb >> j) & 1u) != 0u : zc > 0.f;
-                        a2v[j] = on ? fmaxf(zc, 0.f) : 0.f;
-                        dzv[j] = on ? da2[j] : 0.f;
-                    }
-                }
-                Split16 s;
-                split16(a2v, s);
-                store_img16(img_a2, kImg128, 128, (uint32_t)row, (uint32_t)(ch * 16), s);
-                split16(dzv, s);
-                store_img16(img_dz, kImg128, 128, (uint32_t)row, (uint32_t)(ch * 16), s);
-                tc::tmem_st8(lane_base + kDZ + ch * 8, s.hi);
-                tc::tmem_st8(lane_base + kDZLo + ch * 8, s.lo);
-            }
-            tc::wait_st();
-            tc::fence_before_sync();
-            G4D_CYC(3);   // head epilogue (my chunks)
-            bar_sync(kBarE, 256);
-            G4D_CYC(4);   // wait for the other group
-            // ---- d(a1) += dz W1 (W1 image read MN-major), then the next head's layer 1 straight behind it
-            if (issue_warp) {
-                const bool leader = tc::elect_one_sync();
-                tc::fence_after_sync();
-                const uint32_t w = sW1 + buf * 2u * kImg128;
-                if (leader) {
-                    gemm_bf16x2_ts<128>(tbase + kDA1, tbase + kDZ, tbase + kDZLo, w, w + kImg128, 128, 128, true, da1_started);
-                    tc::umma_commit(bar_da1);
-                }
-                __syncwarp();
-            }
-            da1_started = true;
-            ++seq;
-            if (next_h >= 0 && is_m) {
-                const int nbuf = (int)(seq & 1);
-                if (nbuf == 0) { mbar_wait(bar_w1, ph_w1_0); ph_w1_0 ^= 1u; } else { mbar_wait(bar_w1 + 1, ph_w1_1); ph_w1_1 ^= 1u; }
-                if (issue_warp) {
-                    const bool leader = tc::elect_one_sync();
-                    const uint32_t w = sW1 + nbuf * 2u * kImg128;
-                    if (leader) {
-                        gemm_bf16x2_ts<128>(tbase + kD, tbase + kA1, tbase + kA1Lo, w, w + kImg128, 128, 128, false, false);
-                        tc::umma_commit(bar_l1);
-                    }
-                    __syncwarp();
-                }
-            }
-            // the dz W1 chain has retired: DZ may be overwritten, and W1 buffer `buf` takes the pair after next
-            mbar_wait(bar_da1, ph_da1); ph_da1 ^= 1u;
-            tc::fence_after_sync();
-            if (issuer && seq + 1 < total_uses) load_w1(nth_head((int)((seq + 1) % nheads)), buf);
-            h = next_h;
-            G4D_CYC(5);   // MMA waits
+            if (lane == 0) mbar_arrive1(bar_empty + slot);      // this warp's MMAs on the slot have retired
         }
 
-        // ---- dh = d(a1) * (hidden > 0) -> A operand (DZ region) + DH image
+        // ---- dh = d(a1) * [h0 > 0] -> A fragments + DH image; d(feat) = dh W0 (W0 image read MN-major) -> [N][F] fp32
         {
-            uint8_t* img_dh = bd.img.dh + (size_t)tile * 2 * kImg128;
-#pragma unroll 1
-            for (int ch = ch_lo; ch < ch_hi; ++ch) {
-                uint32_t v[16];
-                tc::tmem_ld16(lane_base + kDA1 + ch * 16, v);
-                tc::wait_ld();
-                float dh[16];
-                const uint32_t bits = (uint32_t)((ch < 4 ? hm0 : hm1) >> ((ch & 3) * 16)) & 0xffffu;
+            wg::Frags<8> dh;
+            uint8_t* img = bd.img.dh + (size_t)tile * 2 * kImg128;
 #pragma unroll
-                for (int j = 0; j < 16; ++j) dh[j] = ((bits >> j) & 1u) ? __uint_as_float(v[j]) : 0.f;
-                Split16 s;
-                split16(dh, s);
-                store_img16(img_dh, kImg128, 128, (uint32_t)row, (uint32_t)(ch * 16), s);
-                tc::tmem_st8(lane_base + kDZ + ch * 8, s.hi);
-                tc::tmem_st8(lane_base + kDZLo + ch * 8, s.lo);
+            for (int j = 0; j < 16; ++j) {
+                const int c = 8 * j + 2 * t;
+                uint32_t w[4];
+                put16(dh, j, bit_of(hm0, c) ? da1[4 * j] : 0.f, bit_of(hm0, c + 1) ? da1[4 * j + 1] : 0.f,
+                      bit_of(hm1, c) ? da1[4 * j + 2] : 0.f, bit_of(hm1, c + 1) ? da1[4 * j + 3] : 0.f, w);
+                store_words(img, kImg128, 128, ra, rb, (uint32_t)c, w);
             }
-            tc::wait_st();
-            tc::fence_before_sync();
-            G4D_CYC(1);
-            bar_sync(kBarE, 256);
-            G4D_CYC(4);
-        }
-        if (is_m) {
-            // ---- d(feat) = dh W0  (W0 image read MN-major: rows = hidden j = K, cols = feature f = N) -> [N][F] fp32
-            if (issue_warp) {
-                const bool leader = tc::elect_one_sync();
-                tc::fence_after_sync();
-                if (leader) {
-                    gemm_bf16x2_ts<128>(tbase + kD, tbase + kDZ, tbase + kDZLo, sW0, sW0 + 128u * F * 2, F, F, true, false);
-                    tc::umma_commit(bar_g6);
-                }
-                __syncwarp();
-            }
-            mbar_wait(bar_g6, ph_g6); ph_g6 ^= 1u;
-            tc::fence_after_sync();
-            if (has_next) bar_arrive(kBarXFree, 256);   // the DZ region (next tile's feature operand) is free
+            float df[F / 2];
+            gemm3_rs<F, 8, 1>(df, dh, wg::desc_mnmajor(sW0, F), wg::desc_mnmajor(sW0 + 128u * F * 2u, F), (2u * (F / 8) * 128u) >> 4, false);
 #pragma unroll
-            for (int c0 = 0; c0 < F; c0 += 16) {
-                uint32_t v[16];
-                tc::tmem_ld16(lane_base + kD + c0, v);
-                tc::wait_ld();
-                if (valid) {
-                    float4* dst = reinterpret_cast<float4*>(bd.dfeat + gi * F + c0);
-#pragma unroll
-                    for (int q = 0; q < 4; ++q)
-                        dst[q] = make_float4(__uint_as_float(v[4 * q]), __uint_as_float(v[4 * q + 1]), __uint_as_float(v[4 * q + 2]),
-                                             __uint_as_float(v[4 * q + 3]));
-                }
-            }
-            tc::fence_before_sync();
-            G4D_CYC(5);
-        } else if (has_next) {
-            load_features(tile + gridDim.x);
-            bar_sync(kBarXFree, 256);
-            tc::fence_after_sync();
-            write_features(tile + gridDim.x);
-            G4D_CYC(5);
-        }
-    }
-    if (is_m) {
-        // db2 flush: finish the butterflies (remaining lane bits) and add once per warp
-#pragma unroll
-        for (int hh = 0; hh < 4; ++hh) {
-            float x = acc_b2s[hh];
-            x += __shfl_xor_sync(0xffffffffu, x, 4); x += __shfl_xor_sync(0xffffffffu, x, 2); x += __shfl_xor_sync(0xffffffffu, x, 1);
-            const int idx = ((lane >> 4) & 1) * 2 + ((lane >> 3) & 1);
-            if ((d.head_mask & (1 << hh)) && (lane & 7) == 0 && idx < head_out(hh)) atomicAdd(bd.g_b2[hh] + idx, x);
-        }
-        if (d.head_mask & G4D_HEAD_SHS) {
-#pragma unroll
-            for (int k = 0; k < 6; ++k) {
-                float x = acc_b2sh[k];
-                x += __shfl_xor_sync(0xffffffffu, x, 2); x += __shfl_xor_sync(0xffffffffu, x, 1);
-                const int idx = ((lane >> 4) & 1) * 24 + ((lane >> 3) & 1) * 12 + ((lane >> 2) & 1) * 6 + k;
-                if ((lane & 3) == 0) atomicAdd(bd.g_b2[4] + idx, x);
+            for (int j = 0; j < F / 8; ++j) {
+                const int c = 8 * j + 2 * t;
+                if (g0 < n) *reinterpret_cast<float2*>(bd.dfeat + g0 * F + c) = make_float2(df[4 * j], df[4 * j + 1]);
+                if (g1 < n) *reinterpret_cast<float2*>(bd.dfeat + g1 * F + c) = make_float2(df[4 * j + 2], df[4 * j + 3]);
             }
         }
     }
-    if (prober) {
-        // slots (M: 0..5, G: 6..11): 0 wait features + layer 0, 1 epilogue 0 + dh epilogue, 2 dout/DOUT/db2, 3 head epilogues,
-        //                           4 waiting for the other group, 5 MMA waits + tile tail
-        for (int i = 0; i < 6; ++i) bd.dbg[blockIdx.x * 12 + i + (is_m ? 0 : 6)] = cyc[i + (is_m ? 0 : 6)];
-    }
-#undef G4D_CYC
-    tc::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc(tbase, tc::kTmemCols);
 }
 
 // ---- HexPlane gather / scatter at full occupancy (C/4 threads per Gaussian, one channel vector each) ---------------
@@ -752,21 +539,121 @@ __global__ void __launch_bounds__(256, 2) bwd_scatter_kernel(BwdScatterDesc sd, 
 
 // ======================================================================================================
 // Kernel B: weight gradients from the operand images.
-//   CTA (group, chunk): group 0..4 = head, group 5 = layer 0.  128 threads; thread 0 streams + issues, all read out.
+//   CTA (group, chunk): group = an active head or layer 0.  Two warpgroups, warpgroup w accumulates output rows
+//   [64 w, 64 w + 64) (hidden units j); thread 0 streams the stages.
 // ======================================================================================================
 struct BwdBDesc {
     BwdImages img;
     int head_mask, F, nheads, chunks_head, chunks_l0;
     int64_t ntiles;
     float* g_w0; float* g_b0;
-    float* g_w1[G4D_NUM_HEADS]; float* g_b1[G4D_NUM_HEADS]; float* g_w2[G4D_NUM_HEADS];
+    float* g_w1[G4D_NUM_HEADS]; float* g_b1[G4D_NUM_HEADS]; float* g_w2[G4D_NUM_HEADS]; float* g_b2[G4D_NUM_HEADS];
 };
 
-__global__ void __launch_bounds__(128, 1) deform_tc_bwd_wgrad_kernel(BwdBDesc b) {
+constexpr uint32_t kHalf128 = kImg128 / 2;                          // 16 KB: 64 rows x 128 cols bf16
+constexpr uint32_t kStage = 3u * 2u * kHalf128 + 2u * 64 * 48 * 2;   // 108 KB: X | Y | A2 | DOUT, each (hi half | lo half)
+constexpr uint32_t kOnes = 64u * 64u * 2u;                           // all-ones bf16 operand
+
+// NW = columns of dW (128, or F for layer 0); KP = columns of the DOUT image (16 for the small heads, 48 for the SH head, 0 for
+// layer 0)
+template <int NW, int KP>
+__device__ __forceinline__ void wgrad_group(const BwdBDesc& b, int h, int64_t t0, int64_t t1, uint8_t* smem, uint64_t* bar_ld) {
+    constexpr bool layer0 = KP == 0;
+    constexpr int NW2 = KP > 0 ? KP : 8;
+    const int tid = threadIdx.x, wgi = tid >> 7, t128 = tid & 127, lane = tid & 31, g = lane >> 2, t = lane & 3;
+    const int kp16 = KP;
+    const uint32_t yp = layer0 ? 128u * NW * 2u : kImg128;             // bytes of one part (hi or lo) of Y
+    const uint32_t dp = 128u * kp16 * 2u;                              // ... of DOUT
+    const int64_t nwork = t1 > t0 ? 2 * (t1 - t0) : 0;
+    // work item w = 2 (t - t0) + hf: rows [64 hf, 64 hf + 64) of tile t; the images are row-group major, so that half of a
+    // part is one contiguous half of its bytes
+    auto load = [&](int64_t w) {
+        const int st = (int)(w & 1), hf = (int)(w & 1);
+        const int64_t tl = t0 + (w >> 1);
+        uint8_t* base = smem + st * kStage;
+        uint8_t *dX = base, *dY = base + 2 * kHalf128, *dA2 = base + 4 * kHalf128, *dDO = base + 6 * kHalf128;
+        const uint8_t* srcX = (layer0 ? b.img.dh : b.img.dz[h]) + (size_t)tl * 2 * kImg128;
+        const uint8_t* srcY = layer0 ? b.img.feat + (size_t)tl * b.img.feat_bytes : b.img.a1 + (size_t)tl * 2 * kImg128;
+        const uint32_t bytes = 2u * kHalf128 + yp + (layer0 ? 0u : 2u * kHalf128 + dp);
+        mbar_expect_tx(&bar_ld[st], bytes);
+        tma_bulk_g2s(dX, srcX + hf * kHalf128, kHalf128, &bar_ld[st]);
+        tma_bulk_g2s(dX + kHalf128, srcX + kImg128 + hf * kHalf128, kHalf128, &bar_ld[st]);
+        tma_bulk_g2s(dY, srcY + hf * (yp / 2), yp / 2, &bar_ld[st]);
+        tma_bulk_g2s(dY + yp / 2, srcY + yp + hf * (yp / 2), yp / 2, &bar_ld[st]);
+        if (!layer0) {
+            const uint8_t* srcA = b.img.a2[h] + (size_t)tl * 2 * kImg128;
+            const uint8_t* srcD = b.img.dout[h] + (size_t)tl * 2 * dp;
+            tma_bulk_g2s(dA2, srcA + hf * kHalf128, kHalf128, &bar_ld[st]);
+            tma_bulk_g2s(dA2 + kHalf128, srcA + kImg128 + hf * kHalf128, kHalf128, &bar_ld[st]);
+            tma_bulk_g2s(dDO, srcD + hf * (dp / 2), dp / 2, &bar_ld[st]);
+            tma_bulk_g2s(dDO + dp / 2, srcD + dp + hf * (dp / 2), dp / 2, &bar_ld[st]);
+        }
+    };
+    float accW[NW / 2], accW2[NW2 / 2], accB[4], accB2[NW2 / 2];
+    if (tid == 0) {
+        if (nwork > 0) load(0);
+        if (nwork > 1) load(1);
+    }
+    const uint32_t ones = wg::smem_addr(smem + 2 * kStage);
+    // all-ones operands: B of the bias sums ([64 Gaussians][8], MN-major) and A of db2 ([64][64 Gaussians], K-major)
+    const uint64_t ones_b = wg::desc_mnmajor(ones, 8), ones_a = wg::desc_kmajor(ones, 64, 8);
+    // MN-major operand images of 64 rows (Gaussians = K): one K = 16 step is two rows of core matrices
+    const uint32_t step128 = (2u * 16u * 128u) >> 4;
+    const uint32_t a_off = (uint32_t)wgi * 64u * 16u;                  // this warpgroup's 64 output rows (M) inside X / A2
+    for (int64_t w = 0; w < nwork; ++w) {
+        const int st = (int)(w & 1);
+        mbar_wait(&bar_ld[st], (uint32_t)(w >> 1) & 1u);
+        const uint32_t base = wg::smem_addr(smem + st * kStage);
+        const uint32_t x = base, y = base + 2 * kHalf128, a2 = base + 4 * kHalf128, dd = base + 6 * kHalf128;
+        const bool acc = w > 0;
+        const uint64_t xh = wg::desc_mnmajor(x + a_off, 128), xl = wg::desc_mnmajor(x + kHalf128 + a_off, 128);
+        if constexpr (layer0) {
+            gemm3_ss<NW, 1, 1>(accW, xh, xl, step128, wg::desc_mnmajor(y, NW), wg::desc_mnmajor(y + yp / 2, NW), (2u * (NW / 8) * 128u) >> 4,
+                               acc, false, false);
+        } else {
+            gemm3_ss<NW, 1, 1>(accW, xh, xl, step128, wg::desc_mnmajor(y, 128), wg::desc_mnmajor(y + kHalf128, 128), step128, acc, false, false);
+            const uint64_t ah = wg::desc_mnmajor(a2 + a_off, 128), al = wg::desc_mnmajor(a2 + kHalf128 + a_off, 128);
+            const uint64_t dh = wg::desc_mnmajor(dd, (uint32_t)kp16), dl = wg::desc_mnmajor(dd + dp / 2, (uint32_t)kp16);
+            const uint32_t dstep = (2u * (uint32_t)(kp16 / 8) * 128u) >> 4;
+            gemm3_ss<NW2, 1, 1>(accW2, ah, al, step128, dh, dl, dstep, acc, false, false);
+            if (wgi == 0) gemm3_ss<NW2, 0, 1>(accB2, ones_a, ones_a, 16, dh, dl, dstep, acc, true, false);
+        }
+        gemm3_ss<8, 1, 1>(accB, xh, xl, step128, ones_b, ones_b, 16, acc, false, true);
+        __syncthreads();                                  // both warpgroups are done with stage st
+        if (tid == 0 && w + 2 < nwork) load(w + 2);
+    }
+    if (nwork == 0) return;
+    // ---- flush: thread rows j0 = 64 wgi + 16 warp + g and j0 + 8 of every accumulator
+    const int j0 = wgi * 64 + ((t128 >> 5) << 4) + g, j1 = j0 + 8;
+    float* gw = layer0 ? b.g_w0 : b.g_w1[h];
+#pragma unroll
+    for (int q = 0; q < NW / 8; ++q) {
+        const int c = 8 * q + 2 * t;
+        atomicAdd(gw + (size_t)j0 * NW + c, accW[4 * q]); atomicAdd(gw + (size_t)j0 * NW + c + 1, accW[4 * q + 1]);
+        atomicAdd(gw + (size_t)j1 * NW + c, accW[4 * q + 2]); atomicAdd(gw + (size_t)j1 * NW + c + 1, accW[4 * q + 3]);
+    }
+    float* gb = layer0 ? b.g_b0 : b.g_b1[h];
+    if (t == 0) { atomicAdd(gb + j0, accB[0]); atomicAdd(gb + j1, accB[2]); }    // (every column of the ones product is the sum)
+    if constexpr (!layer0) {
+        const int ko = head_out(h);
+#pragma unroll
+        for (int q = 0; q < NW2 / 8; ++q) {
+            const int c = 8 * q + 2 * t;
+            if (c < ko) { atomicAdd(b.g_w2[h] + (size_t)c * 128 + j0, accW2[4 * q]); atomicAdd(b.g_w2[h] + (size_t)c * 128 + j1, accW2[4 * q + 2]); }
+            if (c + 1 < ko) { atomicAdd(b.g_w2[h] + (size_t)(c + 1) * 128 + j0, accW2[4 * q + 1]); atomicAdd(b.g_w2[h] + (size_t)(c + 1) * 128 + j1, accW2[4 * q + 3]); }
+            // db2: every row of 1^T DOUT is the same sum -- warpgroup 0, row 0 (lanes 0-3 of warp 0) flushes it
+            if (wgi == 0 && tid < 4) {
+                if (c < ko) atomicAdd(b.g_b2[h] + c, accB2[4 * q]);
+                if (c + 1 < ko) atomicAdd(b.g_b2[h] + c + 1, accB2[4 * q + 1]);
+            }
+        }
+    }
+}
+
+__global__ void __launch_bounds__(256, 1) deform_tc_bwd_wgrad_kernel(BwdBDesc b) {
     extern __shared__ __align__(1024) uint8_t smem[];
-    __shared__ uint32_t tmem_base_s;
-    __shared__ __align__(8) uint64_t bar_ld[2], bar_mma[2], bar_done;
-    const int tid = threadIdx.x, warp = tid >> 5;
+    __shared__ __align__(8) uint64_t bar_ld[2];
+    const int tid = threadIdx.x;
     // CTAs [0, nheads * chunks_head) serve the active heads, the rest layer 0 (CTA counts proportional to the bytes per tile)
     const bool layer0 = (int)blockIdx.x >= b.nheads * b.chunks_head;
     const int chunk = layer0 ? (int)blockIdx.x - b.nheads * b.chunks_head : (int)blockIdx.x % b.chunks_head;
@@ -777,129 +664,22 @@ __global__ void __launch_bounds__(128, 1) deform_tc_bwd_wgrad_kernel(BwdBDesc b)
         for (int i = 0; i < (int)blockIdx.x / b.chunks_head; ++i) m &= m - 1;
         h = __ffs(m) - 1;
     }
-    const int kp16 = (h == 4) ? 48 : 16;
-    // Two pipeline stages of HALF a tile each (64 Gaussians = the K extent of one MMA chain): the images are row-group major,
-    // so rows [64 hf, 64 hf + 64) of a part are one contiguous half of its bytes.  While the tensor core chews on one stage the
-    // TMA fills the other.  Per stage: X (DZ_h or DH) | Y (A1 or FEAT) | A2_h | DOUT_h, each as (hi half | lo half).
-    constexpr uint32_t kHalf128 = kImg128 / 2;                       // 16 KB: 64 rows x 128 cols bf16
-    constexpr uint32_t kStage = 3u * 2u * kHalf128 + 2u * 64 * 48 * 2;   // 108 KB
-    uint8_t* sOnes = smem + 2 * kStage;
-    // ones image [64 g][16]: bf16 1.0 = 0x3F80
-    for (int i = tid; i < 64 * 16; i += 128) reinterpret_cast<uint16_t*>(sOnes)[i] = 0x3F80;
-    if (warp == 0) tc::tmem_alloc(&tmem_base_s, tc::kTmemCols);
+    uint16_t* ones = reinterpret_cast<uint16_t*>(smem + 2 * kStage);
+    for (int i = tid; i < (int)(kOnes / 2); i += 256) ones[i] = 0x3F80;     // bf16 1.0
     if (tid == 0) {
-        mbar_init(&bar_ld[0], 1); mbar_init(&bar_ld[1], 1); mbar_init(&bar_mma[0], 1); mbar_init(&bar_mma[1], 1); mbar_init(&bar_done, 1);
+        mbar_init(&bar_ld[0], 1); mbar_init(&bar_ld[1], 1);
         fence_barrier_init();
     }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    tc::fence_before_sync();
+    wg::fence_proxy_async();                      // the ones image is read by the tensor cores
     __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t tbase = __shfl_sync(0xffffffffu, tmem_base_s, 0);    // warp-uniform for the compiler
-    const uint32_t lane_base = tbase + ((uint32_t)((warp & 3) * 32) << 16);
-    const uint32_t colW = 0, colW2 = 128, colB = 192;   // accumulators: dW (128 or F cols) | dW2^T (kp16) | bias (16)
     const int64_t per = (b.ntiles + nch - 1) / nch;
     const int64_t t0 = (int64_t)chunk * per, t1 = (t0 + per < b.ntiles) ? t0 + per : b.ntiles;
-    const uint32_t yp = layer0 ? 128u * b.F * 2u : kImg128;            // bytes of one part (hi or lo) of Y
-    const uint32_t dp = 128u * kp16 * 2u;                              // ... of DOUT
-    const int64_t nwork = t1 > t0 ? 2 * (t1 - t0) : 0;
-    bool started = false;
-    if (warp == 0 && nwork > 0) {
-        // warp 0 walks the work list converged; one elected lane issues the TMA copies and the MMAs (tc_umma.cuh)
-        const bool leader = tc::elect_one_sync();
-        auto load = [&](int64_t w) {
-            const int st = (int)(w & 1), hf = (int)(w & 1);             // work item w = 2 (t - t0) + hf uses stage w & 1
-            const int64_t t = t0 + (w >> 1);
-            uint8_t* base = smem + st * kStage;
-            uint8_t *dX = base, *dY = base + 2 * kHalf128, *dA2 = base + 4 * kHalf128, *dDO = base + 6 * kHalf128;
-            const uint8_t* srcX = (layer0 ? b.img.dh : b.img.dz[h]) + (size_t)t * 2 * kImg128;
-            const uint8_t* srcY = layer0 ? b.img.feat + (size_t)t * b.img.feat_bytes : b.img.a1 + (size_t)t * 2 * kImg128;
-            const uint32_t bytes = 2u * kHalf128 + yp + (layer0 ? 0u : 2u * kHalf128 + dp);
-            mbar_expect_tx(&bar_ld[st], bytes);
-            tma_bulk_g2s(dX, srcX + hf * kHalf128, kHalf128, &bar_ld[st]);
-            tma_bulk_g2s(dX + kHalf128, srcX + kImg128 + hf * kHalf128, kHalf128, &bar_ld[st]);
-            tma_bulk_g2s(dY, srcY + hf * (yp / 2), yp / 2, &bar_ld[st]);
-            tma_bulk_g2s(dY + yp / 2, srcY + yp + hf * (yp / 2), yp / 2, &bar_ld[st]);
-            if (!layer0) {
-                const uint8_t* srcA = b.img.a2[h] + (size_t)t * 2 * kImg128;
-                const uint8_t* srcD = b.img.dout[h] + (size_t)t * 2 * dp;
-                tma_bulk_g2s(dA2, srcA + hf * kHalf128, kHalf128, &bar_ld[st]);
-                tma_bulk_g2s(dA2 + kHalf128, srcA + kImg128 + hf * kHalf128, kHalf128, &bar_ld[st]);
-                tma_bulk_g2s(dDO, srcD + hf * (dp / 2), dp / 2, &bar_ld[st]);
-                tma_bulk_g2s(dDO + dp / 2, srcD + dp + hf * (dp / 2), dp / 2, &bar_ld[st]);
-            }
-        };
-        uint32_t ph_ld[2] = {0u, 0u}, ph_mma[2] = {0u, 0u};
-        if (leader) load(0);
-        __syncwarp();
-        for (int64_t w = 0; w < nwork; ++w) {
-            const int st = (int)(w & 1);
-            if (w + 1 < nwork) {
-                const int ns = st ^ 1;
-                if (w >= 1) { mbar_wait(&bar_mma[ns], ph_mma[ns]); ph_mma[ns] ^= 1u; }   // MMAs of work item w-1 have released stage ns
-                if (leader) load(w + 1);
-                __syncwarp();
-            }
-            mbar_wait(&bar_ld[st], ph_ld[st]); ph_ld[st] ^= 1u;
-            tc::fence_after_sync();
-            const uint32_t base = tc::smem_addr(smem + st * kStage), ones = tc::smem_addr(sOnes);
-            const uint32_t x = base, y = base + 2 * kHalf128, a2 = base + 4 * kHalf128, dd = base + 6 * kHalf128;
-            if (leader) {
-                if (layer0) {
-                    gemm_bf16x2_ss_mn<64>(tbase + colW, x, x + kHalf128, 128, y, y + yp / 2, (uint32_t)b.F, (uint32_t)b.F, started, false);
-                } else {
-                    gemm_bf16x2_ss_mn<64>(tbase + colW, x, x + kHalf128, 128, y, y + kHalf128, 128, 128, started, false);
-                    gemm_bf16x2_ss_mn<64>(tbase + colW2, a2, a2 + kHalf128, 128, dd, dd + dp / 2, (uint32_t)kp16, (uint32_t)kp16, started, false);
-                }
-                gemm_bf16x2_ss_mn<64>(tbase + colB, x, x + kHalf128, 128, ones, ones, 16, 16, started, true);
-                tc::umma_commit(&bar_mma[st]);
-            }
-            __syncwarp();
-            started = true;
-        }
-        if (leader) tc::umma_commit(&bar_done);        // covers every MMA issued above
-        __syncwarp();
-        mbar_wait(&bar_done, 0);
-    }
-    started = nwork > 0;
-    __syncthreads();
-    tc::fence_after_sync();
-    if (started || true) {
-        // every thread owns one output row j (its TMEM lane)
-        const int j = tid;
-        const bool any = t1 > t0;
-        if (any) {
-            const int ncolW = layer0 ? b.F : 128;
-            float* gw = layer0 ? b.g_w0 : b.g_w1[h];
-            for (int c0 = 0; c0 < ncolW; c0 += 16) {
-                uint32_t v[16];
-                tc::tmem_ld16(lane_base + colW + c0, v);
-                tc::wait_ld();
-#pragma unroll
-                for (int i = 0; i < 16; ++i) atomicAdd(gw + (size_t)j * ncolW + c0 + i, __uint_as_float(v[i]));
-            }
-            {
-                uint32_t v[16];
-                tc::tmem_ld16(lane_base + colB, v);
-                tc::wait_ld();
-                atomicAdd((layer0 ? b.g_b0 : b.g_b1[h]) + j, __uint_as_float(v[0]));
-            }
-            if (!layer0) {
-                const int ko = head_out(h);
-                for (int c0 = 0; c0 < kp16; c0 += 16) {
-                    uint32_t v[16];
-                    tc::tmem_ld16(lane_base + colW2 + c0, v);
-                    tc::wait_ld();
-#pragma unroll
-                    for (int i = 0; i < 16; ++i)
-                        if (c0 + i < ko) atomicAdd(b.g_w2[h] + (size_t)(c0 + i) * 128 + j, __uint_as_float(v[i]));
-                }
-            }
-        }
-    }
-    tc::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc(tbase, tc::kTmemCols);
+    if (!layer0) {
+        if (h == 4) wgrad_group<128, 48>(b, h, t0, t1, smem, bar_ld);
+        else wgrad_group<128, 16>(b, h, t0, t1, smem, bar_ld);
+    } else if (b.F == 32) wgrad_group<32, 0>(b, 5, t0, t1, smem, bar_ld);
+    else if (b.F == 48) wgrad_group<48, 0>(b, 5, t0, t1, smem, bar_ld);
+    else wgrad_group<64, 0>(b, 5, t0, t1, smem, bar_ld);
 }
 
 // ======================================================================================================
@@ -917,26 +697,26 @@ size_t tc_deform_backward_scratch_bytes(const DeformDesc& d, int64_t n) {
 }
 
 template <int C, int L>
-static cudaError_t launch_a(const BwdADesc& bd, float time, int64_t n, const float* xyz, int sm_count, cudaStream_t st) {
+static cudaError_t launch_a(const BwdADesc& bd, int64_t n, int sm_count, cudaStream_t st) {
     const BwdSmemA Ls = bwd_smem_a(C * L, bd.d.head_mask & G4D_HEAD_SHS);
     const size_t bytes = Ls.total + 1024;
     cudaError_t e = cudaFuncSetAttribute(deform_tc_bwd_dgrad_kernel<C, L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
     if (e != cudaSuccess) return e;
     const int64_t ntiles = (n + 127) / 128;
     const int grid = (int)(ntiles < sm_count ? ntiles : sm_count);
-    deform_tc_bwd_dgrad_kernel<C, L><<<grid, 256, bytes, st>>>(bd, Ls, time, n, xyz);
+    deform_tc_bwd_dgrad_kernel<C, L><<<grid, 256, bytes, st>>>(bd, Ls, n);
     return cudaGetLastError();
 }
 
 cudaError_t launch_deform_backward_tc(const DeformDesc& d, const G4DDeformParams& prm, const G4DDeformGrads& grads,
                                       const TcBwdWeights& w, float time, int64_t n, const float* xyz,
                                       const float* const go[G4D_NUM_HEADS], float* const gi[G4D_NUM_HEADS],
-                                      const uint32_t* relu_bits, const float* saved_feat, long long* dbg, uint8_t* scratch,
-                                      int sm_count, cudaStream_t st) {
+                                      const uint32_t* relu_bits, const float* saved_feat, uint8_t* scratch, int sm_count,
+                                      cudaStream_t st) {
     if (n == 0) return cudaSuccess;
     const int64_t ntiles = (n + 127) / 128;
     BwdADesc a{};
-    a.d = d; a.w = w; a.relu_bits = relu_bits; a.dbg = dbg;
+    a.d = d; a.w = w; a.relu_bits = relu_bits;
     uint8_t* p = scratch;
     auto take = [&](size_t bytes) { uint8_t* o = p; p += (bytes + 255) & ~(size_t)255; return o; };
     a.img.feat_bytes = 2u * 128 * d.F * 2;
@@ -944,7 +724,7 @@ cudaError_t launch_deform_backward_tc(const DeformDesc& d, const G4DDeformParams
     a.img.dh = take((size_t)ntiles * 2 * kImg128);
     a.img.feat = take((size_t)ntiles * a.img.feat_bytes);
     for (int h = 0; h < G4D_NUM_HEADS; ++h) {
-        a.go[h] = go[h]; a.gi[h] = gi[h]; a.g_b2[h] = grads.b2[h];
+        a.go[h] = go[h];
         if (!(d.head_mask & (1 << h))) continue;
         a.img.dz[h] = take((size_t)ntiles * 2 * kImg128);
         a.img.a2[h] = take((size_t)ntiles * 2 * kImg128);
@@ -979,9 +759,9 @@ cudaError_t launch_deform_backward_tc(const DeformDesc& d, const G4DDeformParams
         else return cudaErrorInvalidValue;
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
     }
-    if (d.C == 16 && d.levels == 2) e = launch_a<16, 2>(a, time, n, xyz, sm_count, st);
-    else if (d.C == 16 && d.levels == 3) e = launch_a<16, 3>(a, time, n, xyz, sm_count, st);
-    else if (d.C == 32 && d.levels == 2) e = launch_a<32, 2>(a, time, n, xyz, sm_count, st);
+    if (d.C == 16 && d.levels == 2) e = launch_a<16, 2>(a, n, sm_count, st);
+    else if (d.C == 16 && d.levels == 3) e = launch_a<16, 3>(a, n, sm_count, st);
+    else if (d.C == 32 && d.levels == 2) e = launch_a<32, 2>(a, n, sm_count, st);
     else return cudaErrorInvalidValue;
     if (e != cudaSuccess) return e;
     // scatter d(feat) into the planes, d(xyz), residual copies
@@ -1009,11 +789,11 @@ cudaError_t launch_deform_backward_tc(const DeformDesc& d, const G4DDeformParams
         b.nheads = nheads; b.chunks_head = ch; b.chunks_l0 = c0;
     }
     b.g_w0 = grads.w0; b.g_b0 = grads.b0;
-    for (int h = 0; h < G4D_NUM_HEADS; ++h) { b.g_w1[h] = grads.w1[h]; b.g_b1[h] = grads.b1[h]; b.g_w2[h] = grads.w2[h]; }
-    const size_t smem_b = (size_t)2 * (3 * kImg128 + 2 * 64 * 48 * 2) + 64 * 16 * 2 + 1024;   // two half-tile stages + ones
+    for (int h = 0; h < G4D_NUM_HEADS; ++h) { b.g_w1[h] = grads.w1[h]; b.g_b1[h] = grads.b1[h]; b.g_w2[h] = grads.w2[h]; b.g_b2[h] = grads.b2[h]; }
+    const size_t smem_b = (size_t)2 * kStage + kOnes + 1024;   // two half-tile stages + the all-ones operand
     e = cudaFuncSetAttribute(deform_tc_bwd_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_b);
     if (e != cudaSuccess) return e;
-    deform_tc_bwd_wgrad_kernel<<<b.nheads * b.chunks_head + b.chunks_l0, 128, smem_b, st>>>(b);
+    deform_tc_bwd_wgrad_kernel<<<b.nheads * b.chunks_head + b.chunks_l0, 256, smem_b, st>>>(b);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     return launch_distribute_time_grad(d, sc.trow_grad, sc.g_planes, time, st);
 }

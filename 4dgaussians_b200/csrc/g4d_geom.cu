@@ -275,10 +275,8 @@ deform_kernel(DeformDesc d, DeformSmem L, const CameraDev* __restrict__ camp, fl
     }
 }
 
-cudaError_t launch_deform_tc(const DeformDesc& d, const TcWeights& tw, int mode, const CameraDev* cam, float time,
-                             bool use_cam_time, int64_t n, const DeformIO& io, int sm_count, cudaStream_t st);
-cudaError_t launch_deform_f16(const DeformDesc& d, const TcWeights& tw, int mode, const CameraDev* cam, bool use_cam_time,
-                              int64_t n, const DeformIO& io, int sm_count, cudaStream_t st);
+cudaError_t launch_deform_tc(const DeformDesc& d, const TcWeights& tw, int mode, const CameraDev* cam, bool use_cam_time,
+                             int64_t n, const DeformIO& io, int sm_count, cudaStream_t st);
 
 template <int TG, int WD, int MODE>
 static cudaError_t launch_deform_t(const DeformDesc& d, const CameraDev* cam, float time, bool use_cam_time, int64_t n,
@@ -302,8 +300,7 @@ cudaError_t launch_deform(const DeformDesc& d, int mode, const CameraDev* cam, f
     if (n == 0) return cudaSuccess;
     DeformIO io{xyz, scaling, rotation, opacity, shs, sh_dc, sh_rest, out_xyz, out_scaling, out_rotation, out_opacity,
                 out_shs, g, fo, out_radii};
-    if (tw && tw->arith == 2) return launch_deform_f16(d, *tw, mode, cam, use_cam_time, n, io, sm_count, st);
-    if (tw) return launch_deform_tc(d, *tw, mode, cam, time, use_cam_time, n, io, sm_count, st);
+    if (tw) return launch_deform_tc(d, *tw, mode, cam, use_cam_time, n, io, sm_count, st);
     if (d.WD == 128) {
         return mode == 0 ? launch_deform_t<64, 128, 0>(d, cam, time, use_cam_time, n, io, sm_count, st)
                          : launch_deform_t<64, 128, 1>(d, cam, time, use_cam_time, n, io, sm_count, st);

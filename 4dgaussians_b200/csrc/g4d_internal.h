@@ -84,39 +84,38 @@ struct FusedOutputs {   // what the fused forward saves for its backward (may be
     float* rot_norm;   // |q| before F.normalize (needed by its backward)
 };
 
-// tensor-core weight images (g4d_deform_tc.cu): (hi | lo) TF32 parts in the canonical K-major smem layout
+// tensor-core weight images (g4d_deform_tc.cu): (hi | lo) parts in the canonical K-major shared-memory layout (tc_wgmma.cuh),
+// FP16x2 (scaled f16) or 3xTF32 words
 struct TcWeights {
-    const float* w0;                   // packed (hi | lo), [128][F] canonical
-    const float* w1[G4D_NUM_HEADS];    // packed (hi | lo), [128][128]
-    const float* w2[G4D_NUM_HEADS];    // packed (hi | lo), [kp16][128]
-    int kp16[G4D_NUM_HEADS];
+    const float* w0;                   // packed (hi | lo), [128][F]
+    const float* w1[G4D_NUM_HEADS];    // packed (hi | lo) K-parts, [128][128]
+    const float* w2[G4D_NUM_HEADS];    // SH head only: packed (hi | lo), [48][128]
     long long* dbg;                    // optional [grid][12] per-phase cycle counters (debug)
     float* feat;                       // [N][F] fp32 staging of the HexPlane features (deform_features_kernel)
     uint32_t* relu_bits;               // optional [6][N][4]: ReLU sign bits saved for the backward (G4D_RELU_BITS_WORDS)
-    int arith;                         // 1: 3xTF32 images / kernel (g4d_deform_tc.cu), 2: FP16x2 images / kernel (g4d_deform_f16.cu)
+    int arith;                         // 1: 3xTF32, 2: FP16x2 (G4D_OPT_TENSOR_CORES)
     uint32_t* status;                  // host-mapped word: set to 1 by the FP16x2 kernel when a value left the f16 operand range
 };
 
 size_t tc_packed_floats(const G4DDeformParams& prm);
-cudaError_t launch_tc_pack_weights(const G4DDeformParams& prm, float* blob, TcWeights* out, cudaStream_t st);
-bool tc_deform_supported(const DeformDesc& d);
-// FP16x2 variant (g4d_deform_f16.cu): same blob, same TcWeights, byte images
-cudaError_t launch_f16_pack_weights(const G4DDeformParams& prm, float* blob, TcWeights* out, cudaStream_t st);
-bool f16_deform_supported(const DeformDesc& d);
+cudaError_t launch_tc_pack_weights(const G4DDeformParams& prm, int arith, float* blob, TcWeights* out, cudaStream_t st);
+bool tc_deform_supported(const DeformDesc& d, int arith);
 
-// tensor-core backward (g4d_deform_tc_bwd.cu): BF16 (hi | lo) weight images in the 8x8-core layout of tc_umma.cuh
+// tensor-core backward (g4d_deform_tc_bwd.cu): BF16 (hi | lo) weight images in the 8x8-core layout of tc_wgmma.cuh
 struct TcBwdWeights {
     const uint8_t* w0;                    // image [128][F]
     const uint8_t* w1[G4D_NUM_HEADS];     // image [128][128]
+    const uint8_t* w2sh;                  // SH head: image of W2^T [128][48]
 };
 size_t tc_bwd_weight_bytes(const G4DDeformParams& prm);
 cudaError_t launch_tc_bwd_pack_weights(const G4DDeformParams& prm, uint8_t* blob, TcBwdWeights* out, cudaStream_t st);
+bool tc_backward_supported(const DeformDesc& d);
 size_t tc_deform_backward_scratch_bytes(const DeformDesc& d, int64_t n);
 cudaError_t launch_deform_backward_tc(const DeformDesc& d, const G4DDeformParams& prm, const G4DDeformGrads& grads,
                                       const TcBwdWeights& w, float time, int64_t n, const float* xyz,
                                       const float* const go[G4D_NUM_HEADS], float* const gi[G4D_NUM_HEADS],
-                                      const uint32_t* relu_bits, const float* saved_feat, long long* dbg, uint8_t* scratch,
-                                      int sm_count, cudaStream_t st);
+                                      const uint32_t* relu_bits, const float* saved_feat, uint8_t* scratch, int sm_count,
+                                      cudaStream_t st);
 // collapsed time-row gradients -> the two time rows of each (axis, t) plane (g4d_backward.cu)
 cudaError_t launch_distribute_time_grad(const DeformDesc& d, float* const (*trow_grad)[3], float* const (*g_planes)[6], float time,
                                         cudaStream_t st);
@@ -179,8 +178,5 @@ cudaError_t launch_adam_flat(float* p, const float* g, float* m, float* v, int64
 size_t knn_scratch_bytes(int64_t n);
 cudaError_t launch_knn_dist2(int64_t n, const float* xyz, float* out, void* scratch, int sm_count, cudaStream_t st);
 
-// tcgen05 building-block self test: g4d_tc_selftest.cu -> libg4d_selftest.so (test-only library, not in libg4d.so)
-cudaError_t launch_umma16_selftest(const int cfg[8], const float* A, const float* B, float* D, cudaStream_t st);
-cudaError_t launch_umma_selftest(const int cfg[8], const float* A, const float* B, float* scratch_packed, float* D, cudaStream_t st);
 
 }  // namespace g4d

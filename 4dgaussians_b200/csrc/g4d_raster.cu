@@ -8,6 +8,13 @@
 
 namespace g4d {
 
+// Two-lane float arithmetic of the packed blend kernels.  Hopper has no packed FP32 instructions, so each is two scalar
+// round-to-nearest operations (never contracted, whatever -fmad says): the per-lane results are exactly those of the scalar
+// expression tree.
+G4D_D float2 f2_add(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+G4D_D float2 f2_mul(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+G4D_D float2 f2_fma(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+
 // ------------------------------------------------------------------------------------------------------
 // A.3 blend forward: one 16x16 CTA per tile, instances staged through shared memory in batches of 256.
 template <int PPT>
@@ -113,10 +120,10 @@ blend_forward_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, const uin
 }
 
 // Packed variant (two pixels per thread as f32x2 lanes): the two pixels of a thread share their column, so dx, the dx^2 term and
-// the instance record are scalar and everything that depends on the row is ONE packed instruction (FADD2 / FMUL2 / FFMA2, sm_100)
-// instead of two; the per-pixel decisions are selects, not branches.  Same expression tree per lane as blend_forward_kernel<2>
-// up to the association of `power` (tests: image vs oracle 1e-4, outliers = threshold flips).  The scalar kernel is issue bound
-// (ncu: 83 % issue slots busy, IPC 3.3); this one issues ~17 instead of ~27 instructions per evaluated (pixel, instance) pair.
+// the instance record are scalar and only what depends on the row is evaluated per lane (f2_add / f2_mul / f2_fma); the
+// per-pixel decisions are selects, not branches.  Same expression tree per lane as blend_forward_kernel<2>
+// up to the association of `power` (tests: image vs oracle 1e-4, outliers = threshold flips).  The row-independent terms are
+// computed once per instance for both pixels.
 __global__ void __launch_bounds__(kTilePixels / 2)
 blend_forward_packed_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, const uint32_t* __restrict__ ids,
                             const uint2* __restrict__ ranges, float* __restrict__ final_T, uint32_t* __restrict__ n_contrib,
@@ -172,28 +179,28 @@ blend_forward_packed_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, co
                 const float4 b = s1[j];
                 const float2 c = s2[j];
                 const float dx = a.x - pxf;
-                const float2 dy = __fadd2_rn(make_float2(a.y, a.y), npy);
+                const float2 dy = f2_add(make_float2(a.y, a.y), npy);
                 const float q = a.z * dx * dx, nr = -(a.w * dx);
-                const float2 s = __ffma2_rn(make_float2(b.x, b.x), __fmul2_rn(dy, dy), make_float2(q, q));
-                const float2 pw = __ffma2_rn(dy, make_float2(nr, nr), __fmul2_rn(s, make_float2(-0.5f, -0.5f)));
+                const float2 s = f2_fma(make_float2(b.x, b.x), f2_mul(dy, dy), make_float2(q, q));
+                const float2 pw = f2_fma(dy, make_float2(nr, nr), f2_mul(s, make_float2(-0.5f, -0.5f)));
                 // exp(power) = ex2(power * log2 e); .ftz: a power below -87 flushes to 0 instead of a denormal (alpha < 1/255 either way)
-                const float2 pl = __fmul2_rn(pw, make_float2(1.4426950408889634f, 1.4426950408889634f));
+                const float2 pl = f2_mul(pw, make_float2(1.4426950408889634f, 1.4426950408889634f));
                 float ex0, ex1;
                 asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(ex0) : "f"(pl.x));
                 asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(ex1) : "f"(pl.y));
-                float2 al = __fmul2_rn(make_float2(b.y, b.y), make_float2(ex0, ex1));
+                float2 al = f2_mul(make_float2(b.y, b.y), make_float2(ex0, ex1));
                 al.x = fminf(kAlphaMax, al.x); al.y = fminf(kAlphaMax, al.y);
                 const bool c0 = !done0 && pw.x <= 0.f && al.x >= kAlphaMin, c1 = !done1 && pw.y <= 0.f && al.y >= kAlphaMin;
-                const float2 tt = __fmul2_rn(T, __fadd2_rn(make_float2(1.f, 1.f), make_float2(-al.x, -al.y)));
+                const float2 tt = f2_mul(T, f2_add(make_float2(1.f, 1.f), make_float2(-al.x, -al.y)));
                 const bool st0 = c0 && tt.x < kTransmittanceStop, st1 = c1 && tt.y < kTransmittanceStop;
                 done0 = done0 || st0; done1 = done1 || st1;
                 const bool k0 = c0 && !st0, k1 = c1 && !st1;
-                float2 w = __fmul2_rn(al, T);
+                float2 w = f2_mul(al, T);
                 w.x = k0 ? w.x : 0.f; w.y = k1 ? w.y : 0.f;
-                C0 = __ffma2_rn(make_float2(b.z, b.z), w, C0);
-                C1 = __ffma2_rn(make_float2(b.w, b.w), w, C1);
-                C2 = __ffma2_rn(make_float2(c.x, c.x), w, C2);
-                D = __ffma2_rn(make_float2(c.y, c.y), w, D);
+                C0 = f2_fma(make_float2(b.z, b.z), w, C0);
+                C1 = f2_fma(make_float2(b.w, b.w), w, C1);
+                C2 = f2_fma(make_float2(c.x, c.x), w, C2);
+                D = f2_fma(make_float2(c.y, c.y), w, D);
                 T.x = k0 ? tt.x : T.x; T.y = k1 ? tt.y : T.y;
                 last0 = k0 ? contributor : last0; last1 = k1 ? contributor : last1;
             }
@@ -405,7 +412,7 @@ blend_backward_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, const ui
 }
 
 // Packed variant of the backward (two pixels per thread as f32x2 lanes, see blend_forward_packed_kernel): the per-pixel gradient
-// arithmetic is one packed instruction per pixel PAIR, validity is a select instead of a branch, and the power / alpha are
+// arithmetic is one f2_* operation per pixel PAIR, validity is a select instead of a branch, and the power / alpha are
 // formed exactly as the packed forward forms them (same threshold decisions).  The warp reduction and the REDs are unchanged.
 __global__ void __launch_bounds__(kTilePixels / 2)
 blend_backward_packed_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, const uint32_t* __restrict__ ids,
@@ -487,32 +494,32 @@ blend_backward_packed_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, c
                 const float4 a = s0[j];
                 const float4 b = s1[j];
                 const float dx = a.x - pxf;
-                const float2 dy = __fadd2_rn(make_float2(a.y, a.y), npy);
+                const float2 dy = f2_add(make_float2(a.y, a.y), npy);
                 const float q = a.z * dx * dx, nr = -(a.w * dx);
-                const float2 sq = __ffma2_rn(make_float2(b.x, b.x), __fmul2_rn(dy, dy), make_float2(q, q));
-                const float2 pw = __ffma2_rn(dy, make_float2(nr, nr), __fmul2_rn(sq, make_float2(-0.5f, -0.5f)));
-                const float2 pl = __fmul2_rn(pw, make_float2(1.4426950408889634f, 1.4426950408889634f));
+                const float2 sq = f2_fma(make_float2(b.x, b.x), f2_mul(dy, dy), make_float2(q, q));
+                const float2 pw = f2_fma(dy, make_float2(nr, nr), f2_mul(sq, make_float2(-0.5f, -0.5f)));
+                const float2 pl = f2_mul(pw, make_float2(1.4426950408889634f, 1.4426950408889634f));
                 float2 G;
                 asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(G.x) : "f"(pl.x));
                 asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(G.y) : "f"(pl.y));
-                float2 al = __fmul2_rn(make_float2(b.y, b.y), G);
+                float2 al = f2_mul(make_float2(b.y, b.y), G);
                 al.x = fminf(kAlphaMax, al.x); al.y = fminf(kAlphaMax, al.y);
                 const bool v0 = lpos < last0 && pw.x <= 0.f && al.x >= kAlphaMin, v1 = lpos < last1 && pw.y <= 0.f && al.y >= kAlphaMin;
                 if (!__any_sync(0xffffffffu, v0 || v1)) continue;
                 const float c0 = b.z, c1 = b.w, c2 = s2[j];
-                const float2 om = __fadd2_rn(one2, make_float2(-al.x, -al.y));
+                const float2 om = f2_add(one2, make_float2(-al.x, -al.y));
                 const float2 ra = make_float2(__fdividef(1.f, om.x), __fdividef(1.f, om.y));   // alpha <= 0.99
-                const float2 Tn = __fmul2_rn(T, ra);
-                float2 w = __fmul2_rn(al, Tn);
-                const float2 oml = __fadd2_rn(one2, make_float2(-la.x, -la.y));
-                const float2 a0n = __ffma2_rn(la, lc0, __fmul2_rn(oml, ac0));
-                const float2 a1n = __ffma2_rn(la, lc1, __fmul2_rn(oml, ac1));
-                const float2 a2n = __ffma2_rn(la, lc2, __fmul2_rn(oml, ac2));
-                float2 dLa = __fmul2_rn(__fadd2_rn(make_float2(c0, c0), make_float2(-a0n.x, -a0n.y)), dp0);
-                dLa = __ffma2_rn(__fadd2_rn(make_float2(c1, c1), make_float2(-a1n.x, -a1n.y)), dp1, dLa);
-                dLa = __ffma2_rn(__fadd2_rn(make_float2(c2, c2), make_float2(-a2n.x, -a2n.y)), dp2, dLa);
-                dLa = __fmul2_rn(dLa, Tn);
-                dLa = __ffma2_rn(__fmul2_rn(nTfin, ra), bgdot, dLa);
+                const float2 Tn = f2_mul(T, ra);
+                float2 w = f2_mul(al, Tn);
+                const float2 oml = f2_add(one2, make_float2(-la.x, -la.y));
+                const float2 a0n = f2_fma(la, lc0, f2_mul(oml, ac0));
+                const float2 a1n = f2_fma(la, lc1, f2_mul(oml, ac1));
+                const float2 a2n = f2_fma(la, lc2, f2_mul(oml, ac2));
+                float2 dLa = f2_mul(f2_add(make_float2(c0, c0), make_float2(-a0n.x, -a0n.y)), dp0);
+                dLa = f2_fma(f2_add(make_float2(c1, c1), make_float2(-a1n.x, -a1n.y)), dp1, dLa);
+                dLa = f2_fma(f2_add(make_float2(c2, c2), make_float2(-a2n.x, -a2n.y)), dp2, dLa);
+                dLa = f2_mul(dLa, Tn);
+                dLa = f2_fma(f2_mul(nTfin, ra), bgdot, dLa);
                 // commit the per-pixel state of the pixels this instance is valid for; mask the contributions of the others
                 T.x = v0 ? Tn.x : T.x; T.y = v1 ? Tn.y : T.y;
                 ac0.x = v0 ? a0n.x : ac0.x; ac0.y = v1 ? a0n.y : ac0.y;
@@ -526,22 +533,22 @@ blend_backward_packed_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, c
                 dLa.x = v0 ? dLa.x : 0.f; dLa.y = v1 ? dLa.y : 0.f;
                 float v[8];
                 {
-                    const float2 p5 = __fmul2_rn(w, dp0), p6 = __fmul2_rn(w, dp1), p7 = __fmul2_rn(w, dp2);
+                    const float2 p5 = f2_mul(w, dp0), p6 = f2_mul(w, dp1), p7 = f2_mul(w, dp2);
                     v[5] = p5.x + p5.y; v[6] = p6.x + p6.y; v[7] = p7.x + p7.y;
                 }
-                const float2 dLdG = __fmul2_rn(make_float2(b.y, b.y), dLa);
-                const float2 gdx = __fmul2_rn(G, make_float2(dx, dx)), gdy = __fmul2_rn(G, dy);
+                const float2 dLdG = f2_mul(make_float2(b.y, b.y), dLa);
+                const float2 gdx = f2_mul(G, make_float2(dx, dx)), gdy = f2_mul(G, dy);
                 {
-                    const float2 t0 = __ffma2_rn(gdy, make_float2(-a.w, -a.w), __fmul2_rn(gdx, make_float2(-a.z, -a.z)));
-                    const float2 t1 = __ffma2_rn(gdx, make_float2(-a.w, -a.w), __fmul2_rn(gdy, make_float2(-b.x, -b.x)));
-                    const float2 u0 = __fmul2_rn(dLdG, t0), u1 = __fmul2_rn(dLdG, t1);
-                    const float2 u2 = __fmul2_rn(__fmul2_rn(gdx, make_float2(dx, dx)), dLdG);
-                    const float2 u3 = __fmul2_rn(__fmul2_rn(gdx, dy), dLdG);
-                    const float2 u4 = __fmul2_rn(__fmul2_rn(gdy, dy), dLdG);
+                    const float2 t0 = f2_fma(gdy, make_float2(-a.w, -a.w), f2_mul(gdx, make_float2(-a.z, -a.z)));
+                    const float2 t1 = f2_fma(gdx, make_float2(-a.w, -a.w), f2_mul(gdy, make_float2(-b.x, -b.x)));
+                    const float2 u0 = f2_mul(dLdG, t0), u1 = f2_mul(dLdG, t1);
+                    const float2 u2 = f2_mul(f2_mul(gdx, make_float2(dx, dx)), dLdG);
+                    const float2 u3 = f2_mul(f2_mul(gdx, dy), dLdG);
+                    const float2 u4 = f2_mul(f2_mul(gdy, dy), dLdG);
                     v[0] = (u0.x + u0.y) * ddx; v[1] = (u1.x + u1.y) * ddy;
                     v[2] = -0.5f * (u2.x + u2.y); v[3] = -(u3.x + u3.y); v[4] = -0.5f * (u4.x + u4.y);
                 }
-                const float2 po = __fmul2_rn(G, dLa);
+                const float2 po = f2_mul(G, dLa);
                 float v_op = po.x + po.y;
                 float u[4];
 #pragma unroll
@@ -572,7 +579,7 @@ cudaError_t launch_blend_backward(const CameraDev* cam, int grid_x, int grid_y, 
                                   const float* dL_dcolor, float* g_mean2D, float* g_conic, float* g_opacity, float* g_rgb,
                                   int warp_cull, cudaStream_t st) {
     if (grid_x * grid_y == 0) return cudaSuccess;
-    // pixels per thread: 2 measured best at C3 (tools/profile_step.py; G4D_BLEND_BWD_PPT overrides for experiments)
+    // pixels per thread: 2 (G4D_BLEND_BWD_PPT overrides for experiments)
     static int ppt = []() { const char* e = getenv("G4D_BLEND_BWD_PPT"); const int v = e ? atoi(e) : 2; return (v == 1 || v == 4) ? v : 2; }();
     static int packed = []() { const char* e = getenv("G4D_BLEND_BWD_PACKED"); return e ? atoi(e) : 1; }();
     if (packed && ppt == 2) {

@@ -1,501 +1,132 @@
-// g4d_tc_selftest.cu -- single-CTA self test of the tcgen05 building blocks in tc_umma.cuh:
-//   D[128 x N] = A[128 x K] * B[N x K]^T   with 3xTF32, A through TMEM, B through shared memory.
-// The layout / descriptor hypotheses are runtime parameters so that one GPU session can tell which encoding the
-// hardware accepts (there is no GPU in the build container).  Debug entry point g4d_debug_umma (include/g4d.h).
-#include "g4d_internal.h"
-#include "tc_umma.cuh"
+// g4d_tc_selftest.cu -- self test of the wgmma building blocks of tc_wgmma.cuh (test-only library libg4d_selftest.so).
+//
+// D[128 x N] = A[128 x K] * B[N x K]^T by two warpgroups (rows 0-63 / 64-127), one operand arrangement per mode, each with
+// the hi / lo split and three products the kernels use:
+//   0  3xTF32, A register fragments, B K-major                  (deform forward, G4D_OPT_TENSOR_CORES = 1)
+//   1  FP16x2, A register fragments, B K-major                  (deform forward, default)
+//   2  BF16x2, A register fragments, B MN-major (transposed)    (backward dgrad: d(a1) = dz W1, d(feat) = dh W0)
+//   3  BF16x2, A and B from shared memory, both MN-major        (backward wgrad: dW = X^T Y over the Gaussians)
+//   4  BF16x2, A and B from shared memory, both K-major
+#include <cuda_runtime.h>
+
+#include "tc_wgmma.cuh"
 
 namespace g4d {
+namespace {
 
-struct UmmaTestCfg {
-    int N, K;
-    int layout_mode;   // 0: K cores contiguous (LBO=128, SBO=(K/4)*128); 1: 8-row groups contiguous (SBO=128, LBO=(N/8)*128)
-    int swap_desc;     // 1: put LBO in the SBO field and vice versa
-    int a_cols_per_k;  // TMEM columns the A operand advances per element of K (1 for 32-bit types)
-    int use_tma;       // 1: B arrives pre-packed (hi | lo) in global memory and is staged with cp.async.bulk
-    int single_pass;   // 1: plain TF32 (hi*hi only)
-    int version_bit;   // descriptor version field (1 on sm_100)
-};
-
-__global__ void __launch_bounds__(128, 1)
-umma_selftest_kernel(UmmaTestCfg c, const float* __restrict__ A, const float* __restrict__ B, const float* __restrict__ Bpacked,
-                     float* __restrict__ D) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    __shared__ uint32_t tmem_base_s;
-    __shared__ __align__(8) uint64_t bar_mma, bar_tma;
-    const int tid = threadIdx.x, warp = tid >> 5;
-    const uint32_t N = c.N, K = c.K;
-    uint8_t* b_hi = smem_raw;
-    uint8_t* b_lo = smem_raw + N * K * 4;
-    if (warp == 0) tc::tmem_alloc(&tmem_base_s, tc::kTmemCols);
-    if (tid == 0) { mbar_init(&bar_mma, 1); mbar_init(&bar_tma, 1); fence_barrier_init(); }
-    tc::fence_before_sync();
-    __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t tbase = tmem_base_s;
-    const uint32_t lane_base = (uint32_t)((warp & 3) * 32) << 16;
-    const uint32_t lbo = c.layout_mode == 0 ? 128u : (N >> 3) * 128u;
-    const uint32_t sbo = c.layout_mode == 0 ? (K >> 2) * 128u : 128u;
-    // ---- B -> shared memory (canonical layout), hi and lo parts
-    if (c.use_tma) {
-        if (tid == 0) {
-            mbar_expect_tx(&bar_tma, 2 * N * K * 4);
-            tma_bulk_g2s(b_hi, Bpacked, N * K * 4, &bar_tma);
-            tma_bulk_g2s(b_lo, Bpacked + N * K, N * K * 4, &bar_tma);
-        }
-        mbar_wait(&bar_tma, 0);
-    } else {
-        for (uint32_t i = tid; i < N * K; i += blockDim.x) {
-            const uint32_t n = i / K, k = i % K;
+template <int N>
+__global__ void __launch_bounds__(256, 1) wgmma_selftest_kernel(int K, int mode, const float* __restrict__ A, const float* __restrict__ B,
+                                                               float* __restrict__ D) {
+    extern __shared__ __align__(1024) uint8_t smem[];
+    const int tid = threadIdx.x, wgi = tid >> 7, t128 = tid & 127, lane = tid & 31, g = lane >> 2, t = lane & 3;
+    const int r0 = wgi * 64 + ((t128 >> 5) << 4) + g, r1 = r0 + 8;
+    const bool tf32 = mode == 0;
+    const uint32_t es = tf32 ? 4u : 2u;
+    uint8_t* sB = smem;                                  // (hi | lo) image of B
+    uint8_t* sA = smem + 2u * N * K * es;                // (hi | lo) image of A (modes 3, 4)
+    const uint32_t bpart = (uint32_t)N * K * es, apart = 128u * K * 2u;
+    for (int e = tid; e < N * K; e += 256) {
+        const uint32_t nn = e / K, k = e % K;
+        const float v = B[e];
+        if (tf32) {
             uint32_t hi, lo;
-            tc::tf32_split(B[i], hi, lo);
-            const uint32_t off = (n >> 3) * sbo + (k >> 2) * lbo + (n & 7) * 16 + (k & 3) * 4;
-            *reinterpret_cast<uint32_t*>(b_hi + off) = hi;
-            *reinterpret_cast<uint32_t*>(b_lo + off) = lo;
+            wg::tf32_split(v, hi, lo);
+            *reinterpret_cast<uint32_t*>(sB + wg::img32_off(nn, k, K)) = hi;
+            *reinterpret_cast<uint32_t*>(sB + bpart + wg::img32_off(nn, k, K)) = lo;
+        } else {
+            uint32_t hi, lo;
+            if (mode == 1) wg::f16_split2(v, 0.f, hi, lo); else wg::bf16_split2(v, 0.f, hi, lo);
+            const uint32_t off = (mode == 2 || mode == 3) ? wg::img16_off(k, nn, N) : wg::img16_off(nn, k, K);
+            *reinterpret_cast<uint16_t*>(sB + off) = (uint16_t)hi;
+            *reinterpret_cast<uint16_t*>(sB + bpart + off) = (uint16_t)lo;
         }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> tensor-core (async proxy) reads
     }
-    // ---- A -> TMEM: thread r owns lane r; hi at columns [0, K*cpk), lo right after
-    {
-        const int r = tid;
-        const uint32_t cpk = c.a_cols_per_k;
-        for (uint32_t k0 = 0; k0 < K; k0 += 8) {
-            uint32_t hi[8], lo[8];
+    if (mode >= 3) {
+        for (int e = tid; e < 128 * K; e += 256) {
+            const uint32_t m = e / K, k = e % K;
+            uint32_t hi, lo;
+            wg::bf16_split2(A[e], 0.f, hi, lo);
+            const uint32_t off = mode == 3 ? wg::img16_off(k, m, 128) : wg::img16_off(m, k, K);
+            *reinterpret_cast<uint16_t*>(sA + off) = (uint16_t)hi;
+            *reinterpret_cast<uint16_t*>(sA + apart + off) = (uint16_t)lo;
+        }
+    }
+    wg::fence_proxy_async();
+    __syncthreads();
+    const uint32_t b = wg::smem_addr(sB), a = wg::smem_addr(sA);
+    float d[N / 2];
+    const int ks = tf32 ? 8 : 16;
+    for (int s = 0; s < K / ks; ++s) {
+        wg::Frags<1> f;
+        if (mode <= 2) {
+            if (tf32) {
+                const int c0 = 8 * s + t, c1 = c0 + 4;
+                wg::tf32_split(A[r0 * K + c0], f.hi[0][0], f.lo[0][0]);
+                wg::tf32_split(A[r1 * K + c0], f.hi[0][1], f.lo[0][1]);
+                wg::tf32_split(A[r0 * K + c1], f.hi[0][2], f.lo[0][2]);
+                wg::tf32_split(A[r1 * K + c1], f.hi[0][3], f.lo[0][3]);
+            } else {
 #pragma unroll
-            for (int j = 0; j < 8; ++j) tc::tf32_split(A[r * K + k0 + j], hi[j], lo[j]);
-            tc::tmem_st8(tbase + lane_base + k0 * cpk, hi);
-            tc::tmem_st8(tbase + lane_base + K * cpk + k0 * cpk, lo);
-        }
-        tc::wait_st();
-    }
-    tc::fence_before_sync();
-    __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t d_col = 256;
-    if (tid == 0) {
-        const uint32_t idesc = tc::make_idesc_tf32(128, N);
-        bool acc = false;
-        const int passes = c.single_pass ? 1 : 3;
-        for (int p = 0; p < passes; ++p) {
-            const uint32_t a = tbase + ((c.single_pass || p != 0) ? 0u : K * c.a_cols_per_k);
-            const uint8_t* b = (!c.single_pass && p == 1) ? b_lo : b_hi;
-            for (uint32_t ks = 0; ks < K; ks += 8) {
-                const uint32_t saddr = tc::smem_addr(b) + (ks >> 2) * lbo;
-                uint64_t bd = c.swap_desc ? tc::make_smem_desc(saddr, sbo, lbo) : tc::make_smem_desc(saddr, lbo, sbo);
-                if (!c.version_bit) bd &= ~(1ull << 46);
-                tc::umma_tf32_ts(tbase + d_col, a + ks * c.a_cols_per_k, bd, idesc, acc);
-                acc = true;
-            }
-        }
-        tc::umma_commit(&bar_mma);
-    }
-    mbar_wait(&bar_mma, 0);
-    tc::fence_after_sync();
-    {
-        const int r = tid;
-        for (uint32_t n0 = 0; n0 < N; n0 += 8) {
-            uint32_t v[8];
-            tc::tmem_ld8(tbase + lane_base + d_col + n0, v);
-            tc::wait_ld();
-#pragma unroll
-            for (int j = 0; j < 8; ++j) D[r * N + n0 + j] = __uint_as_float(v[j]);
-        }
-    }
-    tc::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc(tbase, tc::kTmemCols);
-}
-
-// pack an [N][K] fp32 matrix into (hi | lo) canonical tf32 images (layout_mode 0)
-__global__ void pack_canonical_kernel(const float* __restrict__ src, float* __restrict__ dst, int N, int K) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= N * K) return;
-    const uint32_t n = i / K, k = i % K;
-    uint32_t hi, lo;
-    tc::tf32_split(src[i], hi, lo);
-    const uint32_t off = tc::canon_off(n, k, K) >> 2;
-    reinterpret_cast<uint32_t*>(dst)[off] = hi;
-    reinterpret_cast<uint32_t*>(dst)[N * K + off] = lo;
-}
-
-cudaError_t launch_umma_selftest(const int cfg[8], const float* A, const float* B, float* scratch_packed, float* D, cudaStream_t st) {
-    UmmaTestCfg c{cfg[0], cfg[1], cfg[2], cfg[3], cfg[4], cfg[5], cfg[6], cfg[7]};
-    if (c.N < 16 || c.N > 128 || (c.N % 16) || c.K < 8 || c.K > 128 || (c.K % 8) || c.a_cols_per_k < 1 || c.a_cols_per_k > 2)
-        return cudaErrorInvalidValue;
-    if (c.use_tma) {
-        pack_canonical_kernel<<<(c.N * c.K + 255) / 256, 256, 0, st>>>(B, scratch_packed, c.N, c.K);
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return e;
-    }
-    const size_t smem = (size_t)2 * c.N * c.K * 4 + 1024;
-    cudaError_t e = cudaFuncSetAttribute(umma_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    umma_selftest_kernel<<<1, 128, smem, st>>>(c, A, B, scratch_packed, D);
-    return cudaGetLastError();
-}
-
-}  // namespace g4d
-
-// ------------------------------------------------------------------------------------------------------
-// Self test #2: kind::f16 (BF16 hi+lo, 3 products) with every operand role the backward kernels use.
-//   D[128 x N] = A[128 x K] * B[N x K]^T
-// a_mode: 0 = TMEM (two bf16 per 32-bit column), 1 = smem K-major image of A[M][K], 2 = smem MN-major image built from
-//         the TRANSPOSED matrix At[K][M] (the layout a [g][j] activation image has when g is the contraction index)
-// b_mode: 0 = smem K-major image of B[N][K], 1 = smem MN-major image built from Bt[K][N]
-// pack_hi_first: TMEM packing order of the two K elements in a column (0: even k in the low half)
-// ------------------------------------------------------------------------------------------------------
-namespace g4d {
-
-struct Umma16Cfg { int N, K, a_mode, b_mode, pack_hi_first, single_pass, r0, r1; };
-
-__global__ void __launch_bounds__(128, 1)
-umma16_selftest_kernel(Umma16Cfg c, const float* __restrict__ A, const float* __restrict__ B, float* __restrict__ D) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    __shared__ uint32_t tmem_base_s;
-    __shared__ __align__(8) uint64_t bar_mma;
-    const int tid = threadIdx.x, warp = tid >> 5;
-    const uint32_t N = c.N, K = c.K, M = 128;
-    // images: A hi, A lo (128 x K or K x 128), B hi, B lo
-    uint8_t* a_img[2] = {smem_raw, smem_raw + M * K * 2};
-    uint8_t* b_img[2] = {smem_raw + 2 * M * K * 2, smem_raw + 2 * M * K * 2 + N * K * 2};
-    if (warp == 0) tc::tmem_alloc(&tmem_base_s, tc::kTmemCols);
-    if (tid == 0) { mbar_init(&bar_mma, 1); fence_barrier_init(); }
-    tc::fence_before_sync();
-    __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t tbase = tmem_base_s;
-    const uint32_t lane_base = (uint32_t)((warp & 3) * 32) << 16;
-    // ---- B images
-    for (uint32_t i = tid; i < N * K; i += blockDim.x) {
-        const uint32_t n = i / K, k = i % K;
-        uint16_t hi, lo;
-        tc::bf16_split(B[i], hi, lo);
-        const uint32_t off = c.b_mode == 0 ? tc::img16_off(n, k, K) : tc::img16_off(k, n, N);
-        *reinterpret_cast<uint16_t*>(b_img[0] + off) = hi;
-        *reinterpret_cast<uint16_t*>(b_img[1] + off) = lo;
-    }
-    // ---- A: images or TMEM
-    if (c.a_mode != 0) {
-        for (uint32_t i = tid; i < M * K; i += blockDim.x) {
-            const uint32_t m = i / K, k = i % K;
-            uint16_t hi, lo;
-            tc::bf16_split(A[i], hi, lo);
-            const uint32_t off = c.a_mode == 1 ? tc::img16_off(m, k, K) : tc::img16_off(k, m, M);
-            *reinterpret_cast<uint16_t*>(a_img[0] + off) = hi;
-            *reinterpret_cast<uint16_t*>(a_img[1] + off) = lo;
-        }
-    } else {
-        const int r = tid;
-        for (uint32_t k0 = 0; k0 < K; k0 += 16) {   // 16 K elements = 8 columns
-            uint32_t hi[8], lo[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                uint16_t h0, l0, h1, l1;
-                tc::bf16_split(A[r * K + k0 + 2 * j], h0, l0);
-                tc::bf16_split(A[r * K + k0 + 2 * j + 1], h1, l1);
-                hi[j] = c.pack_hi_first ? ((uint32_t)h0 << 16 | h1) : ((uint32_t)h1 << 16 | h0);
-                lo[j] = c.pack_hi_first ? ((uint32_t)l0 << 16 | l1) : ((uint32_t)l1 << 16 | l0);
-            }
-            tc::tmem_st8(tbase + lane_base + (k0 >> 1), hi);
-            tc::tmem_st8(tbase + lane_base + 128 + (k0 >> 1), lo);
-        }
-        tc::wait_st();
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    tc::fence_before_sync();
-    __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t d_col = 256;
-    if (tid == 0) {
-        const uint32_t idesc = tc::make_idesc_bf16(128, N, c.a_mode == 2, c.b_mode == 1);
-        // per-operand descriptor strides and the byte step of one K = 16 MMA
-        const uint32_t a_lbo = c.a_mode == 1 ? 128u : (M >> 3) * 128u, a_sbo = c.a_mode == 1 ? (K >> 3) * 128u : 128u;
-        const uint32_t a_step = c.a_mode == 1 ? 2u * 128u : 2u * (M >> 3) * 128u;
-        const uint32_t b_lbo = c.b_mode == 0 ? 128u : (N >> 3) * 128u, b_sbo = c.b_mode == 0 ? (K >> 3) * 128u : 128u;
-        const uint32_t b_step = c.b_mode == 0 ? 2u * 128u : 2u * (N >> 3) * 128u;
-        bool acc = false;
-        const int passes = c.single_pass ? 1 : 3;
-        for (int p = 0; p < passes; ++p) {
-            const int ai = (!c.single_pass && p == 0) ? 1 : 0, bi = (!c.single_pass && p == 1) ? 1 : 0;
-            for (uint32_t ks = 0; ks < K; ks += 16) {
-                const uint64_t bd = tc::make_smem_desc(tc::smem_addr(b_img[bi]) + (ks >> 4) * b_step, b_lbo, b_sbo);
-                if (c.a_mode == 0) {
-                    tc::umma_bf16_ts(tbase + d_col, tbase + (ai ? 128u : 0u) + (ks >> 1), bd, idesc, acc);
-                } else {
-                    const uint64_t ad = tc::make_smem_desc(tc::smem_addr(a_img[ai]) + (ks >> 4) * a_step, a_lbo, a_sbo);
-                    tc::umma_bf16_ss(tbase + d_col, ad, bd, idesc, acc);
-                }
-                acc = true;
-            }
-        }
-        tc::umma_commit(&bar_mma);
-    }
-    mbar_wait(&bar_mma, 0);
-    tc::fence_after_sync();
-    {
-        const int r = tid;
-        for (uint32_t n0 = 0; n0 < N; n0 += 8) {
-            uint32_t v[8];
-            tc::tmem_ld8(tbase + lane_base + d_col + n0, v);
-            tc::wait_ld();
-#pragma unroll
-            for (int j = 0; j < 8; ++j) D[r * N + n0 + j] = __uint_as_float(v[j]);
-        }
-    }
-    tc::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc(tbase, tc::kTmemCols);
-}
-
-cudaError_t launch_umma16_selftest(const int cfg[8], const float* A, const float* B, float* D, cudaStream_t st) {
-    Umma16Cfg c{cfg[0], cfg[1], cfg[2], cfg[3], cfg[4], cfg[5], cfg[6], cfg[7]};
-    if (c.N < 16 || c.N > 128 || (c.N % 16) || c.K < 16 || c.K > 128 || (c.K % 16)) return cudaErrorInvalidValue;
-    const size_t smem = (size_t)2 * 128 * c.K * 2 + (size_t)2 * c.N * c.K * 2 + 1024;
-    cudaError_t e = cudaFuncSetAttribute(umma16_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    umma16_selftest_kernel<<<1, 128, smem, st>>>(c, A, B, D);
-    return cudaGetLastError();
-}
-
-
-// ---- dispatch-rate microbenchmark ------------------------------------------------------------------------------------------
-// One CTA per launch block: thread 256 issues `ndisp` identical tcgen05.mma (M = 128, N, one K step) back to back and waits
-// for their completion; meanwhile `readers` warps (0..8) hammer OTHER TMEM columns with tcgen05.ld (op 1) or tcgen05.st
-// (op 2).  Answers: what does a dispatch cost as a function of N and of where A lives, and do TMEM<->register transfers
-// share a port with the tensor pipe's operand reads?  Data are zeros; only clocks matter.
-struct RateCfg { int N, a_smem, kind_tf32, readers, reader_op, ndisp, d_cols_apart, pad; };
-
-__global__ void __launch_bounds__(288, 1) umma_rate_kernel(RateCfg c, long long* __restrict__ out) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    __shared__ uint32_t tmem_base_s;
-    __shared__ __align__(8) uint64_t bar_mma;
-    __shared__ volatile int done_flag;
-    const int tid = threadIdx.x, warp = tid >> 5;
-    for (int i = tid; i < 16384 / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(smem_raw)[i] = 0u;   // A (4 KB) | B (8 KB)
-    if (warp == 0) tc::tmem_alloc(&tmem_base_s, tc::kTmemCols);
-    if (tid == 0) { mbar_init(&bar_mma, 1); fence_barrier_init(); done_flag = 0; }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    tc::fence_before_sync();
-    __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t tbase = __shfl_sync(0xffffffffu, tmem_base_s, 0);    // warp-uniform for the compiler (UTCHMMA operands are uniform registers)
-    const uint32_t lane_base = tbase + ((uint32_t)((warp & 3) * 32) << 16);
-    if (warp < 8) {   // zero the whole TMEM (no NaN patterns in the accumulators)
-        uint32_t z[16];
-#pragma unroll
-        for (int j = 0; j < 16; ++j) z[j] = 0u;
-        for (uint32_t col = (uint32_t)(warp >> 2) * 256u; col < (uint32_t)(warp >> 2) * 256u + 256u; col += 16) tc::tmem_st16(lane_base + col, z);
-        tc::wait_st();
-    }
-    tc::fence_before_sync();
-    __syncthreads();
-    tc::fence_after_sync();
-    long long iters = 0;
-    if (warp == 8) {
-        // converged warp, one elected issuer: operands in uniform registers, no waterfall loop around UTCHMMA
-        uint32_t leader_;
-        asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(leader_));
-        const bool leader = leader_ != 0;
-        {
-            const uint32_t N = (uint32_t)c.N;
-            const uint32_t idesc = c.kind_tf32 ? tc::make_idesc_tf32(128, N) : tc::make_idesc_bf16(128, N, false, false);
-            const uint32_t a_s = tc::smem_addr(smem_raw), b_s = tc::smem_addr(smem_raw + 4096);
-            // one K step: two 128-byte cores per 8-row group -> LBO 128, SBO 256
-            const uint64_t ad = tc::make_smem_desc(a_s, 128u, 256u), bd = tc::make_smem_desc(b_s, 128u, 256u);
-            const uint32_t d0 = tbase, d1 = tbase + (uint32_t)c.d_cols_apart, a_t = tbase + 496u;   // A operand: 8 columns at the very end
-            const long long t0 = clock64();
-            for (int i = 0; i < c.ndisp; ++i) {
-                const uint32_t dd = (i & 1) ? d1 : d0;
-                if (leader) {
-                    if (c.kind_tf32) {
-                        tc::umma_tf32_ts(dd, a_t, bd, idesc, true);
-                    } else if (c.a_smem) {
-                        tc::umma_bf16_ss(dd, ad, bd, idesc, true);
+                for (int hlf = 0; hlf < 2; ++hlf) {
+                    const int c = 16 * s + 8 * hlf + 2 * t;
+                    if (mode == 1) {
+                        wg::f16_split2(A[r0 * K + c], A[r0 * K + c + 1], f.hi[0][2 * hlf], f.lo[0][2 * hlf]);
+                        wg::f16_split2(A[r1 * K + c], A[r1 * K + c + 1], f.hi[0][2 * hlf + 1], f.lo[0][2 * hlf + 1]);
                     } else {
-                        tc::umma_bf16_ts(dd, a_t, bd, idesc, true);
+                        wg::bf16_split2(A[r0 * K + c], A[r0 * K + c + 1], f.hi[0][2 * hlf], f.lo[0][2 * hlf]);
+                        wg::bf16_split2(A[r1 * K + c], A[r1 * K + c + 1], f.hi[0][2 * hlf + 1], f.lo[0][2 * hlf + 1]);
                     }
                 }
             }
-            const long long t1 = clock64();
-            if (leader) tc::umma_commit(&bar_mma);
-            mbar_wait(&bar_mma, 0);
-            const long long t2 = clock64();
-            if (leader) {
-                done_flag = 1;
-                out[blockIdx.x * 4 + 0] = t1 - t0;   // issue loop (blocks when the queue is full)
-                out[blockIdx.x * 4 + 1] = t2 - t0;   // until the last dispatch retired
-            }
         }
-    } else if (warp < c.readers && c.reader_op) {
-        uint32_t v[16];
-#pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] = 0u;
-        const uint32_t col0 = 256u + (uint32_t)(warp >> 2) * 112u;   // columns [256, 480): never touched by the MMAs
-        while (!done_flag) {
-#pragma unroll 1
-            for (uint32_t k = 0; k < 7; ++k) {
-                if (c.reader_op == 1) { tc::tmem_ld16(lane_base + col0 + k * 16u, v); tc::wait_ld(); }
-                else { tc::tmem_st16(lane_base + col0 + k * 16u, v); tc::wait_st(); }
-                ++iters;
-            }
+        wg::fence_regs(d);
+        wg::fence();
+        for (int p = 0; p < 3; ++p) {
+            const uint32_t acc = (s > 0 || p > 0) ? 1u : 0u;
+            const uint32_t bb = b + (p == 1 ? bpart : 0u);
+            const uint32_t aa = a + (p == 0 ? apart : 0u);
+            if (mode == 0) wg::mma_tf32_rs<N>(d, p == 0 ? f.lo[0] : f.hi[0], wg::desc_kmajor(bb, K, 4) + 16u * s, acc);
+            else if (mode == 1) wg::mma_f16_rs<N, 0>(d, p == 0 ? f.lo[0] : f.hi[0], wg::desc_kmajor(bb, K, 8) + 16u * s, acc);
+            else if (mode == 2) wg::mma_bf16_rs<N, 1>(d, p == 0 ? f.lo[0] : f.hi[0], wg::desc_mnmajor(bb, N) + 2u * (N / 8) * 8u * s, acc);
+            else if (mode == 3)
+                wg::mma_bf16_ss<N, 1, 1>(d, wg::desc_mnmajor(aa + wgi * 1024u, 128) + 2u * 16u * 8u * s,
+                                         wg::desc_mnmajor(bb, N) + 2u * (N / 8) * 8u * s, acc);
+            else
+                wg::mma_bf16_ss<N, 0, 0>(d, wg::desc_kmajor(aa + wgi * 64u * (K / 8) * 16u, K, 8) + 16u * s,
+                                         wg::desc_kmajor(bb, K, 8) + 16u * s, acc);
         }
-        if ((tid & 31) == 0) atomicAdd(reinterpret_cast<unsigned long long*>(out + blockIdx.x * 4 + 2), (unsigned long long)iters + (v[3] & 1u));
+        wg::commit();
+        wg::wait_all();
+        wg::fence_regs(d);
     }
-    tc::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc(tbase, tc::kTmemCols);
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j) {
+        const int c = 8 * j + 2 * t;
+        D[r0 * N + c] = d[4 * j]; D[r0 * N + c + 1] = d[4 * j + 1];
+        D[r1 * N + c] = d[4 * j + 2]; D[r1 * N + c + 1] = d[4 * j + 3];
+    }
 }
 
-cudaError_t launch_umma_rate(const int cfg[8], long long* out, int blocks, cudaStream_t st) {
-    RateCfg c{cfg[0], cfg[1], cfg[2], cfg[3], cfg[4], cfg[5], cfg[6], 0};
-    if (c.N < 16 || c.N > 256 || (c.N % 16) || c.readers < 0 || c.readers > 8 || c.ndisp < 1) return cudaErrorInvalidValue;
-    if (c.d_cols_apart + c.N > 256 && c.d_cols_apart != 0) return cudaErrorInvalidValue;
-    const size_t smem = 200 * 1024;    // one CTA per SM
-    cudaError_t e = cudaFuncSetAttribute(umma_rate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+template <int N>
+cudaError_t launch_n(int K, int mode, const float* A, const float* B, float* D, cudaStream_t st) {
+    const size_t bytes = 2u * N * K * 4u + 2u * 128u * K * 2u;
+    cudaError_t e = cudaFuncSetAttribute(wgmma_selftest_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
     if (e != cudaSuccess) return e;
-    umma_rate_kernel<<<blocks, 288, smem, st>>>(c, out);
+    wgmma_selftest_kernel<N><<<1, 256, bytes, st>>>(K, mode, A, B, D);
     return cudaGetLastError();
 }
 
-
-// ---- realistic variant: a stream of [128 x N x 128] GEMMs as the forward issues them ------------------------------------------
-// 3 products x (128 / Kstep) k-steps with the real operand walk: A (hi | lo) in TMEM columns [256, 512) (or in shared memory),
-// B (hi | lo) image [N][128] in the K-major core-matrix layout.  distinct = 0 repeats the first k-step's addresses instead.
-struct GemmRateCfg { int N, a_smem, kind_tf32, readers, reader_op, ngemm, distinct, n_split, swz; };
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr) {   // K-major SWIZZLE_128B: SBO = 1024 (8 rows x 128 B), LBO unused
-    return (uint64_t)((saddr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t)(1024u >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-
-__global__ void __launch_bounds__(288, 1) umma_gemm_rate_kernel(GemmRateCfg c, long long* __restrict__ out) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    __shared__ uint32_t tmem_base_s;
-    __shared__ __align__(8) uint64_t bar_mma;
-    __shared__ volatile int done_flag;
-    const int tid = threadIdx.x, warp = tid >> 5;
-    for (int i = tid; i < 196608 / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(smem_raw)[i] = 0u;
-    if (warp == 0) tc::tmem_alloc(&tmem_base_s, tc::kTmemCols);
-    if (tid == 0) { mbar_init(&bar_mma, 1); fence_barrier_init(); done_flag = 0; }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    tc::fence_before_sync();
-    __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t tbase = __shfl_sync(0xffffffffu, tmem_base_s, 0);
-    const uint32_t lane_base = tbase + ((uint32_t)((warp & 3) * 32) << 16);
-    if (warp < 8) {
-        uint32_t z[16];
-#pragma unroll
-        for (int j = 0; j < 16; ++j) z[j] = 0u;
-        for (uint32_t col = (uint32_t)(warp >> 2) * 256u; col < (uint32_t)(warp >> 2) * 256u + 256u; col += 16) tc::tmem_st16(lane_base + col, z);
-        tc::wait_st();
-    }
-    tc::fence_before_sync();
-    __syncthreads();
-    tc::fence_after_sync();
-    long long iters = 0;
-    if (warp == 8) {
-        uint32_t leader_;
-        asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(leader_));
-        const bool leader = leader_ != 0;
-        {
-            const uint32_t N = (uint32_t)c.N, esz = c.kind_tf32 ? 4u : 2u, kstep = c.kind_tf32 ? 8u : 16u, nks = 128u / kstep;
-            const uint32_t nsplit = c.n_split > 1 ? (uint32_t)c.n_split : 1u, Nd = N / nsplit;       // dispatch width
-            const uint32_t idesc = c.kind_tf32 ? tc::make_idesc_tf32(128, Nd) : tc::make_idesc_bf16(128, Nd, false, false);
-            const uint32_t row_grp = (128u * esz / 16u) * 128u;                 // SBO: one 8-row group = 128 K elements
-            const uint32_t b_img = N * 128u * esz, a_img = 128u * 128u * esz;
-            const uint32_t b_s = tc::smem_addr(smem_raw), a_s = b_s + 2u * b_img;
-            const uint32_t a_cols = 128u * esz / 4u;                            // TMEM columns of one A part
-            const long long t0 = clock64();
-            for (int g = 0; g < c.ngemm; ++g) {
-                for (uint32_t h = 0; h < nsplit; ++h) {
-                    const uint32_t dcol = tbase + h * Nd;
-                    for (uint32_t p = 0; p < 3; ++p) {
-                        for (uint32_t ks = 0; ks < nks; ++ks) {
-                            const uint32_t kk = c.distinct ? ks : 0u;
-                            const uint32_t boff = (p == 1 ? b_img : 0u) + h * (Nd / 8u) * row_grp + kk * 256u;
-                            // SWIZZLE_128B: [N][128 B] K-blocks of 4 k-steps; a k-step advances the start address by 32 B
-                            const uint32_t boff_sw = (p == 1 ? b_img : 0u) + (kk >> 2) * (N * 128u) + h * (Nd / 8u) * 1024u + (kk & 3u) * 32u;
-                            const uint64_t bd = c.swz ? make_smem_desc_sw128(b_s + boff_sw) : tc::make_smem_desc(b_s + boff, 128u, row_grp);
-                            const bool acc = p > 0 || ks > 0;
-                            if (!leader) continue;
-                            if (c.kind_tf32) {
-                                tc::umma_tf32_ts(dcol, tbase + 256u + (p == 0 ? a_cols : 0u) + kk * 8u, bd, idesc, acc);
-                            } else if (c.a_smem) {
-                                const uint64_t ad = c.swz ? make_smem_desc_sw128(a_s + (p == 0 ? a_img : 0u) + (kk >> 2) * (128u * 128u) + (kk & 3u) * 32u)
-                                                          : tc::make_smem_desc(a_s + (p == 0 ? a_img : 0u) + kk * 256u, 128u, row_grp);
-                                tc::umma_bf16_ss(dcol, ad, bd, idesc, acc);
-                            } else {
-                                tc::umma_bf16_ts(dcol, tbase + 256u + (p == 0 ? a_cols : 0u) + kk * 8u, bd, idesc, acc);
-                            }
-                        }
-                    }
-                }
-            }
-            const long long t1 = clock64();
-            if (leader) tc::umma_commit(&bar_mma);
-            mbar_wait(&bar_mma, 0);
-            const long long t2 = clock64();
-            if (leader) {
-                done_flag = 1;
-                out[blockIdx.x * 4 + 0] = t1 - t0;
-                out[blockIdx.x * 4 + 1] = t2 - t0;
-            }
-        }
-    } else if (warp < c.readers && c.reader_op) {
-        uint32_t v[16];
-#pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] = 0u;
-        const uint32_t col0 = 128u + (uint32_t)(warp >> 2) * 48u;   // columns [128, 224): not touched by the MMAs (N <= 128)
-        while (!done_flag) {
-#pragma unroll 1
-            for (uint32_t k = 0; k < 3; ++k) {
-                if (c.reader_op == 1) { tc::tmem_ld16(lane_base + col0 + k * 16u, v); tc::wait_ld(); }
-                else { tc::tmem_st16(lane_base + col0 + k * 16u, v); tc::wait_st(); }
-                ++iters;
-            }
-        }
-        if ((tid & 31) == 0) atomicAdd(reinterpret_cast<unsigned long long*>(out + blockIdx.x * 4 + 2), (unsigned long long)iters + (v[3] & 1u));
-    }
-    tc::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc(tbase, tc::kTmemCols);
-}
-
-cudaError_t launch_umma_gemm_rate(const int cfg[8], long long* out, int blocks, cudaStream_t st) {
-    GemmRateCfg c{cfg[0], cfg[1], cfg[2], cfg[3], cfg[4], cfg[5], cfg[6] & 1, cfg[7], (cfg[6] >> 1) & 1};
-    if ((c.N != 64 && c.N != 128) || c.readers < 0 || c.readers > 8 || c.ngemm < 1) return cudaErrorInvalidValue;
-    if (c.kind_tf32 && c.a_smem) return cudaErrorInvalidValue;
-    const size_t smem = 196608 + 1024;
-    cudaError_t e = cudaFuncSetAttribute(umma_gemm_rate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    umma_gemm_rate_kernel<<<blocks, 288, smem, st>>>(c, out);
-    return cudaGetLastError();
-}
-
+}  // namespace
 }  // namespace g4d
 
-// ---- C entry of the stand-alone self-test library (libg4d_selftest.so; NOT part of libg4d.so / include/g4d.h) -------------
-// cfg = {N, K, layout_mode, swap_desc, a_cols_per_k, use_tma, single_pass | 16 for the bf16 variant, version_bit}
-extern "C" int g4d_selftest_umma(const int* cfg, const float* A, const float* B, float* D, void* stream) {
-    if (!cfg || !A || !B || !D) return -2;
+// cfg = (N, K, mode): N in {16, 48, 128}, K a multiple of 16 up to 128, mode 0..4 (above)
+extern "C" int g4d_selftest_wgmma(const int* cfg, const float* A, const float* B, float* D, void* stream) {
+    const int N = cfg[0], K = cfg[1], mode = cfg[2];
+    if (K <= 0 || K > 128 || K % 16 != 0 || mode < 0 || mode > 4) return -1;
     cudaStream_t st = (cudaStream_t)stream;
-    if (cfg[6] == 16) return g4d::launch_umma16_selftest(cfg, A, B, D, st) == cudaSuccess ? 0 : -1;
-    static float* scratch = nullptr;
-    if (!scratch && cudaMalloc(&scratch, (size_t)2 * 128 * 128 * 4 + 256) != cudaSuccess) return -3;
-    return g4d::launch_umma_selftest(cfg, A, B, scratch, D, st) == cudaSuccess ? 0 : -1;
-}
-
-// cfg = {N, a_smem, kind_tf32, reader warps, reader op (0 none, 1 tcgen05.ld, 2 tcgen05.st), dispatches, column distance of the
-// two alternating accumulators (0: one accumulator), 0}; out[blocks][4] (device, zeroed by the caller):
-// issue cycles, total cycles, reader iterations (16 columns x 32 lanes each)
-extern "C" int g4d_selftest_umma_rate(const int* cfg, long long* out, int blocks, void* stream) {
-    if (!cfg || !out || blocks < 1) return -2;
-    return g4d::launch_umma_rate(cfg, out, blocks, (cudaStream_t)stream) == cudaSuccess ? 0 : -1;
-}
-
-// cfg = {N (64 | 128), a_smem, kind_tf32, reader warps, reader op, GEMMs, bit 0: distinct addresses (1 = the real operand walk) |
-// bit 1: SWIZZLE_128B operand images instead of the SWIZZLE_NONE core-matrix layout,
-// n_split (dispatch width N / n_split)}; out as above
-extern "C" int g4d_selftest_umma_gemm_rate(const int* cfg, long long* out, int blocks, void* stream) {
-    if (!cfg || !out || blocks < 1) return -2;
-    return g4d::launch_umma_gemm_rate(cfg, out, blocks, (cudaStream_t)stream) == cudaSuccess ? 0 : -1;
+    cudaError_t e = cudaErrorInvalidValue;
+    if (N == 128) e = g4d::launch_n<128>(K, mode, A, B, D, st);
+    else if (N == 48) e = g4d::launch_n<48>(K, mode, A, B, D, st);
+    else if (N == 16) e = g4d::launch_n<16>(K, mode, A, B, D, st);
+    return e == cudaSuccess ? 0 : -1;
 }

@@ -1,5 +1,5 @@
 """Drop-in for ``scene.deformation.deform_network`` (/root/reference/scene/deformation.py:161-216) backed by
-the sm_100a kernels of libg4d.so.
+the sm_90a kernels of libg4d.so.
 
 Contract kept (SURVEY.md §8b, App. B.4):
   * ctor reads the same ``args`` fields; ``forward(point, scales, rotations, opacity, shs, times_sel)`` -> 5-tuple;
@@ -10,7 +10,7 @@ Contract kept (SURVEY.md §8b, App. B.4):
     scene/__init__.py:83 and scene/gaussian_model.py:539-564;
   * parameters are ordinary leaf ``nn.Parameter`` objects that an optimizer updates in place.
 
-B200-native storage: every plane Parameter is a ``[1,C,H,W]`` tensor in ``torch.channels_last`` memory, i.e.
+Kernel-native storage: every plane Parameter is a ``[1,C,H,W]`` tensor in ``torch.channels_last`` memory, i.e.
 physically ``[H][W][C]`` -- the kernels read it (and scatter gradients into a same-layout tensor) directly, no
 per-step transposes; shape-wise it is indistinguishable from the reference's tensor.
 """

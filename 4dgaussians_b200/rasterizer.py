@@ -2,7 +2,7 @@
 (/root/reference/gaussian_renderer/__init__.py:14; merge_many_4dgs.py:33; scene/dataset_readers.py:485).
 
 Same names, argument meaning and error behaviour as the upstream Python surface (SURVEY.md §8b, App. A.5);
-behind it the hand-written sm_100a kernels of libg4d.so through the C-ABI (include/g4d.h).  PyTorch is only
+behind it the hand-written sm_90a kernels of libg4d.so through the C-ABI (include/g4d.h).  PyTorch is only
 plumbing here: device memory, the current stream, autograd bookkeeping.
 """
 from __future__ import annotations

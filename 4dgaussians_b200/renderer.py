@@ -3,7 +3,7 @@
 Same signature, same result dict (``render, viewspace_points, visibility_filter, radii, depth``), same quirks
 (``time`` may be a float / 0-d tensor / int; PanopticSports cameras are dicts carrying a prebuilt settings object).
 What changes is underneath: when ``pc._deformation`` is the g4d ``deform_network`` the whole of
-deform -> activations -> rasterize runs as ONE C-ABI call into hand-written sm_100a kernels
+deform -> activations -> rasterize runs as ONE C-ABI call into hand-written sm_90a kernels
 (``g4d_render_forward`` / ``g4d_render_backward``): no [N,F] feature temporaries, no ``time.repeat(N,1)``,
 no ``torch.cat`` of the SH features, no per-call ``.cuda()`` copies of the camera matrices.
 """

@@ -169,6 +169,8 @@ def hidden_args(net: str):
         "shs128": dict(channels=16, resolution=[8, 8, 8, 6], multires=[1, 2], net_width=128, no_do=True, no_dshs=False,
                        no_dx=True, no_ds=True, no_dr=True),                                       # only the 48-wide head
         "c32w128": dict(channels=32, resolution=[10, 9, 8, 6], multires=[1, 2], net_width=128, no_do=False, no_dshs=True),
+        # F = 64 with all five heads: the largest shared-memory layout of the tensor-core kernels
+        "c32w128sh": dict(channels=32, resolution=[10, 9, 8, 6], multires=[1, 2], net_width=128, no_do=False, no_dshs=False),
     }
     c = cfgs[net]
     return Namespace(net_width=c["net_width"], timebase_pe=4, defor_depth=1, posebase_pe=10, scale_rotation_pe=2, opacity_pe=2,

@@ -1,7 +1,7 @@
 """Data-parallel training harness around the render path (SURVEY.md 8f N1).
 
 Mirrors the shape of the reference's fine-stage loop -- /root/reference/train.py:108-296 (``scene_reconstruction``) with the
-optimizer / densification bookkeeping of /root/reference/scene/gaussian_model.py:165-212, 316-413, 415-523 -- but B200-first:
+optimizer / densification bookkeeping of /root/reference/scene/gaussian_model.py:165-212, 316-413, 415-523 -- but GPU-first:
 
   * scene replicated, views sharded round-robin over ranks (one process per GPU); every rank renders its B views
     (fused forward + backward), the image loss and the HexPlane regularisers are the fused kernels of ``losses.py``;

@@ -5,6 +5,7 @@
     python bench.py --gpus N --steps K --warmup W            # our arm (CUDA path through the public API)
     python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU implementation of the path
     python bench.py --workload C1|C2|C3|C4                   # other BASELINE.json configs (default C3, the metric's)
+    python bench.py ... --dump-outputs DIR                   # also write the outputs of the last view of the last timed step
 
 A "step" is one pass of the hot path over one BATCH of synthetic views: `--views-per-step` (default 32) fused
 deform + rasterize FORWARDS of the workload, back to back -- so that `--steps 20` times >= 0.5 s of device work instead of
@@ -14,7 +15,7 @@ L1 loss + flat-bucket all-reduce + Adam).
 
 Timing: one CUDA-event pair per step on the launching stream, W warm-up steps (same code path and the same output
 bindings as the timed steps), an L2 flush (512 MiB write) between steps outside the event pairs -- inside a step every
-view moves ~0.3 GB (instance lists + images), more than the 126 MB L2, so consecutive views evict one another --
+view moves ~0.3 GB (instance lists + images), more than the 50 MB L2 of an H100, so consecutive views evict one another --
 barrier + synchronize on both sides of the timed region, MAX over ranks.
 `value` = inputs resident in HBM; `e2e` = the same steps through the public `render()` with the camera arriving from host
 memory and every rendered image copied to pinned host memory (double-buffered, on a copy stream, inside the step's event
@@ -72,7 +73,7 @@ def _hbm_peak():
     j = _peaks_json()
     if "hbm_gbs" in j:
         return float(j["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 def mlp_flops_per_gaussian(net):
@@ -88,16 +89,15 @@ def _tensor_roofline(net, n, geom_ms):
     if "bf16_tflops_sustained" in j:
         peak, src = float(j["bf16_tflops_sustained"]), "measured (MEASURED_PEAKS.json bf16_tflops_sustained)"
     else:
-        peak, src = 2250.0, "fallback (nominal dense bf16 2.25 PFLOP/s)"
+        peak, src = 989.0, "fallback (H100 SXM data sheet, dense bf16 989 TFLOP/s)"
     flops = mlp_flops_per_gaussian(net) * n
     ach = flops / (geom_ms * 1e-3) / 1e12 if geom_ms > 0 else 0.0
-    return {"bound": "tensor", "kernel": "deform_features + deform_f16_kernel (stage `geom`: HexPlane gather, then the fused "
-                                         "deform MLP + activations + projection + SH colour on tcgen05)", "achieved": ach, "peak": peak,
+    return {"bound": "tensor", "kernel": "deform_features + deform_tc_kernel (stage `geom`: HexPlane gather, then the fused "
+                                         "deform MLP + activations + projection + SH colour on wgmma)", "achieved": ach, "peak": peak,
             "unit": "TFLOP/s", "frac": ach / peak if peak else None, "peak_source": src, "algorithmic_flops": flops,
             "kernel_ms": geom_ms,
             "note": "fp32-accurate FP16x2 operands: every algorithmic MAC is 3 tensor-core MACs at the f16 rate, so the ceiling "
-                    "of this scheme is peak/3 (frac 0.333) -- 0.28 with the measured 76-cycle 128x128x16 dispatch; net_width 64 "
-                    "(dnerf) runs the FP32 FFMA kernel"}
+                    "of this scheme is peak/3 (frac 0.333); net_width 64 (dnerf) runs the FP32 FFMA kernel"}
 
 
 def _blend_roofline(pairs, blend_ms, sm_count):
@@ -105,7 +105,7 @@ def _blend_roofline(pairs, blend_ms, sm_count):
     pairs = sum over pixels of the index of the last instance the pixel had to look at (n_contrib) = the evaluations the
     reference algorithm performs; 27 flop + 1 ex2 each (dx,dy; quadratic form; exp; alpha clamp/tests; T update; 4 FMA)."""
     j = _peaks_json()
-    mhz = float(j.get("sm_max_mhz", 1965.0))
+    mhz = float(j.get("sm_max_mhz", 1980.0))
     fp32 = sm_count * 128 * 2 * mhz * 1e6           # flop/s
     mufu = sm_count * 16 * mhz * 1e6                # ex2/s
     peak_pairs = min(fp32 / 27.0, mufu)
@@ -295,7 +295,7 @@ def run_ours(args):
             out = resident_step(i)
         gc.collect(); gc.disable()     # a host hiccup shows up 1:1 in a ~1 ms view
         barrier()
-        # ranks leave the collective barrier at different times and an idle B200 drops its clocks within milliseconds:
+        # ranks leave the collective barrier at different times and an idle GPU drops its clocks within milliseconds:
         # one more untimed step, then the synchronize that brackets the timed region
         out = resident_step(Wm)
         torch.cuda.synchronize(dev)
@@ -309,6 +309,8 @@ def run_ours(args):
         barrier()
         t_wall = time.perf_counter() - t_wall0
         gc.enable()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out)
     step_ms = [a.elapsed_time(b) for a, b in ev]
     # the stage events of the last view of the last timed step (same context: no-grad renders release it at once)
     in_region_stage_ms = ws._free_contexts[-1].stage_times() if ws._free_contexts else {}
@@ -364,9 +366,10 @@ def run_ours(args):
         main_stream.wait_event(done[0]); main_stream.wait_event(done[1])   # the step ends when its last image is on the host
 
     with torch.no_grad():
-        e2e_step(0)
+        for i in range(Wm):                 # same warm-up as the resident arm: W steps, the barrier, one untimed step
+            e2e_step(i)
         barrier()
-        e2e_step(1)
+        e2e_step(Wm)
         torch.cuda.synchronize(dev)
         for i in range(K):
             flush.fill_(i & 0xFF)
@@ -387,7 +390,7 @@ def run_ours(args):
     # ------------------------------------------------------------------ training step (B=2 views, fwd+bwd, all-reduce, Adam)
     train = None
     if not args.no_train:
-        train = run_train_steps(g4d, synth, lib, w, scene, mod, dev, dist, world, rank, max(3, min(K, 10)), 5, flush)
+        train = run_train_steps(g4d, synth, lib, w, scene, mod, dev, dist, world, rank, K, Wm, flush)
     clocks = sampler.stop() if rank == 0 else None     # sampled from the start of the timed region to the end of the train steps
 
     eager = None
@@ -415,9 +418,9 @@ def run_ours(args):
             pass
         ms_per_view = total_ms / (K * V)
         srt = sorted(step_ms)
-        # headline roofline = the geometry kernel (the one VERDICT.md r1 names).  It does 780 algorithmic flop per byte of its
-        # SURVEY-8d traffic, far above the machine balance (1442 TFLOP/s / 6.5 TB/s = 222 flop/B): its roof is the tensor pipe,
-        # so `bound` is "tensor"; the HBM view of the same stage is kept next to it (geom_hbm_*), DRAM traffic from ncu.
+        # headline roofline = the geometry kernel.  It does 780 algorithmic flop per byte of its SURVEY-8d traffic, far above
+        # the H100's balance (989 TFLOP/s / 3.35 TB/s = 295 flop/B): its roof is the tensor pipe, so `bound` is "tensor"; the
+        # HBM view of the same stage is kept next to it (geom_hbm_*).
         geom_ms = fwd_stages.get("geom", 0.0)
         if NETS[w["net"]]["Wd"] == 128 and geom_ms > 0:
             roofline_main = _tensor_roofline(w["net"], w["n"], geom_ms)
@@ -444,10 +447,10 @@ def run_ours(args):
                        "focal_px": w["focal"], "orbit_radius": w["radius"], "scale_mean": w["scale_mean"],
                        "tile_instances_R": R, "visible_gaussians": float(np.mean(vis)) if vis else None,
                        "l2": "flushed between timed steps (512 MiB write, outside the event pairs); inside a step each view "
-                             "moves ~%.2f GB > 126 MB L2" % (ab["total"] / 1e9),
+                             "moves ~%.2f GB > 50 MB L2" % (ab["total"] / 1e9),
                        "binning": "host sync on R (exact sizing)" if args.host_sync else
                                   "device-side R, capacity-bounded, no host sync (overflow-checked)",
-                       "mlp": "tcgen05 FP16x2 forward (hi+lo operands, 3 products, fp32-accurate), BF16x2 tcgen05 backward" if NETS[w["net"]]["Wd"] == 128
+                       "mlp": "wgmma FP16x2 forward (hi+lo operands, 3 products, fp32-accurate), BF16x2 wgmma backward" if NETS[w["net"]]["Wd"] == 128
                               else "FP32 FFMA (net_width 64)",
                        "launch": "programmatic dependent launch between the kernels of a view" if os.environ.get("G4D_PDL", "1") != "0"
                                  else "ordinary stream order (G4D_PDL=0)",
@@ -468,7 +471,7 @@ def run_ours(args):
             "gpu_launches_note": "own kernels per view (fused forward): " + ", ".join(LAUNCH_LIST[0 if NETS[w["net"]]["Wd"] == 128 else 1]),
             "clocks": clocks,
             "roofline": roofline_main,
-            "roofline_hbm": {"bound": "hbm", "kernel": {"geom": "deform_features + deform_f16_kernel (fused deform+activate+project, tcgen05)"
+            "roofline_hbm": {"bound": "hbm", "kernel": {"geom": "deform_features + deform_tc_kernel (fused deform+activate+project, wgmma)"
                                                         if NETS[w["net"]]["Wd"] == 128 else "deform_kernel (FFMA)",
                                                         "blend": "blend_forward_kernel", "binning": "bin_sort + bin_place + bin_fix"}[dom],
                              "what": "the longest stage of the forward against the HBM roof (SURVEY 8d bytes of that stage)",
@@ -486,13 +489,35 @@ def run_ours(args):
             "parity_check": parity, "gpu_eager_baseline": eager,
         }
         if world == 1 and not args.no_cpu_baseline:
-            line["cpu_baseline"] = cpu_reference_arm(wl, steps=2, warmup=1)["cpu_baseline"]
+            line["cpu_baseline"] = cpu_reference_arm(wl, steps=args.cpu_baseline_views, warmup=1)["cpu_baseline"]
         print(json.dumps(line))
     if dist is not None:
         dist.destroy_process_group()
 
 
-LAUNCH_LIST = (["pack_camera", "collapse_time_rows", "deform_features", "deform_f16_kernel", "bin_sort (cooperative)",
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(path, out):
+    """The arrays render() returned for ONE view -- the last of the `--views-per-step` views of the last timed step -- as
+    float32 <path>/<name>.npy (render [3,H,W], depth [1,H,W], radii [N]).  The inputs are fixed by the arguments (seeded
+    scene, orbit cameras), so two builds can be compared output for output.  When the three together exceed the 64 MiB
+    budget, each is stored as the same fixed sample of its flattened elements: the first `keep` entries, in ascending order,
+    of torch.randperm(numel) under a generator seeded 0 (reproducible from numel and keep alone, so nothing else is written)."""
+    os.makedirs(path, exist_ok=True)
+    arrays = {k: out[k].detach().float().reshape(-1) for k in ("render", "depth", "radii")}
+    total = sum(a.numel() for a in arrays.values()) * 4
+    for name, a in arrays.items():
+        if total > DUMP_BYTES:
+            keep = int(a.numel() * DUMP_BYTES / total * 0.95)
+            gen = torch.Generator().manual_seed(0)
+            idx = torch.randperm(a.numel(), generator=gen)[:keep].sort().values
+            np.save(os.path.join(path, name + ".npy"), a.cpu()[idx].numpy())
+        else:
+            np.save(os.path.join(path, name + ".npy"), a.reshape(out[name].shape).cpu().numpy())
+
+
+LAUNCH_LIST = (["pack_camera", "collapse_time_rows", "deform_features", "deform_tc_kernel", "bin_sort (cooperative)",
                 "bin_place", "bin_fix", "blend_forward"],
                ["pack_camera", "collapse_time_rows", "deform_kernel", "bin_sort (cooperative)", "bin_place", "bin_fix", "blend_forward"])
 
@@ -716,10 +741,8 @@ def run_reference(args):
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
-    steps = min(args.steps, 8)          # one step = one full view (~1-2 s of CPU work): bounded sample
-    line = cpu_reference_arm(args.workload, steps=steps, warmup=min(args.warmup, 2))
+    line = cpu_reference_arm(args.workload, steps=args.steps, warmup=args.warmup)
     line["n_gpus"] = args.gpus
-    line["steps"] = steps
     print(json.dumps(line))
 
 
@@ -732,9 +755,14 @@ def main():
     ap.add_argument("--workload", default="C3", choices=["C1", "C2", "C3", "C4"])
     ap.add_argument("--views-per-step", dest="views_per_step", type=int, default=32)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--cpu-baseline-views", dest="cpu_baseline_views", type=int, default=2,
+                    help="views timed by the `cpu_baseline` sample of the g4d arm (one view = 1-2 s of CPU work)")
     ap.add_argument("--no-parity-check", action="store_true")
     ap.add_argument("--no-eager-baseline", action="store_true")
     ap.add_argument("--no-train", action="store_true")
+    ap.add_argument("--dump-outputs", dest="dump_outputs", default=None, metavar="DIR",
+                    help="write render, depth and radii of the last view of the last timed step as float32 DIR/<name>.npy "
+                         "(bench_outputs/ inside the tree is git-ignored)")
     ap.add_argument("--host-sync", dest="host_sync", action="store_true",
                     help="size the instance buffer exactly with one host read of R per forward (the reference's behaviour) "
                          "instead of the default capacity-bounded device-side binning")

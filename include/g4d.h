@@ -1,5 +1,5 @@
 /*
- * g4d -- C-ABI of the B200-native fused deform + rasterize render path for 4D Gaussian Splatting.
+ * g4d -- C-ABI of the H100-native fused deform + rasterize render path for 4D Gaussian Splatting.
  *
  * Plain C, plain pointers and sizes, no torch types.  Every pointer named `d_*` or documented as
  * "device" is a CUDA device pointer on the workspace's device; everything else is host memory.
@@ -221,11 +221,12 @@ enum { G4D_OPT_SYNC_MODE = 1,  /* 1 (default): size the instance buffer exactly 
        G4D_OPT_STAGE_TIMING = 4, /* 1: bracket every stage with CUDA events on the launching stream
                                    (bench.py's live per-kernel durations); 0 (default): off */
        G4D_OPT_TENSOR_CORES = 5, /* the deformation MLP's forward when the configuration allows tensor cores (net_width 128,
-                                   C in {16,32}, F <= 64): 2 (default) tcgen05 with FP16x2 operands (hi + lo halves, 3 products,
+                                   C in {16,32}, F <= 64): 2 (default) wgmma with FP16x2 operands (hi + lo halves, 3 products,
                                    fp32-accurate; operands must stay below 65504 after scaling -- activations < 8188, features
-                                   < 1023, weights < 255 -- else the NEXT call returns G4D_ERR_OVERFLOW), two tiles in flight per
-                                   SM; 1: tcgen05 3xTF32 (no range limit); 0: FP32 FFMA kernels */
-       G4D_OPT_TC_DEBUG = 6,     /* 1: the tensor-core kernel records per-phase cycle counters (g4d_debug_tc_cycles) */
+                                   < 1023, weights < 255 -- else the NEXT call returns G4D_ERR_OVERFLOW); 1: wgmma 3xTF32 (no
+                                   range limit); 0: FP32 FFMA kernels */
+       G4D_OPT_TC_DEBUG = 6,     /* 1: the tensor-core forward records cycle counters per CTA (g4d_debug_tc_cycles: [0] whole
+                                   kernel, [1] waiting for W1 images, [2..11] unused) */
        G4D_OPT_KEEP_DEFORMED = 8, /* 1: a no-grad fused forward (G4D_CAM_NO_GRAD) still stores the deformed + activated tensors
                                    * (G4D_BUF_DEFORMED / _SHS reads); default 0: it skips those 48-240 B / Gaussian of writes */
        G4D_OPT_WARP_CULL = 7,    /* 1 (default): the blend kernels skip, per warp, instances that cannot reach alpha >= 1/255
@@ -269,7 +270,7 @@ enum { G4D_STAGE_PREP = 0,        /* camera pack, weight pack, time-row collapse
        G4D_STAGE_COUNT = 10 };
 int g4d_context_stage_times(G4DContext *ctx, float *out_ms, int capacity);
 
-/* DEBUG: mean per-CTA cycles the last tensor-core deform launch spent in each of its 12 phases (G4D_OPT_TC_DEBUG). */
+/* DEBUG: mean per-CTA cycle counters of the last tensor-core deform launch (G4D_OPT_TC_DEBUG). */
 int g4d_debug_tc_cycles(G4DWorkspace *ws, double *out12);
 
 #ifdef __cplusplus

@@ -1,7 +1,7 @@
 """CPU restatement of simple_knn._C.distCUDA2 (SURVEY.md 8f N4).  TEST INFRASTRUCTURE ONLY.
 
 PARITY UNPINNED by the reference: submodules/simple-knn is an empty directory in /root/reference (no source, no tests, no
-binary on the GPU box: profiles/r2_probe_step0.txt).  Anchored on the call site scene/gaussian_model.py:148
+binary).  Anchored on the call site scene/gaussian_model.py:148
 (``dist2 = torch.clamp_min(distCUDA2(points), 0.0000001); scales = log(sqrt(dist2))``) and on the published algorithm of
 graphdeco-inria/simple-knn (spatial.cu / simple_knn.cu): exact 3 nearest neighbours by squared Euclidean distance, self
 excluded by index, result (d0 + d1 + d2) / 3 in fp32.

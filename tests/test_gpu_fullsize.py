@@ -1,6 +1,6 @@
 """Full-size GPU parity: BASELINE.json configs C1 (70k, 800x800, dnerf net -> FFMA kernels), C2 (200k, 536x960, hypernerf
 net, L=3) and C3 (300k, 1352x1014, dynerf net, 5 heads) against the CPU oracle -- the sizes at which the persistent tile
-loops (148 CTAs x 16 tiles), the 85 x 64 tile grid, ~3 M tile instances and the chunked counting placement actually run.
+loops (132 CTAs x 18 tiles on an H100), the 85 x 64 tile grid, ~3 M tile instances and the chunked counting placement actually run.
 
 Structure of the proof for the fused path (SURVEY 7 "bit-exact ... given identical post-deformation inputs"):
   (i)   the deformed + activated tensors the fused kernel produced are within fp32 rounding of the oracle's deformation;

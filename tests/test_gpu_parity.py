@@ -85,7 +85,7 @@ def test_rasterizer_forward_indices_bit_exact_and_image(ci):
 @pytest.mark.parametrize("n", [8_000, 14_000, 25_000, 45_000])
 def test_binning_long_sub_segments_bit_exact(n):
     """Every Gaussian covers (nearly) every tile of a 4 x 3 tile image: a (tile, chunk) sub-segment of the placement holds
-    ~n / 148 entries -- 54, 95, 169, 304 -- i.e. the warp-cooperative rank paths of bin_fix_kernel with 2, 4 and 8 entries per
+    ~n / 132 entries on an H100 -- 61, 106, 189, 341 -- i.e. the warp-cooperative rank paths of bin_fix_kernel with 2, 4 and 8 entries per
     lane and the > 256 fallback.  Sorted keys / ids / ranges stay bit-identical to the reference order."""
     c = dict(n=n, seed=11, wh=(64, 48), theta=35.0, radius=3.0, deg=0, bg=(0.0, 0.0, 0.0), scale_mean=0.3)
     cam, ins, rc = _raster_case(**c)
@@ -339,7 +339,8 @@ class _Pipe:
 
 FUSED_CASES = [dict(net="small64", n=900, wh=(96, 64), theta=20.0, radius=4.0, t=0.3, deg=3, bg=(1.0, 1.0, 1.0), scale=0.08),
                dict(net="small128", n=1100, wh=(80, 112), theta=-50.0, radius=2.0, t=0.8, deg=2, bg=(0.0, 0.0, 0.0), scale=0.05),
-               dict(net="dynerf", n=2500, wh=(203, 152), theta=100.0, radius=2.2, t=0.5, deg=3, bg=(0.0, 0.0, 0.0), scale=0.04)]
+               dict(net="dynerf", n=2500, wh=(203, 152), theta=100.0, radius=2.2, t=0.5, deg=3, bg=(0.0, 0.0, 0.0), scale=0.04),
+               dict(net="c32w128sh", n=1300, wh=(120, 90), theta=30.0, radius=2.4, t=0.6, deg=3, bg=(0.2, 0.1, 0.0), scale=0.05)]
 
 
 def _fused_setup(c, stage="fine", grad=True):
@@ -575,26 +576,31 @@ def test_full_size_binning_properties():
 
 
 # --------------------------------------------------------------------------------------------------- tensor cores
-def test_tcgen05_building_blocks_selftest():
-    """D[128,N] = A[128,K] B[N,K]^T through TMEM / tcgen05.mma kind::tf32 with 3xTF32: fp32-level accuracy."""
+def test_wgmma_building_blocks_selftest():
+    """D[128,N] = A[128,K] B[N,K]^T through the wgmma building blocks in every operand arrangement the kernels use (register or
+    shared-memory A, K-major or MN-major operands) with the hi / lo split and three products: fp32-level accuracy for 3xTF32 and
+    FP16x2, ~16 bits for BF16x2."""
     import ctypes as C
     lib = g4d._lib.load_selftest()      # own tiny library: the self test is not part of the product libg4d.so
-    for (N, K, tma) in ((128, 128, 1), (128, 32, 1), (48, 64, 0), (16, 64, 1)):
-        gen = torch.Generator().manual_seed(N + K)
-        A = torch.randn(128, K, generator=gen).cuda(); B = torch.randn(N, K, generator=gen).cuda()
-        D = torch.zeros(128, N, device="cuda")
-        cfg = (C.c_int * 8)(N, K, 0, 0, 1, tma, 0, 1)
-        assert lib.g4d_selftest_umma(cfg, A.data_ptr(), B.data_ptr(), D.data_ptr(), 0) == 0
-        torch.cuda.synchronize()
-        ref = A.double() @ B.double().t()
-        assert float((D.double() - ref).abs().max() / ref.abs().max()) <= 2e-6, (N, K)
+    tol = {0: 2e-6, 1: 2e-6, 2: 3e-5, 3: 3e-5, 4: 3e-5}
+    for mode in range(5):
+        for (N, K) in ((128, 128), (128, 32), (48, 64), (16, 64), (48, 48)):
+            gen = torch.Generator().manual_seed(N + K + mode)
+            A = torch.randn(128, K, generator=gen).cuda(); B = torch.randn(N, K, generator=gen).cuda()
+            D = torch.zeros(128, N, device="cuda")
+            cfg = (C.c_int * 3)(N, K, mode)
+            assert lib.g4d_selftest_wgmma(cfg, A.data_ptr(), B.data_ptr(), D.data_ptr(), 0) == 0
+            torch.cuda.synchronize()
+            ref = A.double() @ B.double().t()
+            err = float((D.double() - ref).abs().max() / ref.abs().max())
+            assert err <= tol[mode], (mode, N, K, err)
 
 
 @pytest.mark.parametrize("tcmode", [2, 1])
 @pytest.mark.parametrize("net,n", [("small128", 1000), ("dynerf", 5000), ("hypernerf", 3000), ("dynerf", 40000)])
 def test_tensor_core_mlp_matches_ffma_path(net, n, tcmode):
-    """The tcgen05 MLPs (2: FP16x2 operands, two tiles in flight per SM -- the default; 1: 3xTF32) and the FP32 FFMA MLP are
-    implementations of the same function.  40000 Gaussians = 313 tiles: CTAs with one pair, one and a half, and two pairs."""
+    """The wgmma MLPs (2: FP16x2 operands -- the default; 1: 3xTF32) and the FP32 FFMA MLP are implementations of the same
+    function.  40000 Gaussians = 313 tiles of 128 (FP16x2) / 625 of 64 (3xTF32): persistent CTAs with two to five tiles."""
     mod = make_module(net, seed=7)
     ins, _ = _deform_inputs(n, 9)
     ws = g4d._lib.Workspace.get(0)
@@ -672,6 +678,35 @@ def test_fp16x2_range_violation_is_reported_and_tf32_path_has_no_limit():
         ws.set_option(g4d._lib.OPT_TENSOR_CORES, 2)
 
 
+def test_fp16x2_weight_out_of_range_is_reported():
+    """A weight whose scaled value (2^8 w) leaves the f16 range saturates when the FP16x2 images are packed: the pack kernel
+    raises the same flag as the forward, the NEXT call returns G4D_ERR_OVERFLOW, and after the weight is back in range the
+    images are re-packed and the results agree with the FFMA kernels again."""
+    mod = make_module("small128", seed=12)
+    n = 500
+    ins, _ = _deform_inputs(n, 5)
+    t = torch.tensor(0.4).repeat(n, 1).cuda()
+    ws = g4d._lib.Workspace.get(0)
+    w1 = mod.deformation_net.pos_deform[1].weight
+    keep = float(w1[0, 0])
+    try:
+        with torch.no_grad():
+            ws.set_option(g4d._lib.OPT_TENSOR_CORES, 2)
+            w1[0, 0] = 300.0                                            # 2^8 * 300 > 65504
+            mod(*ins, t)
+            torch.cuda.synchronize()
+            with pytest.raises(g4d._lib.G4DError, match="f16 operand range"):
+                mod(*ins, t)
+            w1[0, 0] = keep
+            c = [o.clone() for o in mod(*ins, t)]
+            ws.set_option(g4d._lib.OPT_TENSOR_CORES, 0)
+            d = [o.clone() for o in mod(*ins, t)]
+            for x, y in zip(c, d):
+                assert float((x - y).abs().max()) <= 5e-6
+    finally:
+        ws.set_option(g4d._lib.OPT_TENSOR_CORES, 2)
+
+
 def test_no_grad_render_skips_saved_tensors_unless_asked():
     """A torch.no_grad() render does not store the deformed tensors (they only serve a backward); G4D_OPT_KEEP_DEFORMED keeps
     them for the debug reads; the image is the same either way."""
@@ -707,7 +742,7 @@ def test_no_grad_render_skips_saved_tensors_unless_asked():
 @pytest.mark.parametrize("tcmode", [2, 1])
 @pytest.mark.parametrize("net,n", [("small128", 700), ("dynerf", 21000), ("hypernerf", 40000)])
 def test_tensor_core_backward_matches_ffma_path(net, n, tcmode):
-    """BF16x2 tcgen05 backward (dgrad + wgrad kernels) against the FP32 FFMA backward: same gradients for every input
+    """BF16x2 wgmma backward (dgrad + wgrad kernels) against the FP32 FFMA backward: same gradients for every input
     and every parameter.  n is chosen so that some CTAs own one tile and others two or three (persistent loop).
     The two paths take their ReLU signs from different places (bits saved by the tensor-core forward vs the FFMA kernel's own
     fp32 recomputation), so a Gaussian with a pre-activation within rounding of 0 may legitimately differ: the upstream
