@@ -6,13 +6,14 @@
 //   /root/reference/scene/deformation.py:97-148              heads ReLU-Linear-ReLU-Linear, residual add
 //
 // Layout decisions (DESIGN.md §3):
-//   * planes are channel-last [H][W][C] so one bilinear tap is one contiguous 64/128-byte line (L2 resident);
-//   * the three time planes are collapsed once per view to 1-D rows (every Gaussian shares t), halving taps;
+//   * the HexPlane sampling (channel-last planes, collapsed time rows) is hexplane.cuh's, shared with every other
+//     deformation kernel;
 //   * a CTA of 256 threads owns TG Gaussians; activations live in shared memory row-major [TG][K+4];
 //     W0^T and one head's W1^T are staged in shared memory ([K][Wd], W1^T by a TMA bulk copy that overlaps
 //     the previous head's epilogue); each thread accumulates an RM x (Wd/16) register tile with FFMA.
 #pragma once
 #include "g4d_common.cuh"
+#include "hexplane.cuh"
 
 namespace g4d {
 
@@ -93,24 +94,8 @@ G4D_D void tma_bulk_g2s(void* dst_smem, const void* src_gmem, uint32_t bytes, vo
 }
 G4D_D void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 
-// ---- bilinear sampling ------------------------------------------------------------------------------
-struct Tap1D { int i0, i1; float w0, w1; };
-
-// grid_sample unnormalise (align_corners=True) + border clamp + floor   (ATen grid_sampler_2d semantics)
-G4D_D Tap1D make_tap(float u, int size) {
-    float x = ((u + 1.f) / 2.f) * (float)(size - 1);
-    x = fminf(fmaxf(x, 0.f), (float)(size - 1));
-    float x0 = floorf(x);
-    Tap1D t;
-    t.i0 = (int)x0;
-    t.i1 = min(t.i0 + 1, size - 1);
-    t.w0 = (x0 + 1.f) - x;
-    t.w1 = x - x0;
-    return t;
-}
-
-// Phase 1: thread (g, q) accumulates the plane product for channel vectors v = q, q+TPG, ... of every level and
-// writes feat[g][l*C + 4v .. 4v+3] into a0.  coord[g] = (px, py, pz, t) already normalised (t raw).
+// Phase 1: thread (g, q) samples the channel vectors v = q, q+TPG, ... of every level and writes feat[g][l*C + 4v .. 4v+3]
+// into a0.  coord[g] = (px, py, pz, t) already normalised (t raw).
 template <int TG>
 G4D_D void sample_features(const DeformDesc& d, const float* __restrict__ coord, float* __restrict__ a0, int lda0) {
     constexpr int TPG = kDeformThreads / TG;
@@ -122,34 +107,8 @@ G4D_D void sample_features(const DeformDesc& d, const float* __restrict__ coord,
         Tap1D tx[3];
 #pragma unroll
         for (int a = 0; a < 3; ++a) tx[a] = make_tap(pcs[a], d.res[l][a]);
-        for (int v = q; v < C4; v += TPG) {
-            float4 prod = make_float4(1.f, 1.f, 1.f, 1.f);
-#pragma unroll
-            for (int k = 0; k < 6; ++k) {
-                const int c0 = plane_axis0(k), c1 = plane_axis1(k);
-                float4 s;
-                if (c1 == 3) {   // collapsed time row: 1-D lerp along c0
-                    const float4* row = reinterpret_cast<const float4*>(d.trow[l][c0]);
-                    const float4 r0 = __ldg(row + tx[c0].i0 * C4 + v), r1 = __ldg(row + tx[c0].i1 * C4 + v);
-                    const float w0 = tx[c0].w0, w1 = tx[c0].w1;
-                    s.x = fmaf(r1.x, w1, r0.x * w0); s.y = fmaf(r1.y, w1, r0.y * w0);
-                    s.z = fmaf(r1.z, w1, r0.z * w0); s.w = fmaf(r1.w, w1, r0.w * w0);
-                } else {
-                    const int W = d.res[l][c0];
-                    const float4* pl = reinterpret_cast<const float4*>(d.planes[l][k]);
-                    const Tap1D &X = tx[c0], &Y = tx[c1];
-                    const float4 nw = __ldg(pl + (Y.i0 * W + X.i0) * C4 + v), ne = __ldg(pl + (Y.i0 * W + X.i1) * C4 + v);
-                    const float4 sw = __ldg(pl + (Y.i1 * W + X.i0) * C4 + v), se = __ldg(pl + (Y.i1 * W + X.i1) * C4 + v);
-                    const float wnw = X.w0 * Y.w0, wne = X.w1 * Y.w0, wsw = X.w0 * Y.w1, wse = X.w1 * Y.w1;
-                    s.x = fmaf(se.x, wse, fmaf(sw.x, wsw, fmaf(ne.x, wne, nw.x * wnw)));
-                    s.y = fmaf(se.y, wse, fmaf(sw.y, wsw, fmaf(ne.y, wne, nw.y * wnw)));
-                    s.z = fmaf(se.z, wse, fmaf(sw.z, wsw, fmaf(ne.z, wne, nw.z * wnw)));
-                    s.w = fmaf(se.w, wse, fmaf(sw.w, wsw, fmaf(ne.w, wne, nw.w * wnw)));
-                }
-                prod.x *= s.x; prod.y *= s.y; prod.z *= s.z; prod.w *= s.w;
-            }
-            *reinterpret_cast<float4*>(a0 + g * lda0 + l * d.C + 4 * v) = prod;
-        }
+        for (int v = q; v < C4; v += TPG)
+            *reinterpret_cast<float4*>(a0 + g * lda0 + l * d.C + 4 * v) = sample_vector(d.planes[l], d.trow[l], d.res[l], tx, v, C4);
     }
 }
 

@@ -2,7 +2,7 @@
 // network (HexPlane scatter + MLP dgrad/wgrad).
 // Reference autograd path replaced: loss.backward() at /root/reference/train.py:219 through
 // _RasterizeGaussians.backward, F.normalize/exp/sigmoid, nn.Linear, F.grid_sample.
-#include "deform_bwd_common.cuh"
+#include "g4d_internal.h"
 #include "g4d_math.cuh"
 
 namespace g4d {
@@ -107,6 +107,25 @@ cudaError_t launch_preprocess_backward(const CameraDev* cam, int64_t n, const Ra
 //   T  distributes the collapsed time-row gradients onto the two time rows of each time plane.
 // ======================================================================================================
 
+struct DeformBwdBuffers {
+    float* feat;                      // [N][F]
+    float* a1;                        // [N][WD]
+    float* da1[G4D_NUM_HEADS];        // [N][WD] per active head
+    float* trow_grad[G4D_MAX_LEVELS][3];
+};
+
+struct DeformBwdDesc {
+    DeformDesc d;
+    const float* w0;                  // torch layout [WD][F]
+    const float* w1[G4D_NUM_HEADS];   // torch layout [WD][WD]
+    float* g_w0; float* g_b0;
+    float* g_w1[G4D_NUM_HEADS]; float* g_b1[G4D_NUM_HEADS];
+    float* g_w2[G4D_NUM_HEADS]; float* g_b2[G4D_NUM_HEADS];
+    float* g_planes[G4D_MAX_LEVELS][6];
+    const float* go[G4D_NUM_HEADS];   // dL/d(out) per head: xyz[N,3], scaling[N,3], rotation[N,4], opacity[N,1], shs[N,48] (NULL = 0)
+    float* gi[G4D_NUM_HEADS];         // dL/d(in), same shapes (NULL = not wanted)
+};
+
 // acc[r][c] += sum_k A[ty*RM + r][k] * Bt[tx + 16*c][k]       (both operands K-contiguous in shared memory)
 template <int RM, int CN>
 G4D_D void tile_gemm_nt(const float* __restrict__ A, int lda, const float* __restrict__ Bt, int ldb, int K, int ty, int tx,
@@ -145,9 +164,7 @@ deform_bwd_prepass_kernel(DeformDesc d, DeformSmem L, float time, int64_t n, con
     for (int i = tid * 4; i < n0; i += kDeformThreads * 4)
         *reinterpret_cast<float4*>(smem + L.w0t + i) = __ldg(reinterpret_cast<const float4*>(d.w0t + i));
     for (int i = tid; i < WD; i += kDeformThreads) smem[L.b0 + i] = __ldg(d.b0 + i);
-    float amax[3], ascale[3];
-#pragma unroll
-    for (int a = 0; a < 3; ++a) { amax[a] = __ldg(d.aabb + a); ascale[a] = 2.0f / (__ldg(d.aabb + 3 + a) - amax[a]); }
+    const AabbNorm nrm(d.aabb);
     float* coord = smem + L.coord;
     __syncthreads();
     for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
@@ -155,9 +172,9 @@ deform_bwd_prepass_kernel(DeformDesc d, DeformSmem L, float time, int64_t n, con
         if (tid < TG) {
             float4 c = make_float4(0.f, 0.f, 0.f, time);
             if (tid < rem) {
-                c.x = (xyz[(base + tid) * 3 + 0] - amax[0]) * ascale[0] - 1.0f;
-                c.y = (xyz[(base + tid) * 3 + 1] - amax[1]) * ascale[1] - 1.0f;
-                c.z = (xyz[(base + tid) * 3 + 2] - amax[2]) * ascale[2] - 1.0f;
+                c.x = nrm(0, xyz[(base + tid) * 3 + 0]);
+                c.y = nrm(1, xyz[(base + tid) * 3 + 1]);
+                c.z = nrm(2, xyz[(base + tid) * 3 + 2]);
             }
             *reinterpret_cast<float4*>(coord + 4 * tid) = c;
         }
@@ -414,9 +431,7 @@ deform_bwd_final_kernel(DeformBwdDesc bd, FinalSmem L, float time, int64_t n, co
     for (int m = 0; m < MAXF; ++m) gW0[m] = 0.f;
     float gB0 = 0.f;
     const int w0_j = tid % WD, w0_g = tid / WD;
-    float amax[3], ascale[3];
-#pragma unroll
-    for (int a = 0; a < 3; ++a) { amax[a] = __ldg(d.aabb + a); ascale[a] = 2.0f / (__ldg(d.aabb + 3 + a) - amax[a]); }
+    const AabbNorm nrm(d.aabb);
     const int64_t ntiles = (n + TG - 1) / TG;
     constexpr int TPG = kDeformThreads / TG;
     __syncthreads();
@@ -447,9 +462,9 @@ deform_bwd_final_kernel(DeformBwdDesc bd, FinalSmem L, float time, int64_t n, co
         if (tid < TG) {
             float4 c = make_float4(0.f, 0.f, 0.f, time);
             if (tid < rem) {
-                c.x = (xyz[(base + tid) * 3 + 0] - amax[0]) * ascale[0] - 1.0f;
-                c.y = (xyz[(base + tid) * 3 + 1] - amax[1]) * ascale[1] - 1.0f;
-                c.z = (xyz[(base + tid) * 3 + 2] - amax[2]) * ascale[2] - 1.0f;
+                c.x = nrm(0, xyz[(base + tid) * 3 + 0]);
+                c.y = nrm(1, xyz[(base + tid) * 3 + 1]);
+                c.z = nrm(2, xyz[(base + tid) * 3 + 2]);
             }
             *reinterpret_cast<float4*>(coord + 4 * tid) = c;
         }
@@ -488,71 +503,12 @@ deform_bwd_final_kernel(DeformBwdDesc bd, FinalSmem L, float time, int64_t n, co
             float gpix[3] = {0.f, 0.f, 0.f};   // dL/d(normalised coordinate) per axis
             if (g < rem) {
                 for (int l = 0; l < d.levels; ++l) {
-                    TapG tx[3];
+                    Tap1D tx[3];
 #pragma unroll
-                    for (int a = 0; a < 3; ++a) tx[a] = make_tap_g(pcs[a], d.res[l][a]);
+                    for (int a = 0; a < 3; ++a) tx[a] = make_tap(pcs[a], d.res[l][a]);
                     for (int v = q; v < C4; v += TPG) {
-                        float4 s[6], dsx[6], dsy[6];   // sample, d(sample)/d(x_pix of c0), d/d(y_pix of c1)
-#pragma unroll
-                        for (int k = 0; k < 6; ++k) {
-                            const int c0 = plane_axis0(k), c1 = plane_axis1(k);
-                            if (c1 == 3) {
-                                const float4* row = reinterpret_cast<const float4*>(d.trow[l][c0]);
-                                const float4 r0 = __ldg(row + tx[c0].i0 * C4 + v), r1 = __ldg(row + tx[c0].i1 * C4 + v);
-                                const float w0 = tx[c0].w0, w1 = tx[c0].w1;
-                                s[k] = make_float4(fmaf(r1.x, w1, r0.x * w0), fmaf(r1.y, w1, r0.y * w0), fmaf(r1.z, w1, r0.z * w0),
-                                                   fmaf(r1.w, w1, r0.w * w0));
-                                dsx[k] = make_float4(r1.x - r0.x, r1.y - r0.y, r1.z - r0.z, r1.w - r0.w);
-                                dsy[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-                            } else {
-                                const int W = d.res[l][c0];
-                                const float4* pl = reinterpret_cast<const float4*>(d.planes[l][k]);
-                                const TapG &X = tx[c0], &Y = tx[c1];
-                                const float4 nw = __ldg(pl + (Y.i0 * W + X.i0) * C4 + v), ne = __ldg(pl + (Y.i0 * W + X.i1) * C4 + v);
-                                const float4 sw = __ldg(pl + (Y.i1 * W + X.i0) * C4 + v), se = __ldg(pl + (Y.i1 * W + X.i1) * C4 + v);
-                                const float wnw = X.w0 * Y.w0, wne = X.w1 * Y.w0, wsw = X.w0 * Y.w1, wse = X.w1 * Y.w1;
-                                s[k] = make_float4(fmaf(se.x, wse, fmaf(sw.x, wsw, fmaf(ne.x, wne, nw.x * wnw))),
-                                                   fmaf(se.y, wse, fmaf(sw.y, wsw, fmaf(ne.y, wne, nw.y * wnw))),
-                                                   fmaf(se.z, wse, fmaf(sw.z, wsw, fmaf(ne.z, wne, nw.z * wnw))),
-                                                   fmaf(se.w, wse, fmaf(sw.w, wsw, fmaf(ne.w, wne, nw.w * wnw))));
-                                dsx[k] = make_float4((ne.x - nw.x) * Y.w0 + (se.x - sw.x) * Y.w1, (ne.y - nw.y) * Y.w0 + (se.y - sw.y) * Y.w1,
-                                                     (ne.z - nw.z) * Y.w0 + (se.z - sw.z) * Y.w1, (ne.w - nw.w) * Y.w0 + (se.w - sw.w) * Y.w1);
-                                dsy[k] = make_float4((sw.x - nw.x) * X.w0 + (se.x - ne.x) * X.w1, (sw.y - nw.y) * X.w0 + (se.y - ne.y) * X.w1,
-                                                     (sw.z - nw.z) * X.w0 + (se.z - ne.z) * X.w1, (sw.w - nw.w) * X.w0 + (se.w - ne.w) * X.w1);
-                            }
-                        }
                         const float4 df = *reinterpret_cast<const float4*>(sDF + g * L.ldf + l * d.C + 4 * v);
-                        // prefix / suffix products so that a zero sample does not poison the others
-                        float4 pre[6], suf[6];
-                        pre[0] = make_float4(1.f, 1.f, 1.f, 1.f);
-#pragma unroll
-                        for (int k = 1; k < 6; ++k) pre[k] = make_float4(pre[k - 1].x * s[k - 1].x, pre[k - 1].y * s[k - 1].y, pre[k - 1].z * s[k - 1].z, pre[k - 1].w * s[k - 1].w);
-                        suf[5] = make_float4(1.f, 1.f, 1.f, 1.f);
-#pragma unroll
-                        for (int k = 4; k >= 0; --k) suf[k] = make_float4(suf[k + 1].x * s[k + 1].x, suf[k + 1].y * s[k + 1].y, suf[k + 1].z * s[k + 1].z, suf[k + 1].w * s[k + 1].w);
-#pragma unroll
-                        for (int k = 0; k < 6; ++k) {
-                            const int c0 = plane_axis0(k), c1 = plane_axis1(k);
-                            const float4 gs = make_float4(df.x * pre[k].x * suf[k].x, df.y * pre[k].y * suf[k].y,
-                                                          df.z * pre[k].z * suf[k].z, df.w * pre[k].w * suf[k].w);
-                            gpix[c0] += (gs.x * dsx[k].x + gs.y * dsx[k].y + gs.z * dsx[k].z + gs.w * dsx[k].w) * tx[c0].gmul;
-                            if (c1 == 3) {
-                                float* row = buf.trow_grad[l][c0];
-                                const float w0 = tx[c0].w0, w1 = tx[c0].w1;
-                                red_add_v4(row + (tx[c0].i0 * C4 + v) * 4, make_float4(gs.x * w0, gs.y * w0, gs.z * w0, gs.w * w0));
-                                red_add_v4(row + (tx[c0].i1 * C4 + v) * 4, make_float4(gs.x * w1, gs.y * w1, gs.z * w1, gs.w * w1));
-                            } else {
-                                gpix[c1] += (gs.x * dsy[k].x + gs.y * dsy[k].y + gs.z * dsy[k].z + gs.w * dsy[k].w) * tx[c1].gmul;
-                                const int W = d.res[l][c0];
-                                float* pl = bd.g_planes[l][k];
-                                const TapG &X = tx[c0], &Y = tx[c1];
-                                const float wnw = X.w0 * Y.w0, wne = X.w1 * Y.w0, wsw = X.w0 * Y.w1, wse = X.w1 * Y.w1;
-                                red_add_v4(pl + ((Y.i0 * W + X.i0) * C4 + v) * 4, make_float4(gs.x * wnw, gs.y * wnw, gs.z * wnw, gs.w * wnw));
-                                red_add_v4(pl + ((Y.i0 * W + X.i1) * C4 + v) * 4, make_float4(gs.x * wne, gs.y * wne, gs.z * wne, gs.w * wne));
-                                red_add_v4(pl + ((Y.i1 * W + X.i0) * C4 + v) * 4, make_float4(gs.x * wsw, gs.y * wsw, gs.z * wsw, gs.w * wsw));
-                                red_add_v4(pl + ((Y.i1 * W + X.i1) * C4 + v) * 4, make_float4(gs.x * wse, gs.y * wse, gs.z * wse, gs.w * wse));
-                            }
-                        }
+                        scatter_vector(d.planes[l], d.trow[l], d.res[l], bd.g_planes[l], buf.trow_grad[l], tx, v, C4, df, gpix);
                     }
                 }
             }
@@ -564,7 +520,7 @@ deform_bwd_final_kernel(DeformBwdDesc bd, FinalSmem L, float time, int64_t n, co
                 const int64_t gi = base + g;
 #pragma unroll
                 for (int a = 0; a < 3; ++a)
-                    bd.gi[0][gi * 3 + a] = (bd.go[0] ? bd.go[0][gi * 3 + a] : 0.f) + gpix[a] * ascale[a];
+                    bd.gi[0][gi * 3 + a] = (bd.go[0] ? bd.go[0][gi * 3 + a] : 0.f) + gpix[a] * nrm.scale[a];
             }
         }
         // residual path of the other inputs: d(out)/d(in) = identity

@@ -140,42 +140,6 @@ cudaError_t launch_tc_pack_weights(const G4DDeformParams& prm, int arith, float*
     return cudaGetLastError();
 }
 
-// One channel vector (4 channels) of one level: product over the 6 planes of the bilinear samples.
-__device__ __forceinline__ float4 sample_vector(const DeformDesc* __restrict__ dp, int l, int v, int C4, float px, float py, float pz) {
-    const DeformDesc& d = *dp;   // lives in shared memory (a by-reference kernel parameter would be spilled to the stack)
-    const float pcs[3] = {px, py, pz};
-    Tap1D tx[3];
-#pragma unroll
-    for (int a = 0; a < 3; ++a) tx[a] = make_tap(pcs[a], d.res[l][a]);
-    float4 prod = make_float4(1.f, 1.f, 1.f, 1.f);
-#pragma unroll
-    for (int k = 0; k < 6; ++k) {
-        const int c0 = plane_axis0(k), c1 = plane_axis1(k);
-        float4 s;
-        if (c1 == 3) {
-            const float4* rowp = reinterpret_cast<const float4*>(d.trow[l][c0]);
-            const float4 r0 = __ldg(rowp + tx[c0].i0 * C4 + v), r1 = __ldg(rowp + tx[c0].i1 * C4 + v);
-            const float w0 = tx[c0].w0, w1 = tx[c0].w1;
-            s.x = fmaf(r1.x, w1, r0.x * w0); s.y = fmaf(r1.y, w1, r0.y * w0);
-            s.z = fmaf(r1.z, w1, r0.z * w0); s.w = fmaf(r1.w, w1, r0.w * w0);
-        } else {
-            const int W = d.res[l][c0];
-            const float4* pl = reinterpret_cast<const float4*>(d.planes[l][k]);
-            const Tap1D &X = tx[c0], &Y = tx[c1];
-            const float4 nw = __ldg(pl + (Y.i0 * W + X.i0) * C4 + v), ne = __ldg(pl + (Y.i0 * W + X.i1) * C4 + v);
-            const float4 sw = __ldg(pl + (Y.i1 * W + X.i0) * C4 + v), se = __ldg(pl + (Y.i1 * W + X.i1) * C4 + v);
-            const float wnw = X.w0 * Y.w0, wne = X.w1 * Y.w0, wsw = X.w0 * Y.w1, wse = X.w1 * Y.w1;
-            s.x = fmaf(se.x, wse, fmaf(sw.x, wsw, fmaf(ne.x, wne, nw.x * wnw)));
-            s.y = fmaf(se.y, wse, fmaf(sw.y, wsw, fmaf(ne.y, wne, nw.y * wnw)));
-            s.z = fmaf(se.z, wse, fmaf(sw.z, wsw, fmaf(ne.z, wne, nw.z * wnw)));
-            s.w = fmaf(se.w, wse, fmaf(sw.w, wsw, fmaf(ne.w, wne, nw.w * wnw)));
-        }
-        prod.x *= s.x; prod.y *= s.y; prod.z *= s.z; prod.w *= s.w;
-    }
-    return prod;
-}
-
-
 // ---- fragments ----------------------------------------------------------------------------------------------------------
 using wg::Frags;
 
@@ -531,6 +495,7 @@ deform_tc_kernel(DeformDesc d, TcWeights tw, TcSmem Ls, const CameraDev* __restr
 }
 
 // ---- HexPlane gather at full occupancy: C/4 threads per Gaussian, one channel vector each -> feat [N][F] fp32 -----------
+// (the forward chain launches it dependent on collapse_time_rows, the tensor-core backward as an ordinary launch)
 template <int C4>
 __global__ void __launch_bounds__(256) deform_features_kernel(DeformDesc d, int64_t n, const float* __restrict__ xyz, float* __restrict__ feat) {
     pdl_wait();         // the collapsed time rows come from the previous kernel of the stream
@@ -539,22 +504,24 @@ __global__ void __launch_bounds__(256) deform_features_kernel(DeformDesc d, int6
     const int64_t g = t / C4;
     const int v = (int)(t % C4);
     if (g >= n) return;
+    const AabbNorm nrm(d.aabb);
     float pcs[3];
 #pragma unroll
-    for (int a = 0; a < 3; ++a) {
-        const float amax = __ldg(d.aabb + a), ascale = 2.0f / (__ldg(d.aabb + 3 + a) - amax);
-        pcs[a] = (xyz[3 * g + a] - amax) * ascale - 1.0f;
+    for (int a = 0; a < 3; ++a) pcs[a] = nrm(a, xyz[3 * g + a]);
+    for (int l = 0; l < d.levels; ++l) {
+        Tap1D tx[3];
+#pragma unroll
+        for (int a = 0; a < 3; ++a) tx[a] = make_tap(pcs[a], d.res[l][a]);
+        *reinterpret_cast<float4*>(feat + g * d.F + l * d.C + 4 * v) = sample_vector(d.planes[l], d.trow[l], d.res[l], tx, v, C4);
     }
-    for (int l = 0; l < d.levels; ++l)
-        *reinterpret_cast<float4*>(feat + g * d.F + l * d.C + 4 * v) = sample_vector(&d, l, v, C4, pcs[0], pcs[1], pcs[2]);
 }
 
-cudaError_t launch_deform_features(const DeformDesc& d, int64_t n, const float* xyz, float* feat, cudaStream_t st) {
+cudaError_t launch_deform_features(const DeformDesc& d, int64_t n, const float* xyz, float* feat, bool pdl, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
     const int C4 = d.C / 4;
     const unsigned grid = (unsigned)((n * C4 + 255) / 256);
-    if (C4 == 4) return launch_k(deform_features_kernel<4>, dim3(grid), dim3(256), 0, st, true, d, n, xyz, feat);
-    if (C4 == 8) return launch_k(deform_features_kernel<8>, dim3(grid), dim3(256), 0, st, true, d, n, xyz, feat);
+    if (C4 == 4) return launch_k(deform_features_kernel<4>, dim3(grid), dim3(256), 0, st, pdl, d, n, xyz, feat);
+    if (C4 == 8) return launch_k(deform_features_kernel<8>, dim3(grid), dim3(256), 0, st, pdl, d, n, xyz, feat);
     return cudaErrorInvalidValue;
 }
 
@@ -584,7 +551,7 @@ cudaError_t launch_deform_tc(const DeformDesc& d, const TcWeights& tw, int mode,
     if (n == 0) return cudaSuccess;
     if (!tw.feat) return cudaErrorInvalidValue;
     {
-        cudaError_t e = launch_deform_features(d, n, io.xyz, tw.feat, st);
+        cudaError_t e = launch_deform_features(d, n, io.xyz, tw.feat, true, st);
         if (e != cudaSuccess) return e;
     }
     const TcSmem Ls = tc_smem_layout(tw.arith, d.F, (d.head_mask & G4D_HEAD_SHS) != 0);

@@ -9,8 +9,9 @@
 //               signs come from the bits the forward saved (G4D_RELU_BITS_WORDS), so this is the gradient of the forward
 //               that ran.  Everything the weight gradients need is written ONCE to global memory as ready-to-use MMA operand
 //               images (8x8 bf16 core-matrix layout) so that kernel B is pure TMA + MMA.
-//               HexPlane gather (bwd_features_kernel, skipped when the forward's staging buffer was kept) and scatter
-//               (bwd_scatter_kernel: plane REDs, d(xyz), residual paths) run around it at full occupancy.
+//               HexPlane gather (the forward's deform_features_kernel, skipped when the forward's staging buffer was kept)
+//               and scatter (bwd_scatter_kernel: plane REDs, d(xyz), residual paths; hexplane.cuh) run around it at full
+//               occupancy.
 //  B  "wgrad":  dW1_h = DZ_h^T A1, dW2_h^T = A2_h^T DOUT_h, db1_h = DZ_h^T 1, db2_h = 1^T DOUT_h, dW0 = DH^T FEAT, db0 = DH^T 1
 //               as split-K GEMMs over the Gaussian index (operands MN-major straight from the images), accumulators in
 //               registers across the CTA's tiles (warpgroup w: output rows [64 w, 64 w + 64)), one atomic flush per CTA;
@@ -18,7 +19,7 @@
 //
 // Replaces the autograd backward of scene/deformation.py:67-148 + scene/hexplane.py:73-106 (loss.backward(), train.py:219).
 // Compiled with the default FMA contraction (no index-producing math here).
-#include "deform_bwd_common.cuh"
+#include "g4d_internal.h"
 #include "tc_wgmma.cuh"
 
 namespace g4d {
@@ -182,7 +183,7 @@ struct BwdADesc {
     TcBwdWeights w;
     BwdImages img;
     const float* go[G4D_NUM_HEADS];
-    const float* feat;           // [N][F] fp32 (bwd_features_kernel)
+    const float* feat;           // [N][F] fp32 (deform_features_kernel)
     float* dfeat;                // [N][F] fp32 -> bwd_scatter_kernel
     const uint32_t* relu_bits;   // [6][N][4] + tag (g4d.h G4D_RELU_BITS_WORDS) or NULL
 };
@@ -441,54 +442,7 @@ deform_tc_bwd_dgrad_kernel(BwdADesc bd, BwdSmemA Ls, int64_t n) {
     }
 }
 
-// ---- HexPlane gather / scatter at full occupancy (C/4 threads per Gaussian, one channel vector each) ---------------
-G4D_D float4 hexplane_vector(const DeformDesc& d, int l, int v, int C4, const float pcs[3]) {
-    Tap1D tx[3];
-#pragma unroll
-    for (int a = 0; a < 3; ++a) tx[a] = make_tap(pcs[a], d.res[l][a]);
-    float4 prod = make_float4(1.f, 1.f, 1.f, 1.f);
-#pragma unroll
-    for (int k = 0; k < 6; ++k) {
-        const int c0 = plane_axis0(k), c1 = plane_axis1(k);
-        float4 sv;
-        if (c1 == 3) {
-            const float4* rowp = reinterpret_cast<const float4*>(d.trow[l][c0]);
-            const float4 r0 = __ldg(rowp + tx[c0].i0 * C4 + v), r1 = __ldg(rowp + tx[c0].i1 * C4 + v);
-            const float w0 = tx[c0].w0, w1 = tx[c0].w1;
-            sv = make_float4(fmaf(r1.x, w1, r0.x * w0), fmaf(r1.y, w1, r0.y * w0), fmaf(r1.z, w1, r0.z * w0), fmaf(r1.w, w1, r0.w * w0));
-        } else {
-            const int W = d.res[l][c0];
-            const float4* pl = reinterpret_cast<const float4*>(d.planes[l][k]);
-            const Tap1D &X = tx[c0], &Y = tx[c1];
-            const float4 nw = __ldg(pl + (Y.i0 * W + X.i0) * C4 + v), ne = __ldg(pl + (Y.i0 * W + X.i1) * C4 + v);
-            const float4 sw = __ldg(pl + (Y.i1 * W + X.i0) * C4 + v), se = __ldg(pl + (Y.i1 * W + X.i1) * C4 + v);
-            const float wnw = X.w0 * Y.w0, wne = X.w1 * Y.w0, wsw = X.w0 * Y.w1, wse = X.w1 * Y.w1;
-            sv = make_float4(fmaf(se.x, wse, fmaf(sw.x, wsw, fmaf(ne.x, wne, nw.x * wnw))),
-                             fmaf(se.y, wse, fmaf(sw.y, wsw, fmaf(ne.y, wne, nw.y * wnw))),
-                             fmaf(se.z, wse, fmaf(sw.z, wsw, fmaf(ne.z, wne, nw.z * wnw))),
-                             fmaf(se.w, wse, fmaf(sw.w, wsw, fmaf(ne.w, wne, nw.w * wnw))));
-        }
-        prod.x *= sv.x; prod.y *= sv.y; prod.z *= sv.z; prod.w *= sv.w;
-    }
-    return prod;
-}
-
-template <int C4>
-__global__ void __launch_bounds__(256) bwd_features_kernel(DeformDesc d, int64_t n, const float* __restrict__ xyz, float* __restrict__ feat) {
-    const int64_t t = (int64_t)blockIdx.x * 256 + threadIdx.x;
-    const int64_t g = t / C4;
-    const int v = (int)(t % C4);
-    if (g >= n) return;
-    float pcs[3];
-#pragma unroll
-    for (int a = 0; a < 3; ++a) {
-        const float amax = __ldg(d.aabb + a), ascale = 2.0f / (__ldg(d.aabb + 3 + a) - amax);
-        pcs[a] = (xyz[3 * g + a] - amax) * ascale - 1.0f;
-    }
-    for (int l = 0; l < d.levels; ++l)
-        *reinterpret_cast<float4*>(feat + g * d.F + l * d.C + 4 * v) = hexplane_vector(d, l, v, C4, pcs);
-}
-
+// ---- HexPlane scatter at full occupancy (C/4 threads per Gaussian, one channel vector each) -----------------------
 struct BwdScatterDesc {
     DeformDesc d;
     const float* dfeat;                     // [N][F]
@@ -513,18 +467,17 @@ __global__ void __launch_bounds__(256, 2) bwd_scatter_kernel(BwdScatterDesc sd, 
         for (int64_t i = lo + threadIdx.x; i < hi; i += 256) sd.gi[hh][i] = sd.go[hh] ? sd.go[hh][i] : 0.f;
     }
     float gpix[3] = {0.f, 0.f, 0.f};
-    float ascale[3] = {0.f, 0.f, 0.f};
+    const AabbNorm nrm(d.aabb);
     if (g < n) {
         float pcs[3];
 #pragma unroll
-        for (int a = 0; a < 3; ++a) {
-            const float amax = __ldg(d.aabb + a);
-            ascale[a] = 2.0f / (__ldg(d.aabb + 3 + a) - amax);
-            pcs[a] = (xyz[3 * g + a] - amax) * ascale[a] - 1.0f;
-        }
+        for (int a = 0; a < 3; ++a) pcs[a] = nrm(a, xyz[3 * g + a]);
         for (int l = 0; l < d.levels; ++l) {
+            Tap1D tx[3];
+#pragma unroll
+            for (int a = 0; a < 3; ++a) tx[a] = make_tap(pcs[a], d.res[l][a]);
             const float4 df = __ldg(reinterpret_cast<const float4*>(sd.dfeat + g * d.F + l * d.C + 4 * v));
-            scatter_vector(d, sd.g_planes, sd.trow_grad, l, v, C4, pcs, df, gpix);
+            scatter_vector(d.planes[l], d.trow[l], d.res[l], sd.g_planes[l], sd.trow_grad[l], tx, v, C4, df, gpix);
         }
     }
     // the C4 threads of a Gaussian are adjacent lanes
@@ -533,7 +486,7 @@ __global__ void __launch_bounds__(256, 2) bwd_scatter_kernel(BwdScatterDesc sd, 
         for (int o = 1; o < C4; o <<= 1) gpix[a] += __shfl_xor_sync(0xffffffffu, gpix[a], o);
     if (g < n && v == 0 && sd.gi[0]) {
 #pragma unroll
-        for (int a = 0; a < 3; ++a) sd.gi[0][g * 3 + a] = (sd.go[0] ? sd.go[0][g * 3 + a] : 0.f) + gpix[a] * ascale[a];
+        for (int a = 0; a < 3; ++a) sd.gi[0][g * 3 + a] = (sd.go[0] ? sd.go[0][g * 3 + a] : 0.f) + gpix[a] * nrm.scale[a];
     }
 }
 
@@ -749,16 +702,8 @@ cudaError_t launch_deform_backward_tc(const DeformDesc& d, const G4DDeformParams
     for (int h = 0; h < G4D_NUM_HEADS; ++h) { sc.go[h] = go[h]; sc.gi[h] = gi[h]; }
     cudaError_t e = cudaMemsetAsync(rows, 0, row_floats * 4, st);
     if (e != cudaSuccess) return e;
-    const int C4 = d.C / 4;
-    // gather at full occupancy (skipped when the forward's feature staging buffer was kept for this backward)
-    if (!saved_feat) {
-        const int64_t threads = n * C4;
-        const unsigned grid = (unsigned)((threads + 255) / 256);
-        if (C4 == 4) bwd_features_kernel<4><<<grid, 256, 0, st>>>(d, n, xyz, feat);
-        else if (C4 == 8) bwd_features_kernel<8><<<grid, 256, 0, st>>>(d, n, xyz, feat);
-        else return cudaErrorInvalidValue;
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    }
+    // the forward's gather (skipped when the forward's feature staging buffer was kept for this backward)
+    if (!saved_feat && (e = launch_deform_features(d, n, xyz, feat, false, st)) != cudaSuccess) return e;
     if (d.C == 16 && d.levels == 2) e = launch_a<16, 2>(a, n, sm_count, st);
     else if (d.C == 16 && d.levels == 3) e = launch_a<16, 3>(a, n, sm_count, st);
     else if (d.C == 32 && d.levels == 2) e = launch_a<32, 2>(a, n, sm_count, st);
@@ -766,7 +711,7 @@ cudaError_t launch_deform_backward_tc(const DeformDesc& d, const G4DDeformParams
     if (e != cudaSuccess) return e;
     // scatter d(feat) into the planes, d(xyz), residual copies
     {
-        const int gpb = 256 / C4;
+        const int C4 = d.C / 4, gpb = 256 / C4;
         const unsigned grid = (unsigned)((n + gpb - 1) / gpb);
         if (C4 == 4) bwd_scatter_kernel<4><<<grid, 256, 0, st>>>(sc, n, xyz);
         else bwd_scatter_kernel<8><<<grid, 256, 0, st>>>(sc, n, xyz);

@@ -186,12 +186,7 @@ deform_kernel(DeformDesc d, DeformSmem L, const CameraDev* __restrict__ camp, fl
     }
     uint32_t phase = 0;
     const float t = use_cam_time ? cam.time : time_arg;
-    float amax[3], ascale[3];
-#pragma unroll
-    for (int a = 0; a < 3; ++a) {
-        amax[a] = __ldg(d.aabb + a);
-        ascale[a] = 2.0f / (__ldg(d.aabb + 3 + a) - amax[a]);
-    }
+    const AabbNorm nrm(d.aabb);
     float* in_xyz = smem + L.in;
     float* in_sc = in_xyz + TG * 3;
     float* in_rot = in_sc + TG * 3;
@@ -214,9 +209,9 @@ deform_kernel(DeformDesc d, DeformSmem L, const CameraDev* __restrict__ camp, fl
         __syncthreads();
         if (tid < TG) {
             float4 c;
-            c.x = (in_xyz[3 * tid + 0] - amax[0]) * ascale[0] - 1.0f;
-            c.y = (in_xyz[3 * tid + 1] - amax[1]) * ascale[1] - 1.0f;
-            c.z = (in_xyz[3 * tid + 2] - amax[2]) * ascale[2] - 1.0f;
+            c.x = nrm(0, in_xyz[3 * tid + 0]);
+            c.y = nrm(1, in_xyz[3 * tid + 1]);
+            c.z = nrm(2, in_xyz[3 * tid + 2]);
             c.w = t;
             *reinterpret_cast<float4*>(coord + 4 * tid) = c;
         }

@@ -100,6 +100,8 @@ struct TcWeights {
 size_t tc_packed_floats(const G4DDeformParams& prm);
 cudaError_t launch_tc_pack_weights(const G4DDeformParams& prm, int arith, float* blob, TcWeights* out, cudaStream_t st);
 bool tc_deform_supported(const DeformDesc& d, int arith);
+// HexPlane gather xyz -> feat [N][F] fp32; pdl: launched dependent on the previous kernel of the forward chain (DESIGN.md §4.6)
+cudaError_t launch_deform_features(const DeformDesc& d, int64_t n, const float* xyz, float* feat, bool pdl, cudaStream_t st);
 
 // tensor-core backward (g4d_deform_tc_bwd.cu): BF16 (hi | lo) weight images in the 8x8-core layout of tc_wgmma.cuh
 struct TcBwdWeights {

@@ -1,14 +1,12 @@
 // g4d_raster.cu -- the per-tile front-to-back alpha compositing forward / back-to-front backward.
 // SURVEY.md Appendix A.3-A.4 (binning, A.2, lives in g4d_bin.cu).
 // Reference stage replaced: the CUDA rasterizer behind /root/reference/gaussian_renderer/__init__.py:120-128.
-#include <cstdlib>
-
 #include "g4d_internal.h"
 #include "raster_cull.cuh"
 
 namespace g4d {
 
-// Two-lane float arithmetic of the packed blend kernels.  Hopper has no packed FP32 instructions, so each is two scalar
+// Two-lane float arithmetic of the blend kernels.  Hopper has no packed FP32 instructions, so each is two scalar
 // round-to-nearest operations (never contracted, whatever -fmad says): the per-lane results are exactly those of the scalar
 // expression tree.
 G4D_D float2 f2_add(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
@@ -16,118 +14,15 @@ G4D_D float2 f2_mul(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x)
 G4D_D float2 f2_fma(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
 
 // ------------------------------------------------------------------------------------------------------
-// A.3 blend forward: one 16x16 CTA per tile, instances staged through shared memory in batches of 256.
-template <int PPT>
-__global__ void __launch_bounds__(kTilePixels / PPT)
+// A.3 blend forward: one 16x16 CTA per tile, instances staged through shared memory in batches of 256.  A warp owns a compact
+// 16 x 4 pixel strip of the tile and culls instances against it; two pixels per thread, evaluated as f32x2 lanes: the two
+// pixels of a thread share their column, so dx, the dx^2 term and the instance record are scalar and computed once per
+// instance, and only what depends on the row is evaluated per lane (f2_add / f2_mul / f2_fma).  The per-pixel decisions are
+// selects, not branches.  power = fma(dy, -(conic.y dx), -0.5 (conic.z dy^2 + conic.x dx^2)) per lane.
+__global__ void __launch_bounds__(kTilePixels / 2)
 blend_forward_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, const uint32_t* __restrict__ ids,
                      const uint2* __restrict__ ranges, float* __restrict__ final_T, uint32_t* __restrict__ n_contrib,
                      float* __restrict__ out_color, float* __restrict__ out_depth, int warp_cull) {
-    constexpr int NT = kTilePixels / PPT;
-    __shared__ float4 s0[kTilePixels];
-    __shared__ float4 s1[kTilePixels];
-    __shared__ float2 s2[kTilePixels];
-    const int H = cam->H, W = cam->W;
-    const int tile = blockIdx.y * gridDim.x + blockIdx.x;
-    const uint2 range = ranges[tile];
-    const int rounds = (int)((range.y - range.x + kTilePixels - 1) / kTilePixels);
-    int todo = (int)(range.y - range.x);
-    // a warp owns a compact 16 x (2 PPT) pixel strip of the tile: lane l, pixel k -> (l & 15, 2 PPT warp + (l >> 4) + 2 k)
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    float pxf[PPT], pyf[PPT], T[PPT], C0[PPT], C1[PPT], C2[PPT], D[PPT];
-    uint32_t last_contributor[PPT];
-    bool done[PPT], inside[PPT];
-    bool all_done = true;
-#pragma unroll
-    for (int k = 0; k < PPT; ++k) {
-        const int px = blockIdx.x * kTile + (lane & 15), py = blockIdx.y * kTile + 2 * PPT * warp + (lane >> 4) + 2 * k;
-        inside[k] = px < W && py < H;
-        pxf[k] = (float)px; pyf[k] = (float)py;
-        T[k] = 1.f; C0[k] = C1[k] = C2[k] = D[k] = 0.f;
-        last_contributor[k] = 0;
-        done[k] = !inside[k];
-        all_done = all_done && done[k];
-    }
-    // strip rectangle for the per-warp exact cull (same predicate as G4D_OPT_TIGHT_CULL, on 16 x 2 PPT pixels)
-    const float sx0 = (float)(blockIdx.x * kTile), sx1 = sx0 + (float)(kTile - 1);
-    const float sy0 = (float)(blockIdx.y * kTile + 2 * PPT * warp), sy1 = sy0 + (float)(2 * PPT - 1);
-    for (int i = 0; i < rounds; ++i, todo -= kTilePixels) {
-        if (__syncthreads_count(all_done) == NT) break;
-#pragma unroll
-        for (int k = 0; k < PPT; ++k) {
-            const int slot = threadIdx.x + k * NT;
-            const int progress = i * kTilePixels + slot;
-            if (range.x + progress < range.y) {
-                const uint32_t id = ids[range.x + progress];
-                s0[slot] = g.rec0[id];
-                s1[slot] = g.rec1[id];
-                s2[slot] = g.rec2[id];
-            }
-        }
-        __syncthreads();
-        const int cnt = min(kTilePixels, todo);
-        for (int base = 0; base < cnt; base += 32) {
-            if (__all_sync(0xffffffffu, all_done)) break;
-            // lane l tests instance base + l against the warp's strip: instances that cannot reach alpha >= 1/255 on any
-            // of its pixels are skipped by the whole warp (they would be skipped pixel by pixel anyway)
-            const int jt = base + lane;
-            bool hit = jt < cnt;
-            if (hit && warp_cull) hit = rect_contributes(s0[jt], s1[jt], sx0, sx1, sy0, sy1);
-            uint32_t mask = __ballot_sync(0xffffffffu, hit);
-            while (mask) {
-                const int j = base + __ffs(mask) - 1;
-                mask &= mask - 1;
-                const uint32_t contributor = (uint32_t)(i * kTilePixels + j + 1);
-                const float4 a = s0[j];
-                const float4 b = s1[j];
-                const float2 c = s2[j];
-#pragma unroll
-                for (int k = 0; k < PPT; ++k) {
-                    if (!done[k]) {
-                        const float dx = a.x - pxf[k], dy = a.y - pyf[k];
-                        const float power = -0.5f * (a.z * dx * dx + b.x * dy * dy) - a.w * dx * dy;
-                        const float alpha = fminf(kAlphaMax, b.y * __expf(power));
-                        if (power <= 0.f && alpha >= kAlphaMin) {
-                            const float test_T = T[k] * (1.f - alpha);
-                            if (test_T < kTransmittanceStop) done[k] = true;
-                            else {
-                                const float w = alpha * T[k];
-                                C0[k] = fmaf(b.z, w, C0[k]); C1[k] = fmaf(b.w, w, C1[k]); C2[k] = fmaf(c.x, w, C2[k]);
-                                D[k] = fmaf(c.y, w, D[k]);
-                                T[k] = test_T;
-                                last_contributor[k] = contributor;
-                            }
-                        }
-                    }
-                }
-            }
-            all_done = true;
-#pragma unroll
-            for (int k = 0; k < PPT; ++k) all_done = all_done && done[k];
-        }
-    }
-#pragma unroll
-    for (int k = 0; k < PPT; ++k) {
-        if (!inside[k]) continue;
-        const size_t pix = (size_t)pyf[k] * W + (size_t)pxf[k];
-        const size_t hw = (size_t)H * W;
-        final_T[pix] = T[k];
-        n_contrib[pix] = last_contributor[k];
-        out_color[pix] = fmaf(T[k], cam->bg[0], C0[k]);
-        out_color[hw + pix] = fmaf(T[k], cam->bg[1], C1[k]);
-        out_color[2 * hw + pix] = fmaf(T[k], cam->bg[2], C2[k]);
-        out_depth[pix] = D[k];
-    }
-}
-
-// Packed variant (two pixels per thread as f32x2 lanes): the two pixels of a thread share their column, so dx, the dx^2 term and
-// the instance record are scalar and only what depends on the row is evaluated per lane (f2_add / f2_mul / f2_fma); the
-// per-pixel decisions are selects, not branches.  Same expression tree per lane as blend_forward_kernel<2>
-// up to the association of `power` (tests: image vs oracle 1e-4, outliers = threshold flips).  The row-independent terms are
-// computed once per instance for both pixels.
-__global__ void __launch_bounds__(kTilePixels / 2)
-blend_forward_packed_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, const uint32_t* __restrict__ ids,
-                            const uint2* __restrict__ ranges, float* __restrict__ final_T, uint32_t* __restrict__ n_contrib,
-                            float* __restrict__ out_color, float* __restrict__ out_depth, int warp_cull) {
     constexpr int PPT = 2, NT = kTilePixels / PPT;
     __shared__ float4 s0[kTilePixels];
     __shared__ float4 s1[kTilePixels];
@@ -140,6 +35,7 @@ blend_forward_packed_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, co
     const int rounds = (int)((range.y - range.x + kTilePixels - 1) / kTilePixels);
     int todo = (int)(range.y - range.x);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    // warp w owns pixel rows [4w, 4w + 4) of the tile: lane l -> column l & 15, rows 4w + (l >> 4) and 4w + (l >> 4) + 2
     const int px = blockIdx.x * kTile + (lane & 15), py0 = blockIdx.y * kTile + 2 * PPT * warp + (lane >> 4), py1 = py0 + 2;
     const bool in0 = px < W && py0 < H, in1 = px < W && py1 < H;
     const float pxf = (float)px;
@@ -167,6 +63,8 @@ blend_forward_packed_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, co
         const int cnt = min(kTilePixels, todo);
         for (int base = 0; base < cnt; base += 32) {
             if (__all_sync(0xffffffffu, all_done)) break;
+            // lane l tests instance base + l against the warp's strip: instances that cannot reach alpha >= 1/255 on any
+            // of its pixels are skipped by the whole warp (they would be skipped pixel by pixel anyway)
             const int jt = base + lane;
             bool hit = jt < cnt;
             if (hit && warp_cull) hit = rect_contributes(s0[jt], s1[jt], sx0, sx1, sy0, sy1);
@@ -227,20 +125,8 @@ blend_forward_packed_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, co
 cudaError_t launch_blend_forward(const CameraDev* cam, int grid_x, int grid_y, GeomBuffers g, BinBuffers b, ImageBuffers im,
                                  float* out_color, float* out_depth, int warp_cull, cudaStream_t st) {
     if (grid_x * grid_y == 0) return cudaSuccess;
-    static int ppt = []() { const char* e = getenv("G4D_BLEND_FWD_PPT"); const int v = e ? atoi(e) : 2; return (v == 1 || v == 4) ? v : 2; }();
-    static int packed = []() { const char* e = getenv("G4D_BLEND_FWD_PACKED"); return e ? atoi(e) : 1; }();
-    if (packed && ppt == 2) {
-        return launch_k(blend_forward_packed_kernel, dim3(grid_x, grid_y), dim3(kTilePixels / 2), 0, st, true, cam, g, b.ids_sorted,
-                        b.ranges, im.final_T, im.n_contrib, out_color, out_depth, warp_cull);
-    }
-#define G4D_LAUNCH_BF(P)                                                                                                  \
-    blend_forward_kernel<P><<<dim3(grid_x, grid_y), kTilePixels / P, 0, st>>>(cam, g, b.ids_sorted, b.ranges, im.final_T, \
-                                                                               im.n_contrib, out_color, out_depth, warp_cull)
-    if (ppt == 1) G4D_LAUNCH_BF(1);
-    else if (ppt == 4) G4D_LAUNCH_BF(4);
-    else G4D_LAUNCH_BF(2);
-#undef G4D_LAUNCH_BF
-    return cudaGetLastError();
+    return launch_k(blend_forward_kernel, dim3(grid_x, grid_y), dim3(kTilePixels / 2), 0, st, true, cam, g, b.ids_sorted, b.ranges,
+                    im.final_T, im.n_contrib, out_color, out_depth, warp_cull);
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -253,173 +139,15 @@ G4D_D float warp_sum(float v) {
     return v;
 }
 
-// PPT pixels per thread (256 / PPT threads per tile): the per-Gaussian warp reduction -- half of the instruction count with
-// one pixel per thread -- is shared by PPT x 32 pixels, and the staged record is read once per thread instead of per pixel.
-template <int PPT>
-__global__ void __launch_bounds__(kTilePixels / PPT)
+// Two pixels per thread as f32x2 lanes, like the forward: the per-pixel gradient arithmetic is one f2_* operation per pixel
+// PAIR, validity is a select instead of a branch, and power / alpha are formed exactly as the forward forms them (same
+// threshold decisions).
+__global__ void __launch_bounds__(kTilePixels / 2)
 blend_backward_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, const uint32_t* __restrict__ ids,
                       const uint2* __restrict__ ranges, const float* __restrict__ final_T,
                       const uint32_t* __restrict__ n_contrib, const float* __restrict__ dL_dcolor,
                       float* __restrict__ g_mean2D, float* __restrict__ g_conic, float* __restrict__ g_opacity,
                       float* __restrict__ g_rgb, int warp_cull) {
-    constexpr int NT = kTilePixels / PPT;
-    __shared__ float4 s0[kTilePixels];
-    __shared__ float4 s1[kTilePixels];
-    __shared__ float s2[kTilePixels];
-    __shared__ uint32_t sid[kTilePixels];
-    const int H = cam->H, W = cam->W;
-    const int tile = blockIdx.y * gridDim.x + blockIdx.x;
-    const uint2 range = ranges[tile];
-    const int total = (int)(range.y - range.x);
-    const int rounds = (total + kTilePixels - 1) / kTilePixels;
-    const size_t hw = (size_t)H * W;
-    // a warp owns a compact 16 x (2 PPT) pixel strip of the tile: lane l, pixel k -> (l & 15, 2 PPT warp + (l >> 4) + 2 k)
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const float sx0 = (float)(blockIdx.x * kTile), sx1 = sx0 + (float)(kTile - 1);
-    const float sy0 = (float)(blockIdx.y * kTile + 2 * PPT * warp), sy1 = sy0 + (float)(2 * PPT - 1);
-    float pxf[PPT], pyf[PPT], Tfin[PPT], T[PPT], dp0[PPT], dp1[PPT], dp2[PPT], bgdot[PPT];
-    float ac0[PPT], ac1[PPT], ac2[PPT], lc0[PPT], lc1[PPT], lc2[PPT], last_alpha[PPT];
-    int last[PPT];
-    int my_last = 0;
-#pragma unroll
-    for (int k = 0; k < PPT; ++k) {
-        const int px = blockIdx.x * kTile + (lane & 15), py = blockIdx.y * kTile + 2 * PPT * warp + (lane >> 4) + 2 * k;
-        const bool inside = px < W && py < H;
-        const size_t pix = (size_t)py * W + px;
-        pxf[k] = (float)px; pyf[k] = (float)py;
-        Tfin[k] = inside ? final_T[pix] : 0.f;
-        T[k] = Tfin[k];
-        last[k] = inside ? (int)n_contrib[pix] : 0;
-        dp0[k] = dp1[k] = dp2[k] = 0.f;
-        if (inside) { dp0[k] = dL_dcolor[pix]; dp1[k] = dL_dcolor[hw + pix]; dp2[k] = dL_dcolor[2 * hw + pix]; }
-        bgdot[k] = cam->bg[0] * dp0[k] + cam->bg[1] * dp1[k] + cam->bg[2] * dp2[k];
-        ac0[k] = ac1[k] = ac2[k] = lc0[k] = lc1[k] = lc2[k] = last_alpha[k] = 0.f;
-        my_last = max(my_last, last[k]);
-    }
-    const float ddx = 0.5f * (float)W, ddy = 0.5f * (float)H;
-    // block-wide maximum of n_contrib: entries beyond it contribute to no pixel of the tile
-    const int max_last = __reduce_max_sync(0xffffffffu, my_last);
-    __shared__ int s_max[NT / 32];
-    if ((threadIdx.x & 31) == 0) s_max[threadIdx.x >> 5] = max_last;
-    __syncthreads();
-    int tile_last = 0;
-#pragma unroll
-    for (int w = 0; w < NT / 32; ++w) tile_last = max(tile_last, s_max[w]);
-    // warp-level reduction plan: after the butterfly lane l holds value (l >> 2) of {mean2D.xy, conic.xyz, rgb}; lanes
-    // 0,4,..,28 add one value each, lane 1 adds the opacity gradient -- one predicated RED instruction per Gaussian
-    const bool hi16 = lane & 16, hi8 = lane & 8, hi4 = lane & 4;
-    const int vidx = lane >> 2;
-    const bool red_lane = (lane & 3) == 0 || lane == 1;
-    float* red_base = lane == 1 ? g_opacity : vidx < 2 ? g_mean2D + vidx : vidx < 5 ? g_conic + (vidx - 2) : g_rgb + (vidx - 5);
-    const uint32_t red_stride = lane == 1 ? 1u : vidx < 2 ? 2u : 3u;
-
-    for (int i = 0; i < rounds; ++i) {
-        // batch i covers list positions [total - (i+1)*256, total - i*256) traversed from the back
-        const int hi = total - i * kTilePixels;           // exclusive upper position of this batch
-        if (hi - kTilePixels >= tile_last) continue;      // whole batch behind every pixel's last contributor
-        __syncthreads();
-#pragma unroll
-        for (int k = 0; k < PPT; ++k) {
-            const int slot = threadIdx.x + k * NT;
-            const int pos = hi - 1 - slot;                // slot s stages list position hi-1-s
-            if (pos >= 0) {
-                const uint32_t id = ids[range.x + pos];
-                sid[slot] = id;
-                s0[slot] = g.rec0[id];
-                s1[slot] = g.rec1[id];
-                s2[slot] = g.rec2[id].x;
-            }
-        }
-        __syncthreads();
-        const int cnt = min(kTilePixels, hi);
-        for (int base = 0; base < cnt; base += 32) {
-          // lane l tests instance base + l: behind every pixel of this warp's strip, or unable to reach alpha >= 1/255
-          // anywhere on the strip (same predicate as the exact tile cull) -> skipped by the whole warp
-          const int jt = base + lane;
-          bool hit = jt < cnt && (hi - 1 - jt) < max_last;
-          if (hit && warp_cull) hit = rect_contributes(s0[jt], s1[jt], sx0, sx1, sy0, sy1);
-          uint32_t mask = __ballot_sync(0xffffffffu, hit);
-          while (mask) {
-            const int j = base + __ffs(mask) - 1;
-            mask &= mask - 1;
-            const int lpos = hi - 1 - j;                  // position in the tile list (0-based)
-            const float4 a = s0[j];
-            const float4 b = s1[j];
-            float Gk[PPT], alphak[PPT], dxk[PPT], dyk[PPT];
-            bool validk[PPT];
-            bool any_valid = false;
-#pragma unroll
-            for (int k = 0; k < PPT; ++k) {
-                dxk[k] = a.x - pxf[k]; dyk[k] = a.y - pyf[k];
-                const float power = -0.5f * (a.z * dxk[k] * dxk[k] + b.x * dyk[k] * dyk[k]) - a.w * dxk[k] * dyk[k];
-                Gk[k] = __expf(power);
-                alphak[k] = fminf(kAlphaMax, b.y * Gk[k]);
-                validk[k] = lpos < last[k] && power <= 0.f && alphak[k] >= kAlphaMin;
-                any_valid = any_valid || validk[k];
-            }
-            if (!__any_sync(0xffffffffu, any_valid)) continue;
-            float v[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};   // mean2D.xy, conic.xyz, rgb
-            float v_op = 0.f;
-            const float c0 = b.z, c1 = b.w, c2 = s2[j];
-#pragma unroll
-            for (int k = 0; k < PPT; ++k) {
-                if (!validk[k]) continue;
-                const float alpha = alphak[k], G = Gk[k], dx = dxk[k], dy = dyk[k];
-                const float ra = __fdividef(1.f, 1.f - alpha);   // alpha <= 0.99: well inside the fast-division range
-                T[k] = T[k] * ra;
-                const float w = alpha * T[k];
-                ac0[k] = last_alpha[k] * lc0[k] + (1.f - last_alpha[k]) * ac0[k]; lc0[k] = c0;
-                ac1[k] = last_alpha[k] * lc1[k] + (1.f - last_alpha[k]) * ac1[k]; lc1[k] = c1;
-                ac2[k] = last_alpha[k] * lc2[k] + (1.f - last_alpha[k]) * ac2[k]; lc2[k] = c2;
-                float dL_dalpha = (c0 - ac0[k]) * dp0[k] + (c1 - ac1[k]) * dp1[k] + (c2 - ac2[k]) * dp2[k];
-                v[5] += w * dp0[k]; v[6] += w * dp1[k]; v[7] += w * dp2[k];
-                dL_dalpha *= T[k];
-                last_alpha[k] = alpha;
-                dL_dalpha += (-Tfin[k] * ra) * bgdot[k];
-                const float dL_dG = b.y * dL_dalpha;
-                const float gdx = G * dx, gdy = G * dy;
-                v[0] += dL_dG * (-gdx * a.z - gdy * a.w) * ddx;
-                v[1] += dL_dG * (-gdy * b.x - gdx * a.w) * ddy;
-                v[2] += -0.5f * gdx * dx * dL_dG;
-                v[3] += -gdx * dy * dL_dG;
-                v[4] += -0.5f * gdy * dy * dL_dG;
-                v_op += G * dL_dalpha;
-            }
-            // transposing butterfly: 8 values x 32 lanes -> value (lane >> 2) summed over the warp in 9 shuffles
-            float u[4];
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                const float send = hi16 ? v[k] : v[k + 4];
-                u[k] = (hi16 ? v[k + 4] : v[k]) + __shfl_xor_sync(0xffffffffu, send, 16);
-            }
-            float x2[2];
-#pragma unroll
-            for (int k = 0; k < 2; ++k) {
-                const float send = hi8 ? u[k] : u[k + 2];
-                x2[k] = (hi8 ? u[k + 2] : u[k]) + __shfl_xor_sync(0xffffffffu, send, 8);
-            }
-            float x = (hi4 ? x2[1] : x2[0]) + __shfl_xor_sync(0xffffffffu, hi4 ? x2[0] : x2[1], 4);
-            x += __shfl_xor_sync(0xffffffffu, x, 2);
-            x += __shfl_xor_sync(0xffffffffu, x, 1);
-            v_op = warp_sum(v_op);
-            if (red_lane) {
-                const uint32_t id = sid[j];
-                atomicAdd(red_base + red_stride * id, lane == 1 ? v_op : x);
-            }
-          }
-        }
-    }
-}
-
-// Packed variant of the backward (two pixels per thread as f32x2 lanes, see blend_forward_packed_kernel): the per-pixel gradient
-// arithmetic is one f2_* operation per pixel PAIR, validity is a select instead of a branch, and the power / alpha are
-// formed exactly as the packed forward forms them (same threshold decisions).  The warp reduction and the REDs are unchanged.
-__global__ void __launch_bounds__(kTilePixels / 2)
-blend_backward_packed_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, const uint32_t* __restrict__ ids,
-                             const uint2* __restrict__ ranges, const float* __restrict__ final_T,
-                             const uint32_t* __restrict__ n_contrib, const float* __restrict__ dL_dcolor,
-                             float* __restrict__ g_mean2D, float* __restrict__ g_conic, float* __restrict__ g_opacity,
-                             float* __restrict__ g_rgb, int warp_cull) {
     constexpr int PPT = 2, NT = kTilePixels / PPT;
     __shared__ float4 s0[kTilePixels];
     __shared__ float4 s1[kTilePixels];
@@ -434,6 +162,7 @@ blend_backward_packed_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, c
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const float sx0 = (float)(blockIdx.x * kTile), sx1 = sx0 + (float)(kTile - 1);
     const float sy0 = (float)(blockIdx.y * kTile + 2 * PPT * warp), sy1 = sy0 + (float)(2 * PPT - 1);
+    // warp w owns pixel rows [4w, 4w + 4) of the tile: lane l -> column l & 15, rows 4w + (l >> 4) and 4w + (l >> 4) + 2
     const int px = blockIdx.x * kTile + (lane & 15), py0 = blockIdx.y * kTile + 2 * PPT * warp + (lane >> 4), py1 = py0 + 2;
     const bool in0 = px < W && py0 < H, in1 = px < W && py1 < H;
     const size_t pix0 = (size_t)py0 * W + px, pix1 = (size_t)py1 * W + px;
@@ -450,6 +179,7 @@ blend_backward_packed_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, c
     const float2 nTfin = make_float2(-Tfin.x, -Tfin.y);
     float2 ac0 = make_float2(0.f, 0.f), ac1 = ac0, ac2 = ac0, lc0 = ac0, lc1 = ac0, lc2 = ac0, la = ac0;
     const float ddx = 0.5f * (float)W, ddy = 0.5f * (float)H;
+    // block-wide maximum of n_contrib: entries beyond it contribute to no pixel of the tile
     const int max_last = __reduce_max_sync(0xffffffffu, max(last0, last1));
     __shared__ int s_max[NT / 32];
     if ((threadIdx.x & 31) == 0) s_max[threadIdx.x >> 5] = max_last;
@@ -457,6 +187,8 @@ blend_backward_packed_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, c
     int tile_last = 0;
 #pragma unroll
     for (int w = 0; w < NT / 32; ++w) tile_last = max(tile_last, s_max[w]);
+    // warp-level reduction plan: after the butterfly lane l holds value (l >> 2) of {mean2D.xy, conic.xyz, rgb}; lanes
+    // 0,4,..,28 add one value each, lane 1 adds the opacity gradient -- one predicated RED instruction per Gaussian
     const bool hi16 = lane & 16, hi8 = lane & 8, hi4 = lane & 4;
     const int vidx = lane >> 2;
     const bool red_lane = (lane & 3) == 0 || lane == 1;
@@ -465,8 +197,9 @@ blend_backward_packed_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, c
     const float2 one2 = make_float2(1.f, 1.f);
 
     for (int i = 0; i < rounds; ++i) {
+        // batch i covers list positions [total - (i+1)*256, total - i*256) traversed from the back; slot s stages position hi-1-s
         const int hi = total - i * kTilePixels;
-        if (hi - kTilePixels >= tile_last) continue;
+        if (hi - kTilePixels >= tile_last) continue;      // whole batch behind every pixel's last contributor
         __syncthreads();
 #pragma unroll
         for (int k = 0; k < PPT; ++k) {
@@ -483,6 +216,8 @@ blend_backward_packed_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, c
         __syncthreads();
         const int cnt = min(kTilePixels, hi);
         for (int base = 0; base < cnt; base += 32) {
+            // lane l tests instance base + l: behind every pixel of this warp's strip, or unable to reach alpha >= 1/255
+            // anywhere on the strip (same predicate as the exact tile cull) -> skipped by the whole warp
             const int jt = base + lane;
             bool hit = jt < cnt && (hi - 1 - jt) < max_last;
             if (hit && warp_cull) hit = rect_contributes(s0[jt], s1[jt], sx0, sx1, sy0, sy1);
@@ -550,6 +285,7 @@ blend_backward_packed_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, c
                 }
                 const float2 po = f2_mul(G, dLa);
                 float v_op = po.x + po.y;
+                // transposing butterfly: 8 values x 32 lanes -> value (lane >> 2) summed over the warp in 9 shuffles
                 float u[4];
 #pragma unroll
                 for (int k = 0; k < 4; ++k) {
@@ -579,23 +315,8 @@ cudaError_t launch_blend_backward(const CameraDev* cam, int grid_x, int grid_y, 
                                   const float* dL_dcolor, float* g_mean2D, float* g_conic, float* g_opacity, float* g_rgb,
                                   int warp_cull, cudaStream_t st) {
     if (grid_x * grid_y == 0) return cudaSuccess;
-    // pixels per thread: 2 (G4D_BLEND_BWD_PPT overrides for experiments)
-    static int ppt = []() { const char* e = getenv("G4D_BLEND_BWD_PPT"); const int v = e ? atoi(e) : 2; return (v == 1 || v == 4) ? v : 2; }();
-    static int packed = []() { const char* e = getenv("G4D_BLEND_BWD_PACKED"); return e ? atoi(e) : 1; }();
-    if (packed && ppt == 2) {
-        blend_backward_packed_kernel<<<dim3(grid_x, grid_y), kTilePixels / 2, 0, st>>>(cam, g, b.ids_sorted, b.ranges, im.final_T,
-                                                                                       im.n_contrib, dL_dcolor, g_mean2D, g_conic,
-                                                                                       g_opacity, g_rgb, warp_cull);
-        return cudaGetLastError();
-    }
-#define G4D_LAUNCH_BB(P)                                                                                               \
-    blend_backward_kernel<P><<<dim3(grid_x, grid_y), kTilePixels / P, 0, st>>>(cam, g, b.ids_sorted, b.ranges, im.final_T, \
-                                                                                im.n_contrib, dL_dcolor, g_mean2D, g_conic, \
-                                                                                g_opacity, g_rgb, warp_cull)
-    if (ppt == 1) G4D_LAUNCH_BB(1);
-    else if (ppt == 4) G4D_LAUNCH_BB(4);
-    else G4D_LAUNCH_BB(2);
-#undef G4D_LAUNCH_BB
+    blend_backward_kernel<<<dim3(grid_x, grid_y), kTilePixels / 2, 0, st>>>(cam, g, b.ids_sorted, b.ranges, im.final_T, im.n_contrib,
+                                                                             dL_dcolor, g_mean2D, g_conic, g_opacity, g_rgb, warp_cull);
     return cudaGetLastError();
 }
 
