@@ -32,9 +32,15 @@ int fail(int code, const char* what, const char* detail = nullptr) {
         }                                                                                   \
     } while (0)
 
+// device memory that grows by 1.5x on demand and is freed with its owner (on the owner's device)
 struct DevBuf {
     void* p = nullptr;
     size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    DevBuf(DevBuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+    ~DevBuf() { if (p) cudaFree(p); }
     cudaError_t ensure(size_t bytes) {
         if (bytes <= cap) return cudaSuccess;
         size_t want = bytes + bytes / 2 + 256;
@@ -44,9 +50,52 @@ struct DevBuf {
         cap = want;
         return cudaSuccess;
     }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
     template <class T> T* as() const { return reinterpret_cast<T*>(p); }
 };
+
+// grow `buf` to the size of a layout and place it there: layout(Carve&) takes the layout's ranges, and runs once to count
+// the bytes and once on the buffer
+template <class Layout> cudaError_t ensure_layout(DevBuf& buf, Layout layout) {
+    Carve size;
+    layout(size);
+    const cudaError_t e = buf.ensure(size.bytes());
+    if (e != cudaSuccess) return e;
+    Carve place(buf.p);
+    layout(place);
+    return cudaSuccess;
+}
+
+// FP32 transposes of W0 and of the active heads' W1 (the FFMA kernels' operands)
+struct FfmaWeights {
+    float* w0t;
+    float* w1t[G4D_NUM_HEADS];
+};
+
+// weight images derived from the caller's parameters, rebuilt when G4DDeformParams.version or the w0 pointer changes (or,
+// for the tensor-core forward, the arithmetic)
+template <class Images>
+struct WeightCache {
+    DevBuf buf;
+    Images img{};   // where the images sit in buf
+    uint64_t version = 0;
+    const void* key = nullptr;
+    int arith = 0;
+    bool valid = false;
+    // pack(buf.p, &img) (re)builds the images unless they were built from these parameters
+    template <class Pack> cudaError_t refresh(const G4DDeformParams* p, int arith_, size_t bytes, Pack pack) {
+        if (valid && version == p->version && key == (const void*)p->w0 && arith == arith_) return cudaSuccess;
+        valid = false;
+        cudaError_t e = buf.ensure(bytes);
+        if (e == cudaSuccess) e = pack(buf.p, &img);
+        if (e != cudaSuccess) return e;
+        version = p->version; key = (const void*)p->w0; arith = arith_; valid = true;
+        return cudaSuccess;
+    }
+};
+
+// pinned host words of a workspace: the exact-mode read-back of R, and the flag an FP16x2 tensor-core kernel sets (through
+// the host mapping) when a value left the f16 operand range
+struct PinnedWords { uint32_t num_rendered, pad0[7], f16_range, pad1[7]; };
 
 }  // namespace
 
@@ -60,25 +109,15 @@ struct G4DWorkspace {
     int tensor_cores = 2;      // 0: FP32 FFMA kernels, 1: wgmma 3xTF32, 2 (default): wgmma FP16x2
     int warp_cull = 1;
     int keep_deformed = 0;
-    DevBuf tc_packed;
-    TcWeights tcw{};
-    DevBuf tc_bwd_packed, tc_feat;
-    TcBwdWeights tcbw{};
-    uint64_t tc_bwd_version = 0;
-    const void* tc_bwd_key = nullptr;
-    uint64_t tc_version = ~0ull;
-    const void* tc_key = nullptr;
-    DevBuf tc_dbg;
     int tc_debug = 0;
-    // packed (transposed) MLP weights, refreshed when G4DDeformParams.version changes
-    uint64_t packed_version = ~0ull;
-    const void* packed_key = nullptr;
-    DevBuf packed;
-    float* w0t = nullptr;
-    float* w1t[G4D_NUM_HEADS] = {nullptr, nullptr, nullptr, nullptr, nullptr};
+    WeightCache<FfmaWeights> packed;     // FFMA forward and backward
+    WeightCache<TcWeights> tc;           // tensor-core forward (the weight fields and status of TcWeights)
+    WeightCache<TcBwdWeights> tc_bwd;    // tensor-core backward
+    DevBuf tc_feat;     // HexPlane feature staging of a tensor-core forward that keeps no features
+    DevBuf tc_dbg;      // G4D_OPT_TC_DEBUG cycle counters
     DevBuf trow;        // time rows for the context-free deform entry points
-    DevBuf scratch;     // misc per-call scratch (deform backward)
-    uint32_t* h_pinned = nullptr;
+    DevBuf scratch;     // misc per-call scratch (deform backward, kNN)
+    PinnedWords* pinned = nullptr;
 };
 
 struct G4DContext {
@@ -118,8 +157,6 @@ int g_pdl = []() { const char* e = getenv("G4D_PDL"); return e ? atoi(e) != 0 : 
 
 namespace {
 
-size_t align_up(size_t v, size_t a = 256) { return (v + a - 1) / a * a; }
-
 // RAII bracket of one stage with CUDA events on the launching stream (only when G4D_OPT_STAGE_TIMING is on)
 struct StageTimer {
     G4DContext* c; int stage; cudaStream_t st; bool on;
@@ -141,30 +178,24 @@ void reset_stage_flags(G4DContext* c, int first, int last) { for (int i = first;
 
 int ensure_geom(G4DContext* c, int64_t n) {
     const size_t N = (size_t)(n > 0 ? n : 1);
-    size_t off = 0;
-    auto take = [&](size_t bytes) { size_t o = off; off += align_up(bytes); return o; };
-    const size_t o0 = take(N * 16), o1 = take(N * 16), o2 = take(N * 8), o3 = take(N * 4), o4 = take(N * 8), o5 = take(N * 4),
-                 o7 = take(N), o8 = take(N * 4);
-    G4D_CUDA(c->geom.ensure(off));
-    char* base = c->geom.as<char>();
-    c->g.rec0 = (float4*)(base + o0); c->g.rec1 = (float4*)(base + o1); c->g.rec2 = (float2*)(base + o2);
-    c->g.radii = (int32_t*)(base + o3); c->g.rect = (uint2*)(base + o4); c->g.tiles_touched = (uint32_t*)(base + o5);
-    c->g.clamped = (uint8_t*)(base + o7);
-    c->g.perm = (uint32_t*)(base + o8);
-    c->g.depth_range = &c->cam.as<CameraDev>()->depth_min;
+    GeomBuffers& g = c->g;
+    auto layout = [&](Carve& m) {
+        g.rec0 = m.take<float4>(N); g.rec1 = m.take<float4>(N); g.rec2 = m.take<float2>(N); g.radii = m.take<int32_t>(N);
+        g.rect = m.take<uint2>(N); g.tiles_touched = m.take<uint32_t>(N); g.clamped = m.take<uint8_t>(N); g.perm = m.take<uint32_t>(N);
+    };
+    G4D_CUDA(ensure_layout(c->geom, layout));
+    g.depth_range = &c->cam.as<CameraDev>()->depth_min;
     return G4D_OK;
 }
 
 int ensure_image(G4DContext* c, int H, int W) {
     const size_t P = (size_t)H * W;
     const int gx = (W + kTile - 1) / kTile, gy = (H + kTile - 1) / kTile;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { size_t o = off; off += align_up(bytes); return o; };
-    const size_t o0 = take(P * 4), o1 = take(P * 4), o2 = take((size_t)gx * gy * 8);
-    G4D_CUDA(c->img.ensure(off));
-    char* base = c->img.as<char>();
-    c->im.final_T = (float*)(base + o0); c->im.n_contrib = (uint32_t*)(base + o1);
-    c->b.ranges = (uint2*)(base + o2);
+    auto layout = [&](Carve& m) {
+        c->im.final_T = m.take<float>(P); c->im.n_contrib = m.take<uint32_t>(P);
+        c->b.ranges = m.take<uint2>((size_t)gx * gy);
+    };
+    G4D_CUDA(ensure_layout(c->img, layout));
     c->H = H; c->W = W; c->grid_x = gx; c->grid_y = gy;
     return G4D_OK;
 }
@@ -181,15 +212,14 @@ int ensure_bin(G4DContext* c, int64_t r) {
 
 int ensure_fused(G4DContext* c, int64_t n, bool with_sh) {
     const size_t N = (size_t)(n > 0 ? n : 1);
-    size_t off = 0;
-    auto take = [&](size_t bytes) { size_t o = off; off += align_up(bytes); return o; };
-    const size_t o0 = take(N * 12), o1 = take(N * 12), o2 = take(N * 16), o3 = take(N * 4), o5 = take(N * 4),
-                 o4 = take(with_sh ? N * 192 : 16);
-    G4D_CUDA(c->fused.ensure(off));
-    char* base = c->fused.as<char>();
-    c->fo.means3D = (float*)(base + o0); c->fo.scales = (float*)(base + o1); c->fo.rotations = (float*)(base + o2);
-    c->fo.opacities = (float*)(base + o3); c->fo.rot_norm = (float*)(base + o5);
-    c->fo.shs = with_sh ? (float*)(base + o4) : nullptr;
+    FusedOutputs& fo = c->fo;
+    auto layout = [&](Carve& m) {
+        fo.means3D = m.take<float>(3 * N); fo.scales = m.take<float>(3 * N); fo.rotations = m.take<float>(4 * N);
+        fo.opacities = m.take<float>(N); fo.rot_norm = m.take<float>(N);
+        float* shs = m.take<float>(with_sh ? 48 * N : 4);
+        fo.shs = with_sh ? shs : nullptr;
+    };
+    G4D_CUDA(ensure_layout(c->fused, layout));
     return G4D_OK;
 }
 
@@ -205,111 +235,36 @@ int check_params(const G4DDeformParams* p) {
     return G4D_OK;
 }
 
-// (re)build the transposed weight copies when the caller bumped the version
 int refresh_packed(G4DWorkspace* ws, const G4DDeformParams* p, cudaStream_t st) {
-    const int F = p->levels * p->channels, WD = p->net_width;
-    if (ws->packed_version == p->version && ws->packed_key == (const void*)p->w0 && ws->w0t) return G4D_OK;
-    size_t floats = (size_t)F * WD + (size_t)G4D_NUM_HEADS * WD * WD;
-    G4D_CUDA(ws->packed.ensure(floats * 4));
-    float* base = ws->packed.as<float>();
-    ws->w0t = base;
-    for (int h = 0; h < G4D_NUM_HEADS; ++h) ws->w1t[h] = base + (size_t)F * WD + (size_t)h * WD * WD;
-    G4D_CUDA(launch_pack_weights(*p, ws->w0t, ws->w1t, st));
-    ws->packed_version = p->version;
-    ws->packed_key = (const void*)p->w0;
+    const size_t F = (size_t)p->levels * p->channels, WD = (size_t)p->net_width;
+    auto pack = [&](void* blob, FfmaWeights* w) {
+        w->w0t = static_cast<float*>(blob);
+        for (int h = 0; h < G4D_NUM_HEADS; ++h) w->w1t[h] = w->w0t + F * WD + h * WD * WD;
+        return launch_pack_weights(*p, w->w0t, w->w1t, st);
+    };
+    G4D_CUDA(ws->packed.refresh(p, 0, (F * WD + G4D_NUM_HEADS * WD * WD) * 4, pack));
     return G4D_OK;
 }
 
-bool forward_on_tensor_cores(const G4DWorkspace* ws, const DeformDesc& d) {
-    return ws->tensor_cores != 0 && tc_deform_supported(d, ws->tensor_cores);
-}
-
-// tensor-core weight images, same caching rule as refresh_packed
 int refresh_tc(G4DWorkspace* ws, const G4DDeformParams* p, cudaStream_t st) {
     const int arith = ws->tensor_cores == 2 ? 2 : 1;
-    ws->tcw.status = ws->h_pinned + 8;
-    if (arith == 2 && ws->h_pinned[8]) {
-        ws->h_pinned[8] = 0;
-        ws->tc_version = ~0ull;      // re-pack (and re-check) the weights on the next call: they may be the out-of-range values
+    if (arith == 2 && ws->pinned->f16_range) {
+        ws->pinned->f16_range = 0;
+        ws->tc.valid = false;      // re-pack (and re-check) the weights on the next call: they may be the out-of-range values
         return fail(G4D_ERR_OVERFLOW, "an earlier FP16x2 tensor-core launch met a value outside the f16 operand range (activation >= 8188, "
                                       "feature >= 1023 or weight >= 255): its results were saturated; set G4D_OPT_TENSOR_CORES = 1 (3xTF32)");
     }
-    if (ws->tc_version == p->version && ws->tc_key == (const void*)p->w0 && ws->tc_packed.p && ws->tcw.arith == arith) return G4D_OK;
-    G4D_CUDA(ws->tc_packed.ensure(tc_packed_floats(*p) * 4));
-    G4D_CUDA(launch_tc_pack_weights(*p, arith, ws->tc_packed.as<float>(), &ws->tcw, st));
-    ws->tcw.arith = arith;
-    ws->tc_version = p->version;
-    ws->tc_key = (const void*)p->w0;
+    auto pack = [&](void* blob, TcWeights* w) {
+        w->arith = arith;
+        w->status = &ws->pinned->f16_range;
+        return launch_tc_pack_weights(*p, arith, static_cast<float*>(blob), w, st);
+    };
+    G4D_CUDA(ws->tc.refresh(p, arith, tc_packed_floats(*p) * 4, pack));
     return G4D_OK;
 }
 
-int refresh_tc_bwd(G4DWorkspace* ws, const G4DDeformParams* p, cudaStream_t st) {
-    if (ws->tc_bwd_version == p->version && ws->tc_bwd_key == (const void*)p->w0 && ws->tc_bwd_packed.p) return G4D_OK;
-    G4D_CUDA(ws->tc_bwd_packed.ensure(tc_bwd_weight_bytes(*p)));
-    G4D_CUDA(launch_tc_bwd_pack_weights(*p, ws->tc_bwd_packed.as<uint8_t>(), &ws->tcbw, st));
-    ws->tc_bwd_version = p->version;
-    ws->tc_bwd_key = (const void*)p->w0;
-    return G4D_OK;
-}
-
-// backward of the deformation network: tensor-core path when the configuration allows, FFMA path otherwise
-int deform_backward_dispatch(G4DWorkspace* ws, const DeformDesc& d, const G4DDeformParams* prm, const G4DDeformGrads* grads,
-                             float time, int64_t n, const float* xyz, const float* const go[G4D_NUM_HEADS],
-                             float* const gi[G4D_NUM_HEADS], const uint32_t* relu_bits, const float* saved_feat, cudaStream_t st) {
-    int rc;
-    if (ws->tensor_cores && tc_backward_supported(d)) {
-        if ((rc = refresh_tc_bwd(ws, prm, st)) != G4D_OK) return rc;
-        G4D_CUDA(ws->scratch.ensure(tc_deform_backward_scratch_bytes(d, n)));
-        G4D_CUDA(launch_deform_backward_tc(d, *prm, *grads, ws->tcbw, time, n, xyz, go, gi, relu_bits, saved_feat, ws->scratch.as<uint8_t>(),
-                                           ws->sm_count, st));
-        return G4D_OK;
-    }
-    if ((rc = refresh_packed(ws, prm, st)) != G4D_OK) return rc;
-    DeformDesc df = d;                       // the transposes may just have been (re)allocated: take the current pointers
-    df.w0t = ws->w0t;
-    for (int h = 0; h < G4D_NUM_HEADS; ++h) df.w1t[h] = ws->w1t[h];
-    G4D_CUDA(ws->scratch.ensure(deform_backward_scratch_bytes(df, n)));
-    G4D_CUDA(launch_deform_backward(df, *prm, *grads, time, n, xyz, go, gi, ws->scratch.as<float>(), ws->sm_count, st));
-    return G4D_OK;
-}
-
-// ReLU sign bits saved by the tensor-core forward for its backward; the trailing tag word says whether they were written
-constexpr int kReluTagByte = 0x5A;
-int attach_relu_bits(G4DWorkspace* ws, bool use_tc, bool save, uint32_t* relu_bits, int64_t n, cudaStream_t st) {
-    const bool tc = use_tc;
-    use_tc = use_tc && save;
-    ws->tcw.relu_bits = use_tc ? relu_bits : nullptr;
-    ws->tcw.feat = nullptr;
-    if (tc) {   // feature staging buffer of the tensor-core forward
-        G4D_CUDA(ws->tc_feat.ensure((size_t)(n > 0 ? n : 1) * 64 * 4 + 256));
-        ws->tcw.feat = ws->tc_feat.as<float>();
-    }
-    if (relu_bits) G4D_CUDA(cudaMemsetAsync(relu_bits + (size_t)24 * (size_t)n, use_tc ? kReluTagByte : 0, 16, st));
-    return G4D_OK;
-}
-
-int attach_tc_debug(G4DWorkspace* ws, cudaStream_t st) {
-    ws->tcw.dbg = nullptr;
-    if (!ws->tc_debug) return G4D_OK;
-    G4D_CUDA(ws->tc_dbg.ensure((size_t)ws->sm_count * 12 * 8));
-    G4D_CUDA(cudaMemsetAsync(ws->tc_dbg.p, 0, (size_t)ws->sm_count * 12 * 8, st));
-    ws->tcw.dbg = ws->tc_dbg.as<long long>();
-    return G4D_OK;
-}
-
-int setup_trow(DevBuf& buf, float* (*ptrs)[3], const G4DDeformParams* p) {
-    size_t floats = 0;
-    for (int l = 0; l < p->levels; ++l)
-        for (int a = 0; a < 3; ++a) floats += (size_t)p->res[l][a] * p->channels;
-    cudaError_t e = buf.ensure(floats * 4);
-    if (e != cudaSuccess) return fail(G4D_ERR_NOMEM, "time-row buffer");
-    float* q = buf.as<float>();
-    for (int l = 0; l < p->levels; ++l)
-        for (int a = 0; a < 3; ++a) { ptrs[l][a] = q; q += (size_t)p->res[l][a] * p->channels; }
-    return G4D_OK;
-}
-
-DeformDesc make_desc(const G4DWorkspace* ws, const G4DDeformParams* p, float* const (*trow)[3]) {
+// w: the FP32 transposes, on the FFMA paths (the tensor-core kernels do not read them)
+DeformDesc make_desc(const G4DDeformParams* p, float* const (*trow)[3], const FfmaWeights* w) {
     DeformDesc d{};
     d.levels = p->levels; d.C = p->channels; d.F = p->levels * p->channels; d.WD = p->net_width; d.head_mask = p->head_mask;
     for (int l = 0; l < p->levels; ++l) {
@@ -317,9 +272,86 @@ DeformDesc make_desc(const G4DWorkspace* ws, const G4DDeformParams* p, float* co
         for (int k = 0; k < 6; ++k) d.planes[l][k] = p->planes[l][k];
         for (int a = 0; a < 3; ++a) d.trow[l][a] = trow[l][a];
     }
-    d.aabb = p->aabb; d.w0t = ws->w0t; d.b0 = p->b0;
-    for (int h = 0; h < G4D_NUM_HEADS; ++h) { d.w1t[h] = ws->w1t[h]; d.b1[h] = p->b1[h]; d.w2[h] = p->w2[h]; d.b2[h] = p->b2[h]; }
+    d.aabb = p->aabb; d.w0t = w ? w->w0t : nullptr; d.b0 = p->b0;
+    for (int h = 0; h < G4D_NUM_HEADS; ++h) {
+        d.w1t[h] = w ? w->w1t[h] : nullptr; d.b1[h] = p->b1[h]; d.w2[h] = p->w2[h]; d.b2[h] = p->b2[h];
+    }
     return d;
+}
+
+// the deformation network of one forward call
+struct DeformSetup {
+    DeformDesc d;
+    bool tc;         // the forward runs on the tensor cores
+    TcWeights tw;    // tc: weight images, range flag and debug counters; the caller adds its feat / relu_bits buffers
+};
+
+// the time planes interpolated at `time`, into `rows` (pointers in trow)
+int collapse_time_rows(DevBuf& rows, float* (*trow)[3], const G4DDeformParams* p, const CameraDev* cam, float time, cudaStream_t st) {
+    const TimeRows tr(p->levels, p->res, p->channels);
+    if (rows.ensure(tr.total() * 4) != cudaSuccess) return fail(G4D_ERR_NOMEM, "time-row buffer");
+    tr.place(rows.as<float>(), trow);
+    G4D_CUDA(launch_collapse_time_rows(*p, cam, time, trow, st));
+    return G4D_OK;
+}
+
+// Collapse the time rows, pick the forward's path from the params and bring the weight images that path reads up to date.
+// The desc is built after that refresh, which may move the transposes it embeds.
+int setup_deform(G4DWorkspace* ws, const G4DDeformParams* p, DevBuf& rows, float* (*trow)[3], const CameraDev* cam, float time,
+                 cudaStream_t st, DeformSetup* out) {
+    int rc;
+    if ((rc = collapse_time_rows(rows, trow, p, cam, time, st)) != G4D_OK) return rc;
+    out->tc = ws->tensor_cores != 0 && tc_deform_supported(*p, ws->tensor_cores);
+    if (!out->tc) {
+        if ((rc = refresh_packed(ws, p, st)) != G4D_OK) return rc;
+        out->d = make_desc(p, trow, &ws->packed.img);
+        return G4D_OK;
+    }
+    if ((rc = refresh_tc(ws, p, st)) != G4D_OK) return rc;
+    out->d = make_desc(p, trow, nullptr);
+    out->tw = ws->tc.img;
+    if (ws->tc_debug) {   // per-CTA phase cycle counters (g4d_debug_tc_cycles)
+        G4D_CUDA(ws->tc_dbg.ensure((size_t)ws->sm_count * 12 * 8));
+        G4D_CUDA(cudaMemsetAsync(ws->tc_dbg.p, 0, (size_t)ws->sm_count * 12 * 8, st));
+        out->tw.dbg = ws->tc_dbg.as<long long>();
+    }
+    return G4D_OK;
+}
+
+// Buffers of this forward call.  feat: where a tensor-core forward stages the HexPlane features [N][F] (NULL: the
+// workspace's); relu_bits: where it saves the ReLU signs for a backward, or NULL.  The tag word behind the bits tells the
+// backward whether this forward wrote them.
+int attach_forward_buffers(G4DWorkspace* ws, DeformSetup& s, float* feat, uint32_t* relu_bits, int64_t n, cudaStream_t st) {
+    if (s.tc && !feat) {
+        G4D_CUDA(ws->tc_feat.ensure((size_t)(n > 0 ? n : 1) * 64 * 4 + 256));
+        feat = ws->tc_feat.as<float>();
+    }
+    s.tw.feat = feat;
+    s.tw.relu_bits = relu_bits;
+    if (relu_bits) G4D_CUDA(cudaMemsetAsync(relu_bits + (size_t)24 * (size_t)n, s.tc ? kReluBitsTagByte : 0, 16, st));
+    return G4D_OK;
+}
+
+// backward of the deformation network with the time rows trow: tensor-core path when the configuration allows, FFMA path
+// otherwise; the desc is built after the weight images of that path are current
+int deform_backward_dispatch(G4DWorkspace* ws, const G4DDeformParams* prm, float* const (*trow)[3], const G4DDeformGrads* grads,
+                             float time, int64_t n, const float* xyz, const float* const go[G4D_NUM_HEADS],
+                             float* const gi[G4D_NUM_HEADS], const uint32_t* relu_bits, const float* saved_feat, cudaStream_t st) {
+    int rc;
+    if (ws->tensor_cores && tc_backward_supported(*prm)) {
+        auto pack = [&](void* blob, TcBwdWeights* w) { return launch_tc_bwd_pack_weights(*prm, static_cast<uint8_t*>(blob), w, st); };
+        G4D_CUDA(ws->tc_bwd.refresh(prm, 0, tc_bwd_weight_bytes(*prm), pack));
+        const DeformDesc d = make_desc(prm, trow, nullptr);
+        G4D_CUDA(ws->scratch.ensure(tc_deform_backward_scratch_bytes(d, n)));
+        G4D_CUDA(launch_deform_backward_tc(d, *prm, *grads, ws->tc_bwd.img, time, n, xyz, go, gi, relu_bits, saved_feat,
+                                           ws->scratch.as<uint8_t>(), ws->sm_count, st));
+        return G4D_OK;
+    }
+    if ((rc = refresh_packed(ws, prm, st)) != G4D_OK) return rc;
+    const DeformDesc d = make_desc(prm, trow, &ws->packed.img);
+    G4D_CUDA(ws->scratch.ensure(deform_backward_scratch_bytes(d, n)));
+    G4D_CUDA(launch_deform_backward(d, *prm, *grads, time, n, xyz, go, gi, ws->scratch.as<float>(), ws->sm_count, st));
+    return G4D_OK;
 }
 
 int check_camera(const G4DCamera* cam) {
@@ -387,9 +419,9 @@ int bin_and_blend(G4DContext* c, const G4DCamera* cam, int64_t n, float* out_col
         }
         c->bin_ctl = lay.ctl;
         if (!nosync) {
-            G4D_CUDA(cudaMemcpyAsync(ws->h_pinned, &lay.ctl->R, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+            G4D_CUDA(cudaMemcpyAsync(&ws->pinned->num_rendered, &lay.ctl->R, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
             G4D_CUDA(cudaStreamSynchronize(st));   // exact mode: the one host sync of the path (as in the reference, A.2)
-            const int64_t R = (int64_t)ws->h_pinned[0];
+            const int64_t R = (int64_t)ws->pinned->num_rendered;
             c->R = R; c->learned = true;
             int64_t want = R;
             if (!ws->sync_mode) want = R + R / 2;                 // head-room for the asynchronous forwards that follow
@@ -477,16 +509,15 @@ G4DWorkspace* g4d_workspace_create(int device) {
     ws->device = device;
     cudaDeviceProp prop{};
     if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) ws->sm_count = prop.multiProcessorCount;
-    if (cudaMallocHost((void**)&ws->h_pinned, 64) != cudaSuccess) { delete ws; fail(G4D_ERR_NOMEM, "cudaMallocHost"); return nullptr; }
-    for (int i = 0; i < 16; ++i) ws->h_pinned[i] = 0;      // [0]: R read-back, [8]: FP16x2 range flag (written by the kernel)
+    if (cudaMallocHost((void**)&ws->pinned, sizeof(PinnedWords)) != cudaSuccess) { delete ws; fail(G4D_ERR_NOMEM, "cudaMallocHost"); return nullptr; }
+    *ws->pinned = PinnedWords{};
     return ws;
 }
 
 void g4d_workspace_destroy(G4DWorkspace* ws) {
     if (!ws) return;
     cudaSetDevice(ws->device);
-    ws->packed.release(); ws->tc_packed.release(); ws->tc_bwd_packed.release(); ws->tc_feat.release(); ws->trow.release(); ws->scratch.release();
-    if (ws->h_pinned) cudaFreeHost(ws->h_pinned);
+    if (ws->pinned) cudaFreeHost(ws->pinned);
     delete ws;
 }
 
@@ -508,8 +539,6 @@ void g4d_context_destroy(G4DContext* c) {
     if (c->ev_created) for (int i = 0; i < 2 * G4D_STAGE_COUNT; ++i) cudaEventDestroy(c->ev[i]);
     for (int i = 0; i < G4DContext::kSlots; ++i) if (c->ev_r[i]) cudaEventDestroy(c->ev_r[i]);
     if (c->h_r) cudaFreeHost(c->h_r);
-    c->cam.release(); c->geom.release(); c->bin.release(); c->binaux.release(); c->img.release(); c->fused.release(); c->gscratch.release(); c->gdeform.release(); c->relu.release(); c->feat.release();
-    c->trow.release();
     delete c;
 }
 
@@ -570,19 +599,12 @@ int g4d_deform_forward(G4DWorkspace* ws, const G4DDeformParams* prm, int64_t n, 
     cudaStream_t st = (cudaStream_t)stream;
     G4D_CUDA(cudaSetDevice(ws->device));
     float* trow[G4D_MAX_LEVELS][3] = {};
-    if ((rc = setup_trow(ws->trow, trow, prm)) != G4D_OK) return rc;
-    G4D_CUDA(launch_collapse_time_rows(*prm, nullptr, time, false, trow, st));
-    const bool use_tc = forward_on_tensor_cores(ws, make_desc(ws, prm, trow));
-    if (!use_tc && (rc = refresh_packed(ws, prm, st)) != G4D_OK) return rc;     // FP32 transposes: only the FFMA kernels read them
-    const DeformDesc d = make_desc(ws, prm, trow);
-    GeomBuffers g{};
-    FusedOutputs fo{};
-    if (use_tc && (rc = refresh_tc(ws, prm, st)) != G4D_OK) return rc;
-    if (use_tc && (rc = attach_tc_debug(ws, st)) != G4D_OK) return rc;
-    if ((rc = attach_relu_bits(ws, use_tc, true, relu_bits, n, st)) != G4D_OK) return rc;
-    G4D_CUDA(launch_deform(d, 0, nullptr, time, false, n, xyz, scaling, rotation, opacity, shs, nullptr, nullptr, out_xyz,
-                           out_scaling, out_rotation, out_opacity, out_shs, g, fo, nullptr, ws->sm_count, st,
-                           use_tc ? &ws->tcw : nullptr));
+    DeformSetup s{};
+    if ((rc = setup_deform(ws, prm, ws->trow, trow, nullptr, time, st, &s)) != G4D_OK) return rc;
+    if ((rc = attach_forward_buffers(ws, s, nullptr, relu_bits, n, st)) != G4D_OK) return rc;
+    const DeformIO io{xyz, scaling, rotation, opacity, shs, nullptr, nullptr, out_xyz, out_scaling, out_rotation, out_opacity,
+                      out_shs, GeomBuffers{}, FusedOutputs{}, nullptr};
+    G4D_CUDA(launch_deform(s.d, 0, nullptr, time, n, io, ws->sm_count, st, s.tc ? &s.tw : nullptr));
     return G4D_OK;
 }
 
@@ -742,12 +764,10 @@ int g4d_deform_backward(G4DWorkspace* ws, const G4DDeformParams* prm, G4DDeformG
     cudaStream_t st = (cudaStream_t)stream;
     G4D_CUDA(cudaSetDevice(ws->device));
     float* trow[G4D_MAX_LEVELS][3] = {};
-    if ((rc = setup_trow(ws->trow, trow, prm)) != G4D_OK) return rc;
-    G4D_CUDA(launch_collapse_time_rows(*prm, nullptr, time, false, trow, st));
-    const DeformDesc d = make_desc(ws, prm, trow);      // (the dispatcher refreshes the weight images its path needs)
+    if ((rc = collapse_time_rows(ws->trow, trow, prm, nullptr, time, st)) != G4D_OK) return rc;
     const float* go[G4D_NUM_HEADS] = {g_out_xyz, g_out_scaling, g_out_rotation, g_out_opacity, g_out_shs};
     float* gi[G4D_NUM_HEADS] = {g_in_xyz, g_in_scaling, g_in_rotation, g_in_opacity, g_in_shs};
-    return deform_backward_dispatch(ws, d, prm, grads, time, n, xyz, go, gi, relu_bits, nullptr, st);
+    return deform_backward_dispatch(ws, prm, trow, grads, time, n, xyz, go, gi, relu_bits, nullptr, st);
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -777,37 +797,30 @@ int g4d_render_forward(G4DContext* c, const G4DCamera* cam, const G4DDeformParam
     // a no-grad render needs none of the saved tensors: skip their stores (48 B + 192 B of deformed SH per Gaussian)
     c->fo_valid = !(cam->debug & G4D_CAM_NO_GRAD) || ws->keep_deformed;
     const FusedOutputs fo_arg = c->fo_valid ? c->fo : FusedOutputs{};
+    DeformSetup s{};
     {
         StageTimer tm(c, G4D_STAGE_PREP, st);
         G4D_CUDA(launch_pack_camera(*cam, dcam, st));
+        if (prm && (rc = setup_deform(ws, prm, c->trow, c->trow_ptr, dcam, cam->time, st, &s)) != G4D_OK) return rc;
+    }
+    {
+        StageTimer tm(c, G4D_STAGE_GEOM, st);
         if (prm) {
-            if ((rc = setup_trow(c->trow, c->trow_ptr, prm)) != G4D_OK) return rc;
-            G4D_CUDA(launch_collapse_time_rows(*prm, dcam, cam->time, false, c->trow_ptr, st));
+            c->relu_saved = s.tc && !(cam->debug & G4D_CAM_NO_GRAD);
+            if (c->relu_saved) {   // a backward will follow: it re-uses the ReLU signs and the staged HexPlane features
+                G4D_CUDA(c->relu.ensure(G4D_RELU_BITS_WORDS(n) * 4));
+                G4D_CUDA(c->feat.ensure((size_t)(n > 0 ? n : 1) * (size_t)s.d.F * 4 + 256));
+            }
+            if ((rc = attach_forward_buffers(ws, s, c->relu_saved ? c->feat.as<float>() : nullptr,
+                                             c->relu_saved ? c->relu.as<uint32_t>() : nullptr, n, st)) != G4D_OK) return rc;
+            const DeformIO io{g->xyz, g->scaling, g->rotation, g->opacity, shs, dc, g->features_rest,
+                              nullptr, nullptr, nullptr, nullptr, nullptr, c->g, fo_arg, out_radii};
+            G4D_CUDA(launch_deform(s.d, 1, dcam, cam->time, n, io, ws->sm_count, st, s.tc ? &s.tw : nullptr));
+        } else {
+            G4D_CUDA(launch_activate_preprocess(dcam, n, g->xyz, g->scaling, g->rotation, g->opacity, shs, dc, g->features_rest,
+                                                c->g, fo_arg, out_radii, st));
         }
     }
-    StageTimer* geom_tm = new StageTimer(c, G4D_STAGE_GEOM, st);
-    struct Del { StageTimer*& p; ~Del() { delete p; p = nullptr; } } del{geom_tm};
-    if (prm) {
-        const bool use_tc = forward_on_tensor_cores(ws, make_desc(ws, prm, c->trow_ptr));
-        if (!use_tc && (rc = refresh_packed(ws, prm, st)) != G4D_OK) return rc;
-        const DeformDesc d = make_desc(ws, prm, c->trow_ptr);
-        if (use_tc && (rc = refresh_tc(ws, prm, st)) != G4D_OK) return rc;
-        if (use_tc && (rc = attach_tc_debug(ws, st)) != G4D_OK) return rc;
-        c->relu_saved = use_tc && !(cam->debug & G4D_CAM_NO_GRAD);
-        if (c->relu_saved) G4D_CUDA(c->relu.ensure(G4D_RELU_BITS_WORDS(n) * 4));
-        if ((rc = attach_relu_bits(ws, use_tc, c->relu_saved, c->relu_saved ? c->relu.as<uint32_t>() : nullptr, n, st)) != G4D_OK) return rc;
-        if (c->relu_saved) {   // a backward will follow: keep the staged HexPlane features with the context (it re-uses them)
-            G4D_CUDA(c->feat.ensure((size_t)(n > 0 ? n : 1) * (size_t)d.F * 4 + 256));
-            ws->tcw.feat = c->feat.as<float>();
-        }
-        G4D_CUDA(launch_deform(d, 1, dcam, cam->time, false, n, g->xyz, g->scaling, g->rotation, g->opacity, shs, dc,
-                               g->features_rest, nullptr, nullptr, nullptr, nullptr, nullptr, c->g, fo_arg, out_radii,
-                               ws->sm_count, st, use_tc ? &ws->tcw : nullptr));
-    } else {
-        G4D_CUDA(launch_activate_preprocess(dcam, n, g->xyz, g->scaling, g->rotation, g->opacity, shs, dc, g->features_rest,
-                                            c->g, fo_arg, out_radii, st));
-    }
-    delete geom_tm; geom_tm = nullptr;
     if ((rc = debug_sync(cam, st, "deform+preprocess")) != G4D_OK) return rc;
     rc = bin_and_blend(c, cam, n, out_color, out_depth, st);
     if (rc != G4D_OK) return rc;
@@ -851,13 +864,13 @@ int g4d_render_backward(G4DContext* c, const G4DCamera* cam, const G4DDeformPara
         return debug_sync(cam, st, "activation_backward");
     }
     // gradients w.r.t. the deformed tensors land in scratch, then flow through the deformation network
-    size_t off = 0;
-    auto take = [&](size_t bytes) { size_t o = off; off += align_up(bytes); return o; };
-    const size_t o0 = take(N * 12), o1 = take(N * 12), o2 = take(N * 16), o3 = take(N * 4), o4 = take(c->fused_sh ? N * 192 : 16);
-    G4D_CUDA(c->gdeform.ensure(off));
-    char* base = c->gdeform.as<char>();
-    float* gd_xyz = (float*)(base + o0); float* gd_sc = (float*)(base + o1); float* gd_rot = (float*)(base + o2);
-    float* gd_op = (float*)(base + o3); float* gd_sh = c->fused_sh ? (float*)(base + o4) : nullptr;
+    float *gd_xyz, *gd_sc, *gd_rot, *gd_op, *gd_sh;
+    auto layout = [&](Carve& m) {
+        gd_xyz = m.take<float>(3 * N); gd_sc = m.take<float>(3 * N); gd_rot = m.take<float>(4 * N); gd_op = m.take<float>(N);
+        gd_sh = m.take<float>(c->fused_sh ? 48 * N : 4);
+    };
+    G4D_CUDA(ensure_layout(c->gdeform, layout));
+    if (!c->fused_sh) gd_sh = nullptr;
     // SH gradient: identity residual path -> written straight into the caller's sinks; the fused copy (when the SHS
     // head is active) additionally feeds the network's backward
     if (c->fused_sh && !split) { sh_fused_sink = gg->features_dc; }
@@ -866,12 +879,12 @@ int g4d_render_backward(G4DContext* c, const G4DCamera* cam, const G4DDeformPara
     if (rc != G4D_OK) return rc;
     if (c->fused_sh && !split) G4D_CUDA(cudaMemcpyAsync(gg->features_dc, gd_sh, N * 192, cudaMemcpyDeviceToDevice, st));
     G4D_CUDA(launch_activation_backward(n, c->fo, gd_sc, gd_rot, gd_op, st));
-    const DeformDesc d = make_desc(ws, prm, c->trow_ptr);
     const float* go[G4D_NUM_HEADS] = {gd_xyz, gd_sc, gd_rot, gd_op, gd_sh};
     float* gi[G4D_NUM_HEADS] = {gg->xyz, gg->scaling, gg->rotation, gg->opacity, nullptr};
     {
         StageTimer tm(c, G4D_STAGE_DEFORM_BWD, st);
-        if ((rc = deform_backward_dispatch(ws, d, prm, pgrads, cam->time, n, g->xyz, go, gi, c->relu_saved ? c->relu.as<uint32_t>() : nullptr,
+        if ((rc = deform_backward_dispatch(ws, prm, c->trow_ptr, pgrads, cam->time, n, g->xyz, go, gi,
+                                           c->relu_saved ? c->relu.as<uint32_t>() : nullptr,
                                            c->relu_saved ? c->feat.as<float>() : nullptr, st)) != G4D_OK) return rc;
     }
     return debug_sync(cam, st, "deform_backward");

@@ -568,28 +568,37 @@ cudaError_t launch_distribute_time_grad(const DeformDesc& d, float* const (*trow
                                         cudaStream_t st) {
     TimeGradDesc t{};
     t.levels = d.levels; t.C = d.C;
+    const TimeRows tr(d.levels, d.res, d.C);
     const int tk[3] = {2, 4, 5};
-    int total = 0;
     for (int l = 0; l < d.levels; ++l) {
         for (int a = 0; a < 4; ++a) t.res[l][a] = d.res[l][a];
-        for (int a = 0; a < 3; ++a) {
-            t.row_grad[l][a] = trow_grad[l][a]; t.plane_grad[l][a] = g_planes[l][tk[a]];
-            t.start[l * 3 + a] = total; total += d.res[l][a] * d.C;
-        }
+        for (int a = 0; a < 3; ++a) { t.row_grad[l][a] = trow_grad[l][a]; t.plane_grad[l][a] = g_planes[l][tk[a]]; }
     }
-    t.start[d.levels * 3] = total;
+    for (int m = 0; m <= 3 * d.levels; ++m) t.start[m] = tr.start[m];
+    const int total = (int)tr.total();
     distribute_time_grad_kernel<<<(total + 255) / 256, 256, 0, st>>>(t, time);
     return cudaGetLastError();
 }
 
-size_t deform_backward_scratch_bytes(const DeformDesc& d, int64_t n) {
-    int active = 0;
-    for (int h = 0; h < G4D_NUM_HEADS; ++h) active += (d.head_mask >> h) & 1;
-    size_t rows = 0;
-    for (int l = 0; l < d.levels; ++l)
-        for (int a = 0; a < 3; ++a) rows += (size_t)d.res[l][a] * d.C;
+// the scratch of the FFMA backward: FEAT [N][F], A1 [N][WD], DA1 of every active head [N][WD], the time-row gradients;
+// returns the number of active heads
+static int carve_backward_scratch(Carve& m, const DeformDesc& d, const TimeRows& tr, int64_t n, DeformBwdBuffers& buf) {
     const size_t N = (size_t)(n > 0 ? n : 1);
-    return (N * d.F + N * d.WD * (1 + active) + rows) * sizeof(float) + 4096;
+    buf.feat = m.take<float>(N * d.F);
+    buf.a1 = m.take<float>(N * d.WD);
+    int active = 0;
+    for (int h = 0; h < G4D_NUM_HEADS; ++h)
+        if (d.head_mask & (1 << h)) { buf.da1[h] = m.take<float>(N * d.WD); ++active; }
+    float* rows = m.take<float>(tr.total());
+    if (rows) tr.place(rows, buf.trow_grad);
+    return active;
+}
+
+size_t deform_backward_scratch_bytes(const DeformDesc& d, int64_t n) {
+    Carve m;
+    DeformBwdBuffers buf{};
+    carve_backward_scratch(m, d, TimeRows(d.levels, d.res, d.C), n, buf);
+    return m.bytes();
 }
 
 template <int TG, int WD>
@@ -597,24 +606,10 @@ static cudaError_t launch_deform_backward_t(const DeformBwdDesc& bd, float time,
                                             int sm_count, cudaStream_t st) {
     const DeformDesc& d = bd.d;
     DeformBwdBuffers buf{};
-    const size_t N = (size_t)n;
-    float* p = scratch;
-    auto take = [&](size_t floats) { float* o = p; p += (floats + 63) & ~(size_t)63; return o; };
-    buf.feat = take(N * d.F);
-    buf.a1 = take(N * WD);
-    int active = 0;
-    for (int h = 0; h < G4D_NUM_HEADS; ++h)
-        if (d.head_mask & (1 << h)) { buf.da1[h] = take(N * WD); ++active; }
-    size_t row_floats = 0;
-    for (int l = 0; l < d.levels; ++l)
-        for (int a = 0; a < 3; ++a) row_floats += (size_t)d.res[l][a] * d.C;
-    float* rows = take(row_floats);
-    {
-        float* q = rows;
-        for (int l = 0; l < d.levels; ++l)
-            for (int a = 0; a < 3; ++a) { buf.trow_grad[l][a] = q; q += (size_t)d.res[l][a] * d.C; }
-    }
-    cudaError_t e = cudaMemsetAsync(rows, 0, row_floats * sizeof(float), st);
+    const TimeRows tr(d.levels, d.res, d.C);
+    Carve m(scratch);
+    const int active = carve_backward_scratch(m, d, tr, n, buf);
+    cudaError_t e = cudaMemsetAsync(buf.trow_grad[0][0], 0, tr.total() * sizeof(float), st);
     if (e != cudaSuccess) return e;
     const int64_t ntiles = (n + TG - 1) / TG;
     // P

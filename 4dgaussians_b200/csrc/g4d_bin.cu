@@ -607,32 +607,38 @@ __global__ void __launch_bounds__(256, 4) bin_fix_kernel(BinPlaceArgs a, int chu
 namespace {
 constexpr size_t kCountSmemBudget = 160 * 1024;
 constexpr size_t kPlaceSmemBudget = 96 * 1024;
-size_t align256(size_t v) { return (v + 255) / 256 * 256; }
+
+// the aux area of the binning: sort ping-pong buffers, per-chunk histograms and counts, tile totals and starts, BinCtl
+void carve_bin_aux(Carve& m, int64_t n, int num_tiles, int sm_count, BinSortArgs& a, uint32_t*& tile_start) {
+    const size_t N = (size_t)(n > 0 ? n : 1), G = (size_t)sm_count;
+    a.kA = m.take<uint32_t>(N); a.vA = m.take<uint32_t>(N); a.kB = m.take<uint32_t>(N); a.vB = m.take<uint32_t>(N);
+    a.H = m.take<uint32_t>(G * kRadix); a.S = m.take<uint32_t>(2 * G); a.chunk_start = m.take<uint32_t>(G + 1);
+    a.M = m.take<uint32_t>(G * (size_t)num_tiles);
+    a.tile_total = m.take<uint32_t>((size_t)num_tiles);
+    tile_start = m.take<uint32_t>((size_t)num_tiles);
+    a.ctl = m.take<BinCtl>(1);
+}
 }  // namespace
 
 size_t bin_aux_bytes(int64_t n, int num_tiles, int sm_count) {
-    const size_t N = (size_t)(n > 0 ? n : 1), G = (size_t)sm_count;
-    return 4 * align256(N * 4) + align256(G * kRadix * 4) + align256(2 * G * 4) + align256((G + 1) * 4) +
-           align256(G * (size_t)num_tiles * 4) + 2 * align256((size_t)num_tiles * 4) + align256(sizeof(BinCtl));
+    Carve m;
+    BinSortArgs a{};
+    uint32_t* tile_start;
+    carve_bin_aux(m, n, num_tiles, sm_count, a, tile_start);
+    return m.bytes();
 }
 
 cudaError_t launch_bin_sort(int64_t n, int grid_x, int grid_y, const GeomBuffers& g, void* aux, int tight, int sm_count,
                             BinLayout* out, cudaStream_t st) {
     const int num_tiles = grid_x * grid_y;
-    const size_t N = (size_t)(n > 0 ? n : 1), G = (size_t)sm_count;
-    char* p = (char*)aux;
-    auto take = [&](size_t bytes) { char* r = p; p += align256(bytes); return r; };
     BinSortArgs a{};
     a.n = n; a.rec2 = g.rec2; a.tiles_touched = g.tiles_touched; a.rect = g.rect; a.rec0 = g.rec0; a.rec1 = g.rec1;
     a.depth_range = g.depth_range;
     a.grid_bar = reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(g.depth_range) - offsetof(CameraDev, depth_min) + offsetof(CameraDev, grid_bar));
-    a.kA = (uint32_t*)take(N * 4); a.vA = (uint32_t*)take(N * 4); a.kB = (uint32_t*)take(N * 4); a.vB = (uint32_t*)take(N * 4);
     a.perm = g.perm;
-    a.H = (uint32_t*)take(G * kRadix * 4); a.S = (uint32_t*)take(2 * G * 4); a.chunk_start = (uint32_t*)take((G + 1) * 4);
-    a.M = (uint32_t*)take(G * (size_t)num_tiles * 4);
-    a.tile_total = (uint32_t*)take((size_t)num_tiles * 4);
-    uint32_t* tile_start = (uint32_t*)take((size_t)num_tiles * 4);
-    a.ctl = (BinCtl*)take(sizeof(BinCtl));
+    Carve m(aux);
+    uint32_t* tile_start;
+    carve_bin_aux(m, n, num_tiles, sm_count, a, tile_start);
     a.grid_x = grid_x; a.grid_y = grid_y; a.num_tiles = num_tiles; a.tight = tight;
     int rows = (int)(kCountSmemBudget / ((size_t)grid_x * 4));
     if (rows < 1) return cudaErrorInvalidValue;

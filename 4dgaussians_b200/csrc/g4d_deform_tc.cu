@@ -525,10 +525,11 @@ cudaError_t launch_deform_features(const DeformDesc& d, int64_t n, const float* 
     return cudaErrorInvalidValue;
 }
 
-bool tc_deform_supported(const DeformDesc& d, int arith) {
-    if (d.WD != 128) return false;
-    if (!((d.C == 16 && (d.levels == 2 || d.levels == 3)) || (d.C == 32 && d.levels == 2))) return false;
-    return tc_smem_layout(arith, d.F, (d.head_mask & G4D_HEAD_SHS) != 0).total + kTcStaticSmem <= kMaxSmemPerBlock;
+bool tc_deform_supported(const G4DDeformParams& prm, int arith) {
+    const int C = prm.channels, L = prm.levels;
+    if (prm.net_width != 128) return false;
+    if (!((C == 16 && (L == 2 || L == 3)) || (C == 32 && L == 2))) return false;
+    return tc_smem_layout(arith, C * L, (prm.head_mask & G4D_HEAD_SHS) != 0).total + kTcStaticSmem <= kMaxSmemPerBlock;
 }
 
 template <int ARITH, int MODE, int C, int L>
@@ -546,8 +547,8 @@ static cudaError_t launch_deform_tc_t(const DeformDesc& d, const TcWeights& tw, 
     return launch_k(deform_tc_kernel<ARITH, MODE, C, L, false>, dim3(grid), dim3(threads), bytes, st, true, d, tw, Ls, cam, use_cam ? 1 : 0, n, io);
 }
 
-cudaError_t launch_deform_tc(const DeformDesc& d, const TcWeights& tw, int mode, const CameraDev* cam, bool use_cam_time,
-                             int64_t n, const DeformIO& io, int sm_count, cudaStream_t st) {
+cudaError_t launch_deform_tc(const DeformDesc& d, const TcWeights& tw, int mode, const CameraDev* cam, int64_t n,
+                             const DeformIO& io, int sm_count, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
     if (!tw.feat) return cudaErrorInvalidValue;
     {
@@ -558,7 +559,7 @@ cudaError_t launch_deform_tc(const DeformDesc& d, const TcWeights& tw, int mode,
     const size_t bytes = Ls.total;
     const int64_t ntiles = (n + 64 * (tw.arith == 2 ? 2 : 1) - 1) / (64 * (tw.arith == 2 ? 2 : 1));
     const int grid = (int)(ntiles < sm_count ? ntiles : sm_count);
-    const bool use_cam = mode == 1 || use_cam_time;
+    const bool use_cam = mode == 1;
 #define G4D_TC_CASE(AR, CC, LL)                                                                                        \
     if (tw.arith == AR && d.C == CC && d.levels == LL)                                                                 \
         return mode == 0 ? launch_deform_tc_t<AR, 0, CC, LL>(d, tw, Ls, bytes, grid, cam, use_cam, n, io, st)          \

@@ -169,10 +169,11 @@ cudaError_t launch_tc_bwd_pack_weights(const G4DDeformParams& prm, uint8_t* blob
     return cudaGetLastError();
 }
 
-bool tc_backward_supported(const DeformDesc& d) {
-    if (d.WD != 128) return false;
-    if (!((d.C == 16 && (d.levels == 2 || d.levels == 3)) || (d.C == 32 && d.levels == 2))) return false;
-    return bwd_smem_a(d.F, (d.head_mask & G4D_HEAD_SHS) != 0).total + 1024 <= 227 * 1024;
+bool tc_backward_supported(const G4DDeformParams& prm) {
+    const int C = prm.channels, L = prm.levels;
+    if (prm.net_width != 128) return false;
+    if (!((C == 16 && (L == 2 || L == 3)) || (C == 32 && L == 2))) return false;
+    return bwd_smem_a(C * L, (prm.head_mask & G4D_HEAD_SHS) != 0).total + 1024 <= 227 * 1024;
 }
 
 // ======================================================================================================
@@ -226,7 +227,7 @@ deform_tc_bwd_dgrad_kernel(BwdADesc bd, BwdSmemA Ls, int64_t n) {
             if (d.head_mask & (1 << h)) hseq |= (uint32_t)h << (3 * k++);
     }
     // saved ReLU signs are used when the forward that produced them says so (tag word behind the bits)
-    const bool use_bits = bd.relu_bits && __ldg(bd.relu_bits + (size_t)24 * (size_t)n) == 0x5A5A5A5Au;
+    const bool use_bits = bd.relu_bits && __ldg(bd.relu_bits + (size_t)24 * (size_t)n) == kReluBitsTag;
     const int64_t ntiles = (n + 127) / 128;
     const int64_t my_tiles = (int64_t)blockIdx.x < ntiles ? (ntiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
     const uint32_t total_items = (uint32_t)(my_tiles * nheads);
@@ -638,15 +639,32 @@ __global__ void __launch_bounds__(256, 1) deform_tc_bwd_wgrad_kernel(BwdBDesc b)
 // ======================================================================================================
 // host side
 // ======================================================================================================
-size_t tc_deform_backward_scratch_bytes(const DeformDesc& d, int64_t n) {
+// the scratch of the tensor-core backward: the operand images of kernel B (per tile of 128 Gaussians), the fp32 features and
+// their gradient [ntiles * 128][F], the time-row gradients
+struct TcBwdScratch { BwdImages img; float* feat; float* dfeat; float* trow_grad; };
+static TcBwdScratch carve_tc_backward_scratch(Carve& m, const DeformDesc& d, const TimeRows& tr, int64_t n) {
     const size_t ntiles = (size_t)((n + 127) / 128);
-    size_t per_tile = 2 * (size_t)2 * kImg128 + (size_t)2 * 128 * d.F * 2;   // a1, dh, feat
-    for (int h = 0; h < G4D_NUM_HEADS; ++h)
-        if (d.head_mask & (1 << h)) per_tile += 2 * (size_t)2 * kImg128 + (size_t)2 * 128 * (h == 4 ? 48 : 16) * 2;
-    size_t rows = 0;
-    for (int l = 0; l < d.levels; ++l)
-        for (int a = 0; a < 3; ++a) rows += (size_t)d.res[l][a] * d.C;
-    return ntiles * per_tile + rows * 4 + (size_t)2 * ntiles * 128 * d.F * 4 + 16384;
+    TcBwdScratch s{};
+    s.img.feat_bytes = 2u * 128 * d.F * 2;
+    s.img.a1 = m.take<uint8_t>(ntiles * 2 * kImg128);
+    s.img.dh = m.take<uint8_t>(ntiles * 2 * kImg128);
+    s.img.feat = m.take<uint8_t>(ntiles * s.img.feat_bytes);
+    for (int h = 0; h < G4D_NUM_HEADS; ++h) {
+        if (!(d.head_mask & (1 << h))) continue;
+        s.img.dz[h] = m.take<uint8_t>(ntiles * 2 * kImg128);
+        s.img.a2[h] = m.take<uint8_t>(ntiles * 2 * kImg128);
+        s.img.dout[h] = m.take<uint8_t>(ntiles * 2 * 128 * (h == 4 ? 48 : 16) * 2);
+    }
+    s.feat = m.take<float>(ntiles * 128 * d.F);
+    s.dfeat = m.take<float>(ntiles * 128 * d.F);
+    s.trow_grad = m.take<float>(tr.total());
+    return s;
+}
+
+size_t tc_deform_backward_scratch_bytes(const DeformDesc& d, int64_t n) {
+    Carve m;
+    carve_tc_backward_scratch(m, d, TimeRows(d.levels, d.res, d.C), n);
+    return m.bytes();
 }
 
 template <int C, int L>
@@ -668,42 +686,23 @@ cudaError_t launch_deform_backward_tc(const DeformDesc& d, const G4DDeformParams
                                       cudaStream_t st) {
     if (n == 0) return cudaSuccess;
     const int64_t ntiles = (n + 127) / 128;
+    const TimeRows tr(d.levels, d.res, d.C);
+    Carve m(scratch);
+    const TcBwdScratch s = carve_tc_backward_scratch(m, d, tr, n);
     BwdADesc a{};
-    a.d = d; a.w = w; a.relu_bits = relu_bits;
-    uint8_t* p = scratch;
-    auto take = [&](size_t bytes) { uint8_t* o = p; p += (bytes + 255) & ~(size_t)255; return o; };
-    a.img.feat_bytes = 2u * 128 * d.F * 2;
-    a.img.a1 = take((size_t)ntiles * 2 * kImg128);
-    a.img.dh = take((size_t)ntiles * 2 * kImg128);
-    a.img.feat = take((size_t)ntiles * a.img.feat_bytes);
-    for (int h = 0; h < G4D_NUM_HEADS; ++h) {
-        a.go[h] = go[h];
-        if (!(d.head_mask & (1 << h))) continue;
-        a.img.dz[h] = take((size_t)ntiles * 2 * kImg128);
-        a.img.a2[h] = take((size_t)ntiles * 2 * kImg128);
-        a.img.dout[h] = take((size_t)ntiles * 2 * 128 * (h == 4 ? 48 : 16) * 2);
-    }
-    float* feat = reinterpret_cast<float*>(take((size_t)ntiles * 128 * d.F * 4));
-    float* dfeat = reinterpret_cast<float*>(take((size_t)ntiles * 128 * d.F * 4));
-    a.feat = saved_feat ? saved_feat : feat; a.dfeat = dfeat;   // saved_feat: the features the forward of this view staged
-    size_t row_floats = 0;
-    for (int l = 0; l < d.levels; ++l)
-        for (int k = 0; k < 3; ++k) row_floats += (size_t)d.res[l][k] * d.C;
-    float* rows = reinterpret_cast<float*>(take(row_floats * 4));
+    a.d = d; a.w = w; a.relu_bits = relu_bits; a.img = s.img;
+    for (int h = 0; h < G4D_NUM_HEADS; ++h) a.go[h] = go[h];
+    a.feat = saved_feat ? saved_feat : s.feat; a.dfeat = s.dfeat;   // saved_feat: the features the forward of this view staged
     BwdScatterDesc sc{};
-    sc.d = d; sc.dfeat = dfeat;
-    {
-        float* q = rows;
-        for (int l = 0; l < d.levels; ++l) {
-            for (int k = 0; k < 6; ++k) sc.g_planes[l][k] = grads.planes[l][k];
-            for (int k = 0; k < 3; ++k) { sc.trow_grad[l][k] = q; q += (size_t)d.res[l][k] * d.C; }
-        }
-    }
+    sc.d = d; sc.dfeat = s.dfeat;
+    for (int l = 0; l < d.levels; ++l)
+        for (int k = 0; k < 6; ++k) sc.g_planes[l][k] = grads.planes[l][k];
+    tr.place(s.trow_grad, sc.trow_grad);
     for (int h = 0; h < G4D_NUM_HEADS; ++h) { sc.go[h] = go[h]; sc.gi[h] = gi[h]; }
-    cudaError_t e = cudaMemsetAsync(rows, 0, row_floats * 4, st);
+    cudaError_t e = cudaMemsetAsync(s.trow_grad, 0, tr.total() * 4, st);
     if (e != cudaSuccess) return e;
     // the forward's gather (skipped when the forward's feature staging buffer was kept for this backward)
-    if (!saved_feat && (e = launch_deform_features(d, n, xyz, feat, false, st)) != cudaSuccess) return e;
+    if (!saved_feat && (e = launch_deform_features(d, n, xyz, s.feat, false, st)) != cudaSuccess) return e;
     if (d.C == 16 && d.levels == 2) e = launch_a<16, 2>(a, n, sm_count, st);
     else if (d.C == 16 && d.levels == 3) e = launch_a<16, 3>(a, n, sm_count, st);
     else if (d.C == 32 && d.levels == 2) e = launch_a<32, 2>(a, n, sm_count, st);

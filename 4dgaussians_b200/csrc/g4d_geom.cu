@@ -103,21 +103,19 @@ __global__ void collapse_time_rows_kernel(CollapseDesc d, const CameraDev* cam, 
     d.row[l][a][e] = fmaf(v1, ty.w1, v0 * ty.w0);
 }
 
-cudaError_t launch_collapse_time_rows(const G4DDeformParams& p, const CameraDev* cam, float time, bool use_cam_time,
-                                      float* const (*trow)[3], cudaStream_t st) {
+cudaError_t launch_collapse_time_rows(const G4DDeformParams& p, const CameraDev* cam, float time, float* const (*trow)[3],
+                                      cudaStream_t st) {
     CollapseDesc d{};
     d.levels = p.levels; d.C = p.channels;
-    int total = 0;
+    const TimeRows tr(p.levels, p.res, p.channels);
     const int tk[3] = {2, 4, 5};
     for (int l = 0; l < p.levels; ++l) {
         for (int a = 0; a < 4; ++a) d.res[l][a] = p.res[l][a];
-        for (int a = 0; a < 3; ++a) {
-            d.plane[l][a] = p.planes[l][tk[a]]; d.row[l][a] = trow[l][a];
-            d.start[l * 3 + a] = total; total += p.res[l][a] * p.channels;
-        }
+        for (int a = 0; a < 3; ++a) { d.plane[l][a] = p.planes[l][tk[a]]; d.row[l][a] = trow[l][a]; }
     }
-    d.start[p.levels * 3] = total;
-    return launch_k(collapse_time_rows_kernel, dim3((total + 255) / 256), dim3(256), 0, st, true, d, cam, time, use_cam_time ? 1 : 0);
+    for (int m = 0; m <= 3 * p.levels; ++m) d.start[m] = tr.start[m];
+    const int total = (int)tr.total();
+    return launch_k(collapse_time_rows_kernel, dim3((total + 255) / 256), dim3(256), 0, st, true, d, cam, time, 0);
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -270,12 +268,12 @@ deform_kernel(DeformDesc d, DeformSmem L, const CameraDev* __restrict__ camp, fl
     }
 }
 
-cudaError_t launch_deform_tc(const DeformDesc& d, const TcWeights& tw, int mode, const CameraDev* cam, bool use_cam_time,
-                             int64_t n, const DeformIO& io, int sm_count, cudaStream_t st);
+cudaError_t launch_deform_tc(const DeformDesc& d, const TcWeights& tw, int mode, const CameraDev* cam, int64_t n,
+                             const DeformIO& io, int sm_count, cudaStream_t st);
 
 template <int TG, int WD, int MODE>
-static cudaError_t launch_deform_t(const DeformDesc& d, const CameraDev* cam, float time, bool use_cam_time, int64_t n,
-                                   const DeformIO& io, int sm_count, cudaStream_t st) {
+static cudaError_t launch_deform_t(const DeformDesc& d, const CameraDev* cam, float time, int64_t n, const DeformIO& io,
+                                   int sm_count, cudaStream_t st) {
     const DeformSmem L = deform_smem_layout(TG, d.F, WD, d.head_mask);
     const size_t bytes = (size_t)L.total_floats * sizeof(float);
     if (bytes > 227 * 1024) return cudaErrorInvalidConfiguration;
@@ -283,25 +281,20 @@ static cudaError_t launch_deform_t(const DeformDesc& d, const CameraDev* cam, fl
     if (e != cudaSuccess) return e;
     const int64_t ntiles = (n + TG - 1) / TG;
     const int grid = (int)(ntiles < sm_count ? ntiles : sm_count);
-    deform_kernel<TG, WD, MODE><<<grid, kDeformThreads, bytes, st>>>(d, L, cam, time, use_cam_time ? 1 : 0, n, io);
+    deform_kernel<TG, WD, MODE><<<grid, kDeformThreads, bytes, st>>>(d, L, cam, time, 0, n, io);
     return cudaGetLastError();
 }
 
-cudaError_t launch_deform(const DeformDesc& d, int mode, const CameraDev* cam, float time, bool use_cam_time, int64_t n,
-                          const float* xyz, const float* scaling, const float* rotation, const float* opacity,
-                          const float* shs, const float* sh_dc, const float* sh_rest, float* out_xyz, float* out_scaling,
-                          float* out_rotation, float* out_opacity, float* out_shs, GeomBuffers g, FusedOutputs fo,
-                          int32_t* out_radii, int sm_count, cudaStream_t st, const TcWeights* tw) {
+cudaError_t launch_deform(const DeformDesc& d, int mode, const CameraDev* cam, float time, int64_t n, const DeformIO& io,
+                          int sm_count, cudaStream_t st, const TcWeights* tw) {
     if (n == 0) return cudaSuccess;
-    DeformIO io{xyz, scaling, rotation, opacity, shs, sh_dc, sh_rest, out_xyz, out_scaling, out_rotation, out_opacity,
-                out_shs, g, fo, out_radii};
-    if (tw) return launch_deform_tc(d, *tw, mode, cam, use_cam_time, n, io, sm_count, st);
+    if (tw) return launch_deform_tc(d, *tw, mode, cam, n, io, sm_count, st);
     if (d.WD == 128) {
-        return mode == 0 ? launch_deform_t<64, 128, 0>(d, cam, time, use_cam_time, n, io, sm_count, st)
-                         : launch_deform_t<64, 128, 1>(d, cam, time, use_cam_time, n, io, sm_count, st);
+        return mode == 0 ? launch_deform_t<64, 128, 0>(d, cam, time, n, io, sm_count, st)
+                         : launch_deform_t<64, 128, 1>(d, cam, time, n, io, sm_count, st);
     } else if (d.WD == 64) {
-        return mode == 0 ? launch_deform_t<128, 64, 0>(d, cam, time, use_cam_time, n, io, sm_count, st)
-                         : launch_deform_t<128, 64, 1>(d, cam, time, use_cam_time, n, io, sm_count, st);
+        return mode == 0 ? launch_deform_t<128, 64, 0>(d, cam, time, n, io, sm_count, st)
+                         : launch_deform_t<128, 64, 1>(d, cam, time, n, io, sm_count, st);
     }
     return cudaErrorInvalidValue;
 }

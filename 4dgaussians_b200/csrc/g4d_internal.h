@@ -8,6 +8,35 @@
 
 namespace g4d {
 
+// Hands out consecutive sub-ranges of one buffer, each starting on a 256-byte boundary, in the order they are taken.
+// Without a base it hands out null pointers and only counts bytes: one layout function then both sizes a buffer
+// (Carve{}, then bytes()) and places its pointers (Carve{base}).
+struct Carve {
+    char* base;
+    size_t off = 0;
+    explicit Carve(void* b = nullptr) : base(static_cast<char*>(b)) {}
+    template <class T> T* take(size_t count) {
+        T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
+        off += (count * sizeof(T) + 255) / 256 * 256;
+        return p;
+    }
+    size_t bytes() const { return off; }
+};
+
+// The collapsed time rows of a deformation network, level-major, time axis a = x, y, z within a level: row (l, a) holds
+// res[l][a] * C floats from start[3 * l + a]; start[3 * levels] is the total.  The same layout holds their gradients.
+struct TimeRows {
+    int levels = 0;
+    int start[G4D_MAX_LEVELS * 3 + 1] = {};
+    TimeRows(int levels_, const int32_t (*res)[4], int C) : levels(levels_) {
+        for (int m = 0; m < 3 * levels; ++m) start[m + 1] = start[m] + res[m / 3][m % 3] * C;
+    }
+    size_t total() const { return (size_t)start[3 * levels]; }
+    void place(float* base, float* (*rows)[3]) const {
+        for (int m = 0; m < 3 * levels; ++m) rows[m / 3][m % 3] = base + start[m];
+    }
+};
+
 // per-Gaussian projected record kept by a forward (SoA; sizes in DESIGN.md §3)
 struct GeomBuffers {
     float4* rec0;        // (px, py, conic.x, conic.y)
@@ -56,7 +85,7 @@ struct BinPlaceArgs {
     int grid_x, grid_y, num_tiles, band_rows, tight;
 };
 struct BinLayout { uint32_t* chunk_start; uint32_t* M; uint32_t* tile_total; uint32_t* tile_start; BinCtl* ctl; int chunks; };
-size_t bin_aux_bytes(int64_t n, int num_tiles, int sm_count);
+size_t bin_aux_bytes(int64_t n, int num_tiles, int sm_count);   // size of launch_bin_sort's aux area
 // depth sort + chunking + per-(tile, chunk) counts + scan over the chunks: M, tile_total, ctl->R.  One cooperative launch.
 cudaError_t launch_bin_sort(int64_t n, int grid_x, int grid_y, const GeomBuffers& g, void* aux, int tight, int sm_count,
                             BinLayout* out, cudaStream_t st);
@@ -84,6 +113,22 @@ struct FusedOutputs {   // what the fused forward saves for its backward (may be
     float* rot_norm;   // |q| before F.normalize (needed by its backward)
 };
 
+// tensors of one deformation launch (mode 0 reads xyz .. shs and writes out_*; mode 1 also reads sh_dc / sh_rest and writes
+// g, fo and out_radii)
+struct DeformIO {
+    const float *xyz, *scaling, *rotation, *opacity, *shs, *sh_dc, *sh_rest;
+    float *out_xyz, *out_scaling, *out_rotation, *out_opacity, *out_shs;
+    GeomBuffers g;
+    FusedOutputs fo;
+    int32_t* out_radii;
+};
+
+// tag word behind the ReLU sign bits (G4D_RELU_BITS_WORDS): the tensor-core forward that wrote the bits sets it (as the
+// byte pattern of a memset), anything else clears it
+constexpr uint32_t kReluBitsTag = 0x5A5A5A5Au;
+constexpr int kReluBitsTagByte = 0x5A;
+static_assert(kReluBitsTag == 0x01010101u * (uint32_t)kReluBitsTagByte, "the tag is one byte repeated");
+
 // tensor-core weight images (g4d_deform_tc.cu): (hi | lo) parts in the canonical K-major shared-memory layout (tc_wgmma.cuh),
 // FP16x2 (scaled f16) or 3xTF32 words
 struct TcWeights {
@@ -99,7 +144,7 @@ struct TcWeights {
 
 size_t tc_packed_floats(const G4DDeformParams& prm);
 cudaError_t launch_tc_pack_weights(const G4DDeformParams& prm, int arith, float* blob, TcWeights* out, cudaStream_t st);
-bool tc_deform_supported(const DeformDesc& d, int arith);
+bool tc_deform_supported(const G4DDeformParams& prm, int arith);
 // HexPlane gather xyz -> feat [N][F] fp32; pdl: launched dependent on the previous kernel of the forward chain (DESIGN.md §4.6)
 cudaError_t launch_deform_features(const DeformDesc& d, int64_t n, const float* xyz, float* feat, bool pdl, cudaStream_t st);
 
@@ -111,8 +156,8 @@ struct TcBwdWeights {
 };
 size_t tc_bwd_weight_bytes(const G4DDeformParams& prm);
 cudaError_t launch_tc_bwd_pack_weights(const G4DDeformParams& prm, uint8_t* blob, TcBwdWeights* out, cudaStream_t st);
-bool tc_backward_supported(const DeformDesc& d);
-size_t tc_deform_backward_scratch_bytes(const DeformDesc& d, int64_t n);
+bool tc_backward_supported(const G4DDeformParams& prm);
+size_t tc_deform_backward_scratch_bytes(const DeformDesc& d, int64_t n);   // size of launch_deform_backward_tc's scratch
 cudaError_t launch_deform_backward_tc(const DeformDesc& d, const G4DDeformParams& prm, const G4DDeformGrads& grads,
                                       const TcBwdWeights& w, float time, int64_t n, const float* xyz,
                                       const float* const go[G4D_NUM_HEADS], float* const gi[G4D_NUM_HEADS],
@@ -125,16 +170,14 @@ cudaError_t launch_distribute_time_grad(const DeformDesc& d, float* const (*trow
 // ---- launchers (defined in g4d_geom.cu / g4d_raster.cu / g4d_backward.cu) -----------------------------
 cudaError_t launch_pack_camera(const G4DCamera& cam, CameraDev* dst, cudaStream_t st);
 cudaError_t launch_pack_weights(const G4DDeformParams& p, float* w0t, float* const* w1t, cudaStream_t st);
-cudaError_t launch_collapse_time_rows(const G4DDeformParams& p, const CameraDev* cam, float time, bool use_cam_time,
-                                      float* const (*trow)[3], cudaStream_t st);
+cudaError_t launch_collapse_time_rows(const G4DDeformParams& p, const CameraDev* cam, float time, float* const (*trow)[3],
+                                      cudaStream_t st);
 cudaError_t launch_preprocess(const CameraDev* cam, int64_t n, const RasterInputs& in, GeomBuffers g, int32_t* out_radii,
                               cudaStream_t st);
-// mode 0: deform only (writes the five out_* tensors); mode 1: fused deform + preprocess
-cudaError_t launch_deform(const DeformDesc& d, int mode, const CameraDev* cam, float time, bool use_cam_time, int64_t n,
-                          const float* xyz, const float* scaling, const float* rotation, const float* opacity,
-                          const float* shs, const float* sh_dc, const float* sh_rest, float* out_xyz, float* out_scaling,
-                          float* out_rotation, float* out_opacity, float* out_shs, GeomBuffers g, FusedOutputs fo,
-                          int32_t* out_radii, int sm_count, cudaStream_t st, const TcWeights* tw = nullptr);
+// mode 0: deform only (writes the five out_* tensors); mode 1: fused deform + preprocess (camera from cam).  tw: run on the
+// tensor cores with these weight images and buffers
+cudaError_t launch_deform(const DeformDesc& d, int mode, const CameraDev* cam, float time, int64_t n, const DeformIO& io,
+                          int sm_count, cudaStream_t st, const TcWeights* tw = nullptr);
 
 cudaError_t launch_blend_forward(const CameraDev* cam, int grid_x, int grid_y, GeomBuffers g, BinBuffers b, ImageBuffers im,
                                  float* out_color, float* out_depth, int warp_cull, cudaStream_t st);
@@ -147,7 +190,7 @@ cudaError_t launch_preprocess_backward(const CameraDev* cam, int64_t n, const Ra
                                        float* g_means2D_out, float* g_scales, float* g_rotations, float* g_shs,
                                        float* g_sh_dc, float* g_sh_rest, cudaStream_t st);   // fused and split SH sinks may both be given
 
-size_t deform_backward_scratch_bytes(const DeformDesc& d, int64_t n);
+size_t deform_backward_scratch_bytes(const DeformDesc& d, int64_t n);   // size of launch_deform_backward's scratch
 // go[h] / gi[h]: gradient w.r.t. the outputs / inputs of head h's residual tensor (xyz, scaling, rotation, opacity, shs)
 cudaError_t launch_deform_backward(const DeformDesc& d, const G4DDeformParams& prm, const G4DDeformGrads& grads, float time,
                                    int64_t n, const float* xyz, const float* const go[G4D_NUM_HEADS],
@@ -177,7 +220,7 @@ cudaError_t launch_adam_flat(float* p, const float* g, float* m, float* v, int64
                              float b1, float b2, float eps, int64_t step, float grad_scale, int sm_count, cudaStream_t st);
 
 // ---- 3-nearest-neighbour mean squared distance (g4d_knn.cu) ---------------------------------------------------------
-size_t knn_scratch_bytes(int64_t n);
+size_t knn_scratch_bytes(int64_t n);   // size of launch_knn_dist2's scratch
 cudaError_t launch_knn_dist2(int64_t n, const float* xyz, float* out, void* scratch, int sm_count, cudaStream_t st);
 
 

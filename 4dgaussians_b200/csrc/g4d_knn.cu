@@ -168,37 +168,45 @@ __global__ void __launch_bounds__(128) knn_search_kernel(const float* __restrict
     out[me] = ((best[0] + best[1]) + best[2]) / 3.0f;
 }
 
-size_t a256(size_t v) { return (v + 255) / 256 * 256; }
+constexpr size_t kCells = (size_t)128 * 128 * 128 + 1;   // at most 128 cells per axis, + the end of the last one
+
+// bounding box words, the grid, per-cell counts and starts, per-point cell and the points sorted by cell
+struct KnnScratch { uint32_t* mm; KnnGrid* grid; uint32_t* cnt; uint32_t* start; uint32_t* cell_of; uint32_t* sorted; };
+KnnScratch carve_knn_scratch(Carve& m, int64_t n) {
+    const size_t N = (size_t)(n > 0 ? n : 1);
+    KnnScratch s;
+    s.mm = m.take<uint32_t>(16);
+    s.grid = m.take<KnnGrid>(1);
+    s.cnt = m.take<uint32_t>(kCells);
+    s.start = m.take<uint32_t>(kCells);
+    s.cell_of = m.take<uint32_t>(N);
+    s.sorted = m.take<uint32_t>(N);
+    return s;
+}
 
 }  // namespace
 
 size_t knn_scratch_bytes(int64_t n) {
-    const size_t N = (size_t)(n > 0 ? n : 1), cells = (size_t)128 * 128 * 128 + 1;
-    return a256(64) + a256(sizeof(KnnGrid)) + 2 * a256(cells * 4) + 2 * a256(N * 4);
+    Carve m;
+    carve_knn_scratch(m, n);
+    return m.bytes();
 }
 
 cudaError_t launch_knn_dist2(int64_t n, const float* xyz, float* out, void* scratch, int sm_count, cudaStream_t st) {
     if (n <= 0) return cudaSuccess;
-    const size_t N = (size_t)n, cells = (size_t)128 * 128 * 128 + 1;
-    char* p = (char*)scratch;
-    auto take = [&](size_t b) { char* r = p; p += a256(b); return r; };
-    uint32_t* mm = (uint32_t*)take(64);
-    KnnGrid* grid = (KnnGrid*)take(sizeof(KnnGrid));
-    uint32_t* cnt = (uint32_t*)take(cells * 4);
-    uint32_t* start = (uint32_t*)take(cells * 4);
-    uint32_t* cell_of = (uint32_t*)take(N * 4);
-    uint32_t* sorted = (uint32_t*)take(N * 4);
+    Carve m(scratch);
+    const KnnScratch s = carve_knn_scratch(m, n);
     cudaError_t e;
     const uint32_t init[6] = {0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0u, 0u, 0u};
-    if ((e = cudaMemcpyAsync(mm, init, sizeof(init), cudaMemcpyHostToDevice, st)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(cnt, 0, cells * 4, st)) != cudaSuccess) return e;
+    if ((e = cudaMemcpyAsync(s.mm, init, sizeof(init), cudaMemcpyHostToDevice, st)) != cudaSuccess) return e;
+    if ((e = cudaMemsetAsync(s.cnt, 0, kCells * 4, st)) != cudaSuccess) return e;
     int blocks = (int)((n + 255) / 256);
-    knn_bbox_kernel<<<blocks < sm_count * 8 ? blocks : sm_count * 8, 256, 0, st>>>(xyz, n, mm);
-    knn_setup_kernel<<<1, 1, 0, st>>>(mm, n, grid);
-    knn_count_kernel<<<blocks, 256, 0, st>>>(xyz, grid, cnt, cell_of);
-    knn_scan_kernel<<<1, 1024, 0, st>>>(grid, cnt, start);
-    knn_scatter_kernel<<<blocks, 256, 0, st>>>(grid, cell_of, start, cnt, sorted);
-    knn_search_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(xyz, grid, start, sorted, out);
+    knn_bbox_kernel<<<blocks < sm_count * 8 ? blocks : sm_count * 8, 256, 0, st>>>(xyz, n, s.mm);
+    knn_setup_kernel<<<1, 1, 0, st>>>(s.mm, n, s.grid);
+    knn_count_kernel<<<blocks, 256, 0, st>>>(xyz, s.grid, s.cnt, s.cell_of);
+    knn_scan_kernel<<<1, 1024, 0, st>>>(s.grid, s.cnt, s.start);
+    knn_scatter_kernel<<<blocks, 256, 0, st>>>(s.grid, s.cell_of, s.start, s.cnt, s.sorted);
+    knn_search_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(xyz, s.grid, s.start, s.sorted, out);
     return cudaGetLastError();
 }
 

@@ -7,14 +7,6 @@
 
 namespace g4d {
 
-struct DeformIO {
-    const float *xyz, *scaling, *rotation, *opacity, *shs, *sh_dc, *sh_rest;
-    float *out_xyz, *out_scaling, *out_rotation, *out_opacity, *out_shs;
-    GeomBuffers g;
-    FusedOutputs fo;
-    int32_t* out_radii;
-};
-
 // depth range of the visible Gaussians for the binning sort (keys are sorted as bits - min: fewer radix passes).  One RED
 // pair per warp: the lanes that reach this point reduce among themselves first.
 G4D_D void note_depth_range(const GeomBuffers& g, uint32_t tiles, float depth) {
