@@ -10,7 +10,7 @@ this package never compiles or falls back to anything: use ``__graft_entry__.bui
 from . import _lib  # noqa: F401
 from .deformation import deform_network  # noqa: F401
 from .rasterizer import GaussianRasterizationSettings, GaussianRasterizer  # noqa: F401
-from .renderer import render  # noqa: F401
+from .renderer import render, render_cameras  # noqa: F401
 from . import losses  # noqa: F401
 
-__all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "deform_network", "render"]
+__all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "deform_network", "render", "render_cameras"]

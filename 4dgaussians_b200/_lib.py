@@ -32,12 +32,13 @@ ABI_SYMBOLS = [
     "g4d_context_destroy", "g4d_context_stats", "g4d_deform_forward", "g4d_deform_backward", "g4d_rasterize_forward",
     "g4d_rasterize_backward", "g4d_render_forward", "g4d_render_backward", "g4d_workspace_set_option", "g4d_context_read",
     "g4d_context_stage_times", "g4d_debug_tc_cycles", "g4d_l1_loss", "g4d_l1_loss_backward", "g4d_ssim", "g4d_ssim_backward",
-    "g4d_plane_regulation", "g4d_dist2_knn3", "g4d_adam_step",
+    "g4d_plane_regulation", "g4d_dist2_knn3", "g4d_adam_step", "g4d_render_forward_cameras", "g4d_render_backward_cameras",
 ]
 
 fp = C.c_void_p   # device pointers travel as integers
 ABI_VERSION = 3
 CAM_DEBUG, CAM_NO_GRAD = 1, 2      # G4DCamera.debug bits
+MAX_CAMERAS = 32                   # G4D_MAX_CAMERAS: cameras of one g4d_render_forward_cameras call
 
 
 def relu_bits_words(n: int) -> int:
@@ -128,6 +129,11 @@ def load():
                                            fp, fp, fp, C.c_void_p]
         lib.g4d_render_backward.argtypes = [C.c_void_p, C.POINTER(Camera), C.POINTER(DeformParams), C.POINTER(DeformGrads),
                                             C.POINTER(Gaussians), fp, C.POINTER(GaussianGrads), C.c_void_p]
+        pp = C.POINTER(C.c_void_p)     # host array of device pointers / contexts
+        lib.g4d_render_forward_cameras.argtypes = [pp, C.c_int32, C.POINTER(Camera), C.POINTER(DeformParams), C.POINTER(Gaussians),
+                                                   pp, pp, pp, C.c_void_p]
+        lib.g4d_render_backward_cameras.argtypes = [pp, C.c_int32, C.POINTER(Camera), C.POINTER(DeformParams), C.POINTER(DeformGrads),
+                                                    C.POINTER(Gaussians), pp, C.POINTER(GaussianGrads), pp, C.c_void_p]
         lib.g4d_l1_loss.argtypes = [C.c_void_p, fp, fp, C.c_int64, C.c_float, fp, C.c_void_p]
         lib.g4d_l1_loss_backward.argtypes = [C.c_void_p, fp, fp, C.c_int64, C.c_float, fp, fp, C.c_void_p]
         lib.g4d_ssim.argtypes = [C.c_void_p, fp, fp, C.c_int32, C.c_int32, C.c_int32, C.c_float, fp, fp, C.c_void_p]

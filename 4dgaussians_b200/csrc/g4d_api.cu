@@ -2,6 +2,7 @@
 // No torch types, no CPU fallback: every entry point either runs the CUDA path or returns an error code.
 #include <cstdio>
 #include <cstdlib>
+#include <atomic>
 #include <cstring>
 #include <mutex>
 #include <string>
@@ -130,6 +131,12 @@ struct G4DContext {
     const void* bin_ctl = nullptr;    // device BinCtl of the last forward
     bool learned = false;             // R of an earlier exact forward is known (no-sync mode needs a learnt capacity)
     bool has_forward = false, is_fused = false, fused_sh = false, deformed = false, fo_valid = false;
+    // multi-camera forward (g4d_render_forward_cameras) whose state this context holds: serial number of that call (0: the
+    // last forward was a single-camera one), this camera's position and the number of cameras; on camera 0, whether the
+    // forward kept what the group backward reads
+    uint64_t group = 0;
+    int group_pos = 0, group_size = 0;
+    bool group_grad = false;
     GeomBuffers g{};
     BinBuffers b{};
     ImageBuffers im{};
@@ -622,7 +629,7 @@ int g4d_rasterize_forward(G4DContext* c, const G4DCamera* cam, int64_t n, const 
     cudaStream_t st = (cudaStream_t)stream;
     G4D_CUDA(cudaSetDevice(c->ws->device));
     if ((rc = check_pending(c)) != G4D_OK) return rc;
-    c->has_forward = false; c->is_fused = false; c->deformed = false;
+    c->has_forward = false; c->is_fused = false; c->deformed = false; c->group = 0;
     if ((rc = ensure_geom(c, n)) != G4D_OK) return rc;
     if ((rc = ensure_image(c, cam->image_height, cam->image_width)) != G4D_OK) return rc;
     reset_stage_flags(c, 0, G4D_STAGE_COUNT - 1);
@@ -770,22 +777,32 @@ int g4d_deform_backward(G4DWorkspace* ws, const G4DDeformParams* prm, G4DDeformG
     return deform_backward_dispatch(ws, prm, trow, grads, time, n, xyz, go, gi, relu_bits, nullptr, st);
 }
 
+}  // extern "C"
+
 // ------------------------------------------------------------------------------------------------------
-int g4d_render_forward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* prm, const G4DGaussians* g,
-                       float* out_color, float* out_depth, int32_t* out_radii, void* stream) {
-    if (!c) return fail(G4D_ERR_ARG, "context is NULL");
+namespace {
+
+int check_render_args(const G4DCamera* cam, const G4DDeformParams* prm, const G4DGaussians* g, const float* out_color,
+                      const float* out_depth, const int32_t* out_radii) {
     int rc = check_camera(cam);
     if (rc != G4D_OK) return rc;
     if (prm && (rc = check_params(prm)) != G4D_OK) return rc;
     if (!g || g->n < 0 || g->n >= (1ll << 31) || !out_color || !out_depth) return fail(G4D_ERR_ARG, "bad gaussians / outputs");
-    const int64_t n = g->n;
-    if (n > 0 && (!g->xyz || !g->scaling || !g->rotation || !g->opacity || !g->features_dc || !out_radii))
+    if (g->n > 0 && (!g->xyz || !g->scaling || !g->rotation || !g->opacity || !g->features_dc || !out_radii))
         return fail(G4D_ERR_ARG, "NULL gaussian tensor");
-    cudaStream_t st = (cudaStream_t)stream;
+    return G4D_OK;
+}
+
+// The fused forward of one camera on c.  keep_fo: store the deformed, activated tensors even under G4D_CAM_NO_GRAD (other
+// cameras of the same call read them).
+int fused_forward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* prm, const G4DGaussians* g, float* out_color,
+                  float* out_depth, int32_t* out_radii, bool keep_fo, cudaStream_t st) {
+    const int64_t n = g->n;
     G4DWorkspace* ws = c->ws;
+    int rc;
     G4D_CUDA(cudaSetDevice(ws->device));
     if ((rc = check_pending(c)) != G4D_OK) return rc;
-    c->has_forward = false;
+    c->has_forward = false; c->group = 0;
     const bool with_sh = prm && (prm->head_mask & G4D_HEAD_SHS);
     if ((rc = ensure_geom(c, n)) != G4D_OK) return rc;
     if ((rc = ensure_image(c, cam->image_height, cam->image_width)) != G4D_OK) return rc;
@@ -795,7 +812,7 @@ int g4d_render_forward(G4DContext* c, const G4DCamera* cam, const G4DDeformParam
     const float* shs = g->features_rest ? nullptr : g->features_dc;
     const float* dc = g->features_rest ? g->features_dc : nullptr;
     // a no-grad render needs none of the saved tensors: skip their stores (48 B + 192 B of deformed SH per Gaussian)
-    c->fo_valid = !(cam->debug & G4D_CAM_NO_GRAD) || ws->keep_deformed;
+    c->fo_valid = !(cam->debug & G4D_CAM_NO_GRAD) || ws->keep_deformed || keep_fo;
     const FusedOutputs fo_arg = c->fo_valid ? c->fo : FusedOutputs{};
     DeformSetup s{};
     {
@@ -828,31 +845,41 @@ int g4d_render_forward(G4DContext* c, const G4DCamera* cam, const G4DDeformParam
     return G4D_OK;
 }
 
-int g4d_render_backward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* prm, G4DDeformGrads* pgrads,
-                        const G4DGaussians* g, const float* dL_dcolor, G4DGaussianGrads* gg, void* stream) {
-    if (!c) return fail(G4D_ERR_ARG, "context is NULL");
-    if (!c->has_forward || !c->is_fused || !g || c->n != g->n) return fail(G4D_ERR_STATE, "g4d_render_backward needs the matching g4d_render_forward on this context");
-    if (!c->fo_valid) return fail(G4D_ERR_STATE, "g4d_render_backward after a G4D_CAM_NO_GRAD forward: nothing was saved for it");
-    if ((prm != nullptr) != c->deformed) return fail(G4D_ERR_STATE, "deform params differ from the forward's");
-    int rc = check_camera(cam);
-    if (rc != G4D_OK) return rc;
-    if (prm && (rc = check_params(prm)) != G4D_OK) return rc;
-    if (prm && !pgrads) return fail(G4D_ERR_ARG, "pgrads is NULL");
-    if (cam->image_height != c->H || cam->image_width != c->W) return fail(G4D_ERR_STATE, "camera differs from the forward's");
+// the post-activation inputs of the rasterizer stages of a fused forward on c: its stored deformed tensors, and the SH
+// coefficients (deformed when the SHS head is active, the caller's otherwise)
+RasterInputs deformed_inputs(const G4DContext* c, const G4DGaussians* g) {
+    const bool split = g->features_rest != nullptr;
+    return RasterInputs{c->fo.means3D, c->fo.scales, c->fo.rotations, c->fo.opacities,
+                        c->fused_sh ? c->fo.shs : (split ? nullptr : g->features_dc), split ? g->features_dc : nullptr,
+                        g->features_rest};
+}
+
+// gradients w.r.t. the deformed tensors of a fine-stage backward: scratch on c (the network's backward reads them)
+struct DeformedGrads { float *xyz, *sc, *rot, *op, *sh; };
+int deformed_grads(G4DContext* c, int64_t n, DeformedGrads* out) {
+    const size_t N = (size_t)n;
+    DeformedGrads& d = *out;
+    auto layout = [&](Carve& m) {
+        d.xyz = m.take<float>(3 * N); d.sc = m.take<float>(3 * N); d.rot = m.take<float>(4 * N); d.op = m.take<float>(N);
+        d.sh = m.take<float>(c->fused_sh ? 48 * N : 4);
+    };
+    G4D_CUDA(ensure_layout(c->gdeform, layout));
+    if (!c->fused_sh) d.sh = nullptr;
+    return G4D_OK;
+}
+
+// The backward of a fused forward of one camera on c (arguments checked by the caller).  gg->means2D may be NULL.
+int fused_backward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* prm, G4DDeformGrads* pgrads, const G4DGaussians* g,
+                   const float* dL_dcolor, const G4DGaussianGrads* gg, cudaStream_t st) {
     const int64_t n = g->n;
-    if (!dL_dcolor || !gg || (n > 0 && (!gg->xyz || !gg->scaling || !gg->rotation || !gg->opacity || !gg->features_dc || !gg->means2D)))
-        return fail(G4D_ERR_ARG, "NULL gradient pointer");
-    if (g->features_rest && n > 0 && !gg->features_rest) return fail(G4D_ERR_ARG, "features_rest gradient sink is NULL");
-    cudaStream_t st = (cudaStream_t)stream;
     G4DWorkspace* ws = c->ws;
+    int rc;
     G4D_CUDA(cudaSetDevice(ws->device));
     if ((rc = check_pending(c)) != G4D_OK) return rc;
     if (n == 0) return G4D_OK;
     const size_t N = (size_t)n;
     const bool split = g->features_rest != nullptr;
-    RasterInputs in{c->fo.means3D, c->fo.scales, c->fo.rotations, c->fo.opacities,
-                    c->fused_sh ? c->fo.shs : (split ? nullptr : g->features_dc), split ? g->features_dc : nullptr,
-                    g->features_rest};
+    const RasterInputs in = deformed_inputs(c, g);
     float* sh_fused_sink = split ? nullptr : gg->features_dc;
     float* sh_dc_sink = split ? gg->features_dc : nullptr;
     float* sh_rest_sink = split ? gg->features_rest : nullptr;
@@ -864,22 +891,16 @@ int g4d_render_backward(G4DContext* c, const G4DCamera* cam, const G4DDeformPara
         return debug_sync(cam, st, "activation_backward");
     }
     // gradients w.r.t. the deformed tensors land in scratch, then flow through the deformation network
-    float *gd_xyz, *gd_sc, *gd_rot, *gd_op, *gd_sh;
-    auto layout = [&](Carve& m) {
-        gd_xyz = m.take<float>(3 * N); gd_sc = m.take<float>(3 * N); gd_rot = m.take<float>(4 * N); gd_op = m.take<float>(N);
-        gd_sh = m.take<float>(c->fused_sh ? 48 * N : 4);
-    };
-    G4D_CUDA(ensure_layout(c->gdeform, layout));
-    if (!c->fused_sh) gd_sh = nullptr;
+    DeformedGrads d;
+    if ((rc = deformed_grads(c, n, &d)) != G4D_OK) return rc;
     // SH gradient: identity residual path -> written straight into the caller's sinks; the fused copy (when the SHS
     // head is active) additionally feeds the network's backward
-    if (c->fused_sh && !split) { sh_fused_sink = gg->features_dc; }
-    rc = raster_backward_stages(c, cam, n, in, dL_dcolor, gd_xyz, gg->means2D, c->fused_sh ? gd_sh : sh_fused_sink, sh_dc_sink,
-                                sh_rest_sink, gd_op, gd_sc, gd_rot, st);
+    rc = raster_backward_stages(c, cam, n, in, dL_dcolor, d.xyz, gg->means2D, c->fused_sh ? d.sh : sh_fused_sink, sh_dc_sink,
+                                sh_rest_sink, d.op, d.sc, d.rot, st);
     if (rc != G4D_OK) return rc;
-    if (c->fused_sh && !split) G4D_CUDA(cudaMemcpyAsync(gg->features_dc, gd_sh, N * 192, cudaMemcpyDeviceToDevice, st));
-    G4D_CUDA(launch_activation_backward(n, c->fo, gd_sc, gd_rot, gd_op, st));
-    const float* go[G4D_NUM_HEADS] = {gd_xyz, gd_sc, gd_rot, gd_op, gd_sh};
+    if (c->fused_sh && !split) G4D_CUDA(cudaMemcpyAsync(gg->features_dc, d.sh, N * 192, cudaMemcpyDeviceToDevice, st));
+    G4D_CUDA(launch_activation_backward(n, c->fo, d.sc, d.rot, d.op, st));
+    const float* go[G4D_NUM_HEADS] = {d.xyz, d.sc, d.rot, d.op, d.sh};
     float* gi[G4D_NUM_HEADS] = {gg->xyz, gg->scaling, gg->rotation, gg->opacity, nullptr};
     {
         StageTimer tm(c, G4D_STAGE_DEFORM_BWD, st);
@@ -888,6 +909,194 @@ int g4d_render_backward(G4DContext* c, const G4DCamera* cam, const G4DDeformPara
                                            c->relu_saved ? c->feat.as<float>() : nullptr, st)) != G4D_OK) return rc;
     }
     return debug_sync(cam, st, "deform_backward");
+}
+
+// k cameras on k contexts: 1 <= k <= G4D_MAX_CAMERAS, one time bit for bit, pairwise distinct contexts of one workspace.
+// The cameras are checked before any context is looked at.
+int check_camera_group(G4DContext* const* ctx, int32_t k, const G4DCamera* cams) {
+    if (k < 1 || k > G4D_MAX_CAMERAS) return fail(G4D_ERR_ARG, "the number of cameras must be in 1..G4D_MAX_CAMERAS");
+    if (!cams) return fail(G4D_ERR_ARG, "cameras are NULL");
+    int rc;
+    for (int i = 0; i < k; ++i) {
+        if ((rc = check_camera(&cams[i])) != G4D_OK) return rc;
+        if (memcmp(&cams[i].time, &cams[0].time, sizeof(float)) != 0)
+            return fail(G4D_ERR_ARG, "the cameras of one call must share their time bit for bit");
+    }
+    if (!ctx) return fail(G4D_ERR_ARG, "contexts are NULL");
+    for (int i = 0; i < k; ++i) {
+        if (!ctx[i]) return fail(G4D_ERR_ARG, "context is NULL");
+        if (ctx[i]->ws != ctx[0]->ws) return fail(G4D_ERR_ARG, "the contexts of one call must belong to one workspace");
+        for (int j = 0; j < i; ++j)
+            if (ctx[j] == ctx[i]) return fail(G4D_ERR_ARG, "the contexts of one call must be pairwise distinct");
+    }
+    return G4D_OK;
+}
+
+std::atomic<uint64_t> g_group_serial{0};
+
+}  // namespace
+
+extern "C" {
+
+int g4d_render_forward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* prm, const G4DGaussians* g,
+                       float* out_color, float* out_depth, int32_t* out_radii, void* stream) {
+    if (!c) return fail(G4D_ERR_ARG, "context is NULL");
+    int rc = check_render_args(cam, prm, g, out_color, out_depth, out_radii);
+    if (rc != G4D_OK) return rc;
+    return fused_forward(c, cam, prm, g, out_color, out_depth, out_radii, false, (cudaStream_t)stream);
+}
+
+int g4d_render_backward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* prm, G4DDeformGrads* pgrads,
+                        const G4DGaussians* g, const float* dL_dcolor, G4DGaussianGrads* gg, void* stream) {
+    if (!c) return fail(G4D_ERR_ARG, "context is NULL");
+    if (!c->has_forward || !c->is_fused || !g || c->n != g->n) return fail(G4D_ERR_STATE, "g4d_render_backward needs the matching g4d_render_forward on this context");
+    if (c->group) return fail(G4D_ERR_STATE, "the last forward on this context was g4d_render_forward_cameras: use g4d_render_backward_cameras");
+    if (!c->fo_valid) return fail(G4D_ERR_STATE, "g4d_render_backward after a G4D_CAM_NO_GRAD forward: nothing was saved for it");
+    if ((prm != nullptr) != c->deformed) return fail(G4D_ERR_STATE, "deform params differ from the forward's");
+    int rc = check_camera(cam);
+    if (rc != G4D_OK) return rc;
+    if (prm && (rc = check_params(prm)) != G4D_OK) return rc;
+    if (prm && !pgrads) return fail(G4D_ERR_ARG, "pgrads is NULL");
+    if (cam->image_height != c->H || cam->image_width != c->W) return fail(G4D_ERR_STATE, "camera differs from the forward's");
+    const int64_t n = g->n;
+    if (!dL_dcolor || !gg || (n > 0 && (!gg->xyz || !gg->scaling || !gg->rotation || !gg->opacity || !gg->features_dc || !gg->means2D)))
+        return fail(G4D_ERR_ARG, "NULL gradient pointer");
+    if (g->features_rest && n > 0 && !gg->features_rest) return fail(G4D_ERR_ARG, "features_rest gradient sink is NULL");
+    return fused_backward(c, cam, prm, pgrads, g, dL_dcolor, gg, (cudaStream_t)stream);
+}
+
+// ------------------------------------------------------------------------------------------------------
+int g4d_render_forward_cameras(G4DContext* const* ctx, int32_t k, const G4DCamera* cams, const G4DDeformParams* prm,
+                               const G4DGaussians* g, float* const* out_color, float* const* out_depth,
+                               int32_t* const* out_radii, void* stream) {
+    int rc = check_camera_group(ctx, k, cams);
+    if (rc != G4D_OK) return rc;
+    if (!out_color || !out_depth || !out_radii) return fail(G4D_ERR_ARG, "output arrays are NULL");
+    for (int i = 0; i < k; ++i)
+        if ((rc = check_render_args(&cams[i], prm, g, out_color[i], out_depth[i], out_radii[i])) != G4D_OK) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    G4DContext* c0 = ctx[0];
+    G4D_CUDA(cudaSetDevice(c0->ws->device));
+    for (int i = 0; i < k; ++i) {
+        if ((rc = check_pending(ctx[i])) != G4D_OK) return rc;
+        ctx[i]->has_forward = false; ctx[i]->group = 0;
+    }
+    // camera 0: the fused forward of g4d_render_forward; it keeps the deformed tensors when other cameras read them
+    if ((rc = fused_forward(c0, &cams[0], prm, g, out_color[0], out_depth[0], out_radii[0], k > 1, st)) != G4D_OK) return rc;
+    const int64_t n = g->n;
+    if (k > 1) {
+        ExtraCameras ec{};
+        ec.count = k - 1;
+        for (int i = 1; i < k; ++i) {
+            G4DContext* c = ctx[i];
+            if ((rc = ensure_geom(c, n)) != G4D_OK) return rc;
+            if ((rc = ensure_image(c, cams[i].image_height, cams[i].image_width)) != G4D_OK) return rc;
+            reset_stage_flags(c, 0, G4D_STAGE_COUNT - 1);
+            {
+                StageTimer tm(c, G4D_STAGE_PREP, st);
+                G4D_CUDA(launch_pack_camera(cams[i], c->cam.as<CameraDev>(), st));
+            }
+            ec.cam[i - 1] = c->cam.as<CameraDev>(); ec.g[i - 1] = c->g; ec.out_radii[i - 1] = out_radii[i];
+        }
+        {
+            StageTimer tm(ctx[1], G4D_STAGE_GEOM, st);
+            G4D_CUDA(launch_project_cameras(ec, n, deformed_inputs(c0, g), st));
+        }
+        if ((rc = debug_sync(&cams[1], st, "project_cameras")) != G4D_OK) return rc;
+        for (int i = 1; i < k; ++i) {
+            G4DContext* c = ctx[i];
+            if ((rc = bin_and_blend(c, &cams[i], n, out_color[i], out_depth[i], st)) != G4D_OK) return rc;
+            c->is_fused = true; c->deformed = c0->deformed; c->fused_sh = c0->fused_sh; c->fo_valid = false;
+        }
+    }
+    const uint64_t serial = ++g_group_serial;
+    for (int i = 0; i < k; ++i) { ctx[i]->group = serial; ctx[i]->group_pos = i; ctx[i]->group_size = k; }
+    c0->group_grad = !(cams[0].debug & G4D_CAM_NO_GRAD);
+    return G4D_OK;
+}
+
+int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCamera* cams, const G4DDeformParams* prm,
+                                G4DDeformGrads* pgrads, const G4DGaussians* g, const float* const* dL_dcolor,
+                                G4DGaussianGrads* gg, float* const* g_means2D, void* stream) {
+    int rc = check_camera_group(ctx, k, cams);
+    if (rc != G4D_OK) return rc;
+    if (!g || !dL_dcolor || !gg) return fail(G4D_ERR_ARG, "NULL argument");
+    if (gg->means2D) return fail(G4D_ERR_ARG, "gg->means2D must be NULL: the screen-space gradients go to g_means2D[i]");
+    G4DContext* c0 = ctx[0];
+    for (int i = 0; i < k; ++i) {
+        const G4DContext* c = ctx[i];
+        if (!c->has_forward || !c->group || c->group != c0->group || c->group_pos != i || c->group_size != k || c->n != g->n)
+            return fail(G4D_ERR_STATE, "g4d_render_backward_cameras needs the matching g4d_render_forward_cameras on these contexts, "
+                                       "with no other forward on any of them since");
+        if (cams[i].image_height != c->H || cams[i].image_width != c->W) return fail(G4D_ERR_STATE, "camera differs from the forward's");
+    }
+    if (!c0->group_grad || !c0->fo_valid) return fail(G4D_ERR_STATE, "g4d_render_backward_cameras after a G4D_CAM_NO_GRAD forward: nothing was saved for it");
+    if ((prm != nullptr) != c0->deformed) return fail(G4D_ERR_STATE, "deform params differ from the forward's");
+    if (prm && (rc = check_params(prm)) != G4D_OK) return rc;
+    if (prm && !pgrads) return fail(G4D_ERR_ARG, "pgrads is NULL");
+    const int64_t n = g->n;
+    if (n > 0 && (!gg->xyz || !gg->scaling || !gg->rotation || !gg->opacity || !gg->features_dc))
+        return fail(G4D_ERR_ARG, "NULL gradient pointer");
+    if (g->features_rest && n > 0 && !gg->features_rest) return fail(G4D_ERR_ARG, "features_rest gradient sink is NULL");
+    cudaStream_t st = (cudaStream_t)stream;
+    G4DWorkspace* ws = c0->ws;
+    G4D_CUDA(cudaSetDevice(ws->device));
+    for (int i = 0; i < k; ++i)
+        if ((rc = check_pending(ctx[i])) != G4D_OK) return rc;
+    if (k == 1 && dL_dcolor[0]) {     // one camera: the single-camera backward
+        G4DGaussianGrads g1 = *gg;
+        g1.means2D = g_means2D ? g_means2D[0] : nullptr;
+        return fused_backward(c0, &cams[0], prm, pgrads, g, dL_dcolor[0], &g1, st);
+    }
+    if (n == 0) return G4D_OK;
+    const size_t N = (size_t)n;
+    const bool split = g->features_rest != nullptr;
+    float* sh_fused_sink = split ? nullptr : gg->features_dc;
+    float* sh_dc_sink = split ? gg->features_dc : nullptr;
+    float* sh_rest_sink = split ? gg->features_rest : nullptr;
+    DeformedGrads d{gg->xyz, gg->scaling, gg->rotation, gg->opacity, nullptr};   // coarse: straight into the caller's sinks
+    if (c0->deformed && (rc = deformed_grads(c0, n, &d)) != G4D_OK) return rc;
+    // blend backward of every camera in the loss, each into its own scratch: d(mean2D), d(conic), d(rgb), d(opacity)
+    BackwardCameras bc{};
+    for (int i = 0; i < k; ++i) {
+        G4DContext* c = ctx[i];
+        reset_stage_flags(c, G4D_STAGE_BLEND_BWD, G4D_STAGE_DEFORM_BWD);
+        if (!dL_dcolor[i]) {
+            if (g_means2D && g_means2D[i]) G4D_CUDA(cudaMemsetAsync(g_means2D[i], 0, N * 12, st));
+            continue;
+        }
+        G4D_CUDA(c->gscratch.ensure(N * 9 * 4 + 256));
+        float* gb = c->gscratch.as<float>();
+        G4D_CUDA(cudaMemsetAsync(gb, 0, N * 9 * 4, st));
+        {
+            StageTimer tm(c, G4D_STAGE_BLEND_BWD, st);
+            G4D_CUDA(launch_blend_backward(c->cam.as<CameraDev>(), c->grid_x, c->grid_y, c->g, c->b, c->im, dL_dcolor[i], gb,
+                                           gb + 2 * N, gb + 8 * N, gb + 5 * N, ws->warp_cull, st));
+        }
+        if ((rc = debug_sync(&cams[i], st, "blend_backward")) != G4D_OK) return rc;
+        const int j = bc.count++;
+        bc.cam[j] = c->cam.as<CameraDev>(); bc.radii[j] = c->g.radii; bc.clamped[j] = c->g.clamped; bc.grad[j] = gb;
+        bc.g_means2D[j] = g_means2D ? g_means2D[i] : nullptr;
+    }
+    {
+        StageTimer tm(c0, G4D_STAGE_GEOM_BWD, st);
+        G4D_CUDA(launch_preprocess_backward_cameras(bc, n, deformed_inputs(c0, g), d.xyz, d.sc, d.rot, d.op,
+                                                    c0->fused_sh ? d.sh : sh_fused_sink, sh_dc_sink, sh_rest_sink, st));
+    }
+    if ((rc = debug_sync(&cams[0], st, "preprocess_backward_cameras")) != G4D_OK) return rc;
+    if (c0->fused_sh && !split) G4D_CUDA(cudaMemcpyAsync(gg->features_dc, d.sh, N * 192, cudaMemcpyDeviceToDevice, st));
+    G4D_CUDA(launch_activation_backward(n, c0->fo, d.sc, d.rot, d.op, st));
+    if (!c0->deformed) return debug_sync(&cams[0], st, "activation_backward");
+    // the network's backward, once, on the gradients summed over the cameras
+    const float* go[G4D_NUM_HEADS] = {d.xyz, d.sc, d.rot, d.op, d.sh};
+    float* gi[G4D_NUM_HEADS] = {gg->xyz, gg->scaling, gg->rotation, gg->opacity, nullptr};
+    {
+        StageTimer tm(c0, G4D_STAGE_DEFORM_BWD, st);
+        if ((rc = deform_backward_dispatch(ws, prm, c0->trow_ptr, pgrads, cams[0].time, n, g->xyz, go, gi,
+                                           c0->relu_saved ? c0->relu.as<uint32_t>() : nullptr,
+                                           c0->relu_saved ? c0->feat.as<float>() : nullptr, st)) != G4D_OK) return rc;
+    }
+    return debug_sync(&cams[0], st, "deform_backward");
 }
 
 // ------------------------------------------------------------------------------------------------------

@@ -92,6 +92,93 @@ cudaError_t launch_preprocess_backward(const CameraDev* cam, int64_t n, const Ra
     return cudaGetLastError();
 }
 
+// Per-Gaussian backward of several cameras at one timestamp (g4d_render_backward_cameras): the deformed state and the SH
+// coefficients are loaded once, gaussian_backward runs for every camera that sees the Gaussian, and the sums -- mean,
+// scale and rotation in registers, SH in the warp's shared-memory rows, opacity from the cameras' blend backward passes --
+// are written once.  Each camera's screen-space gradient goes to its own sink.
+__global__ void __launch_bounds__(128)
+preprocess_backward_cameras_kernel(BackwardCameras bc, int64_t n, RasterInputs in, float* __restrict__ g_means3D,
+                                   float* __restrict__ g_scales, float* __restrict__ g_rotations, float* __restrict__ g_opacities,
+                                   float* __restrict__ g_shs, float* __restrict__ g_sh_dc, float* __restrict__ g_sh_rest) {
+    constexpr int kRow = 49;
+    constexpr int kCamWords = (int)(sizeof(CameraDev) / 4);
+    extern __shared__ float sh_smem[];             // [warps][2][32 * kRow]: SH coefficients, SH gradient sums
+    __shared__ CameraDev cams[G4D_MAX_CAMERAS];
+    for (int i = threadIdx.x; i < bc.count * kCamWords; i += blockDim.x) {
+        const int c = i / kCamWords, w = i - c * kCamWords;
+        reinterpret_cast<uint32_t*>(&cams[c])[w] = reinterpret_cast<const uint32_t*>(bc.cam[c])[w];
+    }
+    __syncthreads();
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    float* ld = sh_smem + (size_t)warp * 2 * 32 * kRow;
+    float* st = ld + 32 * kRow;
+    const int64_t g0 = (int64_t)blockIdx.x * blockDim.x + warp * 32;
+    const int cnt = (int)(n - g0 < 32 ? (n - g0 > 0 ? n - g0 : 0) : 32);
+    if (cnt == 0) return;
+    const int64_t gi = g0 + lane;
+    for (int idx = lane; idx < cnt * 48; idx += 32) {
+        const int i = idx / 48, e = idx - i * 48;
+        float v;
+        if (in.shs) v = __ldg(in.shs + g0 * 48 + idx);
+        else v = e < 3 ? __ldg(in.sh_dc + (g0 + i) * 3 + e) : __ldg(in.sh_rest + (g0 + i) * 45 + (e - 3));
+        ld[i * kRow + e] = v;
+        st[i * kRow + e] = 0.f;
+    }
+    __syncwarp();
+    if (lane < cnt) {
+        const Vec3 p{in.means3D[3 * gi], in.means3D[3 * gi + 1], in.means3D[3 * gi + 2]};
+        const Vec3 sc{in.scales[3 * gi], in.scales[3 * gi + 1], in.scales[3 * gi + 2]};
+        const float4 q4 = *reinterpret_cast<const float4*>(in.rotations + 4 * gi);
+        const float* row = ld + lane * kRow;
+        float* srow = st + lane * kRow;
+        float gm[3] = {0.f, 0.f, 0.f}, gs[3] = {0.f, 0.f, 0.f}, gr[4] = {0.f, 0.f, 0.f, 0.f}, gop = 0.f;
+        for (int c = 0; c < bc.count; ++c) {
+            const float* gb = bc.grad[c];
+            gop += gb[8 * n + gi];
+            const bool vis = bc.radii[c][gi] > 0;
+            if (bc.g_means2D[c]) {
+                bc.g_means2D[c][3 * gi] = vis ? gb[2 * gi] : 0.f;
+                bc.g_means2D[c][3 * gi + 1] = vis ? gb[2 * gi + 1] : 0.f;
+                bc.g_means2D[c][3 * gi + 2] = 0.f;
+            }
+            if (!vis) continue;
+            const float gm2[2] = {gb[2 * gi], gb[2 * gi + 1]};
+            const float gc[3] = {gb[2 * n + 3 * gi], gb[2 * n + 3 * gi + 1], gb[2 * n + 3 * gi + 2]};
+            const float grgb[3] = {gb[5 * n + 3 * gi], gb[5 * n + 3 * gi + 1], gb[5 * n + 3 * gi + 2]};
+            GaussGrad gg;
+            gaussian_backward(cams[c], p, sc, Quat{q4.x, q4.y, q4.z, q4.w}, (uint32_t)bc.clamped[c][gi], gm2, gc, grgb,
+                              [&](int k, int ch) { return row[3 * k + ch]; },
+                              [&](int k, int ch, float v) { srow[3 * k + ch] += v; }, gg);
+            for (int k = 0; k < 3; ++k) { gm[k] += gg.mean[k]; gs[k] += gg.scale[k]; }
+            for (int k = 0; k < 4; ++k) gr[k] += gg.rot[k];
+        }
+        for (int k = 0; k < 3; ++k) { g_means3D[3 * gi + k] = gm[k]; g_scales[3 * gi + k] = gs[k]; }
+        for (int k = 0; k < 4; ++k) g_rotations[4 * gi + k] = gr[k];
+        g_opacities[gi] = gop;
+    }
+    __syncwarp();
+    for (int idx = lane; idx < cnt * 48; idx += 32) {
+        const int i = idx / 48, e = idx - i * 48;
+        const float v = st[i * kRow + e];
+        if (g_shs) g_shs[g0 * 48 + idx] = v;
+        if (e < 3) { if (g_sh_dc) g_sh_dc[(g0 + i) * 3 + e] = v; }
+        else if (g_sh_rest) g_sh_rest[(g0 + i) * 45 + (e - 3)] = v;
+    }
+}
+
+cudaError_t launch_preprocess_backward_cameras(const BackwardCameras& bc, int64_t n, const RasterInputs& in, float* g_means3D,
+                                               float* g_scales, float* g_rotations, float* g_opacities, float* g_shs,
+                                               float* g_sh_dc, float* g_sh_rest, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    constexpr int kThreads = 128;
+    const size_t smem = (size_t)(kThreads / 32) * 2 * 32 * 49 * sizeof(float);   // 50 KB: SH staging and sums
+    cudaError_t e = cudaFuncSetAttribute(preprocess_backward_cameras_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    preprocess_backward_cameras_kernel<<<(unsigned)((n + kThreads - 1) / kThreads), kThreads, smem, st>>>(
+        bc, n, in, g_means3D, g_scales, g_rotations, g_opacities, g_shs, g_sh_dc, g_sh_rest);
+    return cudaGetLastError();
+}
+
 // ======================================================================================================
 // Backward of the deformation network.
 //

@@ -156,6 +156,63 @@ cudaError_t launch_preprocess(const CameraDev* cam, int64_t n, const RasterInput
 }
 
 // ------------------------------------------------------------------------------------------------------
+// Extra cameras of a multi-camera forward (g4d_render_forward_cameras): one thread per Gaussian reads the deformed,
+// activated state camera 0's fused forward stored (44 B, plus 192 B of SH staged per warp through shared memory) ONCE and
+// projects it into every other camera with the fused kernels' projection and colour code: the inputs are the very floats
+// those kernels held in registers, so each camera's records equal its own render()'s bit for bit.
+__global__ void __launch_bounds__(256) project_cameras_kernel(ExtraCameras ec, int64_t n, RasterInputs in) {
+    constexpr int kRow = 49;                       // padded SH row (as preprocess_backward_kernel)
+    constexpr int kCamWords = (int)(sizeof(CameraDev) / 4);
+    extern __shared__ float sh_smem[];             // [warps][32 * kRow]
+    __shared__ CameraDev cams[kMaxExtraCameras];
+    pdl_wait();         // the cameras (pack_camera) and camera 0's stored tensors
+    pdl_trigger();
+    for (int i = threadIdx.x; i < ec.count * kCamWords; i += blockDim.x) {
+        const int c = i / kCamWords, w = i - c * kCamWords;
+        reinterpret_cast<uint32_t*>(&cams[c])[w] = reinterpret_cast<const uint32_t*>(ec.cam[c])[w];
+    }
+    __syncthreads();
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    float* ld = sh_smem + (size_t)warp * 32 * kRow;
+    const int64_t g0 = (int64_t)blockIdx.x * blockDim.x + warp * 32;
+    const int cnt = (int)(n - g0 < 32 ? (n - g0 > 0 ? n - g0 : 0) : 32);
+    if (cnt == 0) return;                          // whole warp
+    for (int idx = lane; idx < cnt * 48; idx += 32) {
+        const int i = idx / 48, e = idx - i * 48;
+        float v;
+        if (in.shs) v = __ldg(in.shs + g0 * 48 + idx);
+        else v = e < 3 ? __ldg(in.sh_dc + (g0 + i) * 3 + e) : __ldg(in.sh_rest + (g0 + i) * 45 + (e - 3));
+        ld[i * kRow + e] = v;
+    }
+    __syncwarp();
+    if (lane >= cnt) return;
+    const int64_t gi = g0 + lane;
+    const Vec3 p{in.means3D[3 * gi], in.means3D[3 * gi + 1], in.means3D[3 * gi + 2]};
+    const Vec3 sc{in.scales[3 * gi], in.scales[3 * gi + 1], in.scales[3 * gi + 2]};
+    const float4 q4 = *reinterpret_cast<const float4*>(in.rotations + 4 * gi);
+    const float op = in.opacities[gi];
+    const float* row = ld + lane * kRow;
+    for (int c = 0; c < ec.count; ++c) {
+        const CameraDev& cam = cams[c];
+        Projected pr;
+        const bool ok = project_gaussian(cam, p, sc, Quat{q4.x, q4.y, q4.z, q4.w}, pr);
+        float rgb[3] = {0.f, 0.f, 0.f};
+        uint32_t bits = 0;
+        if (ok) sh_to_rgb(cam, p, [&](int k, int ch) { return row[3 * k + ch]; }, rgb, bits);
+        store_projected(ec.g[c], gi, ok, pr, op, rgb, bits, ec.out_radii[c]);
+    }
+}
+
+cudaError_t launch_project_cameras(const ExtraCameras& ec, int64_t n, const RasterInputs& in, cudaStream_t st) {
+    if (n == 0 || ec.count == 0) return cudaSuccess;
+    constexpr int kThreads = 256;
+    const size_t smem = (size_t)(kThreads / 32) * 32 * 49 * sizeof(float);   // 49 KB: SH staging
+    cudaError_t e = cudaFuncSetAttribute(project_cameras_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    return launch_k(project_cameras_kernel, dim3((unsigned)((n + kThreads - 1) / kThreads)), dim3(kThreads), smem, st, true, ec, n, in);
+}
+
+// ------------------------------------------------------------------------------------------------------
 // Persistent kernel: one CTA per SM, each looping over tiles of TG Gaussians.
 //   MODE 0: deformation network only (drop-in for deform_network.forward; outputs pre-activation tensors)
 //   MODE 1: fused deformation + activations + projection (the render() hot path)

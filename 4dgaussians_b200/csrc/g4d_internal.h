@@ -195,6 +195,34 @@ size_t deform_backward_scratch_bytes(const DeformDesc& d, int64_t n);   // size 
 cudaError_t launch_deform_backward(const DeformDesc& d, const G4DDeformParams& prm, const G4DDeformGrads& grads, float time,
                                    int64_t n, const float* xyz, const float* const go[G4D_NUM_HEADS],
                                    float* const gi[G4D_NUM_HEADS], float* scratch, int sm_count, cudaStream_t st);
+// ---- several cameras at one timestamp (g4d_render_forward_cameras / _backward_cameras) -----------------------------
+constexpr int kMaxExtraCameras = G4D_MAX_CAMERAS - 1;
+// cameras 1..k-1 of a multi-camera forward: camera c reads cam[c] and writes its own context's records g[c] and out_radii[c]
+struct ExtraCameras {
+    int count;
+    const CameraDev* cam[kMaxExtraCameras];
+    GeomBuffers g[kMaxExtraCameras];
+    int32_t* out_radii[kMaxExtraCameras];
+};
+// one thread per Gaussian: the deformed, activated tensors `in` (camera 0's FusedOutputs) are read once and projected into
+// every extra camera (g4d_geom.cu; launched dependent on its predecessor, DESIGN.md §4.6)
+cudaError_t launch_project_cameras(const ExtraCameras& ec, int64_t n, const RasterInputs& in, cudaStream_t st);
+
+// cameras of a multi-camera backward that are part of the loss
+struct BackwardCameras {
+    int count;
+    const CameraDev* cam[G4D_MAX_CAMERAS];
+    const int32_t* radii[G4D_MAX_CAMERAS];
+    const uint8_t* clamped[G4D_MAX_CAMERAS];
+    const float* grad[G4D_MAX_CAMERAS];    // the camera's blend backward: d(mean2D) [2N], d(conic) [3N], d(rgb) [3N], d(opacity) [N]
+    float* g_means2D[G4D_MAX_CAMERAS];     // [N,3] screen-space gradient of the camera, or NULL
+};
+// per-Gaussian backward of all those cameras in one pass: the gradients w.r.t. means3D, scales, rotations, opacity and the
+// SH coefficients are summed over the cameras and written once (OVERWRITTEN); SH sinks as launch_preprocess_backward
+cudaError_t launch_preprocess_backward_cameras(const BackwardCameras& bc, int64_t n, const RasterInputs& in, float* g_means3D,
+                                               float* g_scales, float* g_rotations, float* g_opacities, float* g_shs,
+                                               float* g_sh_dc, float* g_sh_rest, cudaStream_t st);
+
 // coarse stage of render(): activations + projection without the deformation network
 cudaError_t launch_activate_preprocess(const CameraDev* cam, int64_t n, const float* xyz, const float* scaling,
                                        const float* rotation, const float* opacity, const float* shs, const float* sh_dc,

@@ -170,6 +170,24 @@ int g4d_render_forward(G4DContext *ctx, const G4DCamera *cam, const G4DDeformPar
 int g4d_render_backward(G4DContext *ctx, const G4DCamera *cam, const G4DDeformParams *prm, G4DDeformGrads *pgrads,
                         const G4DGaussians *g, const float *dL_dcolor, G4DGaussianGrads *ggrads, void *stream);
 
+/* ---- one timestamp seen by several cameras (a camera rig at frame t) ------------------------------
+ * k cameras, 1 <= k <= G4D_MAX_CAMERAS, on k pairwise distinct contexts of one workspace.  Every cams[i].time must be
+ * bitwise equal to cams[0].time (else G4D_ERR_ARG before any launch); image sizes may differ.  The deformation network
+ * runs ONCE: camera 0 runs the g4d_render_forward sequence on ctx[0] (k == 1 is g4d_render_forward), cameras 1..k-1 are
+ * projected from ctx[0]'s deformed, activated tensors and binned / blended on their own contexts.  out_color[i] [3,H_i,W_i],
+ * out_depth[i] [1,H_i,W_i], out_radii[i] [N].  G4D_CAM_NO_GRAD on cams[0] skips the state only the backward reads.
+ * The backward takes the same k contexts: dL_dcolor[i] == NULL leaves camera i out of the loss; gg receives the per-Gaussian
+ * gradients summed over the cameras (OVERWRITTEN; gg->means2D must be NULL), g_means2D[i] ([N,3], may be NULL) camera i's
+ * screen-space gradient; the network's backward runs once, ACCUMULATED into pgrads.  It returns G4D_ERR_STATE when any of
+ * the contexts ran another forward since; g4d_render_backward / g4d_rasterize_backward refuse a member context. */
+#define G4D_MAX_CAMERAS 32
+int g4d_render_forward_cameras(G4DContext *const *ctx, int32_t k, const G4DCamera *cams, const G4DDeformParams *prm,
+                               const G4DGaussians *g, float *const *out_color, float *const *out_depth,
+                               int32_t *const *out_radii, void *stream);
+int g4d_render_backward_cameras(G4DContext *const *ctx, int32_t k, const G4DCamera *cams, const G4DDeformParams *prm,
+                                G4DDeformGrads *pgrads, const G4DGaussians *g, const float *const *dL_dcolor,
+                                G4DGaussianGrads *gg, float *const *g_means2D, void *stream);
+
 /* ---- losses either side of the path (SURVEY.md 8f N2) -----------------------------------------------
  * Every `*_accum` is a DEVICE float that is ADDED to (caller zeroes); `upstream` is a DEVICE float holding dL/d(loss
  * term) (what autograd hands the backward of a scalar), NULL = 1.
