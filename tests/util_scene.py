@@ -104,6 +104,31 @@ def rel_err(got, ref, floor=1e-3):
     return float(np.abs(got - ref).max() / max(floor, np.abs(ref).max()))
 
 
+def row_errors(got, ref, floor=1e-4):
+    """[rows] e_i = max_k |got_ik - ref_ik| / max(max_k |ref_ik|, floor * max|ref|), rows = the leading axis."""
+    ref = np.asarray(ref, dtype=np.float64)
+    rows = ref.shape[0]
+    r = ref.reshape(rows, -1)
+    g = np.asarray(got, dtype=np.float64).reshape(rows, -1)
+    d = np.abs(g - r).max(axis=1, initial=0.0)
+    scale = np.maximum(np.abs(r).max(axis=1, initial=0.0), floor * np.abs(r).max(initial=0.0))
+    e = np.where(d > 0, np.inf, 0.0)            # a row of an all-zero reference must be exactly zero
+    np.divide(d, scale, out=e, where=scale > 0)
+    return e
+
+
+def row_err(got, ref, floor=1e-4):
+    """Per-row relative error: (max_i e_i, the worst five rows as (index, got row, ref row)), e_i as in row_errors.  Every row
+    is measured against its own magnitude (down to floor x the tensor's max), so a row that is wrong by 100 % fails even when
+    it is tiny next to the largest row -- strictly stronger than rel_err at the same tolerance."""
+    e = row_errors(got, ref, floor)
+    rows = e.shape[0]
+    g = np.asarray(got, dtype=np.float64).reshape(rows, -1)
+    r = np.asarray(ref, dtype=np.float64).reshape(rows, -1)
+    worst = np.argsort(-e, kind="stable")[:5]
+    return (float(e.max()) if rows else 0.0), [(int(i), g[i].tolist(), r[i].tolist()) for i in worst]
+
+
 def rel_err_bulk(got, ref, floor=1e-3, q=99.9):
     """(q-th percentile, max) of |got - ref| relative to max|ref|.  For gradients that pass through ReLU / floor()
     decisions: an input sitting within fp32 rounding of a kink may legitimately land on the other side on the GPU."""
@@ -147,3 +172,122 @@ def kink_rows(cfg, prm, xyz, t, delta_act=2e-6, delta_grid=2e-4):
             z = a @ w1.detach().double().t() + b1.detach().double()
             mask |= (z.abs() < delta_act).any(dim=1)
     return mask
+
+
+# ---------------------------------------------------------------------------------------------------
+# decomposed fp64 oracle of the fused backward: raster oracle on the GPU's own deformed tensors, then an fp64 chain
+# ---------------------------------------------------------------------------------------------------
+SCENE_LEAVES = ("xyz", "scaling", "rotation", "opacity", "features_dc", "features_rest")
+
+
+def params_fp64(prm):
+    """fp64 copies of the oracle parameters as fresh leaves that collect gradients."""
+    p = prm.to(torch.float64)
+    p.aabb = p.aabb.detach()
+    p.planes = [[q.detach().requires_grad_(True) for q in lvl] for lvl in p.planes]
+    p.w0, p.b0 = p.w0.detach().requires_grad_(True), p.b0.detach().requires_grad_(True)
+    p.heads = {k: tuple(q.detach().requires_grad_(True) for q in v) for k, v in p.heads.items()}
+    return p
+
+
+def _deform_activate(cfg, prm, leaves, t):
+    shs = torch.cat([leaves["features_dc"], leaves["features_rest"]], dim=1)
+    from oracle import deform_ref as dr
+    pts, sc, rot, op, sh = dr.deform_forward(cfg, prm, leaves["xyz"], leaves["scaling"], leaves["rotation"], leaves["opacity"],
+                                             shs, float(t))
+    s, r, o = dr.activate(sc, rot, op)
+    return pts, s, r, o, sh
+
+
+def deformed_fp64(cfg, prm, scene, t, chunk=65536):
+    """(means3D [N,3], shs [N,16,3]) of the fine stage in fp64, without gradients."""
+    p64 = prm.to(torch.float64)
+    n = scene["xyz"].shape[0]
+    pts, shs = [], []
+    with torch.no_grad():
+        for a in range(0, n, chunk):
+            lv = {k: scene[k][a:a + chunk].detach().double() for k in SCENE_LEAVES}
+            p, _, _, _, sh = _deform_activate(cfg, p64, lv, t)
+            pts.append(p); shs.append(sh)
+    return torch.cat(pts), torch.cat(shs)
+
+
+def colour_kink_rows(means3D, shs, cameras, sh_degree, delta=1e-5):
+    """[N] bool: Gaussians in front of one of the cameras (view depth > 0.2, the projection's cull) with an SH colour channel
+    within delta of the clamp max(colour + 0.5, 0).  Inputs in fp64.  The fused kernels evaluate the SH polynomial in
+    another association order than the oracle, so on such a row the clamp decision (and with it the colour gradient) may
+    legitimately differ."""
+    from oracle.dense_ref import _sh_color
+    x = means3D.double()
+    mask = torch.zeros(x.shape[0], dtype=torch.bool)
+    for cam in cameras:
+        v = cam.world_view_transform.double().reshape(16)
+        tz = v[2] * x[:, 0] + v[6] * x[:, 1] + v[10] * x[:, 2] + v[14]
+        d = x - cam.camera_center.double()
+        c = _sh_color(sh_degree, shs.double(), d / d.norm(dim=-1, keepdim=True)) + 0.5
+        mask |= (tz > 0.2) & (c.abs() < delta).any(dim=1)
+    return mask
+
+
+def raster_oracle_inputs(deformed, shs):
+    """The raster oracle's (means3D, scales, rots, opacities, shs) from the post-activation tensors deformed [N,11]
+    (means3D | scales | rots | opacity, the layout of the context's "deformed" buffer) and shs [N,16,3]."""
+    d = np.asarray(deformed, np.float32)
+    return (np.ascontiguousarray(d[:, 0:3]), np.ascontiguousarray(d[:, 3:6]), np.ascontiguousarray(d[:, 6:10]),
+            np.ascontiguousarray(d[:, 10:11]), np.ascontiguousarray(np.asarray(shs, np.float32).reshape(-1, 16, 3)))
+
+
+def threshold_pixels(fwd, W, H, d_alpha=2e-5, d_T=2e-3, d_power=1e-6):
+    """[H,W] bool: pixels where an instance before the pixel's stop (list position < n_contrib) sits within rounding of a
+    discrete decision of the compositing loop (A.3): alpha = 1/255, the clamp alpha = 0.99, T = 1e-4 or power = 0.  This is
+    the predicate (same margins) of test_gpu_fullsize._assert_pixel_outliers_are_threshold_flips, evaluated in fp64 from the
+    oracle's projected records for every pixel.  The blend kernels' ex2-based exponential and libm expf differ in the last
+    ulp, so either side may take the other branch there; when the instance is not the pixel's last contributor and T is
+    small the image moves by less than 1e-4, but that instance's gradient from the pixel appears on one side only."""
+    pr, bn = fwd["proj"], fwd["bin"]
+    gx, gy = (W + 15) // 16, (H + 15) // 16
+    xy = pr.xy.astype(np.float64); co = pr.conic_op.astype(np.float64)
+    nc = fwd["n_contrib"].reshape(H, W)
+    ly, lx = np.divmod(np.arange(256), 16)
+    out = np.zeros((H, W), dtype=bool)
+    for tile in range(gx * gy):
+        ty, tx = divmod(tile, gx)
+        px, py = tx * 16 + lx, ty * 16 + ly
+        inside = (px < W) & (py < H)
+        px, py = px[inside], py[inside]
+        last = nc[py, px].astype(np.int64)
+        m = int(last.max())
+        if m == 0:
+            continue
+        lo = int(bn.ranges[tile][0])
+        ids = bn.ids[lo:lo + m].astype(np.int64)
+        dx = xy[ids, 0][:, None] - px[None, :]
+        dy = xy[ids, 1][:, None] - py[None, :]
+        power = -0.5 * (co[ids, 0][:, None] * dx * dx + co[ids, 2][:, None] * dy * dy) - co[ids, 1][:, None] * dx * dy
+        a = co[ids, 3][:, None] * np.exp(np.minimum(power, 0.0))
+        alpha = np.minimum(0.99, a)
+        T = np.cumprod(np.where((power <= 0) & (alpha >= 1.0 / 255.0), 1.0 - alpha, 1.0), axis=0)
+        near = (np.abs(a * 255.0 - 1.0) < d_alpha) | (np.abs(a - 0.99) < d_alpha) | (np.abs(T / 1e-4 - 1.0) < d_T) | \
+               (np.abs(power) < d_power)
+        near &= np.arange(m)[:, None] < last[None, :]
+        out[py, px] = near.any(axis=0)
+    return out
+
+
+def oracle_chain_backward(cfg, prm, scene, t, cot, chunk=65536):
+    """fp64 chain of the fine stage: gradients of sum <cot, activate(deform(scene))> for the six Gaussian leaves and for every
+    network parameter.  cot: post-activation cotangents as returned by rr.rasterize_backward (means3D, scales, rots,
+    opacities, shs; summed over cameras for a multi-camera loss).  Rows are independent, so the chain runs in chunks of
+    Gaussians; the parameter gradients add up across chunks.  Returns ({leaf: fp64 ndarray}, fp64 DeformParams with .grad)."""
+    p64 = params_fp64(prm)
+    n = scene["xyz"].shape[0]
+    grads = {k: np.zeros(tuple(scene[k].shape), np.float64) for k in SCENE_LEAVES}
+    names = ("means3D", "scales", "rots", "opacities", "shs")
+    for a in range(0, n, chunk):
+        lv = {k: scene[k][a:a + chunk].detach().double().requires_grad_(True) for k in SCENE_LEAVES}
+        outs = _deform_activate(cfg, p64, lv, t)
+        cts = [torch.from_numpy(np.asarray(cot[nm][a:a + chunk], np.float64)).reshape(o.shape) for nm, o in zip(names, outs)]
+        torch.autograd.backward(list(outs), cts)
+        for k in SCENE_LEAVES:
+            grads[k][a:a + chunk] = lv[k].grad.numpy()
+    return grads, p64
