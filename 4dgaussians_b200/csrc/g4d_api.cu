@@ -294,20 +294,20 @@ struct DeformSetup {
 };
 
 // the time planes interpolated at `time`, into `rows` (pointers in trow)
-int collapse_time_rows(DevBuf& rows, float* (*trow)[3], const G4DDeformParams* p, const CameraDev* cam, float time, cudaStream_t st) {
+int collapse_time_rows(DevBuf& rows, float* (*trow)[3], const G4DDeformParams* p, float time, cudaStream_t st) {
     const TimeRows tr(p->levels, p->res, p->channels);
     if (rows.ensure(tr.total() * 4) != cudaSuccess) return fail(G4D_ERR_NOMEM, "time-row buffer");
     tr.place(rows.as<float>(), trow);
-    G4D_CUDA(launch_collapse_time_rows(*p, cam, time, trow, st));
+    G4D_CUDA(launch_collapse_time_rows(*p, time, trow, st));
     return G4D_OK;
 }
 
 // Collapse the time rows, pick the forward's path from the params and bring the weight images that path reads up to date.
 // The desc is built after that refresh, which may move the transposes it embeds.
-int setup_deform(G4DWorkspace* ws, const G4DDeformParams* p, DevBuf& rows, float* (*trow)[3], const CameraDev* cam, float time,
-                 cudaStream_t st, DeformSetup* out) {
+int setup_deform(G4DWorkspace* ws, const G4DDeformParams* p, DevBuf& rows, float* (*trow)[3], float time, cudaStream_t st,
+                 DeformSetup* out) {
     int rc;
-    if ((rc = collapse_time_rows(rows, trow, p, cam, time, st)) != G4D_OK) return rc;
+    if ((rc = collapse_time_rows(rows, trow, p, time, st)) != G4D_OK) return rc;
     out->tc = ws->tensor_cores != 0 && tc_deform_supported(*p, ws->tensor_cores);
     if (!out->tc) {
         if ((rc = refresh_packed(ws, p, st)) != G4D_OK) return rc;
@@ -470,10 +470,16 @@ int bin_and_blend(G4DContext* c, const G4DCamera* cam, int64_t n, float* out_col
     return G4D_OK;
 }
 
+// A caller's SH tensors: fused [N,16,3] in dc, or (split) dc [N,1,3] + rest [N,15,3].  Sh = ShIn for the coefficients,
+// ShOut for their gradient sinks.
+template <class Sh, class T> Sh caller_sh(bool split, T* dc, T* rest = nullptr) {
+    return split ? Sh{nullptr, dc, rest} : Sh{dc, nullptr, nullptr};
+}
+
 // blend backward + per-Gaussian backward on `in`; opacity gradient lands in g_opacities (zeroed here)
 int raster_backward_stages(G4DContext* c, const G4DCamera* cam, int64_t n, const RasterInputs& in, const float* dL_dcolor,
-                           float* g_means3D, float* g_means2D, float* g_shs, float* g_sh_dc, float* g_sh_rest,
-                           float* g_opacities, float* g_scales, float* g_rotations, cudaStream_t st) {
+                           float* g_means3D, float* g_means2D, const ShOut& g_sh, float* g_opacities, float* g_scales,
+                           float* g_rotations, cudaStream_t st) {
     const CameraDev* dcam = c->cam.as<CameraDev>();
     const size_t N = (size_t)(n > 0 ? n : 1);
     G4D_CUDA(c->gscratch.ensure(N * 8 * 4 + 256));
@@ -493,7 +499,7 @@ int raster_backward_stages(G4DContext* c, const G4DCamera* cam, int64_t n, const
     if ((rc = debug_sync(cam, st, "blend_backward")) != G4D_OK) return rc;
     StageTimer tm(c, G4D_STAGE_GEOM_BWD, st);
     G4D_CUDA(launch_preprocess_backward(dcam, n, in, c->g, g_mean2D, g_conic, g_rgb, g_means3D, g_means2D, g_scales,
-                                        g_rotations, g_shs, g_sh_dc, g_sh_rest, st));
+                                        g_rotations, g_sh, st));
     return debug_sync(cam, st, "preprocess_backward");
 }
 
@@ -607,11 +613,11 @@ int g4d_deform_forward(G4DWorkspace* ws, const G4DDeformParams* prm, int64_t n, 
     G4D_CUDA(cudaSetDevice(ws->device));
     float* trow[G4D_MAX_LEVELS][3] = {};
     DeformSetup s{};
-    if ((rc = setup_deform(ws, prm, ws->trow, trow, nullptr, time, st, &s)) != G4D_OK) return rc;
+    if ((rc = setup_deform(ws, prm, ws->trow, trow, time, st, &s)) != G4D_OK) return rc;
     if ((rc = attach_forward_buffers(ws, s, nullptr, relu_bits, n, st)) != G4D_OK) return rc;
-    const DeformIO io{xyz, scaling, rotation, opacity, shs, nullptr, nullptr, out_xyz, out_scaling, out_rotation, out_opacity,
+    const DeformIO io{xyz, scaling, rotation, opacity, caller_sh<ShIn>(false, shs), out_xyz, out_scaling, out_rotation, out_opacity,
                       out_shs, GeomBuffers{}, FusedOutputs{}, nullptr};
-    G4D_CUDA(launch_deform(s.d, 0, nullptr, time, n, io, ws->sm_count, st, s.tc ? &s.tw : nullptr));
+    G4D_CUDA(launch_deform(s.d, 0, nullptr, n, io, ws->sm_count, st, s.tc ? &s.tw : nullptr));
     return G4D_OK;
 }
 
@@ -637,7 +643,7 @@ int g4d_rasterize_forward(G4DContext* c, const G4DCamera* cam, int64_t n, const 
         StageTimer tm(c, G4D_STAGE_PREP, st);
         G4D_CUDA(launch_pack_camera(*cam, c->cam.as<CameraDev>(), st));
     }
-    RasterInputs in{means3D, scales, rotations, opacities, shs, nullptr, nullptr};
+    const RasterInputs in{means3D, scales, rotations, opacities, caller_sh<ShIn>(false, shs)};
     {
         StageTimer tm(c, G4D_STAGE_GEOM, st);
         G4D_CUDA(launch_preprocess(c->cam.as<CameraDev>(), n, in, c->g, out_radii, st));
@@ -660,9 +666,9 @@ int g4d_rasterize_backward(G4DContext* c, const G4DCamera* cam, int64_t n, const
     G4D_CUDA(cudaSetDevice(c->ws->device));
     if ((rc = check_pending(c)) != G4D_OK) return rc;
     (void)opacities;
-    RasterInputs in{means3D, scales, rotations, opacities, shs, nullptr, nullptr};
-    return raster_backward_stages(c, cam, n, in, dL_dcolor, g_means3D, g_means2D, g_shs, nullptr, nullptr, g_opacities,
-                                  g_scales, g_rotations, st);
+    const RasterInputs in{means3D, scales, rotations, opacities, caller_sh<ShIn>(false, shs)};
+    return raster_backward_stages(c, cam, n, in, dL_dcolor, g_means3D, g_means2D, caller_sh<ShOut>(false, g_shs),
+                                  g_opacities, g_scales, g_rotations, st);
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -771,7 +777,7 @@ int g4d_deform_backward(G4DWorkspace* ws, const G4DDeformParams* prm, G4DDeformG
     cudaStream_t st = (cudaStream_t)stream;
     G4D_CUDA(cudaSetDevice(ws->device));
     float* trow[G4D_MAX_LEVELS][3] = {};
-    if ((rc = collapse_time_rows(ws->trow, trow, prm, nullptr, time, st)) != G4D_OK) return rc;
+    if ((rc = collapse_time_rows(ws->trow, trow, prm, time, st)) != G4D_OK) return rc;
     const float* go[G4D_NUM_HEADS] = {g_out_xyz, g_out_scaling, g_out_rotation, g_out_opacity, g_out_shs};
     float* gi[G4D_NUM_HEADS] = {g_in_xyz, g_in_scaling, g_in_rotation, g_in_opacity, g_in_shs};
     return deform_backward_dispatch(ws, prm, trow, grads, time, n, xyz, go, gi, relu_bits, nullptr, st);
@@ -809,8 +815,6 @@ int fused_forward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* pr
     if ((rc = ensure_fused(c, n, with_sh)) != G4D_OK) return rc;
     CameraDev* dcam = c->cam.as<CameraDev>();
     reset_stage_flags(c, 0, G4D_STAGE_COUNT - 1);
-    const float* shs = g->features_rest ? nullptr : g->features_dc;
-    const float* dc = g->features_rest ? g->features_dc : nullptr;
     // a no-grad render needs none of the saved tensors: skip their stores (48 B + 192 B of deformed SH per Gaussian)
     c->fo_valid = !(cam->debug & G4D_CAM_NO_GRAD) || ws->keep_deformed || keep_fo;
     const FusedOutputs fo_arg = c->fo_valid ? c->fo : FusedOutputs{};
@@ -818,10 +822,13 @@ int fused_forward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* pr
     {
         StageTimer tm(c, G4D_STAGE_PREP, st);
         G4D_CUDA(launch_pack_camera(*cam, dcam, st));
-        if (prm && (rc = setup_deform(ws, prm, c->trow, c->trow_ptr, dcam, cam->time, st, &s)) != G4D_OK) return rc;
+        if (prm && (rc = setup_deform(ws, prm, c->trow, c->trow_ptr, cam->time, st, &s)) != G4D_OK) return rc;
     }
     {
         StageTimer tm(c, G4D_STAGE_GEOM, st);
+        const DeformIO io{g->xyz, g->scaling, g->rotation, g->opacity,
+                          caller_sh<ShIn>(g->features_rest != nullptr, g->features_dc, g->features_rest),
+                          nullptr, nullptr, nullptr, nullptr, nullptr, c->g, fo_arg, out_radii};
         if (prm) {
             c->relu_saved = s.tc && !(cam->debug & G4D_CAM_NO_GRAD);
             if (c->relu_saved) {   // a backward will follow: it re-uses the ReLU signs and the staged HexPlane features
@@ -830,12 +837,9 @@ int fused_forward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* pr
             }
             if ((rc = attach_forward_buffers(ws, s, c->relu_saved ? c->feat.as<float>() : nullptr,
                                              c->relu_saved ? c->relu.as<uint32_t>() : nullptr, n, st)) != G4D_OK) return rc;
-            const DeformIO io{g->xyz, g->scaling, g->rotation, g->opacity, shs, dc, g->features_rest,
-                              nullptr, nullptr, nullptr, nullptr, nullptr, c->g, fo_arg, out_radii};
-            G4D_CUDA(launch_deform(s.d, 1, dcam, cam->time, n, io, ws->sm_count, st, s.tc ? &s.tw : nullptr));
+            G4D_CUDA(launch_deform(s.d, 1, dcam, n, io, ws->sm_count, st, s.tc ? &s.tw : nullptr));
         } else {
-            G4D_CUDA(launch_activate_preprocess(dcam, n, g->xyz, g->scaling, g->rotation, g->opacity, shs, dc, g->features_rest,
-                                                c->g, fo_arg, out_radii, st));
+            G4D_CUDA(launch_activate_preprocess(dcam, n, io, st));
         }
     }
     if ((rc = debug_sync(cam, st, "deform+preprocess")) != G4D_OK) return rc;
@@ -848,10 +852,10 @@ int fused_forward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* pr
 // the post-activation inputs of the rasterizer stages of a fused forward on c: its stored deformed tensors, and the SH
 // coefficients (deformed when the SHS head is active, the caller's otherwise)
 RasterInputs deformed_inputs(const G4DContext* c, const G4DGaussians* g) {
-    const bool split = g->features_rest != nullptr;
-    return RasterInputs{c->fo.means3D, c->fo.scales, c->fo.rotations, c->fo.opacities,
-                        c->fused_sh ? c->fo.shs : (split ? nullptr : g->features_dc), split ? g->features_dc : nullptr,
-                        g->features_rest};
+    RasterInputs in{c->fo.means3D, c->fo.scales, c->fo.rotations, c->fo.opacities,
+                    caller_sh<ShIn>(g->features_rest != nullptr, g->features_dc, g->features_rest)};
+    if (c->fused_sh) in.sh = ShIn{c->fo.shs, nullptr, nullptr};
+    return in;
 }
 
 // gradients w.r.t. the deformed tensors of a fine-stage backward: scratch on c (the network's backward reads them)
@@ -868,6 +872,20 @@ int deformed_grads(G4DContext* c, int64_t n, DeformedGrads* out) {
     return G4D_OK;
 }
 
+// The SH gradient sinks of the backward of a fused forward on c: the caller's.  With the SHS head active the gradient also
+// feeds the network's backward: the fused sink is then the scratch d_sh, which copy_fused_sh_grad passes on to a caller sink
+// in the fused layout.
+ShOut fused_sh_sinks(const G4DContext* c, const G4DGaussians* g, const G4DGaussianGrads* gg, float* d_sh) {
+    ShOut o = caller_sh<ShOut>(g->features_rest != nullptr, gg->features_dc, gg->features_rest);
+    if (c->fused_sh) o.shs = d_sh;
+    return o;
+}
+int copy_fused_sh_grad(const G4DContext* c, const G4DGaussians* g, const G4DGaussianGrads* gg, const float* d_sh, cudaStream_t st) {
+    if (c->fused_sh && !g->features_rest)
+        G4D_CUDA(cudaMemcpyAsync(gg->features_dc, d_sh, (size_t)g->n * 192, cudaMemcpyDeviceToDevice, st));
+    return G4D_OK;
+}
+
 // The backward of a fused forward of one camera on c (arguments checked by the caller).  gg->means2D may be NULL.
 int fused_backward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* prm, G4DDeformGrads* pgrads, const G4DGaussians* g,
                    const float* dL_dcolor, const G4DGaussianGrads* gg, cudaStream_t st) {
@@ -877,14 +895,9 @@ int fused_backward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* p
     G4D_CUDA(cudaSetDevice(ws->device));
     if ((rc = check_pending(c)) != G4D_OK) return rc;
     if (n == 0) return G4D_OK;
-    const size_t N = (size_t)n;
-    const bool split = g->features_rest != nullptr;
     const RasterInputs in = deformed_inputs(c, g);
-    float* sh_fused_sink = split ? nullptr : gg->features_dc;
-    float* sh_dc_sink = split ? gg->features_dc : nullptr;
-    float* sh_rest_sink = split ? gg->features_rest : nullptr;
     if (!c->deformed) {
-        rc = raster_backward_stages(c, cam, n, in, dL_dcolor, gg->xyz, gg->means2D, sh_fused_sink, sh_dc_sink, sh_rest_sink,
+        rc = raster_backward_stages(c, cam, n, in, dL_dcolor, gg->xyz, gg->means2D, fused_sh_sinks(c, g, gg, nullptr),
                                     gg->opacity, gg->scaling, gg->rotation, st);
         if (rc != G4D_OK) return rc;
         G4D_CUDA(launch_activation_backward(n, c->fo, gg->scaling, gg->rotation, gg->opacity, st));
@@ -895,10 +908,10 @@ int fused_backward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* p
     if ((rc = deformed_grads(c, n, &d)) != G4D_OK) return rc;
     // SH gradient: identity residual path -> written straight into the caller's sinks; the fused copy (when the SHS
     // head is active) additionally feeds the network's backward
-    rc = raster_backward_stages(c, cam, n, in, dL_dcolor, d.xyz, gg->means2D, c->fused_sh ? d.sh : sh_fused_sink, sh_dc_sink,
-                                sh_rest_sink, d.op, d.sc, d.rot, st);
+    rc = raster_backward_stages(c, cam, n, in, dL_dcolor, d.xyz, gg->means2D, fused_sh_sinks(c, g, gg, d.sh), d.op, d.sc, d.rot,
+                                st);
     if (rc != G4D_OK) return rc;
-    if (c->fused_sh && !split) G4D_CUDA(cudaMemcpyAsync(gg->features_dc, d.sh, N * 192, cudaMemcpyDeviceToDevice, st));
+    if ((rc = copy_fused_sh_grad(c, g, gg, d.sh, st)) != G4D_OK) return rc;
     G4D_CUDA(launch_activation_backward(n, c->fo, d.sc, d.rot, d.op, st));
     const float* go[G4D_NUM_HEADS] = {d.xyz, d.sc, d.rot, d.op, d.sh};
     float* gi[G4D_NUM_HEADS] = {gg->xyz, gg->scaling, gg->rotation, gg->opacity, nullptr};
@@ -1050,10 +1063,6 @@ int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCame
     }
     if (n == 0) return G4D_OK;
     const size_t N = (size_t)n;
-    const bool split = g->features_rest != nullptr;
-    float* sh_fused_sink = split ? nullptr : gg->features_dc;
-    float* sh_dc_sink = split ? gg->features_dc : nullptr;
-    float* sh_rest_sink = split ? gg->features_rest : nullptr;
     DeformedGrads d{gg->xyz, gg->scaling, gg->rotation, gg->opacity, nullptr};   // coarse: straight into the caller's sinks
     if (c0->deformed && (rc = deformed_grads(c0, n, &d)) != G4D_OK) return rc;
     // blend backward of every camera in the loss, each into its own scratch: d(mean2D), d(conic), d(rgb), d(opacity)
@@ -1081,10 +1090,10 @@ int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCame
     {
         StageTimer tm(c0, G4D_STAGE_GEOM_BWD, st);
         G4D_CUDA(launch_preprocess_backward_cameras(bc, n, deformed_inputs(c0, g), d.xyz, d.sc, d.rot, d.op,
-                                                    c0->fused_sh ? d.sh : sh_fused_sink, sh_dc_sink, sh_rest_sink, st));
+                                                    fused_sh_sinks(c0, g, gg, d.sh), st));
     }
     if ((rc = debug_sync(&cams[0], st, "preprocess_backward_cameras")) != G4D_OK) return rc;
-    if (c0->fused_sh && !split) G4D_CUDA(cudaMemcpyAsync(gg->features_dc, d.sh, N * 192, cudaMemcpyDeviceToDevice, st));
+    if ((rc = copy_fused_sh_grad(c0, g, gg, d.sh, st)) != G4D_OK) return rc;
     G4D_CUDA(launch_activation_backward(n, c0->fo, d.sc, d.rot, d.op, st));
     if (!c0->deformed) return debug_sync(&cams[0], st, "activation_backward");
     // the network's backward, once, on the gradients summed over the cameras

@@ -11,33 +11,24 @@ __global__ void __launch_bounds__(256)
 preprocess_backward_kernel(const CameraDev* __restrict__ camp, int64_t n, RasterInputs in, GeomBuffers g,
                            const float* __restrict__ g_mean2D, const float* __restrict__ g_conic,
                            const float* __restrict__ g_rgb, float* __restrict__ g_means3D, float* __restrict__ g_means2D_out,
-                           float* __restrict__ g_scales, float* __restrict__ g_rotations, float* __restrict__ g_shs,
-                           float* __restrict__ g_sh_dc, float* __restrict__ g_sh_rest) {
+                           float* __restrict__ g_scales, float* __restrict__ g_rotations, ShOut g_sh) {
     // SH coefficients travel through shared memory: a warp reads / writes the 32 x 48 floats of its Gaussians as contiguous
     // 128-byte lines instead of 48 scalar accesses per thread at a 192-byte stride
-    constexpr int kRow = 49;                       // padded row: lane i <-> row i is bank-conflict free (49 odd)
-    extern __shared__ float sh_smem[];             // [warps][2][32 * kRow]
+    extern __shared__ float sh_smem[];             // [warps][2][32 * kShRow]
     __shared__ CameraDev cam;
-    for (int i = threadIdx.x; i < (int)(sizeof(CameraDev) / 4); i += blockDim.x)
-        reinterpret_cast<uint32_t*>(&cam)[i] = reinterpret_cast<const uint32_t*>(camp)[i];
+    stage_cameras(&cam, &camp, 1);
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    float* ld = sh_smem + (size_t)warp * 2 * 32 * kRow;
-    float* st = ld + 32 * kRow;
+    float* ld = sh_smem + (size_t)warp * 2 * 32 * kShRow;
+    float* st = ld + 32 * kShRow;
     const int64_t g0 = (int64_t)blockIdx.x * blockDim.x + warp * 32;
     const int cnt = (int)(n - g0 < 32 ? (n - g0 > 0 ? n - g0 : 0) : 32);
     if (cnt == 0) return;                          // whole warp
     const int64_t gi = g0 + lane;
     const bool active = lane < cnt;
-    for (int idx = lane; idx < cnt * 48; idx += 32) {
-        const int i = idx / 48, e = idx - i * 48;
-        float v;
-        if (in.shs) v = __ldg(in.shs + g0 * 48 + idx);
-        else v = e < 3 ? __ldg(in.sh_dc + (g0 + i) * 3 + e) : __ldg(in.sh_rest + (g0 + i) * 45 + (e - 3));
-        ld[i * kRow + e] = v;
-    }
+    in.sh.stage_warp(g0, cnt, lane, ld);
     __syncwarp();
-    auto sh_store = [&](int k, int ch, float v) { st[lane * kRow + 3 * k + ch] = v; };
+    auto sh_store = [&](int k, int ch, float v) { st[lane * kShRow + 3 * k + ch] = v; };
     if (active) {
         if (g_means2D_out) {
             const bool vis = g.radii[gi] > 0;
@@ -58,7 +49,7 @@ preprocess_backward_kernel(const CameraDev* __restrict__ camp, int64_t n, Raster
             const float gc[3] = {g_conic[3 * gi], g_conic[3 * gi + 1], g_conic[3 * gi + 2]};
             const float gr[3] = {g_rgb[3 * gi], g_rgb[3 * gi + 1], g_rgb[3 * gi + 2]};
             GaussGrad gg;
-            const float* row = ld + lane * kRow;
+            const float* row = ld + lane * kShRow;
             gaussian_backward(cam, p, sc, Quat{q4.x, q4.y, q4.z, q4.w}, (uint32_t)g.clamped[gi], gm2, gc, gr,
                               [&](int k, int ch) { return row[3 * k + ch]; }, sh_store, gg);
             for (int k = 0; k < 3; ++k) { g_means3D[3 * gi + k] = gg.mean[k]; g_scales[3 * gi + k] = gg.scale[k]; }
@@ -66,29 +57,23 @@ preprocess_backward_kernel(const CameraDev* __restrict__ camp, int64_t n, Raster
         }
     }
     __syncwarp();
-    for (int idx = lane; idx < cnt * 48; idx += 32) {
-        const int i = idx / 48, e = idx - i * 48;
-        const float v = st[i * kRow + e];
-        if (g_shs) g_shs[g0 * 48 + idx] = v;
-        if (e < 3) { if (g_sh_dc) g_sh_dc[(g0 + i) * 3 + e] = v; }
-        else if (g_sh_rest) g_sh_rest[(g0 + i) * 45 + (e - 3)] = v;
-    }
+    g_sh.store_warp(g0, cnt, lane, st);
 }
 
 cudaError_t launch_preprocess_backward(const CameraDev* cam, int64_t n, const RasterInputs& in, GeomBuffers g,
                                        const float* g_mean2D, const float* g_conic, const float* g_rgb, float* g_means3D,
-                                       float* g_means2D_out, float* g_scales, float* g_rotations, float* g_shs,
-                                       float* g_sh_dc, float* g_sh_rest, cudaStream_t st) {
+                                       float* g_means2D_out, float* g_scales, float* g_rotations, const ShOut& g_sh,
+                                       cudaStream_t st) {
     if (n == 0) return cudaSuccess;
     constexpr int kThreads = 128;
-    const size_t smem = (size_t)(kThreads / 32) * 2 * 32 * 49 * sizeof(float);   // 50 KB: SH staging (see the kernel)
+    const size_t smem = (size_t)(kThreads / 32) * 2 * 32 * kShRow * sizeof(float);   // 50 KB: SH staging (see the kernel)
     {
         cudaError_t e = cudaFuncSetAttribute(preprocess_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
     }
     preprocess_backward_kernel<<<(unsigned)((n + kThreads - 1) / kThreads), kThreads, smem, st>>>(cam, n, in, g, g_mean2D, g_conic, g_rgb,
                                                                                                   g_means3D, g_means2D_out, g_scales,
-                                                                                                  g_rotations, g_shs, g_sh_dc, g_sh_rest);
+                                                                                                  g_rotations, g_sh);
     return cudaGetLastError();
 }
 
@@ -99,38 +84,27 @@ cudaError_t launch_preprocess_backward(const CameraDev* cam, int64_t n, const Ra
 __global__ void __launch_bounds__(128)
 preprocess_backward_cameras_kernel(BackwardCameras bc, int64_t n, RasterInputs in, float* __restrict__ g_means3D,
                                    float* __restrict__ g_scales, float* __restrict__ g_rotations, float* __restrict__ g_opacities,
-                                   float* __restrict__ g_shs, float* __restrict__ g_sh_dc, float* __restrict__ g_sh_rest) {
-    constexpr int kRow = 49;
-    constexpr int kCamWords = (int)(sizeof(CameraDev) / 4);
-    extern __shared__ float sh_smem[];             // [warps][2][32 * kRow]: SH coefficients, SH gradient sums
+                                   ShOut g_sh) {
+    extern __shared__ float sh_smem[];             // [warps][2][32 * kShRow]: SH coefficients, SH gradient sums
     __shared__ CameraDev cams[G4D_MAX_CAMERAS];
-    for (int i = threadIdx.x; i < bc.count * kCamWords; i += blockDim.x) {
-        const int c = i / kCamWords, w = i - c * kCamWords;
-        reinterpret_cast<uint32_t*>(&cams[c])[w] = reinterpret_cast<const uint32_t*>(bc.cam[c])[w];
-    }
+    stage_cameras(cams, bc.cam, bc.count);
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    float* ld = sh_smem + (size_t)warp * 2 * 32 * kRow;
-    float* st = ld + 32 * kRow;
+    float* ld = sh_smem + (size_t)warp * 2 * 32 * kShRow;
+    float* st = ld + 32 * kShRow;
     const int64_t g0 = (int64_t)blockIdx.x * blockDim.x + warp * 32;
     const int cnt = (int)(n - g0 < 32 ? (n - g0 > 0 ? n - g0 : 0) : 32);
     if (cnt == 0) return;
     const int64_t gi = g0 + lane;
-    for (int idx = lane; idx < cnt * 48; idx += 32) {
-        const int i = idx / 48, e = idx - i * 48;
-        float v;
-        if (in.shs) v = __ldg(in.shs + g0 * 48 + idx);
-        else v = e < 3 ? __ldg(in.sh_dc + (g0 + i) * 3 + e) : __ldg(in.sh_rest + (g0 + i) * 45 + (e - 3));
-        ld[i * kRow + e] = v;
-        st[i * kRow + e] = 0.f;
-    }
+    in.sh.stage_warp(g0, cnt, lane, ld);
+    for (int idx = lane; idx < cnt * 48; idx += 32) st[idx / 48 * kShRow + idx % 48] = 0.f;
     __syncwarp();
     if (lane < cnt) {
         const Vec3 p{in.means3D[3 * gi], in.means3D[3 * gi + 1], in.means3D[3 * gi + 2]};
         const Vec3 sc{in.scales[3 * gi], in.scales[3 * gi + 1], in.scales[3 * gi + 2]};
         const float4 q4 = *reinterpret_cast<const float4*>(in.rotations + 4 * gi);
-        const float* row = ld + lane * kRow;
-        float* srow = st + lane * kRow;
+        const float* row = ld + lane * kShRow;
+        float* srow = st + lane * kShRow;
         float gm[3] = {0.f, 0.f, 0.f}, gs[3] = {0.f, 0.f, 0.f}, gr[4] = {0.f, 0.f, 0.f, 0.f}, gop = 0.f;
         for (int c = 0; c < bc.count; ++c) {
             const float* gb = bc.grad[c];
@@ -157,25 +131,19 @@ preprocess_backward_cameras_kernel(BackwardCameras bc, int64_t n, RasterInputs i
         g_opacities[gi] = gop;
     }
     __syncwarp();
-    for (int idx = lane; idx < cnt * 48; idx += 32) {
-        const int i = idx / 48, e = idx - i * 48;
-        const float v = st[i * kRow + e];
-        if (g_shs) g_shs[g0 * 48 + idx] = v;
-        if (e < 3) { if (g_sh_dc) g_sh_dc[(g0 + i) * 3 + e] = v; }
-        else if (g_sh_rest) g_sh_rest[(g0 + i) * 45 + (e - 3)] = v;
-    }
+    g_sh.store_warp(g0, cnt, lane, st);
 }
 
 cudaError_t launch_preprocess_backward_cameras(const BackwardCameras& bc, int64_t n, const RasterInputs& in, float* g_means3D,
-                                               float* g_scales, float* g_rotations, float* g_opacities, float* g_shs,
-                                               float* g_sh_dc, float* g_sh_rest, cudaStream_t st) {
+                                               float* g_scales, float* g_rotations, float* g_opacities, const ShOut& g_sh,
+                                               cudaStream_t st) {
     if (n == 0) return cudaSuccess;
     constexpr int kThreads = 128;
-    const size_t smem = (size_t)(kThreads / 32) * 2 * 32 * 49 * sizeof(float);   // 50 KB: SH staging and sums
+    const size_t smem = (size_t)(kThreads / 32) * 2 * 32 * kShRow * sizeof(float);   // 50 KB: SH staging and sums
     cudaError_t e = cudaFuncSetAttribute(preprocess_backward_cameras_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     preprocess_backward_cameras_kernel<<<(unsigned)((n + kThreads - 1) / kThreads), kThreads, smem, st>>>(
-        bc, n, in, g_means3D, g_scales, g_rotations, g_opacities, g_shs, g_sh_dc, g_sh_rest);
+        bc, n, in, g_means3D, g_scales, g_rotations, g_opacities, g_sh);
     return cudaGetLastError();
 }
 
@@ -241,7 +209,7 @@ G4D_D void tile_gemm_nt(const float* __restrict__ A, int lda, const float* __res
 // ---- kernel P ------------------------------------------------------------------------------------------
 template <int TG, int WD>
 __global__ void __launch_bounds__(kDeformThreads, 1)
-deform_bwd_prepass_kernel(DeformDesc d, DeformSmem L, float time, int64_t n, const float* __restrict__ xyz,
+deform_bwd_prepass_kernel(DeformDesc d, DeformSmem L, int64_t n, const float* __restrict__ xyz,
                           float* __restrict__ feat_out, float* __restrict__ a1_out) {
     extern __shared__ __align__(16) float smem[];
     constexpr int RM = TG / 16, CG = WD / 64;
@@ -257,7 +225,7 @@ deform_bwd_prepass_kernel(DeformDesc d, DeformSmem L, float time, int64_t n, con
     for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const int64_t base = tile * TG, rem = n - base;
         if (tid < TG) {
-            float4 c = make_float4(0.f, 0.f, 0.f, time);
+            float4 c = make_float4(0.f, 0.f, 0.f, 0.f);   // (w unused: time enters through the collapsed time rows)
             if (tid < rem) {
                 c.x = nrm(0, xyz[(base + tid) * 3 + 0]);
                 c.y = nrm(1, xyz[(base + tid) * 3 + 1]);
@@ -499,7 +467,7 @@ inline FinalSmem final_smem_layout(int TG, int F, int WD) {
 
 template <int TG, int WD, int FM>
 __global__ void __launch_bounds__(kDeformThreads, 1)
-deform_bwd_final_kernel(DeformBwdDesc bd, FinalSmem L, float time, int64_t n, const float* __restrict__ xyz,
+deform_bwd_final_kernel(DeformBwdDesc bd, FinalSmem L, int64_t n, const float* __restrict__ xyz,
                         DeformBwdBuffers buf) {
     extern __shared__ __align__(16) float smem[];
     const DeformDesc& d = bd.d;
@@ -547,7 +515,7 @@ deform_bwd_final_kernel(DeformBwdDesc bd, FinalSmem L, float time, int64_t n, co
             *reinterpret_cast<float4*>(sDH + g * L.ldh + 4 * v) = s;
         }
         if (tid < TG) {
-            float4 c = make_float4(0.f, 0.f, 0.f, time);
+            float4 c = make_float4(0.f, 0.f, 0.f, 0.f);   // (w unused: time enters through the collapsed time rows)
             if (tid < rem) {
                 c.x = nrm(0, xyz[(base + tid) * 3 + 0]);
                 c.y = nrm(1, xyz[(base + tid) * 3 + 1]);
@@ -706,7 +674,7 @@ static cudaError_t launch_deform_backward_t(const DeformBwdDesc& bd, float time,
         e = cudaFuncSetAttribute(deform_bwd_prepass_kernel<TG, WD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
         if (e != cudaSuccess) return e;
         const int grid = (int)(ntiles < sm_count ? ntiles : sm_count);
-        deform_bwd_prepass_kernel<TG, WD><<<grid, kDeformThreads, bytes, st>>>(d, L, time, n, xyz, buf.feat, buf.a1);
+        deform_bwd_prepass_kernel<TG, WD><<<grid, kDeformThreads, bytes, st>>>(d, L, n, xyz, buf.feat, buf.a1);
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
     }
     // H
@@ -730,7 +698,7 @@ static cudaError_t launch_deform_backward_t(const DeformBwdDesc& bd, float time,
         do {                                                                                                              \
             e = cudaFuncSetAttribute(deform_bwd_final_kernel<TG, WD, FM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes); \
             if (e != cudaSuccess) return e;                                                                               \
-            deform_bwd_final_kernel<TG, WD, FM><<<grid, kDeformThreads, bytes, st>>>(bd, L, time, n, xyz, buf);            \
+            deform_bwd_final_kernel<TG, WD, FM><<<grid, kDeformThreads, bytes, st>>>(bd, L, n, xyz, buf);            \
         } while (0)
         if (d.F <= 32) G4D_LAUNCH_Q(32);
         else if (d.F <= 64) G4D_LAUNCH_Q(64);

@@ -226,7 +226,7 @@ __device__ __forceinline__ void bar_sync(int id, int count) { asm volatile("bar.
 
 template <int ARITH, int MODE, int C, int L, bool SAVE>
 __global__ void __launch_bounds__(TcArith<ARITH>::NWG * 128, 1)
-deform_tc_kernel(DeformDesc d, TcWeights tw, TcSmem Ls, const CameraDev* __restrict__ camp, int use_cam, int64_t n, DeformIO io) {
+deform_tc_kernel(DeformDesc d, TcWeights tw, TcSmem Ls, const CameraDev* __restrict__ camp, int64_t n, DeformIO io) {
     using A = TcArith<ARITH>;
     constexpr int F = C * L, NS0 = F / A::KS, NS1 = 128 / A::KS, NSP = NS1 / A::PH, TM = 64 * A::NWG, NT = 128 * A::NWG;
     static_assert(F % 16 == 0 && F <= 64, "feature width must be 32, 48 or 64");
@@ -265,10 +265,7 @@ deform_tc_kernel(DeformDesc d, TcWeights tw, TcSmem Ls, const CameraDev* __restr
     }
     pdl_wait();           // from here on: the camera, the staged features
     pdl_trigger();
-    if (use_cam) {
-        for (int i = tid; i < (int)(sizeof(CameraDev) / 4); i += NT)
-            reinterpret_cast<uint32_t*>(&cam)[i] = reinterpret_cast<const uint32_t*>(camp)[i];
-    }
+    if (MODE == 1) stage_cameras(&cam, &camp, 1);
     __syncthreads();
 
     const bool hsh = d.head_mask & G4D_HEAD_SHS;
@@ -477,7 +474,7 @@ deform_tc_kernel(DeformDesc d, TcWeights tw, TcSmem Ls, const CameraDev* __restr
                         if (io.out_shs && hsh) {
 #pragma unroll
                             for (int j = 0; j < 48; j += 4) {
-                                const float4 b = *reinterpret_cast<const float4*>(io.shs + gi * 48 + j);
+                                const float4 b = *reinterpret_cast<const float4*>(io.sh.shs + gi * 48 + j);
                                 *reinterpret_cast<float4*>(io.out_shs + gi * 48 + j) = make_float4(b.x + dsh[j], b.y + dsh[j + 1], b.z + dsh[j + 2], b.w + dsh[j + 3]);
                             }
                         }
@@ -534,17 +531,17 @@ bool tc_deform_supported(const G4DDeformParams& prm, int arith) {
 
 template <int ARITH, int MODE, int C, int L>
 static cudaError_t launch_deform_tc_t(const DeformDesc& d, const TcWeights& tw, const TcSmem& Ls, size_t bytes, int grid,
-                                      const CameraDev* cam, bool use_cam, int64_t n, const DeformIO& io, cudaStream_t st) {
+                                      const CameraDev* cam, int64_t n, const DeformIO& io, cudaStream_t st) {
     constexpr int threads = TcArith<ARITH>::NWG * 128;
     cudaError_t e;
     if (tw.relu_bits) {
         e = cudaFuncSetAttribute(deform_tc_kernel<ARITH, MODE, C, L, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
         if (e != cudaSuccess) return e;
-        return launch_k(deform_tc_kernel<ARITH, MODE, C, L, true>, dim3(grid), dim3(threads), bytes, st, true, d, tw, Ls, cam, use_cam ? 1 : 0, n, io);
+        return launch_k(deform_tc_kernel<ARITH, MODE, C, L, true>, dim3(grid), dim3(threads), bytes, st, true, d, tw, Ls, cam, n, io);
     }
     e = cudaFuncSetAttribute(deform_tc_kernel<ARITH, MODE, C, L, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
     if (e != cudaSuccess) return e;
-    return launch_k(deform_tc_kernel<ARITH, MODE, C, L, false>, dim3(grid), dim3(threads), bytes, st, true, d, tw, Ls, cam, use_cam ? 1 : 0, n, io);
+    return launch_k(deform_tc_kernel<ARITH, MODE, C, L, false>, dim3(grid), dim3(threads), bytes, st, true, d, tw, Ls, cam, n, io);
 }
 
 cudaError_t launch_deform_tc(const DeformDesc& d, const TcWeights& tw, int mode, const CameraDev* cam, int64_t n,
@@ -559,11 +556,10 @@ cudaError_t launch_deform_tc(const DeformDesc& d, const TcWeights& tw, int mode,
     const size_t bytes = Ls.total;
     const int64_t ntiles = (n + 64 * (tw.arith == 2 ? 2 : 1) - 1) / (64 * (tw.arith == 2 ? 2 : 1));
     const int grid = (int)(ntiles < sm_count ? ntiles : sm_count);
-    const bool use_cam = mode == 1;
 #define G4D_TC_CASE(AR, CC, LL)                                                                                        \
     if (tw.arith == AR && d.C == CC && d.levels == LL)                                                                 \
-        return mode == 0 ? launch_deform_tc_t<AR, 0, CC, LL>(d, tw, Ls, bytes, grid, cam, use_cam, n, io, st)          \
-                         : launch_deform_tc_t<AR, 1, CC, LL>(d, tw, Ls, bytes, grid, cam, use_cam, n, io, st);
+        return mode == 0 ? launch_deform_tc_t<AR, 0, CC, LL>(d, tw, Ls, bytes, grid, cam, n, io, st)                   \
+                         : launch_deform_tc_t<AR, 1, CC, LL>(d, tw, Ls, bytes, grid, cam, n, io, st);
     G4D_TC_CASE(2, 16, 2)
     G4D_TC_CASE(2, 16, 3)
     G4D_TC_CASE(2, 32, 2)

@@ -86,8 +86,8 @@ struct CollapseDesc {
 
 // Every Gaussian of a view shares t, so the time-axis interpolation of the three time planes is done once:
 // row[x][c] = plane[y0][x][c]*(y1-y) + plane[y1][x][c]*(y-y0)  with t NOT normalised (hexplane.py:164).
-__global__ void collapse_time_rows_kernel(CollapseDesc d, const CameraDev* cam, float time_arg, int use_cam_time) {
-    pdl_wait();         // cam->time (pack_camera); the rows are read by the previous view's kernels until they complete
+__global__ void collapse_time_rows_kernel(CollapseDesc d, float time) {
+    pdl_wait();         // the row buffer is reused: the previous view's kernels read it until they complete
     pdl_trigger();
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const int nseg = d.levels * 3;
@@ -95,16 +95,14 @@ __global__ void collapse_time_rows_kernel(CollapseDesc d, const CameraDev* cam, 
     int m = 0;
     while (i >= d.start[m + 1]) ++m;
     const int l = m / 3, a = m % 3, e = i - d.start[m];
-    const float t = use_cam_time ? cam->time : time_arg;
     const int T = d.res[l][3];
-    const Tap1D ty = make_tap(t, T);
+    const Tap1D ty = make_tap(time, T);
     const int rowlen = d.res[l][a] * d.C;
     const float v0 = __ldg(d.plane[l][a] + (size_t)ty.i0 * rowlen + e), v1 = __ldg(d.plane[l][a] + (size_t)ty.i1 * rowlen + e);
     d.row[l][a][e] = fmaf(v1, ty.w1, v0 * ty.w0);
 }
 
-cudaError_t launch_collapse_time_rows(const G4DDeformParams& p, const CameraDev* cam, float time, float* const (*trow)[3],
-                                      cudaStream_t st) {
+cudaError_t launch_collapse_time_rows(const G4DDeformParams& p, float time, float* const (*trow)[3], cudaStream_t st) {
     CollapseDesc d{};
     d.levels = p.levels; d.C = p.channels;
     const TimeRows tr(p.levels, p.res, p.channels);
@@ -115,7 +113,7 @@ cudaError_t launch_collapse_time_rows(const G4DDeformParams& p, const CameraDev*
     }
     for (int m = 0; m <= 3 * p.levels; ++m) d.start[m] = tr.start[m];
     const int total = (int)tr.total();
-    return launch_k(collapse_time_rows_kernel, dim3((total + 255) / 256), dim3(256), 0, st, true, d, cam, time, 0);
+    return launch_k(collapse_time_rows_kernel, dim3((total + 255) / 256), dim3(256), 0, st, true, d, time);
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -123,8 +121,7 @@ cudaError_t launch_collapse_time_rows(const G4DDeformParams& p, const CameraDev*
 __global__ void __launch_bounds__(256) preprocess_kernel(const CameraDev* __restrict__ camp, int64_t n, RasterInputs in,
                                                          GeomBuffers g, int32_t* out_radii) {
     __shared__ CameraDev cam;
-    for (int i = threadIdx.x; i < (int)(sizeof(CameraDev) / 4); i += blockDim.x)
-        reinterpret_cast<uint32_t*>(&cam)[i] = reinterpret_cast<const uint32_t*>(camp)[i];
+    stage_cameras(&cam, &camp, 1);
     __syncthreads();
     const int64_t gi = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (gi >= n) return;
@@ -135,16 +132,7 @@ __global__ void __launch_bounds__(256) preprocess_kernel(const CameraDev* __rest
     const bool ok = project_gaussian(cam, p, sc, Quat{q4.x, q4.y, q4.z, q4.w}, pr);
     float rgb[3] = {0.f, 0.f, 0.f};
     uint32_t bits = 0;
-    if (ok) {
-        if (in.shs) {
-            const float* sh = in.shs + gi * 48;
-            sh_to_rgb(cam, p, [&](int k, int ch) { return __ldg(sh + 3 * k + ch); }, rgb, bits);
-        } else {
-            const float* dc = in.sh_dc + gi * 3;
-            const float* rest = in.sh_rest + gi * 45;
-            sh_to_rgb(cam, p, [&](int k, int ch) { return k == 0 ? __ldg(dc + ch) : __ldg(rest + 3 * (k - 1) + ch); }, rgb, bits);
-        }
-    }
+    if (ok) in.sh.with_coeffs(gi, [&](auto sh) { sh_to_rgb(cam, p, sh, rgb, bits); });
     store_projected(g, gi, ok, pr, in.opacities[gi], rgb, bits, out_radii);
 }
 
@@ -161,29 +149,18 @@ cudaError_t launch_preprocess(const CameraDev* cam, int64_t n, const RasterInput
 // projects it into every other camera with the fused kernels' projection and colour code: the inputs are the very floats
 // those kernels held in registers, so each camera's records equal its own render()'s bit for bit.
 __global__ void __launch_bounds__(256) project_cameras_kernel(ExtraCameras ec, int64_t n, RasterInputs in) {
-    constexpr int kRow = 49;                       // padded SH row (as preprocess_backward_kernel)
-    constexpr int kCamWords = (int)(sizeof(CameraDev) / 4);
-    extern __shared__ float sh_smem[];             // [warps][32 * kRow]
+    extern __shared__ float sh_smem[];             // [warps][32 * kShRow]
     __shared__ CameraDev cams[kMaxExtraCameras];
     pdl_wait();         // the cameras (pack_camera) and camera 0's stored tensors
     pdl_trigger();
-    for (int i = threadIdx.x; i < ec.count * kCamWords; i += blockDim.x) {
-        const int c = i / kCamWords, w = i - c * kCamWords;
-        reinterpret_cast<uint32_t*>(&cams[c])[w] = reinterpret_cast<const uint32_t*>(ec.cam[c])[w];
-    }
+    stage_cameras(cams, ec.cam, ec.count);
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    float* ld = sh_smem + (size_t)warp * 32 * kRow;
+    float* ld = sh_smem + (size_t)warp * 32 * kShRow;
     const int64_t g0 = (int64_t)blockIdx.x * blockDim.x + warp * 32;
     const int cnt = (int)(n - g0 < 32 ? (n - g0 > 0 ? n - g0 : 0) : 32);
     if (cnt == 0) return;                          // whole warp
-    for (int idx = lane; idx < cnt * 48; idx += 32) {
-        const int i = idx / 48, e = idx - i * 48;
-        float v;
-        if (in.shs) v = __ldg(in.shs + g0 * 48 + idx);
-        else v = e < 3 ? __ldg(in.sh_dc + (g0 + i) * 3 + e) : __ldg(in.sh_rest + (g0 + i) * 45 + (e - 3));
-        ld[i * kRow + e] = v;
-    }
+    in.sh.stage_warp(g0, cnt, lane, ld);
     __syncwarp();
     if (lane >= cnt) return;
     const int64_t gi = g0 + lane;
@@ -191,7 +168,7 @@ __global__ void __launch_bounds__(256) project_cameras_kernel(ExtraCameras ec, i
     const Vec3 sc{in.scales[3 * gi], in.scales[3 * gi + 1], in.scales[3 * gi + 2]};
     const float4 q4 = *reinterpret_cast<const float4*>(in.rotations + 4 * gi);
     const float op = in.opacities[gi];
-    const float* row = ld + lane * kRow;
+    const float* row = ld + lane * kShRow;
     for (int c = 0; c < ec.count; ++c) {
         const CameraDev& cam = cams[c];
         Projected pr;
@@ -206,7 +183,7 @@ __global__ void __launch_bounds__(256) project_cameras_kernel(ExtraCameras ec, i
 cudaError_t launch_project_cameras(const ExtraCameras& ec, int64_t n, const RasterInputs& in, cudaStream_t st) {
     if (n == 0 || ec.count == 0) return cudaSuccess;
     constexpr int kThreads = 256;
-    const size_t smem = (size_t)(kThreads / 32) * 32 * 49 * sizeof(float);   // 49 KB: SH staging
+    const size_t smem = (size_t)(kThreads / 32) * 32 * kShRow * sizeof(float);   // 49 KB: SH staging
     cudaError_t e = cudaFuncSetAttribute(project_cameras_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     return launch_k(project_cameras_kernel, dim3((unsigned)((n + kThreads - 1) / kThreads)), dim3(kThreads), smem, st, true, ec, n, in);
@@ -218,16 +195,12 @@ cudaError_t launch_project_cameras(const ExtraCameras& ec, int64_t n, const Rast
 //   MODE 1: fused deformation + activations + projection (the render() hot path)
 template <int TG, int WD, int MODE>
 __global__ void __launch_bounds__(kDeformThreads, 1)
-deform_kernel(DeformDesc d, DeformSmem L, const CameraDev* __restrict__ camp, float time_arg, int use_cam_time, int64_t n,
-              DeformIO io) {
+deform_kernel(DeformDesc d, DeformSmem L, const CameraDev* __restrict__ camp, int64_t n, DeformIO io) {
     extern __shared__ __align__(16) float smem[];
     __shared__ CameraDev cam;
     const int tid = threadIdx.x;
     const int64_t ntiles = (n + TG - 1) / TG;
-    if (MODE == 1 || use_cam_time) {
-        for (int i = tid; i < (int)(sizeof(CameraDev) / 4); i += kDeformThreads)
-            reinterpret_cast<uint32_t*>(&cam)[i] = reinterpret_cast<const uint32_t*>(camp)[i];
-    }
+    if (MODE == 1) stage_cameras(&cam, &camp, 1);
     stage_persistent_weights(d, L, smem);
     void* bar = smem + L.mbar;
     if (tid == 0) { mbar_init(bar, 1); fence_barrier_init(); }
@@ -240,7 +213,6 @@ deform_kernel(DeformDesc d, DeformSmem L, const CameraDev* __restrict__ camp, fl
         tma_bulk_g2s(smem + L.w1t, d.w1t[first], (uint32_t)(WD * WD * sizeof(float)), bar);
     }
     uint32_t phase = 0;
-    const float t = use_cam_time ? cam.time : time_arg;
     const AabbNorm nrm(d.aabb);
     float* in_xyz = smem + L.in;
     float* in_sc = in_xyz + TG * 3;
@@ -267,7 +239,7 @@ deform_kernel(DeformDesc d, DeformSmem L, const CameraDev* __restrict__ camp, fl
             c.x = nrm(0, in_xyz[3 * tid + 0]);
             c.y = nrm(1, in_xyz[3 * tid + 1]);
             c.z = nrm(2, in_xyz[3 * tid + 2]);
-            c.w = t;
+            c.w = 0.f;          // (time enters through the collapsed time rows)
             *reinterpret_cast<float4*>(coord + 4 * tid) = c;
         }
         __syncthreads();
@@ -291,18 +263,14 @@ deform_kernel(DeformDesc d, DeformSmem L, const CameraDev* __restrict__ camp, fl
                 for (int i = tid; i < TG * 48; i += kDeformThreads)
                     if (i < rem * 48) {
                         const int g = i / 48, c = i - 48 * g;
-                        io.out_shs[base * 48 + i] = io.shs[base * 48 + i] + out[g * 60 + 11 + c];
+                        io.out_shs[base * 48 + i] = io.sh.shs[base * 48 + i] + out[g * 60 + 11 + c];
                     }
         } else {
             if (hsh && io.fo.shs) {   // deformed SH coefficients are needed again by the backward pass
                 for (int i = tid; i < TG * 48; i += kDeformThreads)
                     if (i < rem * 48) {
                         const int g = i / 48, c = i - 48 * g;
-                        const int64_t gi = base + g;
-                        float b;
-                        if (io.shs) b = io.shs[gi * 48 + c];
-                        else b = c < 3 ? io.sh_dc[gi * 3 + c] : io.sh_rest[gi * 45 + (c - 3)];
-                        io.fo.shs[base * 48 + i] = b + out[g * 60 + 11 + c];
+                        io.fo.shs[base * 48 + i] = io.sh.at(base + g, c) + out[g * 60 + 11 + c];
                     }
             }
             if (tid < TG && tid < rem) {
@@ -329,8 +297,8 @@ cudaError_t launch_deform_tc(const DeformDesc& d, const TcWeights& tw, int mode,
                              const DeformIO& io, int sm_count, cudaStream_t st);
 
 template <int TG, int WD, int MODE>
-static cudaError_t launch_deform_t(const DeformDesc& d, const CameraDev* cam, float time, int64_t n, const DeformIO& io,
-                                   int sm_count, cudaStream_t st) {
+static cudaError_t launch_deform_t(const DeformDesc& d, const CameraDev* cam, int64_t n, const DeformIO& io, int sm_count,
+                                   cudaStream_t st) {
     const DeformSmem L = deform_smem_layout(TG, d.F, WD, d.head_mask);
     const size_t bytes = (size_t)L.total_floats * sizeof(float);
     if (bytes > 227 * 1024) return cudaErrorInvalidConfiguration;
@@ -338,74 +306,43 @@ static cudaError_t launch_deform_t(const DeformDesc& d, const CameraDev* cam, fl
     if (e != cudaSuccess) return e;
     const int64_t ntiles = (n + TG - 1) / TG;
     const int grid = (int)(ntiles < sm_count ? ntiles : sm_count);
-    deform_kernel<TG, WD, MODE><<<grid, kDeformThreads, bytes, st>>>(d, L, cam, time, 0, n, io);
+    deform_kernel<TG, WD, MODE><<<grid, kDeformThreads, bytes, st>>>(d, L, cam, n, io);
     return cudaGetLastError();
 }
 
-cudaError_t launch_deform(const DeformDesc& d, int mode, const CameraDev* cam, float time, int64_t n, const DeformIO& io,
-                          int sm_count, cudaStream_t st, const TcWeights* tw) {
+cudaError_t launch_deform(const DeformDesc& d, int mode, const CameraDev* cam, int64_t n, const DeformIO& io, int sm_count,
+                          cudaStream_t st, const TcWeights* tw) {
     if (n == 0) return cudaSuccess;
     if (tw) return launch_deform_tc(d, *tw, mode, cam, n, io, sm_count, st);
     if (d.WD == 128) {
-        return mode == 0 ? launch_deform_t<64, 128, 0>(d, cam, time, n, io, sm_count, st)
-                         : launch_deform_t<64, 128, 1>(d, cam, time, n, io, sm_count, st);
+        return mode == 0 ? launch_deform_t<64, 128, 0>(d, cam, n, io, sm_count, st)
+                         : launch_deform_t<64, 128, 1>(d, cam, n, io, sm_count, st);
     } else if (d.WD == 64) {
-        return mode == 0 ? launch_deform_t<128, 64, 0>(d, cam, time, n, io, sm_count, st)
-                         : launch_deform_t<128, 64, 1>(d, cam, time, n, io, sm_count, st);
+        return mode == 0 ? launch_deform_t<128, 64, 0>(d, cam, n, io, sm_count, st)
+                         : launch_deform_t<128, 64, 1>(d, cam, n, io, sm_count, st);
     }
     return cudaErrorInvalidValue;
 }
 
 // ------------------------------------------------------------------------------------------------------
-// "coarse" stage of render() (gaussian_renderer/__init__.py:80-81): activations + projection, no deformation.
-__global__ void __launch_bounds__(256)
-activate_preprocess_kernel(const CameraDev* __restrict__ camp, int64_t n, const float* __restrict__ xyz,
-                           const float* __restrict__ scaling, const float* __restrict__ rotation,
-                           const float* __restrict__ opacity, const float* __restrict__ shs, const float* __restrict__ sh_dc,
-                           const float* __restrict__ sh_rest, GeomBuffers g, FusedOutputs fo, int32_t* out_radii) {
+// "coarse" stage of render() (gaussian_renderer/__init__.py:80-81): the fused tail with no network deltas.
+__global__ void __launch_bounds__(256) activate_preprocess_kernel(const CameraDev* __restrict__ camp, int64_t n, DeformIO io) {
     __shared__ CameraDev cam;
-    for (int i = threadIdx.x; i < (int)(sizeof(CameraDev) / 4); i += blockDim.x)
-        reinterpret_cast<uint32_t*>(&cam)[i] = reinterpret_cast<const uint32_t*>(camp)[i];
+    stage_cameras(&cam, &camp, 1);
     __syncthreads();
     const int64_t gi = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (gi >= n) return;
-    const Vec3 p{xyz[3 * gi], xyz[3 * gi + 1], xyz[3 * gi + 2]};
-    const Vec3 sc{expf(scaling[3 * gi]), expf(scaling[3 * gi + 1]), expf(scaling[3 * gi + 2])};
-    const float4 q = *reinterpret_cast<const float4*>(rotation + 4 * gi);
-    const float qn = fmaxf(sqrtf(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w), 1e-12f);
-    const Quat rq{q.x / qn, q.y / qn, q.z / qn, q.w / qn};
-    const float op = 1.f / (1.f + expf(-opacity[gi]));
-    Projected pr;
-    const bool ok = project_gaussian(cam, p, sc, rq, pr);
-    float rgb[3] = {0.f, 0.f, 0.f};
-    uint32_t bits = 0;
-    if (ok) {
-        if (shs) {
-            const float* sh = shs + gi * 48;
-            sh_to_rgb(cam, p, [&](int k, int ch) { return __ldg(sh + 3 * k + ch); }, rgb, bits);
-        } else {
-            const float* dc = sh_dc + gi * 3;
-            const float* rest = sh_rest + gi * 45;
-            sh_to_rgb(cam, p, [&](int k, int ch) { return k == 0 ? __ldg(dc + ch) : __ldg(rest + 3 * (k - 1) + ch); }, rgb, bits);
-        }
-    }
-    store_projected(g, gi, ok, pr, op, rgb, bits, out_radii);
-    if (fo.means3D) {
-        fo.means3D[3 * gi] = p.x; fo.means3D[3 * gi + 1] = p.y; fo.means3D[3 * gi + 2] = p.z;
-        fo.scales[3 * gi] = sc.x; fo.scales[3 * gi + 1] = sc.y; fo.scales[3 * gi + 2] = sc.z;
-        *reinterpret_cast<float4*>(fo.rotations + 4 * gi) = make_float4(rq.r, rq.x, rq.y, rq.z);
-        fo.opacities[gi] = op;
-        if (fo.rot_norm) fo.rot_norm[gi] = qn;
-    }
+    const Vec3 p{io.xyz[3 * gi], io.xyz[3 * gi + 1], io.xyz[3 * gi + 2]};
+    const float sl[3] = {io.scaling[3 * gi], io.scaling[3 * gi + 1], io.scaling[3 * gi + 2]};
+    const float4 q4 = *reinterpret_cast<const float4*>(io.rotation + 4 * gi);
+    const float q[4] = {q4.x, q4.y, q4.z, q4.w};
+    // a delta of -0.f leaves every coefficient as it is (x + -0 == x, also for x = +0), so the add compiles away
+    fused_finish(cam, io, gi, p, sl, q, io.opacity[gi], [](int) { return -0.f; });
 }
 
-cudaError_t launch_activate_preprocess(const CameraDev* cam, int64_t n, const float* xyz, const float* scaling,
-                                       const float* rotation, const float* opacity, const float* shs, const float* sh_dc,
-                                       const float* sh_rest, GeomBuffers g, FusedOutputs fo, int32_t* out_radii,
-                                       cudaStream_t st) {
+cudaError_t launch_activate_preprocess(const CameraDev* cam, int64_t n, const DeformIO& io, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
-    activate_preprocess_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(cam, n, xyz, scaling, rotation, opacity, shs, sh_dc,
-                                                                            sh_rest, g, fo, out_radii);
+    activate_preprocess_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(cam, n, io);
     return cudaGetLastError();
 }
 

@@ -98,13 +98,75 @@ struct ImageBuffers {
     uint32_t* n_contrib; // [H*W]
 };
 
+// ---- SH coefficients: one source and one sink type for both layouts ----------------------------------------------
+// The accessors only move data: they are shared by units compiled with and without FMA contraction.
+constexpr int kShRow = 49;   // floats per Gaussian in a warp's shared-memory SH rows: lane i <-> row i is bank-conflict free
+
+// A Gaussian's 16 x 3 coefficients, fused [N,16,3] in shs, or (shs == NULL) split into dc [N,1,3] + rest [N,15,3]
+struct ShIn {
+    const float *shs, *dc, *rest;
+    // coefficient e = 3 * k + ch of Gaussian gi
+    G4D_D float at(int64_t gi, int e) const {
+        return shs ? __ldg(shs + gi * 48 + e) : e < 3 ? __ldg(dc + gi * 3 + e) : __ldg(rest + gi * 45 + (e - 3));
+    }
+    // f(load) with load(k, ch) -> coefficient k, channel ch of Gaussian gi; the layout is chosen once, outside f
+    template <class F> G4D_D void with_coeffs(int64_t gi, F&& f) const {
+        if (shs) f([=](int k, int ch) { return __ldg(shs + gi * 48 + 3 * k + ch); });
+        else f([=](int k, int ch) { return k == 0 ? __ldg(dc + gi * 3 + ch) : __ldg(rest + gi * 45 + 3 * (k - 1) + ch); });
+    }
+    // all 48 into registers (float4 loads on the fused layout); v[3 * k + ch]
+    G4D_D void load(int64_t gi, float (&v)[48]) const {
+        if (shs) {
+#pragma unroll
+            for (int j = 0; j < 48; j += 4) {
+                const float4 b = __ldg(reinterpret_cast<const float4*>(shs + gi * 48 + j));
+                v[j] = b.x; v[j + 1] = b.y; v[j + 2] = b.z; v[j + 3] = b.w;
+            }
+        } else {
+#pragma unroll
+            for (int j = 0; j < 3; ++j) v[j] = __ldg(dc + gi * 3 + j);
+#pragma unroll
+            for (int j = 0; j < 45; ++j) v[3 + j] = __ldg(rest + gi * 45 + j);
+        }
+    }
+    // warp-wide: Gaussians g0 .. g0 + cnt - 1 into rows[i * kShRow + 3 * k + ch], read as contiguous 128-byte lines
+    G4D_D void stage_warp(int64_t g0, int cnt, int lane, float* rows) const {
+        for (int idx = lane; idx < cnt * 48; idx += 32) {
+            const int i = idx / 48, e = idx - i * 48;
+            rows[i * kShRow + e] = at(g0 + i, e);
+        }
+    }
+};
+
+// gradient sinks of the coefficients; each may be NULL, and the fused and the split sinks may both be given
+struct ShOut {
+    float *shs, *dc, *rest;
+    // warp-wide: the inverse of ShIn::stage_warp
+    G4D_D void store_warp(int64_t g0, int cnt, int lane, const float* rows) const {
+        for (int idx = lane; idx < cnt * 48; idx += 32) {
+            const int i = idx / 48, e = idx - i * 48;
+            const float v = rows[i * kShRow + e];
+            if (shs) shs[g0 * 48 + idx] = v;
+            if (e < 3) { if (dc) dc[(g0 + i) * 3 + e] = v; }
+            else if (rest) rest[(g0 + i) * 45 + (e - 3)] = v;
+        }
+    }
+};
+
+// copies the `count` cameras *src[c] into dst[c] (shared memory), word by word across the block; the caller syncs.
+// (P: a camera pointer type, __restrict__ or not)
+template <class P>
+G4D_D void stage_cameras(CameraDev* dst, const P* src, int count) {
+    for (int c = 0; c < count; ++c)
+        for (int i = threadIdx.x; i < (int)(sizeof(CameraDev) / 4); i += blockDim.x)
+            reinterpret_cast<uint32_t*>(dst + c)[i] = reinterpret_cast<const uint32_t*>(src[c])[i];
+}
+
 // inputs of the rasterizer stage in device memory (post-activation), either caller tensors or the
 // tensors the fused path produced
 struct RasterInputs {
     const float* means3D; const float* scales; const float* rotations; const float* opacities;
-    const float* shs;       // fused [N,16,3] or NULL
-    const float* sh_dc;     // used when shs == NULL: [N,1,3]
-    const float* sh_rest;   //                        [N,15,3]
+    ShIn sh;
 };
 
 struct FusedOutputs {   // what the fused forward saves for its backward (may be NULL in deform-only mode)
@@ -113,10 +175,11 @@ struct FusedOutputs {   // what the fused forward saves for its backward (may be
     float* rot_norm;   // |q| before F.normalize (needed by its backward)
 };
 
-// tensors of one deformation launch (mode 0 reads xyz .. shs and writes out_*; mode 1 also reads sh_dc / sh_rest and writes
-// g, fo and out_radii)
+// tensors of one deformation launch (mode 0 reads xyz .. sh, SH fused, and writes out_*; mode 1, and the coarse stage that
+// has no network, read either SH layout and write g, fo and out_radii)
 struct DeformIO {
-    const float *xyz, *scaling, *rotation, *opacity, *shs, *sh_dc, *sh_rest;
+    const float *xyz, *scaling, *rotation, *opacity;
+    ShIn sh;
     float *out_xyz, *out_scaling, *out_rotation, *out_opacity, *out_shs;
     GeomBuffers g;
     FusedOutputs fo;
@@ -170,25 +233,24 @@ cudaError_t launch_distribute_time_grad(const DeformDesc& d, float* const (*trow
 // ---- launchers (defined in g4d_geom.cu / g4d_raster.cu / g4d_backward.cu) -----------------------------
 cudaError_t launch_pack_camera(const G4DCamera& cam, CameraDev* dst, cudaStream_t st);
 cudaError_t launch_pack_weights(const G4DDeformParams& p, float* w0t, float* const* w1t, cudaStream_t st);
-cudaError_t launch_collapse_time_rows(const G4DDeformParams& p, const CameraDev* cam, float time, float* const (*trow)[3],
-                                      cudaStream_t st);
+cudaError_t launch_collapse_time_rows(const G4DDeformParams& p, float time, float* const (*trow)[3], cudaStream_t st);
 cudaError_t launch_preprocess(const CameraDev* cam, int64_t n, const RasterInputs& in, GeomBuffers g, int32_t* out_radii,
                               cudaStream_t st);
-// mode 0: deform only (writes the five out_* tensors); mode 1: fused deform + preprocess (camera from cam).  tw: run on the
-// tensor cores with these weight images and buffers
-cudaError_t launch_deform(const DeformDesc& d, int mode, const CameraDev* cam, float time, int64_t n, const DeformIO& io,
-                          int sm_count, cudaStream_t st, const TcWeights* tw = nullptr);
+// mode 0: deform only (writes the five out_* tensors; cam unused); mode 1: fused deform + preprocess (camera from cam).
+// tw: run on the tensor cores with these weight images and buffers
+cudaError_t launch_deform(const DeformDesc& d, int mode, const CameraDev* cam, int64_t n, const DeformIO& io, int sm_count,
+                          cudaStream_t st, const TcWeights* tw = nullptr);
 
 cudaError_t launch_blend_forward(const CameraDev* cam, int grid_x, int grid_y, GeomBuffers g, BinBuffers b, ImageBuffers im,
                                  float* out_color, float* out_depth, int warp_cull, cudaStream_t st);
 cudaError_t launch_blend_backward(const CameraDev* cam, int grid_x, int grid_y, GeomBuffers g, BinBuffers b, ImageBuffers im,
                                   const float* dL_dcolor, float* g_mean2D, float* g_conic, float* g_opacity, float* g_rgb,
                                   int warp_cull, cudaStream_t st);
-// per-Gaussian backward; g_shs may alias separate dc/rest sinks through (g_sh_dc, g_sh_rest) when g_shs == NULL
+// per-Gaussian backward
 cudaError_t launch_preprocess_backward(const CameraDev* cam, int64_t n, const RasterInputs& in, GeomBuffers g,
                                        const float* g_mean2D, const float* g_conic, const float* g_rgb, float* g_means3D,
-                                       float* g_means2D_out, float* g_scales, float* g_rotations, float* g_shs,
-                                       float* g_sh_dc, float* g_sh_rest, cudaStream_t st);   // fused and split SH sinks may both be given
+                                       float* g_means2D_out, float* g_scales, float* g_rotations, const ShOut& g_sh,
+                                       cudaStream_t st);
 
 size_t deform_backward_scratch_bytes(const DeformDesc& d, int64_t n);   // size of launch_deform_backward's scratch
 // go[h] / gi[h]: gradient w.r.t. the outputs / inputs of head h's residual tensor (xyz, scaling, rotation, opacity, shs)
@@ -218,16 +280,13 @@ struct BackwardCameras {
     float* g_means2D[G4D_MAX_CAMERAS];     // [N,3] screen-space gradient of the camera, or NULL
 };
 // per-Gaussian backward of all those cameras in one pass: the gradients w.r.t. means3D, scales, rotations, opacity and the
-// SH coefficients are summed over the cameras and written once (OVERWRITTEN); SH sinks as launch_preprocess_backward
+// SH coefficients are summed over the cameras and written once (OVERWRITTEN)
 cudaError_t launch_preprocess_backward_cameras(const BackwardCameras& bc, int64_t n, const RasterInputs& in, float* g_means3D,
-                                               float* g_scales, float* g_rotations, float* g_opacities, float* g_shs,
-                                               float* g_sh_dc, float* g_sh_rest, cudaStream_t st);
+                                               float* g_scales, float* g_rotations, float* g_opacities, const ShOut& g_sh,
+                                               cudaStream_t st);
 
-// coarse stage of render(): activations + projection without the deformation network
-cudaError_t launch_activate_preprocess(const CameraDev* cam, int64_t n, const float* xyz, const float* scaling,
-                                       const float* rotation, const float* opacity, const float* shs, const float* sh_dc,
-                                       const float* sh_rest, GeomBuffers g, FusedOutputs fo, int32_t* out_radii,
-                                       cudaStream_t st);
+// coarse stage of render(): the fused forward's tail without the deformation network (io as for launch_deform mode 1)
+cudaError_t launch_activate_preprocess(const CameraDev* cam, int64_t n, const DeformIO& io, cudaStream_t st);
 // chain rule through exp / normalize / sigmoid (gaussian_renderer/__init__.py:97-99); in-place on the gradient buffers
 cudaError_t launch_activation_backward(int64_t n, const FusedOutputs& fo, float* g_scales, float* g_rotations,
                                        float* g_opacities, cudaStream_t st);

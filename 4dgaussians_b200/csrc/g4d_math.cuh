@@ -175,20 +175,24 @@ G4D_HD bool project_gaussian(const CameraDev& cam, Vec3 p, Vec3 scale, Quat rot,
     return true;
 }
 
-// A.1 step 10.  ShLoad: float operator()(int coeff, int channel).
-template <class ShLoad>
+// A.1 step 10.  ShLoad: float operator()(int coeff, int channel).  UNROLL, for a loader that reads a register array: the loop
+// runs to the constant 16 under the degree mask, so the compiler unrolls it and every coefficient index is a compile-time
+// constant (the full basis is computed, without branches).  Otherwise, for a loader that reads memory, the loop runs to the
+// camera's coefficient count and keeps the basis in a local array: fewer live registers.  The sums are the same either way.
+template <bool UNROLL = false, class ShLoad>
 G4D_HD void sh_to_rgb(const CameraDev& cam, Vec3 p, ShLoad sh, float rgb[3], uint32_t& clamped_bits) {
     float dx = p.x - cam.campos[0], dy = p.y - cam.campos[1], dz = p.z - cam.campos[2];
     float len = sqrtf(dx * dx + dy * dy + dz * dz);
     dx = dx / len; dy = dy / len; dz = dz / len;
     float bas[16];
-    sh_basis(cam.sh_degree, dx, dy, dz, bas);
+    sh_basis(UNROLL ? 3 : cam.sh_degree, dx, dy, dz, bas);
     const int ncoef = (cam.sh_degree + 1) * (cam.sh_degree + 1);
     clamped_bits = 0;
 #pragma unroll
     for (int ch = 0; ch < 3; ++ch) {
         float acc = bas[0] * sh(0, ch);
-        for (int k = 1; k < ncoef; ++k) acc = acc + bas[k] * sh(k, ch);
+        for (int k = 1; k < (UNROLL ? 16 : ncoef); ++k)
+            if (k < ncoef) acc = acc + bas[k] * sh(k, ch);
         acc = acc + 0.5f;
         if (acc < 0.f) clamped_bits |= (1u << ch);
         rgb[ch] = fmaxf_(acc, 0.f);
