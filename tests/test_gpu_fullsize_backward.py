@@ -31,8 +31,8 @@ import torch
 
 from oracle import deform_ref as dr
 from oracle import raster_ref as rr
-from test_gpu_fullsize import STATS as FWD_STATS, _assert_index_data_bit_exact
-from util_scene import (SCENE_LEAVES, cam_tuple, colour_kink_rows, deformed_fp64, g4d, kink_rows, make_module,
+from test_gpu_fullsize import STATS as FWD_STATS
+from util_scene import (SCENE_LEAVES, _assert_index_data_bit_exact, cam_tuple, colour_kink_rows, deformed_fp64, g4d, kink_rows, make_module,
                         oracle_chain_backward, oracle_params_from_module, raster_oracle_inputs, rel_err, row_err, row_errors,
                         synth, threshold_pixels)
 
