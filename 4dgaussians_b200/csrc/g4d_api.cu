@@ -1166,6 +1166,8 @@ int g4d_adam_step(G4DWorkspace* ws, float* param, const float* grad, float* exp_
         return fail(G4D_ERR_ARG, "g4d_adam_step: bad argument");
     if ((numel & 3) || num_segments < 0 || num_segments > G4D_ADAM_MAX_SEGMENTS)
         return fail(G4D_ERR_ARG, "g4d_adam_step: numel must be a multiple of 4 and at most 16 segments");
+    if (((uintptr_t)param | (uintptr_t)grad | (uintptr_t)exp_avg | (uintptr_t)exp_avg_sq) & 15u)   // the kernel moves float4s
+        return fail(G4D_ERR_ARG, "g4d_adam_step: param, grad, exp_avg and exp_avg_sq must be 16-byte aligned");
     for (int i = 0; i < num_segments; ++i)
         if (segments[i].begin < 0 || segments[i].end < segments[i].begin || segments[i].end > numel || (i && segments[i].begin < segments[i - 1].end))
             return fail(G4D_ERR_ARG, "g4d_adam_step: segments must be sorted, disjoint and inside [0, numel)");

@@ -38,36 +38,52 @@ __device__ __forceinline__ float block_sum_f(float v) {
 }
 
 // ---- L1 -----------------------------------------------------------------------------------------------------------
+// kVec: every pointer is 16-byte aligned, float4 loads + a scalar tail in block 0.  Otherwise (a view at an odd storage
+// offset, e.g. batch[1] of a [B,3,H,W] batch with H*W odd) the same sum with scalar loads.
+template <bool kVec>
 __global__ void __launch_bounds__(256) l1_loss_kernel(const float* __restrict__ a, const float* __restrict__ b, int64_t n, float scale,
                                                       float* __restrict__ loss) {
     float acc = 0.f;
-    const int64_t n4 = n >> 2;
-    const float4* a4 = reinterpret_cast<const float4*>(a);
-    const float4* b4 = reinterpret_cast<const float4*>(b);
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
-        const float4 x = a4[i], y = __ldg(b4 + i);
-        acc += fabsf(x.x - y.x) + fabsf(x.y - y.y) + fabsf(x.z - y.z) + fabsf(x.w - y.w);
+    if (kVec) {
+        const int64_t n4 = n >> 2;
+        const float4* a4 = reinterpret_cast<const float4*>(a);
+        const float4* b4 = reinterpret_cast<const float4*>(b);
+        for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
+            const float4 x = a4[i], y = __ldg(b4 + i);
+            acc += fabsf(x.x - y.x) + fabsf(x.y - y.y) + fabsf(x.z - y.z) + fabsf(x.w - y.w);
+        }
+        if (blockIdx.x == 0 && threadIdx.x < (n & 3)) { const int64_t i = (n4 << 2) + threadIdx.x; acc += fabsf(a[i] - b[i]); }
+    } else {
+        for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+            acc += fabsf(a[i] - __ldg(b + i));
     }
-    if (blockIdx.x == 0 && threadIdx.x < (n & 3)) { const int64_t i = (n4 << 2) + threadIdx.x; acc += fabsf(a[i] - b[i]); }
     const float tot = block_sum_f(acc);
     if (threadIdx.x == 0) atomicAdd(loss, tot * scale);
 }
 
 // grad = sign(a - b) * scale * upstream[0]     (torch.abs backward: sign(0) = 0)
+template <bool kVec>
 __global__ void __launch_bounds__(256) l1_grad_kernel(const float* __restrict__ a, const float* __restrict__ b, int64_t n, float scale,
                                                       const float* __restrict__ upstream, float* __restrict__ grad) {
     const float s = scale * (upstream ? __ldg(upstream) : 1.f);
-    const int64_t n4 = n >> 2;
-    const float4* a4 = reinterpret_cast<const float4*>(a);
-    const float4* b4 = reinterpret_cast<const float4*>(b);
-    float4* g4 = reinterpret_cast<float4*>(grad);
     auto sg = [s](float d) { return d > 0.f ? s : (d < 0.f ? -s : 0.f); };
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
-        const float4 x = a4[i], y = __ldg(b4 + i);
-        g4[i] = make_float4(sg(x.x - y.x), sg(x.y - y.y), sg(x.z - y.z), sg(x.w - y.w));
+    if (kVec) {
+        const int64_t n4 = n >> 2;
+        const float4* a4 = reinterpret_cast<const float4*>(a);
+        const float4* b4 = reinterpret_cast<const float4*>(b);
+        float4* g4 = reinterpret_cast<float4*>(grad);
+        for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
+            const float4 x = a4[i], y = __ldg(b4 + i);
+            g4[i] = make_float4(sg(x.x - y.x), sg(x.y - y.y), sg(x.z - y.z), sg(x.w - y.w));
+        }
+        if (blockIdx.x == 0 && threadIdx.x < (n & 3)) { const int64_t i = (n4 << 2) + threadIdx.x; grad[i] = sg(a[i] - b[i]); }
+    } else {
+        for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+            grad[i] = sg(a[i] - __ldg(b + i));
     }
-    if (blockIdx.x == 0 && threadIdx.x < (n & 3)) { const int64_t i = (n4 << 2) + threadIdx.x; grad[i] = sg(a[i] - b[i]); }
 }
+
+inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 // ---- HexPlane regularisers ----------------------------------------------------------------------------------------------
 // plane k of a level, channel-last [H][W][C]; planes 0,1,3 are spatial (xy, xz, yz), planes 2,4,5 carry the time axis
@@ -232,13 +248,19 @@ int grid_for(int64_t work, int sm_count) {
 
 cudaError_t launch_l1_loss(const float* a, const float* b, int64_t n, float scale, float* loss, int sm_count, cudaStream_t st) {
     if (n <= 0) return cudaSuccess;
-    l1_loss_kernel<<<grid_for(n / 4, sm_count), 256, 0, st>>>(a, b, n, scale, loss);
+    if (aligned16(a) && aligned16(b))
+        l1_loss_kernel<true><<<grid_for(n / 4, sm_count), 256, 0, st>>>(a, b, n, scale, loss);
+    else
+        l1_loss_kernel<false><<<grid_for(n, sm_count), 256, 0, st>>>(a, b, n, scale, loss);
     return cudaGetLastError();
 }
 cudaError_t launch_l1_grad(const float* a, const float* b, int64_t n, float scale, const float* upstream, float* grad, int sm_count,
                            cudaStream_t st) {
     if (n <= 0) return cudaSuccess;
-    l1_grad_kernel<<<grid_for(n / 4, sm_count), 256, 0, st>>>(a, b, n, scale, upstream, grad);
+    if (aligned16(a) && aligned16(b) && aligned16(grad))
+        l1_grad_kernel<true><<<grid_for(n / 4, sm_count), 256, 0, st>>>(a, b, n, scale, upstream, grad);
+    else
+        l1_grad_kernel<false><<<grid_for(n, sm_count), 256, 0, st>>>(a, b, n, scale, upstream, grad);
     return cudaGetLastError();
 }
 
@@ -266,14 +288,14 @@ cudaError_t launch_plane_regulation(const G4DDeformParams& prm, const G4DDeformG
 
 cudaError_t launch_ssim_forward(const float* x, const float* y, int C, int H, int W, float scale, float* loss, float* dmu, float* dxx,
                                 float* dxy, cudaStream_t st) {
-    if (C * H * W == 0) return cudaSuccess;
+    if ((int64_t)C * H * W == 0) return cudaSuccess;
     const dim3 grid((W + kSsimT - 1) / kSsimT, (H + kSsimT - 1) / kSsimT, C);
     ssim_forward_kernel<<<grid, kSsimT * kSsimT, 0, st>>>(make_ssim_window(), x, y, H, W, scale, loss, dmu, dxx, dxy);
     return cudaGetLastError();
 }
 cudaError_t launch_ssim_backward(const float* x, const float* y, int C, int H, int W, float scale, const float* upstream,
                                  const float* dmu, const float* dxx, const float* dxy, float* grad, cudaStream_t st) {
-    if (C * H * W == 0) return cudaSuccess;
+    if ((int64_t)C * H * W == 0) return cudaSuccess;
     const dim3 grid((W + kSsimT - 1) / kSsimT, (H + kSsimT - 1) / kSsimT, C);
     ssim_backward_kernel<<<grid, kSsimT * kSsimT, 0, st>>>(make_ssim_window(), x, y, H, W, scale, upstream, dmu, dxx, dxy, grad);
     return cudaGetLastError();

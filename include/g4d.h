@@ -197,7 +197,9 @@ int g4d_render_backward_cameras(G4DContext *const *ctx, int32_t k, const G4DCame
  *                             floats, may be NULL when no backward follows) keeps the per-pixel partial derivatives
  *   g4d_plane_regulation   <- scene/gaussian_model.py:538-577 compute_regulation(time_smoothness_weight, l1_time_planes_weight,
  *                             plane_tv_weight) with scene/regulation.py:22-28 compute_plane_smoothness: value and, when
- *                             `grads` is given, the plane gradients ACCUMULATED into grads->planes (other fields unused) */
+ *                             `grads` is given, the plane gradients ACCUMULATED into grads->planes (other fields unused)
+ * Alignment: g4d_l1_loss / g4d_l1_loss_backward take `out`, `gt` and `grad_out` at any 4-byte alignment (a view at an odd
+ * storage offset is fine); when all of them are 16-byte aligned they run with 128-bit loads, otherwise with scalar loads. */
 int g4d_l1_loss(G4DWorkspace *ws, const float *out, const float *gt, int64_t numel, float scale, float *loss_accum,
                 void *stream);
 int g4d_l1_loss_backward(G4DWorkspace *ws, const float *out, const float *gt, int64_t numel, float scale,
@@ -215,7 +217,8 @@ int g4d_plane_regulation(G4DWorkspace *ws, const G4DDeformParams *prm, G4DDeform
  * g4d_adam_step <- gaussians.optimizer.step() (train.py:290-292; groups scene/gaussian_model.py:165-183): torch.optim.Adam
  * without weight decay over ONE flat buffer; segment i covers elements [begin, end) with its own learning rate (elements in
  * no segment are left untouched); `numel` must be a multiple of 4 (pad the buffers); `step` is the 1-based step count;
- * gradients are multiplied by grad_scale first (1 / world_size after a SUM all-reduce). */
+ * gradients are multiplied by grad_scale first (1 / world_size after a SUM all-reduce).  param, grad, exp_avg and exp_avg_sq
+ * must each be 16-byte aligned (the kernel moves float4s); otherwise G4D_ERR_ARG before any launch. */
 #define G4D_ADAM_MAX_SEGMENTS 16
 typedef struct G4DAdamSegment { int64_t begin, end; float lr; float reserved; } G4DAdamSegment;
 int g4d_adam_step(G4DWorkspace *ws, float *param, const float *grad, float *exp_avg, float *exp_avg_sq, int64_t numel,
