@@ -21,10 +21,14 @@ HEAD_POS, HEAD_SCALES, HEAD_ROT, HEAD_OPACITY, HEAD_SHS = 1, 2, 4, 8, 16
 OPT_SYNC_MODE, OPT_INSTANCE_CAPACITY, OPT_TIGHT_CULL, OPT_STAGE_TIMING, OPT_TENSOR_CORES, OPT_TC_DEBUG, OPT_WARP_CULL = 1, 2, 3, 4, 5, 6, 7
 OPT_KEEP_DEFORMED = 8
 OPT_PDL = 9
+OPT_GATHER_ORDER = 10
 STAGES = ("prep", "geom", "scan", "emit", "sort", "ranges", "blend", "blend_bwd", "geom_bwd", "deform_bwd")
 
 BUF = dict(depth=1, rect=2, tiles_touched=3, xy=4, conic_opacity=5, rgb=6, sorted_keys=7, sorted_ids=8, ranges=9,
-           final_T=10, n_contrib=11, clamped=12, deformed=13, deformed_shs=14, bin_phases=15)
+           final_T=10, n_contrib=11, clamped=12, deformed=13, deformed_shs=14, bin_phases=15, features=16)
+# G4D_BUF_GATHER_ORDER: not one of BUF, whose contents repeat bit for bit from run to run -- the order of the Gaussians inside
+# one cell of the gather's walk order does not
+BUF_GATHER_ORDER = 17
 
 # every symbol include/g4d.h declares (tests/test_abi.py checks the .so exports all of them)
 ABI_SYMBOLS = [
@@ -242,7 +246,7 @@ class Context:
             "sorted_keys": (np.uint64, (-1,)), "sorted_ids": (np.uint32, (-1,)), "ranges": (np.uint32, (-1, 2)),
             "final_T": (np.float32, (-1,)), "n_contrib": (np.uint32, (-1,)), "clamped": (np.uint8, (-1, 3)),
             "deformed": (np.float32, (-1, 11)), "deformed_shs": (np.float32, (-1, 16, 3)),
-            "bin_phases": (np.int64, (-1,))}[name]
+            "bin_phases": (np.int64, (-1,)), "features": (np.float32, (-1,))}[name]
         return raw.view(dt).reshape(shape)
 
     def __del__(self):

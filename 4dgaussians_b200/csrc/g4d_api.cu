@@ -111,6 +111,11 @@ struct G4DWorkspace {
     int warp_cull = 1;
     int keep_deformed = 0;
     int tc_debug = 0;
+    int gather_order = 1;      // G4D_OPT_GATHER_ORDER: 1 spatial walk order of the HexPlane gather, 0 index order
+    DevBuf order_buf;          // the walk order and the scratch that builds it (GatherOrderBuffers)
+    GatherOrderBuffers order{};
+    const float* order_xyz = nullptr;   // the Gaussians the order was built for (nullptr: none)
+    int64_t order_n = 0;
     WeightCache<FfmaWeights> packed;     // FFMA forward and backward
     WeightCache<TcWeights> tc;           // tensor-core forward (the weight fields and status of TcWeights)
     WeightCache<TcBwdWeights> tc_bwd;    // tensor-core backward
@@ -125,6 +130,7 @@ struct G4DContext {
     G4DWorkspace* ws = nullptr;
     DevBuf cam, geom, bin, binaux, img, fused, gscratch, gdeform, trow, relu, feat;
     bool relu_saved = false;
+    int feat_cols = 0;                // F of the features in `feat` (when relu_saved)
     int64_t n = 0;
     int H = 0, W = 0, grid_x = 0, grid_y = 0;
     int64_t R = 0, capacity = 0;
@@ -293,6 +299,29 @@ struct DeformSetup {
     TcWeights tw;    // tc: weight images, range flag and debug counters; the caller adds its feat / relu_bits buffers
 };
 
+// The walk order of the HexPlane gather over xyz [n] into *out (NULL: index order).  Rebuilt when the xyz pointer or n
+// changes, kept otherwise -- also when xyz moved in place (a training step): the features do not depend on the order, so a
+// stale one is still right and only costs L1 hits, but one built for another n is never used.  The rebuild is ordinary launches
+// in stream order behind the earlier forwards that read the order (like the workspace's other buffers), issued ahead of the
+// dependent chain of the forward that follows (DESIGN.md §4.6).
+int gather_order(G4DWorkspace* ws, const float* aabb, const float* xyz, int64_t n, cudaStream_t st, const uint32_t** out) {
+    *out = nullptr;
+    if (!ws->gather_order || n <= 0) return G4D_OK;
+    if (ws->order_xyz != xyz || ws->order_n != n) {
+        ws->order_xyz = nullptr;
+        GatherOrderBuffers& b = ws->order;
+        auto layout = [&](Carve& m) {
+            b.order = m.take<uint32_t>((size_t)n); b.key = m.take<uint2>((size_t)n);
+            b.cell_start = m.take<uint32_t>(kOrderCells); b.block_total = m.take<uint32_t>(kOrderCells / 1024);
+        };
+        G4D_CUDA(ensure_layout(ws->order_buf, layout));
+        G4D_CUDA(launch_gather_order(aabb, n, xyz, b, st));
+        ws->order_xyz = xyz; ws->order_n = n;
+    }
+    *out = ws->order.order;
+    return G4D_OK;
+}
+
 // the time planes interpolated at `time`, into `rows` (pointers in trow)
 int collapse_time_rows(DevBuf& rows, float* (*trow)[3], const G4DDeformParams* p, float time, cudaStream_t st) {
     const TimeRows tr(p->levels, p->res, p->channels);
@@ -302,13 +331,16 @@ int collapse_time_rows(DevBuf& rows, float* (*trow)[3], const G4DDeformParams* p
     return G4D_OK;
 }
 
-// Collapse the time rows, pick the forward's path from the params and bring the weight images that path reads up to date.
-// The desc is built after that refresh, which may move the transposes it embeds.
-int setup_deform(G4DWorkspace* ws, const G4DDeformParams* p, DevBuf& rows, float* (*trow)[3], float time, cudaStream_t st,
-                 DeformSetup* out) {
+// Pick the forward's path from the params, bring the gather's walk order over xyz [n] (tensor-core path) up to date, collapse
+// the time rows and bring the weight images the path reads up to date.  The desc is built after that refresh, which may move
+// the transposes it embeds.
+int setup_deform(G4DWorkspace* ws, const G4DDeformParams* p, const float* xyz, int64_t n, DevBuf& rows, float* (*trow)[3],
+                 float time, cudaStream_t st, DeformSetup* out) {
     int rc;
-    if ((rc = collapse_time_rows(rows, trow, p, time, st)) != G4D_OK) return rc;
     out->tc = ws->tensor_cores != 0 && tc_deform_supported(*p, ws->tensor_cores);
+    const uint32_t* order = nullptr;
+    if (out->tc && (rc = gather_order(ws, p->aabb, xyz, n, st, &order)) != G4D_OK) return rc;
+    if ((rc = collapse_time_rows(rows, trow, p, time, st)) != G4D_OK) return rc;
     if (!out->tc) {
         if ((rc = refresh_packed(ws, p, st)) != G4D_OK) return rc;
         out->d = make_desc(p, trow, &ws->packed.img);
@@ -317,6 +349,7 @@ int setup_deform(G4DWorkspace* ws, const G4DDeformParams* p, DevBuf& rows, float
     if ((rc = refresh_tc(ws, p, st)) != G4D_OK) return rc;
     out->d = make_desc(p, trow, nullptr);
     out->tw = ws->tc.img;
+    out->tw.order = order;
     if (ws->tc_debug) {   // per-CTA phase cycle counters (g4d_debug_tc_cycles)
         G4D_CUDA(ws->tc_dbg.ensure((size_t)ws->sm_count * 12 * 8));
         G4D_CUDA(cudaMemsetAsync(ws->tc_dbg.p, 0, (size_t)ws->sm_count * 12 * 8, st));
@@ -349,8 +382,10 @@ int deform_backward_dispatch(G4DWorkspace* ws, const G4DDeformParams* prm, float
         auto pack = [&](void* blob, TcBwdWeights* w) { return launch_tc_bwd_pack_weights(*prm, static_cast<uint8_t*>(blob), w, st); };
         G4D_CUDA(ws->tc_bwd.refresh(prm, 0, tc_bwd_weight_bytes(*prm), pack));
         const DeformDesc d = make_desc(prm, trow, nullptr);
+        const uint32_t* order = nullptr;   // the walk order of the backward's own gather (none when the forward's features are kept)
+        if (!saved_feat && (rc = gather_order(ws, prm->aabb, xyz, n, st, &order)) != G4D_OK) return rc;
         G4D_CUDA(ws->scratch.ensure(tc_deform_backward_scratch_bytes(d, n)));
-        G4D_CUDA(launch_deform_backward_tc(d, *prm, *grads, ws->tc_bwd.img, time, n, xyz, go, gi, relu_bits, saved_feat,
+        G4D_CUDA(launch_deform_backward_tc(d, *prm, *grads, ws->tc_bwd.img, time, n, xyz, go, gi, relu_bits, saved_feat, order,
                                            ws->scratch.as<uint8_t>(), ws->sm_count, st));
         return G4D_OK;
     }
@@ -520,6 +555,7 @@ G4DWorkspace* g4d_workspace_create(int device) {
     if (cudaSetDevice(device) != cudaSuccess) { fail(G4D_ERR_CUDA, "cudaSetDevice"); return nullptr; }
     G4DWorkspace* ws = new G4DWorkspace();
     ws->device = device;
+    if (const char* e = getenv("G4D_GATHER_ORDER")) ws->gather_order = atoi(e) != 0;
     cudaDeviceProp prop{};
     if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) ws->sm_count = prop.multiProcessorCount;
     if (cudaMallocHost((void**)&ws->pinned, sizeof(PinnedWords)) != cudaSuccess) { delete ws; fail(G4D_ERR_NOMEM, "cudaMallocHost"); return nullptr; }
@@ -567,6 +603,7 @@ int g4d_workspace_set_option(G4DWorkspace* ws, int option, int64_t value) {
         case G4D_OPT_TC_DEBUG: ws->tc_debug = value ? 1 : 0; return G4D_OK;
         case G4D_OPT_KEEP_DEFORMED: ws->keep_deformed = value ? 1 : 0; return G4D_OK;
         case G4D_OPT_PDL: g4d::g_pdl = value ? 1 : 0; return G4D_OK;
+        case G4D_OPT_GATHER_ORDER: ws->gather_order = value ? 1 : 0; return G4D_OK;
         default: return fail(G4D_ERR_ARG, "unknown option");
     }
 }
@@ -613,7 +650,7 @@ int g4d_deform_forward(G4DWorkspace* ws, const G4DDeformParams* prm, int64_t n, 
     G4D_CUDA(cudaSetDevice(ws->device));
     float* trow[G4D_MAX_LEVELS][3] = {};
     DeformSetup s{};
-    if ((rc = setup_deform(ws, prm, ws->trow, trow, time, st, &s)) != G4D_OK) return rc;
+    if ((rc = setup_deform(ws, prm, xyz, n, ws->trow, trow, time, st, &s)) != G4D_OK) return rc;
     if ((rc = attach_forward_buffers(ws, s, nullptr, relu_bits, n, st)) != G4D_OK) return rc;
     const DeformIO io{xyz, scaling, rotation, opacity, caller_sh<ShIn>(false, shs), out_xyz, out_scaling, out_rotation, out_opacity,
                       out_shs, GeomBuffers{}, FusedOutputs{}, nullptr};
@@ -756,6 +793,16 @@ int64_t g4d_context_read(G4DContext* c, int which, void* host_dst, int64_t bytes
             if (!c->bin_ctl) return fail(G4D_ERR_STATE, "no binning has run on this context");
             ok = pull(reinterpret_cast<const char*>(c->bin_ctl) + 16, 16 * 8); outv = tmp; outv.resize(16 * 8);
         } break;
+        case G4D_BUF_FEATURES: {
+            if (!c->is_fused || !c->deformed || !c->relu_saved) return fail(G4D_ERR_STATE, "G4D_BUF_FEATURES needs a grad-enabled tensor-core fused forward");
+            const size_t nb = N * (size_t)c->feat_cols * 4;
+            ok = pull(c->feat.p, nb); outv = tmp; outv.resize(nb);
+        } break;
+        case G4D_BUF_GATHER_ORDER: {
+            const G4DWorkspace* ws = c->ws;
+            const size_t nb = ws->order_xyz ? (size_t)ws->order_n * 4 : 0;
+            ok = pull(ws->order.order, nb); outv = tmp; outv.resize(nb);
+        } break;
         default: return fail(G4D_ERR_ARG, "unknown buffer id");
     }
     if (!ok) return fail(G4D_ERR_CUDA, "cudaMemcpy in g4d_context_read");
@@ -822,7 +869,7 @@ int fused_forward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* pr
     {
         StageTimer tm(c, G4D_STAGE_PREP, st);
         G4D_CUDA(launch_pack_camera(*cam, dcam, st));
-        if (prm && (rc = setup_deform(ws, prm, c->trow, c->trow_ptr, cam->time, st, &s)) != G4D_OK) return rc;
+        if (prm && (rc = setup_deform(ws, prm, g->xyz, n, c->trow, c->trow_ptr, cam->time, st, &s)) != G4D_OK) return rc;
     }
     {
         StageTimer tm(c, G4D_STAGE_GEOM, st);
@@ -834,6 +881,7 @@ int fused_forward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* pr
             if (c->relu_saved) {   // a backward will follow: it re-uses the ReLU signs and the staged HexPlane features
                 G4D_CUDA(c->relu.ensure(G4D_RELU_BITS_WORDS(n) * 4));
                 G4D_CUDA(c->feat.ensure((size_t)(n > 0 ? n : 1) * (size_t)s.d.F * 4 + 256));
+                c->feat_cols = s.d.F;
             }
             if ((rc = attach_forward_buffers(ws, s, c->relu_saved ? c->feat.as<float>() : nullptr,
                                              c->relu_saved ? c->relu.as<uint32_t>() : nullptr, n, st)) != G4D_OK) return rc;

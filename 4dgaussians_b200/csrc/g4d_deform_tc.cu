@@ -491,16 +491,97 @@ deform_tc_kernel(DeformDesc d, TcWeights tw, TcSmem Ls, const CameraDev* __restr
     if (dbg) { tw.dbg[blockIdx.x * 12] = clock64() - t_start; tw.dbg[blockIdx.x * 12 + 1] = t_wait; }
 }
 
+// ---- spatial walk order of the gather: a permutation of [0, n) in Z (Morton) order of each Gaussian's cell on a
+// kOrderGrid^3 grid over the normalised HexPlane coordinates.  Counting sort by cell: count (the atomic also hands each
+// Gaussian its rank inside its cell, in no particular order), exclusive scan of the counts, scatter.
+constexpr int kOrderBits = 6;   // 64 cells per axis: about as fine as level 0 of the planes (dynerf: 64)
+static_assert(kOrderCells == 1 << (3 * kOrderBits) && kOrderCells / 1024 == 256, "one scan CTA per 1024 cells, 256 of them");
+
+G4D_D uint32_t order_cell(const AabbNorm& nrm, const float* __restrict__ xyz, int64_t g) {
+    constexpr float hi = (float)((1 << kOrderBits) - 1);
+    uint32_t code = 0;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        // clamped as make_tap clamps: points outside the aabb, on its faces or with a NaN coordinate land in a valid cell
+        const float x = fminf(fmaxf((nrm(a, xyz[3 * g + a]) + 1.f) * (0.5f * (hi + 1.f)), 0.f), hi);
+        const uint32_t c = (uint32_t)x;
+#pragma unroll
+        for (int b = 0; b < kOrderBits; ++b) code |= ((c >> b) & 1u) << (3 * b + a);
+    }
+    return code;
+}
+
+// exclusive prefix sum of v over the 256 threads of the block (sm: 8 words of shared memory)
+G4D_D uint32_t block_exclusive_scan_256(uint32_t v, uint32_t* sm) {
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    uint32_t inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t y = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc += y;
+    }
+    if (lane == 31) sm[w] = inc;
+    __syncthreads();
+    uint32_t base = 0;
+    for (int i = 0; i < w; ++i) base += sm[i];
+    return base + inc - v;
+}
+
+__global__ void __launch_bounds__(256) order_count_kernel(const float* __restrict__ aabb, int64_t n, const float* __restrict__ xyz,
+                                                         GatherOrderBuffers b) {
+    const int64_t g = (int64_t)blockIdx.x * 256 + threadIdx.x;
+    if (g >= n) return;
+    const uint32_t c = order_cell(AabbNorm(aabb), xyz, g);
+    b.key[g] = make_uint2(c, atomicAdd(b.cell_start + c, 1u));
+}
+
+// per block of 1024 cells: counts -> exclusive prefix inside the block, and the block's total
+__global__ void __launch_bounds__(256) order_scan_kernel(GatherOrderBuffers b) {
+    __shared__ uint32_t sm[8];
+    uint4* p = reinterpret_cast<uint4*>(b.cell_start) + (size_t)blockIdx.x * 256 + threadIdx.x;
+    const uint4 c = *p;
+    const uint32_t s = c.x + c.y + c.z + c.w;
+    const uint32_t e = block_exclusive_scan_256(s, sm);
+    *p = make_uint4(e, e + c.x, e + c.x + c.y, e + c.x + c.y + c.z);
+    if (threadIdx.x == 255) b.block_total[blockIdx.x] = e + s;
+}
+
+__global__ void __launch_bounds__(256) order_scatter_kernel(int64_t n, GatherOrderBuffers b) {
+    __shared__ uint32_t sm[8], base[256];
+    base[threadIdx.x] = block_exclusive_scan_256(b.block_total[threadIdx.x], sm);
+    __syncthreads();
+    const int64_t g = (int64_t)blockIdx.x * 256 + threadIdx.x;
+    if (g >= n) return;
+    const uint2 k = b.key[g];
+    b.order[base[k.x >> 10] + b.cell_start[k.x] + k.y] = (uint32_t)g;
+}
+
+cudaError_t launch_gather_order(const float* aabb, int64_t n, const float* xyz, const GatherOrderBuffers& b, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    cudaError_t e = cudaMemsetAsync(b.cell_start, 0, (size_t)kOrderCells * 4, st);
+    if (e != cudaSuccess) return e;
+    const unsigned grid = (unsigned)((n + 255) / 256);
+    order_count_kernel<<<grid, 256, 0, st>>>(aabb, n, xyz, b);
+    order_scan_kernel<<<kOrderCells / 1024, 256, 0, st>>>(b);
+    order_scatter_kernel<<<grid, 256, 0, st>>>(n, b);
+    return cudaGetLastError();
+}
+
 // ---- HexPlane gather at full occupancy: C/4 threads per Gaussian, one channel vector each -> feat [N][F] fp32 -----------
-// (the forward chain launches it dependent on collapse_time_rows, the tensor-core backward as an ordinary launch)
+// (the forward chain launches it dependent on collapse_time_rows, the tensor-core backward as an ordinary launch).  Thread
+// group j gathers Gaussian order[j] (j itself when order is NULL): in spatial order the 8 Gaussians of a warp, and the warps
+// of an SM, tap neighbouring plane texels and share them in L1.  feat[g] depends on xyz[g] alone, so any order gives the
+// same bits.
 template <int C4>
-__global__ void __launch_bounds__(256) deform_features_kernel(DeformDesc d, int64_t n, const float* __restrict__ xyz, float* __restrict__ feat) {
+__global__ void __launch_bounds__(256) deform_features_kernel(DeformDesc d, int64_t n, const float* __restrict__ xyz,
+                                                              const uint32_t* __restrict__ order, float* __restrict__ feat) {
     pdl_wait();         // the collapsed time rows come from the previous kernel of the stream
     pdl_trigger();
     const int64_t t = (int64_t)blockIdx.x * 256 + threadIdx.x;
-    const int64_t g = t / C4;
+    const int64_t j = t / C4;
     const int v = (int)(t % C4);
-    if (g >= n) return;
+    if (j >= n) return;
+    const int64_t g = order ? (int64_t)__ldg(order + j) : j;
     const AabbNorm nrm(d.aabb);
     float pcs[3];
 #pragma unroll
@@ -513,12 +594,13 @@ __global__ void __launch_bounds__(256) deform_features_kernel(DeformDesc d, int6
     }
 }
 
-cudaError_t launch_deform_features(const DeformDesc& d, int64_t n, const float* xyz, float* feat, bool pdl, cudaStream_t st) {
+cudaError_t launch_deform_features(const DeformDesc& d, int64_t n, const float* xyz, const uint32_t* order, float* feat, bool pdl,
+                                   cudaStream_t st) {
     if (n == 0) return cudaSuccess;
     const int C4 = d.C / 4;
     const unsigned grid = (unsigned)((n * C4 + 255) / 256);
-    if (C4 == 4) return launch_k(deform_features_kernel<4>, dim3(grid), dim3(256), 0, st, pdl, d, n, xyz, feat);
-    if (C4 == 8) return launch_k(deform_features_kernel<8>, dim3(grid), dim3(256), 0, st, pdl, d, n, xyz, feat);
+    if (C4 == 4) return launch_k(deform_features_kernel<4>, dim3(grid), dim3(256), 0, st, pdl, d, n, xyz, order, feat);
+    if (C4 == 8) return launch_k(deform_features_kernel<8>, dim3(grid), dim3(256), 0, st, pdl, d, n, xyz, order, feat);
     return cudaErrorInvalidValue;
 }
 
@@ -549,7 +631,7 @@ cudaError_t launch_deform_tc(const DeformDesc& d, const TcWeights& tw, int mode,
     if (n == 0) return cudaSuccess;
     if (!tw.feat) return cudaErrorInvalidValue;
     {
-        cudaError_t e = launch_deform_features(d, n, io.xyz, tw.feat, true, st);
+        cudaError_t e = launch_deform_features(d, n, io.xyz, tw.order, tw.feat, true, st);
         if (e != cudaSuccess) return e;
     }
     const TcSmem Ls = tc_smem_layout(tw.arith, d.F, (d.head_mask & G4D_HEAD_SHS) != 0);

@@ -682,8 +682,8 @@ static cudaError_t launch_a(const BwdADesc& bd, int64_t n, int sm_count, cudaStr
 cudaError_t launch_deform_backward_tc(const DeformDesc& d, const G4DDeformParams& prm, const G4DDeformGrads& grads,
                                       const TcBwdWeights& w, float time, int64_t n, const float* xyz,
                                       const float* const go[G4D_NUM_HEADS], float* const gi[G4D_NUM_HEADS],
-                                      const uint32_t* relu_bits, const float* saved_feat, uint8_t* scratch, int sm_count,
-                                      cudaStream_t st) {
+                                      const uint32_t* relu_bits, const float* saved_feat, const uint32_t* order, uint8_t* scratch,
+                                      int sm_count, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
     const int64_t ntiles = (n + 127) / 128;
     const TimeRows tr(d.levels, d.res, d.C);
@@ -702,7 +702,7 @@ cudaError_t launch_deform_backward_tc(const DeformDesc& d, const G4DDeformParams
     cudaError_t e = cudaMemsetAsync(s.trow_grad, 0, tr.total() * 4, st);
     if (e != cudaSuccess) return e;
     // the forward's gather (skipped when the forward's feature staging buffer was kept for this backward)
-    if (!saved_feat && (e = launch_deform_features(d, n, xyz, s.feat, false, st)) != cudaSuccess) return e;
+    if (!saved_feat && (e = launch_deform_features(d, n, xyz, order, s.feat, false, st)) != cudaSuccess) return e;
     if (d.C == 16 && d.levels == 2) e = launch_a<16, 2>(a, n, sm_count, st);
     else if (d.C == 16 && d.levels == 3) e = launch_a<16, 3>(a, n, sm_count, st);
     else if (d.C == 32 && d.levels == 2) e = launch_a<32, 2>(a, n, sm_count, st);

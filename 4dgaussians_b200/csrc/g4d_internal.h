@@ -200,7 +200,8 @@ struct TcWeights {
     const float* w2[G4D_NUM_HEADS];    // SH head only: packed (hi | lo), [48][128]
     long long* dbg;                    // optional [grid][12] per-phase cycle counters (debug)
     float* feat;                       // [N][F] fp32 staging of the HexPlane features (deform_features_kernel)
-    uint32_t* relu_bits;               // optional [6][N][4]: ReLU sign bits saved for the backward (G4D_RELU_BITS_WORDS)
+    const uint32_t* order;             // optional [N]: the gather's walk order (launch_gather_order); NULL: index order
+    uint32_t* relu_bits;             // optional [6][N][4]: ReLU sign bits saved for the backward (G4D_RELU_BITS_WORDS)
     int arith;                         // 1: 3xTF32, 2: FP16x2 (G4D_OPT_TENSOR_CORES)
     uint32_t* status;                  // host-mapped word: set to 1 by the FP16x2 kernel when a value left the f16 operand range
 };
@@ -208,8 +209,21 @@ struct TcWeights {
 size_t tc_packed_floats(const G4DDeformParams& prm);
 cudaError_t launch_tc_pack_weights(const G4DDeformParams& prm, int arith, float* blob, TcWeights* out, cudaStream_t st);
 bool tc_deform_supported(const G4DDeformParams& prm, int arith);
-// HexPlane gather xyz -> feat [N][F] fp32; pdl: launched dependent on the previous kernel of the forward chain (DESIGN.md §4.6)
-cudaError_t launch_deform_features(const DeformDesc& d, int64_t n, const float* xyz, float* feat, bool pdl, cudaStream_t st);
+// HexPlane gather xyz -> feat [N][F] fp32, Gaussians visited in `order` (NULL: index order; feat[g] stays at row g either
+// way); pdl: launched dependent on the previous kernel of the forward chain (DESIGN.md §4.6)
+cudaError_t launch_deform_features(const DeformDesc& d, int64_t n, const float* xyz, const uint32_t* order, float* feat, bool pdl,
+                                   cudaStream_t st);
+// The gather's spatial walk order (DESIGN.md §4.1): order [n] = a permutation of [0, n) in Z order of the Gaussians' cells on a
+// 64^3 grid over the normalised HexPlane coordinates, and the scratch of the counting sort that builds it.
+constexpr int kOrderCells = 1 << 18;
+struct GatherOrderBuffers {
+    uint32_t* order;         // [n]
+    uint2* key;              // [n] (cell, rank inside the cell)
+    uint32_t* cell_start;    // [kOrderCells] counts, then exclusive prefix inside each block of 1024 cells
+    uint32_t* block_total;   // [kOrderCells / 1024]
+};
+// memset + 3 ordinary launches; aabb as in DeformDesc
+cudaError_t launch_gather_order(const float* aabb, int64_t n, const float* xyz, const GatherOrderBuffers& b, cudaStream_t st);
 
 // tensor-core backward (g4d_deform_tc_bwd.cu): BF16 (hi | lo) weight images in the 8x8-core layout of tc_wgmma.cuh
 struct TcBwdWeights {
@@ -224,8 +238,8 @@ size_t tc_deform_backward_scratch_bytes(const DeformDesc& d, int64_t n);   // si
 cudaError_t launch_deform_backward_tc(const DeformDesc& d, const G4DDeformParams& prm, const G4DDeformGrads& grads,
                                       const TcBwdWeights& w, float time, int64_t n, const float* xyz,
                                       const float* const go[G4D_NUM_HEADS], float* const gi[G4D_NUM_HEADS],
-                                      const uint32_t* relu_bits, const float* saved_feat, uint8_t* scratch, int sm_count,
-                                      cudaStream_t st);
+                                      const uint32_t* relu_bits, const float* saved_feat, const uint32_t* order, uint8_t* scratch,
+                                      int sm_count, cudaStream_t st);
 // collapsed time-row gradients -> the two time rows of each (axis, t) plane (g4d_backward.cu)
 cudaError_t launch_distribute_time_grad(const DeformDesc& d, float* const (*trow_grad)[3], float* const (*g_planes)[6], float time,
                                         cudaStream_t st);

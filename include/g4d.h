@@ -252,9 +252,13 @@ enum { G4D_OPT_SYNC_MODE = 1,  /* 1 (default): size the instance buffer exactly 
                                    * (G4D_BUF_DEFORMED / _SHS reads); default 0: it skips those 48-240 B / Gaussian of writes */
        G4D_OPT_WARP_CULL = 7,    /* 1 (default): the blend kernels skip, per warp, instances that cannot reach alpha >= 1/255
                                   *    on any pixel of the warp's 16 x 4 strip (results unchanged); 0 = test every pixel */
-       G4D_OPT_PDL = 9           /* 1 (default): the kernels of a forward are launched programmatically dependent on one another
+       G4D_OPT_PDL = 9,          /* 1 (default): the kernels of a forward are launched programmatically dependent on one another
                                   *    (a kernel's set-up overlaps the tail of its predecessor; results unchanged); 0: ordinary
-                                  *    stream order.  PROCESS-wide, not per workspace (also: environment G4D_PDL=0) */ };
+                                  *    stream order.  PROCESS-wide, not per workspace (also: environment G4D_PDL=0) */
+       G4D_OPT_GATHER_ORDER = 10 /* 1 (default): the tensor-core path gathers the HexPlane features of the Gaussians in a spatial
+                                  *    (Z) order, built on the device when the xyz pointer or N changes and kept otherwise (results
+                                  *    unchanged: every Gaussian's features come from its own taps); 0: index order.  Per workspace;
+                                  *    a workspace created with G4D_GATHER_ORDER=0 in the environment starts at 0 */ };
 int g4d_workspace_set_option(G4DWorkspace *ws, int option, int64_t value);
 
 /* copy an internal per-forward buffer to HOST memory (tests / debugging; synchronises).
@@ -273,9 +277,13 @@ enum { G4D_BUF_DEPTH = 1,      /* float  [N]  view-space depth                  
        G4D_BUF_CLAMPED = 12,   /* uint8  [N,3]                                    */
        G4D_BUF_DEFORMED = 13,  /* float  [N,11] (xyz, scale, rot, opacity) post-activation, fused path */
        G4D_BUF_DEFORMED_SHS = 14, /* float [N,48] deformed SH coefficients (fused path with the SHS head active) */
-       G4D_BUF_BIN_PHASES = 15 /* int64 [16] profiling: SM clock of CTA 0 at the phase boundaries of bin_sort (0 start,
+       G4D_BUF_BIN_PHASES = 15, /* int64 [16] profiling: SM clock of CTA 0 at the phase boundaries of bin_sort (0 start,
                                   1 after the key range, 2 after the depth sort, 3 after chunking, 4 after counting,
-                                  5 end), [15] = significant key bits */ };
+                                  5 end), [15] = significant key bits */
+       G4D_BUF_FEATURES = 16,  /* float [N,F] HexPlane features staged by a grad-enabled tensor-core fused forward */
+       G4D_BUF_GATHER_ORDER = 17 /* uint32 [N'] the workspace's walk order of the HexPlane gather (G4D_OPT_GATHER_ORDER), built
+                                  for the last N' Gaussians it was rebuilt for; 0 bytes when none was built.  The order of the
+                                  Gaussians inside one grid cell may differ from one build to the next */ };
 int64_t g4d_context_read(G4DContext *ctx, int which, void *host_dst, int64_t bytes);
 
 /* per-stage device time (ms) of the LAST forward / backward on this context, measured with CUDA events on the
