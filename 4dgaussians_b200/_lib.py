@@ -37,6 +37,8 @@ ABI_SYMBOLS = [
     "g4d_rasterize_backward", "g4d_render_forward", "g4d_render_backward", "g4d_workspace_set_option", "g4d_context_read",
     "g4d_context_stage_times", "g4d_debug_tc_cycles", "g4d_l1_loss", "g4d_l1_loss_backward", "g4d_ssim", "g4d_ssim_backward",
     "g4d_plane_regulation", "g4d_dist2_knn3", "g4d_adam_step", "g4d_render_forward_cameras", "g4d_render_backward_cameras",
+    "g4d_context_set_time_source", "g4d_workspace_freeze", "g4d_workspace_graph_status", "g4d_adam_scalars",
+    "g4d_adam_step_device",
 ]
 
 fp = C.c_void_p   # device pointers travel as integers
@@ -81,6 +83,15 @@ class GaussianGrads(C.Structure):
 
 class AdamSegment(C.Structure):
     _fields_ = [("begin", C.c_int64), ("end", C.c_int64), ("lr", C.c_float), ("reserved", C.c_float)]
+
+
+class AdamScalars(C.Structure):
+    _fields_ = [("lr", C.c_float * 16), ("inv_bc1", C.c_float), ("inv_sqrt_bc2", C.c_float), ("grad_scale", C.c_float),
+                ("reserved", C.c_float)]
+
+
+class GraphStatus(C.Structure):
+    _fields_ = [("overflows", C.c_int64), ("max_instances", C.c_int64), ("f16_range", C.c_int32), ("reserved", C.c_int32)]
 
 
 class Stats(C.Structure):
@@ -147,6 +158,13 @@ def load():
         lib.g4d_adam_step.argtypes = [C.c_void_p, fp, fp, fp, fp, C.c_int64, C.POINTER(AdamSegment), C.c_int32, C.c_float, C.c_float,
                                       C.c_float, C.c_int64, C.c_float, C.c_void_p]
         lib.g4d_dist2_knn3.argtypes = [C.c_void_p, C.c_int64, fp, fp, C.c_void_p]
+        lib.g4d_context_set_time_source.argtypes = [C.c_void_p, fp]
+        lib.g4d_workspace_freeze.argtypes = [C.c_void_p, C.c_int]
+        lib.g4d_workspace_graph_status.argtypes = [C.c_void_p, C.c_int, C.POINTER(GraphStatus)]
+        lib.g4d_adam_scalars.argtypes = [C.POINTER(AdamSegment), C.c_int32, C.c_float, C.c_float, C.c_int64, C.c_float,
+                                         C.POINTER(AdamScalars)]
+        lib.g4d_adam_step_device.argtypes = [C.c_void_p, fp, fp, fp, fp, C.c_int64, C.POINTER(AdamSegment), C.c_int32, C.c_float,
+                                             C.c_float, C.c_float, fp, C.c_void_p]
         if lib.g4d_abi_version() != ABI_VERSION:
             raise G4DError("libg4d.so ABI version mismatch")
         _lib = lib
@@ -172,7 +190,9 @@ def check(rc: int, what: str = "g4d"):
 
 
 class Workspace:
-    """One per (process, device).  Owns scratch memory and the packed-weight cache."""
+    """One per (process, device) through ``get``.  Owns scratch memory and the packed-weight cache.  ``Workspace(device)``
+    makes a private one, destroyed with its last reference (a CUDA graph owns one, so that eager calls on the shared
+    workspace can never move a buffer the graph points at)."""
     _by_device: Dict[int, "Workspace"] = {}
 
     def __init__(self, device: int):
@@ -190,6 +210,27 @@ class Workspace:
             ws = cls(int(device))
             cls._by_device[int(device)] = ws
         return ws
+
+    def freeze(self, on: bool = True):
+        """While frozen, a call that would reallocate a buffer of this workspace or of its contexts raises (G4D_ERR_STATE)."""
+        check(load().g4d_workspace_freeze(self.handle, int(bool(on))), "g4d_workspace_freeze")
+
+    def graph_status(self, sync: bool = True) -> GraphStatus:
+        """Read and clear the overflow / FP16-range record of the forwards captured on this workspace."""
+        s = GraphStatus()
+        check(load().g4d_workspace_graph_status(self.handle, int(bool(sync)), C.byref(s)), "g4d_workspace_graph_status")
+        return s
+
+    def __del__(self):
+        try:
+            if self.handle and _lib is not None and self._by_device.get(self.device) is not self:
+                for ctx in self._free_contexts:     # (a cycle: the pool's contexts may be collected after their workspace)
+                    ctx.__del__()
+                self._free_contexts = []
+                _lib.g4d_workspace_destroy(self.handle)
+                self.handle = None
+        except Exception:
+            pass
 
     def set_option(self, option: int, value: int):
         check(load().g4d_workspace_set_option(self.handle, option, int(value)), "g4d_workspace_set_option")
@@ -214,6 +255,10 @@ class Context:
         self.handle = load().g4d_context_create(ws.handle)
         if not self.handle:
             raise G4DError("g4d_context_create: %s" % load().g4d_last_error().decode())
+
+    def set_time_source(self, d_time: Optional[int]):
+        """Read the timestamp of every forward / backward on this context from the device float at d_time (None: the camera's)."""
+        check(load().g4d_context_set_time_source(self.handle, d_time), "g4d_context_set_time_source")
 
     def stats(self) -> Stats:
         s = Stats()

@@ -16,15 +16,28 @@ namespace {
 
 thread_local std::string t_last_error;
 
+// What the entry point running on this thread allows (CallScope): while its stream captures a CUDA graph nothing may run that
+// a replay could not repeat, and while its workspace is frozen or its stream captures no buffer may be reallocated (a graph
+// keeps the addresses it captured).
+// growth_refused: set by the DevBuf::ensure that refused, so that its caller reports the refusal and not a CUDA error.
+struct CallState { bool capturing = false, no_growth = false, growth_refused = false; };
+thread_local CallState t_call;
+
 int fail(int code, const char* what, const char* detail = nullptr) {
     t_last_error = what;
     if (detail) { t_last_error += ": "; t_last_error += detail; }
     return code;
 }
 
+int growth_refused(const char* what) {
+    t_call.growth_refused = false;
+    return fail(G4D_ERR_STATE, "a buffer would have to grow while the workspace is frozen or the stream is capturing", what);
+}
+
 #define G4D_CUDA(expr)                                                                      \
     do {                                                                                    \
         cudaError_t e__ = (expr);                                                           \
+        if (e__ != cudaSuccess && t_call.growth_refused) return growth_refused(#expr);      \
         if (e__ != cudaSuccess) {                                                           \
             char buf__[64];                                                                 \
             snprintf(buf__, sizeof(buf__), " (%s:%d)", __FILE__, __LINE__);                 \
@@ -33,7 +46,8 @@ int fail(int code, const char* what, const char* detail = nullptr) {
         }                                                                                   \
     } while (0)
 
-// device memory that grows by 1.5x on demand and is freed with its owner (on the owner's device)
+// device memory that grows by 1.5x on demand and is freed with its owner (on the owner's device); it refuses to grow (and
+// frees nothing) under t_call.no_growth
 struct DevBuf {
     void* p = nullptr;
     size_t cap = 0;
@@ -44,6 +58,7 @@ struct DevBuf {
     ~DevBuf() { if (p) cudaFree(p); }
     cudaError_t ensure(size_t bytes) {
         if (bytes <= cap) return cudaSuccess;
+        if (t_call.no_growth) { t_call.growth_refused = true; return cudaErrorNotPermitted; }
         size_t want = bytes + bytes / 2 + 256;
         if (p) { cudaError_t e = cudaFree(p); p = nullptr; cap = 0; if (e != cudaSuccess) return e; }
         cudaError_t e = cudaMalloc(&p, want);
@@ -82,9 +97,10 @@ struct WeightCache {
     const void* key = nullptr;
     int arith = 0;
     bool valid = false;
-    // pack(buf.p, &img) (re)builds the images unless they were built from these parameters
+    // pack(buf.p, &img) (re)builds the images unless they were built from these parameters; a capture always rebuilds them,
+    // so that every replay packs the parameters as they are then
     template <class Pack> cudaError_t refresh(const G4DDeformParams* p, int arith_, size_t bytes, Pack pack) {
-        if (valid && version == p->version && key == (const void*)p->w0 && arith == arith_) return cudaSuccess;
+        if (valid && !t_call.capturing && version == p->version && key == (const void*)p->w0 && arith == arith_) return cudaSuccess;
         valid = false;
         cudaError_t e = buf.ensure(bytes);
         if (e == cudaSuccess) e = pack(buf.p, &img);
@@ -94,9 +110,10 @@ struct WeightCache {
     }
 };
 
-// pinned host words of a workspace: the exact-mode read-back of R, and the flag an FP16x2 tensor-core kernel sets (through
-// the host mapping) when a value left the f16 operand range
-struct PinnedWords { uint32_t num_rendered, pad0[7], f16_range, pad1[7]; };
+// pinned host words of a workspace: the exact-mode read-back of R, the flag an FP16x2 tensor-core kernel sets (through
+// the host mapping) when a value left the f16 operand range, and the overflow record of captured forwards (count, largest
+// R: launch_record_overflow)
+struct PinnedWords { uint32_t num_rendered, pad0[7], f16_range, pad1[7], overflow[2], pad2[6]; };
 
 }  // namespace
 
@@ -112,6 +129,7 @@ struct G4DWorkspace {
     int keep_deformed = 0;
     int tc_debug = 0;
     int gather_order = 1;      // G4D_OPT_GATHER_ORDER: 1 spatial walk order of the HexPlane gather, 0 index order
+    int frozen = 0;            // g4d_workspace_freeze
     DevBuf order_buf;          // the walk order and the scratch that builds it (GatherOrderBuffers)
     GatherOrderBuffers order{};
     const float* order_xyz = nullptr;   // the Gaussians the order was built for (nullptr: none)
@@ -134,6 +152,7 @@ struct G4DContext {
     int64_t n = 0;
     int H = 0, W = 0, grid_x = 0, grid_y = 0;
     int64_t R = 0, capacity = 0;
+    const float* time_src = nullptr;  // g4d_context_set_time_source (device; NULL: G4DCamera.time)
     const void* bin_ctl = nullptr;    // device BinCtl of the last forward
     bool learned = false;             // R of an earlier exact forward is known (no-sync mode needs a learnt capacity)
     bool has_forward = false, is_fused = false, fused_sh = false, deformed = false, fo_valid = false;
@@ -188,6 +207,43 @@ struct StageTimer {
     }
 };
 void reset_stage_flags(G4DContext* c, int first, int last) { for (int i = first; i <= last; ++i) c->ev_used[i] = false; }
+
+// t_call for one entry point on workspace ws and stream st, restored when it returns; rc != G4D_OK when the capture status
+// of st cannot be read
+struct CallScope {
+    CallState saved;
+    int rc = G4D_OK;
+    CallScope(const G4DWorkspace* ws, cudaStream_t st) : saved(t_call) {
+        cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+        const cudaError_t e = cudaStreamIsCapturing(st, &cs);
+        if (e != cudaSuccess) {
+            (void)cudaGetLastError();
+            rc = fail(G4D_ERR_STATE, "cudaStreamIsCapturing", cudaGetErrorString(e));
+        }
+        t_call.capturing = cs != cudaStreamCaptureStatusNone;
+        t_call.no_growth = ws->frozen || t_call.capturing;
+        t_call.growth_refused = false;
+    }
+    ~CallScope() { t_call = saved; }
+};
+
+// What a capture refuses, checked before any launch: host events (stage timing), host syncs (G4D_CAM_DEBUG) and, for a
+// forward on the contexts fwd[0, k), the exact-mode read-back of R and a capacity that has not been learnt yet.
+int refuse_capture(const G4DWorkspace* ws, const G4DCamera* cams, int k, G4DContext* const* fwd) {
+    if (!t_call.capturing) return G4D_OK;
+    if (ws->stage_timing) return fail(G4D_ERR_STATE, "cannot capture with G4D_OPT_STAGE_TIMING: it records host-managed events");
+    for (int i = 0; i < k; ++i)
+        if (cams[i].debug & G4D_CAM_DEBUG) return fail(G4D_ERR_STATE, "cannot capture with G4D_CAM_DEBUG: it synchronises after every stage");
+    if (!fwd) return G4D_OK;
+    if (ws->sync_mode)
+        return fail(G4D_ERR_STATE, "cannot capture a forward in exact sync mode (G4D_OPT_SYNC_MODE = 1): it reads the instance count "
+                                   "back on the host; set the option to 0");
+    for (int i = 0; i < k; ++i)
+        if (!fwd[i]->learned || fwd[i]->capacity <= 0)
+            return fail(G4D_ERR_STATE, "cannot capture a forward on a context that has not learnt its instance capacity: run one "
+                                       "forward on it outside the capture first");
+    return G4D_OK;
+}
 
 int ensure_geom(G4DContext* c, int64_t n) {
     const size_t N = (size_t)(n > 0 ? n : 1);
@@ -261,7 +317,7 @@ int refresh_packed(G4DWorkspace* ws, const G4DDeformParams* p, cudaStream_t st) 
 
 int refresh_tc(G4DWorkspace* ws, const G4DDeformParams* p, cudaStream_t st) {
     const int arith = ws->tensor_cores == 2 ? 2 : 1;
-    if (arith == 2 && ws->pinned->f16_range) {
+    if (arith == 2 && !t_call.capturing && ws->pinned->f16_range) {   // (a capture leaves the flag to g4d_workspace_graph_status)
         ws->pinned->f16_range = 0;
         ws->tc.valid = false;      // re-pack (and re-check) the weights on the next call: they may be the out-of-range values
         return fail(G4D_ERR_OVERFLOW, "an earlier FP16x2 tensor-core launch met a value outside the f16 operand range (activation >= 8188, "
@@ -323,9 +379,10 @@ int gather_order(G4DWorkspace* ws, const float* aabb, const float* xyz, int64_t 
 }
 
 // the time planes interpolated at `time`, into `rows` (pointers in trow)
-int collapse_time_rows(DevBuf& rows, float* (*trow)[3], const G4DDeformParams* p, float time, cudaStream_t st) {
+int collapse_time_rows(DevBuf& rows, float* (*trow)[3], const G4DDeformParams* p, TimeArg time, cudaStream_t st) {
     const TimeRows tr(p->levels, p->res, p->channels);
-    if (rows.ensure(tr.total() * 4) != cudaSuccess) return fail(G4D_ERR_NOMEM, "time-row buffer");
+    if (rows.ensure(tr.total() * 4) != cudaSuccess)
+        return t_call.growth_refused ? growth_refused("time-row buffer") : fail(G4D_ERR_NOMEM, "time-row buffer");
     tr.place(rows.as<float>(), trow);
     G4D_CUDA(launch_collapse_time_rows(*p, time, trow, st));
     return G4D_OK;
@@ -335,7 +392,7 @@ int collapse_time_rows(DevBuf& rows, float* (*trow)[3], const G4DDeformParams* p
 // the time rows and bring the weight images the path reads up to date.  The desc is built after that refresh, which may move
 // the transposes it embeds.
 int setup_deform(G4DWorkspace* ws, const G4DDeformParams* p, const float* xyz, int64_t n, DevBuf& rows, float* (*trow)[3],
-                 float time, cudaStream_t st, DeformSetup* out) {
+                 TimeArg time, cudaStream_t st, DeformSetup* out) {
     int rc;
     out->tc = ws->tensor_cores != 0 && tc_deform_supported(*p, ws->tensor_cores);
     const uint32_t* order = nullptr;
@@ -375,7 +432,7 @@ int attach_forward_buffers(G4DWorkspace* ws, DeformSetup& s, float* feat, uint32
 // backward of the deformation network with the time rows trow: tensor-core path when the configuration allows, FFMA path
 // otherwise; the desc is built after the weight images of that path are current
 int deform_backward_dispatch(G4DWorkspace* ws, const G4DDeformParams* prm, float* const (*trow)[3], const G4DDeformGrads* grads,
-                             float time, int64_t n, const float* xyz, const float* const go[G4D_NUM_HEADS],
+                             TimeArg time, int64_t n, const float* xyz, const float* const go[G4D_NUM_HEADS],
                              float* const gi[G4D_NUM_HEADS], const uint32_t* relu_bits, const float* saved_feat, cudaStream_t st) {
     int rc;
     if (ws->tensor_cores && tc_backward_supported(*prm)) {
@@ -415,6 +472,7 @@ int debug_sync(const G4DCamera* cam, cudaStream_t st, const char* stage) {
 
 // no-sync mode: the previous forward's instance count arrives asynchronously; look at it before reusing the context
 int check_pending(G4DContext* c) {
+    if (t_call.capturing) return G4D_OK;   // (no host reads in a capture: its overflows go to g4d_workspace_graph_status)
     for (int k = 0; k < G4DContext::kSlots; ++k) {
         const int s = (c->slot + k) % G4DContext::kSlots;   // k = 0: the slot about to be reused (oldest forward: must be resolved), then the newer ones
         if (!c->pending[s]) continue;
@@ -448,6 +506,7 @@ int bin_and_blend(G4DContext* c, const G4DCamera* cam, int64_t n, float* out_col
     const int num_tiles = c->grid_x * c->grid_y;
     const uint32_t kNoCap = 0xFFFFFFFFu;
     const uint32_t* readback = nullptr;
+    uint32_t cap_place = 0;
     if (n > 0) {
         if (ws->sm_count > 1024) return fail(G4D_ERR_ARG, "more than 1024 SMs are not supported by the binning kernel");
         G4D_CUDA(c->binaux.ensure(bin_aux_bytes(n, num_tiles, ws->sm_count)));
@@ -479,7 +538,7 @@ int bin_and_blend(G4DContext* c, const G4DCamera* cam, int64_t n, float* out_col
         if ((rc = debug_sync(cam, st, "bin_sort")) != G4D_OK) return rc;
         {
             StageTimer tm(c, G4D_STAGE_EMIT, st);
-            const uint32_t cap_place = (uint32_t)(c->capacity < (int64_t)kNoCap ? c->capacity : (int64_t)kNoCap);
+            cap_place = (uint32_t)(c->capacity < (int64_t)kNoCap ? c->capacity : (int64_t)kNoCap);
             G4D_CUDA(launch_bin_place(c->grid_x, c->grid_y, c->g, lay, c->b.ids_sorted, c->b.kbuf, c->b.ranges, cap_place, ws->tight_cull, st));
         }
     } else {
@@ -492,7 +551,9 @@ int bin_and_blend(G4DContext* c, const G4DCamera* cam, int64_t n, float* out_col
         StageTimer tm(c, G4D_STAGE_BLEND, st);
         G4D_CUDA(launch_blend_forward(dcam, c->grid_x, c->grid_y, c->g, c->b, c->im, out_color, out_depth, ws->warp_cull, st));
     }
-    if (readback) {
+    if (readback && t_call.capturing) {
+        G4D_CUDA(launch_record_overflow(static_cast<const BinCtl*>(c->bin_ctl), cap_place, ws->pinned->overflow, st));
+    } else if (readback) {
         const int sl = c->slot;
         c->slot = (c->slot + 1) % G4DContext::kSlots;
         G4D_CUDA(cudaMemcpyAsync(c->h_r + sl, readback, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
@@ -648,9 +709,11 @@ int g4d_deform_forward(G4DWorkspace* ws, const G4DDeformParams* prm, int64_t n, 
     if ((prm->head_mask & G4D_HEAD_SHS) && n > 0 && (!shs || !out_shs)) return fail(G4D_ERR_ARG, "shs / out_shs required when the SHS head is active");
     cudaStream_t st = (cudaStream_t)stream;
     G4D_CUDA(cudaSetDevice(ws->device));
+    CallScope scope(ws, st);
+    if (scope.rc != G4D_OK) return scope.rc;
     float* trow[G4D_MAX_LEVELS][3] = {};
     DeformSetup s{};
-    if ((rc = setup_deform(ws, prm, xyz, n, ws->trow, trow, time, st, &s)) != G4D_OK) return rc;
+    if ((rc = setup_deform(ws, prm, xyz, n, ws->trow, trow, TimeArg{time, nullptr}, st, &s)) != G4D_OK) return rc;
     if ((rc = attach_forward_buffers(ws, s, nullptr, relu_bits, n, st)) != G4D_OK) return rc;
     const DeformIO io{xyz, scaling, rotation, opacity, caller_sh<ShIn>(false, shs), out_xyz, out_scaling, out_rotation, out_opacity,
                       out_shs, GeomBuffers{}, FusedOutputs{}, nullptr};
@@ -671,6 +734,9 @@ int g4d_rasterize_forward(G4DContext* c, const G4DCamera* cam, int64_t n, const 
     if (n >= (1ll << 31)) return fail(G4D_ERR_ARG, "n too large");
     cudaStream_t st = (cudaStream_t)stream;
     G4D_CUDA(cudaSetDevice(c->ws->device));
+    CallScope scope(c->ws, st);
+    if (scope.rc != G4D_OK) return scope.rc;
+    if ((rc = refuse_capture(c->ws, cam, 1, &c)) != G4D_OK) return rc;
     if ((rc = check_pending(c)) != G4D_OK) return rc;
     c->has_forward = false; c->is_fused = false; c->deformed = false; c->group = 0;
     if ((rc = ensure_geom(c, n)) != G4D_OK) return rc;
@@ -678,7 +744,7 @@ int g4d_rasterize_forward(G4DContext* c, const G4DCamera* cam, int64_t n, const 
     reset_stage_flags(c, 0, G4D_STAGE_COUNT - 1);
     {
         StageTimer tm(c, G4D_STAGE_PREP, st);
-        G4D_CUDA(launch_pack_camera(*cam, c->cam.as<CameraDev>(), st));
+        G4D_CUDA(launch_pack_camera(*cam, nullptr, c->cam.as<CameraDev>(), st));
     }
     const RasterInputs in{means3D, scales, rotations, opacities, caller_sh<ShIn>(false, shs)};
     {
@@ -701,6 +767,9 @@ int g4d_rasterize_backward(G4DContext* c, const G4DCamera* cam, int64_t n, const
         return fail(G4D_ERR_ARG, "NULL gradient pointer");
     cudaStream_t st = (cudaStream_t)stream;
     G4D_CUDA(cudaSetDevice(c->ws->device));
+    CallScope scope(c->ws, st);
+    if (scope.rc != G4D_OK) return scope.rc;
+    if ((rc = refuse_capture(c->ws, cam, 1, nullptr)) != G4D_OK) return rc;
     if ((rc = check_pending(c)) != G4D_OK) return rc;
     (void)opacities;
     const RasterInputs in{means3D, scales, rotations, opacities, caller_sh<ShIn>(false, shs)};
@@ -823,11 +892,13 @@ int g4d_deform_backward(G4DWorkspace* ws, const G4DDeformParams* prm, G4DDeformG
     if (n < 0 || (n > 0 && !xyz)) return fail(G4D_ERR_ARG, "xyz required");
     cudaStream_t st = (cudaStream_t)stream;
     G4D_CUDA(cudaSetDevice(ws->device));
+    CallScope scope(ws, st);
+    if (scope.rc != G4D_OK) return scope.rc;
     float* trow[G4D_MAX_LEVELS][3] = {};
-    if ((rc = collapse_time_rows(ws->trow, trow, prm, time, st)) != G4D_OK) return rc;
+    if ((rc = collapse_time_rows(ws->trow, trow, prm, TimeArg{time, nullptr}, st)) != G4D_OK) return rc;
     const float* go[G4D_NUM_HEADS] = {g_out_xyz, g_out_scaling, g_out_rotation, g_out_opacity, g_out_shs};
     float* gi[G4D_NUM_HEADS] = {g_in_xyz, g_in_scaling, g_in_rotation, g_in_opacity, g_in_shs};
-    return deform_backward_dispatch(ws, prm, trow, grads, time, n, xyz, go, gi, relu_bits, nullptr, st);
+    return deform_backward_dispatch(ws, prm, trow, grads, TimeArg{time, nullptr}, n, xyz, go, gi, relu_bits, nullptr, st);
 }
 
 }  // extern "C"
@@ -868,8 +939,9 @@ int fused_forward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* pr
     DeformSetup s{};
     {
         StageTimer tm(c, G4D_STAGE_PREP, st);
-        G4D_CUDA(launch_pack_camera(*cam, dcam, st));
-        if (prm && (rc = setup_deform(ws, prm, g->xyz, n, c->trow, c->trow_ptr, cam->time, st, &s)) != G4D_OK) return rc;
+        G4D_CUDA(launch_pack_camera(*cam, c->time_src, dcam, st));
+        if (prm && (rc = setup_deform(ws, prm, g->xyz, n, c->trow, c->trow_ptr, TimeArg{cam->time, c->time_src}, st, &s)) != G4D_OK)
+            return rc;
     }
     {
         StageTimer tm(c, G4D_STAGE_GEOM, st);
@@ -965,28 +1037,32 @@ int fused_backward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* p
     float* gi[G4D_NUM_HEADS] = {gg->xyz, gg->scaling, gg->rotation, gg->opacity, nullptr};
     {
         StageTimer tm(c, G4D_STAGE_DEFORM_BWD, st);
-        if ((rc = deform_backward_dispatch(ws, prm, c->trow_ptr, pgrads, cam->time, n, g->xyz, go, gi,
+        if ((rc = deform_backward_dispatch(ws, prm, c->trow_ptr, pgrads, TimeArg{cam->time, c->time_src}, n, g->xyz, go, gi,
                                            c->relu_saved ? c->relu.as<uint32_t>() : nullptr,
                                            c->relu_saved ? c->feat.as<float>() : nullptr, st)) != G4D_OK) return rc;
     }
     return debug_sync(cam, st, "deform_backward");
 }
 
-// k cameras on k contexts: 1 <= k <= G4D_MAX_CAMERAS, one time bit for bit, pairwise distinct contexts of one workspace.
-// The cameras are checked before any context is looked at.
+// k cameras on k contexts: 1 <= k <= G4D_MAX_CAMERAS, one time bit for bit (or, when ctx[0] has a time source, that same
+// source on every context), pairwise distinct contexts of one workspace.  The cameras are checked before any context other
+// than ctx[0] is looked at.
 int check_camera_group(G4DContext* const* ctx, int32_t k, const G4DCamera* cams) {
     if (k < 1 || k > G4D_MAX_CAMERAS) return fail(G4D_ERR_ARG, "the number of cameras must be in 1..G4D_MAX_CAMERAS");
     if (!cams) return fail(G4D_ERR_ARG, "cameras are NULL");
     int rc;
+    const float* src = ctx && ctx[0] ? ctx[0]->time_src : nullptr;
     for (int i = 0; i < k; ++i) {
         if ((rc = check_camera(&cams[i])) != G4D_OK) return rc;
-        if (memcmp(&cams[i].time, &cams[0].time, sizeof(float)) != 0)
+        if (!src && memcmp(&cams[i].time, &cams[0].time, sizeof(float)) != 0)
             return fail(G4D_ERR_ARG, "the cameras of one call must share their time bit for bit");
     }
     if (!ctx) return fail(G4D_ERR_ARG, "contexts are NULL");
     for (int i = 0; i < k; ++i) {
         if (!ctx[i]) return fail(G4D_ERR_ARG, "context is NULL");
         if (ctx[i]->ws != ctx[0]->ws) return fail(G4D_ERR_ARG, "the contexts of one call must belong to one workspace");
+        if (ctx[i]->time_src != src)
+            return fail(G4D_ERR_ARG, "the contexts of one call must share their time source (g4d_context_set_time_source), or have none");
         for (int j = 0; j < i; ++j)
             if (ctx[j] == ctx[i]) return fail(G4D_ERR_ARG, "the contexts of one call must be pairwise distinct");
     }
@@ -1004,7 +1080,12 @@ int g4d_render_forward(G4DContext* c, const G4DCamera* cam, const G4DDeformParam
     if (!c) return fail(G4D_ERR_ARG, "context is NULL");
     int rc = check_render_args(cam, prm, g, out_color, out_depth, out_radii);
     if (rc != G4D_OK) return rc;
-    return fused_forward(c, cam, prm, g, out_color, out_depth, out_radii, false, (cudaStream_t)stream);
+    const cudaStream_t st = (cudaStream_t)stream;
+    G4D_CUDA(cudaSetDevice(c->ws->device));
+    CallScope scope(c->ws, st);
+    if (scope.rc != G4D_OK) return scope.rc;
+    if ((rc = refuse_capture(c->ws, cam, 1, &c)) != G4D_OK) return rc;
+    return fused_forward(c, cam, prm, g, out_color, out_depth, out_radii, false, st);
 }
 
 int g4d_render_backward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* prm, G4DDeformGrads* pgrads,
@@ -1023,7 +1104,12 @@ int g4d_render_backward(G4DContext* c, const G4DCamera* cam, const G4DDeformPara
     if (!dL_dcolor || !gg || (n > 0 && (!gg->xyz || !gg->scaling || !gg->rotation || !gg->opacity || !gg->features_dc || !gg->means2D)))
         return fail(G4D_ERR_ARG, "NULL gradient pointer");
     if (g->features_rest && n > 0 && !gg->features_rest) return fail(G4D_ERR_ARG, "features_rest gradient sink is NULL");
-    return fused_backward(c, cam, prm, pgrads, g, dL_dcolor, gg, (cudaStream_t)stream);
+    const cudaStream_t st = (cudaStream_t)stream;
+    G4D_CUDA(cudaSetDevice(c->ws->device));
+    CallScope scope(c->ws, st);
+    if (scope.rc != G4D_OK) return scope.rc;
+    if ((rc = refuse_capture(c->ws, cam, 1, nullptr)) != G4D_OK) return rc;
+    return fused_backward(c, cam, prm, pgrads, g, dL_dcolor, gg, st);
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -1038,6 +1124,9 @@ int g4d_render_forward_cameras(G4DContext* const* ctx, int32_t k, const G4DCamer
     cudaStream_t st = (cudaStream_t)stream;
     G4DContext* c0 = ctx[0];
     G4D_CUDA(cudaSetDevice(c0->ws->device));
+    CallScope scope(c0->ws, st);
+    if (scope.rc != G4D_OK) return scope.rc;
+    if ((rc = refuse_capture(c0->ws, cams, k, ctx)) != G4D_OK) return rc;
     for (int i = 0; i < k; ++i) {
         if ((rc = check_pending(ctx[i])) != G4D_OK) return rc;
         ctx[i]->has_forward = false; ctx[i]->group = 0;
@@ -1055,7 +1144,7 @@ int g4d_render_forward_cameras(G4DContext* const* ctx, int32_t k, const G4DCamer
             reset_stage_flags(c, 0, G4D_STAGE_COUNT - 1);
             {
                 StageTimer tm(c, G4D_STAGE_PREP, st);
-                G4D_CUDA(launch_pack_camera(cams[i], c->cam.as<CameraDev>(), st));
+                G4D_CUDA(launch_pack_camera(cams[i], c->time_src, c->cam.as<CameraDev>(), st));
             }
             ec.cam[i - 1] = c->cam.as<CameraDev>(); ec.g[i - 1] = c->g; ec.out_radii[i - 1] = out_radii[i];
         }
@@ -1102,6 +1191,9 @@ int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCame
     cudaStream_t st = (cudaStream_t)stream;
     G4DWorkspace* ws = c0->ws;
     G4D_CUDA(cudaSetDevice(ws->device));
+    CallScope scope(ws, st);
+    if (scope.rc != G4D_OK) return scope.rc;
+    if ((rc = refuse_capture(ws, cams, k, nullptr)) != G4D_OK) return rc;
     for (int i = 0; i < k; ++i)
         if ((rc = check_pending(ctx[i])) != G4D_OK) return rc;
     if (k == 1 && dL_dcolor[0]) {     // one camera: the single-camera backward
@@ -1149,7 +1241,7 @@ int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCame
     float* gi[G4D_NUM_HEADS] = {gg->xyz, gg->scaling, gg->rotation, gg->opacity, nullptr};
     {
         StageTimer tm(c0, G4D_STAGE_DEFORM_BWD, st);
-        if ((rc = deform_backward_dispatch(ws, prm, c0->trow_ptr, pgrads, cams[0].time, n, g->xyz, go, gi,
+        if ((rc = deform_backward_dispatch(ws, prm, c0->trow_ptr, pgrads, TimeArg{cams[0].time, c0->time_src}, n, g->xyz, go, gi,
                                            c0->relu_saved ? c0->relu.as<uint32_t>() : nullptr,
                                            c0->relu_saved ? c0->feat.as<float>() : nullptr, st)) != G4D_OK) return rc;
     }
@@ -1207,21 +1299,56 @@ int g4d_plane_regulation(G4DWorkspace* ws, const G4DDeformParams* prm, G4DDeform
     return G4D_OK;
 }
 
+}  // extern "C"
+
+namespace {
+// the arguments g4d_adam_step and g4d_adam_step_device share (`who`: the entry point the message names)
+int check_adam_args(const char* who, G4DWorkspace* ws, float* param, const float* grad, float* exp_avg, float* exp_avg_sq,
+                    int64_t numel, const G4DAdamSegment* segments, int32_t num_segments) {
+    if (!ws || numel < 0 || (numel > 0 && (!param || !grad || !exp_avg || !exp_avg_sq || !segments)))
+        return fail(G4D_ERR_ARG, who, "bad argument");
+    if ((numel & 3) || num_segments < 0 || num_segments > G4D_ADAM_MAX_SEGMENTS)
+        return fail(G4D_ERR_ARG, who, "numel must be a multiple of 4 and at most 16 segments");
+    if (((uintptr_t)param | (uintptr_t)grad | (uintptr_t)exp_avg | (uintptr_t)exp_avg_sq) & 15u)   // the kernel moves float4s
+        return fail(G4D_ERR_ARG, who, "param, grad, exp_avg and exp_avg_sq must be 16-byte aligned");
+    for (int i = 0; i < num_segments; ++i)
+        if (segments[i].begin < 0 || segments[i].end < segments[i].begin || segments[i].end > numel || (i && segments[i].begin < segments[i - 1].end))
+            return fail(G4D_ERR_ARG, who, "segments must be sorted, disjoint and inside [0, numel)");
+    return G4D_OK;
+}
+}  // namespace
+
+extern "C" {
+
 int g4d_adam_step(G4DWorkspace* ws, float* param, const float* grad, float* exp_avg, float* exp_avg_sq, int64_t numel,
                   const G4DAdamSegment* segments, int32_t num_segments, float beta1, float beta2, float eps, int64_t step,
                   float grad_scale, void* stream) {
-    if (!ws || numel < 0 || (numel > 0 && (!param || !grad || !exp_avg || !exp_avg_sq || !segments)) || step < 1)
-        return fail(G4D_ERR_ARG, "g4d_adam_step: bad argument");
-    if ((numel & 3) || num_segments < 0 || num_segments > G4D_ADAM_MAX_SEGMENTS)
-        return fail(G4D_ERR_ARG, "g4d_adam_step: numel must be a multiple of 4 and at most 16 segments");
-    if (((uintptr_t)param | (uintptr_t)grad | (uintptr_t)exp_avg | (uintptr_t)exp_avg_sq) & 15u)   // the kernel moves float4s
-        return fail(G4D_ERR_ARG, "g4d_adam_step: param, grad, exp_avg and exp_avg_sq must be 16-byte aligned");
-    for (int i = 0; i < num_segments; ++i)
-        if (segments[i].begin < 0 || segments[i].end < segments[i].begin || segments[i].end > numel || (i && segments[i].begin < segments[i - 1].end))
-            return fail(G4D_ERR_ARG, "g4d_adam_step: segments must be sorted, disjoint and inside [0, numel)");
+    if (step < 1) return fail(G4D_ERR_ARG, "g4d_adam_step: bad argument");
+    const int rc = check_adam_args("g4d_adam_step", ws, param, grad, exp_avg, exp_avg_sq, numel, segments, num_segments);
+    if (rc != G4D_OK) return rc;
     G4D_CUDA(cudaSetDevice(ws->device));
     G4D_CUDA(launch_adam_flat(param, grad, exp_avg, exp_avg_sq, numel, segments, num_segments, beta1, beta2, eps, step, grad_scale,
                               ws->sm_count, (cudaStream_t)stream));
+    return G4D_OK;
+}
+
+int g4d_adam_scalars(const G4DAdamSegment* segments, int32_t num_segments, float beta1, float beta2, int64_t step, float grad_scale,
+                     G4DAdamScalars* out) {
+    if (!out || num_segments < 0 || num_segments > G4D_ADAM_MAX_SEGMENTS || (num_segments > 0 && !segments) || step < 1)
+        return fail(G4D_ERR_ARG, "g4d_adam_scalars: bad argument");
+    adam_scalars(segments, num_segments, beta1, beta2, step, grad_scale, out);
+    return G4D_OK;
+}
+
+int g4d_adam_step_device(G4DWorkspace* ws, float* param, const float* grad, float* exp_avg, float* exp_avg_sq, int64_t numel,
+                         const G4DAdamSegment* segments, int32_t num_segments, float beta1, float beta2, float eps,
+                         const G4DAdamScalars* d_scalars, void* stream) {
+    int rc = check_adam_args("g4d_adam_step_device", ws, param, grad, exp_avg, exp_avg_sq, numel, segments, num_segments);
+    if (rc != G4D_OK) return rc;
+    if (!d_scalars) return fail(G4D_ERR_ARG, "g4d_adam_step_device", "d_scalars is NULL");
+    G4D_CUDA(cudaSetDevice(ws->device));
+    G4D_CUDA(launch_adam_flat_device(param, grad, exp_avg, exp_avg_sq, numel, segments, num_segments, beta1, beta2, eps, d_scalars,
+                                     ws->sm_count, (cudaStream_t)stream));
     return G4D_OK;
 }
 
@@ -1229,8 +1356,37 @@ int g4d_dist2_knn3(G4DWorkspace* ws, int64_t n, const float* xyz, float* out_mea
     if (!ws || n < 0 || (n > 0 && (!xyz || !out_mean_dist2))) return fail(G4D_ERR_ARG, "g4d_dist2_knn3: bad argument");
     if (n >= (1ll << 31)) return fail(G4D_ERR_ARG, "n too large");
     G4D_CUDA(cudaSetDevice(ws->device));
+    CallScope scope(ws, (cudaStream_t)stream);
+    if (scope.rc != G4D_OK) return scope.rc;
     G4D_CUDA(ws->scratch.ensure(knn_scratch_bytes(n)));
     G4D_CUDA(launch_knn_dist2(n, xyz, out_mean_dist2, ws->scratch.p, ws->sm_count, (cudaStream_t)stream));
+    return G4D_OK;
+}
+
+int g4d_context_set_time_source(G4DContext* c, const float* d_time) {
+    if (!c) return fail(G4D_ERR_ARG, "context is NULL");
+    c->time_src = d_time;
+    return G4D_OK;
+}
+
+int g4d_workspace_freeze(G4DWorkspace* ws, int on) {
+    if (!ws) return fail(G4D_ERR_ARG, "workspace is NULL");
+    ws->frozen = on ? 1 : 0;
+    return G4D_OK;
+}
+
+int g4d_workspace_graph_status(G4DWorkspace* ws, int sync, G4DGraphStatus* out) {
+    if (!ws || !out) return fail(G4D_ERR_ARG, "NULL argument");
+    if (sync) {
+        G4D_CUDA(cudaSetDevice(ws->device));
+        G4D_CUDA(cudaDeviceSynchronize());
+    }
+    volatile PinnedWords* w = ws->pinned;
+    *out = G4DGraphStatus{};
+    out->overflows = w->overflow[0];
+    out->max_instances = w->overflow[1];
+    out->f16_range = w->f16_range ? 1 : 0;
+    w->overflow[0] = 0; w->overflow[1] = 0; w->f16_range = 0;
     return G4D_OK;
 }
 

@@ -604,14 +604,14 @@ struct TimeGradDesc {
     int start[G4D_MAX_LEVELS * 3 + 1];
 };
 
-__global__ void distribute_time_grad_kernel(TimeGradDesc d, float time) {
+__global__ void distribute_time_grad_kernel(TimeGradDesc d, TimeArg time) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const int nseg = d.levels * 3;
     if (i >= d.start[nseg]) return;
     int m = 0;
     while (i >= d.start[m + 1]) ++m;
     const int l = m / 3, a = m % 3, e = i - d.start[m];
-    const Tap1D ty = make_tap(time, d.res[l][3]);
+    const Tap1D ty = make_tap(time.get(), d.res[l][3]);
     const int rowlen = d.res[l][a] * d.C;
     const float gv = d.row_grad[l][a][e];
     atomicAdd(d.plane_grad[l][a] + (size_t)ty.i0 * rowlen + e, gv * ty.w0);
@@ -619,7 +619,7 @@ __global__ void distribute_time_grad_kernel(TimeGradDesc d, float time) {
 }
 
 // ---- host side -------------------------------------------------------------------------------------------
-cudaError_t launch_distribute_time_grad(const DeformDesc& d, float* const (*trow_grad)[3], float* const (*g_planes)[6], float time,
+cudaError_t launch_distribute_time_grad(const DeformDesc& d, float* const (*trow_grad)[3], float* const (*g_planes)[6], TimeArg time,
                                         cudaStream_t st) {
     TimeGradDesc t{};
     t.levels = d.levels; t.C = d.C;
@@ -657,7 +657,7 @@ size_t deform_backward_scratch_bytes(const DeformDesc& d, int64_t n) {
 }
 
 template <int TG, int WD>
-static cudaError_t launch_deform_backward_t(const DeformBwdDesc& bd, float time, int64_t n, const float* xyz, float* scratch,
+static cudaError_t launch_deform_backward_t(const DeformBwdDesc& bd, TimeArg time, int64_t n, const float* xyz, float* scratch,
                                             int sm_count, cudaStream_t st) {
     const DeformDesc& d = bd.d;
     DeformBwdBuffers buf{};
@@ -711,7 +711,7 @@ static cudaError_t launch_deform_backward_t(const DeformBwdDesc& bd, float time,
     return cudaSuccess;
 }
 
-cudaError_t launch_deform_backward(const DeformDesc& d, const G4DDeformParams& prm, const G4DDeformGrads& grads, float time,
+cudaError_t launch_deform_backward(const DeformDesc& d, const G4DDeformParams& prm, const G4DDeformGrads& grads, TimeArg time,
                                    int64_t n, const float* xyz, const float* const go[G4D_NUM_HEADS],
                                    float* const gi[G4D_NUM_HEADS], float* scratch, int sm_count, cudaStream_t st) {
     if (n == 0) return cudaSuccess;

@@ -671,4 +671,18 @@ cudaError_t launch_bin_place(int grid_x, int grid_y, const GeomBuffers& g, const
     return launch_k(bin_fix_kernel, dim3((num_tiles * rounds + 7) / 8), dim3(256), 0, st, true, a, lay.chunks);
 }
 
+// One thread, ordinary launch (after the blend: no programmatic edge to break).  The forwards of a stream run one after the
+// other, so the read-modify-write of the host-mapped words needs no atomics.
+__global__ void record_overflow_kernel(const BinCtl* ctl, uint32_t capacity, volatile uint32_t* words) {
+    const uint32_t R = ctl->R;
+    if (R <= capacity) return;
+    words[0] = words[0] + 1u;
+    if (R > words[1]) words[1] = R;
+}
+
+cudaError_t launch_record_overflow(const BinCtl* ctl, uint32_t capacity, uint32_t* words, cudaStream_t st) {
+    record_overflow_kernel<<<1, 1, 0, st>>>(ctl, capacity, words);
+    return cudaGetLastError();
+}
+
 }  // namespace g4d

@@ -680,7 +680,7 @@ static cudaError_t launch_a(const BwdADesc& bd, int64_t n, int sm_count, cudaStr
 }
 
 cudaError_t launch_deform_backward_tc(const DeformDesc& d, const G4DDeformParams& prm, const G4DDeformGrads& grads,
-                                      const TcBwdWeights& w, float time, int64_t n, const float* xyz,
+                                      const TcBwdWeights& w, TimeArg time, int64_t n, const float* xyz,
                                       const float* const go[G4D_NUM_HEADS], float* const gi[G4D_NUM_HEADS],
                                       const uint32_t* relu_bits, const float* saved_feat, const uint32_t* order, uint8_t* scratch,
                                       int sm_count, cudaStream_t st) {

@@ -12,7 +12,7 @@
 namespace g4d {
 
 // ------------------------------------------------------------------------------------------------------
-__global__ void pack_camera_kernel(G4DCamera c, CameraDev* dst) {
+__global__ void pack_camera_kernel(G4DCamera c, const float* d_time, CameraDev* dst) {
     pdl_trigger();      // (ordinary launch: everything before it in the stream has completed)
     const int t = threadIdx.x;
     if (t < 16) {
@@ -29,15 +29,16 @@ __global__ void pack_camera_kernel(G4DCamera c, CameraDev* dst) {
         dst->grid_y = (c.image_height + kTile - 1) / kTile;
         dst->num_tiles = dst->grid_x * dst->grid_y;
         dst->depth_min = 0xFFFFFFFFu; dst->depth_max = 0u;
-        dst->tanfovx = c.tanfovx; dst->tanfovy = c.tanfovy; dst->scale_modifier = c.scale_modifier; dst->time = c.time;
+        dst->tanfovx = c.tanfovx; dst->tanfovy = c.tanfovy; dst->scale_modifier = c.scale_modifier;
+        dst->time = d_time ? *d_time : c.time;
         dst->focal_x = (float)c.image_width / (2.f * c.tanfovx);
         dst->focal_y = (float)c.image_height / (2.f * c.tanfovy);
         dst->grid_bar = 0u; dst->pad3 = 0u;
     }
 }
 
-cudaError_t launch_pack_camera(const G4DCamera& cam, CameraDev* dst, cudaStream_t st) {
-    pack_camera_kernel<<<1, 32, 0, st>>>(cam, dst);
+cudaError_t launch_pack_camera(const G4DCamera& cam, const float* d_time, CameraDev* dst, cudaStream_t st) {
+    pack_camera_kernel<<<1, 32, 0, st>>>(cam, d_time, dst);
     return cudaGetLastError();
 }
 
@@ -86,7 +87,7 @@ struct CollapseDesc {
 
 // Every Gaussian of a view shares t, so the time-axis interpolation of the three time planes is done once:
 // row[x][c] = plane[y0][x][c]*(y1-y) + plane[y1][x][c]*(y-y0)  with t NOT normalised (hexplane.py:164).
-__global__ void collapse_time_rows_kernel(CollapseDesc d, float time) {
+__global__ void collapse_time_rows_kernel(CollapseDesc d, TimeArg time) {
     pdl_wait();         // the row buffer is reused: the previous view's kernels read it until they complete
     pdl_trigger();
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -96,13 +97,13 @@ __global__ void collapse_time_rows_kernel(CollapseDesc d, float time) {
     while (i >= d.start[m + 1]) ++m;
     const int l = m / 3, a = m % 3, e = i - d.start[m];
     const int T = d.res[l][3];
-    const Tap1D ty = make_tap(time, T);
+    const Tap1D ty = make_tap(time.get(), T);   // (after pdl_wait: a source written by the previous kernel is complete)
     const int rowlen = d.res[l][a] * d.C;
     const float v0 = __ldg(d.plane[l][a] + (size_t)ty.i0 * rowlen + e), v1 = __ldg(d.plane[l][a] + (size_t)ty.i1 * rowlen + e);
     d.row[l][a][e] = fmaf(v1, ty.w1, v0 * ty.w0);
 }
 
-cudaError_t launch_collapse_time_rows(const G4DDeformParams& p, float time, float* const (*trow)[3], cudaStream_t st) {
+cudaError_t launch_collapse_time_rows(const G4DDeformParams& p, TimeArg time, float* const (*trow)[3], cudaStream_t st) {
     CollapseDesc d{};
     d.levels = p.levels; d.C = p.channels;
     const TimeRows tr(p.levels, p.res, p.channels);

@@ -37,6 +37,14 @@ struct TimeRows {
     }
 };
 
+// The timestamp of a forward or backward: read from src (device; g4d_context_set_time_source) when it is set, so that a
+// replayed CUDA graph sees the value of the replay, else `value`.
+struct TimeArg {
+    float value;
+    const float* src;
+    G4D_D float get() const { return src ? *src : value; }
+};
+
 // per-Gaussian projected record kept by a forward (SoA; sizes in DESIGN.md §3)
 struct GeomBuffers {
     float4* rec0;        // (px, py, conic.x, conic.y)
@@ -92,6 +100,9 @@ cudaError_t launch_bin_sort(int64_t n, int grid_x, int grid_y, const GeomBuffers
 // tile ranges + placement of every instance into its (tile, chunk) sub-segment + per-sub-segment ordering (2 launches)
 cudaError_t launch_bin_place(int grid_x, int grid_y, const GeomBuffers& g, const BinLayout& lay, uint32_t* ids, uint2* kbuf,
                              uint2* ranges, uint32_t capacity, int tight, cudaStream_t st);
+// the overflow record of a captured no-sync forward: when ctl->R exceeds the capacity, words[0] += 1 and
+// words[1] = max(words[1], R) (host-mapped words, g4d_workspace_graph_status)
+cudaError_t launch_record_overflow(const BinCtl* ctl, uint32_t capacity, uint32_t* words, cudaStream_t st);
 
 struct ImageBuffers {
     float* final_T;      // [H*W]
@@ -236,18 +247,19 @@ cudaError_t launch_tc_bwd_pack_weights(const G4DDeformParams& prm, uint8_t* blob
 bool tc_backward_supported(const G4DDeformParams& prm);
 size_t tc_deform_backward_scratch_bytes(const DeformDesc& d, int64_t n);   // size of launch_deform_backward_tc's scratch
 cudaError_t launch_deform_backward_tc(const DeformDesc& d, const G4DDeformParams& prm, const G4DDeformGrads& grads,
-                                      const TcBwdWeights& w, float time, int64_t n, const float* xyz,
+                                      const TcBwdWeights& w, TimeArg time, int64_t n, const float* xyz,
                                       const float* const go[G4D_NUM_HEADS], float* const gi[G4D_NUM_HEADS],
                                       const uint32_t* relu_bits, const float* saved_feat, const uint32_t* order, uint8_t* scratch,
                                       int sm_count, cudaStream_t st);
 // collapsed time-row gradients -> the two time rows of each (axis, t) plane (g4d_backward.cu)
-cudaError_t launch_distribute_time_grad(const DeformDesc& d, float* const (*trow_grad)[3], float* const (*g_planes)[6], float time,
+cudaError_t launch_distribute_time_grad(const DeformDesc& d, float* const (*trow_grad)[3], float* const (*g_planes)[6], TimeArg time,
                                         cudaStream_t st);
 
 // ---- launchers (defined in g4d_geom.cu / g4d_raster.cu / g4d_backward.cu) -----------------------------
-cudaError_t launch_pack_camera(const G4DCamera& cam, CameraDev* dst, cudaStream_t st);
+// d_time: the camera's timestamp from device memory (NULL: cam.time)
+cudaError_t launch_pack_camera(const G4DCamera& cam, const float* d_time, CameraDev* dst, cudaStream_t st);
 cudaError_t launch_pack_weights(const G4DDeformParams& p, float* w0t, float* const* w1t, cudaStream_t st);
-cudaError_t launch_collapse_time_rows(const G4DDeformParams& p, float time, float* const (*trow)[3], cudaStream_t st);
+cudaError_t launch_collapse_time_rows(const G4DDeformParams& p, TimeArg time, float* const (*trow)[3], cudaStream_t st);
 cudaError_t launch_preprocess(const CameraDev* cam, int64_t n, const RasterInputs& in, GeomBuffers g, int32_t* out_radii,
                               cudaStream_t st);
 // mode 0: deform only (writes the five out_* tensors; cam unused); mode 1: fused deform + preprocess (camera from cam).
@@ -268,7 +280,7 @@ cudaError_t launch_preprocess_backward(const CameraDev* cam, int64_t n, const Ra
 
 size_t deform_backward_scratch_bytes(const DeformDesc& d, int64_t n);   // size of launch_deform_backward's scratch
 // go[h] / gi[h]: gradient w.r.t. the outputs / inputs of head h's residual tensor (xyz, scaling, rotation, opacity, shs)
-cudaError_t launch_deform_backward(const DeformDesc& d, const G4DDeformParams& prm, const G4DDeformGrads& grads, float time,
+cudaError_t launch_deform_backward(const DeformDesc& d, const G4DDeformParams& prm, const G4DDeformGrads& grads, TimeArg time,
                                    int64_t n, const float* xyz, const float* const go[G4D_NUM_HEADS],
                                    float* const gi[G4D_NUM_HEADS], float* scratch, int sm_count, cudaStream_t st);
 // ---- several cameras at one timestamp (g4d_render_forward_cameras / _backward_cameras) -----------------------------
@@ -319,6 +331,11 @@ cudaError_t launch_ssim_backward(const float* x, const float* y, int C, int H, i
 // ---- flat Adam (g4d_optim.cu) ------------------------------------------------------------------------------------------
 cudaError_t launch_adam_flat(float* p, const float* g, float* m, float* v, int64_t numel, const G4DAdamSegment* segs, int nseg,
                              float b1, float b2, float eps, int64_t step, float grad_scale, int sm_count, cudaStream_t st);
+// the per-step scalars launch_adam_flat runs with (g4d_adam_scalars)
+void adam_scalars(const G4DAdamSegment* segs, int nseg, float b1, float b2, int64_t step, float grad_scale, G4DAdamScalars* out);
+// launch_adam_flat with the scalars read from device memory at run time (the segments' lr fields are not read)
+cudaError_t launch_adam_flat_device(float* p, const float* g, float* m, float* v, int64_t numel, const G4DAdamSegment* segs, int nseg,
+                                    float b1, float b2, float eps, const G4DAdamScalars* d_scalars, int sm_count, cudaStream_t st);
 
 // ---- 3-nearest-neighbour mean squared distance (g4d_knn.cu) ---------------------------------------------------------
 size_t knn_scratch_bytes(int64_t n);   // size of launch_knn_dist2's scratch

@@ -1,0 +1,231 @@
+"""CUDA-graph capture of no-grad rendering: ``render()`` and ``render_cameras()`` recorded once and replayed per call.
+
+A replay re-runs the device work of a render with no host work in between: no C-ABI structs rebuilt, no weight-image
+decision, no host synchronisation.  What changes from one call to the next -- the view and projection matrices, the camera
+centre and the timestamp -- goes through one pinned staging block into device memory the captured kernels read
+(``G4DCamera.d_*`` and ``g4d_context_set_time_source``).  Everything else is fixed by the template the graph was built
+from: the model's tensors (their storage; in-place updates are seen), the image size, FoV and SH degree of every view, the
+background and the stage.
+
+The graph owns a private workspace and its contexts, frozen after the capture, so that no eager call can move a buffer
+the graph points at.  Forwards run in no-sync mode (G4D_OPT_SYNC_MODE = 0): the instance capacity is learnt from the
+template views, and a replay whose views need more instances gives incomplete images.  ``check()`` reports that (and the
+FP16x2 range flag of the tensor-core network) as ``G4DError``.
+"""
+from __future__ import annotations
+
+import ctypes as C
+import math
+import struct
+from typing import List, Sequence
+
+import torch
+
+from . import _lib
+from .deformation import deform_network, scalar_time
+from .renderer import _zero_points, settings_from_camera
+from .rasterizer import _dev_f32
+
+_VIEW_FLOATS = 36        # per view in the staging block: view matrix [16], projection matrix [16], camera centre [3], pad
+ERR_OVERFLOW = -5        # G4D_ERR_OVERFLOW
+
+
+def _time_bits(t) -> bytes:
+    return struct.pack("<f", float(t))
+
+
+class GraphedRender:
+    """``render()`` (template: one camera) or ``render_cameras()`` (template: a list of at most 32 cameras at one time)
+    under ``torch.no_grad()``, replayed from a CUDA graph.
+
+    ``__call__`` takes a camera (or a list of cameras) with the template's image sizes and FoVs and returns the result
+    dict(s) ``render()`` returns.  Their tensors are the graph's static outputs: the next call overwrites them.
+    ``min_capacity`` raises the instance capacity learnt from the template views (G4D_OPT_INSTANCE_CAPACITY)."""
+
+    def __init__(self, pc, pipe, bg_color: torch.Tensor, template, stage: str = "fine", scaling_modifier: float = 1.0,
+                 min_capacity: int = 0):
+        self.multi = isinstance(template, (list, tuple))
+        views = list(template) if self.multi else [template]
+        if not views or len(views) > _lib.MAX_CAMERAS:
+            raise ValueError("a graphed render takes 1..%d views, got %d" % (_lib.MAX_CAMERAS, len(views)))
+        if "coarse" in stage:
+            module = None
+        elif "fine" in stage:
+            module = pc._deformation
+            if not isinstance(module, deform_network):
+                raise NotImplementedError("a graphed render needs the g4d deformation network (or the coarse stage)")
+        else:
+            raise NotImplementedError
+        if getattr(pipe, "debug", False):
+            raise ValueError("a graphed render cannot run with pipe.debug (it synchronises after every stage)")
+        xyz = pc.get_xyz
+        dev = xyz.device
+        self.pc, self.k, self.n, self.dev = pc, len(views), int(xyz.shape[0]), dev
+        self.sh_degree = int(pc.active_sh_degree)
+        n, k = self.n, self.k
+        lib = _lib.load()
+        settings = [settings_from_camera(v, pc, pipe, bg_color, scaling_modifier) for v in views]
+        self._shape = [self._view_key(rs) for rs, _ in settings]
+        # the model's tensors are read in place: a copy (non-contiguous or non-fp32 storage) would freeze their values
+        self._tensors = (pc._xyz, pc._scaling, pc._rotation, pc._opacity, pc._features_dc, pc._features_rest)
+        staged = [_dev_f32(t, t.numel(), name) for t, name in zip(self._tensors, ("xyz", "scaling", "rotation", "opacity",
+                                                                                  "features_dc", "features_rest"))]
+        if any(a.data_ptr() != b.data_ptr() for a, b in zip(staged, self._tensors)):
+            raise ValueError("a graphed render reads the model's tensors in place: they must be contiguous fp32 CUDA tensors")
+        self._ptrs = tuple(t.data_ptr() for t in self._tensors)
+        self._bg = _dev_f32(bg_color, 3, "bg")
+
+        self.ws = _lib.Workspace(dev.index if dev.index is not None else torch.cuda.current_device())
+        self.ws.set_option(_lib.OPT_SYNC_MODE, 0)
+        if min_capacity:
+            self.ws.set_option(_lib.OPT_INSTANCE_CAPACITY, int(min_capacity))
+        self.ctxs = [_lib.Context(self.ws) for _ in range(k)]
+        # device block the captured kernels read: k views, then the timestamp; its pinned staging copy
+        self._block = torch.zeros(k * _VIEW_FLOATS + 4, device=dev, dtype=torch.float32)
+        self._staging = torch.zeros(k * _VIEW_FLOATS + 4, dtype=torch.float32, pin_memory=True)
+        self._staging_np = self._staging.numpy()
+        self._staged = torch.cuda.Event()
+        base, fsz = self._block.data_ptr(), 4
+        d_time = base + k * _VIEW_FLOATS * fsz
+        for c in self.ctxs:
+            c.set_time_source(d_time)
+
+        self._cams = (_lib.Camera * k)()
+        for i, (rs, _) in enumerate(settings):
+            cam = self._cams[i]
+            cam.image_height, cam.image_width = int(rs.image_height), int(rs.image_width)
+            cam.sh_degree, cam.debug = self.sh_degree, _lib.CAM_NO_GRAD
+            cam.tanfovx, cam.tanfovy, cam.scale_modifier = float(rs.tanfovx), float(rs.tanfovy), float(rs.scale_modifier)
+            off = base + i * _VIEW_FLOATS * fsz
+            cam.d_viewmatrix, cam.d_projmatrix, cam.d_campos = off, off + 16 * fsz, off + 32 * fsz
+            cam.d_bg = self._bg.data_ptr()
+        self._keep: list = []
+        # fresh: the capture records the weight repack, so every replay packs the parameters as they are then
+        self._prm = module.c_params(self._keep, fresh=True) if module is not None else None
+        self._module = module
+        self._net_key = self._network_key()
+        self._g = _lib.Gaussians(n, *self._ptrs)
+        self.colors = [torch.zeros(3, int(rs.image_height), int(rs.image_width), device=dev) for rs, _ in settings]
+        self.depths = [torch.zeros(1, int(rs.image_height), int(rs.image_width), device=dev) for rs, _ in settings]
+        self.radii = [torch.zeros(n, device=dev, dtype=torch.int32) for _ in range(k)]
+        self.visible = [torch.zeros(n, device=dev, dtype=torch.bool) for _ in range(k)]
+        ptrs = lambda ts: (C.c_void_p * k)(*[t.data_ptr() for t in ts])
+        self._out = (ptrs(self.colors), ptrs(self.depths), ptrs(self.radii))
+        self._handles = (C.c_void_p * k)(*[c.handle for c in self.ctxs])
+        self._lib = lib
+
+        with torch.cuda.device(dev):
+            self._stage(views)
+            # eager: the first call learns each context's instance capacity (it reads R back once), the second is the
+            # no-sync warm-up; the stats read reports an overflow of the warm-up
+            self._launch()
+            self._launch()
+            for c in self.ctxs:
+                c.stats()
+            self.graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(self.graph):
+                self._launch()
+            self.ws.freeze(True)
+            self.ws.graph_status(sync=True)   # (clear: nothing has been replayed yet)
+
+    @staticmethod
+    def _view_key(rs):
+        return (int(rs.image_height), int(rs.image_width), _time_bits(rs.tanfovx), _time_bits(rs.tanfovy), int(rs.sh_degree))
+
+    def _launch(self):
+        """The captured work: one C-ABI render call, then the visibility masks."""
+        stream = int(torch.cuda.current_stream(self.dev).cuda_stream)
+        prm = C.byref(self._prm) if self._prm is not None else None
+        if self.multi:
+            _lib.check(self._lib.g4d_render_forward_cameras(self._handles, self.k, self._cams, prm, C.byref(self._g), *self._out,
+                                                            stream), "g4d_render_forward_cameras")
+        else:
+            _lib.check(self._lib.g4d_render_forward(self.ctxs[0].handle, C.byref(self._cams[0]), prm, C.byref(self._g),
+                                                    self.colors[0].data_ptr(), self.depths[0].data_ptr(),
+                                                    self.radii[0].data_ptr(), stream), "g4d_render_forward")
+        for r, v in zip(self.radii, self.visible):
+            torch.gt(r, 0, out=v)
+
+    def _stage(self, views: Sequence) -> None:
+        """Views and time into the device block: host values through the pinned staging block (one copy), device matrices
+        by device copies behind it."""
+        times = []
+        dev_copies = []
+        self._staged.synchronize()          # the previous call's copy has read the staging block
+        st = self._staging_np
+        for i, v in enumerate(views):
+            if isinstance(v, dict):
+                raise NotImplementedError("PanopticSports cameras are not supported by a graphed render")
+            times.append(scalar_time(v.time))
+            o = i * _VIEW_FLOATS
+            for j, (t, w) in enumerate(((v.world_view_transform, 16), (v.full_proj_transform, 16), (v.camera_center, 3))):
+                t = t if torch.is_tensor(t) else torch.as_tensor(t, dtype=torch.float32)
+                if t.numel() != w:
+                    raise RuntimeError("camera matrix has %d elements, expected %d" % (t.numel(), w))
+                if t.is_cuda:
+                    dev_copies.append((o + 16 * j, w, t))
+                else:
+                    st[o + 16 * j:o + 16 * j + w] = t.detach().reshape(-1).float().numpy()
+        if any(_time_bits(t) != _time_bits(times[0]) for t in times):
+            raise ValueError("a graphed render_cameras renders one timestamp: the cameras' times differ (%s)" % sorted(set(times)))
+        st[self.k * _VIEW_FLOATS] = float(times[0])
+        stream = torch.cuda.current_stream(self.dev)
+        self._block.copy_(self._staging, non_blocking=True)
+        self._staged.record(stream)
+        for o, w, t in dev_copies:
+            self._block[o:o + w].copy_(t.detach().reshape(-1))
+
+    def _network_key(self):
+        """what the captured G4DDeformParams points at: the module, its head mask, aabb and parameter storage"""
+        m = self._module
+        if m is None:
+            return None
+        return (id(self.pc._deformation), m.head_mask(), m.deformation_net.grid.aabb.data_ptr()) + \
+            tuple(p.data_ptr() for p in m.flat_parameters())
+
+    def _check_template(self, views: List) -> None:
+        if len(views) != self.k:
+            raise ValueError("the graph was captured for %d views, got %d" % (self.k, len(views)))
+        pc = self.pc
+        if int(pc.get_xyz.shape[0]) != self.n:
+            raise ValueError("the model has %d Gaussians, the graph was captured for %d" % (pc.get_xyz.shape[0], self.n))
+        if int(pc.active_sh_degree) != self.sh_degree:
+            raise ValueError("the SH degree changed from %d to %d since the capture" % (self.sh_degree, pc.active_sh_degree))
+        if tuple(t.data_ptr() for t in (pc._xyz, pc._scaling, pc._rotation, pc._opacity, pc._features_dc,
+                                        pc._features_rest)) != self._ptrs:
+            raise ValueError("the model's tensors were replaced since the capture: build a new GraphedRender")
+        if self._network_key() != self._net_key:
+            raise ValueError("the deformation network's parameters were replaced (or its head mask changed) since the capture: "
+                             "build a new GraphedRender")
+        for i, v in enumerate(views):
+            key = (int(v.image_height), int(v.image_width), _time_bits(math.tan(v.FoVx * 0.5)), _time_bits(math.tan(v.FoVy * 0.5)),
+                   self.sh_degree)
+            if key != self._shape[i]:
+                raise ValueError("view %d differs from the template (image size or FoV): %s vs %s" % (i, key[:2], self._shape[i][:2]))
+
+    def __call__(self, cameras):
+        if self.multi != isinstance(cameras, (list, tuple)):
+            raise ValueError("the graph was captured for %s" % ("render_cameras() of %d cameras, got one camera" % self.k
+                                                                if self.multi else "render() of one camera, got a list"))
+        views = list(cameras) if self.multi else [cameras]
+        self._check_template(views)
+        with torch.cuda.device(self.dev):
+            self._stage(views)
+            self.graph.replay()
+        pts = _zero_points(self.pc.get_xyz)
+        out = [{"render": c, "viewspace_points": pts, "visibility_filter": v, "radii": r, "depth": d}
+               for c, v, r, d in zip(self.colors, self.visible, self.radii, self.depths)]
+        return out if self.multi else out[0]
+
+    def check(self, sync: bool = True) -> None:
+        """Raise G4DError when a replay since the last check overflowed its instance capacity (its images are incomplete) or
+        met a value outside the FP16x2 operand range.  sync: wait for the replays first."""
+        s = self.ws.graph_status(sync)
+        if s.overflows:
+            raise _lib.G4DError("graphed render failed (code %d): %d replayed view(s) needed up to %d tile instances, more than "
+                                "the capacity learnt at capture; their images are incomplete (build the graph with a larger "
+                                "min_capacity)" % (ERR_OVERFLOW, s.overflows, s.max_instances))
+        if s.f16_range:
+            raise _lib.G4DError("graphed render failed (code %d): an FP16x2 tensor-core launch met a value outside the f16 "
+                                "operand range; its results were saturated (G4D_OPT_TENSOR_CORES = 1 avoids the limit)"
+                                % ERR_OVERFLOW)

@@ -224,6 +224,23 @@ typedef struct G4DAdamSegment { int64_t begin, end; float lr; float reserved; } 
 int g4d_adam_step(G4DWorkspace *ws, float *param, const float *grad, float *exp_avg, float *exp_avg_sq, int64_t numel,
                   const G4DAdamSegment *segments, int32_t num_segments, float beta1, float beta2, float eps, int64_t step,
                   float grad_scale, void *stream);
+/* g4d_adam_step_device: the same update with the per-step scalars read from DEVICE memory when the kernel runs, so that a
+ * captured CUDA graph applies each replay's values: d_scalars points at a G4DAdamScalars in device memory (lr[i] is segment
+ * i's learning rate; the segments' own lr fields are not read; their begin / end are, and are checked as above).
+ * g4d_adam_scalars fills a G4DAdamScalars on the host (no device needed) with exactly the values g4d_adam_step computes from
+ * (segments[i].lr, beta1, beta2, step, grad_scale): the two updates are then bit-identical. */
+typedef struct G4DAdamScalars {
+    float lr[G4D_ADAM_MAX_SEGMENTS];
+    float inv_bc1;        /* 1 / (1 - beta1^step) */
+    float inv_sqrt_bc2;   /* 1 / sqrt(1 - beta2^step) */
+    float grad_scale;
+    float reserved;
+} G4DAdamScalars;
+int g4d_adam_scalars(const G4DAdamSegment *segments, int32_t num_segments, float beta1, float beta2, int64_t step,
+                     float grad_scale, G4DAdamScalars *out);
+int g4d_adam_step_device(G4DWorkspace *ws, float *param, const float *grad, float *exp_avg, float *exp_avg_sq, int64_t numel,
+                         const G4DAdamSegment *segments, int32_t num_segments, float beta1, float beta2, float eps,
+                         const G4DAdamScalars *d_scalars, void *stream);
 
 /* ---- scene initialisation (SURVEY.md 8f N4) -------------------------------------------------------
  * g4d_dist2_knn3 <- simple_knn._C.distCUDA2(points) (scene/gaussian_model.py:22,148; submodule absent from the reference
@@ -301,6 +318,37 @@ int g4d_context_stage_times(G4DContext *ctx, float *out_ms, int capacity);
 
 /* DEBUG: mean per-CTA cycle counters of the last tensor-core deform launch (G4D_OPT_TC_DEBUG). */
 int g4d_debug_tc_cycles(G4DWorkspace *ws, double *out12);
+
+/* ---- CUDA-graph capture (opt-in; INTEGRATION.md "CUDA graphs") -------------------------------------
+ * Every entry point that owns buffers or host-side state asks cudaStreamIsCapturing on its stream (the loss, regulariser and
+ * Adam entry points own neither: they only launch kernels and capture as they are).  While the stream captures, nothing that a replay could not
+ * re-run happens: no host events, no read of a pinned read-back slot, no host sync, no allocation.  An entry point returns
+ * G4D_ERR_STATE (the message names the cause) before any launch when the workspace is in exact sync mode
+ * (G4D_OPT_SYNC_MODE = 1), when a context has not learnt its instance capacity from an earlier forward, with G4D_CAM_DEBUG or
+ * with G4D_OPT_STAGE_TIMING; and when one of its buffers would have to grow it returns G4D_ERR_STATE without freeing
+ * anything.  Buffers are sized where each stage needs them, so that refusal can come after the call has enqueued (or, while
+ * capturing, recorded) its first stages: a capture that met it is unusable (end it and drop the graph), and after an eager
+ * refusal on a frozen workspace the context holds no forward (a backward on it returns G4D_ERR_STATE).
+ *
+ * g4d_context_set_time_source: while d_time (device, one float) is set, every forward and backward on ctx reads its
+ * timestamp from there at run time instead of from G4DCamera.time: the time-row collapse, the network's backward and the
+ * camera record.  NULL restores G4DCamera.time.  g4d_render_forward_cameras / _backward_cameras need either no source on any
+ * of their contexts (the cameras' times are compared) or the same source on all of them.
+ * g4d_workspace_freeze: while on, any call that would reallocate a buffer of ws or of one of its contexts returns
+ * G4D_ERR_STATE and frees nothing (a captured graph keeps pointing at those buffers).
+ * g4d_workspace_graph_status: what the forwards captured on ws met since the last call, then cleared: the no-sync forwards
+ * whose tile instances exceeded the capacity they ran with (the placement clamps: those images are incomplete, nothing is
+ * written out of bounds) and the FP16x2 range flag of G4D_OPT_TENSOR_CORES.  sync != 0: synchronise the device first;
+ * sync == 0 is only valid when no replay on ws can still be running (the record is updated without atomics). */
+typedef struct G4DGraphStatus {
+    int64_t overflows;      /* captured forwards whose instance count exceeded their capacity */
+    int64_t max_instances;  /* the largest such instance count (0 when overflows == 0) */
+    int32_t f16_range;      /* 1: an FP16x2 tensor-core launch met a value outside the f16 operand range */
+    int32_t reserved;
+} G4DGraphStatus;
+int g4d_context_set_time_source(G4DContext *ctx, const float *d_time);
+int g4d_workspace_freeze(G4DWorkspace *ws, int on);
+int g4d_workspace_graph_status(G4DWorkspace *ws, int sync, G4DGraphStatus *out);
 
 #ifdef __cplusplus
 }
