@@ -115,6 +115,25 @@ struct WeightCache {
 // R: launch_record_overflow)
 struct PinnedWords { uint32_t num_rendered, pad0[7], f16_range, pad1[7], overflow[2], pad2[6]; };
 
+// The forward a context holds.  A forward entry point clears the record of every context it writes before its first launch
+// and writes each one whole once the entry point has succeeded; an overflow found by a no-sync read-back clears it.  The
+// backward entry points, g4d_context_read and g4d_context_stats decide from the record alone what the context holds.
+struct ForwardRecord {
+    enum Kind { kNone, kRaster, kFused };   // kRaster: g4d_rasterize_forward; kFused: g4d_render_forward(_cameras)
+    Kind kind = kNone;
+    int64_t n = 0;
+    int H = 0, W = 0;
+    bool deformed = false;    // the deformation network ran (fine stage)
+    bool sh = false;          // the SHS head was active: the deformed SH coefficients are in fo.shs
+    bool kept = false;        // fo holds the deformed, activated tensors
+    int feat_cols = 0;        // F of the HexPlane features in `feat` and the ReLU bits in `relu` kept for a backward (0: none)
+    // g4d_render_forward_cameras: serial number of the call (0: a single-camera forward), this camera's position, the number
+    // of cameras, and whether the group keeps what its backward reads
+    uint64_t group = 0;
+    int group_pos = 0, group_size = 0;
+    bool group_grad = false;
+};
+
 }  // namespace
 
 struct G4DWorkspace {
@@ -147,21 +166,12 @@ struct G4DWorkspace {
 struct G4DContext {
     G4DWorkspace* ws = nullptr;
     DevBuf cam, geom, bin, binaux, img, fused, gscratch, gdeform, trow, relu, feat;
-    bool relu_saved = false;
-    int feat_cols = 0;                // F of the features in `feat` (when relu_saved)
-    int64_t n = 0;
-    int H = 0, W = 0, grid_x = 0, grid_y = 0;
+    ForwardRecord fwd;
+    int grid_x = 0, grid_y = 0;
     int64_t R = 0, capacity = 0;
     const float* time_src = nullptr;  // g4d_context_set_time_source (device; NULL: G4DCamera.time)
     const void* bin_ctl = nullptr;    // device BinCtl of the last forward
     bool learned = false;             // R of an earlier exact forward is known (no-sync mode needs a learnt capacity)
-    bool has_forward = false, is_fused = false, fused_sh = false, deformed = false, fo_valid = false;
-    // multi-camera forward (g4d_render_forward_cameras) whose state this context holds: serial number of that call (0: the
-    // last forward was a single-camera one), this camera's position and the number of cameras; on camera 0, whether the
-    // forward kept what the group backward reads
-    uint64_t group = 0;
-    int group_pos = 0, group_size = 0;
-    bool group_grad = false;
     GeomBuffers g{};
     BinBuffers b{};
     ImageBuffers im{};
@@ -265,7 +275,7 @@ int ensure_image(G4DContext* c, int H, int W) {
         c->b.ranges = m.take<uint2>((size_t)gx * gy);
     };
     G4D_CUDA(ensure_layout(c->img, layout));
-    c->H = H; c->W = W; c->grid_x = gx; c->grid_y = gy;
+    c->grid_x = gx; c->grid_y = gy;
     return G4D_OK;
 }
 
@@ -290,6 +300,19 @@ int ensure_fused(G4DContext* c, int64_t n, bool with_sh) {
     };
     G4D_CUDA(ensure_layout(c->fused, layout));
     return G4D_OK;
+}
+
+// The set-up of one view on c: the buffers of n Gaussians and of the camera's image, the stage flags, and in the PREP stage
+// the device camera (timestamp from d_time when set), then prep()
+template <class Prep>
+int setup_view(G4DContext* c, const G4DCamera* cam, const float* d_time, int64_t n, cudaStream_t st, Prep prep) {
+    int rc;
+    if ((rc = ensure_geom(c, n)) != G4D_OK) return rc;
+    if ((rc = ensure_image(c, cam->image_height, cam->image_width)) != G4D_OK) return rc;
+    reset_stage_flags(c, 0, G4D_STAGE_COUNT - 1);
+    StageTimer tm(c, G4D_STAGE_PREP, st);
+    G4D_CUDA(launch_pack_camera(*cam, d_time, c->cam.as<CameraDev>(), st));
+    return prep();
 }
 
 int check_params(const G4DDeformParams* p) {
@@ -488,7 +511,7 @@ int check_pending(G4DContext* c) {
         if (c->R > c->used_capacity[s]) {
             const int64_t need = c->R + c->R / 2;
             if (need > c->ws->min_capacity) c->ws->min_capacity = need;
-            c->has_forward = false;
+            c->fwd = ForwardRecord{};
             char msg[160];
             snprintf(msg, sizeof(msg), "%lld tile instances did not fit the capacity of %lld used by an earlier no-sync forward; its image is incomplete",
                      (long long)c->R, (long long)c->used_capacity[s]);
@@ -560,10 +583,7 @@ int bin_and_blend(G4DContext* c, const G4DCamera* cam, int64_t n, float* out_col
         G4D_CUDA(cudaEventRecord(c->ev_r[sl], st));
         c->pending[sl] = true; c->used_capacity[sl] = c->capacity;
     }
-    if ((rc = debug_sync(cam, st, "blend_forward")) != G4D_OK) return rc;
-    c->n = n;
-    c->has_forward = true;
-    return G4D_OK;
+    return debug_sync(cam, st, "blend_forward");
 }
 
 // A caller's SH tensors: fused [N,16,3] in dc, or (split) dc [N,1,3] + rest [N,15,3].  Sh = ShIn for the coefficients,
@@ -576,14 +596,16 @@ template <class Sh, class T> Sh caller_sh(bool split, T* dc, T* rest = nullptr) 
 int raster_backward_stages(G4DContext* c, const G4DCamera* cam, int64_t n, const RasterInputs& in, const float* dL_dcolor,
                            float* g_means3D, float* g_means2D, const ShOut& g_sh, float* g_opacities, float* g_scales,
                            float* g_rotations, cudaStream_t st) {
+    using L = BlendGradLayout;
     const CameraDev* dcam = c->cam.as<CameraDev>();
     const size_t N = (size_t)(n > 0 ? n : 1);
-    G4D_CUDA(c->gscratch.ensure(N * 8 * 4 + 256));
-    float* g_mean2D = c->gscratch.as<float>();
-    float* g_conic = g_mean2D + 2 * N;
-    float* g_rgb = g_conic + 3 * N;
+    G4D_CUDA(c->gscratch.ensure(N * L::kOpacity * 4 + 256));   // (the opacity block is the caller's g_opacities)
+    float* gb = c->gscratch.as<float>();
+    float* g_mean2D = gb + L::kMean2D * N;
+    float* g_conic = gb + L::kConic * N;
+    float* g_rgb = gb + L::kRgb * N;
     if (n == 0) return G4D_OK;
-    G4D_CUDA(cudaMemsetAsync(g_mean2D, 0, N * 8 * 4, st));
+    G4D_CUDA(cudaMemsetAsync(gb, 0, N * L::kOpacity * 4, st));
     G4D_CUDA(cudaMemsetAsync(g_opacities, 0, N * 4, st));
     reset_stage_flags(c, G4D_STAGE_BLEND_BWD, G4D_STAGE_DEFORM_BWD);
     {
@@ -685,13 +707,13 @@ int g4d_context_stage_times(G4DContext* c, float* out_ms, int capacity) {
 
 int g4d_context_stats(G4DContext* c, G4DStats* out) {
     if (!c || !out) return fail(G4D_ERR_ARG, "NULL argument");
-    if (!c->has_forward) return fail(G4D_ERR_STATE, "no forward has run on this context");
+    if (c->fwd.kind == ForwardRecord::kNone) return fail(G4D_ERR_STATE, "no forward has run on this context");
     cudaSetDevice(c->ws->device);
     G4D_CUDA(cudaDeviceSynchronize());
     { int rc_ = check_pending(c); if (rc_ != G4D_OK) return rc_; }
     out->num_rendered = c->R; out->instance_capacity = c->capacity; out->tiles_x = c->grid_x; out->tiles_y = c->grid_y;
-    std::vector<int32_t> radii((size_t)c->n);
-    if (c->n) G4D_CUDA(cudaMemcpy(radii.data(), c->g.radii, (size_t)c->n * 4, cudaMemcpyDeviceToHost));
+    std::vector<int32_t> radii((size_t)c->fwd.n);
+    if (c->fwd.n) G4D_CUDA(cudaMemcpy(radii.data(), c->g.radii, (size_t)c->fwd.n * 4, cudaMemcpyDeviceToHost));
     int64_t vis = 0;
     for (int32_t r : radii) vis += r > 0;
     out->num_visible = vis;
@@ -738,20 +760,16 @@ int g4d_rasterize_forward(G4DContext* c, const G4DCamera* cam, int64_t n, const 
     if (scope.rc != G4D_OK) return scope.rc;
     if ((rc = refuse_capture(c->ws, cam, 1, &c)) != G4D_OK) return rc;
     if ((rc = check_pending(c)) != G4D_OK) return rc;
-    c->has_forward = false; c->is_fused = false; c->deformed = false; c->group = 0;
-    if ((rc = ensure_geom(c, n)) != G4D_OK) return rc;
-    if ((rc = ensure_image(c, cam->image_height, cam->image_width)) != G4D_OK) return rc;
-    reset_stage_flags(c, 0, G4D_STAGE_COUNT - 1);
-    {
-        StageTimer tm(c, G4D_STAGE_PREP, st);
-        G4D_CUDA(launch_pack_camera(*cam, nullptr, c->cam.as<CameraDev>(), st));
-    }
+    c->fwd = ForwardRecord{};
+    if ((rc = setup_view(c, cam, nullptr, n, st, [] { return G4D_OK; })) != G4D_OK) return rc;
     const RasterInputs in{means3D, scales, rotations, opacities, caller_sh<ShIn>(false, shs)};
     {
         StageTimer tm(c, G4D_STAGE_GEOM, st);
         G4D_CUDA(launch_preprocess(c->cam.as<CameraDev>(), n, in, c->g, out_radii, st));
     }
-    return bin_and_blend(c, cam, n, out_color, out_depth, st);
+    if ((rc = bin_and_blend(c, cam, n, out_color, out_depth, st)) != G4D_OK) return rc;
+    c->fwd = ForwardRecord{ForwardRecord::kRaster, n, cam->image_height, cam->image_width};
+    return G4D_OK;
 }
 
 int g4d_rasterize_backward(G4DContext* c, const G4DCamera* cam, int64_t n, const float* means3D, const float* shs,
@@ -759,10 +777,10 @@ int g4d_rasterize_backward(G4DContext* c, const G4DCamera* cam, int64_t n, const
                            float* g_means3D, float* g_means2D, float* g_shs, float* g_opacities, float* g_scales,
                            float* g_rotations, void* stream) {
     if (!c) return fail(G4D_ERR_ARG, "context is NULL");
-    if (!c->has_forward || c->is_fused || c->n != n) return fail(G4D_ERR_STATE, "g4d_rasterize_backward needs the matching g4d_rasterize_forward on this context");
+    if (c->fwd.kind != ForwardRecord::kRaster || c->fwd.n != n) return fail(G4D_ERR_STATE, "g4d_rasterize_backward needs the matching g4d_rasterize_forward on this context");
     int rc = check_camera(cam);
     if (rc != G4D_OK) return rc;
-    if (cam->image_height != c->H || cam->image_width != c->W) return fail(G4D_ERR_STATE, "camera differs from the forward's");
+    if (cam->image_height != c->fwd.H || cam->image_width != c->fwd.W) return fail(G4D_ERR_STATE, "camera differs from the forward's");
     if (!dL_dcolor || (n > 0 && (!g_means3D || !g_means2D || !g_shs || !g_opacities || !g_scales || !g_rotations)))
         return fail(G4D_ERR_ARG, "NULL gradient pointer");
     cudaStream_t st = (cudaStream_t)stream;
@@ -779,11 +797,11 @@ int g4d_rasterize_backward(G4DContext* c, const G4DCamera* cam, int64_t n, const
 
 // ------------------------------------------------------------------------------------------------------
 int64_t g4d_context_read(G4DContext* c, int which, void* host_dst, int64_t bytes) {
-    if (!c || !c->has_forward) return fail(G4D_ERR_STATE, "no forward has run on this context");
+    if (!c || c->fwd.kind == ForwardRecord::kNone) return fail(G4D_ERR_STATE, "no forward has run on this context");
     cudaSetDevice(c->ws->device);
     if (cudaDeviceSynchronize() != cudaSuccess) return fail(G4D_ERR_CUDA, "cudaDeviceSynchronize");
     { int rc_ = check_pending(c); if (rc_ != G4D_OK) return rc_; }
-    const size_t N = (size_t)c->n, P = (size_t)c->H * c->W, R = (size_t)c->R, Tn = (size_t)c->grid_x * c->grid_y;
+    const size_t N = (size_t)c->fwd.n, P = (size_t)c->fwd.H * c->fwd.W, R = (size_t)c->R, Tn = (size_t)c->grid_x * c->grid_y;
     std::vector<char> tmp;
     auto pull = [&](const void* src, size_t nbytes) -> bool {
         tmp.resize(nbytes ? nbytes : 1);
@@ -841,7 +859,7 @@ int64_t g4d_context_read(G4DContext* c, int which, void* host_dst, int64_t bytes
             for (size_t i = 0; i < N && ok; ++i) for (int ch = 0; ch < 3; ++ch) outv[i * 3 + ch] = (tmp[i] >> ch) & 1;
         } break;
         case G4D_BUF_DEFORMED: {
-            if (!c->is_fused || !c->fo_valid) return fail(G4D_ERR_STATE, "G4D_BUF_DEFORMED needs a fused forward that kept its tensors (grad-enabled, or G4D_OPT_KEEP_DEFORMED)");
+            if (!c->fwd.kept) return fail(G4D_ERR_STATE, "G4D_BUF_DEFORMED needs a fused forward that kept its tensors (grad-enabled, or G4D_OPT_KEEP_DEFORMED)");
             outv.resize(N * 44);
             std::vector<float> m(N * 3), s(N * 3), r(N * 4), o(N);
             ok = N == 0 || (cudaMemcpy(m.data(), c->fo.means3D, N * 12, cudaMemcpyDeviceToHost) == cudaSuccess &&
@@ -855,7 +873,7 @@ int64_t g4d_context_read(G4DContext* c, int which, void* host_dst, int64_t bytes
             }
         } break;
         case G4D_BUF_DEFORMED_SHS: {
-            if (!c->is_fused || !c->fused_sh || !c->fo.shs || !c->fo_valid) return fail(G4D_ERR_STATE, "G4D_BUF_DEFORMED_SHS needs a fused forward with the SHS head active");
+            if (!c->fwd.kept || !c->fwd.sh) return fail(G4D_ERR_STATE, "G4D_BUF_DEFORMED_SHS needs a fused forward with the SHS head active");
             ok = pull(c->fo.shs, N * 192); outv = tmp; outv.resize(N * 192);
         } break;
         case G4D_BUF_BIN_PHASES: {
@@ -863,8 +881,8 @@ int64_t g4d_context_read(G4DContext* c, int which, void* host_dst, int64_t bytes
             ok = pull(reinterpret_cast<const char*>(c->bin_ctl) + 16, 16 * 8); outv = tmp; outv.resize(16 * 8);
         } break;
         case G4D_BUF_FEATURES: {
-            if (!c->is_fused || !c->deformed || !c->relu_saved) return fail(G4D_ERR_STATE, "G4D_BUF_FEATURES needs a grad-enabled tensor-core fused forward");
-            const size_t nb = N * (size_t)c->feat_cols * 4;
+            if (!c->fwd.feat_cols) return fail(G4D_ERR_STATE, "G4D_BUF_FEATURES needs a grad-enabled tensor-core fused forward");
+            const size_t nb = N * (size_t)c->fwd.feat_cols * 4;
             ok = pull(c->feat.p, nb); outv = tmp; outv.resize(nb);
         } break;
         case G4D_BUF_GATHER_ORDER: {
@@ -917,131 +935,118 @@ int check_render_args(const G4DCamera* cam, const G4DDeformParams* prm, const G4
     return G4D_OK;
 }
 
-// The fused forward of one camera on c.  keep_fo: store the deformed, activated tensors even under G4D_CAM_NO_GRAD (other
-// cameras of the same call read them).
+// The fused forward of one camera on c; *rec: the record of c once the calling entry point has succeeded.  keep_fo: store
+// the deformed, activated tensors even under G4D_CAM_NO_GRAD (other cameras of the same call read them).
 int fused_forward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* prm, const G4DGaussians* g, float* out_color,
-                  float* out_depth, int32_t* out_radii, bool keep_fo, cudaStream_t st) {
+                  float* out_depth, int32_t* out_radii, bool keep_fo, cudaStream_t st, ForwardRecord* rec) {
     const int64_t n = g->n;
     G4DWorkspace* ws = c->ws;
     int rc;
-    G4D_CUDA(cudaSetDevice(ws->device));
-    if ((rc = check_pending(c)) != G4D_OK) return rc;
-    c->has_forward = false; c->group = 0;
     const bool with_sh = prm && (prm->head_mask & G4D_HEAD_SHS);
-    if ((rc = ensure_geom(c, n)) != G4D_OK) return rc;
-    if ((rc = ensure_image(c, cam->image_height, cam->image_width)) != G4D_OK) return rc;
+    // a no-grad render needs none of the saved tensors: skip their stores (48 B + 192 B of deformed SH per Gaussian)
+    const bool kept = !(cam->debug & G4D_CAM_NO_GRAD) || ws->keep_deformed || keep_fo;
+    *rec = ForwardRecord{ForwardRecord::kFused, n, cam->image_height, cam->image_width, prm != nullptr, with_sh, kept};
     if ((rc = ensure_fused(c, n, with_sh)) != G4D_OK) return rc;
     CameraDev* dcam = c->cam.as<CameraDev>();
-    reset_stage_flags(c, 0, G4D_STAGE_COUNT - 1);
-    // a no-grad render needs none of the saved tensors: skip their stores (48 B + 192 B of deformed SH per Gaussian)
-    c->fo_valid = !(cam->debug & G4D_CAM_NO_GRAD) || ws->keep_deformed || keep_fo;
-    const FusedOutputs fo_arg = c->fo_valid ? c->fo : FusedOutputs{};
     DeformSetup s{};
-    {
-        StageTimer tm(c, G4D_STAGE_PREP, st);
-        G4D_CUDA(launch_pack_camera(*cam, c->time_src, dcam, st));
-        if (prm && (rc = setup_deform(ws, prm, g->xyz, n, c->trow, c->trow_ptr, TimeArg{cam->time, c->time_src}, st, &s)) != G4D_OK)
-            return rc;
-    }
+    auto prep = [&] {
+        return prm ? setup_deform(ws, prm, g->xyz, n, c->trow, c->trow_ptr, TimeArg{cam->time, c->time_src}, st, &s) : G4D_OK;
+    };
+    if ((rc = setup_view(c, cam, c->time_src, n, st, prep)) != G4D_OK) return rc;
     {
         StageTimer tm(c, G4D_STAGE_GEOM, st);
         const DeformIO io{g->xyz, g->scaling, g->rotation, g->opacity,
                           caller_sh<ShIn>(g->features_rest != nullptr, g->features_dc, g->features_rest),
-                          nullptr, nullptr, nullptr, nullptr, nullptr, c->g, fo_arg, out_radii};
+                          nullptr, nullptr, nullptr, nullptr, nullptr, c->g, kept ? c->fo : FusedOutputs{}, out_radii};
         if (prm) {
-            c->relu_saved = s.tc && !(cam->debug & G4D_CAM_NO_GRAD);
-            if (c->relu_saved) {   // a backward will follow: it re-uses the ReLU signs and the staged HexPlane features
+            const bool save = s.tc && !(cam->debug & G4D_CAM_NO_GRAD);
+            if (save) {   // a backward will follow: it re-uses the ReLU signs and the staged HexPlane features
                 G4D_CUDA(c->relu.ensure(G4D_RELU_BITS_WORDS(n) * 4));
                 G4D_CUDA(c->feat.ensure((size_t)(n > 0 ? n : 1) * (size_t)s.d.F * 4 + 256));
-                c->feat_cols = s.d.F;
+                rec->feat_cols = s.d.F;
             }
-            if ((rc = attach_forward_buffers(ws, s, c->relu_saved ? c->feat.as<float>() : nullptr,
-                                             c->relu_saved ? c->relu.as<uint32_t>() : nullptr, n, st)) != G4D_OK) return rc;
+            if ((rc = attach_forward_buffers(ws, s, save ? c->feat.as<float>() : nullptr, save ? c->relu.as<uint32_t>() : nullptr,
+                                             n, st)) != G4D_OK) return rc;
             G4D_CUDA(launch_deform(s.d, 1, dcam, n, io, ws->sm_count, st, s.tc ? &s.tw : nullptr));
         } else {
             G4D_CUDA(launch_activate_preprocess(dcam, n, io, st));
         }
     }
     if ((rc = debug_sync(cam, st, "deform+preprocess")) != G4D_OK) return rc;
-    rc = bin_and_blend(c, cam, n, out_color, out_depth, st);
-    if (rc != G4D_OK) return rc;
-    c->is_fused = true; c->deformed = prm != nullptr; c->fused_sh = with_sh;
-    return G4D_OK;
+    return bin_and_blend(c, cam, n, out_color, out_depth, st);
 }
 
 // the post-activation inputs of the rasterizer stages of a fused forward on c: its stored deformed tensors, and the SH
-// coefficients (deformed when the SHS head is active, the caller's otherwise)
-RasterInputs deformed_inputs(const G4DContext* c, const G4DGaussians* g) {
+// coefficients (deformed when the SHS head was active, the caller's otherwise)
+RasterInputs deformed_inputs(const G4DContext* c, bool sh, const G4DGaussians* g) {
     RasterInputs in{c->fo.means3D, c->fo.scales, c->fo.rotations, c->fo.opacities,
                     caller_sh<ShIn>(g->features_rest != nullptr, g->features_dc, g->features_rest)};
-    if (c->fused_sh) in.sh = ShIn{c->fo.shs, nullptr, nullptr};
+    if (sh) in.sh = ShIn{c->fo.shs, nullptr, nullptr};
     return in;
 }
 
-// gradients w.r.t. the deformed tensors of a fine-stage backward: scratch on c (the network's backward reads them)
+// Gradients w.r.t. the deformed tensors of the backward of a fused forward on c: the caller's sinks in the coarse stage,
+// scratch on c in the fine stage (the network's backward reads them)
 struct DeformedGrads { float *xyz, *sc, *rot, *op, *sh; };
-int deformed_grads(G4DContext* c, int64_t n, DeformedGrads* out) {
+int deformed_grads(G4DContext* c, int64_t n, const G4DGaussianGrads* gg, DeformedGrads* out) {
     const size_t N = (size_t)n;
     DeformedGrads& d = *out;
+    d = DeformedGrads{gg->xyz, gg->scaling, gg->rotation, gg->opacity, nullptr};
+    if (!c->fwd.deformed) return G4D_OK;
     auto layout = [&](Carve& m) {
         d.xyz = m.take<float>(3 * N); d.sc = m.take<float>(3 * N); d.rot = m.take<float>(4 * N); d.op = m.take<float>(N);
-        d.sh = m.take<float>(c->fused_sh ? 48 * N : 4);
+        d.sh = m.take<float>(c->fwd.sh ? 48 * N : 4);
     };
     G4D_CUDA(ensure_layout(c->gdeform, layout));
-    if (!c->fused_sh) d.sh = nullptr;
+    if (!c->fwd.sh) d.sh = nullptr;
     return G4D_OK;
 }
 
 // The SH gradient sinks of the backward of a fused forward on c: the caller's.  With the SHS head active the gradient also
-// feeds the network's backward: the fused sink is then the scratch d_sh, which copy_fused_sh_grad passes on to a caller sink
-// in the fused layout.
+// feeds the network's backward: the fused sink is then the scratch d_sh, which fused_backward_tail passes on to a caller
+// sink in the fused layout.
 ShOut fused_sh_sinks(const G4DContext* c, const G4DGaussians* g, const G4DGaussianGrads* gg, float* d_sh) {
     ShOut o = caller_sh<ShOut>(g->features_rest != nullptr, gg->features_dc, gg->features_rest);
-    if (c->fused_sh) o.shs = d_sh;
+    if (c->fwd.sh) o.shs = d_sh;
     return o;
 }
-int copy_fused_sh_grad(const G4DContext* c, const G4DGaussians* g, const G4DGaussianGrads* gg, const float* d_sh, cudaStream_t st) {
-    if (c->fused_sh && !g->features_rest)
-        G4D_CUDA(cudaMemcpyAsync(gg->features_dc, d_sh, (size_t)g->n * 192, cudaMemcpyDeviceToDevice, st));
-    return G4D_OK;
+
+// The tail of the backward of a fused forward on c, after its per-Gaussian backward wrote d: the SH gradient copy, the
+// activation backward and, in the fine stage, the network's backward.  cam: the camera whose time and debug flag it uses.
+int fused_backward_tail(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* prm, G4DDeformGrads* pgrads,
+                        const G4DGaussians* g, const G4DGaussianGrads* gg, const DeformedGrads& d, cudaStream_t st) {
+    const int64_t n = g->n;
+    int rc;
+    if (c->fwd.sh && !g->features_rest)
+        G4D_CUDA(cudaMemcpyAsync(gg->features_dc, d.sh, (size_t)n * 192, cudaMemcpyDeviceToDevice, st));
+    G4D_CUDA(launch_activation_backward(n, c->fo, d.sc, d.rot, d.op, st));
+    if (!c->fwd.deformed) return debug_sync(cam, st, "activation_backward");
+    const float* go[G4D_NUM_HEADS] = {d.xyz, d.sc, d.rot, d.op, d.sh};
+    float* gi[G4D_NUM_HEADS] = {gg->xyz, gg->scaling, gg->rotation, gg->opacity, nullptr};
+    const bool saved = c->fwd.feat_cols != 0;
+    {
+        StageTimer tm(c, G4D_STAGE_DEFORM_BWD, st);
+        if ((rc = deform_backward_dispatch(c->ws, prm, c->trow_ptr, pgrads, TimeArg{cam->time, c->time_src}, n, g->xyz, go, gi,
+                                           saved ? c->relu.as<uint32_t>() : nullptr, saved ? c->feat.as<float>() : nullptr,
+                                           st)) != G4D_OK) return rc;
+    }
+    return debug_sync(cam, st, "deform_backward");
 }
 
 // The backward of a fused forward of one camera on c (arguments checked by the caller).  gg->means2D may be NULL.
 int fused_backward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* prm, G4DDeformGrads* pgrads, const G4DGaussians* g,
                    const float* dL_dcolor, const G4DGaussianGrads* gg, cudaStream_t st) {
     const int64_t n = g->n;
-    G4DWorkspace* ws = c->ws;
     int rc;
-    G4D_CUDA(cudaSetDevice(ws->device));
-    if ((rc = check_pending(c)) != G4D_OK) return rc;
     if (n == 0) return G4D_OK;
-    const RasterInputs in = deformed_inputs(c, g);
-    if (!c->deformed) {
-        rc = raster_backward_stages(c, cam, n, in, dL_dcolor, gg->xyz, gg->means2D, fused_sh_sinks(c, g, gg, nullptr),
-                                    gg->opacity, gg->scaling, gg->rotation, st);
-        if (rc != G4D_OK) return rc;
-        G4D_CUDA(launch_activation_backward(n, c->fo, gg->scaling, gg->rotation, gg->opacity, st));
-        return debug_sync(cam, st, "activation_backward");
-    }
-    // gradients w.r.t. the deformed tensors land in scratch, then flow through the deformation network
     DeformedGrads d;
-    if ((rc = deformed_grads(c, n, &d)) != G4D_OK) return rc;
+    if ((rc = deformed_grads(c, n, gg, &d)) != G4D_OK) return rc;
     // SH gradient: identity residual path -> written straight into the caller's sinks; the fused copy (when the SHS
     // head is active) additionally feeds the network's backward
-    rc = raster_backward_stages(c, cam, n, in, dL_dcolor, d.xyz, gg->means2D, fused_sh_sinks(c, g, gg, d.sh), d.op, d.sc, d.rot,
-                                st);
+    rc = raster_backward_stages(c, cam, n, deformed_inputs(c, c->fwd.sh, g), dL_dcolor, d.xyz, gg->means2D,
+                                fused_sh_sinks(c, g, gg, d.sh), d.op, d.sc, d.rot, st);
     if (rc != G4D_OK) return rc;
-    if ((rc = copy_fused_sh_grad(c, g, gg, d.sh, st)) != G4D_OK) return rc;
-    G4D_CUDA(launch_activation_backward(n, c->fo, d.sc, d.rot, d.op, st));
-    const float* go[G4D_NUM_HEADS] = {d.xyz, d.sc, d.rot, d.op, d.sh};
-    float* gi[G4D_NUM_HEADS] = {gg->xyz, gg->scaling, gg->rotation, gg->opacity, nullptr};
-    {
-        StageTimer tm(c, G4D_STAGE_DEFORM_BWD, st);
-        if ((rc = deform_backward_dispatch(ws, prm, c->trow_ptr, pgrads, TimeArg{cam->time, c->time_src}, n, g->xyz, go, gi,
-                                           c->relu_saved ? c->relu.as<uint32_t>() : nullptr,
-                                           c->relu_saved ? c->feat.as<float>() : nullptr, st)) != G4D_OK) return rc;
-    }
-    return debug_sync(cam, st, "deform_backward");
+    return fused_backward_tail(c, cam, prm, pgrads, g, gg, d, st);
 }
 
 // k cameras on k contexts: 1 <= k <= G4D_MAX_CAMERAS, one time bit for bit (or, when ctx[0] has a time source, that same
@@ -1085,21 +1090,26 @@ int g4d_render_forward(G4DContext* c, const G4DCamera* cam, const G4DDeformParam
     CallScope scope(c->ws, st);
     if (scope.rc != G4D_OK) return scope.rc;
     if ((rc = refuse_capture(c->ws, cam, 1, &c)) != G4D_OK) return rc;
-    return fused_forward(c, cam, prm, g, out_color, out_depth, out_radii, false, st);
+    if ((rc = check_pending(c)) != G4D_OK) return rc;
+    c->fwd = ForwardRecord{};
+    ForwardRecord rec;
+    if ((rc = fused_forward(c, cam, prm, g, out_color, out_depth, out_radii, false, st, &rec)) != G4D_OK) return rc;
+    c->fwd = rec;
+    return G4D_OK;
 }
 
 int g4d_render_backward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* prm, G4DDeformGrads* pgrads,
                         const G4DGaussians* g, const float* dL_dcolor, G4DGaussianGrads* gg, void* stream) {
     if (!c) return fail(G4D_ERR_ARG, "context is NULL");
-    if (!c->has_forward || !c->is_fused || !g || c->n != g->n) return fail(G4D_ERR_STATE, "g4d_render_backward needs the matching g4d_render_forward on this context");
-    if (c->group) return fail(G4D_ERR_STATE, "the last forward on this context was g4d_render_forward_cameras: use g4d_render_backward_cameras");
-    if (!c->fo_valid) return fail(G4D_ERR_STATE, "g4d_render_backward after a G4D_CAM_NO_GRAD forward: nothing was saved for it");
-    if ((prm != nullptr) != c->deformed) return fail(G4D_ERR_STATE, "deform params differ from the forward's");
+    if (c->fwd.kind != ForwardRecord::kFused || !g || c->fwd.n != g->n) return fail(G4D_ERR_STATE, "g4d_render_backward needs the matching g4d_render_forward on this context");
+    if (c->fwd.group) return fail(G4D_ERR_STATE, "the last forward on this context was g4d_render_forward_cameras: use g4d_render_backward_cameras");
+    if (!c->fwd.kept) return fail(G4D_ERR_STATE, "g4d_render_backward after a G4D_CAM_NO_GRAD forward: nothing was saved for it");
+    if ((prm != nullptr) != c->fwd.deformed) return fail(G4D_ERR_STATE, "deform params differ from the forward's");
     int rc = check_camera(cam);
     if (rc != G4D_OK) return rc;
     if (prm && (rc = check_params(prm)) != G4D_OK) return rc;
     if (prm && !pgrads) return fail(G4D_ERR_ARG, "pgrads is NULL");
-    if (cam->image_height != c->H || cam->image_width != c->W) return fail(G4D_ERR_STATE, "camera differs from the forward's");
+    if (cam->image_height != c->fwd.H || cam->image_width != c->fwd.W) return fail(G4D_ERR_STATE, "camera differs from the forward's");
     const int64_t n = g->n;
     if (!dL_dcolor || !gg || (n > 0 && (!gg->xyz || !gg->scaling || !gg->rotation || !gg->opacity || !gg->features_dc || !gg->means2D)))
         return fail(G4D_ERR_ARG, "NULL gradient pointer");
@@ -1109,6 +1119,7 @@ int g4d_render_backward(G4DContext* c, const G4DCamera* cam, const G4DDeformPara
     CallScope scope(c->ws, st);
     if (scope.rc != G4D_OK) return scope.rc;
     if ((rc = refuse_capture(c->ws, cam, 1, nullptr)) != G4D_OK) return rc;
+    if ((rc = check_pending(c)) != G4D_OK) return rc;
     return fused_backward(c, cam, prm, pgrads, g, dL_dcolor, gg, st);
 }
 
@@ -1129,39 +1140,36 @@ int g4d_render_forward_cameras(G4DContext* const* ctx, int32_t k, const G4DCamer
     if ((rc = refuse_capture(c0->ws, cams, k, ctx)) != G4D_OK) return rc;
     for (int i = 0; i < k; ++i) {
         if ((rc = check_pending(ctx[i])) != G4D_OK) return rc;
-        ctx[i]->has_forward = false; ctx[i]->group = 0;
+        ctx[i]->fwd = ForwardRecord{};
     }
     // camera 0: the fused forward of g4d_render_forward; it keeps the deformed tensors when other cameras read them
-    if ((rc = fused_forward(c0, &cams[0], prm, g, out_color[0], out_depth[0], out_radii[0], k > 1, st)) != G4D_OK) return rc;
+    ForwardRecord r0;
+    if ((rc = fused_forward(c0, &cams[0], prm, g, out_color[0], out_depth[0], out_radii[0], k > 1, st, &r0)) != G4D_OK) return rc;
     const int64_t n = g->n;
     if (k > 1) {
         ExtraCameras ec{};
         ec.count = k - 1;
         for (int i = 1; i < k; ++i) {
             G4DContext* c = ctx[i];
-            if ((rc = ensure_geom(c, n)) != G4D_OK) return rc;
-            if ((rc = ensure_image(c, cams[i].image_height, cams[i].image_width)) != G4D_OK) return rc;
-            reset_stage_flags(c, 0, G4D_STAGE_COUNT - 1);
-            {
-                StageTimer tm(c, G4D_STAGE_PREP, st);
-                G4D_CUDA(launch_pack_camera(cams[i], c->time_src, c->cam.as<CameraDev>(), st));
-            }
+            if ((rc = setup_view(c, &cams[i], c->time_src, n, st, [] { return G4D_OK; })) != G4D_OK) return rc;
             ec.cam[i - 1] = c->cam.as<CameraDev>(); ec.g[i - 1] = c->g; ec.out_radii[i - 1] = out_radii[i];
         }
         {
             StageTimer tm(ctx[1], G4D_STAGE_GEOM, st);
-            G4D_CUDA(launch_project_cameras(ec, n, deformed_inputs(c0, g), st));
+            G4D_CUDA(launch_project_cameras(ec, n, deformed_inputs(c0, r0.sh, g), st));
         }
         if ((rc = debug_sync(&cams[1], st, "project_cameras")) != G4D_OK) return rc;
-        for (int i = 1; i < k; ++i) {
-            G4DContext* c = ctx[i];
-            if ((rc = bin_and_blend(c, &cams[i], n, out_color[i], out_depth[i], st)) != G4D_OK) return rc;
-            c->is_fused = true; c->deformed = c0->deformed; c->fused_sh = c0->fused_sh; c->fo_valid = false;
-        }
+        for (int i = 1; i < k; ++i)
+            if ((rc = bin_and_blend(ctx[i], &cams[i], n, out_color[i], out_depth[i], st)) != G4D_OK) return rc;
     }
+    // cameras 1..k-1 keep nothing of their own for a backward: the group backward reads camera 0's tensors
     const uint64_t serial = ++g_group_serial;
-    for (int i = 0; i < k; ++i) { ctx[i]->group = serial; ctx[i]->group_pos = i; ctx[i]->group_size = k; }
-    c0->group_grad = !(cams[0].debug & G4D_CAM_NO_GRAD);
+    for (int i = 0; i < k; ++i) {
+        ForwardRecord r = i == 0 ? r0 : ForwardRecord{ForwardRecord::kFused, n, cams[i].image_height, cams[i].image_width,
+                                                      r0.deformed, r0.sh};
+        r.group = serial; r.group_pos = i; r.group_size = k; r.group_grad = !(cams[0].debug & G4D_CAM_NO_GRAD);
+        ctx[i]->fwd = r;
+    }
     return G4D_OK;
 }
 
@@ -1174,14 +1182,14 @@ int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCame
     if (gg->means2D) return fail(G4D_ERR_ARG, "gg->means2D must be NULL: the screen-space gradients go to g_means2D[i]");
     G4DContext* c0 = ctx[0];
     for (int i = 0; i < k; ++i) {
-        const G4DContext* c = ctx[i];
-        if (!c->has_forward || !c->group || c->group != c0->group || c->group_pos != i || c->group_size != k || c->n != g->n)
+        const ForwardRecord& f = ctx[i]->fwd;
+        if (f.kind == ForwardRecord::kNone || !f.group || f.group != c0->fwd.group || f.group_pos != i || f.group_size != k || f.n != g->n)
             return fail(G4D_ERR_STATE, "g4d_render_backward_cameras needs the matching g4d_render_forward_cameras on these contexts, "
                                        "with no other forward on any of them since");
-        if (cams[i].image_height != c->H || cams[i].image_width != c->W) return fail(G4D_ERR_STATE, "camera differs from the forward's");
+        if (cams[i].image_height != f.H || cams[i].image_width != f.W) return fail(G4D_ERR_STATE, "camera differs from the forward's");
     }
-    if (!c0->group_grad || !c0->fo_valid) return fail(G4D_ERR_STATE, "g4d_render_backward_cameras after a G4D_CAM_NO_GRAD forward: nothing was saved for it");
-    if ((prm != nullptr) != c0->deformed) return fail(G4D_ERR_STATE, "deform params differ from the forward's");
+    if (!c0->fwd.group_grad || !c0->fwd.kept) return fail(G4D_ERR_STATE, "g4d_render_backward_cameras after a G4D_CAM_NO_GRAD forward: nothing was saved for it");
+    if ((prm != nullptr) != c0->fwd.deformed) return fail(G4D_ERR_STATE, "deform params differ from the forward's");
     if (prm && (rc = check_params(prm)) != G4D_OK) return rc;
     if (prm && !pgrads) return fail(G4D_ERR_ARG, "pgrads is NULL");
     const int64_t n = g->n;
@@ -1202,10 +1210,11 @@ int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCame
         return fused_backward(c0, &cams[0], prm, pgrads, g, dL_dcolor[0], &g1, st);
     }
     if (n == 0) return G4D_OK;
+    using L = BlendGradLayout;
     const size_t N = (size_t)n;
-    DeformedGrads d{gg->xyz, gg->scaling, gg->rotation, gg->opacity, nullptr};   // coarse: straight into the caller's sinks
-    if (c0->deformed && (rc = deformed_grads(c0, n, &d)) != G4D_OK) return rc;
-    // blend backward of every camera in the loss, each into its own scratch: d(mean2D), d(conic), d(rgb), d(opacity)
+    DeformedGrads d;
+    if ((rc = deformed_grads(c0, n, gg, &d)) != G4D_OK) return rc;
+    // blend backward of every camera in the loss, each into its own scratch
     BackwardCameras bc{};
     for (int i = 0; i < k; ++i) {
         G4DContext* c = ctx[i];
@@ -1214,13 +1223,14 @@ int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCame
             if (g_means2D && g_means2D[i]) G4D_CUDA(cudaMemsetAsync(g_means2D[i], 0, N * 12, st));
             continue;
         }
-        G4D_CUDA(c->gscratch.ensure(N * 9 * 4 + 256));
+        G4D_CUDA(c->gscratch.ensure(N * L::kFloats * 4 + 256));
         float* gb = c->gscratch.as<float>();
-        G4D_CUDA(cudaMemsetAsync(gb, 0, N * 9 * 4, st));
+        G4D_CUDA(cudaMemsetAsync(gb, 0, N * L::kFloats * 4, st));
         {
             StageTimer tm(c, G4D_STAGE_BLEND_BWD, st);
-            G4D_CUDA(launch_blend_backward(c->cam.as<CameraDev>(), c->grid_x, c->grid_y, c->g, c->b, c->im, dL_dcolor[i], gb,
-                                           gb + 2 * N, gb + 8 * N, gb + 5 * N, ws->warp_cull, st));
+            G4D_CUDA(launch_blend_backward(c->cam.as<CameraDev>(), c->grid_x, c->grid_y, c->g, c->b, c->im, dL_dcolor[i],
+                                           gb + L::kMean2D * N, gb + L::kConic * N, gb + L::kOpacity * N, gb + L::kRgb * N,
+                                           ws->warp_cull, st));
         }
         if ((rc = debug_sync(&cams[i], st, "blend_backward")) != G4D_OK) return rc;
         const int j = bc.count++;
@@ -1229,23 +1239,12 @@ int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCame
     }
     {
         StageTimer tm(c0, G4D_STAGE_GEOM_BWD, st);
-        G4D_CUDA(launch_preprocess_backward_cameras(bc, n, deformed_inputs(c0, g), d.xyz, d.sc, d.rot, d.op,
+        G4D_CUDA(launch_preprocess_backward_cameras(bc, n, deformed_inputs(c0, c0->fwd.sh, g), d.xyz, d.sc, d.rot, d.op,
                                                     fused_sh_sinks(c0, g, gg, d.sh), st));
     }
     if ((rc = debug_sync(&cams[0], st, "preprocess_backward_cameras")) != G4D_OK) return rc;
-    if ((rc = copy_fused_sh_grad(c0, g, gg, d.sh, st)) != G4D_OK) return rc;
-    G4D_CUDA(launch_activation_backward(n, c0->fo, d.sc, d.rot, d.op, st));
-    if (!c0->deformed) return debug_sync(&cams[0], st, "activation_backward");
     // the network's backward, once, on the gradients summed over the cameras
-    const float* go[G4D_NUM_HEADS] = {d.xyz, d.sc, d.rot, d.op, d.sh};
-    float* gi[G4D_NUM_HEADS] = {gg->xyz, gg->scaling, gg->rotation, gg->opacity, nullptr};
-    {
-        StageTimer tm(c0, G4D_STAGE_DEFORM_BWD, st);
-        if ((rc = deform_backward_dispatch(ws, prm, c0->trow_ptr, pgrads, TimeArg{cams[0].time, c0->time_src}, n, g->xyz, go, gi,
-                                           c0->relu_saved ? c0->relu.as<uint32_t>() : nullptr,
-                                           c0->relu_saved ? c0->feat.as<float>() : nullptr, st)) != G4D_OK) return rc;
-    }
-    return debug_sync(&cams[0], st, "deform_backward");
+    return fused_backward_tail(c0, &cams[0], prm, pgrads, g, gg, d, st);
 }
 
 // ------------------------------------------------------------------------------------------------------

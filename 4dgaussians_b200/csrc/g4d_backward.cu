@@ -106,19 +106,23 @@ preprocess_backward_cameras_kernel(BackwardCameras bc, int64_t n, RasterInputs i
         const float* row = ld + lane * kShRow;
         float* srow = st + lane * kShRow;
         float gm[3] = {0.f, 0.f, 0.f}, gs[3] = {0.f, 0.f, 0.f}, gr[4] = {0.f, 0.f, 0.f, 0.f}, gop = 0.f;
+        using L = BlendGradLayout;
         for (int c = 0; c < bc.count; ++c) {
             const float* gb = bc.grad[c];
-            gop += gb[8 * n + gi];
+            const float* gmb = gb + L::kMean2D * n;
+            const float* gcb = gb + L::kConic * n;
+            const float* grb = gb + L::kRgb * n;
+            gop += gb[L::kOpacity * n + gi];
             const bool vis = bc.radii[c][gi] > 0;
             if (bc.g_means2D[c]) {
-                bc.g_means2D[c][3 * gi] = vis ? gb[2 * gi] : 0.f;
-                bc.g_means2D[c][3 * gi + 1] = vis ? gb[2 * gi + 1] : 0.f;
+                bc.g_means2D[c][3 * gi] = vis ? gmb[2 * gi] : 0.f;
+                bc.g_means2D[c][3 * gi + 1] = vis ? gmb[2 * gi + 1] : 0.f;
                 bc.g_means2D[c][3 * gi + 2] = 0.f;
             }
             if (!vis) continue;
-            const float gm2[2] = {gb[2 * gi], gb[2 * gi + 1]};
-            const float gc[3] = {gb[2 * n + 3 * gi], gb[2 * n + 3 * gi + 1], gb[2 * n + 3 * gi + 2]};
-            const float grgb[3] = {gb[5 * n + 3 * gi], gb[5 * n + 3 * gi + 1], gb[5 * n + 3 * gi + 2]};
+            const float gm2[2] = {gmb[2 * gi], gmb[2 * gi + 1]};
+            const float gc[3] = {gcb[3 * gi], gcb[3 * gi + 1], gcb[3 * gi + 2]};
+            const float grgb[3] = {grb[3 * gi], grb[3 * gi + 1], grb[3 * gi + 2]};
             GaussGrad gg;
             gaussian_backward(cams[c], p, sc, Quat{q4.x, q4.y, q4.z, q4.w}, (uint32_t)bc.clamped[c][gi], gm2, gc, grgb,
                               [&](int k, int ch) { return row[3 * k + ch]; },

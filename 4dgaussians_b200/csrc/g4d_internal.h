@@ -267,6 +267,12 @@ cudaError_t launch_preprocess(const CameraDev* cam, int64_t n, const RasterInput
 cudaError_t launch_deform(const DeformDesc& d, int mode, const CameraDev* cam, int64_t n, const DeformIO& io, int sm_count,
                           cudaStream_t st, const TcWeights* tw = nullptr);
 
+// The per-Gaussian gradients of one blend backward in one float buffer, as blocks of N floats: d(mean2D) [2N] from block
+// kMean2D, d(conic) [3N] from kConic, d(rgb) [3N] from kRgb, d(opacity) [N] from kOpacity; kFloats blocks in all.
+struct BlendGradLayout {
+    static constexpr int kMean2D = 0, kConic = 2, kRgb = 5, kOpacity = 8, kFloats = 9;
+};
+
 cudaError_t launch_blend_forward(const CameraDev* cam, int grid_x, int grid_y, GeomBuffers g, BinBuffers b, ImageBuffers im,
                                  float* out_color, float* out_depth, int warp_cull, cudaStream_t st);
 cudaError_t launch_blend_backward(const CameraDev* cam, int grid_x, int grid_y, GeomBuffers g, BinBuffers b, ImageBuffers im,
@@ -302,7 +308,7 @@ struct BackwardCameras {
     const CameraDev* cam[G4D_MAX_CAMERAS];
     const int32_t* radii[G4D_MAX_CAMERAS];
     const uint8_t* clamped[G4D_MAX_CAMERAS];
-    const float* grad[G4D_MAX_CAMERAS];    // the camera's blend backward: d(mean2D) [2N], d(conic) [3N], d(rgb) [3N], d(opacity) [N]
+    const float* grad[G4D_MAX_CAMERAS];    // the camera's blend backward, BlendGradLayout
     float* g_means2D[G4D_MAX_CAMERAS];     // [N,3] screen-space gradient of the camera, or NULL
 };
 // per-Gaussian backward of all those cameras in one pass: the gradients w.r.t. means3D, scales, rotations, opacity and the
