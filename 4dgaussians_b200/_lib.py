@@ -11,6 +11,8 @@ import os
 import threading
 from typing import Dict, Optional
 
+import torch
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libg4d.so")
 
@@ -187,6 +189,31 @@ def check(rc: int, what: str = "g4d"):
     if rc != 0:
         msg = load().g4d_last_error().decode("utf-8", "replace")
         raise G4DError("%s failed (code %d): %s" % (what, rc, msg))
+
+
+def cuda_f32(t: Optional[torch.Tensor], what: str, numel: Optional[int] = None) -> Optional[torch.Tensor]:
+    """``t`` detached, as a contiguous fp32 CUDA tensor (copied only when it is not one already); None passes through.
+    ``numel``: the element count the call expects."""
+    if t is None:
+        return None
+    if not t.is_cuda:
+        raise RuntimeError("%s must be a CUDA tensor (the g4d path has no CPU fallback)" % what)
+    t = t.detach()
+    if t.dtype != torch.float32 or not t.is_contiguous():
+        t = t.float().contiguous()
+    if numel is not None and t.numel() != numel:
+        raise RuntimeError("%s has %d elements, expected %d" % (what, t.numel(), numel))
+    return t
+
+
+def workspace_of(device: torch.device) -> "Workspace":
+    """The shared workspace of a CUDA device (no index: the current device)."""
+    return Workspace.get(device.index if device.index is not None else torch.cuda.current_device())
+
+
+def stream_of(device: torch.device) -> int:
+    """The device's current stream, as the C-ABI takes it."""
+    return int(torch.cuda.current_stream(device).cuda_stream)
 
 
 class Workspace:

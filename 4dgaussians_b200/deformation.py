@@ -18,7 +18,7 @@ from __future__ import annotations
 
 import ctypes as C
 import itertools
-from typing import List, Optional
+from typing import List, Optional, Tuple
 
 import torch
 import torch.nn as nn
@@ -249,9 +249,7 @@ class deform_network(nn.Module):
                 if not p.is_cuda:
                     raise RuntimeError("deform_network parameters must live on a CUDA device (no CPU fallback)")
                 prm.planes[l][k] = p.data_ptr()
-        aabb = net.grid.aabb.detach()
-        if aabb.dtype != torch.float32 or not aabb.is_contiguous():
-            aabb = aabb.float().contiguous()
+        aabb = _lib.cuda_f32(net.grid.aabb, "aabb")
         keep.append(aabb)
         prm.aabb = aabb.data_ptr()
         prm.w0 = net.feature_out[0].weight.data_ptr()
@@ -314,6 +312,15 @@ class deform_network(nn.Module):
         self._sink_cache = [out, None]
         return out
 
+    def c_grad_sinks(self) -> Tuple[_lib.DeformGrads, List[Optional[torch.Tensor]]]:
+        """(C-ABI gradient sinks of flat_parameters(), the gradients autograd receives for them): the parameters' own
+        .grad and Nones when fused accumulation is possible (``grad_sinks``), else ``alloc_grads()`` and those tensors."""
+        sinks = self.grad_sinks()
+        if sinks is not None:
+            return self.c_grads(sinks), [None] * len(sinks)
+        grads = self.alloc_grads()
+        return self.c_grads(grads), grads
+
     def c_grads(self, grads: List[torch.Tensor]) -> _lib.DeformGrads:
         cache = getattr(self, "_sink_cache", None)
         if cache is not None and grads is cache[0] and cache[1] is not None:
@@ -323,14 +330,16 @@ class deform_network(nn.Module):
             cache[1] = g
         return g
 
-    def _build_c_grads(self, grads: List[torch.Tensor]) -> _lib.DeformGrads:
+    def c_plane_grads(self, grads: List[torch.Tensor]) -> _lib.DeformGrads:
+        """C-ABI sinks for the planes only: grads[:6 * levels], level-major; the MLP sinks stay NULL."""
         g = _lib.DeformGrads()
-        L = len(self.deformation_net.grid.grids)
-        i = 0
-        for l in range(L):
-            for k in range(6):
-                g.planes[l][k] = grads[i].data_ptr()
-                i += 1
+        for i in range(len(self.deformation_net.grid.grids) * 6):
+            g.planes[i // 6][i % 6] = grads[i].data_ptr()
+        return g
+
+    def _build_c_grads(self, grads: List[torch.Tensor]) -> _lib.DeformGrads:
+        g = self.c_plane_grads(grads)
+        i = len(self.deformation_net.grid.grids) * 6
         g.w0, g.b0 = grads[i].data_ptr(), grads[i + 1].data_ptr()
         i += 2
         for h in range(5):
@@ -351,25 +360,14 @@ def scalar_time(times_sel) -> float:
     return float(times_sel)
 
 
-def _f32c(t: Optional[torch.Tensor], what: str) -> Optional[torch.Tensor]:
-    if t is None:
-        return None
-    if not t.is_cuda:
-        raise RuntimeError("%s must be a CUDA tensor (the g4d path has no CPU fallback)" % what)
-    t = t.detach()
-    if t.dtype != torch.float32 or not t.is_contiguous():
-        t = t.float().contiguous()
-    return t
-
-
 class _DeformFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, module: deform_network, t: float, grad_mode: bool, xyz, scales, rotations, opacity, shs, *params):
         lib = _lib.load()
         dev = xyz.device
         n = xyz.shape[0]
-        x, s, r, o, sh = (_f32c(v, nm) for v, nm in ((xyz, "point"), (scales, "scales"), (rotations, "rotations"),
-                                                     (opacity, "opacity"), (shs, "shs")))
+        x, s, r, o, sh = (_lib.cuda_f32(v, nm) for v, nm in ((xyz, "point"), (scales, "scales"), (rotations, "rotations"),
+                                                             (opacity, "opacity"), (shs, "shs")))
         keep = []
         needs_bwd = grad_mode and any(ctx.needs_input_grad)      # (grad mode is always off INSIDE Function.forward)
         prm = module.c_params(keep, fresh=needs_bwd)
@@ -383,10 +381,10 @@ class _DeformFunction(torch.autograd.Function):
         # what autograd would save for the ReLU backward: one sign bit per hidden unit (only when a backward can follow)
         relu_bits = torch.empty(_lib.relu_bits_words(n), device=dev, dtype=torch.int32) if needs_bwd else None
         with torch.cuda.device(dev):
-            ws = _lib.Workspace.get(dev.index if dev.index is not None else torch.cuda.current_device())
+            ws = _lib.workspace_of(dev)
             _lib.check(lib.g4d_deform_forward(ws.handle, C.byref(prm), n, ptr(x), ptr(s), ptr(r), ptr(o), ptr(sh), float(t),
                                               ptr(ox), ptr(os_), ptr(orr), ptr(oo), ptr(osh), ptr(relu_bits),
-                                              int(torch.cuda.current_stream(dev).cuda_stream)), "g4d_deform_forward")
+                                              _lib.stream_of(dev)), "g4d_deform_forward")
         ctx.module, ctx.t, ctx.n = module, float(t), n
         ctx.relu_bits = relu_bits
         ctx.save_for_backward(x)
@@ -404,19 +402,12 @@ class _DeformFunction(torch.autograd.Function):
         keep = []
         prm = module.c_params(keep, fresh=True)      # (keeps the "an optimizer step may follow" mark, see param_version)
         hm = prm.head_mask
-        flat = module.flat_parameters()
-        sinks = module.grad_sinks()
-        if sinks is not None:                              # opt-in fused accumulation into the parameters' own .grad
-            pgrads = [None] * len(sinks)
-            cg = module.c_grads(sinks)
-        else:
-            pgrads = module.alloc_grads()                  # one buffer, channel-last views for the planes
-            cg = module.c_grads(pgrads)
+        cg, pgrads = module.c_grad_sinks()
 
         def gin(g, shape_ok):
             if g is None or not shape_ok or g.numel() == 0:
                 return None
-            return _f32c(g, "grad")
+            return _lib.cuda_f32(g, "grad")
         has_s, has_r, has_o, has_sh = ctx.has
         go_x = gin(g_xyz, True)
         go_s, go_r, go_o = gin(g_sc, has_s), gin(g_rot, has_r), gin(g_op, has_o)
@@ -428,10 +419,9 @@ class _DeformFunction(torch.autograd.Function):
         gi_sh = torch.empty(n, 16, 3, device=dev) if (has_sh and (hm & _lib.HEAD_SHS)) else None
         ptr = lambda v: v.data_ptr() if v is not None else None
         with torch.cuda.device(dev):
-            ws = _lib.Workspace.get(dev.index if dev.index is not None else torch.cuda.current_device())
+            ws = _lib.workspace_of(dev)
             _lib.check(lib.g4d_deform_backward(ws.handle, C.byref(prm), C.byref(cg), n, ptr(x), float(t), ptr(go_x), ptr(go_s),
                                                ptr(go_r), ptr(go_o), ptr(go_sh), ptr(gi_x), ptr(gi_s), ptr(gi_r), ptr(gi_o),
-                                               ptr(gi_sh), ptr(ctx.relu_bits),
-                                               int(torch.cuda.current_stream(dev).cuda_stream)), "g4d_deform_backward")
+                                               ptr(gi_sh), ptr(ctx.relu_bits), _lib.stream_of(dev)), "g4d_deform_backward")
         ctx.relu_bits = None
         return (None, None, None, gi_x, gi_s, gi_r, gi_o, gi_sh) + tuple(pgrads)

@@ -16,22 +16,17 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-import struct
 from typing import List, Sequence
 
 import torch
 
 from . import _lib
 from .deformation import deform_network, scalar_time
-from .renderer import _zero_points, settings_from_camera
-from .rasterizer import _dev_f32
+from .rasterizer import camera_from_settings
+from .renderer import _stage_module, _time_bits, _zero_points, settings_from_camera
 
 _VIEW_FLOATS = 36        # per view in the staging block: view matrix [16], projection matrix [16], camera centre [3], pad
 ERR_OVERFLOW = -5        # G4D_ERR_OVERFLOW
-
-
-def _time_bits(t) -> bytes:
-    return struct.pack("<f", float(t))
 
 
 class GraphedRender:
@@ -48,14 +43,9 @@ class GraphedRender:
         views = list(template) if self.multi else [template]
         if not views or len(views) > _lib.MAX_CAMERAS:
             raise ValueError("a graphed render takes 1..%d views, got %d" % (_lib.MAX_CAMERAS, len(views)))
-        if "coarse" in stage:
-            module = None
-        elif "fine" in stage:
-            module = pc._deformation
-            if not isinstance(module, deform_network):
-                raise NotImplementedError("a graphed render needs the g4d deformation network (or the coarse stage)")
-        else:
-            raise NotImplementedError
+        module = _stage_module(pc, stage)
+        if "coarse" not in stage and not isinstance(module, deform_network):
+            raise NotImplementedError("a graphed render needs the g4d deformation network (or the coarse stage)")
         if getattr(pipe, "debug", False):
             raise ValueError("a graphed render cannot run with pipe.debug (it synchronises after every stage)")
         xyz = pc.get_xyz
@@ -68,14 +58,14 @@ class GraphedRender:
         self._shape = [self._view_key(rs) for rs, _ in settings]
         # the model's tensors are read in place: a copy (non-contiguous or non-fp32 storage) would freeze their values
         self._tensors = (pc._xyz, pc._scaling, pc._rotation, pc._opacity, pc._features_dc, pc._features_rest)
-        staged = [_dev_f32(t, t.numel(), name) for t, name in zip(self._tensors, ("xyz", "scaling", "rotation", "opacity",
-                                                                                  "features_dc", "features_rest"))]
+        staged = [_lib.cuda_f32(t, name) for t, name in zip(self._tensors, ("xyz", "scaling", "rotation", "opacity",
+                                                                            "features_dc", "features_rest"))]
         if any(a.data_ptr() != b.data_ptr() for a, b in zip(staged, self._tensors)):
             raise ValueError("a graphed render reads the model's tensors in place: they must be contiguous fp32 CUDA tensors")
         self._ptrs = tuple(t.data_ptr() for t in self._tensors)
-        self._bg = _dev_f32(bg_color, 3, "bg")
+        self._bg = _lib.cuda_f32(bg_color, "bg", 3)
 
-        self.ws = _lib.Workspace(dev.index if dev.index is not None else torch.cuda.current_device())
+        self.ws = _lib.Workspace(dev.index)
         self.ws.set_option(_lib.OPT_SYNC_MODE, 0)
         if min_capacity:
             self.ws.set_option(_lib.OPT_INSTANCE_CAPACITY, int(min_capacity))
@@ -90,15 +80,11 @@ class GraphedRender:
         for c in self.ctxs:
             c.set_time_source(d_time)
 
-        self._cams = (_lib.Camera * k)()
-        for i, (rs, _) in enumerate(settings):
-            cam = self._cams[i]
-            cam.image_height, cam.image_width = int(rs.image_height), int(rs.image_width)
-            cam.sh_degree, cam.debug = self.sh_degree, _lib.CAM_NO_GRAD
-            cam.tanfovx, cam.tanfovy, cam.scale_modifier = float(rs.tanfovx), float(rs.tanfovy), float(rs.scale_modifier)
+        self._cams = (_lib.Camera * k)(*[camera_from_settings(rs._replace(bg=self._bg)) for rs, _ in settings])
+        for i, cam in enumerate(self._cams):      # the view matrices and camera centre: read from the staging block's copy
+            cam.debug = _lib.CAM_NO_GRAD
             off = base + i * _VIEW_FLOATS * fsz
             cam.d_viewmatrix, cam.d_projmatrix, cam.d_campos = off, off + 16 * fsz, off + 32 * fsz
-            cam.d_bg = self._bg.data_ptr()
         self._keep: list = []
         # fresh: the capture records the weight repack, so every replay packs the parameters as they are then
         self._prm = module.c_params(self._keep, fresh=True) if module is not None else None
@@ -134,7 +120,7 @@ class GraphedRender:
 
     def _launch(self):
         """The captured work: one C-ABI render call, then the visibility masks."""
-        stream = int(torch.cuda.current_stream(self.dev).cuda_stream)
+        stream = _lib.stream_of(self.dev)
         prm = C.byref(self._prm) if self._prm is not None else None
         if self.multi:
             _lib.check(self._lib.g4d_render_forward_cameras(self._handles, self.k, self._cams, prm, C.byref(self._g), *self._out,

@@ -17,34 +17,17 @@ import torch
 from . import _lib
 
 
-def _ws(dev):
-    return _lib.Workspace.get(dev.index if dev.index is not None else torch.cuda.current_device())
-
-
-def _stream(dev) -> int:
-    return int(torch.cuda.current_stream(dev).cuda_stream)
-
-
-def _cuda_f32(t: torch.Tensor, what: str) -> torch.Tensor:
-    if not t.is_cuda:
-        raise RuntimeError("%s must be a CUDA tensor (the g4d path has no CPU fallback)" % what)
-    t = t.detach()
-    if t.dtype != torch.float32 or not t.is_contiguous():
-        t = t.float().contiguous()
-    return t
-
-
 class _L1(torch.autograd.Function):
     @staticmethod
     def forward(ctx, out, gt):
         if out.shape != gt.shape:
             raise RuntimeError("l1_loss: shapes differ: %s vs %s" % (tuple(out.shape), tuple(gt.shape)))
-        a, b = _cuda_f32(out, "network_output"), _cuda_f32(gt, "gt")
+        a, b = _lib.cuda_f32(out, "network_output"), _lib.cuda_f32(gt, "gt")
         n = a.numel()
         loss = torch.zeros((), device=a.device, dtype=torch.float32)
         with torch.cuda.device(a.device):
-            _lib.check(_lib.load().g4d_l1_loss(_ws(a.device).handle, a.data_ptr(), b.data_ptr(), n, 1.0 / max(n, 1),
-                                               loss.data_ptr(), _stream(a.device)), "g4d_l1_loss")
+            _lib.check(_lib.load().g4d_l1_loss(_lib.workspace_of(a.device).handle, a.data_ptr(), b.data_ptr(), n,
+                                               1.0 / max(n, 1), loss.data_ptr(), _lib.stream_of(a.device)), "g4d_l1_loss")
         ctx.save_for_backward(a, b)
         ctx.needs_gt = ctx.needs_input_grad[1]
         return loss
@@ -53,11 +36,12 @@ class _L1(torch.autograd.Function):
     def backward(ctx, g):
         a, b = ctx.saved_tensors
         n = a.numel()
-        up = _cuda_f32(g, "grad_output")
+        up = _lib.cuda_f32(g, "grad_output")
         grad = torch.empty_like(a)
         with torch.cuda.device(a.device):
-            _lib.check(_lib.load().g4d_l1_loss_backward(_ws(a.device).handle, a.data_ptr(), b.data_ptr(), n, 1.0 / max(n, 1),
-                                                        up.data_ptr(), grad.data_ptr(), _stream(a.device)), "g4d_l1_loss_backward")
+            _lib.check(_lib.load().g4d_l1_loss_backward(_lib.workspace_of(a.device).handle, a.data_ptr(), b.data_ptr(), n,
+                                                        1.0 / max(n, 1), up.data_ptr(), grad.data_ptr(), _lib.stream_of(a.device)),
+                       "g4d_l1_loss_backward")
         return grad, (-grad if ctx.needs_gt else None)
 
 
@@ -68,7 +52,7 @@ def l1_loss(network_output: torch.Tensor, gt: torch.Tensor) -> torch.Tensor:
 class _SSIM(torch.autograd.Function):
     @staticmethod
     def forward(ctx, img1, img2):
-        a, b = _cuda_f32(img1, "img1"), _cuda_f32(img2, "img2")
+        a, b = _lib.cuda_f32(img1, "img1"), _lib.cuda_f32(img2, "img2")
         if a.shape != b.shape or a.dim() < 3:
             raise RuntimeError("ssim: expects two [..., C, H, W] tensors of the same shape")
         H, W = int(a.shape[-2]), int(a.shape[-1])
@@ -77,9 +61,9 @@ class _SSIM(torch.autograd.Function):
         saved = torch.empty(3 * a.numel(), device=a.device, dtype=torch.float32) if need else None
         val = torch.zeros((), device=a.device, dtype=torch.float32)
         with torch.cuda.device(a.device):
-            _lib.check(_lib.load().g4d_ssim(_ws(a.device).handle, a.data_ptr(), b.data_ptr(), ch, H, W, 1.0 / max(a.numel(), 1),
-                                            val.data_ptr(), saved.data_ptr() if saved is not None else None,
-                                            _stream(a.device)), "g4d_ssim")
+            _lib.check(_lib.load().g4d_ssim(_lib.workspace_of(a.device).handle, a.data_ptr(), b.data_ptr(), ch, H, W,
+                                            1.0 / max(a.numel(), 1), val.data_ptr(), saved.data_ptr() if saved is not None else None,
+                                            _lib.stream_of(a.device)), "g4d_ssim")
         ctx.save_for_backward(a, b, saved)
         return val
 
@@ -90,12 +74,12 @@ class _SSIM(torch.autograd.Function):
             raise NotImplementedError("ssim: gradient w.r.t. the second image (the ground truth) is not provided")
         H, W = int(a.shape[-2]), int(a.shape[-1])
         ch = a.numel() // (H * W)
-        up = _cuda_f32(g, "grad_output")
+        up = _lib.cuda_f32(g, "grad_output")
         grad = torch.empty_like(a)
         with torch.cuda.device(a.device):
-            _lib.check(_lib.load().g4d_ssim_backward(_ws(a.device).handle, a.data_ptr(), b.data_ptr(), ch, H, W,
+            _lib.check(_lib.load().g4d_ssim_backward(_lib.workspace_of(a.device).handle, a.data_ptr(), b.data_ptr(), ch, H, W,
                                                      1.0 / max(a.numel(), 1), up.data_ptr(), saved.data_ptr(), grad.data_ptr(),
-                                                     _stream(a.device)), "g4d_ssim_backward")
+                                                     _lib.stream_of(a.device)), "g4d_ssim_backward")
         return grad, None
 
 
@@ -116,18 +100,12 @@ class _Regulation(torch.autograd.Function):
         need = any(ctx.needs_input_grad)
         loss = torch.zeros((), device=dev, dtype=torch.float32)
         grads = module.alloc_plane_grads() if need else None
-        cg = None
-        if grads is not None:
-            cg = _lib.DeformGrads()
-            i = 0
-            for l in range(prm.levels):
-                for k in range(6):
-                    cg.planes[l][k] = grads[i].data_ptr()
-                    i += 1
+        cg = module.c_plane_grads(grads) if grads is not None else None
         with torch.cuda.device(dev):
-            _lib.check(_lib.load().g4d_plane_regulation(_ws(dev).handle, C.byref(prm), C.byref(cg) if cg is not None else None,
-                                                        float(w_tv), float(w_ts), float(w_l1), None, loss.data_ptr(),
-                                                        _stream(dev)), "g4d_plane_regulation")
+            _lib.check(_lib.load().g4d_plane_regulation(_lib.workspace_of(dev).handle, C.byref(prm),
+                                                        C.byref(cg) if cg is not None else None, float(w_tv), float(w_ts),
+                                                        float(w_l1), None, loss.data_ptr(), _lib.stream_of(dev)),
+                       "g4d_plane_regulation")
         ctx.grads = grads
         return loss
 
@@ -159,18 +137,14 @@ def accumulate_regulation(deformation, time_smoothness_weight: float, l1_time_pl
     keep = []
     prm = deformation.c_params(keep)
     planes = [p for lvl in deformation.deformation_net.grid.grids for p in lvl]
-    cg = _lib.DeformGrads()
-    i = 0
-    for l in range(prm.levels):
-        for k in range(6):
-            g = planes[i].grad
-            if g is None or g.stride() != planes[i].stride() or g.dtype != torch.float32:
-                raise RuntimeError("accumulate_regulation: plane %d has no .grad with the parameter's own layout" % i)
-            cg.planes[l][k] = g.data_ptr()
-            i += 1
+    for i, p in enumerate(planes):
+        if p.grad is None or p.grad.stride() != p.stride() or p.grad.dtype != torch.float32:
+            raise RuntimeError("accumulate_regulation: plane %d has no .grad with the parameter's own layout" % i)
+    cg = deformation.c_plane_grads([p.grad for p in planes])
     dev = planes[0].device
     with torch.cuda.device(dev):
-        _lib.check(_lib.load().g4d_plane_regulation(_ws(dev).handle, C.byref(prm), C.byref(cg), float(plane_tv_weight),
-                                                    float(time_smoothness_weight), float(l1_time_planes_weight), None,
-                                                    loss_accum.data_ptr() if loss_accum is not None else None, _stream(dev)),
+        _lib.check(_lib.load().g4d_plane_regulation(_lib.workspace_of(dev).handle, C.byref(prm), C.byref(cg),
+                                                    float(plane_tv_weight), float(time_smoothness_weight),
+                                                    float(l1_time_planes_weight), None,
+                                                    loss_accum.data_ptr() if loss_accum is not None else None, _lib.stream_of(dev)),
                    "g4d_plane_regulation")

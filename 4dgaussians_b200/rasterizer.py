@@ -31,17 +31,6 @@ class GaussianRasterizationSettings(NamedTuple):
     debug: bool
 
 
-def _dev_f32(t: torch.Tensor, numel: int, what: str) -> torch.Tensor:
-    if not t.is_cuda:
-        raise RuntimeError("%s must be a CUDA tensor (the g4d path has no CPU fallback)" % what)
-    t = t.detach()
-    if t.dtype != torch.float32 or not t.is_contiguous():
-        t = t.float().contiguous()
-    if t.numel() != numel:
-        raise RuntimeError("%s has %d elements, expected %d" % (what, t.numel(), numel))
-    return t
-
-
 def camera_from_settings(rs: GaussianRasterizationSettings, time: float = 0.0, keep=None) -> _lib.Camera:
     """Build the C-ABI camera.  Matrices given as CUDA tensors stay on the device (no D2H sync);
     CPU tensors are copied into the struct."""
@@ -56,7 +45,7 @@ def camera_from_settings(rs: GaussianRasterizationSettings, time: float = 0.0, k
         if not torch.is_tensor(t):
             t = torch.as_tensor(t, dtype=torch.float32)
         if t.is_cuda:
-            t = _dev_f32(t, n, name)
+            t = _lib.cuda_f32(t, name, n)
             if keep is not None:
                 keep.append(t)
             setattr(cam, dfield, t.data_ptr())
@@ -87,21 +76,17 @@ class _ContextLease:
             pass
 
 
-def _stream_ptr(device) -> int:
-    return int(torch.cuda.current_stream(device).cuda_stream)
-
-
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, raster_settings):
         lib = _lib.load()
         dev = means3D.device
         n = means3D.shape[0]
-        m3 = _dev_f32(means3D, n * 3, "means3D")
-        shc = _dev_f32(sh, n * 48, "shs")
-        op = _dev_f32(opacities, n, "opacities")
-        sc = _dev_f32(scales, n * 3, "scales")
-        ro = _dev_f32(rotations, n * 4, "rotations")
+        m3 = _lib.cuda_f32(means3D, "means3D", n * 3)
+        shc = _lib.cuda_f32(sh, "shs", n * 48)
+        op = _lib.cuda_f32(opacities, "opacities", n)
+        sc = _lib.cuda_f32(scales, "scales", n * 3)
+        ro = _lib.cuda_f32(rotations, "rotations", n * 4)
         H, W = int(raster_settings.image_height), int(raster_settings.image_width)
         color = torch.empty(3, H, W, device=dev, dtype=torch.float32)
         depth = torch.empty(1, H, W, device=dev, dtype=torch.float32)
@@ -109,10 +94,10 @@ class _RasterizeGaussians(torch.autograd.Function):
         keep = []
         cam = camera_from_settings(raster_settings, keep=keep)
         with torch.cuda.device(dev):
-            lease = _ContextLease(_lib.Workspace.get(dev.index if dev.index is not None else torch.cuda.current_device()))
+            lease = _ContextLease(_lib.workspace_of(dev))
             _lib.check(lib.g4d_rasterize_forward(lease.ctx.handle, C.byref(cam), n, m3.data_ptr(), shc.data_ptr(), op.data_ptr(),
                                                  sc.data_ptr(), ro.data_ptr(), color.data_ptr(), depth.data_ptr(),
-                                                 radii.data_ptr(), _stream_ptr(dev)), "g4d_rasterize_forward")
+                                                 radii.data_ptr(), _lib.stream_of(dev)), "g4d_rasterize_forward")
         ctx.raster_settings = raster_settings
         ctx.lease = lease
         ctx.n = n
@@ -127,7 +112,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         dev = m3.device
         n = ctx.n
         rs = ctx.raster_settings
-        gcol = _dev_f32(grad_color, 3 * int(rs.image_height) * int(rs.image_width), "grad_out_color")
+        gcol = _lib.cuda_f32(grad_color, "grad_out_color", 3 * int(rs.image_height) * int(rs.image_width))
         g_means3D = torch.empty(n, 3, device=dev)
         g_means2D = torch.empty(n, 3, device=dev)
         g_sh = torch.empty(n, 16, 3, device=dev)
@@ -143,7 +128,7 @@ class _RasterizeGaussians(torch.autograd.Function):
             _lib.check(lib.g4d_rasterize_backward(lease.ctx.handle, C.byref(cam), n, m3.data_ptr(), shc.data_ptr(), op.data_ptr(),
                                                   sc.data_ptr(), ro.data_ptr(), gcol.data_ptr(), g_means3D.data_ptr(),
                                                   g_means2D.data_ptr(), g_sh.data_ptr(), g_op.data_ptr(), g_sc.data_ptr(),
-                                                  g_ro.data_ptr(), _stream_ptr(dev)), "g4d_rasterize_backward")
+                                                  g_ro.data_ptr(), _lib.stream_of(dev)), "g4d_rasterize_backward")
         lease.release()
         ctx.lease = None
         return g_means3D, g_means2D, g_sh, g_op, g_sc, g_ro, None

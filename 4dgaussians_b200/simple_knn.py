@@ -12,16 +12,13 @@ from . import _lib
 def distCUDA2(points: torch.Tensor) -> torch.Tensor:
     if not points.is_cuda:
         raise RuntimeError("distCUDA2 needs a CUDA tensor (the g4d path has no CPU fallback)")
-    p = points.detach()
-    if p.dtype != torch.float32 or not p.is_contiguous():
-        p = p.float().contiguous()
+    p = _lib.cuda_f32(points, "points")
     if p.dim() != 2 or p.shape[1] != 3:
         raise RuntimeError("distCUDA2 expects an [N,3] tensor")
     n = p.shape[0]
     out = torch.empty(n, device=p.device, dtype=torch.float32)
     dev = p.device
     with torch.cuda.device(dev):
-        ws = _lib.Workspace.get(dev.index if dev.index is not None else torch.cuda.current_device())
-        _lib.check(_lib.load().g4d_dist2_knn3(ws.handle, n, p.data_ptr(), out.data_ptr(),
-                                              int(torch.cuda.current_stream(dev).cuda_stream)), "g4d_dist2_knn3")
+        _lib.check(_lib.load().g4d_dist2_knn3(_lib.workspace_of(dev).handle, n, p.data_ptr(), out.data_ptr(),
+                                              _lib.stream_of(dev)), "g4d_dist2_knn3")
     return out

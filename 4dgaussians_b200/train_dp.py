@@ -153,11 +153,11 @@ class FlatState:
         dev = self.device
         off = 4 * b0
         with torch.cuda.device(dev):
-            ws = _lib.Workspace.get(dev.index if dev.index is not None else torch.cuda.current_device())
+            ws = _lib.workspace_of(dev)
             _lib.check(_lib.load().g4d_adam_step(ws.handle, self.param.data_ptr() + off, self.grad.data_ptr() + off,
                                                  self.exp_avg.data_ptr() + off, self.exp_avg_sq.data_ptr() + off, e0 - b0, segs,
                                                  len(clipped), betas[0], betas[1], eps, self.step_count, float(grad_scale),
-                                                 int(torch.cuda.current_stream(dev).cuda_stream)), "g4d_adam_step")
+                                                 _lib.stream_of(dev)), "g4d_adam_step")
 
 
 class GaussianSet:
