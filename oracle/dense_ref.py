@@ -22,6 +22,7 @@ from typing import Dict
 import torch
 
 C0 = 0.28209479177387814
+NEAR_CULL = 0.20000000298023224     # the fp32 constant 0.2f of the kernels' `depth <= 0.2f` cull, exactly
 C1 = 0.4886025119029199
 C2 = [1.0925484305920792, -1.0925484305920792, 0.31539156525252005, -1.0925484305920792, 0.5462742152960396]
 C3 = [-0.5900435899266435, 2.890611442640554, -0.4570457994644658, 0.3731763325901154, -0.4570457994644658,
@@ -45,9 +46,12 @@ def _sh_color(deg, sh, d):
     return res
 
 
-def dense_render(cam: Dict, means3D, scales, rots, opac, shs, pix_offset=None):
+def dense_render(cam: Dict, means3D, scales, rots, opac, shs, pix_offset=None, guard_band_grad=False, alpha_clamp=True):
     """cam: dict(H,W,tanfovx,tanfovy,view[16],proj[16],campos[3],bg[3],sh_degree,scale_modifier).
-    All tensors fp64.  Returns dict(color[3,H,W], depth[1,H,W], radii[N], rect[N,4], n_contrib[H,W])."""
+    All tensors fp64.  Returns dict(color[3,H,W], depth[1,H,W], radii[N], rect[N,4], n_contrib[H,W]).
+    Two opt-in departures from the published algorithm, for tests that show a check would catch a kernel that made them:
+    guard_band_grad passes the gradient straight through a guard-band-clamped t.x / t.y (as if the clamp were not there in
+    the backward); alpha_clamp=False drops the 0.99 clamp of alpha in the forward and the backward."""
     dt = means3D.dtype
     H, W = cam["H"], cam["W"]
     v = torch.as_tensor(cam["view"], dtype=dt).reshape(16)
@@ -65,7 +69,7 @@ def dense_render(cam: Dict, means3D, scales, rots, opac, shs, pix_offset=None):
     hw = xf(pm, 3)
     pw = 1.0 / (hw + 0.0000001)
     ndcx, ndcy = xf(pm, 0) * pw, xf(pm, 1) * pw
-    visible = tz.detach() > 0.2
+    visible = tz.detach() > NEAR_CULL
 
     r, x, y, z = rots[:, 0], rots[:, 1], rots[:, 2], rots[:, 3]
     R = torch.stack([1 - 2 * (y * y + z * z), 2 * (x * y - r * z), 2 * (x * z + r * y),
@@ -83,6 +87,9 @@ def dense_render(cam: Dict, means3D, scales, rots, opac, shs, pix_offset=None):
     cym = (tytz.detach() < -limy) | (tytz.detach() > limy)
     txc = torch.where(cxm, (txtz.clamp(-limx, limx) * tzs).detach(), tx)
     tyc = torch.where(cym, (tytz.clamp(-limy, limy) * tzs).detach(), ty)
+    if guard_band_grad:
+        txc = tx + (txc - tx).detach()
+        tyc = ty + (tyc - ty).detach()
     zero = torch.zeros_like(tzs)
     J = torch.stack([fx / tzs, zero, -(fx * txc) / (tzs * tzs), zero, fy / tzs, -(fy * tyc) / (tzs * tzs)],
                     dim=-1).reshape(N, 2, 3)
@@ -133,7 +140,7 @@ def dense_render(cam: Dict, means3D, scales, rots, opac, shs, pix_offset=None):
     power = -0.5 * (conx[o][None, :] * dx * dx + conz[o][None, :] * dy * dy) - cony[o][None, :] * dx * dy
     G = torch.exp(torch.clamp(power, max=0.0))
     a_raw = opac.reshape(-1)[o][None, :] * G
-    alpha = a_raw + (torch.clamp(a_raw, max=0.99) - a_raw).detach()
+    alpha = a_raw + (torch.clamp(a_raw, max=0.99) - a_raw).detach() if alpha_clamp else a_raw
     valid = member & (power.detach() <= 0) & (alpha.detach() >= 1.0 / 255.0)
     om = torch.where(valid, 1.0 - alpha, torch.ones_like(alpha))
     t_incl = torch.cumprod(om, dim=1)

@@ -8,7 +8,8 @@ import numpy as np
 import pytest
 
 from oracle import raster_ref as rr
-from util_scene import cam_tuple, raster_inputs, synth
+import util_raster_edges as ue
+from util_scene import cam_tuple, raster_inputs, row_errors, synth
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "host_emul", "emul_math.cpp")
@@ -189,3 +190,40 @@ def test_sub_segment_rank_fix_restores_the_depth_order():
         assert sorted(r) == list(range(n)), n                                              # a permutation: no two entries collide
         fixed = np.empty(n, np.int64); fixed[np.asarray(r)] = vals
         assert np.array_equal(fixed, ids), n
+
+
+def _emul_preprocess(lib, rc, m, s, r, o, sh):
+    n = m.shape[0]
+    out = dict(depth=np.zeros(n, np.float32), radii=np.zeros(n, np.int32), xy=np.zeros((n, 2), np.float32),
+               conic_op=np.zeros((n, 4), np.float32), rgb=np.zeros((n, 3), np.float32), clamped=np.zeros((n, 3), np.uint8),
+               rect=np.zeros((n, 4), np.int32), tiles_touched=np.zeros(n, np.uint32))
+    lib.emul_preprocess(C.byref(rc), n, _p(m), _p(s), _p(r), _p(o), _p(sh), *[_p(out[k]) for k in out])
+    return out
+
+
+@pytest.mark.parametrize("name", ue.names())
+def test_edge_scenes_vs_oracle(name):
+    """the scenes of test_raster_edge_scenes.py (guard band, near plane, clamped rects and colours, degenerate covariances,
+    unnormalised quaternions): project_gaussian + sh_to_rgb bit for bit, gaussian_backward per row"""
+    lib = _lib()
+    sc = ue.scene(name)
+    rc, _ = cam_tuple(sc.cam, sc.bg, sh_degree=sc.deg)
+    m, s, r, o, sh = sc.ins
+    ref = rr.preprocess(rc, m, s, r, o, sh)
+    got = _emul_preprocess(lib, rc, m, s, r, o, sh)
+    for k, v in got.items():
+        assert np.array_equal(v.view(np.uint8), getattr(ref, k).view(np.uint8)), k
+    # the cotangents of the oracle's blend backward under a random image gradient: their conic part has the size a real
+    # backward gives it (unit random conic cotangents would hide the covariance terms behind the means2D term)
+    n = m.shape[0]
+    fwd = rr.rasterize_forward(rc, m, s, r, o, sh)
+    dL = np.random.default_rng(len(name)).standard_normal((3, sc.H, sc.W)).astype(np.float32)
+    g2, gc, _, grgb = rr.blend_backward(rc, fwd["proj"], fwd["bin"], fwd["final_T"], fwd["n_contrib"], dL)
+    want = rr.preprocess_backward(rc, m, s, r, sh, ref, g2, gc, grgb)
+    gm = np.zeros((n, 3), np.float32); gs = np.zeros((n, 3), np.float32); gr = np.zeros((n, 4), np.float32)
+    gsh = np.zeros((n, 16, 3), np.float32)
+    lib.emul_backward(C.byref(rc), n, _p(m), _p(s), _p(r), _p(sh), _p(ref.radii), _p(ref.clamped), _p(g2), _p(gc), _p(grgb),
+                      _p(gm), _p(gs), _p(gr), _p(gsh))
+    for g, w, nm in zip((gm, gs, gr, gsh), want, ("mean", "scale", "rot", "sh")):
+        e = row_errors(g, w, 1e-4)
+        assert float(e.max()) <= 2e-3, (nm, float(e.max()), int(np.argmax(e)))

@@ -292,9 +292,11 @@ def raster_oracle_inputs(deformed, shs):
             np.ascontiguousarray(d[:, 10:11]), np.ascontiguousarray(np.asarray(shs, np.float32).reshape(-1, 16, 3)))
 
 
-def threshold_pixels(fwd, W, H, d_alpha=2e-5, d_T=2e-3, d_power=1e-6):
+def threshold_pixels(fwd, W, H, d_alpha=2e-5, d_T=2e-3, d_power=1e-6, include_stop=False):
     """[H,W] bool: pixels where an instance before the pixel's stop (list position < n_contrib) sits within rounding of a
-    discrete decision of the compositing loop (A.3): alpha = 1/255, the clamp alpha = 0.99, T = 1e-4 or power = 0.  This is
+    discrete decision of the compositing loop (A.3): alpha = 1/255, the clamp alpha = 0.99, T = 1e-4 or power = 0.
+    include_stop: also the instance at position n_contrib, whose T < 1e-4 stopped the pixel if it stopped (a flip there
+    changes n_contrib, which a comparison of two fp32 runs sees; a comparison with fp64 needs it here).  This is
     the predicate (same margins) of test_gpu_fullsize._assert_pixel_outliers_are_threshold_flips, evaluated in fp64 from the
     oracle's projected records for every pixel.  The blend kernels' ex2-based exponential and libm expf differ in the last
     ulp, so either side may take the other branch there; when the instance is not the pixel's last contributor and T is
@@ -314,8 +316,8 @@ def threshold_pixels(fwd, W, H, d_alpha=2e-5, d_T=2e-3, d_power=1e-6):
         m = int(last.max())
         if m == 0:
             continue
-        lo = int(bn.ranges[tile][0])
-        ids = bn.ids[lo:lo + m].astype(np.int64)
+        lo, hi = (int(v) for v in bn.ranges[tile])
+        ids = bn.ids[lo:min(hi, lo + m + int(include_stop))].astype(np.int64)
         dx = xy[ids, 0][:, None] - px[None, :]
         dy = xy[ids, 1][:, None] - py[None, :]
         power = -0.5 * (co[ids, 0][:, None] * dx * dx + co[ids, 2][:, None] * dy * dy) - co[ids, 1][:, None] * dx * dy
@@ -324,7 +326,7 @@ def threshold_pixels(fwd, W, H, d_alpha=2e-5, d_T=2e-3, d_power=1e-6):
         T = np.cumprod(np.where((power <= 0) & (alpha >= 1.0 / 255.0), 1.0 - alpha, 1.0), axis=0)
         near = (np.abs(a * 255.0 - 1.0) < d_alpha) | (np.abs(a - 0.99) < d_alpha) | (np.abs(T / 1e-4 - 1.0) < d_T) | \
                (np.abs(power) < d_power)
-        near &= np.arange(m)[:, None] < last[None, :]
+        near &= np.arange(len(ids))[:, None] < last[None, :] + int(include_stop)
         out[py, px] = near.any(axis=0)
     return out
 
