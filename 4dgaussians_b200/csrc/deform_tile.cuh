@@ -1,4 +1,4 @@
-// deform_tile.cuh -- HexPlane sampling + deformation MLP for a tile of TG Gaussians held in shared memory.
+// deform_tile.cuh -- deformation MLP of the FFMA path for a tile of TG Gaussians held in shared memory.
 //
 // Algorithm (verified spec: SURVEY.md Appendix B):
 //   /root/reference/scene/hexplane.py:19-20,73-106,160-183   normalize_aabb, 6-plane bilinear product, level concat
@@ -6,8 +6,8 @@
 //   /root/reference/scene/deformation.py:97-148              heads ReLU-Linear-ReLU-Linear, residual add
 //
 // Layout decisions (DESIGN.md §3):
-//   * the HexPlane sampling (channel-last planes, collapsed time rows) is hexplane.cuh's, shared with every other
-//     deformation kernel;
+//   * the HexPlane features arrive gathered, feat [N][F] (deform_features_kernel, the gather of every path); a tile of
+//     them is loaded into a0;
 //   * a CTA of 256 threads owns TG Gaussians; activations live in shared memory row-major [TG][K+4];
 //     W0^T and one head's W1^T are staged in shared memory ([K][Wd], W1^T by a TMA bulk copy that overlaps
 //     the previous head's epilogue); each thread accumulates an RM x (Wd/16) register tile with FFMA.
@@ -35,7 +35,7 @@ struct DeformDesc {
 
 // shared-memory carve-up (offsets in floats), computed on the host by deform_smem_layout()
 struct DeformSmem {
-    int w0t, b0, w1t, b1, w2, b2, a0, a1, a2, out, in, coord, mbar, total_floats;
+    int w0t, b0, w1t, b1, w2, b2, a0, a1, a2, out, in, mbar, total_floats;
     int lda0, lda1, w2_stride;
     int w2_off[G4D_NUM_HEADS];   // row offset (in rows of w2_stride floats) of head h inside w2
 };
@@ -58,7 +58,6 @@ inline DeformSmem deform_smem_layout(int TG, int F, int WD, int head_mask) {
     s.a2 = take(TG * s.lda1);
     s.out = take(TG * 60);
     s.in = take(TG * 12);
-    s.coord = take(TG * 4);
     s.mbar = take(4);
     s.total_floats = off;
     return s;
@@ -93,24 +92,6 @@ G4D_D void tma_bulk_g2s(void* dst_smem, const void* src_gmem, uint32_t bytes, vo
                  : "memory");
 }
 G4D_D void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-
-// Phase 1: thread (g, q) samples the channel vectors v = q, q+TPG, ... of every level and writes feat[g][l*C + 4v .. 4v+3]
-// into a0.  coord[g] = (px, py, pz, t) already normalised (t raw).
-template <int TG>
-G4D_D void sample_features(const DeformDesc& d, const float* __restrict__ coord, float* __restrict__ a0, int lda0) {
-    constexpr int TPG = kDeformThreads / TG;
-    const int g = threadIdx.x / TPG, q = threadIdx.x % TPG;
-    const float4 pc = *reinterpret_cast<const float4*>(coord + 4 * g);
-    const float pcs[3] = {pc.x, pc.y, pc.z};
-    const int C4 = d.C >> 2;
-    for (int l = 0; l < d.levels; ++l) {
-        Tap1D tx[3];
-#pragma unroll
-        for (int a = 0; a < 3; ++a) tx[a] = make_tap(pcs[a], d.res[l][a]);
-        for (int v = q; v < C4; v += TPG)
-            *reinterpret_cast<float4*>(a0 + g * lda0 + l * d.C + 4 * v) = sample_vector(d.planes[l], d.trow[l], d.res[l], tx, v, C4);
-    }
-}
 
 // ---- register-tiled shared-memory GEMM --------------------------------------------------------------
 // acc[r][c] (+)= sum_k A[ty*RM + r][k] * B[k][col(c)],  col(c) = (c/4)*64 + tx*4 + (c%4)
@@ -221,7 +202,19 @@ G4D_D void stage_persistent_weights(const DeformDesc& d, const DeformSmem& L, fl
     }
 }
 
-// Runs the whole network for the TG Gaussians whose normalised coordinates are in smem[L.coord].
+// a0[g][0 .. F) = feat[base + g][0 .. F) for the tile's Gaussians g < rem, zero for the rows past n; the caller syncs.
+template <int TG>
+G4D_D void load_feature_tile(const float* __restrict__ feat, int F, int64_t base, int64_t rem, float* __restrict__ a0, int lda0) {
+    const int F4 = F >> 2;
+    for (int i = threadIdx.x; i < TG * F4; i += kDeformThreads) {
+        const int g = i / F4, v = i - g * F4;
+        float4 val = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (g < rem) val = __ldg(reinterpret_cast<const float4*>(feat + (base + g) * F + 4 * v));
+        *reinterpret_cast<float4*>(a0 + g * lda0 + 4 * v) = val;
+    }
+}
+
+// Runs the whole network for the TG Gaussians whose features are in smem[L.a0] (load_feature_tile).
 // On return smem[L.out + g*60 + head_col(h) + o] holds the delta of every ACTIVE head (inactive: untouched).
 // `phase` is the running mbarrier parity for the W1 staging buffer (caller keeps it across tiles).
 // PRE: thread 0 has already issued the bulk copy of the FIRST active head's W1^T for this tile.
@@ -231,8 +224,6 @@ G4D_D void deform_mlp_tile(const DeformDesc& d, const DeformSmem& L, float* smem
     const int ty = threadIdx.x >> 4, tx = threadIdx.x & 15;
     void* bar = smem + L.mbar;
 
-    sample_features<TG>(d, smem + L.coord, smem + L.a0, L.lda0);
-    __syncthreads();
     {   // hidden = feat W0^T + b0 ; a1 = relu(hidden)  (every head starts with ReLU: deformation.py:61-65)
         float acc[RM][CG * 4];
 #pragma unroll

@@ -156,7 +156,7 @@ struct G4DWorkspace {
     WeightCache<FfmaWeights> packed;     // FFMA forward and backward
     WeightCache<TcWeights> tc;           // tensor-core forward (the weight fields and status of TcWeights)
     WeightCache<TcBwdWeights> tc_bwd;    // tensor-core backward
-    DevBuf tc_feat;     // HexPlane feature staging of a tensor-core forward that keeps no features
+    DevBuf feat;        // the HexPlane features [N][F] of a forward that keeps none for its backward
     DevBuf tc_dbg;      // G4D_OPT_TC_DEBUG cycle counters
     DevBuf trow;        // time rows for the context-free deform entry points
     DevBuf scratch;     // misc per-call scratch (deform backward, kNN)
@@ -374,8 +374,9 @@ DeformDesc make_desc(const G4DDeformParams* p, float* const (*trow)[3], const Ff
 // the deformation network of one forward call
 struct DeformSetup {
     DeformDesc d;
-    bool tc;         // the forward runs on the tensor cores
-    TcWeights tw;    // tc: weight images, range flag and debug counters; the caller adds its feat / relu_bits buffers
+    bool tc;              // the network runs on the tensor cores
+    TcWeights tw;         // tc: weight images, range flag and debug counters; the caller adds its relu_bits buffer
+    DeformGather gather;  // the walk order; the caller adds the feature buffer
 };
 
 // The walk order of the HexPlane gather over xyz [n] into *out (NULL: index order).  Rebuilt when the xyz pointer or n
@@ -411,15 +412,14 @@ int collapse_time_rows(DevBuf& rows, float* (*trow)[3], const G4DDeformParams* p
     return G4D_OK;
 }
 
-// Pick the forward's path from the params, bring the gather's walk order over xyz [n] (tensor-core path) up to date, collapse
-// the time rows and bring the weight images the path reads up to date.  The desc is built after that refresh, which may move
+// Pick the forward's path from the params, bring the gather's walk order over xyz [n] up to date, collapse the time rows and
+// bring the weight images the path reads up to date.  The desc is built after that refresh, which may move
 // the transposes it embeds.
 int setup_deform(G4DWorkspace* ws, const G4DDeformParams* p, const float* xyz, int64_t n, DevBuf& rows, float* (*trow)[3],
                  TimeArg time, cudaStream_t st, DeformSetup* out) {
     int rc;
     out->tc = ws->tensor_cores != 0 && tc_deform_supported(*p, ws->tensor_cores);
-    const uint32_t* order = nullptr;
-    if (out->tc && (rc = gather_order(ws, p->aabb, xyz, n, st, &order)) != G4D_OK) return rc;
+    if ((rc = gather_order(ws, p->aabb, xyz, n, st, &out->gather.order)) != G4D_OK) return rc;
     if ((rc = collapse_time_rows(rows, trow, p, time, st)) != G4D_OK) return rc;
     if (!out->tc) {
         if ((rc = refresh_packed(ws, p, st)) != G4D_OK) return rc;
@@ -429,7 +429,6 @@ int setup_deform(G4DWorkspace* ws, const G4DDeformParams* p, const float* xyz, i
     if ((rc = refresh_tc(ws, p, st)) != G4D_OK) return rc;
     out->d = make_desc(p, trow, nullptr);
     out->tw = ws->tc.img;
-    out->tw.order = order;
     if (ws->tc_debug) {   // per-CTA phase cycle counters (g4d_debug_tc_cycles)
         G4D_CUDA(ws->tc_dbg.ensure((size_t)ws->sm_count * 12 * 8));
         G4D_CUDA(cudaMemsetAsync(ws->tc_dbg.p, 0, (size_t)ws->sm_count * 12 * 8, st));
@@ -438,41 +437,39 @@ int setup_deform(G4DWorkspace* ws, const G4DDeformParams* p, const float* xyz, i
     return G4D_OK;
 }
 
-// Buffers of this forward call.  feat: where a tensor-core forward stages the HexPlane features [N][F] (NULL: the
-// workspace's); relu_bits: where it saves the ReLU signs for a backward, or NULL.  The tag word behind the bits tells the
-// backward whether this forward wrote them.
+// Buffers of this forward call.  feat: where the gather writes the HexPlane features [N][F] (NULL: the workspace's);
+// relu_bits: where a tensor-core forward saves the ReLU signs for a backward, or NULL.  The tag word behind the bits tells
+// the backward whether this forward wrote them.
 int attach_forward_buffers(G4DWorkspace* ws, DeformSetup& s, float* feat, uint32_t* relu_bits, int64_t n, cudaStream_t st) {
-    if (s.tc && !feat) {
-        G4D_CUDA(ws->tc_feat.ensure((size_t)(n > 0 ? n : 1) * 64 * 4 + 256));
-        feat = ws->tc_feat.as<float>();
+    if (!feat) {
+        G4D_CUDA(ws->feat.ensure((size_t)(n > 0 ? n : 1) * (size_t)s.d.F * 4 + 256));
+        feat = ws->feat.as<float>();
     }
-    s.tw.feat = feat;
+    s.gather.feat = feat;
     s.tw.relu_bits = relu_bits;
     if (relu_bits) G4D_CUDA(cudaMemsetAsync(relu_bits + (size_t)24 * (size_t)n, s.tc ? kReluBitsTagByte : 0, 16, st));
     return G4D_OK;
 }
 
-// backward of the deformation network with the time rows trow: tensor-core path when the configuration allows, FFMA path
-// otherwise; the desc is built after the weight images of that path are current
+// backward of the deformation network with the time rows trow: picks the engine -- tensor-core when the configuration allows,
+// FFMA otherwise -- and brings its weight images up to date; the desc is built after that refresh
 int deform_backward_dispatch(G4DWorkspace* ws, const G4DDeformParams* prm, float* const (*trow)[3], const G4DDeformGrads* grads,
                              TimeArg time, int64_t n, const float* xyz, const float* const go[G4D_NUM_HEADS],
                              float* const gi[G4D_NUM_HEADS], const uint32_t* relu_bits, const float* saved_feat, cudaStream_t st) {
     int rc;
-    if (ws->tensor_cores && tc_backward_supported(*prm)) {
+    const bool tc = ws->tensor_cores && tc_backward_supported(*prm);
+    if (tc) {
         auto pack = [&](void* blob, TcBwdWeights* w) { return launch_tc_bwd_pack_weights(*prm, static_cast<uint8_t*>(blob), w, st); };
         G4D_CUDA(ws->tc_bwd.refresh(prm, 0, tc_bwd_weight_bytes(*prm), pack));
-        const DeformDesc d = make_desc(prm, trow, nullptr);
-        const uint32_t* order = nullptr;   // the walk order of the backward's own gather (none when the forward's features are kept)
-        if (!saved_feat && (rc = gather_order(ws, prm->aabb, xyz, n, st, &order)) != G4D_OK) return rc;
-        G4D_CUDA(ws->scratch.ensure(tc_deform_backward_scratch_bytes(d, n)));
-        G4D_CUDA(launch_deform_backward_tc(d, *prm, *grads, ws->tc_bwd.img, time, n, xyz, go, gi, relu_bits, saved_feat, order,
-                                           ws->scratch.as<uint8_t>(), ws->sm_count, st));
-        return G4D_OK;
+    } else if ((rc = refresh_packed(ws, prm, st)) != G4D_OK) {
+        return rc;
     }
-    if ((rc = refresh_packed(ws, prm, st)) != G4D_OK) return rc;
-    const DeformDesc d = make_desc(prm, trow, &ws->packed.img);
-    G4D_CUDA(ws->scratch.ensure(deform_backward_scratch_bytes(d, n)));
-    G4D_CUDA(launch_deform_backward(d, *prm, *grads, time, n, xyz, go, gi, ws->scratch.as<float>(), ws->sm_count, st));
+    const DeformDesc d = make_desc(prm, trow, tc ? nullptr : &ws->packed.img);
+    const uint32_t* order = nullptr;   // the walk order of the backward's own gather (none when the forward's features are kept)
+    if (!saved_feat && (rc = gather_order(ws, prm->aabb, xyz, n, st, &order)) != G4D_OK) return rc;
+    G4D_CUDA(ws->scratch.ensure(deform_backward_scratch_bytes(d, n, tc)));
+    G4D_CUDA(launch_deform_backward(d, *prm, *grads, tc ? &ws->tc_bwd.img : nullptr, time, n, xyz, go, gi, relu_bits, saved_feat,
+                                    order, ws->scratch.p, ws->sm_count, st));
     return G4D_OK;
 }
 
@@ -739,7 +736,7 @@ int g4d_deform_forward(G4DWorkspace* ws, const G4DDeformParams* prm, int64_t n, 
     if ((rc = attach_forward_buffers(ws, s, nullptr, relu_bits, n, st)) != G4D_OK) return rc;
     const DeformIO io{xyz, scaling, rotation, opacity, caller_sh<ShIn>(false, shs), out_xyz, out_scaling, out_rotation, out_opacity,
                       out_shs, GeomBuffers{}, FusedOutputs{}, nullptr};
-    G4D_CUDA(launch_deform(s.d, 0, nullptr, n, io, ws->sm_count, st, s.tc ? &s.tw : nullptr));
+    G4D_CUDA(launch_deform(s.d, 0, nullptr, n, io, s.gather, ws->sm_count, st, s.tc ? &s.tw : nullptr));
     return G4D_OK;
 }
 
@@ -967,7 +964,7 @@ int fused_forward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* pr
             }
             if ((rc = attach_forward_buffers(ws, s, save ? c->feat.as<float>() : nullptr, save ? c->relu.as<uint32_t>() : nullptr,
                                              n, st)) != G4D_OK) return rc;
-            G4D_CUDA(launch_deform(s.d, 1, dcam, n, io, ws->sm_count, st, s.tc ? &s.tw : nullptr));
+            G4D_CUDA(launch_deform(s.d, 1, dcam, n, io, s.gather, ws->sm_count, st, s.tc ? &s.tw : nullptr));
         } else {
             G4D_CUDA(launch_activate_preprocess(dcam, n, io, st));
         }

@@ -1,5 +1,7 @@
-// g4d_backward.cu -- per-Gaussian backward of the projection stage (A.4) and backward of the deformation
-// network (HexPlane scatter + MLP dgrad/wgrad).
+// g4d_backward.cu -- per-Gaussian backward of the projection stage (A.4) and the backward of the deformation network: the
+// frame every backward runs (HexPlane gather, scatter, time-row distribution) around the FFMA engine here or the tensor-core
+// engine of g4d_deform_tc_bwd.cu.  Compiled with the default FMA contraction: the coordinate normalisation of the scatter
+// rounds explicitly, as the forward's gather does (hexplane.cuh).
 // Reference autograd path replaced: loss.backward() at /root/reference/train.py:219 through
 // _RasterizeGaussians.backward, F.normalize/exp/sigmoid, nn.Linear, F.grid_sample.
 #include "g4d_internal.h"
@@ -152,27 +154,35 @@ cudaError_t launch_preprocess_backward_cameras(const BackwardCameras& bc, int64_
 }
 
 // ======================================================================================================
-// Backward of the deformation network.
+// Backward of the deformation network (DESIGN.md §4): one frame (launch_deform_backward) around one of two engines.
 //
-// Three persistent kernels (DESIGN.md §4):
-//   P  "prepass":  re-sample the HexPlane features and recompute a1 = relu(feat W0^T + b0) for every Gaussian
-//                  -> FEAT [N][F], A1 [N][Wd] in HBM.
-//   H  "heads":    CTA c owns ONE head (c mod #active) for its whole life: W1 (torch layout, padded) and W2 stay in
-//                  shared memory, dW1 / dW2 / db accumulate in REGISTERS across all the CTA's tiles and are flushed
-//                  once with atomics; per tile it recomputes z, a2, forms dz and writes da1_h = dz W1 -> DA1[h] in HBM.
-//   Q  "final":    dh = (sum_h DA1[h]) * (a1 > 0); dW0, db0 in registers; dfeat = dh W0; scatter-add into the planes
-//                  (vector RED; time planes through the collapsed rows), d(xyz) through the bilinear coordinates,
-//                  residual-path input gradients.
-//   T  distributes the collapsed time-row gradients onto the two time rows of each time plane.
+//   gather:   the forward's HexPlane gather, deform_features_kernel -> FEAT [N][F] (skipped when the forward kept its features)
+//   engine:   d(feat) -> DFEAT [N][F] and the network's weight gradients, either
+//             FFMA, three persistent kernels:
+//               P  "prepass":  a1 = relu(feat W0^T + b0) for every Gaussian -> A1 [N][Wd] in HBM.
+//               H  "heads":    CTA c owns ONE head (c mod #active) for its whole life: W1 (torch layout, padded) and W2 stay in
+//                              shared memory, dW1 / dW2 / db accumulate in REGISTERS across all the CTA's tiles and are
+//                              flushed once with atomics; per tile it recomputes z, a2, forms dz and writes da1_h = dz W1
+//                              -> DA1[h] in HBM.
+//               Q  "final":    dh = (sum_h DA1[h]) * (a1 > 0); dW0, db0 in registers; dfeat = dh W0 -> DFEAT.
+//             or tensor-core, kernels A (dgrad, -> DFEAT) and B (wgrad), g4d_deform_tc_bwd.cu, with the scatter between them.
+//   scatter:  bwd_scatter_kernel: DFEAT into the planes (vector RED; time planes through the collapsed rows), d(xyz) through
+//             the bilinear coordinates, residual-path input gradients.
+//   T         distributes the collapsed time-row gradients onto the two time rows of each time plane.
 // ======================================================================================================
 
+// The scratch of a backward: the engine's own -- the FFMA kernels' A1 and DA1 of every active head, or the tensor-core
+// kernels' operand images -- then the features and their gradient and the time-row gradients (both engines).
 struct DeformBwdBuffers {
-    float* feat;                      // [N][F]
-    float* a1;                        // [N][WD]
-    float* da1[G4D_NUM_HEADS];        // [N][WD] per active head
+    const float* feat;                // [N][F]: the gather's, or the features the forward kept
+    float* a1;                        // FFMA: [N][WD]
+    float* da1[G4D_NUM_HEADS];        // FFMA: [N][WD] per active head
+    float* dfeat;                     // [N][F]
     float* trow_grad[G4D_MAX_LEVELS][3];
+    uint8_t* images;                  // tensor-core: tc_bwd_images_bytes
 };
 
+// the arguments of a backward (the FFMA kernels read the network's; the scatter the planes' and the residual paths')
 struct DeformBwdDesc {
     DeformDesc d;
     const float* w0;                  // torch layout [WD][F]
@@ -213,8 +223,7 @@ G4D_D void tile_gemm_nt(const float* __restrict__ A, int lda, const float* __res
 // ---- kernel P ------------------------------------------------------------------------------------------
 template <int TG, int WD>
 __global__ void __launch_bounds__(kDeformThreads, 1)
-deform_bwd_prepass_kernel(DeformDesc d, DeformSmem L, int64_t n, const float* __restrict__ xyz,
-                          float* __restrict__ feat_out, float* __restrict__ a1_out) {
+deform_bwd_prepass_kernel(DeformDesc d, DeformSmem L, int64_t n, const float* __restrict__ feat, float* __restrict__ a1_out) {
     extern __shared__ __align__(16) float smem[];
     constexpr int RM = TG / 16, CG = WD / 64;
     const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
@@ -223,28 +232,10 @@ deform_bwd_prepass_kernel(DeformDesc d, DeformSmem L, int64_t n, const float* __
     for (int i = tid * 4; i < n0; i += kDeformThreads * 4)
         *reinterpret_cast<float4*>(smem + L.w0t + i) = __ldg(reinterpret_cast<const float4*>(d.w0t + i));
     for (int i = tid; i < WD; i += kDeformThreads) smem[L.b0 + i] = __ldg(d.b0 + i);
-    const AabbNorm nrm(d.aabb);
-    float* coord = smem + L.coord;
-    __syncthreads();
     for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const int64_t base = tile * TG, rem = n - base;
-        if (tid < TG) {
-            float4 c = make_float4(0.f, 0.f, 0.f, 0.f);   // (w unused: time enters through the collapsed time rows)
-            if (tid < rem) {
-                c.x = nrm(0, xyz[(base + tid) * 3 + 0]);
-                c.y = nrm(1, xyz[(base + tid) * 3 + 1]);
-                c.z = nrm(2, xyz[(base + tid) * 3 + 2]);
-            }
-            *reinterpret_cast<float4*>(coord + 4 * tid) = c;
-        }
+        load_feature_tile<TG>(feat, d.F, base, rem, smem + L.a0, L.lda0);
         __syncthreads();
-        sample_features<TG>(d, coord, smem + L.a0, L.lda0);
-        __syncthreads();
-        for (int i = tid; i < TG * (d.F >> 2); i += kDeformThreads) {
-            const int g = i / (d.F >> 2), v = i - g * (d.F >> 2);
-            if (g < rem)
-                *reinterpret_cast<float4*>(feat_out + (base + g) * d.F + 4 * v) = *reinterpret_cast<const float4*>(smem + L.a0 + g * L.lda0 + 4 * v);
-        }
         float acc[RM][CG * 4];
 #pragma unroll
         for (int r = 0; r < RM; ++r)
@@ -453,7 +444,7 @@ deform_bwd_heads_kernel(DeformBwdDesc bd, HeadSmem L, int64_t n, int num_active,
 }
 
 // ---- kernel Q ------------------------------------------------------------------------------------------
-struct FinalSmem { int w0, feat, dh, df, coord, total_floats, ldw0, ldf, ldh; };
+struct FinalSmem { int w0, feat, dh, total_floats, ldw0, ldf, ldh; };
 
 inline FinalSmem final_smem_layout(int TG, int F, int WD) {
     FinalSmem s{};
@@ -463,24 +454,20 @@ inline FinalSmem final_smem_layout(int TG, int F, int WD) {
     s.w0 = take(WD * s.ldw0);
     s.feat = take(TG * s.ldf);
     s.dh = take(TG * s.ldh);
-    s.df = take(TG * s.ldf);
-    s.coord = take(TG * 4);
     s.total_floats = off;
     return s;
 }
 
 template <int TG, int WD, int FM>
 __global__ void __launch_bounds__(kDeformThreads, 1)
-deform_bwd_final_kernel(DeformBwdDesc bd, FinalSmem L, int64_t n, const float* __restrict__ xyz,
-                        DeformBwdBuffers buf) {
+deform_bwd_final_kernel(DeformBwdDesc bd, FinalSmem L, int64_t n, DeformBwdBuffers buf) {
     extern __shared__ __align__(16) float smem[];
     const DeformDesc& d = bd.d;
     const int tid = threadIdx.x;
-    const int F = d.F, F4 = F >> 2, C4 = d.C >> 2;
+    const int F = d.F, F4 = F >> 2;
     constexpr int NG = kDeformThreads / WD;
     constexpr int MAXF = FM / NG;                   // dW0 accumulators per thread (F <= FM)
-    float* sW0 = smem + L.w0; float* sF = smem + L.feat; float* sDH = smem + L.dh; float* sDF = smem + L.df;
-    float* coord = smem + L.coord;
+    float* sW0 = smem + L.w0; float* sF = smem + L.feat; float* sDH = smem + L.dh;
     for (int i = tid; i < WD * F4; i += kDeformThreads) {
         const int r = i / F4, v = i - r * F4;
         *reinterpret_cast<float4*>(sW0 + r * L.ldw0 + 4 * v) = __ldg(reinterpret_cast<const float4*>(bd.w0 + r * F + 4 * v));
@@ -490,19 +477,12 @@ deform_bwd_final_kernel(DeformBwdDesc bd, FinalSmem L, int64_t n, const float* _
     for (int m = 0; m < MAXF; ++m) gW0[m] = 0.f;
     float gB0 = 0.f;
     const int w0_j = tid % WD, w0_g = tid / WD;
-    const AabbNorm nrm(d.aabb);
     const int64_t ntiles = (n + TG - 1) / TG;
-    constexpr int TPG = kDeformThreads / TG;
     __syncthreads();
 
     for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const int64_t base = tile * TG, rem = n - base;
-        for (int i = tid; i < TG * F4; i += kDeformThreads) {
-            const int g = i / F4, v = i - g * F4;
-            float4 val = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (g < rem) val = *reinterpret_cast<const float4*>(buf.feat + (base + g) * F + 4 * v);
-            *reinterpret_cast<float4*>(sF + g * L.ldf + 4 * v) = val;
-        }
+        load_feature_tile<TG>(buf.feat, F, base, rem, sF, L.ldf);
         for (int i = tid; i < TG * (WD >> 2); i += kDeformThreads) {
             const int g = i / (WD >> 2), v = i - g * (WD >> 2);
             float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -517,15 +497,6 @@ deform_bwd_final_kernel(DeformBwdDesc bd, FinalSmem L, int64_t n, const float* _
                 s.z = a1.z > 0.f ? s.z : 0.f; s.w = a1.w > 0.f ? s.w : 0.f;
             }
             *reinterpret_cast<float4*>(sDH + g * L.ldh + 4 * v) = s;
-        }
-        if (tid < TG) {
-            float4 c = make_float4(0.f, 0.f, 0.f, 0.f);   // (w unused: time enters through the collapsed time rows)
-            if (tid < rem) {
-                c.x = nrm(0, xyz[(base + tid) * 3 + 0]);
-                c.y = nrm(1, xyz[(base + tid) * 3 + 1]);
-                c.z = nrm(2, xyz[(base + tid) * 3 + 2]);
-            }
-            *reinterpret_cast<float4*>(coord + 4 * tid) = c;
         }
         __syncthreads();
         // dW0[j][f] += sum_g dh[g][j] feat[g][f];  thread owns row j = w0_j and columns f = w0_g + NG*m
@@ -542,52 +513,17 @@ deform_bwd_final_kernel(DeformBwdDesc bd, FinalSmem L, int64_t n, const float* _
             for (int g = 0; g < TG; ++g) s += sDH[g * L.ldh + tid];
             gB0 += s;
         }
-        // dfeat[g][f..f+3] = sum_j dh[g][j] W0[j][f..f+3]
+        // dfeat[g][f..f+3] = sum_j dh[g][j] W0[j][f..f+3]  -> DFEAT (the scatter's input)
         for (int i = tid; i < TG * F4; i += kDeformThreads) {
             const int g = i / F4, v = i - g * F4;
+            if (g >= rem) continue;
             float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
             for (int j = 0; j < WD; ++j) {
                 const float dh = sDH[g * L.ldh + j];
                 const float4 w = *reinterpret_cast<const float4*>(sW0 + j * L.ldw0 + 4 * v);
                 acc.x = fmaf(dh, w.x, acc.x); acc.y = fmaf(dh, w.y, acc.y); acc.z = fmaf(dh, w.z, acc.z); acc.w = fmaf(dh, w.w, acc.w);
             }
-            *reinterpret_cast<float4*>(sDF + g * L.ldf + 4 * v) = acc;
-        }
-        __syncthreads();
-        // scatter into the planes and d(xyz): thread (g, q) handles channel vectors v = q, q+TPG, ...
-        {
-            const int g = tid / TPG, q = tid % TPG;
-            const float4 pc = *reinterpret_cast<const float4*>(coord + 4 * g);
-            const float pcs[3] = {pc.x, pc.y, pc.z};
-            float gpix[3] = {0.f, 0.f, 0.f};   // dL/d(normalised coordinate) per axis
-            if (g < rem) {
-                for (int l = 0; l < d.levels; ++l) {
-                    Tap1D tx[3];
-#pragma unroll
-                    for (int a = 0; a < 3; ++a) tx[a] = make_tap(pcs[a], d.res[l][a]);
-                    for (int v = q; v < C4; v += TPG) {
-                        const float4 df = *reinterpret_cast<const float4*>(sDF + g * L.ldf + l * d.C + 4 * v);
-                        scatter_vector(d.planes[l], d.trow[l], d.res[l], bd.g_planes[l], buf.trow_grad[l], tx, v, C4, df, gpix);
-                    }
-                }
-            }
-            // reduce the TPG partial coordinate gradients of one Gaussian (adjacent lanes)
-#pragma unroll
-            for (int a = 0; a < 3; ++a)
-                for (int o = 1; o < TPG; o <<= 1) gpix[a] += __shfl_xor_sync(0xffffffffu, gpix[a], o);
-            if (q == 0 && g < rem && bd.gi[0]) {
-                const int64_t gi = base + g;
-#pragma unroll
-                for (int a = 0; a < 3; ++a)
-                    bd.gi[0][gi * 3 + a] = (bd.go[0] ? bd.go[0][gi * 3 + a] : 0.f) + gpix[a] * nrm.scale[a];
-            }
-        }
-        // residual path of the other inputs: d(out)/d(in) = identity
-        for (int hh = 1; hh < G4D_NUM_HEADS; ++hh) {
-            if (!bd.gi[hh]) continue;
-            const int ko = head_out(hh);
-            for (int i = tid; i < TG * ko; i += kDeformThreads)
-                if (i < rem * ko) bd.gi[hh][base * ko + i] = bd.go[hh] ? bd.go[hh][base * ko + i] : 0.f;
+            *reinterpret_cast<float4*>(buf.dfeat + (base + g) * F + 4 * v) = acc;
         }
         __syncthreads();
     }
@@ -597,6 +533,73 @@ deform_bwd_final_kernel(DeformBwdDesc bd, FinalSmem L, int64_t n, const float* _
         if (f < F) atomicAdd(bd.g_w0 + w0_j * F + f, gW0[m]);
     }
     if (tid < WD) atomicAdd(bd.g_b0 + tid, gB0);
+}
+
+// ---- HexPlane scatter of every backward at full occupancy: LPG lanes per Gaussian, lane v < C/4 scatters channel vector v --
+// LPG is C/4 rounded up to a power of two (the d(xyz) reduction shuffles over the lanes of one Gaussian); lanes v >= C/4 add
+// nothing.
+constexpr int scatter_lanes(int C4) { return C4 <= 1 ? 1 : C4 <= 2 ? 2 : C4 <= 4 ? 4 : 8; }
+
+struct BwdScatterDesc {
+    DeformDesc d;
+    const float* dfeat;                     // [N][F]
+    float* g_planes[G4D_MAX_LEVELS][6];
+    float* trow_grad[G4D_MAX_LEVELS][3];
+    const float* go[G4D_NUM_HEADS];
+    float* gi[G4D_NUM_HEADS];
+};
+
+template <int C4>
+__global__ void __launch_bounds__(256, 2) bwd_scatter_kernel(BwdScatterDesc sd, int64_t n, const float* __restrict__ xyz) {
+    const DeformDesc& d = sd.d;
+    constexpr int LPG = scatter_lanes(C4);
+    constexpr int GPB = 256 / LPG;          // Gaussians per block
+    const int64_t g0 = (int64_t)blockIdx.x * GPB;
+    const int64_t g = g0 + threadIdx.x / LPG;
+    const int v = threadIdx.x % LPG;
+    // residual path: d(out)/d(in) = identity for scaling / rotation / opacity / shs (contiguous ranges, coalesced)
+    for (int hh = 1; hh < G4D_NUM_HEADS; ++hh) {
+        if (!sd.gi[hh]) continue;
+        const int ko = head_out(hh);
+        const int64_t lo = g0 * ko, hi = (g0 + GPB < n ? g0 + GPB : n) * ko;
+        for (int64_t i = lo + threadIdx.x; i < hi; i += 256) sd.gi[hh][i] = sd.go[hh] ? sd.go[hh][i] : 0.f;
+    }
+    float gpix[3] = {0.f, 0.f, 0.f};
+    const AabbNorm nrm(d.aabb);
+    if (g < n && (LPG == C4 || v < C4)) {
+        float pcs[3];
+#pragma unroll
+        for (int a = 0; a < 3; ++a) pcs[a] = nrm(a, xyz[3 * g + a]);
+        for (int l = 0; l < d.levels; ++l) {
+            Tap1D tx[3];
+#pragma unroll
+            for (int a = 0; a < 3; ++a) tx[a] = make_tap(pcs[a], d.res[l][a]);
+            const float4 df = __ldg(reinterpret_cast<const float4*>(sd.dfeat + g * d.F + l * d.C + 4 * v));
+            scatter_vector(d.planes[l], d.trow[l], d.res[l], sd.g_planes[l], sd.trow_grad[l], tx, v, C4, df, gpix);
+        }
+    }
+    // the LPG lanes of a Gaussian are adjacent
+#pragma unroll
+    for (int a = 0; a < 3; ++a)
+        for (int o = 1; o < LPG; o <<= 1) gpix[a] += __shfl_xor_sync(0xffffffffu, gpix[a], o);
+    if (g < n && v == 0 && sd.gi[0]) {
+#pragma unroll
+        for (int a = 0; a < 3; ++a) sd.gi[0][g * 3 + a] = (sd.go[0] ? sd.go[0][g * 3 + a] : 0.f) + gpix[a] * nrm.scale[a];
+    }
+}
+
+static cudaError_t launch_bwd_scatter(const BwdScatterDesc& sd, int64_t n, const float* xyz, cudaStream_t st) {
+    const int C4 = sd.d.C / 4;
+    const unsigned grid = (unsigned)((n * scatter_lanes(C4) + 255) / 256);
+    switch (C4) {   // every channel width the C-ABI takes: C = 4 .. 32
+#define G4D_SCATTER_CASE(K) \
+        case K: bwd_scatter_kernel<K><<<grid, 256, 0, st>>>(sd, n, xyz); break;
+        G4D_SCATTER_CASE(1) G4D_SCATTER_CASE(2) G4D_SCATTER_CASE(3) G4D_SCATTER_CASE(4)
+        G4D_SCATTER_CASE(5) G4D_SCATTER_CASE(6) G4D_SCATTER_CASE(7) G4D_SCATTER_CASE(8)
+#undef G4D_SCATTER_CASE
+        default: return cudaErrorInvalidValue;
+    }
+    return cudaGetLastError();
 }
 
 // ---- kernel T: collapsed time-row gradients -> the two time rows of each (axis, t) plane --------------------
@@ -623,8 +626,8 @@ __global__ void distribute_time_grad_kernel(TimeGradDesc d, TimeArg time) {
 }
 
 // ---- host side -------------------------------------------------------------------------------------------
-cudaError_t launch_distribute_time_grad(const DeformDesc& d, float* const (*trow_grad)[3], float* const (*g_planes)[6], TimeArg time,
-                                        cudaStream_t st) {
+static cudaError_t launch_distribute_time_grad(const DeformDesc& d, float* const (*trow_grad)[3], float* const (*g_planes)[6],
+                                               TimeArg time, cudaStream_t st) {
     TimeGradDesc t{};
     t.levels = d.levels; t.C = d.C;
     const TimeRows tr(d.levels, d.res, d.C);
@@ -639,46 +642,49 @@ cudaError_t launch_distribute_time_grad(const DeformDesc& d, float* const (*trow
     return cudaGetLastError();
 }
 
-// the scratch of the FFMA backward: FEAT [N][F], A1 [N][WD], DA1 of every active head [N][WD], the time-row gradients;
-// returns the number of active heads
-static int carve_backward_scratch(Carve& m, const DeformDesc& d, const TimeRows& tr, int64_t n, DeformBwdBuffers& buf) {
+// carves the scratch; *gathered: where the gather writes the features (buf.feat until the forward's replace them)
+static DeformBwdBuffers carve_backward_scratch(Carve& m, const DeformDesc& d, int64_t n, bool tc, float** gathered) {
     const size_t N = (size_t)(n > 0 ? n : 1);
-    buf.feat = m.take<float>(N * d.F);
-    buf.a1 = m.take<float>(N * d.WD);
-    int active = 0;
-    for (int h = 0; h < G4D_NUM_HEADS; ++h)
-        if (d.head_mask & (1 << h)) { buf.da1[h] = m.take<float>(N * d.WD); ++active; }
+    const TimeRows tr(d.levels, d.res, d.C);
+    DeformBwdBuffers b{};
+    if (tc) {
+        b.images = m.take<uint8_t>(tc_bwd_images_bytes(d, n));
+    } else {
+        b.a1 = m.take<float>(N * d.WD);
+        for (int h = 0; h < G4D_NUM_HEADS; ++h)
+            if (d.head_mask & (1 << h)) b.da1[h] = m.take<float>(N * d.WD);
+    }
+    const size_t rows128 = (N + 127) / 128 * 128;   // whole tiles of the tensor-core kernels
+    b.feat = *gathered = m.take<float>(rows128 * d.F);
+    b.dfeat = m.take<float>(rows128 * d.F);
     float* rows = m.take<float>(tr.total());
-    if (rows) tr.place(rows, buf.trow_grad);
-    return active;
+    if (rows) tr.place(rows, b.trow_grad);
+    return b;
 }
 
-size_t deform_backward_scratch_bytes(const DeformDesc& d, int64_t n) {
+size_t deform_backward_scratch_bytes(const DeformDesc& d, int64_t n, bool tc) {
     Carve m;
-    DeformBwdBuffers buf{};
-    carve_backward_scratch(m, d, TimeRows(d.levels, d.res, d.C), n, buf);
+    float* gathered;
+    carve_backward_scratch(m, d, n, tc, &gathered);
     return m.bytes();
 }
 
+// FFMA engine: P, H, Q
 template <int TG, int WD>
-static cudaError_t launch_deform_backward_t(const DeformBwdDesc& bd, TimeArg time, int64_t n, const float* xyz, float* scratch,
-                                            int sm_count, cudaStream_t st) {
+static cudaError_t launch_ffma_engine(const DeformBwdDesc& bd, int64_t n, const DeformBwdBuffers& buf, int sm_count, cudaStream_t st) {
     const DeformDesc& d = bd.d;
-    DeformBwdBuffers buf{};
-    const TimeRows tr(d.levels, d.res, d.C);
-    Carve m(scratch);
-    const int active = carve_backward_scratch(m, d, tr, n, buf);
-    cudaError_t e = cudaMemsetAsync(buf.trow_grad[0][0], 0, tr.total() * sizeof(float), st);
-    if (e != cudaSuccess) return e;
+    int active = 0;
+    for (int h = 0; h < G4D_NUM_HEADS; ++h) active += (d.head_mask >> h) & 1;
     const int64_t ntiles = (n + TG - 1) / TG;
+    const int grid = (int)(ntiles < sm_count ? ntiles : sm_count);
+    cudaError_t e;
     // P
     {
         const DeformSmem L = deform_smem_layout(TG, d.F, WD, 0);
         const size_t bytes = (size_t)L.total_floats * 4;
         e = cudaFuncSetAttribute(deform_bwd_prepass_kernel<TG, WD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
         if (e != cudaSuccess) return e;
-        const int grid = (int)(ntiles < sm_count ? ntiles : sm_count);
-        deform_bwd_prepass_kernel<TG, WD><<<grid, kDeformThreads, bytes, st>>>(d, L, n, xyz, buf.feat, buf.a1);
+        deform_bwd_prepass_kernel<TG, WD><<<grid, kDeformThreads, bytes, st>>>(d, L, n, buf.feat, buf.a1);
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
     }
     // H
@@ -687,38 +693,38 @@ static cudaError_t launch_deform_backward_t(const DeformBwdDesc& bd, TimeArg tim
         const size_t bytes = (size_t)L.total_floats * 4;
         e = cudaFuncSetAttribute(deform_bwd_heads_kernel<TG, WD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
         if (e != cudaSuccess) return e;
-        int grid = sm_count;
-        if ((int64_t)grid > ntiles * active) grid = (int)(ntiles * active);
-        if (grid < active) grid = active;
-        deform_bwd_heads_kernel<TG, WD><<<grid, kDeformThreads, bytes, st>>>(bd, L, n, active, buf);
+        int hgrid = sm_count;
+        if ((int64_t)hgrid > ntiles * active) hgrid = (int)(ntiles * active);
+        if (hgrid < active) hgrid = active;
+        deform_bwd_heads_kernel<TG, WD><<<hgrid, kDeformThreads, bytes, st>>>(bd, L, n, active, buf);
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
     }
     // Q
-    {
-        const FinalSmem L = final_smem_layout(TG, d.F, WD);
-        const size_t bytes = (size_t)L.total_floats * 4;
-        const int grid = (int)(ntiles < sm_count ? ntiles : sm_count);
+    const FinalSmem L = final_smem_layout(TG, d.F, WD);
+    const size_t bytes = (size_t)L.total_floats * 4;
 #define G4D_LAUNCH_Q(FM)                                                                                                  \
-        do {                                                                                                              \
-            e = cudaFuncSetAttribute(deform_bwd_final_kernel<TG, WD, FM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes); \
-            if (e != cudaSuccess) return e;                                                                               \
-            deform_bwd_final_kernel<TG, WD, FM><<<grid, kDeformThreads, bytes, st>>>(bd, L, n, xyz, buf);            \
-        } while (0)
-        if (d.F <= 32) G4D_LAUNCH_Q(32);
-        else if (d.F <= 64) G4D_LAUNCH_Q(64);
-        else G4D_LAUNCH_Q(128);
+    do {                                                                                                                  \
+        e = cudaFuncSetAttribute(deform_bwd_final_kernel<TG, WD, FM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes); \
+        if (e != cudaSuccess) return e;                                                                                   \
+        deform_bwd_final_kernel<TG, WD, FM><<<grid, kDeformThreads, bytes, st>>>(bd, L, n, buf);                         \
+    } while (0)
+    if (d.F <= 32) G4D_LAUNCH_Q(32);
+    else if (d.F <= 64) G4D_LAUNCH_Q(64);
+    else G4D_LAUNCH_Q(128);
 #undef G4D_LAUNCH_Q
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    }
-    // T
-    if ((e = launch_distribute_time_grad(d, buf.trow_grad, bd.g_planes, time, st)) != cudaSuccess) return e;
-    return cudaSuccess;
+    return cudaGetLastError();
 }
 
-cudaError_t launch_deform_backward(const DeformDesc& d, const G4DDeformParams& prm, const G4DDeformGrads& grads, TimeArg time,
-                                   int64_t n, const float* xyz, const float* const go[G4D_NUM_HEADS],
-                                   float* const gi[G4D_NUM_HEADS], float* scratch, int sm_count, cudaStream_t st) {
+cudaError_t launch_deform_backward(const DeformDesc& d, const G4DDeformParams& prm, const G4DDeformGrads& grads, const TcBwdWeights* tc,
+                                   TimeArg time, int64_t n, const float* xyz, const float* const go[G4D_NUM_HEADS],
+                                   float* const gi[G4D_NUM_HEADS], const uint32_t* relu_bits, const float* saved_feat,
+                                   const uint32_t* order, void* scratch, int sm_count, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
+    const TimeRows tr(d.levels, d.res, d.C);
+    Carve m(scratch);
+    float* gathered;
+    DeformBwdBuffers buf = carve_backward_scratch(m, d, n, tc != nullptr, &gathered);
+    if (saved_feat) buf.feat = saved_feat;   // the features the forward of this view gathered
     DeformBwdDesc bd{};
     bd.d = d;
     bd.w0 = prm.w0; bd.g_w0 = grads.w0; bd.g_b0 = grads.b0;
@@ -726,11 +732,25 @@ cudaError_t launch_deform_backward(const DeformDesc& d, const G4DDeformParams& p
         bd.w1[h] = prm.w1[h]; bd.g_w1[h] = grads.w1[h]; bd.g_b1[h] = grads.b1[h]; bd.g_w2[h] = grads.w2[h]; bd.g_b2[h] = grads.b2[h];
         bd.go[h] = go[h]; bd.gi[h] = gi[h];
     }
-    for (int l = 0; l < d.levels; ++l)
-        for (int k = 0; k < 6; ++k) bd.g_planes[l][k] = grads.planes[l][k];
-    if (d.WD == 128) return launch_deform_backward_t<64, 128>(bd, time, n, xyz, scratch, sm_count, st);
-    if (d.WD == 64) return launch_deform_backward_t<128, 64>(bd, time, n, xyz, scratch, sm_count, st);
-    return cudaErrorInvalidValue;
+    BwdScatterDesc sc{};
+    sc.d = d; sc.dfeat = buf.dfeat;
+    for (int l = 0; l < d.levels; ++l) {
+        for (int k = 0; k < 6; ++k) bd.g_planes[l][k] = sc.g_planes[l][k] = grads.planes[l][k];
+        for (int a = 0; a < 3; ++a) sc.trow_grad[l][a] = buf.trow_grad[l][a];
+    }
+    for (int h = 0; h < G4D_NUM_HEADS; ++h) { sc.go[h] = go[h]; sc.gi[h] = gi[h]; }
+    cudaError_t e = cudaMemsetAsync(buf.trow_grad[0][0], 0, tr.total() * 4, st);
+    if (e != cudaSuccess) return e;
+    if (!saved_feat && (e = launch_deform_features(d, n, xyz, order, gathered, false, st)) != cudaSuccess) return e;
+    // the engine: d(feat) -> DFEAT and the weight gradients (the tensor-core wgrad kernel after the scatter)
+    if (tc) e = launch_tc_bwd_dgrad(d, *tc, n, go, relu_bits, buf.feat, buf.dfeat, buf.images, sm_count, st);
+    else if (d.WD == 128) e = launch_ffma_engine<64, 128>(bd, n, buf, sm_count, st);
+    else if (d.WD == 64) e = launch_ffma_engine<128, 64>(bd, n, buf, sm_count, st);
+    else e = cudaErrorInvalidValue;
+    if (e != cudaSuccess) return e;
+    if ((e = launch_bwd_scatter(sc, n, xyz, st)) != cudaSuccess) return e;
+    if (tc && (e = launch_tc_bwd_wgrad(d, grads, n, buf.images, sm_count, st)) != cudaSuccess) return e;
+    return launch_distribute_time_grad(d, buf.trow_grad, bd.g_planes, time, st);
 }
 
 // ------------------------------------------------------------------------------------------------------

@@ -568,7 +568,8 @@ cudaError_t launch_gather_order(const float* aabb, int64_t n, const float* xyz, 
 }
 
 // ---- HexPlane gather at full occupancy: C/4 threads per Gaussian, one channel vector each -> feat [N][F] fp32 -----------
-// (the forward chain launches it dependent on collapse_time_rows, the tensor-core backward as an ordinary launch).  Thread
+// The gather of every path (FFMA and tensor-core network, forward and backward): the forward launches it dependent on
+// collapse_time_rows, the backward as an ordinary launch.  Thread
 // group j gathers Gaussian order[j] (j itself when order is NULL): in spatial order the 8 Gaussians of a warp, and the warps
 // of an SM, tap neighbouring plane texels and share them in L1.  feat[g] depends on xyz[g] alone, so any order gives the
 // same bits.
@@ -599,8 +600,13 @@ cudaError_t launch_deform_features(const DeformDesc& d, int64_t n, const float* 
     if (n == 0) return cudaSuccess;
     const int C4 = d.C / 4;
     const unsigned grid = (unsigned)((n * C4 + 255) / 256);
-    if (C4 == 4) return launch_k(deform_features_kernel<4>, dim3(grid), dim3(256), 0, st, pdl, d, n, xyz, order, feat);
-    if (C4 == 8) return launch_k(deform_features_kernel<8>, dim3(grid), dim3(256), 0, st, pdl, d, n, xyz, order, feat);
+    switch (C4) {   // every channel width the C-ABI takes: C = 4 .. 32
+#define G4D_GATHER_CASE(K) \
+        case K: return launch_k(deform_features_kernel<K>, dim3(grid), dim3(256), 0, st, pdl, d, n, xyz, order, feat);
+        G4D_GATHER_CASE(1) G4D_GATHER_CASE(2) G4D_GATHER_CASE(3) G4D_GATHER_CASE(4)
+        G4D_GATHER_CASE(5) G4D_GATHER_CASE(6) G4D_GATHER_CASE(7) G4D_GATHER_CASE(8)
+#undef G4D_GATHER_CASE
+    }
     return cudaErrorInvalidValue;
 }
 
@@ -630,10 +636,6 @@ cudaError_t launch_deform_tc(const DeformDesc& d, const TcWeights& tw, int mode,
                              const DeformIO& io, int sm_count, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
     if (!tw.feat) return cudaErrorInvalidValue;
-    {
-        cudaError_t e = launch_deform_features(d, n, io.xyz, tw.order, tw.feat, true, st);
-        if (e != cudaSuccess) return e;
-    }
     const TcSmem Ls = tc_smem_layout(tw.arith, d.F, (d.head_mask & G4D_HEAD_SHS) != 0);
     const size_t bytes = Ls.total;
     const int64_t ntiles = (n + 64 * (tw.arith == 2 ? 2 : 1) - 1) / (64 * (tw.arith == 2 ? 2 : 1));

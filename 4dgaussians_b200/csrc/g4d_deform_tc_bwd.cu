@@ -9,9 +9,8 @@
 //               signs come from the bits the forward saved (G4D_RELU_BITS_WORDS), so this is the gradient of the forward
 //               that ran.  Everything the weight gradients need is written ONCE to global memory as ready-to-use MMA operand
 //               images (8x8 bf16 core-matrix layout) so that kernel B is pure TMA + MMA.
-//               HexPlane gather (the forward's deform_features_kernel, skipped when the forward's staging buffer was kept)
-//               and scatter (bwd_scatter_kernel: plane REDs, d(xyz), residual paths; hexplane.cuh) run around it at full
-//               occupancy.
+//               The HexPlane gather before it and the scatter after it are the ones every backward runs
+//               (launch_deform_backward, g4d_backward.cu).
 //  B  "wgrad":  dW1_h = DZ_h^T A1, dW2_h^T = A2_h^T DOUT_h, db1_h = DZ_h^T 1, db2_h = 1^T DOUT_h, dW0 = DH^T FEAT, db0 = DH^T 1
 //               as split-K GEMMs over the Gaussian index (operands MN-major straight from the images), accumulators in
 //               registers across the CTA's tiles (warpgroup w: output rows [64 w, 64 w + 64)), one atomic flush per CTA;
@@ -185,7 +184,7 @@ struct BwdADesc {
     BwdImages img;
     const float* go[G4D_NUM_HEADS];
     const float* feat;           // [N][F] fp32 (deform_features_kernel)
-    float* dfeat;                // [N][F] fp32 -> bwd_scatter_kernel
+    float* dfeat;                // [N][F] fp32 -> the scatter (bwd_scatter_kernel)
     const uint32_t* relu_bits;   // [6][N][4] + tag (g4d.h G4D_RELU_BITS_WORDS) or NULL
 };
 
@@ -443,54 +442,6 @@ deform_tc_bwd_dgrad_kernel(BwdADesc bd, BwdSmemA Ls, int64_t n) {
     }
 }
 
-// ---- HexPlane scatter at full occupancy (C/4 threads per Gaussian, one channel vector each) -----------------------
-struct BwdScatterDesc {
-    DeformDesc d;
-    const float* dfeat;                     // [N][F]
-    float* g_planes[G4D_MAX_LEVELS][6];
-    float* trow_grad[G4D_MAX_LEVELS][3];
-    const float* go[G4D_NUM_HEADS];
-    float* gi[G4D_NUM_HEADS];
-};
-
-template <int C4>
-__global__ void __launch_bounds__(256, 2) bwd_scatter_kernel(BwdScatterDesc sd, int64_t n, const float* __restrict__ xyz) {
-    const DeformDesc& d = sd.d;
-    constexpr int GPB = 256 / C4;           // Gaussians per block
-    const int64_t g0 = (int64_t)blockIdx.x * GPB;
-    const int64_t g = g0 + threadIdx.x / C4;
-    const int v = threadIdx.x % C4;
-    // residual path: d(out)/d(in) = identity for scaling / rotation / opacity / shs (contiguous ranges, coalesced)
-    for (int hh = 1; hh < G4D_NUM_HEADS; ++hh) {
-        if (!sd.gi[hh]) continue;
-        const int ko = head_out(hh);
-        const int64_t lo = g0 * ko, hi = (g0 + GPB < n ? g0 + GPB : n) * ko;
-        for (int64_t i = lo + threadIdx.x; i < hi; i += 256) sd.gi[hh][i] = sd.go[hh] ? sd.go[hh][i] : 0.f;
-    }
-    float gpix[3] = {0.f, 0.f, 0.f};
-    const AabbNorm nrm(d.aabb);
-    if (g < n) {
-        float pcs[3];
-#pragma unroll
-        for (int a = 0; a < 3; ++a) pcs[a] = nrm(a, xyz[3 * g + a]);
-        for (int l = 0; l < d.levels; ++l) {
-            Tap1D tx[3];
-#pragma unroll
-            for (int a = 0; a < 3; ++a) tx[a] = make_tap(pcs[a], d.res[l][a]);
-            const float4 df = __ldg(reinterpret_cast<const float4*>(sd.dfeat + g * d.F + l * d.C + 4 * v));
-            scatter_vector(d.planes[l], d.trow[l], d.res[l], sd.g_planes[l], sd.trow_grad[l], tx, v, C4, df, gpix);
-        }
-    }
-    // the C4 threads of a Gaussian are adjacent lanes
-#pragma unroll
-    for (int a = 0; a < 3; ++a)
-        for (int o = 1; o < C4; o <<= 1) gpix[a] += __shfl_xor_sync(0xffffffffu, gpix[a], o);
-    if (g < n && v == 0 && sd.gi[0]) {
-#pragma unroll
-        for (int a = 0; a < 3; ++a) sd.gi[0][g * 3 + a] = (sd.go[0] ? sd.go[0][g * 3 + a] : 0.f) + gpix[a] * nrm.scale[a];
-    }
-}
-
 // ======================================================================================================
 // Kernel B: weight gradients from the operand images.
 //   CTA (group, chunk): group = an active head or layer 0.  Two warpgroups, warpgroup w accumulates output rows
@@ -637,33 +588,29 @@ __global__ void __launch_bounds__(256, 1) deform_tc_bwd_wgrad_kernel(BwdBDesc b)
 }
 
 // ======================================================================================================
-// host side
+// host side: the tensor-core engine of the deformation backward (launch_deform_backward, g4d_backward.cu, runs the gather,
+// the scatter and the time-row distribution around it)
 // ======================================================================================================
-// the scratch of the tensor-core backward: the operand images of kernel B (per tile of 128 Gaussians), the fp32 features and
-// their gradient [ntiles * 128][F], the time-row gradients
-struct TcBwdScratch { BwdImages img; float* feat; float* dfeat; float* trow_grad; };
-static TcBwdScratch carve_tc_backward_scratch(Carve& m, const DeformDesc& d, const TimeRows& tr, int64_t n) {
+// the operand images kernel A writes for kernel B, per tile of 128 Gaussians
+static BwdImages carve_images(Carve& m, const DeformDesc& d, int64_t n) {
     const size_t ntiles = (size_t)((n + 127) / 128);
-    TcBwdScratch s{};
-    s.img.feat_bytes = 2u * 128 * d.F * 2;
-    s.img.a1 = m.take<uint8_t>(ntiles * 2 * kImg128);
-    s.img.dh = m.take<uint8_t>(ntiles * 2 * kImg128);
-    s.img.feat = m.take<uint8_t>(ntiles * s.img.feat_bytes);
+    BwdImages img{};
+    img.feat_bytes = 2u * 128 * d.F * 2;
+    img.a1 = m.take<uint8_t>(ntiles * 2 * kImg128);
+    img.dh = m.take<uint8_t>(ntiles * 2 * kImg128);
+    img.feat = m.take<uint8_t>(ntiles * img.feat_bytes);
     for (int h = 0; h < G4D_NUM_HEADS; ++h) {
         if (!(d.head_mask & (1 << h))) continue;
-        s.img.dz[h] = m.take<uint8_t>(ntiles * 2 * kImg128);
-        s.img.a2[h] = m.take<uint8_t>(ntiles * 2 * kImg128);
-        s.img.dout[h] = m.take<uint8_t>(ntiles * 2 * 128 * (h == 4 ? 48 : 16) * 2);
+        img.dz[h] = m.take<uint8_t>(ntiles * 2 * kImg128);
+        img.a2[h] = m.take<uint8_t>(ntiles * 2 * kImg128);
+        img.dout[h] = m.take<uint8_t>(ntiles * 2 * 128 * (h == 4 ? 48 : 16) * 2);
     }
-    s.feat = m.take<float>(ntiles * 128 * d.F);
-    s.dfeat = m.take<float>(ntiles * 128 * d.F);
-    s.trow_grad = m.take<float>(tr.total());
-    return s;
+    return img;
 }
 
-size_t tc_deform_backward_scratch_bytes(const DeformDesc& d, int64_t n) {
+size_t tc_bwd_images_bytes(const DeformDesc& d, int64_t n) {
     Carve m;
-    carve_tc_backward_scratch(m, d, TimeRows(d.levels, d.res, d.C), n);
+    carve_images(m, d, n);
     return m.bytes();
 }
 
@@ -679,46 +626,26 @@ static cudaError_t launch_a(const BwdADesc& bd, int64_t n, int sm_count, cudaStr
     return cudaGetLastError();
 }
 
-cudaError_t launch_deform_backward_tc(const DeformDesc& d, const G4DDeformParams& prm, const G4DDeformGrads& grads,
-                                      const TcBwdWeights& w, TimeArg time, int64_t n, const float* xyz,
-                                      const float* const go[G4D_NUM_HEADS], float* const gi[G4D_NUM_HEADS],
-                                      const uint32_t* relu_bits, const float* saved_feat, const uint32_t* order, uint8_t* scratch,
-                                      int sm_count, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    const int64_t ntiles = (n + 127) / 128;
-    const TimeRows tr(d.levels, d.res, d.C);
-    Carve m(scratch);
-    const TcBwdScratch s = carve_tc_backward_scratch(m, d, tr, n);
+cudaError_t launch_tc_bwd_dgrad(const DeformDesc& d, const TcBwdWeights& w, int64_t n, const float* const go[G4D_NUM_HEADS],
+                                const uint32_t* relu_bits, const float* feat, float* dfeat, uint8_t* images, int sm_count,
+                                cudaStream_t st) {
+    Carve m(images);
     BwdADesc a{};
-    a.d = d; a.w = w; a.relu_bits = relu_bits; a.img = s.img;
+    a.d = d; a.w = w; a.relu_bits = relu_bits; a.img = carve_images(m, d, n);
     for (int h = 0; h < G4D_NUM_HEADS; ++h) a.go[h] = go[h];
-    a.feat = saved_feat ? saved_feat : s.feat; a.dfeat = s.dfeat;   // saved_feat: the features the forward of this view staged
-    BwdScatterDesc sc{};
-    sc.d = d; sc.dfeat = s.dfeat;
-    for (int l = 0; l < d.levels; ++l)
-        for (int k = 0; k < 6; ++k) sc.g_planes[l][k] = grads.planes[l][k];
-    tr.place(s.trow_grad, sc.trow_grad);
-    for (int h = 0; h < G4D_NUM_HEADS; ++h) { sc.go[h] = go[h]; sc.gi[h] = gi[h]; }
-    cudaError_t e = cudaMemsetAsync(s.trow_grad, 0, tr.total() * 4, st);
-    if (e != cudaSuccess) return e;
-    // the forward's gather (skipped when the forward's feature staging buffer was kept for this backward)
-    if (!saved_feat && (e = launch_deform_features(d, n, xyz, order, s.feat, false, st)) != cudaSuccess) return e;
-    if (d.C == 16 && d.levels == 2) e = launch_a<16, 2>(a, n, sm_count, st);
-    else if (d.C == 16 && d.levels == 3) e = launch_a<16, 3>(a, n, sm_count, st);
-    else if (d.C == 32 && d.levels == 2) e = launch_a<32, 2>(a, n, sm_count, st);
-    else return cudaErrorInvalidValue;
-    if (e != cudaSuccess) return e;
-    // scatter d(feat) into the planes, d(xyz), residual copies
-    {
-        const int C4 = d.C / 4, gpb = 256 / C4;
-        const unsigned grid = (unsigned)((n + gpb - 1) / gpb);
-        if (C4 == 4) bwd_scatter_kernel<4><<<grid, 256, 0, st>>>(sc, n, xyz);
-        else bwd_scatter_kernel<8><<<grid, 256, 0, st>>>(sc, n, xyz);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    }
-    // kernel B
+    a.feat = feat; a.dfeat = dfeat;
+    if (d.C == 16 && d.levels == 2) return launch_a<16, 2>(a, n, sm_count, st);
+    if (d.C == 16 && d.levels == 3) return launch_a<16, 3>(a, n, sm_count, st);
+    if (d.C == 32 && d.levels == 2) return launch_a<32, 2>(a, n, sm_count, st);
+    return cudaErrorInvalidValue;
+}
+
+cudaError_t launch_tc_bwd_wgrad(const DeformDesc& d, const G4DDeformGrads& grads, int64_t n, uint8_t* images, int sm_count,
+                                cudaStream_t st) {
+    const int64_t ntiles = (n + 127) / 128;
+    Carve m(images);
     BwdBDesc b{};
-    b.img = a.img; b.head_mask = d.head_mask; b.F = d.F; b.ntiles = ntiles;
+    b.img = carve_images(m, d, n); b.head_mask = d.head_mask; b.F = d.F; b.ntiles = ntiles;
     {
         int nheads = 0;
         for (int h = 0; h < G4D_NUM_HEADS; ++h) nheads += (d.head_mask >> h) & 1;
@@ -735,11 +662,10 @@ cudaError_t launch_deform_backward_tc(const DeformDesc& d, const G4DDeformParams
     b.g_w0 = grads.w0; b.g_b0 = grads.b0;
     for (int h = 0; h < G4D_NUM_HEADS; ++h) { b.g_w1[h] = grads.w1[h]; b.g_b1[h] = grads.b1[h]; b.g_w2[h] = grads.w2[h]; b.g_b2[h] = grads.b2[h]; }
     const size_t smem_b = (size_t)2 * kStage + kOnes + 1024;   // two half-tile stages + the all-ones operand
-    e = cudaFuncSetAttribute(deform_tc_bwd_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_b);
+    cudaError_t e = cudaFuncSetAttribute(deform_tc_bwd_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_b);
     if (e != cudaSuccess) return e;
     deform_tc_bwd_wgrad_kernel<<<b.nheads * b.chunks_head + b.chunks_l0, 256, smem_b, st>>>(b);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    return launch_distribute_time_grad(d, sc.trow_grad, sc.g_planes, time, st);
+    return cudaGetLastError();
 }
 
 }  // namespace g4d

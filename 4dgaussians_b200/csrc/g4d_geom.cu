@@ -191,12 +191,13 @@ cudaError_t launch_project_cameras(const ExtraCameras& ec, int64_t n, const Rast
 }
 
 // ------------------------------------------------------------------------------------------------------
-// Persistent kernel: one CTA per SM, each looping over tiles of TG Gaussians.
+// Persistent kernel: one CTA per SM, each looping over tiles of TG Gaussians whose HexPlane features feat [N][F] the gather
+// wrote (an ordinary launch: the gather has completed).
 //   MODE 0: deformation network only (drop-in for deform_network.forward; outputs pre-activation tensors)
 //   MODE 1: fused deformation + activations + projection (the render() hot path)
 template <int TG, int WD, int MODE>
 __global__ void __launch_bounds__(kDeformThreads, 1)
-deform_kernel(DeformDesc d, DeformSmem L, const CameraDev* __restrict__ camp, int64_t n, DeformIO io) {
+deform_kernel(DeformDesc d, DeformSmem L, const CameraDev* __restrict__ camp, int64_t n, const float* __restrict__ feat, DeformIO io) {
     extern __shared__ __align__(16) float smem[];
     __shared__ CameraDev cam;
     const int tid = threadIdx.x;
@@ -214,12 +215,10 @@ deform_kernel(DeformDesc d, DeformSmem L, const CameraDev* __restrict__ camp, in
         tma_bulk_g2s(smem + L.w1t, d.w1t[first], (uint32_t)(WD * WD * sizeof(float)), bar);
     }
     uint32_t phase = 0;
-    const AabbNorm nrm(d.aabb);
     float* in_xyz = smem + L.in;
     float* in_sc = in_xyz + TG * 3;
     float* in_rot = in_sc + TG * 3;
     float* in_op = in_rot + TG * 4;
-    float* coord = smem + L.coord;
     float* out = smem + L.out;
     const bool hp = d.head_mask & G4D_HEAD_POS, hs = d.head_mask & G4D_HEAD_SCALES, hr = d.head_mask & G4D_HEAD_ROT,
                ho = d.head_mask & G4D_HEAD_OPACITY, hsh = d.head_mask & G4D_HEAD_SHS;
@@ -234,15 +233,7 @@ deform_kernel(DeformDesc d, DeformSmem L, const CameraDev* __restrict__ camp, in
         }
         for (int i = tid; i < TG * 4; i += kDeformThreads) in_rot[i] = (i < rem * 4 && io.rotation) ? io.rotation[base * 4 + i] : 0.f;
         for (int i = tid; i < TG; i += kDeformThreads) in_op[i] = (i < rem && io.opacity) ? io.opacity[base + i] : 0.f;
-        __syncthreads();
-        if (tid < TG) {
-            float4 c;
-            c.x = nrm(0, in_xyz[3 * tid + 0]);
-            c.y = nrm(1, in_xyz[3 * tid + 1]);
-            c.z = nrm(2, in_xyz[3 * tid + 2]);
-            c.w = 0.f;          // (time enters through the collapsed time rows)
-            *reinterpret_cast<float4*>(coord + 4 * tid) = c;
-        }
+        load_feature_tile<TG>(feat, d.F, base, rem, smem + L.a0, L.lda0);
         __syncthreads();
         deform_mlp_tile<TG, WD>(d, L, smem, phase, tile + gridDim.x < ntiles);
 
@@ -298,8 +289,8 @@ cudaError_t launch_deform_tc(const DeformDesc& d, const TcWeights& tw, int mode,
                              const DeformIO& io, int sm_count, cudaStream_t st);
 
 template <int TG, int WD, int MODE>
-static cudaError_t launch_deform_t(const DeformDesc& d, const CameraDev* cam, int64_t n, const DeformIO& io, int sm_count,
-                                   cudaStream_t st) {
+static cudaError_t launch_deform_t(const DeformDesc& d, const CameraDev* cam, int64_t n, const float* feat, const DeformIO& io,
+                                   int sm_count, cudaStream_t st) {
     const DeformSmem L = deform_smem_layout(TG, d.F, WD, d.head_mask);
     const size_t bytes = (size_t)L.total_floats * sizeof(float);
     if (bytes > 227 * 1024) return cudaErrorInvalidConfiguration;
@@ -307,20 +298,27 @@ static cudaError_t launch_deform_t(const DeformDesc& d, const CameraDev* cam, in
     if (e != cudaSuccess) return e;
     const int64_t ntiles = (n + TG - 1) / TG;
     const int grid = (int)(ntiles < sm_count ? ntiles : sm_count);
-    deform_kernel<TG, WD, MODE><<<grid, kDeformThreads, bytes, st>>>(d, L, cam, n, io);
+    deform_kernel<TG, WD, MODE><<<grid, kDeformThreads, bytes, st>>>(d, L, cam, n, feat, io);
     return cudaGetLastError();
 }
 
-cudaError_t launch_deform(const DeformDesc& d, int mode, const CameraDev* cam, int64_t n, const DeformIO& io, int sm_count,
-                          cudaStream_t st, const TcWeights* tw) {
+cudaError_t launch_deform(const DeformDesc& d, int mode, const CameraDev* cam, int64_t n, const DeformIO& io, const DeformGather& gather,
+                          int sm_count, cudaStream_t st, const TcWeights* tw) {
     if (n == 0) return cudaSuccess;
-    if (tw) return launch_deform_tc(d, *tw, mode, cam, n, io, sm_count, st);
+    // the HexPlane gather of every path, dependent on the time-row collapse before it (DESIGN.md §4.6)
+    cudaError_t e = launch_deform_features(d, n, io.xyz, gather.order, gather.feat, true, st);
+    if (e != cudaSuccess) return e;
+    if (tw) {
+        TcWeights t = *tw;
+        t.feat = gather.feat; t.order = gather.order;
+        return launch_deform_tc(d, t, mode, cam, n, io, sm_count, st);
+    }
     if (d.WD == 128) {
-        return mode == 0 ? launch_deform_t<64, 128, 0>(d, cam, n, io, sm_count, st)
-                         : launch_deform_t<64, 128, 1>(d, cam, n, io, sm_count, st);
+        return mode == 0 ? launch_deform_t<64, 128, 0>(d, cam, n, gather.feat, io, sm_count, st)
+                         : launch_deform_t<64, 128, 1>(d, cam, n, gather.feat, io, sm_count, st);
     } else if (d.WD == 64) {
-        return mode == 0 ? launch_deform_t<128, 64, 0>(d, cam, n, io, sm_count, st)
-                         : launch_deform_t<128, 64, 1>(d, cam, n, io, sm_count, st);
+        return mode == 0 ? launch_deform_t<128, 64, 0>(d, cam, n, gather.feat, io, sm_count, st)
+                         : launch_deform_t<128, 64, 1>(d, cam, n, gather.feat, io, sm_count, st);
     }
     return cudaErrorInvalidValue;
 }

@@ -210,8 +210,8 @@ struct TcWeights {
     const float* w1[G4D_NUM_HEADS];    // packed (hi | lo) K-parts, [128][128]
     const float* w2[G4D_NUM_HEADS];    // SH head only: packed (hi | lo), [48][128]
     long long* dbg;                    // optional [grid][12] per-phase cycle counters (debug)
-    float* feat;                       // [N][F] fp32 staging of the HexPlane features (deform_features_kernel)
-    const uint32_t* order;             // optional [N]: the gather's walk order (launch_gather_order); NULL: index order
+    float* feat;                       // the HexPlane features [N][F] and the walk order that gathered them (launch_deform's
+    const uint32_t* order;             // DeformGather)
     uint32_t* relu_bits;             // optional [6][N][4]: ReLU sign bits saved for the backward (G4D_RELU_BITS_WORDS)
     int arith;                         // 1: 3xTF32, 2: FP16x2 (G4D_OPT_TENSOR_CORES)
     uint32_t* status;                  // host-mapped word: set to 1 by the FP16x2 kernel when a value left the f16 operand range
@@ -245,15 +245,14 @@ struct TcBwdWeights {
 size_t tc_bwd_weight_bytes(const G4DDeformParams& prm);
 cudaError_t launch_tc_bwd_pack_weights(const G4DDeformParams& prm, uint8_t* blob, TcBwdWeights* out, cudaStream_t st);
 bool tc_backward_supported(const G4DDeformParams& prm);
-size_t tc_deform_backward_scratch_bytes(const DeformDesc& d, int64_t n);   // size of launch_deform_backward_tc's scratch
-cudaError_t launch_deform_backward_tc(const DeformDesc& d, const G4DDeformParams& prm, const G4DDeformGrads& grads,
-                                      const TcBwdWeights& w, TimeArg time, int64_t n, const float* xyz,
-                                      const float* const go[G4D_NUM_HEADS], float* const gi[G4D_NUM_HEADS],
-                                      const uint32_t* relu_bits, const float* saved_feat, const uint32_t* order, uint8_t* scratch,
-                                      int sm_count, cudaStream_t st);
-// collapsed time-row gradients -> the two time rows of each (axis, t) plane (g4d_backward.cu)
-cudaError_t launch_distribute_time_grad(const DeformDesc& d, float* const (*trow_grad)[3], float* const (*g_planes)[6], TimeArg time,
-                                        cudaStream_t st);
+// The tensor-core engine of the deformation backward (launch_deform_backward runs it): kernel A (dgrad) writes d(feat) [N][F]
+// and the operand images of kernel B (wgrad), which writes the weight gradients.  `images`: tc_bwd_images_bytes of scratch.
+size_t tc_bwd_images_bytes(const DeformDesc& d, int64_t n);
+cudaError_t launch_tc_bwd_dgrad(const DeformDesc& d, const TcBwdWeights& w, int64_t n, const float* const go[G4D_NUM_HEADS],
+                                const uint32_t* relu_bits, const float* feat, float* dfeat, uint8_t* images, int sm_count,
+                                cudaStream_t st);
+cudaError_t launch_tc_bwd_wgrad(const DeformDesc& d, const G4DDeformGrads& grads, int64_t n, uint8_t* images, int sm_count,
+                                cudaStream_t st);
 
 // ---- launchers (defined in g4d_geom.cu / g4d_raster.cu / g4d_backward.cu) -----------------------------
 // d_time: the camera's timestamp from device memory (NULL: cam.time)
@@ -262,10 +261,16 @@ cudaError_t launch_pack_weights(const G4DDeformParams& p, float* w0t, float* con
 cudaError_t launch_collapse_time_rows(const G4DDeformParams& p, TimeArg time, float* const (*trow)[3], cudaStream_t st);
 cudaError_t launch_preprocess(const CameraDev* cam, int64_t n, const RasterInputs& in, GeomBuffers g, int32_t* out_radii,
                               cudaStream_t st);
-// mode 0: deform only (writes the five out_* tensors; cam unused); mode 1: fused deform + preprocess (camera from cam).
-// tw: run on the tensor cores with these weight images and buffers
-cudaError_t launch_deform(const DeformDesc& d, int mode, const CameraDev* cam, int64_t n, const DeformIO& io, int sm_count,
-                          cudaStream_t st, const TcWeights* tw = nullptr);
+// The HexPlane gather of a forward: feat [N][F] fp32 receives the features, Gaussians visited in `order` (NULL: index order).
+struct DeformGather {
+    float* feat;
+    const uint32_t* order;
+};
+// The gather (launch_deform_features, dependent on the time-row collapse before it), then the network: mode 0: deform only
+// (writes the five out_* tensors; cam unused); mode 1: fused deform + preprocess (camera from cam).  tw: the network runs on
+// the tensor cores with these weight images and buffers, else on the FFMA kernel (an ordinary launch).
+cudaError_t launch_deform(const DeformDesc& d, int mode, const CameraDev* cam, int64_t n, const DeformIO& io, const DeformGather& gather,
+                          int sm_count, cudaStream_t st, const TcWeights* tw = nullptr);
 
 // The per-Gaussian gradients of one blend backward in one float buffer, as blocks of N floats: d(mean2D) [2N] from block
 // kMean2D, d(conic) [3N] from kConic, d(rgb) [3N] from kRgb, d(opacity) [N] from kOpacity; kFloats blocks in all.
@@ -284,11 +289,15 @@ cudaError_t launch_preprocess_backward(const CameraDev* cam, int64_t n, const Ra
                                        float* g_means2D_out, float* g_scales, float* g_rotations, const ShOut& g_sh,
                                        cudaStream_t st);
 
-size_t deform_backward_scratch_bytes(const DeformDesc& d, int64_t n);   // size of launch_deform_backward's scratch
-// go[h] / gi[h]: gradient w.r.t. the outputs / inputs of head h's residual tensor (xyz, scaling, rotation, opacity, shs)
-cudaError_t launch_deform_backward(const DeformDesc& d, const G4DDeformParams& prm, const G4DDeformGrads& grads, TimeArg time,
-                                   int64_t n, const float* xyz, const float* const go[G4D_NUM_HEADS],
-                                   float* const gi[G4D_NUM_HEADS], float* scratch, int sm_count, cudaStream_t st);
+// Backward of the deformation network (g4d_backward.cu): the HexPlane gather (skipped when saved_feat holds the features
+// the forward gathered; order: its walk order), an engine -- the tensor-core kernels with the images tc, or the FFMA kernels
+// (tc NULL) -- the scatter and the time-row gradients.  go[h] / gi[h]: gradient w.r.t. the outputs / inputs of head h's
+// residual tensor (xyz, scaling, rotation, opacity, shs).  relu_bits: the signs a tensor-core forward saved, or NULL.
+size_t deform_backward_scratch_bytes(const DeformDesc& d, int64_t n, bool tc);   // size of launch_deform_backward's scratch
+cudaError_t launch_deform_backward(const DeformDesc& d, const G4DDeformParams& prm, const G4DDeformGrads& grads, const TcBwdWeights* tc,
+                                   TimeArg time, int64_t n, const float* xyz, const float* const go[G4D_NUM_HEADS],
+                                   float* const gi[G4D_NUM_HEADS], const uint32_t* relu_bits, const float* saved_feat,
+                                   const uint32_t* order, void* scratch, int sm_count, cudaStream_t st);
 // ---- several cameras at one timestamp (g4d_render_forward_cameras / _backward_cameras) -----------------------------
 constexpr int kMaxExtraCameras = G4D_MAX_CAMERAS - 1;
 // cameras 1..k-1 of a multi-camera forward: camera c reads cam[c] and writes its own context's records g[c] and out_radii[c]

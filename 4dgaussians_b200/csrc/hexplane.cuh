@@ -3,8 +3,9 @@
 //
 // Planes are channel-last [H][W][C], so one bilinear tap of a channel vector (4 channels) is one float4; the three time planes
 // are collapsed once per view into 1-D rows (every Gaussian of a view shares t).  The functions take one level's entries of
-// DeformDesc (planes[l], trow[l], res[l]) and the taps of the normalised (x, y, z) at that level.  The forward sample is
-// explicit fmaf() and single multiplies only: it rounds the same in the -fmad=false translation units as in the others.
+// DeformDesc (planes[l], trow[l], res[l]) and the taps of the normalised (x, y, z) at that level.  The normalisation and the
+// forward sample are explicit roundings (__fmul_rn / __fadd_rn, fmaf()) and single multiplies only: they round the same in the
+// -fmad=false translation units as in the others, so a backward taps the very cells its forward sampled.
 #pragma once
 #include "g4d_common.cuh"
 
@@ -20,7 +21,8 @@ struct AabbNorm {
 #pragma unroll
         for (int a = 0; a < 3; ++a) { amax[a] = __ldg(aabb + a); scale[a] = 2.0f / (__ldg(aabb + 3 + a) - amax[a]); }
     }
-    G4D_D float operator()(int a, float x) const { return (x - amax[a]) * scale[a] - 1.0f; }
+    // (never contracted to an FMA: a coordinate one ulp off can fall into the neighbouring texel cell)
+    G4D_D float operator()(int a, float x) const { return __fadd_rn(__fmul_rn(x - amax[a], scale[a]), -1.0f); }
 };
 
 // grid_sample unnormalise (align_corners=True) + border clamp + floor (ATen grid_sampler_2d semantics).  gmul is the

@@ -171,6 +171,13 @@ def hidden_args(net: str):
         "c32w128": dict(channels=32, resolution=[10, 9, 8, 6], multires=[1, 2], net_width=128, no_do=False, no_dshs=True),
         # F = 64 with all five heads: the largest shared-memory layout of the tensor-core kernels
         "c32w128sh": dict(channels=32, resolution=[10, 9, 8, 6], multires=[1, 2], net_width=128, no_do=False, no_dshs=False),
+        # channel widths the tensor-core kernels do not take (FFMA network; the shared gather and scatter at C/4 = 1, 3, 5, 6)
+        # and the widest feature vector, F = 128 (at net_width 64 without the SH head: the FFMA kernel's shared memory)
+        "c4w64": dict(channels=4, resolution=[9, 8, 10, 5], multires=[1, 2], net_width=64, no_do=False, no_dshs=True),
+        "c12w128": dict(channels=12, resolution=[8, 10, 9, 6], multires=[1, 2, 4], net_width=128, no_do=False, no_dshs=False),
+        "c20w64": dict(channels=20, resolution=[10, 9, 8, 7], multires=[1, 2], net_width=64, no_do=True, no_dshs=False),
+        "c24w128": dict(channels=24, resolution=[9, 10, 8, 6], multires=[1, 2], net_width=128, no_do=False, no_dshs=True),
+        "f128w64": dict(channels=32, resolution=[6, 7, 5, 4], multires=[1, 2, 3, 4], net_width=64, no_do=False, no_dshs=True),
     }
     c = cfgs[net]
     return Namespace(net_width=c["net_width"], timebase_pe=4, defor_depth=1, posebase_pe=10, scale_rotation_pe=2, opacity_pe=2,

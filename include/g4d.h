@@ -272,7 +272,7 @@ enum { G4D_OPT_SYNC_MODE = 1,  /* 1 (default): size the instance buffer exactly 
        G4D_OPT_PDL = 9,          /* 1 (default): the kernels of a forward are launched programmatically dependent on one another
                                   *    (a kernel's set-up overlaps the tail of its predecessor; results unchanged); 0: ordinary
                                   *    stream order.  PROCESS-wide, not per workspace (also: environment G4D_PDL=0) */
-       G4D_OPT_GATHER_ORDER = 10 /* 1 (default): the tensor-core path gathers the HexPlane features of the Gaussians in a spatial
+       G4D_OPT_GATHER_ORDER = 10 /* 1 (default): every path gathers the HexPlane features of the Gaussians in a spatial
                                   *    (Z) order, built on the device when the xyz pointer or N changes and kept otherwise (results
                                   *    unchanged: every Gaussian's features come from its own taps); 0: index order.  Per workspace;
                                   *    a workspace created with G4D_GATHER_ORDER=0 in the environment starts at 0 */ };

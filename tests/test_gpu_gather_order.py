@@ -88,27 +88,27 @@ def test_order_is_a_permutation(ws, n):
     _assert_permutation(_read_order(ctx), n)
 
 
-def _outputs(out, ctx):
-    return [out["render"].detach(), out["depth"].detach(), out["radii"]] + [torch.from_numpy(ctx.read(b).copy()) for b in
-                                                                           ("features", "deformed", "deformed_shs", "sorted_ids")]
+def _outputs(out, ctx, features=True):
+    bufs = ("features", "deformed", "deformed_shs", "sorted_ids") if features else ("deformed", "sorted_ids")
+    return [out["render"].detach(), out["depth"].detach(), out["radii"]] + [torch.from_numpy(ctx.read(b).copy()) for b in bufs]
 
 
-@pytest.mark.gpu
-def test_full_size_C3_same_bits_in_either_order(ws):
-    w = synth.WORKLOADS["C3"]
-    _, _, pc = _model(w["n"], seed=0, grad=True, scale=w["scale_mean"])
+def _same_bits_in_either_order(ws, workload):
+    w = synth.WORKLOADS[workload]
+    _, _, pc = _model(w["n"], seed=0, net=w["net"], grad=True, scale=w["scale_mean"])
     cams = synth.orbit_cameras(2, w["width"], w["height"], radius=w["radius"], focal=w["focal"])
     for cam in cams:
         cam.time = 0.35
+    tc = workload == "C3"
     res = {}
     for order in (1, 0, 1):
         out = _render(pc, cams[0], ws, order, grad=True)
-        res.setdefault(order, []).append(_outputs(out, out["render"].grad_fn.lease.ctx))
+        res.setdefault(order, []).append(_outputs(out, out["render"].grad_fn.lease.ctx, features=tc))
         del out
-    assert len(res[1][0]) == len(res[0][0]) == 7
+    assert len(res[1][0]) == len(res[0][0]) == (7 if tc else 5)
     for got in (res[1][0], res[1][1]):
         for i, (a, b) in enumerate(zip(got, res[0][0])):
-            assert torch.equal(a, b), i
+            assert torch.equal(a, b), (workload, i)
     assert int((res[0][0][2] > 0).sum()) > 1000
     # render_cameras, k = 2: deformed once, both cameras from the same features
     multi = {}
@@ -118,7 +118,14 @@ def test_full_size_C3_same_bits_in_either_order(ws):
             outs = g4d.render_cameras(cams, pc, _Pipe, torch.zeros(3, device="cuda"))
         multi[order] = [(o["render"].clone(), o["depth"].clone(), o["radii"].clone()) for o in outs]
     for a, b in zip(multi[1], multi[0]):
-        assert all(torch.equal(x, y) for x, y in zip(a, b))
+        assert all(torch.equal(x, y) for x, y in zip(a, b)), workload
+
+
+@pytest.mark.gpu
+def test_full_size_C3_same_bits_in_either_order(ws):
+    """C3 (the tensor-core network), then an FFMA arm at C1 size (dnerf net, net_width 64), which keeps no features."""
+    _same_bits_in_either_order(ws, "C3")
+    _same_bits_in_either_order(ws, "C1")
 
 
 @pytest.mark.gpu

@@ -214,7 +214,9 @@ def _deform_inputs(n, seed, dev="cuda"):
     return [t.to(dev) for t in (xyz, sc, rot, op, shs)], probes
 
 
-@pytest.mark.parametrize("net,n", [("small64", 1000), ("small128", 517), ("dnerf", 4099), ("hypernerf", 2050), ("dynerf", 3001)])
+@pytest.mark.parametrize("net,n", [("small64", 1000), ("small128", 517), ("dnerf", 4099), ("hypernerf", 2050), ("dynerf", 3001),
+                                   ("c4w64", 1), ("c4w64", 777), ("c12w128", 301), ("c20w64", 1), ("c20w64", 389),
+                                   ("c24w128", 643), ("f128w64", 1), ("f128w64", 259)])
 @pytest.mark.parametrize("t", [0.0, 0.37, 1.0])
 def test_deform_forward_vs_oracle(net, n, t):
     mod = make_module(net, seed=3)
@@ -252,7 +254,8 @@ def test_deform_forward_vs_reference_golden(name):
 
 
 @pytest.mark.parametrize("net,n", [("small64", 700), ("small128", 517), ("small128", 300), ("dynerf", 1500), ("dnerf", 1300),
-                                   ("hypernerf", 2050)])
+                                   ("hypernerf", 2050), ("c4w64", 1), ("c4w64", 777), ("c12w128", 1), ("c12w128", 301),
+                                   ("c20w64", 389), ("c24w128", 1), ("c24w128", 643), ("f128w64", 259)])
 def test_deform_backward_vs_oracle(net, n):
     t = 0.61
     mod = make_module(net, seed=4)
