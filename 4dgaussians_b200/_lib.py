@@ -18,6 +18,7 @@ LIB_PATH = os.path.join(HERE, "libg4d.so")
 
 MAX_LEVELS = 4
 NUM_HEADS = 5
+MAX_DEPTH = 8                      # G4D_MAX_DEPTH: defor_depth of the deformation network's trunk
 HEAD_POS, HEAD_SCALES, HEAD_ROT, HEAD_OPACITY, HEAD_SHS = 1, 2, 4, 8, 16
 
 OPT_SYNC_MODE, OPT_INSTANCE_CAPACITY, OPT_TIGHT_CULL, OPT_STAGE_TIMING, OPT_TENSOR_CORES, OPT_TC_DEBUG, OPT_WARP_CULL = 1, 2, 3, 4, 5, 6, 7
@@ -65,12 +66,13 @@ class DeformParams(C.Structure):
     _fields_ = [("levels", C.c_int32), ("channels", C.c_int32), ("net_width", C.c_int32), ("head_mask", C.c_int32),
                 ("res", (C.c_int32 * 4) * MAX_LEVELS), ("planes", (fp * 6) * MAX_LEVELS), ("aabb", fp),
                 ("w0", fp), ("b0", fp), ("w1", fp * NUM_HEADS), ("b1", fp * NUM_HEADS), ("w2", fp * NUM_HEADS),
-                ("b2", fp * NUM_HEADS), ("version", C.c_uint64)]
+                ("b2", fp * NUM_HEADS), ("version", C.c_uint64),
+                ("depth", C.c_int32), ("reserved", C.c_int32), ("wt", fp * (MAX_DEPTH - 1)), ("bt", fp * (MAX_DEPTH - 1))]
 
 
 class DeformGrads(C.Structure):
     _fields_ = [("planes", (fp * 6) * MAX_LEVELS), ("w0", fp), ("b0", fp), ("w1", fp * NUM_HEADS), ("b1", fp * NUM_HEADS),
-                ("w2", fp * NUM_HEADS), ("b2", fp * NUM_HEADS)]
+                ("w2", fp * NUM_HEADS), ("b2", fp * NUM_HEADS), ("wt", fp * (MAX_DEPTH - 1)), ("bt", fp * (MAX_DEPTH - 1))]
 
 
 class Gaussians(C.Structure):

@@ -3,14 +3,16 @@
 // Algorithm (verified spec: SURVEY.md Appendix B):
 //   /root/reference/scene/hexplane.py:19-20,73-106,160-183   normalize_aabb, 6-plane bilinear product, level concat
 //   /root/reference/scene/deformation.py:67-83               hidden = Linear(F->Wd)(feat)      (no activation)
+//   /root/reference/scene/deformation.py:55-60               defor_depth D > 1: hidden = W_j relu(hidden) + b_j, j < D
 //   /root/reference/scene/deformation.py:97-148              heads ReLU-Linear-ReLU-Linear, residual add
 //
 // Layout decisions (DESIGN.md §3):
 //   * the HexPlane features arrive gathered, feat [N][F] (deform_features_kernel, the gather of every path); a tile of
 //     them is loaded into a0;
 //   * a CTA of 256 threads owns TG Gaussians; activations live in shared memory row-major [TG][K+4];
-//     W0^T and one head's W1^T are staged in shared memory ([K][Wd], W1^T by a TMA bulk copy that overlaps
-//     the previous head's epilogue); each thread accumulates an RM x (Wd/16) register tile with FFMA.
+//     W0^T and one W x W image are staged in shared memory ([K][Wd]); the W x W slot takes each trunk layer's W_j^T and
+//     then each head's W1^T by a TMA bulk copy that overlaps the previous GEMM's epilogue; each thread accumulates an
+//     RM x (Wd/16) register tile with FFMA.
 #pragma once
 #include "g4d_common.cuh"
 #include "hexplane.cuh"
@@ -31,16 +33,19 @@ struct DeformDesc {
     const float* b1[G4D_NUM_HEADS];
     const float* w2[G4D_NUM_HEADS];           // torch layout [k][WD]
     const float* b2[G4D_NUM_HEADS];
+    int ntrunk;                               // trunk layers behind W0: max(defor_depth, 1) - 1
+    const float* wtt[G4D_MAX_DEPTH - 1];      // packed [WD][WD]: W_j^T of trunk layer j = 1 .. ntrunk
+    const float* bt[G4D_MAX_DEPTH - 1];       // [WD]
 };
 
 // shared-memory carve-up (offsets in floats), computed on the host by deform_smem_layout()
 struct DeformSmem {
-    int w0t, b0, w1t, b1, w2, b2, a0, a1, a2, out, in, mbar, total_floats;
+    int w0t, b0, w1t, b1, bt, w2, b2, a0, a1, a2, out, in, mbar, total_floats;
     int lda0, lda1, w2_stride;
     int w2_off[G4D_NUM_HEADS];   // row offset (in rows of w2_stride floats) of head h inside w2
 };
 
-inline DeformSmem deform_smem_layout(int TG, int F, int WD, int head_mask) {
+inline DeformSmem deform_smem_layout(int TG, int F, int WD, int head_mask, int ntrunk) {
     DeformSmem s{};
     int off = 0;
     auto take = [&](int n) { int o = off; off += (n + 3) & ~3; return o; };
@@ -49,6 +54,7 @@ inline DeformSmem deform_smem_layout(int TG, int F, int WD, int head_mask) {
     s.b0 = take(WD);
     s.w1t = take(WD * WD);
     s.b1 = take(G4D_NUM_HEADS * WD);
+    s.bt = take(ntrunk * WD);
     int rows = 0;
     for (int h = 0; h < G4D_NUM_HEADS; ++h) { s.w2_off[h] = rows; if (head_mask & (1 << h)) rows += head_out(h); }
     s.w2 = take(rows * s.w2_stride);
@@ -184,12 +190,30 @@ G4D_D void head_output(const float* __restrict__ A2, int lda, const float* __res
     }
 }
 
+// The W x W images one tile streams through the slot at L.w1t, in order: the trunk layers' W_j^T, then the active heads' W1^T.
+G4D_D int wslot_images(const DeformDesc& d) { return d.ntrunk + __popc((unsigned)d.head_mask & ((1u << G4D_NUM_HEADS) - 1)); }
+G4D_D const float* wslot_image(const DeformDesc& d, int i) {
+    if (i < d.ntrunk) return d.wtt[i];
+    i -= d.ntrunk;
+    for (int h = 0; h < G4D_NUM_HEADS; ++h)
+        if (d.head_mask & (1 << h)) { if (i == 0) return d.w1t[h]; --i; }
+    return nullptr;
+}
+// thread 0: the bulk copy of image i of the tile's list into the slot
+template <int WD>
+G4D_D void wslot_issue(const DeformDesc& d, const DeformSmem& L, float* smem, int i) {
+    mbar_expect_tx(smem + L.mbar, (uint32_t)(WD * WD * sizeof(float)));
+    tma_bulk_g2s(smem + L.w1t, wslot_image(d, i), (uint32_t)(WD * WD * sizeof(float)), smem + L.mbar);
+}
+
 // Per-CTA one-time staging of the persistent weights (W0^T, biases, W2 of the active heads).
 G4D_D void stage_persistent_weights(const DeformDesc& d, const DeformSmem& L, float* smem) {
     const int n0 = d.F * d.WD;
     for (int i = threadIdx.x * 4; i < n0; i += kDeformThreads * 4)
         *reinterpret_cast<float4*>(smem + L.w0t + i) = __ldg(reinterpret_cast<const float4*>(d.w0t + i));
     for (int i = threadIdx.x; i < d.WD; i += kDeformThreads) smem[L.b0 + i] = __ldg(d.b0 + i);
+    for (int j = 0; j < d.ntrunk; ++j)
+        for (int i = threadIdx.x; i < d.WD; i += kDeformThreads) smem[L.bt + j * d.WD + i] = __ldg(d.bt[j] + i);
     for (int h = 0; h < G4D_NUM_HEADS; ++h) {
         if (!(d.head_mask & (1 << h))) continue;
         for (int i = threadIdx.x; i < d.WD; i += kDeformThreads) smem[L.b1 + h * d.WD + i] = __ldg(d.b1[h] + i);
@@ -216,28 +240,51 @@ G4D_D void load_feature_tile(const float* __restrict__ feat, int F, int64_t base
 
 // Runs the whole network for the TG Gaussians whose features are in smem[L.a0] (load_feature_tile).
 // On return smem[L.out + g*60 + head_col(h) + o] holds the delta of every ACTIVE head (inactive: untouched).
-// `phase` is the running mbarrier parity for the W1 staging buffer (caller keeps it across tiles).
-// PRE: thread 0 has already issued the bulk copy of the FIRST active head's W1^T for this tile.
+// `phase` is the running mbarrier parity for the W x W staging slot (caller keeps it across tiles).
+// PRE: thread 0 has already issued the bulk copy of image 0 of the tile's list (wslot_image): the first trunk layer's W_j^T,
+// or with no trunk layer the first active head's W1^T.  Each image's GEMM issues the next one of the list -- past the last,
+// image 0 again when prefetch_next_tile -- so the next copy overlaps the epilogue.
 template <int TG, int WD>
 G4D_D void deform_mlp_tile(const DeformDesc& d, const DeformSmem& L, float* smem, uint32_t& phase, bool prefetch_next_tile) {
     constexpr int RM = TG / 16, CG = WD / 64;
     const int ty = threadIdx.x >> 4, tx = threadIdx.x & 15;
     void* bar = smem + L.mbar;
+    const int nimg = wslot_images(d);
+    auto prefetch_after = [&](int i) {   // thread 0, once everyone is done reading image i
+        if (i + 1 < nimg) wslot_issue<WD>(d, L, smem, i + 1);
+        else if (prefetch_next_tile) wslot_issue<WD>(d, L, smem, 0);
+    };
+    // the trunk ping-pongs between a1 and a2 and ends in a1, where the heads read relu(h_{D-1})
+    float* cur = smem + ((d.ntrunk & 1) ? L.a2 : L.a1);
 
-    {   // hidden = feat W0^T + b0 ; a1 = relu(hidden)  (every head starts with ReLU: deformation.py:61-65)
+    {   // hidden = feat W0^T + b0 ; relu(hidden)  (every head and trunk layer starts with ReLU: deformation.py:55-65)
         float acc[RM][CG * 4];
 #pragma unroll
         for (int r = 0; r < RM; ++r)
 #pragma unroll
             for (int c = 0; c < CG * 4; ++c) acc[r][c] = 0.f;
         tile_gemm<RM, CG>(smem + L.a0, L.lda0, smem + L.w0t, WD, d.F, ty, tx, acc);
-        tile_store<RM, CG, true>(smem + L.a1, L.lda1, smem + L.b0, ty, tx, acc);
+        tile_store<RM, CG, true>(cur, L.lda1, smem + L.b0, ty, tx, acc);
     }
     __syncthreads();
-    int first = -1;
-    for (int h = G4D_NUM_HEADS - 1; h >= 0; --h)
-        if (d.head_mask & (1 << h)) first = h;
-    for (int h = 0; h < G4D_NUM_HEADS; ++h) {
+#pragma unroll 1
+    for (int j = 0; j < d.ntrunk; ++j) {   // hidden = relu(hidden) W_j^T + b_j
+        float* nxt = smem + (cur == smem + L.a1 ? L.a2 : L.a1);
+        mbar_wait(bar, phase);   // W_j^T has landed
+        phase ^= 1u;
+        float acc[RM][CG * 4];
+#pragma unroll
+        for (int r = 0; r < RM; ++r)
+#pragma unroll
+            for (int c = 0; c < CG * 4; ++c) acc[r][c] = 0.f;
+        tile_gemm<RM, CG>(cur, L.lda1, smem + L.w1t, WD, WD, ty, tx, acc);
+        __syncthreads();   // everyone is done reading W_j^T and cur
+        if (threadIdx.x == 0) prefetch_after(j);
+        tile_store<RM, CG, true>(nxt, L.lda1, smem + L.bt + j * WD, ty, tx, acc);
+        __syncthreads();
+        cur = nxt;
+    }
+    for (int h = 0, img = d.ntrunk; h < G4D_NUM_HEADS; ++h) {
         if (!(d.head_mask & (1 << h))) continue;
         mbar_wait(bar, phase);   // W1^T of head h has landed
         phase ^= 1u;
@@ -249,16 +296,8 @@ G4D_D void deform_mlp_tile(const DeformDesc& d, const DeformSmem& L, float* smem
                 for (int c = 0; c < CG * 4; ++c) acc[r][c] = 0.f;
             tile_gemm<RM, CG>(smem + L.a1, L.lda1, smem + L.w1t, WD, WD, ty, tx, acc);
             __syncthreads();   // everyone is done reading W1^T (and the previous head's a2)
-            if (threadIdx.x == 0) {   // overlap the next W1^T fetch with this head's epilogue
-                int nh = -1;
-                for (int h2 = h + 1; h2 < G4D_NUM_HEADS; ++h2)
-                    if (d.head_mask & (1 << h2)) { nh = h2; break; }
-                if (nh < 0 && prefetch_next_tile) nh = first;
-                if (nh >= 0) {
-                    mbar_expect_tx(bar, (uint32_t)(WD * WD * sizeof(float)));
-                    tma_bulk_g2s(smem + L.w1t, d.w1t[nh], (uint32_t)(WD * WD * sizeof(float)), bar);
-                }
-            }
+            if (threadIdx.x == 0) prefetch_after(img);   // overlap the next image's fetch with this head's epilogue
+            ++img;
             tile_store<RM, CG, true>(smem + L.a2, L.lda1, smem + L.b1 + h * WD, ty, tx, acc);
         }
         __syncthreads();

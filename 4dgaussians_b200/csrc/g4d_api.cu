@@ -81,10 +81,11 @@ template <class Layout> cudaError_t ensure_layout(DevBuf& buf, Layout layout) {
     return cudaSuccess;
 }
 
-// FP32 transposes of W0 and of the active heads' W1 (the FFMA kernels' operands)
+// FP32 transposes of W0, of the active heads' W1 and of the trunk layers' W_j (the FFMA kernels' operands)
 struct FfmaWeights {
     float* w0t;
     float* w1t[G4D_NUM_HEADS];
+    float* wtt[G4D_MAX_DEPTH - 1];
 };
 
 // weight images derived from the caller's parameters, rebuilt when G4DDeformParams.version or the w0 pointer changes (or,
@@ -321,6 +322,9 @@ int check_params(const G4DDeformParams* p) {
     if (p->channels < 4 || p->channels > 32 || (p->channels & 3)) return fail(G4D_ERR_ARG, "channels must be a multiple of 4, <= 32");
     if (p->net_width != 64 && p->net_width != 128) return fail(G4D_ERR_ARG, "net_width must be 64 or 128");
     if (p->levels * p->channels > 128) return fail(G4D_ERR_ARG, "levels*channels must be <= 128");
+    if (p->depth < 0 || p->depth > G4D_MAX_DEPTH) return fail(G4D_ERR_ARG, "depth (defor_depth) must be in 0..G4D_MAX_DEPTH (8)");
+    for (int j = 1; j < p->depth; ++j)
+        if (!p->wt[j - 1] || !p->bt[j - 1]) return fail(G4D_ERR_ARG, "trunk layer weight or bias (wt / bt) is NULL for a layer below depth");
     for (int l = 0; l < p->levels; ++l)
         for (int a = 0; a < 4; ++a)
             if (p->res[l][a] < 2 || p->res[l][a] > 65535) return fail(G4D_ERR_ARG, "plane resolution out of range");
@@ -329,12 +333,14 @@ int check_params(const G4DDeformParams* p) {
 
 int refresh_packed(G4DWorkspace* ws, const G4DDeformParams* p, cudaStream_t st) {
     const size_t F = (size_t)p->levels * p->channels, WD = (size_t)p->net_width;
+    const size_t ntrunk = p->depth > 1 ? (size_t)p->depth - 1 : 0;
     auto pack = [&](void* blob, FfmaWeights* w) {
         w->w0t = static_cast<float*>(blob);
         for (int h = 0; h < G4D_NUM_HEADS; ++h) w->w1t[h] = w->w0t + F * WD + h * WD * WD;
-        return launch_pack_weights(*p, w->w0t, w->w1t, st);
+        for (size_t j = 0; j < G4D_MAX_DEPTH - 1; ++j) w->wtt[j] = j < ntrunk ? w->w0t + F * WD + (G4D_NUM_HEADS + j) * WD * WD : nullptr;
+        return launch_pack_weights(*p, w->w0t, w->w1t, w->wtt, st);
     };
-    G4D_CUDA(ws->packed.refresh(p, 0, (F * WD + G4D_NUM_HEADS * WD * WD) * 4, pack));
+    G4D_CUDA(ws->packed.refresh(p, 0, (F * WD + (G4D_NUM_HEADS + ntrunk) * WD * WD) * 4, pack));
     return G4D_OK;
 }
 
@@ -368,6 +374,8 @@ DeformDesc make_desc(const G4DDeformParams* p, float* const (*trow)[3], const Ff
     for (int h = 0; h < G4D_NUM_HEADS; ++h) {
         d.w1t[h] = w ? w->w1t[h] : nullptr; d.b1[h] = p->b1[h]; d.w2[h] = p->w2[h]; d.b2[h] = p->b2[h];
     }
+    d.ntrunk = p->depth > 1 ? p->depth - 1 : 0;
+    for (int j = 0; j < d.ntrunk; ++j) { d.wtt[j] = w ? w->wtt[j] : nullptr; d.bt[j] = p->bt[j]; }
     return d;
 }
 

@@ -158,25 +158,34 @@ cudaError_t launch_preprocess_backward_cameras(const BackwardCameras& bc, int64_
 //
 //   gather:   the forward's HexPlane gather, deform_features_kernel -> FEAT [N][F] (skipped when the forward kept its features)
 //   engine:   d(feat) -> DFEAT [N][F] and the network's weight gradients, either
-//             FFMA, three persistent kernels:
-//               P  "prepass":  a1 = relu(feat W0^T + b0) for every Gaussian -> A1 [N][Wd] in HBM.
+//             FFMA, persistent kernels:
+//               P  "prepass":  a_0 = relu(feat W0^T + b0) for every Gaussian -> A[0] [N][Wd] in HBM; with a trunk
+//                              (defor_depth D >= 2) launched once more per trunk layer j = 1 .. D-1: a_j = relu(a_{j-1} W_j^T
+//                              + b_j) -> A[j], with the forward's tile_gemm order (the ReLU signs are recomputed, so only the
+//                              forward's arithmetic makes the gradient the gradient of the forward that ran).  A1 = A[D-1].
 //               H  "heads":    CTA c owns ONE head (c mod #active) for its whole life: W1 (torch layout, padded) and W2 stay in
 //                              shared memory, dW1 / dW2 / db accumulate in REGISTERS across all the CTA's tiles and are
 //                              flushed once with atomics; per tile it recomputes z, a2, forms dz and writes da1_h = dz W1
 //                              -> DA1[h] in HBM.
-//               Q  "final":    dh = (sum_h DA1[h]) * (a1 > 0); dW0, db0 in registers; dfeat = dh W0 -> DFEAT.
+//               T  "trunk":    D >= 2 only, once per trunk layer j = D-1 .. 1: dz_j = dA_j * (a_j > 0) with dA_{D-1} =
+//                              sum_h DA1[h]; dW_j, db_j in registers; dA_{j-1} = dz_j W_j -> a ping-pong pair of [N][Wd].
+//               Q  "final":    dh = dA_0 * (a_0 > 0), dA_0 = sum_h DA1[h] when D <= 1; dW0, db0 in registers;
+//                              dfeat = dh W0 -> DFEAT.
 //             or tensor-core, kernels A (dgrad, -> DFEAT) and B (wgrad), g4d_deform_tc_bwd.cu, with the scatter between them.
 //   scatter:  bwd_scatter_kernel: DFEAT into the planes (vector RED; time planes through the collapsed rows), d(xyz) through
 //             the bilinear coordinates, residual-path input gradients.
 //   T         distributes the collapsed time-row gradients onto the two time rows of each time plane.
 // ======================================================================================================
 
-// The scratch of a backward: the engine's own -- the FFMA kernels' A1 and DA1 of every active head, or the tensor-core
-// kernels' operand images -- then the features and their gradient and the time-row gradients (both engines).
+// The scratch of a backward: the engine's own -- the FFMA kernels' activations and DA1 of every active head (and with a trunk
+// its dA ping-pong pair), or the tensor-core kernels' operand images -- then the features and their gradient and the time-row
+// gradients (both engines).
 struct DeformBwdBuffers {
     const float* feat;                // [N][F]: the gather's, or the features the forward kept
-    float* a1;                        // FFMA: [N][WD]
+    float* a1;                        // FFMA: [N][WD] relu(h_{D-1}), the heads' input (= act[ntrunk])
+    float* act[G4D_MAX_DEPTH];        // FFMA: [N][WD] a_j = relu(h_j), j = 0 .. ntrunk
     float* da1[G4D_NUM_HEADS];        // FFMA: [N][WD] per active head
+    float* dact[2];                   // FFMA with a trunk: [N][WD] dA_j ping-pong
     float* dfeat;                     // [N][F]
     float* trow_grad[G4D_MAX_LEVELS][3];
     uint8_t* images;                  // tensor-core: tc_bwd_images_bytes
@@ -187,6 +196,8 @@ struct DeformBwdDesc {
     DeformDesc d;
     const float* w0;                  // torch layout [WD][F]
     const float* w1[G4D_NUM_HEADS];   // torch layout [WD][WD]
+    const float* wt[G4D_MAX_DEPTH - 1];   // trunk, torch layout [WD][WD]
+    float* g_wt[G4D_MAX_DEPTH - 1]; float* g_bt[G4D_MAX_DEPTH - 1];
     float* g_w0; float* g_b0;
     float* g_w1[G4D_NUM_HEADS]; float* g_b1[G4D_NUM_HEADS];
     float* g_w2[G4D_NUM_HEADS]; float* g_b2[G4D_NUM_HEADS];
@@ -221,27 +232,42 @@ G4D_D void tile_gemm_nt(const float* __restrict__ A, int lda, const float* __res
 }
 
 // ---- kernel P ------------------------------------------------------------------------------------------
+inline DeformSmem prepass_smem_layout(int TG, int K, int WD) {
+    DeformSmem s{};
+    int off = 0;
+    auto take = [&](int n) { int o = off; off += (n + 3) & ~3; return o; };
+    s.lda0 = K + 4;
+    s.w0t = take(K * WD);
+    s.b0 = take(WD);
+    s.a0 = take(TG * s.lda0);
+    s.total_floats = off;
+    return s;
+}
+
+// out = relu(in wt + bias) for one layer: in [N][K] (the features, K = F; or a trunk layer's input a_{j-1}, K = WD), wt the
+// packed transpose [K][WD], staged at L.w0t, the bias at L.b0, the input tile at L.a0 (prepass_smem_layout).
 template <int TG, int WD>
 __global__ void __launch_bounds__(kDeformThreads, 1)
-deform_bwd_prepass_kernel(DeformDesc d, DeformSmem L, int64_t n, const float* __restrict__ feat, float* __restrict__ a1_out) {
+deform_bwd_prepass_kernel(DeformSmem L, int64_t n, int K, const float* __restrict__ in, const float* __restrict__ wt,
+                          const float* __restrict__ bias, float* __restrict__ a1_out) {
     extern __shared__ __align__(16) float smem[];
     constexpr int RM = TG / 16, CG = WD / 64;
     const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
     const int64_t ntiles = (n + TG - 1) / TG;
-    const int n0 = d.F * WD;
+    const int n0 = K * WD;
     for (int i = tid * 4; i < n0; i += kDeformThreads * 4)
-        *reinterpret_cast<float4*>(smem + L.w0t + i) = __ldg(reinterpret_cast<const float4*>(d.w0t + i));
-    for (int i = tid; i < WD; i += kDeformThreads) smem[L.b0 + i] = __ldg(d.b0 + i);
+        *reinterpret_cast<float4*>(smem + L.w0t + i) = __ldg(reinterpret_cast<const float4*>(wt + i));
+    for (int i = tid; i < WD; i += kDeformThreads) smem[L.b0 + i] = __ldg(bias + i);
     for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const int64_t base = tile * TG, rem = n - base;
-        load_feature_tile<TG>(feat, d.F, base, rem, smem + L.a0, L.lda0);
+        load_feature_tile<TG>(in, K, base, rem, smem + L.a0, L.lda0);
         __syncthreads();
         float acc[RM][CG * 4];
 #pragma unroll
         for (int r = 0; r < RM; ++r)
 #pragma unroll
             for (int c = 0; c < CG * 4; ++c) acc[r][c] = 0.f;
-        tile_gemm<RM, CG>(smem + L.a0, L.lda0, smem + L.w0t, WD, d.F, ty, tx, acc);
+        tile_gemm<RM, CG>(smem + L.a0, L.lda0, smem + L.w0t, WD, K, ty, tx, acc);
 #pragma unroll
         for (int c = 0; c < CG; ++c) {
             const float4 bv = *reinterpret_cast<const float4*>(smem + L.b0 + c * 64 + tx * 4);
@@ -443,6 +469,130 @@ deform_bwd_heads_kernel(DeformBwdDesc bd, HeadSmem L, int64_t n, int num_active,
     else if (tid - WD < kout) atomicAdd(bd.g_b2[h] + (tid - WD), gB2);
 }
 
+// dst[g][0 .. WD) = dA[g] * (act[g] > 0) for the tile's rows g < rem, zero for the rows past n; dA is in [N][WD], or, when
+// in == NULL, the sum of the active heads' DA1.  The caller syncs.
+template <int TG, int WD>
+G4D_D void load_masked_grad(const DeformDesc& d, const DeformBwdBuffers& buf, const float* __restrict__ in,
+                            const float* __restrict__ act, int64_t base, int64_t rem, float* __restrict__ dst, int ld) {
+    for (int i = threadIdx.x; i < TG * (WD >> 2); i += kDeformThreads) {
+        const int g = i / (WD >> 2), v = i - g * (WD >> 2);
+        float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (g < rem) {
+            if (in) {
+                s = *reinterpret_cast<const float4*>(in + (base + g) * WD + 4 * v);
+            } else {
+                for (int h = 0; h < G4D_NUM_HEADS; ++h) {
+                    if (!(d.head_mask & (1 << h))) continue;
+                    const float4 t = *reinterpret_cast<const float4*>(buf.da1[h] + (base + g) * WD + 4 * v);
+                    s.x += t.x; s.y += t.y; s.z += t.z; s.w += t.w;
+                }
+            }
+            const float4 a = *reinterpret_cast<const float4*>(act + (base + g) * WD + 4 * v);
+            s.x = a.x > 0.f ? s.x : 0.f; s.y = a.y > 0.f ? s.y : 0.f;
+            s.z = a.z > 0.f ? s.z : 0.f; s.w = a.w > 0.f ? s.w : 0.f;
+        }
+        *reinterpret_cast<float4*>(dst + g * ld + 4 * v) = s;
+    }
+}
+
+// ---- kernel T ------------------------------------------------------------------------------------------
+// One trunk layer j (1 <= j <= ntrunk): dz = dA_j * (a_j > 0) with dA_j from `din` (NULL: the heads' DA1 sum, j = ntrunk);
+// dW_j += dz^T a_{j-1} and db_j += sum dz in registers, flushed once per CTA; dA_{j-1} = dz W_j -> dout.
+struct TrunkSmem { int w, a, dz, total_floats, ldw, lda; };
+
+inline TrunkSmem trunk_smem_layout(int TG, int WD) {
+    TrunkSmem s{};
+    int off = 0;
+    auto take = [&](int n) { int o = off; off += (n + 3) & ~3; return o; };
+    s.ldw = WD + 4; s.lda = WD + 4;
+    s.w = take(WD * s.ldw);
+    s.a = take(TG * s.lda);
+    s.dz = take(TG * s.lda);
+    s.total_floats = off;
+    return s;
+}
+
+template <int TG, int WD>
+__global__ void __launch_bounds__(kDeformThreads, 1)
+deform_bwd_trunk_kernel(DeformBwdDesc bd, TrunkSmem L, int64_t n, int j, DeformBwdBuffers buf, const float* __restrict__ din,
+                        float* __restrict__ dout) {
+    extern __shared__ __align__(16) float smem[];
+    constexpr int RM = TG / 16, CG = WD / 64, JR = WD / 16;
+    const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
+    float* sW = smem + L.w; float* sA = smem + L.a; float* sDZ = smem + L.dz;
+    const float* act_in = buf.act[j - 1];
+    for (int i = tid; i < WD * (WD >> 2); i += kDeformThreads) {   // W_j [o][i] in torch layout, rows padded to ldw
+        const int r = i / (WD >> 2), v = i - r * (WD >> 2);
+        *reinterpret_cast<float4*>(sW + r * L.ldw + 4 * v) = __ldg(reinterpret_cast<const float4*>(bd.wt[j - 1] + r * WD + 4 * v));
+    }
+    float gW[JR][CG * 4];
+#pragma unroll
+    for (int a = 0; a < JR; ++a)
+#pragma unroll
+        for (int b = 0; b < CG * 4; ++b) gW[a][b] = 0.f;
+    float gB = 0.f;
+    const int64_t ntiles = (n + TG - 1) / TG;
+    __syncthreads();
+
+    for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+        const int64_t base = tile * TG, rem = n - base;
+        load_feature_tile<TG>(act_in, WD, base, rem, sA, L.lda);
+        load_masked_grad<TG, WD>(bd.d, buf, din, buf.act[j], base, rem, sDZ, L.lda);
+        __syncthreads();
+        if (tid < WD) {
+            float s = 0.f;
+            for (int g = 0; g < TG; ++g) s += sDZ[g * L.lda + tid];
+            gB += s;
+        }
+        // dW_j[o][i] += sum_g dz[g][o] a_{j-1}[g][i];  thread (ty, tx): o = ty*JR + a, i = c*64 + tx*4 + b
+        for (int g = 0; g < TG; ++g) {
+            float dzv[JR];
+#pragma unroll
+            for (int a = 0; a < JR; a += 4) {
+                const float4 t4 = *reinterpret_cast<const float4*>(sDZ + g * L.lda + ty * JR + a);
+                dzv[a] = t4.x; dzv[a + 1] = t4.y; dzv[a + 2] = t4.z; dzv[a + 3] = t4.w;
+            }
+            float4 av[CG];
+#pragma unroll
+            for (int c = 0; c < CG; ++c) av[c] = *reinterpret_cast<const float4*>(sA + g * L.lda + c * 64 + tx * 4);
+#pragma unroll
+            for (int a = 0; a < JR; ++a)
+#pragma unroll
+                for (int c = 0; c < CG; ++c) {
+                    gW[a][c * 4 + 0] = fmaf(dzv[a], av[c].x, gW[a][c * 4 + 0]);
+                    gW[a][c * 4 + 1] = fmaf(dzv[a], av[c].y, gW[a][c * 4 + 1]);
+                    gW[a][c * 4 + 2] = fmaf(dzv[a], av[c].z, gW[a][c * 4 + 2]);
+                    gW[a][c * 4 + 3] = fmaf(dzv[a], av[c].w, gW[a][c * 4 + 3]);
+                }
+        }
+        {   // dA_{j-1} = dz W_j -> HBM
+            float acc[RM][CG * 4];
+#pragma unroll
+            for (int r = 0; r < RM; ++r)
+#pragma unroll
+                for (int c = 0; c < CG * 4; ++c) acc[r][c] = 0.f;
+            tile_gemm<RM, CG>(sDZ, L.lda, sW, L.ldw, WD, ty, tx, acc);
+#pragma unroll
+            for (int c = 0; c < CG; ++c)
+#pragma unroll
+                for (int r = 0; r < RM; ++r) {
+                    const int g = ty * RM + r;
+                    if (g < rem)
+                        *reinterpret_cast<float4*>(dout + (base + g) * WD + c * 64 + tx * 4) =
+                            make_float4(acc[r][c * 4 + 0], acc[r][c * 4 + 1], acc[r][c * 4 + 2], acc[r][c * 4 + 3]);
+                }
+        }
+        __syncthreads();
+    }
+#pragma unroll
+    for (int a = 0; a < JR; ++a)
+#pragma unroll
+        for (int c = 0; c < CG; ++c)
+#pragma unroll
+            for (int b = 0; b < 4; ++b) atomicAdd(bd.g_wt[j - 1] + (ty * JR + a) * WD + c * 64 + tx * 4 + b, gW[a][c * 4 + b]);
+    if (tid < WD) atomicAdd(bd.g_bt[j - 1] + tid, gB);
+}
+
 // ---- kernel Q ------------------------------------------------------------------------------------------
 struct FinalSmem { int w0, feat, dh, total_floats, ldw0, ldf, ldh; };
 
@@ -458,9 +608,10 @@ inline FinalSmem final_smem_layout(int TG, int F, int WD) {
     return s;
 }
 
+// din: dA_0 from the last T launch, or NULL (no trunk): the heads' DA1 sum
 template <int TG, int WD, int FM>
 __global__ void __launch_bounds__(kDeformThreads, 1)
-deform_bwd_final_kernel(DeformBwdDesc bd, FinalSmem L, int64_t n, DeformBwdBuffers buf) {
+deform_bwd_final_kernel(DeformBwdDesc bd, FinalSmem L, int64_t n, DeformBwdBuffers buf, const float* __restrict__ din) {
     extern __shared__ __align__(16) float smem[];
     const DeformDesc& d = bd.d;
     const int tid = threadIdx.x;
@@ -483,21 +634,7 @@ deform_bwd_final_kernel(DeformBwdDesc bd, FinalSmem L, int64_t n, DeformBwdBuffe
     for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const int64_t base = tile * TG, rem = n - base;
         load_feature_tile<TG>(buf.feat, F, base, rem, sF, L.ldf);
-        for (int i = tid; i < TG * (WD >> 2); i += kDeformThreads) {
-            const int g = i / (WD >> 2), v = i - g * (WD >> 2);
-            float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (g < rem) {
-                for (int h = 0; h < G4D_NUM_HEADS; ++h) {
-                    if (!(d.head_mask & (1 << h))) continue;
-                    const float4 t = *reinterpret_cast<const float4*>(buf.da1[h] + (base + g) * WD + 4 * v);
-                    s.x += t.x; s.y += t.y; s.z += t.z; s.w += t.w;
-                }
-                const float4 a1 = *reinterpret_cast<const float4*>(buf.a1 + (base + g) * WD + 4 * v);
-                s.x = a1.x > 0.f ? s.x : 0.f; s.y = a1.y > 0.f ? s.y : 0.f;
-                s.z = a1.z > 0.f ? s.z : 0.f; s.w = a1.w > 0.f ? s.w : 0.f;
-            }
-            *reinterpret_cast<float4*>(sDH + g * L.ldh + 4 * v) = s;
-        }
+        load_masked_grad<TG, WD>(d, buf, din, buf.act[0], base, rem, sDH, L.ldh);
         __syncthreads();
         // dW0[j][f] += sum_g dh[g][j] feat[g][f];  thread owns row j = w0_j and columns f = w0_g + NG*m
         for (int g = 0; g < TG; ++g) {
@@ -650,9 +787,13 @@ static DeformBwdBuffers carve_backward_scratch(Carve& m, const DeformDesc& d, in
     if (tc) {
         b.images = m.take<uint8_t>(tc_bwd_images_bytes(d, n));
     } else {
-        b.a1 = m.take<float>(N * d.WD);
+        b.a1 = b.act[d.ntrunk] = m.take<float>(N * d.WD);
         for (int h = 0; h < G4D_NUM_HEADS; ++h)
             if (d.head_mask & (1 << h)) b.da1[h] = m.take<float>(N * d.WD);
+        if (d.ntrunk > 0) {   // a_0 .. a_{D-2} and the dA pair: N * WD * 4 B each
+            for (int j = 0; j < d.ntrunk; ++j) b.act[j] = m.take<float>(N * d.WD);
+            for (int k = 0; k < 2; ++k) b.dact[k] = m.take<float>(N * d.WD);
+        }
     }
     const size_t rows128 = (N + 127) / 128 * 128;   // whole tiles of the tensor-core kernels
     b.feat = *gathered = m.take<float>(rows128 * d.F);
@@ -669,7 +810,7 @@ size_t deform_backward_scratch_bytes(const DeformDesc& d, int64_t n, bool tc) {
     return m.bytes();
 }
 
-// FFMA engine: P, H, Q
+// FFMA engine: P (once per layer up to a_{D-1}), H, T (once per trunk layer), Q
 template <int TG, int WD>
 static cudaError_t launch_ffma_engine(const DeformBwdDesc& bd, int64_t n, const DeformBwdBuffers& buf, int sm_count, cudaStream_t st) {
     const DeformDesc& d = bd.d;
@@ -679,12 +820,14 @@ static cudaError_t launch_ffma_engine(const DeformBwdDesc& bd, int64_t n, const 
     const int grid = (int)(ntiles < sm_count ? ntiles : sm_count);
     cudaError_t e;
     // P
-    {
-        const DeformSmem L = deform_smem_layout(TG, d.F, WD, 0);
+    for (int j = 0; j <= d.ntrunk; ++j) {
+        const int K = j == 0 ? d.F : WD;
+        const DeformSmem L = prepass_smem_layout(TG, K, WD);
         const size_t bytes = (size_t)L.total_floats * 4;
         e = cudaFuncSetAttribute(deform_bwd_prepass_kernel<TG, WD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
         if (e != cudaSuccess) return e;
-        deform_bwd_prepass_kernel<TG, WD><<<grid, kDeformThreads, bytes, st>>>(d, L, n, buf.feat, buf.a1);
+        if (j == 0) deform_bwd_prepass_kernel<TG, WD><<<grid, kDeformThreads, bytes, st>>>(L, n, K, buf.feat, d.w0t, d.b0, buf.act[0]);
+        else deform_bwd_prepass_kernel<TG, WD><<<grid, kDeformThreads, bytes, st>>>(L, n, K, buf.act[j - 1], d.wtt[j - 1], d.bt[j - 1], buf.act[j]);
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
     }
     // H
@@ -699,6 +842,19 @@ static cudaError_t launch_ffma_engine(const DeformBwdDesc& bd, int64_t n, const 
         deform_bwd_heads_kernel<TG, WD><<<hgrid, kDeformThreads, bytes, st>>>(bd, L, n, active, buf);
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
     }
+    // T: dA_{j-1} from dA_j, j = ntrunk .. 1 (dA_ntrunk: the heads' DA1 sum)
+    const float* din = nullptr;
+    if (d.ntrunk > 0) {
+        const TrunkSmem L = trunk_smem_layout(TG, WD);
+        const size_t bytes = (size_t)L.total_floats * 4;
+        e = cudaFuncSetAttribute(deform_bwd_trunk_kernel<TG, WD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+        if (e != cudaSuccess) return e;
+        for (int j = d.ntrunk, k = 0; j >= 1; --j, k ^= 1) {
+            deform_bwd_trunk_kernel<TG, WD><<<grid, kDeformThreads, bytes, st>>>(bd, L, n, j, buf, din, buf.dact[k]);
+            if ((e = cudaGetLastError()) != cudaSuccess) return e;
+            din = buf.dact[k];
+        }
+    }
     // Q
     const FinalSmem L = final_smem_layout(TG, d.F, WD);
     const size_t bytes = (size_t)L.total_floats * 4;
@@ -706,7 +862,7 @@ static cudaError_t launch_ffma_engine(const DeformBwdDesc& bd, int64_t n, const 
     do {                                                                                                                  \
         e = cudaFuncSetAttribute(deform_bwd_final_kernel<TG, WD, FM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes); \
         if (e != cudaSuccess) return e;                                                                                   \
-        deform_bwd_final_kernel<TG, WD, FM><<<grid, kDeformThreads, bytes, st>>>(bd, L, n, buf);                         \
+        deform_bwd_final_kernel<TG, WD, FM><<<grid, kDeformThreads, bytes, st>>>(bd, L, n, buf, din);                    \
     } while (0)
     if (d.F <= 32) G4D_LAUNCH_Q(32);
     else if (d.F <= 64) G4D_LAUNCH_Q(64);
@@ -732,6 +888,7 @@ cudaError_t launch_deform_backward(const DeformDesc& d, const G4DDeformParams& p
         bd.w1[h] = prm.w1[h]; bd.g_w1[h] = grads.w1[h]; bd.g_b1[h] = grads.b1[h]; bd.g_w2[h] = grads.w2[h]; bd.g_b2[h] = grads.b2[h];
         bd.go[h] = go[h]; bd.gi[h] = gi[h];
     }
+    for (int j = 0; j < d.ntrunk; ++j) { bd.wt[j] = prm.wt[j]; bd.g_wt[j] = grads.wt[j]; bd.g_bt[j] = grads.bt[j]; }
     BwdScatterDesc sc{};
     sc.d = d; sc.dfeat = buf.dfeat;
     for (int l = 0; l < d.levels; ++l) {

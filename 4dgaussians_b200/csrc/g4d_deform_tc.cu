@@ -612,7 +612,7 @@ cudaError_t launch_deform_features(const DeformDesc& d, int64_t n, const float* 
 
 bool tc_deform_supported(const G4DDeformParams& prm, int arith) {
     const int C = prm.channels, L = prm.levels;
-    if (prm.net_width != 128) return false;
+    if (prm.net_width != 128 || prm.depth > 1) return false;   // no trunk layers (deep trunks: the FFMA kernels)
     if (!((C == 16 && (L == 2 || L == 3)) || (C == 32 && L == 2))) return false;
     return tc_smem_layout(arith, C * L, (prm.head_mask & G4D_HEAD_SHS) != 0).total + kTcStaticSmem <= kMaxSmemPerBlock;
 }

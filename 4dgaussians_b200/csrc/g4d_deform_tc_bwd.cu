@@ -170,7 +170,7 @@ cudaError_t launch_tc_bwd_pack_weights(const G4DDeformParams& prm, uint8_t* blob
 
 bool tc_backward_supported(const G4DDeformParams& prm) {
     const int C = prm.channels, L = prm.levels;
-    if (prm.net_width != 128) return false;
+    if (prm.net_width != 128 || prm.depth > 1) return false;   // no trunk layers (deep trunks: the FFMA kernels)
     if (!((C == 16 && (L == 2 || L == 3)) || (C == 32 && L == 2))) return false;
     return bwd_smem_a(C * L, (prm.head_mask & G4D_HEAD_SHS) != 0).total + 1024 <= 227 * 1024;
 }

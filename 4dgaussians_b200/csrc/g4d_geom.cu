@@ -43,12 +43,13 @@ cudaError_t launch_pack_camera(const G4DCamera& cam, const float* d_time, Camera
 }
 
 // ------------------------------------------------------------------------------------------------------
+constexpr int kPackMax = 1 + G4D_NUM_HEADS + G4D_MAX_DEPTH - 1;   // W0, the heads' W1, the trunk's W_j
 struct PackDesc {
-    const float* src[1 + G4D_NUM_HEADS];
-    float* dst[1 + G4D_NUM_HEADS];
-    int rows[1 + G4D_NUM_HEADS];   // src is [rows][cols] (torch [out][in]); dst is [cols][rows]
-    int cols[1 + G4D_NUM_HEADS];
-    int start[2 + G4D_NUM_HEADS];  // prefix sums of element counts
+    const float* src[kPackMax];
+    float* dst[kPackMax];
+    int rows[kPackMax];            // src is [rows][cols] (torch [out][in]); dst is [cols][rows]
+    int cols[kPackMax];
+    int start[kPackMax + 1];       // prefix sums of element counts
     int count;
 };
 
@@ -62,7 +63,7 @@ __global__ void pack_weights_kernel(PackDesc p) {
     p.dst[m][e] = __ldg(p.src[m] + r * p.cols[m] + c);
 }
 
-cudaError_t launch_pack_weights(const G4DDeformParams& prm, float* w0t, float* const* w1t, cudaStream_t st) {
+cudaError_t launch_pack_weights(const G4DDeformParams& prm, float* w0t, float* const* w1t, float* const* wtt, cudaStream_t st) {
     PackDesc p{};
     const int F = prm.levels * prm.channels, WD = prm.net_width;
     int m = 0, total = 0;
@@ -70,6 +71,9 @@ cudaError_t launch_pack_weights(const G4DDeformParams& prm, float* w0t, float* c
     for (int h = 0; h < G4D_NUM_HEADS; ++h) {
         if (!(prm.head_mask & (1 << h))) continue;
         p.src[m] = prm.w1[h]; p.dst[m] = w1t[h]; p.rows[m] = WD; p.cols[m] = WD; p.start[m] = total; total += WD * WD; ++m;
+    }
+    for (int j = 1; j < prm.depth; ++j) {
+        p.src[m] = prm.wt[j - 1]; p.dst[m] = wtt[j - 1]; p.rows[m] = WD; p.cols[m] = WD; p.start[m] = total; total += WD * WD; ++m;
     }
     p.start[m] = total; p.count = m;
     pack_weights_kernel<<<(total + 255) / 256, 256, 0, st>>>(p);
@@ -207,13 +211,7 @@ deform_kernel(DeformDesc d, DeformSmem L, const CameraDev* __restrict__ camp, in
     void* bar = smem + L.mbar;
     if (tid == 0) { mbar_init(bar, 1); fence_barrier_init(); }
     __syncthreads();
-    int first = -1;
-    for (int h = G4D_NUM_HEADS - 1; h >= 0; --h)
-        if (d.head_mask & (1 << h)) first = h;
-    if (tid == 0 && first >= 0 && (int64_t)blockIdx.x < ntiles) {
-        mbar_expect_tx(bar, (uint32_t)(WD * WD * sizeof(float)));
-        tma_bulk_g2s(smem + L.w1t, d.w1t[first], (uint32_t)(WD * WD * sizeof(float)), bar);
-    }
+    if (tid == 0 && wslot_images(d) > 0 && (int64_t)blockIdx.x < ntiles) wslot_issue<WD>(d, L, smem, 0);   // deform_mlp_tile's PRE
     uint32_t phase = 0;
     float* in_xyz = smem + L.in;
     float* in_sc = in_xyz + TG * 3;
@@ -289,17 +287,34 @@ cudaError_t launch_deform_tc(const DeformDesc& d, const TcWeights& tw, int mode,
                              const DeformIO& io, int sm_count, cudaStream_t st);
 
 template <int TG, int WD, int MODE>
-static cudaError_t launch_deform_t(const DeformDesc& d, const CameraDev* cam, int64_t n, const float* feat, const DeformIO& io,
-                                   int sm_count, cudaStream_t st) {
-    const DeformSmem L = deform_smem_layout(TG, d.F, WD, d.head_mask);
-    const size_t bytes = (size_t)L.total_floats * sizeof(float);
-    if (bytes > 227 * 1024) return cudaErrorInvalidConfiguration;
+static cudaError_t launch_deform_t(const DeformDesc& d, const DeformSmem& L, size_t bytes, const CameraDev* cam, int64_t n,
+                                   const float* feat, const DeformIO& io, int sm_count, cudaStream_t st) {
     cudaError_t e = cudaFuncSetAttribute(deform_kernel<TG, WD, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
     if (e != cudaSuccess) return e;
     const int64_t ntiles = (n + TG - 1) / TG;
     const int grid = (int)(ntiles < sm_count ? ntiles : sm_count);
     deform_kernel<TG, WD, MODE><<<grid, kDeformThreads, bytes, st>>>(d, L, cam, n, feat, io);
     return cudaGetLastError();
+}
+
+// The FFMA network runs tiles of TG Gaussians when their shared memory (dynamic and static) fits in an SM, and of TG / 2
+// otherwise: wide features with the SH head, or those plus the trunk biases, at net_width 128 (every configuration the C-ABI
+// takes fits at TG / 2).  tile_gemm's sums run over K in the same order whatever the tile, so both tiles give the same bits.
+template <int TG, int WD, int MODE>
+static cudaError_t launch_deform_tiles(const DeformDesc& d, const CameraDev* cam, int64_t n, const float* feat, const DeformIO& io,
+                                       int sm_count, cudaStream_t st) {
+    constexpr size_t kMaxSmem = 227 * 1024;
+    const DeformSmem L = deform_smem_layout(TG, d.F, WD, d.head_mask, d.ntrunk);
+    const size_t bytes = (size_t)L.total_floats * sizeof(float);
+    cudaFuncAttributes a{};
+    cudaError_t e = cudaFuncGetAttributes(&a, deform_kernel<TG, WD, MODE>);
+    if (e != cudaSuccess) return e;
+    if (bytes + a.sharedSizeBytes <= kMaxSmem) return launch_deform_t<TG, WD, MODE>(d, L, bytes, cam, n, feat, io, sm_count, st);
+    const DeformSmem H = deform_smem_layout(TG / 2, d.F, WD, d.head_mask, d.ntrunk);
+    const size_t hbytes = (size_t)H.total_floats * sizeof(float);
+    if ((e = cudaFuncGetAttributes(&a, deform_kernel<TG / 2, WD, MODE>)) != cudaSuccess) return e;
+    if (hbytes + a.sharedSizeBytes > kMaxSmem) return cudaErrorInvalidConfiguration;
+    return launch_deform_t<TG / 2, WD, MODE>(d, H, hbytes, cam, n, feat, io, sm_count, st);
 }
 
 cudaError_t launch_deform(const DeformDesc& d, int mode, const CameraDev* cam, int64_t n, const DeformIO& io, const DeformGather& gather,
@@ -314,11 +329,11 @@ cudaError_t launch_deform(const DeformDesc& d, int mode, const CameraDev* cam, i
         return launch_deform_tc(d, t, mode, cam, n, io, sm_count, st);
     }
     if (d.WD == 128) {
-        return mode == 0 ? launch_deform_t<64, 128, 0>(d, cam, n, gather.feat, io, sm_count, st)
-                         : launch_deform_t<64, 128, 1>(d, cam, n, gather.feat, io, sm_count, st);
+        return mode == 0 ? launch_deform_tiles<64, 128, 0>(d, cam, n, gather.feat, io, sm_count, st)
+                         : launch_deform_tiles<64, 128, 1>(d, cam, n, gather.feat, io, sm_count, st);
     } else if (d.WD == 64) {
-        return mode == 0 ? launch_deform_t<128, 64, 0>(d, cam, n, gather.feat, io, sm_count, st)
-                         : launch_deform_t<128, 64, 1>(d, cam, n, gather.feat, io, sm_count, st);
+        return mode == 0 ? launch_deform_tiles<128, 64, 0>(d, cam, n, gather.feat, io, sm_count, st)
+                         : launch_deform_tiles<128, 64, 1>(d, cam, n, gather.feat, io, sm_count, st);
     }
     return cudaErrorInvalidValue;
 }

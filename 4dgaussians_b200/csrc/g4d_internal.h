@@ -257,7 +257,7 @@ cudaError_t launch_tc_bwd_wgrad(const DeformDesc& d, const G4DDeformGrads& grads
 // ---- launchers (defined in g4d_geom.cu / g4d_raster.cu / g4d_backward.cu) -----------------------------
 // d_time: the camera's timestamp from device memory (NULL: cam.time)
 cudaError_t launch_pack_camera(const G4DCamera& cam, const float* d_time, CameraDev* dst, cudaStream_t st);
-cudaError_t launch_pack_weights(const G4DDeformParams& p, float* w0t, float* const* w1t, cudaStream_t st);
+cudaError_t launch_pack_weights(const G4DDeformParams& p, float* w0t, float* const* w1t, float* const* wtt, cudaStream_t st);
 cudaError_t launch_collapse_time_rows(const G4DDeformParams& p, TimeArg time, float* const (*trow)[3], cudaStream_t st);
 cudaError_t launch_preprocess(const CameraDev* cam, int64_t n, const RasterInputs& in, GeomBuffers g, int32_t* out_radii,
                               cudaStream_t st);

@@ -69,7 +69,9 @@ class HexPlaneField(nn.Module):
 
 class Deformation(nn.Module):
     """Mirrors scene/deformation.py:16-160 for the live configuration (no_grid / grid_pe / empty_voxel /
-    static_mlp / apply_rotation are dead options in every shipped config and are rejected)."""
+    static_mlp / apply_rotation are dead options in every shipped config and are rejected).  ``feature_out`` is built as
+    the reference builds it: ``Linear(F, W)`` followed by ``[ReLU, Linear(W, W)] * (D - 1)`` (D = 0 and 1 are the same
+    network), so state_dict keys and shapes match for every depth the kernels take."""
 
     def __init__(self, D=8, W=256, args=None):
         super().__init__()
@@ -78,10 +80,17 @@ class Deformation(nn.Module):
                 getattr(args, "static_mlp", False) or getattr(args, "apply_rotation", False):
             raise NotImplementedError("no_grid / grid_pe / empty_voxel / static_mlp / apply_rotation are dead options "
                                       "in the reference configs and are not provided by the g4d path")
-        if D > 1:
-            raise NotImplementedError("defor_depth > 1 is not used by any reference config")
+        if not 0 <= D <= _lib.MAX_DEPTH:
+            raise NotImplementedError("defor_depth must be in 0..%d (the trunk layers the g4d kernels take), got %d"
+                                      % (_lib.MAX_DEPTH, D))
+        if W not in (64, 128):
+            raise NotImplementedError("net_width must be 64 or 128, got %d: one fp32 W x W weight image of a wider network "
+                                      "does not fit in an SM's shared memory (the FFMA network kernels stage one whole)" % W)
         self.grid = HexPlaneField(args.bounds, args.kplanes_config, args.multires)
-        self.feature_out = nn.Sequential(nn.Linear(self.grid.feat_dim, W))
+        trunk = [nn.Linear(self.grid.feat_dim, W)]
+        for _ in range(D - 1):
+            trunk += [nn.ReLU(), nn.Linear(W, W)]
+        self.feature_out = nn.Sequential(*trunk)
         for name, k in zip(_HEADS, _HEAD_OUT):
             setattr(self, name, nn.Sequential(nn.ReLU(), nn.Linear(W, W), nn.ReLU(), nn.Linear(W, k)))
         self.ratio = 0
@@ -162,8 +171,13 @@ class deform_network(nn.Module):
         return ((0 if a.no_dx else _lib.HEAD_POS) | (0 if a.no_ds else _lib.HEAD_SCALES) | (0 if a.no_dr else _lib.HEAD_ROT)
                 | (0 if a.no_do else _lib.HEAD_OPACITY) | (0 if a.no_dshs else _lib.HEAD_SHS))
 
+    def trunk_layers(self) -> List[nn.Linear]:
+        """feature_out.{2j} for j = 1 .. D-1: the trunk layers behind feature_out.0"""
+        return list(self.deformation_net.feature_out)[2::2]
+
     def flat_parameters(self) -> List[torch.Tensor]:
-        """planes (level-major), w0, b0, then (w1, b1, w2, b2) per head -- the order _DeformFunction uses.
+        """planes (level-major), w0, b0, then (w1, b1, w2, b2) per head, then (w, b) per trunk layer -- the order
+        _DeformFunction uses.
         The list of Parameter OBJECTS is cached (they survive .to() / load_state_dict / optimizer steps, which all write in
         place); ``invalidate_cache()`` drops it after module surgery."""
         if self._flat_cache is None:
@@ -173,6 +187,8 @@ class deform_network(nn.Module):
             for name in _HEADS:
                 seq = getattr(net, name)
                 out += [seq[1].weight, seq[1].bias, seq[3].weight, seq[3].bias]
+            for lin in self.trunk_layers():
+                out += [lin.weight, lin.bias]
             self._flat_cache = out
         return list(self._flat_cache)
 
@@ -258,6 +274,9 @@ class deform_network(nn.Module):
             seq = getattr(net, name)
             prm.w1[h], prm.b1[h] = seq[1].weight.data_ptr(), seq[1].bias.data_ptr()
             prm.w2[h], prm.b2[h] = seq[3].weight.data_ptr(), seq[3].bias.data_ptr()
+        prm.depth = int(net.D)
+        for j, lin in enumerate(self.trunk_layers()):
+            prm.wt[j], prm.bt[j] = lin.weight.data_ptr(), lin.bias.data_ptr()
         return prm
 
     def alloc_grads(self) -> List[torch.Tensor]:
@@ -345,6 +364,9 @@ class deform_network(nn.Module):
         for h in range(5):
             g.w1[h], g.b1[h], g.w2[h], g.b2[h] = (grads[i + j].data_ptr() for j in range(4))
             i += 4
+        for j in range(len(self.trunk_layers())):
+            g.wt[j], g.bt[j] = grads[i].data_ptr(), grads[i + 1].data_ptr()
+            i += 2
         return g
 
 

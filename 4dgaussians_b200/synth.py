@@ -178,9 +178,17 @@ def hidden_args(net: str):
         "c20w64": dict(channels=20, resolution=[10, 9, 8, 7], multires=[1, 2], net_width=64, no_do=True, no_dshs=False),
         "c24w128": dict(channels=24, resolution=[9, 10, 8, 6], multires=[1, 2], net_width=128, no_do=False, no_dshs=True),
         "f128w64": dict(channels=32, resolution=[6, 7, 5, 4], multires=[1, 2, 3, 4], net_width=64, no_do=False, no_dshs=True),
+        # F = 60 with all five heads at net_width 128: the FFMA kernel's tile of 64 Gaussians only just fits (no room for trunk
+        # biases: the half tile)
+        "c20w128sh": dict(channels=20, resolution=[8, 10, 9, 6], multires=[1, 2, 4], net_width=128, no_do=False, no_dshs=False),
+        # deformation networks with trunk layers (defor_depth 3): the dnerf heads at width 64, the dynerf heads at 128
+        "deep64": dict(channels=32, resolution=[12, 10, 9, 7], multires=[1, 2], net_width=64, no_do=True, no_dshs=True,
+                       defor_depth=3),
+        "deep128": dict(channels=16, resolution=[9, 12, 10, 8], multires=[1, 2], net_width=128, no_do=False, no_dshs=False,
+                        defor_depth=3),
     }
     c = cfgs[net]
-    return Namespace(net_width=c["net_width"], timebase_pe=4, defor_depth=1, posebase_pe=10, scale_rotation_pe=2, opacity_pe=2,
+    return Namespace(net_width=c["net_width"], timebase_pe=4, defor_depth=c.get("defor_depth", 1), posebase_pe=10, scale_rotation_pe=2, opacity_pe=2,
                      timenet_width=64, timenet_output=32, bounds=1.6, grid_pe=0,
                      kplanes_config={"grid_dimensions": 2, "input_coordinate_dim": 4, "output_coordinate_dim": c["channels"],
                                      "resolution": list(c["resolution"])},

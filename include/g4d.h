@@ -39,6 +39,7 @@ extern "C" {
 #define G4D_CAM_NO_GRAD 2
 #define G4D_MAX_LEVELS 4
 #define G4D_NUM_HEADS 5 /* pos, scales, rotations, opacity, shs (scene/deformation.py:61-65) */
+#define G4D_MAX_DEPTH 8 /* defor_depth: Linear layers of the trunk feature_out (scene/deformation.py:55-60) */
 
 enum {
     G4D_OK = 0,
@@ -77,7 +78,7 @@ typedef struct G4DCamera {
 typedef struct G4DDeformParams {
     int32_t levels;    /* len(multires) <= G4D_MAX_LEVELS */
     int32_t channels;  /* kplanes output_coordinate_dim: multiple of 4, <= 32 */
-    int32_t net_width; /* 64, 128 or 256 */
+    int32_t net_width; /* 64 or 128 */
     int32_t head_mask; /* G4D_HEAD_* bits */
     int32_t res[G4D_MAX_LEVELS][4]; /* per level: resolution of x, y, z, t */
     /* device: plane k of level l, CHANNEL-LAST [H][W][C]; (H,W) = (res[c1], res[c0]) for the k-th
@@ -88,6 +89,14 @@ typedef struct G4DDeformParams {
     const float *w1[G4D_NUM_HEADS], *b1[G4D_NUM_HEADS]; /* device: <head>.1  [Wd][Wd], [Wd] */
     const float *w2[G4D_NUM_HEADS], *b2[G4D_NUM_HEADS]; /* device: <head>.3  [k][Wd], [k]; k = 3,3,4,1,48 */
     uint64_t version; /* caller bumps it whenever any weight changed (packed copies are cached) */
+    /* the trunk behind feature_out.0: h_j = W_j relu(h_{j-1}) + b_j for j = 1 .. depth-1, every head reads h_{depth-1}.
+     * depth 0 and 1 both mean no trunk layer (feature_out.0 alone); at most G4D_MAX_DEPTH, with every levels / channels /
+     * head_mask / net_width the other fields allow.  A zero-filled tail is the network without trunk layers, so a caller
+     * zero-initialises the struct. */
+    int32_t depth;     /* defor_depth */
+    int32_t reserved;
+    const float *wt[G4D_MAX_DEPTH - 1], *bt[G4D_MAX_DEPTH - 1]; /* device: wt[j-1], bt[j-1] = feature_out.{2j}  [Wd][Wd], [Wd],
+                                                                 * j = 1 .. depth-1 (non-NULL); the rest are not read */
 } G4DDeformParams;
 
 /* gradient sinks mirroring G4DDeformParams (device, same layouts; ACCUMULATED into, caller zeroes) */
@@ -96,6 +105,7 @@ typedef struct G4DDeformGrads {
     float *w0, *b0;
     float *w1[G4D_NUM_HEADS], *b1[G4D_NUM_HEADS];
     float *w2[G4D_NUM_HEADS], *b2[G4D_NUM_HEADS];
+    float *wt[G4D_MAX_DEPTH - 1], *bt[G4D_MAX_DEPTH - 1]; /* the trunk layers j = 1 .. depth-1 */
 } G4DDeformGrads;
 
 /* the GaussianModel tensors render() reads (scene/gaussian_model.py:108-131), all device */
@@ -259,10 +269,11 @@ enum { G4D_OPT_SYNC_MODE = 1,  /* 1 (default): size the instance buffer exactly 
        G4D_OPT_STAGE_TIMING = 4, /* 1: bracket every stage with CUDA events on the launching stream
                                    (bench.py's live per-kernel durations); 0 (default): off */
        G4D_OPT_TENSOR_CORES = 5, /* the deformation MLP's forward when the configuration allows tensor cores (net_width 128,
-                                   C in {16,32}, F <= 64): 2 (default) wgmma with FP16x2 operands (hi + lo halves, 3 products,
+                                   C in {16,32}, F <= 64, and no trunk layers): 2 (default) wgmma with FP16x2 operands (hi + lo halves, 3 products,
                                    fp32-accurate; operands must stay below 65504 after scaling -- activations < 8188, features
                                    < 1023, weights < 255 -- else the NEXT call returns G4D_ERR_OVERFLOW); 1: wgmma 3xTF32 (no
-                                   range limit); 0: FP32 FFMA kernels */
+                                   range limit); 0: FP32 FFMA kernels.  The tensor-core kernels take the network with
+                                   no trunk layers (depth <= 1); a deeper one runs on the FFMA kernels whatever the value */
        G4D_OPT_TC_DEBUG = 6,     /* 1: the tensor-core forward records cycle counters per CTA (g4d_debug_tc_cycles: [0] whole
                                    kernel, [1] waiting for W1 images, [2..11] unused) */
        G4D_OPT_KEEP_DEFORMED = 8, /* 1: a no-grad fused forward (G4D_CAM_NO_GRAD) still stores the deformed + activated tensors
