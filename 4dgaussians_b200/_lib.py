@@ -59,7 +59,8 @@ class Camera(C.Structure):
     _fields_ = [("image_height", C.c_int32), ("image_width", C.c_int32), ("sh_degree", C.c_int32), ("debug", C.c_int32),
                 ("tanfovx", C.c_float), ("tanfovy", C.c_float), ("scale_modifier", C.c_float), ("time", C.c_float),
                 ("viewmatrix", C.c_float * 16), ("projmatrix", C.c_float * 16), ("campos", C.c_float * 3),
-                ("bg", C.c_float * 3), ("d_viewmatrix", fp), ("d_projmatrix", fp), ("d_campos", fp), ("d_bg", fp)]
+                ("bg", C.c_float * 3), ("d_viewmatrix", fp), ("d_projmatrix", fp), ("d_campos", fp), ("d_bg", fp),
+                ("sh_coeffs", C.c_int32), ("reserved", C.c_int32)]
 
 
 class DeformParams(C.Structure):
@@ -206,6 +207,32 @@ def cuda_f32(t: Optional[torch.Tensor], what: str, numel: Optional[int] = None) 
     if numel is not None and t.numel() != numel:
         raise RuntimeError("%s has %d elements, expected %d" % (what, t.numel(), numel))
     return t
+
+
+SH_COEFFS = (1, 4, 9, 16)          # M = (max_sh_degree + 1)^2 of the SH degrees 0..3 the kernels take
+
+
+def sh_coeffs(sh: torch.Tensor, n: int, what: str, skip: int = 0) -> int:
+    """M, the SH coefficients per Gaussian, of ``sh`` holding M - skip of them per Gaussian: [N, M - skip, 3] (the reference
+    takes M = sh.size(1)) or any shape of N * 3 * (M - skip) elements.  Raises unless M is 1, 4, 9 or 16."""
+    if sh.dim() == 3 and sh.shape[0] == n and sh.shape[2] == 3:
+        m = sh.shape[1] + skip
+    else:
+        m = sh.numel() // (3 * n) + skip if n > 0 and sh.numel() % (3 * n) == 0 else -1
+    if m not in SH_COEFFS:
+        raise RuntimeError("%s of shape %s holds no SH degree 0..3 for %d Gaussians: expected [N, M%s, 3] with M = "
+                           "(max_sh_degree + 1)^2 in %s" % (what, tuple(sh.shape), n, " - %d" % skip if skip else "", SH_COEFFS))
+    return m
+
+
+def check_sh_degree(m: int, active: int, head_mask: int = 0):
+    """The active degree and the network the C-ABI accepts with M coefficients (its G4D_ERR_ARG refusals, raised first)."""
+    if not 0 <= active <= 3 or (active + 1) ** 2 > m:
+        raise ValueError("active SH degree %d needs (degree + 1)^2 = %d coefficients; the model stores %d (max_sh_degree %d)"
+                         % (active, (active + 1) ** 2, m, SH_COEFFS.index(m)))
+    if (head_mask & HEAD_SHS) and m != 16:
+        raise ValueError("the deformation network's SH head (no_dshs=False) deforms 16 SH coefficients per Gaussian: it needs "
+                         "max_sh_degree 3, the model has %d" % SH_COEFFS.index(m))
 
 
 def workspace_of(device: torch.device) -> "Workspace":

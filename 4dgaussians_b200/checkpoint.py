@@ -84,8 +84,8 @@ def read_ply_vertices(path: str) -> Dict[str, np.ndarray]:
 
 
 def save_ply(path: str, xyz, features_dc, features_rest, opacity, scaling, rotation):
-    """GaussianModel.save_ply (scene/gaussian_model.py:250-268).  features are [N,1,3] / [N,15,3]; f_dc / f_rest columns
-    are channel-major (``transpose(1, 2).flatten(start_dim=1)``)."""
+    """GaussianModel.save_ply (scene/gaussian_model.py:250-268).  features are [N,1,3] / [N,M-1,3] with M = (max_sh_degree
+    + 1)^2, written as 3M - 3 f_rest columns; f_dc / f_rest columns are channel-major (``transpose(1, 2).flatten(start_dim=1)``)."""
     t = lambda a: a.detach().float().cpu()
     xyz_, op, sc, rot = t(xyz).numpy(), t(opacity).numpy().reshape(-1, 1), t(scaling).numpy(), t(rotation).numpy()
     f_dc = t(features_dc).transpose(1, 2).flatten(start_dim=1).contiguous().numpy()

@@ -127,6 +127,7 @@ struct ForwardRecord {
     bool deformed = false;    // the deformation network ran (fine stage)
     bool sh = false;          // the SHS head was active: the deformed SH coefficients are in fo.shs
     bool kept = false;        // fo holds the deformed, activated tensors
+    int sh_coeffs = 0;        // M: SH coefficients per Gaussian of the forward's inputs (its camera's sh_coeffs)
     int feat_cols = 0;        // F of the HexPlane features in `feat` and the ReLU bits in `relu` kept for a backward (0: none)
     // g4d_render_forward_cameras: serial number of the call (0: a single-camera forward), this camera's position, the number
     // of cameras, and whether the group keeps what its backward reads
@@ -481,11 +482,18 @@ int deform_backward_dispatch(G4DWorkspace* ws, const G4DDeformParams* prm, float
     return G4D_OK;
 }
 
+// M of a camera: the SH coefficients per Gaussian of the tensors it is rendered with (0 in G4DCamera.sh_coeffs means 16)
+int sh_coeffs(const G4DCamera* cam) { return cam->sh_coeffs ? cam->sh_coeffs : kShCoeffs; }
+
 int check_camera(const G4DCamera* cam) {
     if (!cam) return fail(G4D_ERR_ARG, "camera is NULL");
     if (cam->image_height <= 0 || cam->image_width <= 0 || cam->image_height > 16384 || cam->image_width > 16384)
         return fail(G4D_ERR_ARG, "image size out of range");
     if (cam->sh_degree < 0 || cam->sh_degree > 3) return fail(G4D_ERR_ARG, "sh_degree must be 0..3");
+    const int m = sh_coeffs(cam);
+    if (m != 1 && m != 4 && m != 9 && m != 16) return fail(G4D_ERR_ARG, "sh_coeffs must be 0, 1, 4, 9 or 16");
+    if ((cam->sh_degree + 1) * (cam->sh_degree + 1) > m)
+        return fail(G4D_ERR_ARG, "sh_degree needs more SH coefficients than sh_coeffs gives ((sh_degree + 1)^2 > M)");
     if (!(cam->tanfovx > 0.f) || !(cam->tanfovy > 0.f)) return fail(G4D_ERR_ARG, "tanfov must be positive");
     return G4D_OK;
 }
@@ -591,10 +599,10 @@ int bin_and_blend(G4DContext* c, const G4DCamera* cam, int64_t n, float* out_col
     return debug_sync(cam, st, "blend_forward");
 }
 
-// A caller's SH tensors: fused [N,16,3] in dc, or (split) dc [N,1,3] + rest [N,15,3].  Sh = ShIn for the coefficients,
-// ShOut for their gradient sinks.
-template <class Sh, class T> Sh caller_sh(bool split, T* dc, T* rest = nullptr) {
-    return split ? Sh{nullptr, dc, rest} : Sh{dc, nullptr, nullptr};
+// A caller's SH tensors of M coefficients: fused [N,M,3] in dc, or (split) dc [N,1,3] + rest [N,M-1,3].  Sh = ShIn for the
+// coefficients, ShOut for their gradient sinks.
+template <class Sh, class T> Sh caller_sh(int m, bool split, T* dc, T* rest = nullptr) {
+    return split ? Sh{nullptr, dc, rest, m} : Sh{dc, nullptr, nullptr, m};
 }
 
 // blend backward + per-Gaussian backward on `in`; opacity gradient lands in g_opacities (zeroed here)
@@ -742,7 +750,7 @@ int g4d_deform_forward(G4DWorkspace* ws, const G4DDeformParams* prm, int64_t n, 
     DeformSetup s{};
     if ((rc = setup_deform(ws, prm, xyz, n, ws->trow, trow, TimeArg{time, nullptr}, st, &s)) != G4D_OK) return rc;
     if ((rc = attach_forward_buffers(ws, s, nullptr, relu_bits, n, st)) != G4D_OK) return rc;
-    const DeformIO io{xyz, scaling, rotation, opacity, caller_sh<ShIn>(false, shs), out_xyz, out_scaling, out_rotation, out_opacity,
+    const DeformIO io{xyz, scaling, rotation, opacity, caller_sh<ShIn>(kShCoeffs, false, shs), out_xyz, out_scaling, out_rotation, out_opacity,
                       out_shs, GeomBuffers{}, FusedOutputs{}, nullptr};
     G4D_CUDA(launch_deform(s.d, 0, nullptr, n, io, s.gather, ws->sm_count, st, s.tc ? &s.tw : nullptr));
     return G4D_OK;
@@ -767,13 +775,14 @@ int g4d_rasterize_forward(G4DContext* c, const G4DCamera* cam, int64_t n, const 
     if ((rc = check_pending(c)) != G4D_OK) return rc;
     c->fwd = ForwardRecord{};
     if ((rc = setup_view(c, cam, nullptr, n, st, [] { return G4D_OK; })) != G4D_OK) return rc;
-    const RasterInputs in{means3D, scales, rotations, opacities, caller_sh<ShIn>(false, shs)};
+    const RasterInputs in{means3D, scales, rotations, opacities, caller_sh<ShIn>(sh_coeffs(cam), false, shs)};
     {
         StageTimer tm(c, G4D_STAGE_GEOM, st);
         G4D_CUDA(launch_preprocess(c->cam.as<CameraDev>(), n, in, c->g, out_radii, st));
     }
     if ((rc = bin_and_blend(c, cam, n, out_color, out_depth, st)) != G4D_OK) return rc;
     c->fwd = ForwardRecord{ForwardRecord::kRaster, n, cam->image_height, cam->image_width};
+    c->fwd.sh_coeffs = sh_coeffs(cam);
     return G4D_OK;
 }
 
@@ -786,6 +795,7 @@ int g4d_rasterize_backward(G4DContext* c, const G4DCamera* cam, int64_t n, const
     int rc = check_camera(cam);
     if (rc != G4D_OK) return rc;
     if (cam->image_height != c->fwd.H || cam->image_width != c->fwd.W) return fail(G4D_ERR_STATE, "camera differs from the forward's");
+    if (sh_coeffs(cam) != c->fwd.sh_coeffs) return fail(G4D_ERR_STATE, "sh_coeffs differs from the forward's");
     if (!dL_dcolor || (n > 0 && (!g_means3D || !g_means2D || !g_shs || !g_opacities || !g_scales || !g_rotations)))
         return fail(G4D_ERR_ARG, "NULL gradient pointer");
     cudaStream_t st = (cudaStream_t)stream;
@@ -795,8 +805,9 @@ int g4d_rasterize_backward(G4DContext* c, const G4DCamera* cam, int64_t n, const
     if ((rc = refuse_capture(c->ws, cam, 1, nullptr)) != G4D_OK) return rc;
     if ((rc = check_pending(c)) != G4D_OK) return rc;
     (void)opacities;
-    const RasterInputs in{means3D, scales, rotations, opacities, caller_sh<ShIn>(false, shs)};
-    return raster_backward_stages(c, cam, n, in, dL_dcolor, g_means3D, g_means2D, caller_sh<ShOut>(false, g_shs),
+    const int m = sh_coeffs(cam);
+    const RasterInputs in{means3D, scales, rotations, opacities, caller_sh<ShIn>(m, false, shs)};
+    return raster_backward_stages(c, cam, n, in, dL_dcolor, g_means3D, g_means2D, caller_sh<ShOut>(m, false, g_shs),
                                   g_opacities, g_scales, g_rotations, st);
 }
 
@@ -929,11 +940,19 @@ int g4d_deform_backward(G4DWorkspace* ws, const G4DDeformParams* prm, G4DDeformG
 // ------------------------------------------------------------------------------------------------------
 namespace {
 
+// the SHS head adds a delta to all 16 coefficients (deformation.py:142): it needs models with all 16
+int check_sh_head(const G4DCamera* cam, const G4DDeformParams* prm) {
+    if (prm && (prm->head_mask & G4D_HEAD_SHS) && sh_coeffs(cam) != kShCoeffs)
+        return fail(G4D_ERR_ARG, "the SHS head deforms 16 SH coefficients: it needs sh_coeffs 16");
+    return G4D_OK;
+}
+
 int check_render_args(const G4DCamera* cam, const G4DDeformParams* prm, const G4DGaussians* g, const float* out_color,
                       const float* out_depth, const int32_t* out_radii) {
     int rc = check_camera(cam);
     if (rc != G4D_OK) return rc;
     if (prm && (rc = check_params(prm)) != G4D_OK) return rc;
+    if ((rc = check_sh_head(cam, prm)) != G4D_OK) return rc;
     if (!g || g->n < 0 || g->n >= (1ll << 31) || !out_color || !out_depth) return fail(G4D_ERR_ARG, "bad gaussians / outputs");
     if (g->n > 0 && (!g->xyz || !g->scaling || !g->rotation || !g->opacity || !g->features_dc || !out_radii))
         return fail(G4D_ERR_ARG, "NULL gaussian tensor");
@@ -950,7 +969,8 @@ int fused_forward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* pr
     const bool with_sh = prm && (prm->head_mask & G4D_HEAD_SHS);
     // a no-grad render needs none of the saved tensors: skip their stores (48 B + 192 B of deformed SH per Gaussian)
     const bool kept = !(cam->debug & G4D_CAM_NO_GRAD) || ws->keep_deformed || keep_fo;
-    *rec = ForwardRecord{ForwardRecord::kFused, n, cam->image_height, cam->image_width, prm != nullptr, with_sh, kept};
+    *rec = ForwardRecord{ForwardRecord::kFused, n, cam->image_height, cam->image_width, prm != nullptr, with_sh, kept,
+                         sh_coeffs(cam)};
     if ((rc = ensure_fused(c, n, with_sh)) != G4D_OK) return rc;
     CameraDev* dcam = c->cam.as<CameraDev>();
     DeformSetup s{};
@@ -961,7 +981,7 @@ int fused_forward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* pr
     {
         StageTimer tm(c, G4D_STAGE_GEOM, st);
         const DeformIO io{g->xyz, g->scaling, g->rotation, g->opacity,
-                          caller_sh<ShIn>(g->features_rest != nullptr, g->features_dc, g->features_rest),
+                          caller_sh<ShIn>(rec->sh_coeffs, g->features_rest != nullptr, g->features_dc, g->features_rest),
                           nullptr, nullptr, nullptr, nullptr, nullptr, c->g, kept ? c->fo : FusedOutputs{}, out_radii};
         if (prm) {
             const bool save = s.tc && !(cam->debug & G4D_CAM_NO_GRAD);
@@ -981,12 +1001,12 @@ int fused_forward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* pr
     return bin_and_blend(c, cam, n, out_color, out_depth, st);
 }
 
-// the post-activation inputs of the rasterizer stages of a fused forward on c: its stored deformed tensors, and the SH
+// the post-activation inputs of the rasterizer stages of the fused forward f on c: its stored deformed tensors, and the SH
 // coefficients (deformed when the SHS head was active, the caller's otherwise)
-RasterInputs deformed_inputs(const G4DContext* c, bool sh, const G4DGaussians* g) {
+RasterInputs deformed_inputs(const G4DContext* c, const ForwardRecord& f, const G4DGaussians* g) {
     RasterInputs in{c->fo.means3D, c->fo.scales, c->fo.rotations, c->fo.opacities,
-                    caller_sh<ShIn>(g->features_rest != nullptr, g->features_dc, g->features_rest)};
-    if (sh) in.sh = ShIn{c->fo.shs, nullptr, nullptr};
+                    caller_sh<ShIn>(f.sh_coeffs, g->features_rest != nullptr, g->features_dc, g->features_rest)};
+    if (f.sh) in.sh = ShIn{c->fo.shs, nullptr, nullptr};
     return in;
 }
 
@@ -1011,7 +1031,7 @@ int deformed_grads(G4DContext* c, int64_t n, const G4DGaussianGrads* gg, Deforme
 // feeds the network's backward: the fused sink is then the scratch d_sh, which fused_backward_tail passes on to a caller
 // sink in the fused layout.
 ShOut fused_sh_sinks(const G4DContext* c, const G4DGaussians* g, const G4DGaussianGrads* gg, float* d_sh) {
-    ShOut o = caller_sh<ShOut>(g->features_rest != nullptr, gg->features_dc, gg->features_rest);
+    ShOut o = caller_sh<ShOut>(c->fwd.sh_coeffs, g->features_rest != nullptr, gg->features_dc, gg->features_rest);
     if (c->fwd.sh) o.shs = d_sh;
     return o;
 }
@@ -1048,7 +1068,7 @@ int fused_backward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* p
     if ((rc = deformed_grads(c, n, gg, &d)) != G4D_OK) return rc;
     // SH gradient: identity residual path -> written straight into the caller's sinks; the fused copy (when the SHS
     // head is active) additionally feeds the network's backward
-    rc = raster_backward_stages(c, cam, n, deformed_inputs(c, c->fwd.sh, g), dL_dcolor, d.xyz, gg->means2D,
+    rc = raster_backward_stages(c, cam, n, deformed_inputs(c, c->fwd, g), dL_dcolor, d.xyz, gg->means2D,
                                 fused_sh_sinks(c, g, gg, d.sh), d.op, d.sc, d.rot, st);
     if (rc != G4D_OK) return rc;
     return fused_backward_tail(c, cam, prm, pgrads, g, gg, d, st);
@@ -1064,6 +1084,7 @@ int check_camera_group(G4DContext* const* ctx, int32_t k, const G4DCamera* cams)
     const float* src = ctx && ctx[0] ? ctx[0]->time_src : nullptr;
     for (int i = 0; i < k; ++i) {
         if ((rc = check_camera(&cams[i])) != G4D_OK) return rc;
+        if (sh_coeffs(&cams[i]) != sh_coeffs(&cams[0])) return fail(G4D_ERR_ARG, "the cameras of one call must share sh_coeffs");
         if (!src && memcmp(&cams[i].time, &cams[0].time, sizeof(float)) != 0)
             return fail(G4D_ERR_ARG, "the cameras of one call must share their time bit for bit");
     }
@@ -1113,12 +1134,15 @@ int g4d_render_backward(G4DContext* c, const G4DCamera* cam, const G4DDeformPara
     int rc = check_camera(cam);
     if (rc != G4D_OK) return rc;
     if (prm && (rc = check_params(prm)) != G4D_OK) return rc;
+    if ((rc = check_sh_head(cam, prm)) != G4D_OK) return rc;
     if (prm && !pgrads) return fail(G4D_ERR_ARG, "pgrads is NULL");
     if (cam->image_height != c->fwd.H || cam->image_width != c->fwd.W) return fail(G4D_ERR_STATE, "camera differs from the forward's");
+    if (sh_coeffs(cam) != c->fwd.sh_coeffs) return fail(G4D_ERR_STATE, "sh_coeffs differs from the forward's");
     const int64_t n = g->n;
     if (!dL_dcolor || !gg || (n > 0 && (!gg->xyz || !gg->scaling || !gg->rotation || !gg->opacity || !gg->features_dc || !gg->means2D)))
         return fail(G4D_ERR_ARG, "NULL gradient pointer");
-    if (g->features_rest && n > 0 && !gg->features_rest) return fail(G4D_ERR_ARG, "features_rest gradient sink is NULL");
+    if (g->features_rest && n > 0 && !gg->features_rest && sh_coeffs(cam) > 1)     // (M = 1: features_rest holds nothing)
+        return fail(G4D_ERR_ARG, "features_rest gradient sink is NULL");
     const cudaStream_t st = (cudaStream_t)stream;
     G4D_CUDA(cudaSetDevice(c->ws->device));
     CallScope scope(c->ws, st);
@@ -1161,7 +1185,7 @@ int g4d_render_forward_cameras(G4DContext* const* ctx, int32_t k, const G4DCamer
         }
         {
             StageTimer tm(ctx[1], G4D_STAGE_GEOM, st);
-            G4D_CUDA(launch_project_cameras(ec, n, deformed_inputs(c0, r0.sh, g), st));
+            G4D_CUDA(launch_project_cameras(ec, n, deformed_inputs(c0, r0, g), st));
         }
         if ((rc = debug_sync(&cams[1], st, "project_cameras")) != G4D_OK) return rc;
         for (int i = 1; i < k; ++i)
@@ -1171,7 +1195,7 @@ int g4d_render_forward_cameras(G4DContext* const* ctx, int32_t k, const G4DCamer
     const uint64_t serial = ++g_group_serial;
     for (int i = 0; i < k; ++i) {
         ForwardRecord r = i == 0 ? r0 : ForwardRecord{ForwardRecord::kFused, n, cams[i].image_height, cams[i].image_width,
-                                                      r0.deformed, r0.sh};
+                                                      r0.deformed, r0.sh, false, r0.sh_coeffs};
         r.group = serial; r.group_pos = i; r.group_size = k; r.group_grad = !(cams[0].debug & G4D_CAM_NO_GRAD);
         ctx[i]->fwd = r;
     }
@@ -1192,15 +1216,18 @@ int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCame
             return fail(G4D_ERR_STATE, "g4d_render_backward_cameras needs the matching g4d_render_forward_cameras on these contexts, "
                                        "with no other forward on any of them since");
         if (cams[i].image_height != f.H || cams[i].image_width != f.W) return fail(G4D_ERR_STATE, "camera differs from the forward's");
+        if (sh_coeffs(&cams[i]) != f.sh_coeffs) return fail(G4D_ERR_STATE, "sh_coeffs differs from the forward's");
     }
     if (!c0->fwd.group_grad || !c0->fwd.kept) return fail(G4D_ERR_STATE, "g4d_render_backward_cameras after a G4D_CAM_NO_GRAD forward: nothing was saved for it");
     if ((prm != nullptr) != c0->fwd.deformed) return fail(G4D_ERR_STATE, "deform params differ from the forward's");
     if (prm && (rc = check_params(prm)) != G4D_OK) return rc;
+    if ((rc = check_sh_head(&cams[0], prm)) != G4D_OK) return rc;
     if (prm && !pgrads) return fail(G4D_ERR_ARG, "pgrads is NULL");
     const int64_t n = g->n;
     if (n > 0 && (!gg->xyz || !gg->scaling || !gg->rotation || !gg->opacity || !gg->features_dc))
         return fail(G4D_ERR_ARG, "NULL gradient pointer");
-    if (g->features_rest && n > 0 && !gg->features_rest) return fail(G4D_ERR_ARG, "features_rest gradient sink is NULL");
+    if (g->features_rest && n > 0 && !gg->features_rest && sh_coeffs(&cams[0]) > 1)
+        return fail(G4D_ERR_ARG, "features_rest gradient sink is NULL");
     cudaStream_t st = (cudaStream_t)stream;
     G4DWorkspace* ws = c0->ws;
     G4D_CUDA(cudaSetDevice(ws->device));
@@ -1244,7 +1271,7 @@ int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCame
     }
     {
         StageTimer tm(c0, G4D_STAGE_GEOM_BWD, st);
-        G4D_CUDA(launch_preprocess_backward_cameras(bc, n, deformed_inputs(c0, c0->fwd.sh, g), d.xyz, d.sc, d.rot, d.op,
+        G4D_CUDA(launch_preprocess_backward_cameras(bc, n, deformed_inputs(c0, c0->fwd, g), d.xyz, d.sc, d.rot, d.op,
                                                     fused_sh_sinks(c0, g, gg, d.sh), st));
     }
     if ((rc = debug_sync(&cams[0], st, "preprocess_backward_cameras")) != G4D_OK) return rc;

@@ -9,6 +9,8 @@
 
 namespace g4d {
 
+// FULL: M = 16 SH coefficients per Gaussian (ShIn), else M = in.sh.m = g_sh.m
+template <bool FULL>
 __global__ void __launch_bounds__(256)
 preprocess_backward_kernel(const CameraDev* __restrict__ camp, int64_t n, RasterInputs in, GeomBuffers g,
                            const float* __restrict__ g_mean2D, const float* __restrict__ g_conic,
@@ -28,7 +30,7 @@ preprocess_backward_kernel(const CameraDev* __restrict__ camp, int64_t n, Raster
     if (cnt == 0) return;                          // whole warp
     const int64_t gi = g0 + lane;
     const bool active = lane < cnt;
-    in.sh.stage_warp(g0, cnt, lane, ld);
+    in.sh.stage_warp<FULL>(g0, cnt, lane, ld);
     __syncwarp();
     auto sh_store = [&](int k, int ch, float v) { st[lane * kShRow + 3 * k + ch] = v; };
     if (active) {
@@ -59,7 +61,7 @@ preprocess_backward_kernel(const CameraDev* __restrict__ camp, int64_t n, Raster
         }
     }
     __syncwarp();
-    g_sh.store_warp(g0, cnt, lane, st);
+    g_sh.store_warp<FULL>(g0, cnt, lane, st);
 }
 
 cudaError_t launch_preprocess_backward(const CameraDev* cam, int64_t n, const RasterInputs& in, GeomBuffers g,
@@ -69,11 +71,12 @@ cudaError_t launch_preprocess_backward(const CameraDev* cam, int64_t n, const Ra
     if (n == 0) return cudaSuccess;
     constexpr int kThreads = 128;
     const size_t smem = (size_t)(kThreads / 32) * 2 * 32 * kShRow * sizeof(float);   // 50 KB: SH staging (see the kernel)
+    auto kernel = g_sh.m == kShCoeffs ? preprocess_backward_kernel<true> : preprocess_backward_kernel<false>;
     {
-        cudaError_t e = cudaFuncSetAttribute(preprocess_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
     }
-    preprocess_backward_kernel<<<(unsigned)((n + kThreads - 1) / kThreads), kThreads, smem, st>>>(cam, n, in, g, g_mean2D, g_conic, g_rgb,
+    kernel<<<(unsigned)((n + kThreads - 1) / kThreads), kThreads, smem, st>>>(cam, n, in, g, g_mean2D, g_conic, g_rgb,
                                                                                                   g_means3D, g_means2D_out, g_scales,
                                                                                                   g_rotations, g_sh);
     return cudaGetLastError();
@@ -83,6 +86,7 @@ cudaError_t launch_preprocess_backward(const CameraDev* cam, int64_t n, const Ra
 // coefficients are loaded once, gaussian_backward runs for every camera that sees the Gaussian, and the sums -- mean,
 // scale and rotation in registers, SH in the warp's shared-memory rows, opacity from the cameras' blend backward passes --
 // are written once.  Each camera's screen-space gradient goes to its own sink.
+template <bool FULL>
 __global__ void __launch_bounds__(128)
 preprocess_backward_cameras_kernel(BackwardCameras bc, int64_t n, RasterInputs in, float* __restrict__ g_means3D,
                                    float* __restrict__ g_scales, float* __restrict__ g_rotations, float* __restrict__ g_opacities,
@@ -98,7 +102,7 @@ preprocess_backward_cameras_kernel(BackwardCameras bc, int64_t n, RasterInputs i
     const int cnt = (int)(n - g0 < 32 ? (n - g0 > 0 ? n - g0 : 0) : 32);
     if (cnt == 0) return;
     const int64_t gi = g0 + lane;
-    in.sh.stage_warp(g0, cnt, lane, ld);
+    in.sh.stage_warp<FULL>(g0, cnt, lane, ld);
     for (int idx = lane; idx < cnt * 48; idx += 32) st[idx / 48 * kShRow + idx % 48] = 0.f;
     __syncwarp();
     if (lane < cnt) {
@@ -137,7 +141,7 @@ preprocess_backward_cameras_kernel(BackwardCameras bc, int64_t n, RasterInputs i
         g_opacities[gi] = gop;
     }
     __syncwarp();
-    g_sh.store_warp(g0, cnt, lane, st);
+    g_sh.store_warp<FULL>(g0, cnt, lane, st);
 }
 
 cudaError_t launch_preprocess_backward_cameras(const BackwardCameras& bc, int64_t n, const RasterInputs& in, float* g_means3D,
@@ -146,9 +150,10 @@ cudaError_t launch_preprocess_backward_cameras(const BackwardCameras& bc, int64_
     if (n == 0) return cudaSuccess;
     constexpr int kThreads = 128;
     const size_t smem = (size_t)(kThreads / 32) * 2 * 32 * kShRow * sizeof(float);   // 50 KB: SH staging and sums
-    cudaError_t e = cudaFuncSetAttribute(preprocess_backward_cameras_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    auto kernel = g_sh.m == kShCoeffs ? preprocess_backward_cameras_kernel<true> : preprocess_backward_cameras_kernel<false>;
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    preprocess_backward_cameras_kernel<<<(unsigned)((n + kThreads - 1) / kThreads), kThreads, smem, st>>>(
+    kernel<<<(unsigned)((n + kThreads - 1) / kThreads), kThreads, smem, st>>>(
         bc, n, in, g_means3D, g_scales, g_rotations, g_opacities, g_sh);
     return cudaGetLastError();
 }

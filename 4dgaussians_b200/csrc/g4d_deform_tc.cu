@@ -224,6 +224,7 @@ __device__ __forceinline__ void mbar_arrive(void* bar) {
 }
 __device__ __forceinline__ void bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 
+// MODE as deform_kernel's (g4d_geom.cu): 0 deform only, 1 fused with M = 16 SH coefficients, 2 fused with M < 16
 template <int ARITH, int MODE, int C, int L, bool SAVE>
 __global__ void __launch_bounds__(TcArith<ARITH>::NWG * 128, 1)
 deform_tc_kernel(DeformDesc d, TcWeights tw, TcSmem Ls, const CameraDev* __restrict__ camp, int64_t n, DeformIO io) {
@@ -265,7 +266,7 @@ deform_tc_kernel(DeformDesc d, TcWeights tw, TcSmem Ls, const CameraDev* __restr
     }
     pdl_wait();           // from here on: the camera, the staged features
     pdl_trigger();
-    if (MODE == 1) stage_cameras(&cam, &camp, 1);
+    if (MODE != 0) stage_cameras(&cam, &camp, 1);
     __syncthreads();
 
     const bool hsh = d.head_mask & G4D_HEAD_SHS;
@@ -479,7 +480,8 @@ deform_tc_kernel(DeformDesc d, TcWeights tw, TcSmem Ls, const CameraDev* __restr
                             }
                         }
                     } else {
-                        fused_finish_colour(cam, io, gi, p, hsh, dsh);
+                        if (MODE == 1) fused_finish_colour(cam, io, gi, p, hsh, dsh);
+                        else fused_finish_colour_reduced(cam, io, gi, p);
                     }
                 }
             }
@@ -642,8 +644,9 @@ cudaError_t launch_deform_tc(const DeformDesc& d, const TcWeights& tw, int mode,
     const int grid = (int)(ntiles < sm_count ? ntiles : sm_count);
 #define G4D_TC_CASE(AR, CC, LL)                                                                                        \
     if (tw.arith == AR && d.C == CC && d.levels == LL)                                                                 \
-        return mode == 0 ? launch_deform_tc_t<AR, 0, CC, LL>(d, tw, Ls, bytes, grid, cam, n, io, st)                   \
-                         : launch_deform_tc_t<AR, 1, CC, LL>(d, tw, Ls, bytes, grid, cam, n, io, st);
+        return mode == 0                   ? launch_deform_tc_t<AR, 0, CC, LL>(d, tw, Ls, bytes, grid, cam, n, io, st)  \
+               : io.sh.m == kShCoeffs ? launch_deform_tc_t<AR, 1, CC, LL>(d, tw, Ls, bytes, grid, cam, n, io, st)  \
+                                      : launch_deform_tc_t<AR, 2, CC, LL>(d, tw, Ls, bytes, grid, cam, n, io, st);
     G4D_TC_CASE(2, 16, 2)
     G4D_TC_CASE(2, 16, 3)
     G4D_TC_CASE(2, 32, 2)

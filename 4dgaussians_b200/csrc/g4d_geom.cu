@@ -122,7 +122,8 @@ cudaError_t launch_collapse_time_rows(const G4DDeformParams& p, TimeArg time, fl
 }
 
 // ------------------------------------------------------------------------------------------------------
-// Standalone preprocess: one thread per Gaussian, inputs are post-activation (A.1).
+// Standalone preprocess: one thread per Gaussian, inputs are post-activation (A.1).  FULL: M = 16 (ShIn).
+template <bool FULL>
 __global__ void __launch_bounds__(256) preprocess_kernel(const CameraDev* __restrict__ camp, int64_t n, RasterInputs in,
                                                          GeomBuffers g, int32_t* out_radii) {
     __shared__ CameraDev cam;
@@ -137,14 +138,16 @@ __global__ void __launch_bounds__(256) preprocess_kernel(const CameraDev* __rest
     const bool ok = project_gaussian(cam, p, sc, Quat{q4.x, q4.y, q4.z, q4.w}, pr);
     float rgb[3] = {0.f, 0.f, 0.f};
     uint32_t bits = 0;
-    if (ok) in.sh.with_coeffs(gi, [&](auto sh) { sh_to_rgb(cam, p, sh, rgb, bits); });
+    if (ok) in.sh.with_coeffs<FULL>(gi, [&](auto sh) { sh_to_rgb(cam, p, sh, rgb, bits); });
     store_projected(g, gi, ok, pr, in.opacities[gi], rgb, bits, out_radii);
 }
 
 cudaError_t launch_preprocess(const CameraDev* cam, int64_t n, const RasterInputs& in, GeomBuffers g, int32_t* out_radii,
                               cudaStream_t st) {
     if (n == 0) return cudaSuccess;
-    preprocess_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(cam, n, in, g, out_radii);
+    const unsigned blocks = (unsigned)((n + 255) / 256);
+    if (in.sh.m == kShCoeffs) preprocess_kernel<true><<<blocks, 256, 0, st>>>(cam, n, in, g, out_radii);
+    else preprocess_kernel<false><<<blocks, 256, 0, st>>>(cam, n, in, g, out_radii);
     return cudaGetLastError();
 }
 
@@ -153,6 +156,7 @@ cudaError_t launch_preprocess(const CameraDev* cam, int64_t n, const RasterInput
 // activated state camera 0's fused forward stored (44 B, plus 192 B of SH staged per warp through shared memory) ONCE and
 // projects it into every other camera with the fused kernels' projection and colour code: the inputs are the very floats
 // those kernels held in registers, so each camera's records equal its own render()'s bit for bit.
+template <bool FULL>
 __global__ void __launch_bounds__(256) project_cameras_kernel(ExtraCameras ec, int64_t n, RasterInputs in) {
     extern __shared__ float sh_smem[];             // [warps][32 * kShRow]
     __shared__ CameraDev cams[kMaxExtraCameras];
@@ -165,7 +169,7 @@ __global__ void __launch_bounds__(256) project_cameras_kernel(ExtraCameras ec, i
     const int64_t g0 = (int64_t)blockIdx.x * blockDim.x + warp * 32;
     const int cnt = (int)(n - g0 < 32 ? (n - g0 > 0 ? n - g0 : 0) : 32);
     if (cnt == 0) return;                          // whole warp
-    in.sh.stage_warp(g0, cnt, lane, ld);
+    in.sh.stage_warp<FULL>(g0, cnt, lane, ld);
     __syncwarp();
     if (lane >= cnt) return;
     const int64_t gi = g0 + lane;
@@ -189,16 +193,18 @@ cudaError_t launch_project_cameras(const ExtraCameras& ec, int64_t n, const Rast
     if (n == 0 || ec.count == 0) return cudaSuccess;
     constexpr int kThreads = 256;
     const size_t smem = (size_t)(kThreads / 32) * 32 * kShRow * sizeof(float);   // 49 KB: SH staging
-    cudaError_t e = cudaFuncSetAttribute(project_cameras_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    auto kernel = in.sh.m == kShCoeffs ? project_cameras_kernel<true> : project_cameras_kernel<false>;
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    return launch_k(project_cameras_kernel, dim3((unsigned)((n + kThreads - 1) / kThreads)), dim3(kThreads), smem, st, true, ec, n, in);
+    return launch_k(kernel, dim3((unsigned)((n + kThreads - 1) / kThreads)), dim3(kThreads), smem, st, true, ec, n, in);
 }
 
 // ------------------------------------------------------------------------------------------------------
 // Persistent kernel: one CTA per SM, each looping over tiles of TG Gaussians whose HexPlane features feat [N][F] the gather
 // wrote (an ordinary launch: the gather has completed).
 //   MODE 0: deformation network only (drop-in for deform_network.forward; outputs pre-activation tensors)
-//   MODE 1: fused deformation + activations + projection (the render() hot path)
+//   MODE 1: fused deformation + activations + projection (the render() hot path), M = 16 SH coefficients per Gaussian
+//   MODE 2: MODE 1 for models with M = io.sh.m < 16 (no SHS head)
 template <int TG, int WD, int MODE>
 __global__ void __launch_bounds__(kDeformThreads, 1)
 deform_kernel(DeformDesc d, DeformSmem L, const CameraDev* __restrict__ camp, int64_t n, const float* __restrict__ feat, DeformIO io) {
@@ -206,7 +212,7 @@ deform_kernel(DeformDesc d, DeformSmem L, const CameraDev* __restrict__ camp, in
     __shared__ CameraDev cam;
     const int tid = threadIdx.x;
     const int64_t ntiles = (n + TG - 1) / TG;
-    if (MODE == 1) stage_cameras(&cam, &camp, 1);
+    if (MODE != 0) stage_cameras(&cam, &camp, 1);
     stage_persistent_weights(d, L, smem);
     void* bar = smem + L.mbar;
     if (tid == 0) { mbar_init(bar, 1); fence_barrier_init(); }
@@ -260,7 +266,7 @@ deform_kernel(DeformDesc d, DeformSmem L, const CameraDev* __restrict__ camp, in
                 for (int i = tid; i < TG * 48; i += kDeformThreads)
                     if (i < rem * 48) {
                         const int g = i / 48, c = i - 48 * g;
-                        io.fo.shs[base * 48 + i] = io.sh.at(base + g, c) + out[g * 60 + 11 + c];
+                        io.fo.shs[base * 48 + i] = io.sh.at<true>(base + g, c) + out[g * 60 + 11 + c];   // (SHS head: M = 16)
                     }
             }
             if (tid < TG && tid < rem) {
@@ -276,7 +282,7 @@ deform_kernel(DeformDesc d, DeformSmem L, const CameraDev* __restrict__ camp, in
                 if (hr) { q[0] += o[6]; q[1] += o[7]; q[2] += o[8]; q[3] += o[9]; }
                 if (ho) ol += o[10];
                 const float* dsh = o + 11;
-                fused_finish(cam, io, gi, p, sl, q, ol, [&](int i) { return hsh ? dsh[i] : 0.f; });
+                fused_finish<MODE == 1>(cam, io, gi, p, sl, q, ol, [&](int i) { return hsh ? dsh[i] : 0.f; });
             }
         }
         __syncthreads();
@@ -328,18 +334,22 @@ cudaError_t launch_deform(const DeformDesc& d, int mode, const CameraDev* cam, i
         t.feat = gather.feat; t.order = gather.order;
         return launch_deform_tc(d, t, mode, cam, n, io, sm_count, st);
     }
+    const bool full = io.sh.m == kShCoeffs;
     if (d.WD == 128) {
         return mode == 0 ? launch_deform_tiles<64, 128, 0>(d, cam, n, gather.feat, io, sm_count, st)
-                         : launch_deform_tiles<64, 128, 1>(d, cam, n, gather.feat, io, sm_count, st);
+             : full      ? launch_deform_tiles<64, 128, 1>(d, cam, n, gather.feat, io, sm_count, st)
+                         : launch_deform_tiles<64, 128, 2>(d, cam, n, gather.feat, io, sm_count, st);
     } else if (d.WD == 64) {
         return mode == 0 ? launch_deform_tiles<128, 64, 0>(d, cam, n, gather.feat, io, sm_count, st)
-                         : launch_deform_tiles<128, 64, 1>(d, cam, n, gather.feat, io, sm_count, st);
+             : full      ? launch_deform_tiles<128, 64, 1>(d, cam, n, gather.feat, io, sm_count, st)
+                         : launch_deform_tiles<128, 64, 2>(d, cam, n, gather.feat, io, sm_count, st);
     }
     return cudaErrorInvalidValue;
 }
 
 // ------------------------------------------------------------------------------------------------------
-// "coarse" stage of render() (gaussian_renderer/__init__.py:80-81): the fused tail with no network deltas.
+// "coarse" stage of render() (gaussian_renderer/__init__.py:80-81): the fused tail with no network deltas.  FULL: M = 16.
+template <bool FULL>
 __global__ void __launch_bounds__(256) activate_preprocess_kernel(const CameraDev* __restrict__ camp, int64_t n, DeformIO io) {
     __shared__ CameraDev cam;
     stage_cameras(&cam, &camp, 1);
@@ -351,12 +361,14 @@ __global__ void __launch_bounds__(256) activate_preprocess_kernel(const CameraDe
     const float4 q4 = *reinterpret_cast<const float4*>(io.rotation + 4 * gi);
     const float q[4] = {q4.x, q4.y, q4.z, q4.w};
     // a delta of -0.f leaves every coefficient as it is (x + -0 == x, also for x = +0), so the add compiles away
-    fused_finish(cam, io, gi, p, sl, q, io.opacity[gi], [](int) { return -0.f; });
+    fused_finish<FULL>(cam, io, gi, p, sl, q, io.opacity[gi], [](int) { return -0.f; });
 }
 
 cudaError_t launch_activate_preprocess(const CameraDev* cam, int64_t n, const DeformIO& io, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
-    activate_preprocess_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(cam, n, io);
+    const unsigned blocks = (unsigned)((n + 255) / 256);
+    if (io.sh.m == kShCoeffs) activate_preprocess_kernel<true><<<blocks, 256, 0, st>>>(cam, n, io);
+    else activate_preprocess_kernel<false><<<blocks, 256, 0, st>>>(cam, n, io);
     return cudaGetLastError();
 }
 

@@ -113,19 +113,26 @@ struct ImageBuffers {
 // The accessors only move data: they are shared by units compiled with and without FMA contraction.
 constexpr int kShRow = 49;   // floats per Gaussian in a warp's shared-memory SH rows: lane i <-> row i is bank-conflict free
 
-// A Gaussian's 16 x 3 coefficients, fused [N,16,3] in shs, or (shs == NULL) split into dc [N,1,3] + rest [N,15,3]
+// A Gaussian's M x 3 coefficients (M = (max degree + 1)^2: 1, 4, 9 or 16), fused [N,M,3] in shs, or (shs == NULL) split into
+// dc [N,1,3] + rest [N,M-1,3].  Only coefficients k < M exist; the colour reads k < (active degree + 1)^2 <= M.
+// FULL (the accessors' template argument): M = 16 known at compile time, so that the degree-3 kernels keep constant strides;
+// otherwise M = m at run time.  At M = 1 the two layouts are the same [N,1,3] tensor: rest is never read.
 struct ShIn {
     const float *shs, *dc, *rest;
-    // coefficient e = 3 * k + ch of Gaussian gi
-    G4D_D float at(int64_t gi, int e) const {
-        return shs ? __ldg(shs + gi * 48 + e) : e < 3 ? __ldg(dc + gi * 3 + e) : __ldg(rest + gi * 45 + (e - 3));
+    int m = kShCoeffs;
+    template <bool FULL> G4D_D int coeffs() const { return FULL ? kShCoeffs : m; }
+    // coefficient e = 3 * k + ch of Gaussian gi, e < 3M
+    template <bool FULL> G4D_D float at(int64_t gi, int e) const {
+        const int s = 3 * coeffs<FULL>();
+        return shs ? __ldg(shs + gi * s + e) : e < 3 ? __ldg(dc + gi * 3 + e) : __ldg(rest + gi * (s - 3) + (e - 3));
     }
     // f(load) with load(k, ch) -> coefficient k, channel ch of Gaussian gi; the layout is chosen once, outside f
-    template <class F> G4D_D void with_coeffs(int64_t gi, F&& f) const {
-        if (shs) f([=](int k, int ch) { return __ldg(shs + gi * 48 + 3 * k + ch); });
-        else f([=](int k, int ch) { return k == 0 ? __ldg(dc + gi * 3 + ch) : __ldg(rest + gi * 45 + 3 * (k - 1) + ch); });
+    template <bool FULL, class F> G4D_D void with_coeffs(int64_t gi, F&& f) const {
+        const int s = 3 * coeffs<FULL>();
+        if (shs) f([=](int k, int ch) { return __ldg(shs + gi * s + 3 * k + ch); });
+        else f([=](int k, int ch) { return k == 0 ? __ldg(dc + gi * 3 + ch) : __ldg(rest + gi * (s - 3) + 3 * (k - 1) + ch); });
     }
-    // all 48 into registers (float4 loads on the fused layout); v[3 * k + ch]
+    // all 48 of a Gaussian with M = 16 into registers (float4 loads on the fused layout); v[3 * k + ch]
     G4D_D void load(int64_t gi, float (&v)[48]) const {
         if (shs) {
 #pragma unroll
@@ -140,26 +147,29 @@ struct ShIn {
             for (int j = 0; j < 45; ++j) v[3 + j] = __ldg(rest + gi * 45 + j);
         }
     }
-    // warp-wide: Gaussians g0 .. g0 + cnt - 1 into rows[i * kShRow + 3 * k + ch], read as contiguous 128-byte lines
-    G4D_D void stage_warp(int64_t g0, int cnt, int lane, float* rows) const {
-        for (int idx = lane; idx < cnt * 48; idx += 32) {
-            const int i = idx / 48, e = idx - i * 48;
-            rows[i * kShRow + e] = at(g0 + i, e);
+    // warp-wide: Gaussians g0 .. g0 + cnt - 1 into rows[i * kShRow + 3 * k + ch] for k < M, read as contiguous 128-byte lines
+    template <bool FULL> G4D_D void stage_warp(int64_t g0, int cnt, int lane, float* rows) const {
+        const int s = 3 * coeffs<FULL>();
+        for (int idx = lane; idx < cnt * s; idx += 32) {
+            const int i = idx / s, e = idx - i * s;
+            rows[i * kShRow + e] = at<FULL>(g0 + i, e);
         }
     }
 };
 
-// gradient sinks of the coefficients; each may be NULL, and the fused and the split sinks may both be given
+// gradient sinks of the M coefficients (layouts as ShIn's); each may be NULL, and the fused and the split sinks may both be given
 struct ShOut {
     float *shs, *dc, *rest;
+    int m = kShCoeffs;
     // warp-wide: the inverse of ShIn::stage_warp
-    G4D_D void store_warp(int64_t g0, int cnt, int lane, const float* rows) const {
-        for (int idx = lane; idx < cnt * 48; idx += 32) {
-            const int i = idx / 48, e = idx - i * 48;
+    template <bool FULL> G4D_D void store_warp(int64_t g0, int cnt, int lane, const float* rows) const {
+        const int s = 3 * (FULL ? kShCoeffs : m);
+        for (int idx = lane; idx < cnt * s; idx += 32) {
+            const int i = idx / s, e = idx - i * s;
             const float v = rows[i * kShRow + e];
-            if (shs) shs[g0 * 48 + idx] = v;
+            if (shs) shs[g0 * s + idx] = v;
             if (e < 3) { if (dc) dc[(g0 + i) * 3 + e] = v; }
-            else if (rest) rest[(g0 + i) * 45 + (e - 3)] = v;
+            else if (rest) rest[(g0 + i) * (s - 3) + (e - 3)] = v;
         }
     }
 };

@@ -57,7 +57,8 @@ G4D_D void store_saved(const FusedOutputs& fo, int64_t gi, Vec3 p, const Activat
 
 // p, sl (log-scale), q (raw quaternion), ol (opacity logit) already include the network's deltas.
 // ShDelta: float operator()(int flat_index in [0,48)) -> delta of SH coefficient (0 when the SHS head is inactive).
-template <class ShDelta>
+// FULL: io.sh holds M = 16 coefficients, known at compile time (constant strides); else M = io.sh.m.
+template <bool FULL, class ShDelta>
 G4D_D void fused_finish(const CameraDev& cam, const DeformIO& io, int64_t gi, Vec3 p, const float sl[3], const float q[4], float ol,
                         ShDelta dsh) {
     const Activated a = activate(sl, q, ol);
@@ -66,7 +67,7 @@ G4D_D void fused_finish(const CameraDev& cam, const DeformIO& io, int64_t gi, Ve
     float rgb[3] = {0.f, 0.f, 0.f};
     uint32_t bits = 0;
     if (ok)
-        io.sh.with_coeffs(gi, [&](auto sh) {
+        io.sh.with_coeffs<FULL>(gi, [&](auto sh) {
             sh_to_rgb(cam, p, [&](int k, int ch) { return sh(k, ch) + dsh(3 * k + ch); }, rgb, bits);
         });
     store_projected(io.g, gi, ok, pr, a.op, rgb, bits, io.out_radii);
@@ -88,8 +89,15 @@ G4D_D void fused_finish_geometry(const CameraDev& cam, const DeformIO& io, int64
     store_saved(io.fo, gi, p, a);
 }
 
+// the colour fields of the record (rec1.zw, rec2.x, clamped)
+G4D_D void store_colour(const GeomBuffers& g, int64_t gi, const float rgb[3], uint32_t bits) {
+    *reinterpret_cast<float2*>(reinterpret_cast<float*>(&g.rec1[gi]) + 2) = make_float2(rgb[0], rgb[1]);
+    g.rec2[gi].x = rgb[2];
+    g.clamped[gi] = (uint8_t)bits;
+}
+
 // dsh[48]: deltas of the SH coefficients (zeros when the SHS head is inactive); indices are compile-time after
-// unrolling, so dsh stays in registers.
+// unrolling, so dsh stays in registers.  M = 16 coefficients per Gaussian.
 G4D_D void fused_finish_colour(const CameraDev& cam, const DeformIO& io, int64_t gi, Vec3 p, bool hsh, const float (&dsh)[48]) {
     float sh[48];
     io.sh.load(gi, sh);
@@ -102,10 +110,15 @@ G4D_D void fused_finish_colour(const CameraDev& cam, const DeformIO& io, int64_t
     float rgb[3];
     uint32_t bits;
     sh_to_rgb<true>(cam, p, [&](int k, int ch) { return sh[3 * k + ch]; }, rgb, bits);
-    const GeomBuffers& g = io.g;
-    *reinterpret_cast<float2*>(reinterpret_cast<float*>(&g.rec1[gi]) + 2) = make_float2(rgb[0], rgb[1]);
-    g.rec2[gi].x = rgb[2];
-    g.clamped[gi] = (uint8_t)bits;
+    store_colour(io.g, gi, rgb, bits);
+}
+
+// The same for a model with M = io.sh.m < 16 coefficients (no SHS head, so no deltas): read from memory, M at run time.
+G4D_D void fused_finish_colour_reduced(const CameraDev& cam, const DeformIO& io, int64_t gi, Vec3 p) {
+    float rgb[3];
+    uint32_t bits;
+    io.sh.with_coeffs<false>(gi, [&](auto sh) { sh_to_rgb(cam, p, sh, rgb, bits); });
+    store_colour(io.g, gi, rgb, bits);
 }
 
 }  // namespace g4d

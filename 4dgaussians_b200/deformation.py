@@ -394,6 +394,8 @@ class _DeformFunction(torch.autograd.Function):
         needs_bwd = grad_mode and any(ctx.needs_input_grad)      # (grad mode is always off INSIDE Function.forward)
         prm = module.c_params(keep, fresh=needs_bwd)
         hm = prm.head_mask
+        if sh is not None and (hm & _lib.HEAD_SHS):     # the SH head deforms exactly 16 coefficients per Gaussian
+            _lib.check_sh_degree(_lib.sh_coeffs(sh, n, "shs"), 0, hm)
         ox = torch.empty_like(x)
         os_ = torch.empty_like(s) if s is not None else None
         orr = torch.empty_like(r) if r is not None else None

@@ -63,6 +63,8 @@ class GraphedRender:
         if any(a.data_ptr() != b.data_ptr() for a, b in zip(staged, self._tensors)):
             raise ValueError("a graphed render reads the model's tensors in place: they must be contiguous fp32 CUDA tensors")
         self._ptrs = tuple(t.data_ptr() for t in self._tensors)
+        m = _lib.sh_coeffs(pc._features_rest, n, "features_rest", skip=1)
+        _lib.check_sh_degree(m, self.sh_degree, module.head_mask() if module is not None else 0)
         self._bg = _lib.cuda_f32(bg_color, "bg", 3)
 
         self.ws = _lib.Workspace(dev.index)
@@ -80,7 +82,8 @@ class GraphedRender:
         for c in self.ctxs:
             c.set_time_source(d_time)
 
-        self._cams = (_lib.Camera * k)(*[camera_from_settings(rs._replace(bg=self._bg)) for rs, _ in settings])
+        self._cams = (_lib.Camera * k)(*[camera_from_settings(rs._replace(bg=self._bg), sh_coeffs=m)
+                                          for rs, _ in settings])
         for i, cam in enumerate(self._cams):      # the view matrices and camera centre: read from the staging block's copy
             cam.debug = _lib.CAM_NO_GRAD
             off = base + i * _VIEW_FLOATS * fsz

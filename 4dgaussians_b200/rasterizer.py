@@ -31,12 +31,12 @@ class GaussianRasterizationSettings(NamedTuple):
     debug: bool
 
 
-def camera_from_settings(rs: GaussianRasterizationSettings, time: float = 0.0, keep=None) -> _lib.Camera:
-    """Build the C-ABI camera.  Matrices given as CUDA tensors stay on the device (no D2H sync);
-    CPU tensors are copied into the struct."""
+def camera_from_settings(rs: GaussianRasterizationSettings, time: float = 0.0, keep=None, sh_coeffs: int = 16) -> _lib.Camera:
+    """Build the C-ABI camera; sh_coeffs: M, the SH coefficients per Gaussian of the tensors it renders.  Matrices given as
+    CUDA tensors stay on the device (no D2H sync); CPU tensors are copied into the struct."""
     cam = _lib.Camera()
     cam.image_height, cam.image_width = int(rs.image_height), int(rs.image_width)
-    cam.sh_degree, cam.debug = int(rs.sh_degree), int(bool(rs.debug))
+    cam.sh_degree, cam.debug, cam.sh_coeffs = int(rs.sh_degree), int(bool(rs.debug)), int(sh_coeffs)
     cam.tanfovx, cam.tanfovy, cam.scale_modifier, cam.time = float(rs.tanfovx), float(rs.tanfovy), \
         float(rs.scale_modifier), float(time)
     for name, field, dfield, n in (("viewmatrix", "viewmatrix", "d_viewmatrix", 16), ("projmatrix", "projmatrix", "d_projmatrix", 16),
@@ -83,7 +83,9 @@ class _RasterizeGaussians(torch.autograd.Function):
         dev = means3D.device
         n = means3D.shape[0]
         m3 = _lib.cuda_f32(means3D, "means3D", n * 3)
-        shc = _lib.cuda_f32(sh, "shs", n * 48)
+        m = _lib.sh_coeffs(sh, n, "shs")
+        _lib.check_sh_degree(m, int(raster_settings.sh_degree))
+        shc = _lib.cuda_f32(sh, "shs", n * 3 * m)
         op = _lib.cuda_f32(opacities, "opacities", n)
         sc = _lib.cuda_f32(scales, "scales", n * 3)
         ro = _lib.cuda_f32(rotations, "rotations", n * 4)
@@ -92,7 +94,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         depth = torch.empty(1, H, W, device=dev, dtype=torch.float32)
         radii = torch.empty(n, device=dev, dtype=torch.int32)
         keep = []
-        cam = camera_from_settings(raster_settings, keep=keep)
+        cam = camera_from_settings(raster_settings, keep=keep, sh_coeffs=m)
         with torch.cuda.device(dev):
             lease = _ContextLease(_lib.workspace_of(dev))
             _lib.check(lib.g4d_rasterize_forward(lease.ctx.handle, C.byref(cam), n, m3.data_ptr(), shc.data_ptr(), op.data_ptr(),
@@ -100,7 +102,7 @@ class _RasterizeGaussians(torch.autograd.Function):
                                                  radii.data_ptr(), _lib.stream_of(dev)), "g4d_rasterize_forward")
         ctx.raster_settings = raster_settings
         ctx.lease = lease
-        ctx.n = n
+        ctx.n, ctx.m = n, m
         ctx.save_for_backward(m3, shc, op, sc, ro)
         ctx.mark_non_differentiable(radii, depth)
         return color, radii, depth
@@ -115,12 +117,12 @@ class _RasterizeGaussians(torch.autograd.Function):
         gcol = _lib.cuda_f32(grad_color, "grad_out_color", 3 * int(rs.image_height) * int(rs.image_width))
         g_means3D = torch.empty(n, 3, device=dev)
         g_means2D = torch.empty(n, 3, device=dev)
-        g_sh = torch.empty(n, 16, 3, device=dev)
+        g_sh = torch.empty(n, ctx.m, 3, device=dev)
         g_op = torch.empty(n, 1, device=dev)
         g_sc = torch.empty(n, 3, device=dev)
         g_ro = torch.empty(n, 4, device=dev)
         keep = []
-        cam = camera_from_settings(rs, keep=keep)
+        cam = camera_from_settings(rs, keep=keep, sh_coeffs=ctx.m)
         lease = ctx.lease
         if lease is None or lease.ctx is None:
             raise RuntimeError("rasterizer backward called twice (context already released)")

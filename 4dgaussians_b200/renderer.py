@@ -50,17 +50,21 @@ def _fused_forward(module: Optional[deform_network], rss, t, needs_bwd, xyz, sca
     n, k = xyz.shape[0], len(rss)
     x, s = _lib.cuda_f32(xyz, "xyz", n * 3), _lib.cuda_f32(scaling, "scaling", n * 3)
     r, o = _lib.cuda_f32(rotation, "rotation", n * 4), _lib.cuda_f32(opacity, "opacity", n)
-    dc, rest = _lib.cuda_f32(f_dc, "features_dc", n * 3), _lib.cuda_f32(f_rest, "features_rest", n * 45)
+    m = _lib.sh_coeffs(f_rest, n, "features_rest", skip=1)
+    _lib.check_sh_degree(m, int(rss[0].sh_degree), module.head_mask() if module is not None else 0)
+    dc, rest = _lib.cuda_f32(f_dc, "features_dc", n * 3), _lib.cuda_f32(f_rest, "features_rest", n * 3 * (m - 1))
     colors = [torch.empty(3, int(rs.image_height), int(rs.image_width), device=dev, dtype=torch.float32) for rs in rss]
     depths = [torch.empty(1, int(rs.image_height), int(rs.image_width), device=dev, dtype=torch.float32) for rs in rss]
     radii = [torch.empty(n, device=dev, dtype=torch.int32) for _ in rss]
     keep = []
-    cams = [camera_from_settings(rs, time=t, keep=keep) for rs in rss]
+    cams = [camera_from_settings(rs, time=t, keep=keep, sh_coeffs=m) for rs in rss]
     if not needs_bwd:
         for cam in cams:
             cam.debug |= _lib.CAM_NO_GRAD      # torch.no_grad() rendering: nothing is saved for a backward
     # training forwards rebuild the packed weight images (fused optimizers do not bump Tensor._version)
     prm = module.c_params(keep, fresh=needs_bwd) if module is not None else None
+    # at M = 1 rest is empty and its data_ptr() may be 0: the library then takes the fused layout [N,M,3] in dc, which at
+    # M = 1 is the same tensor as the split dc [N,1,3] (include/g4d.h, G4DGaussians)
     g = _lib.Gaussians(n, x.data_ptr(), s.data_ptr(), r.data_ptr(), o.data_ptr(), dc.data_ptr(), rest.data_ptr())
     with torch.cuda.device(dev):
         ws = _lib.workspace_of(dev)
@@ -119,13 +123,15 @@ class _FusedRender(torch.autograd.Function):
             prm = module.c_params(keep, fresh=True)
         cg, pgrads = module.c_grad_sinks() if module is not None else (None, [])
         # one allocation for the per-Gaussian gradients, every segment 16-byte aligned: xyz, scaling, rotation, opacity,
-        # features_dc, features_rest, then means2D of each camera
+        # features_dc, features_rest (M - 1 coefficients), then means2D of each camera: 11 + 3M + 3k floats per Gaussian
         npad = (n + 3) // 4 * 4
-        flat = torch.empty(npad * (59 + 3 * k), device=dev, dtype=torch.float32)
+        m = cams.sh_coeffs if k == 1 else cams[0].sh_coeffs
+        end = 11 + 3 * m
+        flat = torch.empty(npad * (end + 3 * k), device=dev, dtype=torch.float32)
         gx, gs, gr, go, gdc, grest = (flat[a * npad:a * npad + w * n].view(shape) for a, w, shape in
                                       ((0, 3, (n, 3)), (3, 3, (n, 3)), (6, 4, (n, 4)), (10, 1, (n, 1)), (11, 3, (n, 1, 3)),
-                                       (14, 45, (n, 15, 3))))
-        gm2 = [flat[(59 + 3 * i) * npad:(59 + 3 * i) * npad + 3 * n].view(n, 3) for i in range(k)]
+                                       (14, 3 * (m - 1), (n, m - 1, 3))))
+        gm2 = [flat[(end + 3 * i) * npad:(end + 3 * i) * npad + 3 * n].view(n, 3) for i in range(k)]
         gg = _lib.GaussianGrads(gx.data_ptr(), gs.data_ptr(), gr.data_ptr(), go.data_ptr(), gdc.data_ptr(), grest.data_ptr(),
                                 gm2[0].data_ptr() if k == 1 else None)
         with torch.cuda.device(dev):

@@ -95,15 +95,16 @@ def orbit_cameras(count: int, width: int, height: int, *, radius: float = 4.0, f
     return cams
 
 
-def make_scene(n: int, seed: int = 0, scale_mean: float = 0.02, extent: float = 1.3) -> Dict[str, torch.Tensor]:
-    """CPU fp32 tensors with the layouts GaussianModel holds (SURVEY §8a1)."""
+def make_scene(n: int, seed: int = 0, scale_mean: float = 0.02, extent: float = 1.3, sh_degree: int = 3) -> Dict[str, torch.Tensor]:
+    """CPU fp32 tensors with the layouts GaussianModel holds (SURVEY §8a1); features_rest [N, (sh_degree + 1)^2 - 1, 3]: the
+    first coefficients of the degree-3 scene of the same seed."""
     g = torch.Generator().manual_seed(seed)
     xyz = (torch.rand(n, 3, generator=g) * 2 - 1) * extent
     scaling = torch.log(scale_mean * torch.exp(0.5 * torch.randn(n, 3, generator=g)))
     rotation = torch.randn(n, 4, generator=g)
     opacity = torch.logit(0.05 + 0.9 * torch.rand(n, 1, generator=g))
     features_dc = ((torch.rand(n, 1, 3, generator=g) - 0.5) / 0.28209479177387814)
-    features_rest = torch.randn(n, 15, 3, generator=g) * 0.05
+    features_rest = (torch.randn(n, 15, 3, generator=g) * 0.05)[:, :(sh_degree + 1) ** 2 - 1].contiguous()
     aabb = torch.stack([xyz.max(dim=0).values, xyz.min(dim=0).values]) if n > 0 else \
         torch.tensor([[extent] * 3, [-extent] * 3])
     return {"xyz": xyz, "scaling": scaling, "rotation": rotation, "opacity": opacity,
@@ -136,7 +137,7 @@ class SyntheticGaussianModel:
         self._deformation = deformation
         self._deformation_table = torch.ones(self._xyz.shape[0], dtype=torch.bool, device=device)
         self.active_sh_degree = sh_degree
-        self.max_sh_degree = 3
+        self.max_sh_degree = int(round(math.sqrt(self._features_rest.shape[1] + 1))) - 1
         self.scaling_activation = torch.exp
         self.opacity_activation = torch.sigmoid
         self.rotation_activation = torch.nn.functional.normalize

@@ -161,14 +161,20 @@ class FlatState:
 
 
 class GaussianSet:
-    """The GaussianModel tensors render() reads + the densification bookkeeping (scene/gaussian_model.py:46-131, 165-170)."""
+    """The GaussianModel tensors render() reads + the densification bookkeeping (scene/gaussian_model.py:46-131, 165-170).
 
-    def __init__(self, tensors: Dict[str, torch.Tensor], deformation, device="cuda", sh_degree: int = 3):
+    max_sh_degree comes from the tensors: features_rest is [N, (max_sh_degree + 1)^2 - 1, 3].  sh_degree: the active degree
+    (None: the maximum), raised by ``oneupSHdegree`` up to the maximum."""
+
+    def __init__(self, tensors: Dict[str, torch.Tensor], deformation, device="cuda", sh_degree: Optional[int] = None):
         mk = lambda t: nn.Parameter(t.detach().to(device).float().contiguous(), requires_grad=True)
         self._xyz, self._features_dc, self._features_rest = mk(tensors["xyz"]), mk(tensors["features_dc"]), mk(tensors["features_rest"])
         self._opacity, self._scaling, self._rotation = mk(tensors["opacity"]), mk(tensors["scaling"]), mk(tensors["rotation"])
         self._deformation = deformation
-        self.active_sh_degree, self.max_sh_degree = sh_degree, 3
+        m = _lib.sh_coeffs(self._features_rest, self._xyz.shape[0], "features_rest", skip=1)
+        self.max_sh_degree = _lib.SH_COEFFS.index(m)
+        self.active_sh_degree = self.max_sh_degree if sh_degree is None else int(sh_degree)
+        _lib.check_sh_degree(m, self.active_sh_degree)
         self.scaling_activation, self.opacity_activation = torch.exp, torch.sigmoid
         self.rotation_activation = torch.nn.functional.normalize
         self.reset_stats()
@@ -180,6 +186,11 @@ class GaussianSet:
         self.max_radii2D = torch.zeros(n, device=dev)
         self._deformation_table = torch.ones(n, dtype=torch.bool, device=dev)
         self._deformation_accum = torch.zeros(n, 3, device=dev)
+
+    def oneupSHdegree(self):
+        """gaussian_model.py:133-135"""
+        if self.active_sh_degree < self.max_sh_degree:
+            self.active_sh_degree += 1
 
     @property
     def get_xyz(self):

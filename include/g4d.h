@@ -73,6 +73,11 @@ typedef struct G4DCamera {
     /* optional DEVICE sources; when non-NULL they override the host arrays above (the reference
      * passes these four as CUDA tensors) */
     const float *d_viewmatrix, *d_projmatrix, *d_campos, *d_bg;
+    /* SH coefficients M = (max_sh_degree + 1)^2 every Gaussian stores (sh.size(1) upstream): 1, 4, 9 or 16; 0 means 16, so a
+     * zero-filled tail is the degree-3 model.  (sh_degree + 1)^2 <= M; the SHS head of the network needs M = 16; the cameras
+     * of one g4d_render_*_cameras call share M.  Otherwise G4D_ERR_ARG before any launch. */
+    int32_t sh_coeffs;
+    int32_t reserved;
 } G4DCamera;
 
 typedef struct G4DDeformParams {
@@ -116,7 +121,9 @@ typedef struct G4DGaussians {
     const float *rotation;      /* [N,4] raw quaternion, w first */
     const float *opacity;       /* [N,1] logit */
     const float *features_dc;   /* [N,1,3] */
-    const float *features_rest; /* [N,15,3]; NULL => features_dc points at a fused [N,16,3] tensor */
+    const float *features_rest; /* [N,M-1,3] (M: G4DCamera.sh_coeffs); NULL => features_dc points at a fused [N,M,3] tensor.
+                                 * At M = 1 the two layouts are the same [N,1,3] in features_dc and features_rest is not read
+                                 * (it may be NULL: an empty tensor's data pointer) */
 } G4DGaussians;
 
 typedef struct G4DGaussianGrads { /* device, OVERWRITTEN */
@@ -141,7 +148,8 @@ void g4d_context_destroy(G4DContext *ctx);
 int g4d_context_stats(G4DContext *ctx, G4DStats *out);
 
 /* ---- deformation network (drop-in for deform_network.forward) ----------------------------------
- * shs may be NULL when the SHS head is inactive (then out_shs is not written). Outputs are the
+ * shs may be NULL when the SHS head is inactive (then out_shs is not written).  With the SHS head active, shs / out_shs (and
+ * g_out_shs / g_in_shs of the backward) are [N,16,3]: these entry points take no G4DCamera, so no other M.  Outputs are the
  * PRE-activation tensors, same shapes as the inputs. */
 int g4d_deform_forward(G4DWorkspace *ws, const G4DDeformParams *prm, int64_t n, const float *xyz,
                        const float *scaling, const float *rotation, const float *opacity, const float *shs,
@@ -161,13 +169,14 @@ int g4d_deform_backward(G4DWorkspace *ws, const G4DDeformParams *prm, G4DDeformG
 #define G4D_RELU_BITS_WORDS(n) ((size_t)24 * (size_t)(n) + 4) /* [6 layers][n][4 words] + validity tag */
 
 /* ---- rasterizer (drop-in for GaussianRasterizer) ------------------------------------------------
- * Inputs are POST-activation (scales = exp, rotations normalised, opacities = sigmoid), shs [N,16,3].
+ * Inputs are POST-activation (scales = exp, rotations normalised, opacities = sigmoid), shs [N,M,3] (M: cam->sh_coeffs).
  * out_color [3,H,W], out_depth [1,H,W], out_radii [N] int32. */
 int g4d_rasterize_forward(G4DContext *ctx, const G4DCamera *cam, int64_t n, const float *means3D,
                           const float *shs, const float *opacities, const float *scales, const float *rotations,
                           float *out_color, float *out_depth, int32_t *out_radii, void *stream);
-/* all g_* OVERWRITTEN: g_means3D [N,3], g_means2D [N,3], g_shs [N,16,3], g_opacities [N,1], g_scales [N,3],
- * g_rotations [N,4] */
+/* all g_* OVERWRITTEN: g_means3D [N,3], g_means2D [N,3], g_shs [N,M,3], g_opacities [N,1], g_scales [N,3],
+ * g_rotations [N,4].  The gradients of coefficients >= (sh_degree + 1)^2 are 0.  A backward whose M differs from its
+ * forward's returns G4D_ERR_STATE (also g4d_render_backward(_cameras)). */
 int g4d_rasterize_backward(G4DContext *ctx, const G4DCamera *cam, int64_t n, const float *means3D,
                            const float *shs, const float *opacities, const float *scales, const float *rotations,
                            const float *dL_dcolor, float *g_means3D, float *g_means2D, float *g_shs,
