@@ -329,6 +329,25 @@ int check_params(const G4DDeformParams* p) {
     for (int l = 0; l < p->levels; ++l)
         for (int a = 0; a < 4; ++a)
             if (p->res[l][a] < 2 || p->res[l][a] > 65535) return fail(G4D_ERR_ARG, "plane resolution out of range");
+    for (int l = 0; l < p->levels; ++l)
+        for (int k = 0; k < 6; ++k) {
+            // hexplane.cuh addresses a plane with 32-bit offsets: its scatter indexes floats, (Y*W + X)*C + c < 2^31
+            if ((int64_t)p->res[l][plane_axis0(k)] * p->res[l][plane_axis1(k)] * p->channels >= (1ll << 31))
+                return fail(G4D_ERR_ARG, "a plane has H*W*channels >= 2^31 floats: hexplane.cuh's 32-bit offsets cannot address it");
+            // the gather reads the spatial planes' channel vectors as float4 (the time planes: scalar reads of the collapse)
+            if (plane_axis1(k) != 3 && ((uintptr_t)p->planes[l][k] & 15u))
+                return fail(G4D_ERR_ARG, "spatial planes must be 16-byte aligned");
+        }
+    return G4D_OK;
+}
+
+// The spatial-plane gradient sinks of the levels prm uses, which the network backward's scatter adds channel vectors to with
+// red.v4.  (The time-plane sinks take the scalar atomics of the time-row distribution, the regulariser's sinks scalar adds.)
+int check_plane_grads(const G4DDeformParams* p, const G4DDeformGrads* g) {
+    for (int l = 0; l < p->levels; ++l)
+        for (int k = 0; k < 6; ++k)
+            if (plane_axis1(k) != 3 && ((uintptr_t)g->planes[l][k] & 15u))
+                return fail(G4D_ERR_ARG, "spatial-plane gradient sinks must be 16-byte aligned (the scatter adds float4s)");
     return G4D_OK;
 }
 
@@ -923,6 +942,7 @@ int g4d_deform_backward(G4DWorkspace* ws, const G4DDeformParams* prm, G4DDeformG
     int rc = check_params(prm);
     if (rc != G4D_OK) return rc;
     if (!grads) return fail(G4D_ERR_ARG, "grads is NULL");
+    if ((rc = check_plane_grads(prm, grads)) != G4D_OK) return rc;
     if (n < 0 || (n > 0 && !xyz)) return fail(G4D_ERR_ARG, "xyz required");
     cudaStream_t st = (cudaStream_t)stream;
     G4D_CUDA(cudaSetDevice(ws->device));
@@ -1136,6 +1156,7 @@ int g4d_render_backward(G4DContext* c, const G4DCamera* cam, const G4DDeformPara
     if (prm && (rc = check_params(prm)) != G4D_OK) return rc;
     if ((rc = check_sh_head(cam, prm)) != G4D_OK) return rc;
     if (prm && !pgrads) return fail(G4D_ERR_ARG, "pgrads is NULL");
+    if (prm && (rc = check_plane_grads(prm, pgrads)) != G4D_OK) return rc;
     if (cam->image_height != c->fwd.H || cam->image_width != c->fwd.W) return fail(G4D_ERR_STATE, "camera differs from the forward's");
     if (sh_coeffs(cam) != c->fwd.sh_coeffs) return fail(G4D_ERR_STATE, "sh_coeffs differs from the forward's");
     const int64_t n = g->n;
@@ -1223,6 +1244,7 @@ int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCame
     if (prm && (rc = check_params(prm)) != G4D_OK) return rc;
     if ((rc = check_sh_head(&cams[0], prm)) != G4D_OK) return rc;
     if (prm && !pgrads) return fail(G4D_ERR_ARG, "pgrads is NULL");
+    if (prm && (rc = check_plane_grads(prm, pgrads)) != G4D_OK) return rc;
     const int64_t n = g->n;
     if (n > 0 && (!gg->xyz || !gg->scaling || !gg->rotation || !gg->opacity || !gg->features_dc))
         return fail(G4D_ERR_ARG, "NULL gradient pointer");

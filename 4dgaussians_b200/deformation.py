@@ -315,7 +315,9 @@ class deform_network(nn.Module):
     fused_grad_accumulation = False
 
     def grad_sinks(self) -> Optional[List[torch.Tensor]]:
-        """the parameters' own .grad tensors when fused accumulation is possible, else None"""
+        """the parameters' own .grad tensors when fused accumulation is possible, else None.  The plane scatter adds float4s,
+        so a spatial plane's .grad that is not 16-byte aligned (a view into a FlatGradBucket behind a parameter of 4k+1
+        floats, say) takes the staging path."""
         if not self.fused_grad_accumulation:
             return None
         flat = self.flat_parameters()
@@ -323,9 +325,12 @@ class deform_network(nn.Module):
         if cache is not None and len(cache[0]) == len(flat) and all(p.grad is g for p, g in zip(flat, cache[0])):
             return cache[0]                       # same .grad objects as last time: already validated
         out = []
-        for p in flat:
+        nplanes = len(self.deformation_net.grid.grids) * 6
+        for i, p in enumerate(flat):
             g = p.grad
             if g is None or g.dtype != torch.float32 or g.shape != p.shape or g.stride() != p.stride() or g.device != p.device:
+                return None
+            if i < nplanes and i % 6 in (0, 1, 3) and g.data_ptr() % 16:
                 return None
             out.append(g)
         self._sink_cache = [out, None]

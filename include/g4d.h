@@ -87,7 +87,8 @@ typedef struct G4DDeformParams {
     int32_t head_mask; /* G4D_HEAD_* bits */
     int32_t res[G4D_MAX_LEVELS][4]; /* per level: resolution of x, y, z, t */
     /* device: plane k of level l, CHANNEL-LAST [H][W][C]; (H,W) = (res[c1], res[c0]) for the k-th
-     * pair (c0,c1) of combinations(range(4),2)  (scene/hexplane.py:48-70) */
+     * pair (c0,c1) of combinations(range(4),2)  (scene/hexplane.py:48-70); H*W*C < 2^31, and the
+     * spatial planes (k = 0, 1, 3) 16-byte aligned (else G4D_ERR_ARG before any launch) */
     const float *planes[G4D_MAX_LEVELS][6];
     const float *aabb;      /* device [2][3]: row 0 = xyz_max, row 1 = xyz_min */
     const float *w0, *b0;   /* device: feature_out.0  [Wd][F], [Wd] */
@@ -104,7 +105,8 @@ typedef struct G4DDeformParams {
                                                                  * j = 1 .. depth-1 (non-NULL); the rest are not read */
 } G4DDeformParams;
 
-/* gradient sinks mirroring G4DDeformParams (device, same layouts; ACCUMULATED into, caller zeroes) */
+/* gradient sinks mirroring G4DDeformParams (device, same layouts; ACCUMULATED into, caller zeroes); the backward entry
+ * points need the spatial-plane sinks (k = 0, 1, 3) 16-byte aligned (else G4D_ERR_ARG before any launch) */
 typedef struct G4DDeformGrads {
     float *planes[G4D_MAX_LEVELS][6];
     float *w0, *b0;
