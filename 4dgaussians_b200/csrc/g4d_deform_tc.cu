@@ -18,7 +18,8 @@
 //   * weights are the B operand in shared memory: packed once per parameter version into the no-swizzle canonical K-major
 //     image (hi | lo), W0 and the SH head's W2 resident, W1 streamed head by head through a two-slot ring with TMA bulk
 //     copies and mbarriers (full: transaction count; empty: one arrival per consumer warp), one load ahead;
-//   * FP16x2 runs two warpgroups per CTA (128 Gaussians per W1 image load), 3xTF32 one (its A fragments take 128 registers);
+//   * FP16x2 runs three warpgroups per CTA (192 Gaussians per W1 image load) where their shared memory fits, else two
+//     (F = 48 / 64 with the SH head); 3xTF32 runs one (its A fragments take 128 registers);
 //   * layer 2 of the <= 4-wide heads runs in exact fp32 in the epilogue (each lane sums its 32 hidden units, a quad shuffle
 //     completes the row); the SH head's layer 2 (N = 48) is a fourth GEMM;
 //   * the per-Gaussian tail (residual adds, activations, EWA projection, SH colour -- geom_finish.cuh) runs after a hand-over
@@ -32,11 +33,11 @@ namespace g4d {
 
 template <int ARITH> struct TcArith;
 template <> struct TcArith<2> {               // FP16x2
-    static constexpr int KS = 16, ES = 2, EPC = 8, NWG = 2, PH = 1;
+    static constexpr int KS = 16, ES = 2, EPC = 8, PH = 1;
     static constexpr float SF = 64.f, SA = 8.f, SW = 256.f;
 };
 template <> struct TcArith<1> {               // 3xTF32
-    static constexpr int KS = 8, ES = 4, EPC = 4, NWG = 1, PH = 4;
+    static constexpr int KS = 8, ES = 4, EPC = 4, PH = 4;
     static constexpr float SF = 1.f, SA = 1.f, SW = 1.f;
 };
 constexpr float kF16Max = 65504.f;
@@ -48,9 +49,9 @@ constexpr uint32_t kTcStaticSmem = (uint32_t)((sizeof(CameraDev) + 127) & ~(size
 
 struct TcSmem { uint32_t w1, w0, w2, bias, w2s, stage, bars, part_bytes, total; };
 
-// part_bytes: one ring slot = one K-range of one head's W1 image, (hi | lo)
-inline TcSmem tc_smem_layout(int arith, int F, bool sh) {
-    const uint32_t es = arith == 2 ? 2u : 4u, ph = arith == 2 ? 1u : 4u, nwg = arith == 2 ? 2u : 1u;
+// part_bytes: one ring slot = one K-range of one head's W1 image, (hi | lo); one stage slab per consumer warpgroup
+inline TcSmem tc_smem_layout(int arith, int nwg, int F, bool sh) {
+    const uint32_t es = arith == 2 ? 2u : 4u, ph = arith == 2 ? 1u : 4u;
     TcSmem s{};
     uint32_t off = 0;
     auto take = [&](uint32_t bytes) { uint32_t o = off; off += (bytes + 127u) & ~127u; return o; };
@@ -60,10 +61,19 @@ inline TcSmem tc_smem_layout(int arith, int F, bool sh) {
     s.w2 = take(sh ? 2u * 48u * 128u * es : 128u);
     s.bias = take((128 + G4D_NUM_HEADS * 128 + 64) * 4);
     s.w2s = take(4 * 128 * 16);
-    s.stage = take(nwg * 64u * kStageCols * 4u);
+    s.stage = take((uint32_t)nwg * 64u * kStageCols * 4u);
     s.bars = take(64);
     s.total = off;
     return s;
+}
+
+// consumer warpgroups per CTA: FP16x2 the most (3, else 2) whose layout fits a block, 3xTF32 1; 0 when none fits.  More
+// warpgroups share each W1 image load and keep the tensor pipe busy while others run epilogues; every Gaussian's
+// arithmetic is the same at any count.
+inline int tc_warpgroups(int arith, int F, bool sh) {
+    for (int nwg = arith == 2 ? 3 : 1; nwg >= (arith == 2 ? 2 : 1); --nwg)
+        if (tc_smem_layout(arith, nwg, F, sh).total + kTcStaticSmem <= kMaxSmemPerBlock) return nwg;
+    return 0;
 }
 
 // ---- weight packing (once per parameter version) --------------------------------------------------------------
@@ -225,11 +235,12 @@ __device__ __forceinline__ void mbar_arrive(void* bar) {
 __device__ __forceinline__ void bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 
 // MODE as deform_kernel's (g4d_geom.cu): 0 deform only, 1 fused with M = 16 SH coefficients, 2 fused with M < 16
-template <int ARITH, int MODE, int C, int L, bool SAVE>
-__global__ void __launch_bounds__(TcArith<ARITH>::NWG * 128, 1)
+// NWG consumer warpgroups of 64 Gaussians each (tc_warpgroups)
+template <int ARITH, int NWG, int MODE, int C, int L, bool SAVE>
+__global__ void __launch_bounds__(NWG * 128, 1)
 deform_tc_kernel(DeformDesc d, TcWeights tw, TcSmem Ls, const CameraDev* __restrict__ camp, int64_t n, DeformIO io) {
     using A = TcArith<ARITH>;
-    constexpr int F = C * L, NS0 = F / A::KS, NS1 = 128 / A::KS, NSP = NS1 / A::PH, TM = 64 * A::NWG, NT = 128 * A::NWG;
+    constexpr int F = C * L, NS0 = F / A::KS, NS1 = 128 / A::KS, NSP = NS1 / A::PH, TM = 64 * NWG, NT = 128 * NWG;
     static_assert(F % 16 == 0 && F <= 64, "feature width must be 32, 48 or 64");
     constexpr float kInvL0 = A::SA / (A::SF * A::SW), kInvH = 1.f / (A::SA * A::SW), kInvHS = 1.f / A::SW;
     extern __shared__ __align__(128) uint8_t smem[];   // (every operand image and barrier is placed at a multiple of 128 B)
@@ -261,7 +272,7 @@ deform_tc_kernel(DeformDesc d, TcWeights tw, TcSmem Ls, const CameraDev* __restr
     if (tid == 0) {
         mbar_init(bar_w0, 1);
         mbar_init(bar_full, 1); mbar_init(bar_full + 1, 1);
-        mbar_init(bar_empty, 4 * A::NWG); mbar_init(bar_empty + 1, 4 * A::NWG);
+        mbar_init(bar_empty, 4 * NWG); mbar_init(bar_empty + 1, 4 * NWG);
         fence_barrier_init();
     }
     pdl_wait();           // from here on: the camera, the staged features
@@ -490,7 +501,7 @@ deform_tc_kernel(DeformDesc d, TcWeights tw, TcSmem Ls, const CameraDev* __restr
     }
     // range check of everything that went through an f16 conversion (already in operand units)
     if (ARITH == 2 && mx >= kF16Max && tw.status) *reinterpret_cast<volatile uint32_t*>(tw.status) = 1u;
-    if (dbg) { tw.dbg[blockIdx.x * 12] = clock64() - t_start; tw.dbg[blockIdx.x * 12 + 1] = t_wait; }
+    if (dbg) { tw.dbg[blockIdx.x * 12] = clock64() - t_start; tw.dbg[blockIdx.x * 12 + 1] = t_wait; tw.dbg[blockIdx.x * 12 + 2] = NWG; }
 }
 
 // ---- spatial walk order of the gather: a permutation of [0, n) in Z (Morton) order of each Gaussian's cell on a
@@ -616,43 +627,47 @@ bool tc_deform_supported(const G4DDeformParams& prm, int arith) {
     const int C = prm.channels, L = prm.levels;
     if (prm.net_width != 128 || prm.depth > 1) return false;   // no trunk layers (deep trunks: the FFMA kernels)
     if (!((C == 16 && (L == 2 || L == 3)) || (C == 32 && L == 2))) return false;
-    return tc_smem_layout(arith, C * L, (prm.head_mask & G4D_HEAD_SHS) != 0).total + kTcStaticSmem <= kMaxSmemPerBlock;
+    return tc_warpgroups(arith, C * L, (prm.head_mask & G4D_HEAD_SHS) != 0) != 0;
 }
 
-template <int ARITH, int MODE, int C, int L>
-static cudaError_t launch_deform_tc_t(const DeformDesc& d, const TcWeights& tw, const TcSmem& Ls, size_t bytes, int grid,
-                                      const CameraDev* cam, int64_t n, const DeformIO& io, cudaStream_t st) {
-    constexpr int threads = TcArith<ARITH>::NWG * 128;
+template <int ARITH, int NWG, int MODE, int C, int L>
+static cudaError_t launch_deform_tc_t(const DeformDesc& d, const TcWeights& tw, const CameraDev* cam, int64_t n, const DeformIO& io,
+                                      int sm_count, cudaStream_t st) {
+    const TcSmem Ls = tc_smem_layout(ARITH, NWG, d.F, (d.head_mask & G4D_HEAD_SHS) != 0);
+    const size_t bytes = Ls.total;
+    const int64_t ntiles = (n + 64 * NWG - 1) / (64 * NWG);
+    const int grid = (int)(ntiles < sm_count ? ntiles : sm_count);
     cudaError_t e;
     if (tw.relu_bits) {
-        e = cudaFuncSetAttribute(deform_tc_kernel<ARITH, MODE, C, L, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+        e = cudaFuncSetAttribute(deform_tc_kernel<ARITH, NWG, MODE, C, L, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
         if (e != cudaSuccess) return e;
-        return launch_k(deform_tc_kernel<ARITH, MODE, C, L, true>, dim3(grid), dim3(threads), bytes, st, true, d, tw, Ls, cam, n, io);
+        return launch_k(deform_tc_kernel<ARITH, NWG, MODE, C, L, true>, dim3(grid), dim3(NWG * 128), bytes, st, true, d, tw, Ls, cam, n, io);
     }
-    e = cudaFuncSetAttribute(deform_tc_kernel<ARITH, MODE, C, L, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    e = cudaFuncSetAttribute(deform_tc_kernel<ARITH, NWG, MODE, C, L, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
     if (e != cudaSuccess) return e;
-    return launch_k(deform_tc_kernel<ARITH, MODE, C, L, false>, dim3(grid), dim3(threads), bytes, st, true, d, tw, Ls, cam, n, io);
+    return launch_k(deform_tc_kernel<ARITH, NWG, MODE, C, L, false>, dim3(grid), dim3(NWG * 128), bytes, st, true, d, tw, Ls, cam, n, io);
 }
 
 cudaError_t launch_deform_tc(const DeformDesc& d, const TcWeights& tw, int mode, const CameraDev* cam, int64_t n,
                              const DeformIO& io, int sm_count, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
     if (!tw.feat) return cudaErrorInvalidValue;
-    const TcSmem Ls = tc_smem_layout(tw.arith, d.F, (d.head_mask & G4D_HEAD_SHS) != 0);
-    const size_t bytes = Ls.total;
-    const int64_t ntiles = (n + 64 * (tw.arith == 2 ? 2 : 1) - 1) / (64 * (tw.arith == 2 ? 2 : 1));
-    const int grid = (int)(ntiles < sm_count ? ntiles : sm_count);
-#define G4D_TC_CASE(AR, CC, LL)                                                                                        \
-    if (tw.arith == AR && d.C == CC && d.levels == LL)                                                                 \
-        return mode == 0                   ? launch_deform_tc_t<AR, 0, CC, LL>(d, tw, Ls, bytes, grid, cam, n, io, st)  \
-               : io.sh.m == kShCoeffs ? launch_deform_tc_t<AR, 1, CC, LL>(d, tw, Ls, bytes, grid, cam, n, io, st)  \
-                                      : launch_deform_tc_t<AR, 2, CC, LL>(d, tw, Ls, bytes, grid, cam, n, io, st);
-    G4D_TC_CASE(2, 16, 2)
-    G4D_TC_CASE(2, 16, 3)
-    G4D_TC_CASE(2, 32, 2)
-    G4D_TC_CASE(1, 16, 2)
-    G4D_TC_CASE(1, 16, 3)
-    G4D_TC_CASE(1, 32, 2)
+    const int nwg = tc_warpgroups(tw.arith, d.F, (d.head_mask & G4D_HEAD_SHS) != 0);
+    // the (C, L, warpgroups) that tc_warpgroups can choose: F = 32 always fits three FP16x2 warpgroups, F = 48 / 64 fit
+    // three without the SH head and two with it
+#define G4D_TC_CASE(AR, NW, CC, LL)                                                                                          \
+    if (tw.arith == AR && nwg == NW && d.C == CC && d.levels == LL)                                                          \
+        return mode == 0                   ? launch_deform_tc_t<AR, NW, 0, CC, LL>(d, tw, cam, n, io, sm_count, st)         \
+               : io.sh.m == kShCoeffs ? launch_deform_tc_t<AR, NW, 1, CC, LL>(d, tw, cam, n, io, sm_count, st)         \
+                                      : launch_deform_tc_t<AR, NW, 2, CC, LL>(d, tw, cam, n, io, sm_count, st);
+    G4D_TC_CASE(2, 3, 16, 2)
+    G4D_TC_CASE(2, 3, 16, 3)
+    G4D_TC_CASE(2, 2, 16, 3)
+    G4D_TC_CASE(2, 3, 32, 2)
+    G4D_TC_CASE(2, 2, 32, 2)
+    G4D_TC_CASE(1, 1, 16, 2)
+    G4D_TC_CASE(1, 1, 16, 3)
+    G4D_TC_CASE(1, 1, 32, 2)
 #undef G4D_TC_CASE
     return cudaErrorInvalidValue;
 }

@@ -285,8 +285,9 @@ enum { G4D_OPT_SYNC_MODE = 1,  /* 1 (default): size the instance buffer exactly 
                                    < 1023, weights < 255 -- else the NEXT call returns G4D_ERR_OVERFLOW); 1: wgmma 3xTF32 (no
                                    range limit); 0: FP32 FFMA kernels.  The tensor-core kernels take the network with
                                    no trunk layers (depth <= 1); a deeper one runs on the FFMA kernels whatever the value */
-       G4D_OPT_TC_DEBUG = 6,     /* 1: the tensor-core forward records cycle counters per CTA (g4d_debug_tc_cycles: [0] whole
-                                   kernel, [1] waiting for W1 images, [2..11] unused) */
+       G4D_OPT_TC_DEBUG = 6,     /* 1: the tensor-core forward records counters per CTA (g4d_debug_tc_cycles: [0] cycles of the
+                                   whole kernel, [1] cycles waiting for W1 images, [2] the CTA's consumer warpgroups, [3..11]
+                                   unused) */
        G4D_OPT_KEEP_DEFORMED = 8, /* 1: a no-grad fused forward (G4D_CAM_NO_GRAD) still stores the deformed + activated tensors
                                    * (G4D_BUF_DEFORMED / _SHS reads); default 0: it skips those 48-240 B / Gaussian of writes */
        G4D_OPT_WARP_CULL = 7,    /* 1 (default): the blend kernels skip, per warp, instances that cannot reach alpha >= 1/255
@@ -338,7 +339,8 @@ enum { G4D_STAGE_PREP = 0,        /* camera pack, weight pack, time-row collapse
        G4D_STAGE_COUNT = 10 };
 int g4d_context_stage_times(G4DContext *ctx, float *out_ms, int capacity);
 
-/* DEBUG: mean per-CTA cycle counters of the last tensor-core deform launch (G4D_OPT_TC_DEBUG). */
+/* DEBUG: per-CTA counters of the last tensor-core deform launch (G4D_OPT_TC_DEBUG), averaged over the SMs (an SM without a
+ * CTA of the launch counts as 0). */
 int g4d_debug_tc_cycles(G4DWorkspace *ws, double *out12);
 
 /* ---- CUDA-graph capture (opt-in; INTEGRATION.md "CUDA graphs") -------------------------------------
