@@ -88,25 +88,23 @@ struct FfmaWeights {
     float* wtt[G4D_MAX_DEPTH - 1];
 };
 
-// weight images derived from the caller's parameters, rebuilt when G4DDeformParams.version or the w0 pointer changes (or,
-// for the tensor-core forward, the arithmetic)
+// weight images derived from the caller's parameters, rebuilt when G4DDeformParams.version or the w0 pointer changes
 template <class Images>
 struct WeightCache {
     DevBuf buf;
     Images img{};   // where the images sit in buf
     uint64_t version = 0;
     const void* key = nullptr;
-    int arith = 0;
     bool valid = false;
     // pack(buf.p, &img) (re)builds the images unless they were built from these parameters; a capture always rebuilds them,
     // so that every replay packs the parameters as they are then
-    template <class Pack> cudaError_t refresh(const G4DDeformParams* p, int arith_, size_t bytes, Pack pack) {
-        if (valid && !t_call.capturing && version == p->version && key == (const void*)p->w0 && arith == arith_) return cudaSuccess;
+    template <class Pack> cudaError_t refresh(const G4DDeformParams* p, size_t bytes, Pack pack) {
+        if (valid && !t_call.capturing && version == p->version && key == (const void*)p->w0) return cudaSuccess;
         valid = false;
         cudaError_t e = buf.ensure(bytes);
         if (e == cudaSuccess) e = pack(buf.p, &img);
         if (e != cudaSuccess) return e;
-        version = p->version; key = (const void*)p->w0; arith = arith_; valid = true;
+        version = p->version; key = (const void*)p->w0; valid = true;
         return cudaSuccess;
     }
 };
@@ -145,7 +143,7 @@ struct G4DWorkspace {
     int64_t min_capacity = 0;
     int tight_cull = 0;
     int stage_timing = 0;
-    int tensor_cores = 2;      // 0: FP32 FFMA kernels, 1: wgmma 3xTF32, 2 (default): wgmma FP16x2
+    int tensor_cores = 2;      // 0: FP32 FFMA kernels, 2 (default): wgmma FP16x2
     int warp_cull = 1;
     int keep_deformed = 0;
     int tc_debug = 0;
@@ -360,24 +358,22 @@ int refresh_packed(G4DWorkspace* ws, const G4DDeformParams* p, cudaStream_t st) 
         for (size_t j = 0; j < G4D_MAX_DEPTH - 1; ++j) w->wtt[j] = j < ntrunk ? w->w0t + F * WD + (G4D_NUM_HEADS + j) * WD * WD : nullptr;
         return launch_pack_weights(*p, w->w0t, w->w1t, w->wtt, st);
     };
-    G4D_CUDA(ws->packed.refresh(p, 0, (F * WD + (G4D_NUM_HEADS + ntrunk) * WD * WD) * 4, pack));
+    G4D_CUDA(ws->packed.refresh(p, (F * WD + (G4D_NUM_HEADS + ntrunk) * WD * WD) * 4, pack));
     return G4D_OK;
 }
 
 int refresh_tc(G4DWorkspace* ws, const G4DDeformParams* p, cudaStream_t st) {
-    const int arith = ws->tensor_cores == 2 ? 2 : 1;
-    if (arith == 2 && !t_call.capturing && ws->pinned->f16_range) {   // (a capture leaves the flag to g4d_workspace_graph_status)
+    if (!t_call.capturing && ws->pinned->f16_range) {   // (a capture leaves the flag to g4d_workspace_graph_status)
         ws->pinned->f16_range = 0;
         ws->tc.valid = false;      // re-pack (and re-check) the weights on the next call: they may be the out-of-range values
         return fail(G4D_ERR_OVERFLOW, "an earlier FP16x2 tensor-core launch met a value outside the f16 operand range (activation >= 8188, "
-                                      "feature >= 1023 or weight >= 255): its results were saturated; set G4D_OPT_TENSOR_CORES = 1 (3xTF32)");
+                                      "feature >= 1023 or weight >= 255): its results were saturated; set G4D_OPT_TENSOR_CORES = 0 (FFMA kernels, no range limit)");
     }
     auto pack = [&](void* blob, TcWeights* w) {
-        w->arith = arith;
         w->status = &ws->pinned->f16_range;
-        return launch_tc_pack_weights(*p, arith, static_cast<float*>(blob), w, st);
+        return launch_tc_pack_weights(*p, static_cast<float*>(blob), w, st);
     };
-    G4D_CUDA(ws->tc.refresh(p, arith, tc_packed_floats(*p) * 4, pack));
+    G4D_CUDA(ws->tc.refresh(p, tc_packed_floats(*p) * 4, pack));
     return G4D_OK;
 }
 
@@ -446,7 +442,7 @@ int collapse_time_rows(DevBuf& rows, float* (*trow)[3], const G4DDeformParams* p
 int setup_deform(G4DWorkspace* ws, const G4DDeformParams* p, const float* xyz, int64_t n, DevBuf& rows, float* (*trow)[3],
                  TimeArg time, cudaStream_t st, DeformSetup* out) {
     int rc;
-    out->tc = ws->tensor_cores != 0 && tc_deform_supported(*p, ws->tensor_cores);
+    out->tc = ws->tensor_cores != 0 && tc_deform_supported(*p);
     if ((rc = gather_order(ws, p->aabb, xyz, n, st, &out->gather.order)) != G4D_OK) return rc;
     if ((rc = collapse_time_rows(rows, trow, p, time, st)) != G4D_OK) return rc;
     if (!out->tc) {
@@ -488,7 +484,7 @@ int deform_backward_dispatch(G4DWorkspace* ws, const G4DDeformParams* prm, float
     const bool tc = ws->tensor_cores && tc_backward_supported(*prm);
     if (tc) {
         auto pack = [&](void* blob, TcBwdWeights* w) { return launch_tc_bwd_pack_weights(*prm, static_cast<uint8_t*>(blob), w, st); };
-        G4D_CUDA(ws->tc_bwd.refresh(prm, 0, tc_bwd_weight_bytes(*prm), pack));
+        G4D_CUDA(ws->tc_bwd.refresh(prm, tc_bwd_weight_bytes(*prm), pack));
     } else if ((rc = refresh_packed(ws, prm, st)) != G4D_OK) {
         return rc;
     }
@@ -713,7 +709,10 @@ int g4d_workspace_set_option(G4DWorkspace* ws, int option, int64_t value) {
         case G4D_OPT_INSTANCE_CAPACITY: ws->min_capacity = value; return G4D_OK;
         case G4D_OPT_TIGHT_CULL: ws->tight_cull = value ? 1 : 0; return G4D_OK;
         case G4D_OPT_STAGE_TIMING: ws->stage_timing = value ? 1 : 0; return G4D_OK;
-        case G4D_OPT_TENSOR_CORES: ws->tensor_cores = value < 0 || value > 2 ? 2 : (int)value; return G4D_OK;
+        case G4D_OPT_TENSOR_CORES:
+            if (value == 1) return fail(G4D_ERR_ARG, "G4D_OPT_TENSOR_CORES = 1 (3xTF32) was removed; 0 selects the FFMA kernels, which have no range limit");
+            ws->tensor_cores = value == 0 ? 0 : 2;
+            return G4D_OK;
         case G4D_OPT_WARP_CULL: ws->warp_cull = value ? 1 : 0; return G4D_OK;
         case G4D_OPT_TC_DEBUG: ws->tc_debug = value ? 1 : 0; return G4D_OK;
         case G4D_OPT_KEEP_DEFORMED: ws->keep_deformed = value ? 1 : 0; return G4D_OK;

@@ -1,15 +1,14 @@
 // g4d_deform_tc.cu -- tensor-core version of the fused deform + activate + project forward (net_width 128).
 //
 // The deformation MLP (scene/deformation.py:67-148: 93.6 kMAC per Gaussian at the DyNeRF config) runs on the Hopper tensor
-// cores with hand-written wgmma PTX (tc_wgmma.cuh), in one of two arithmetics (G4D_OPT_TENSOR_CORES):
-//   2 (default) FP16x2: x = hi + lo with hi = rn_f16(s x), lo = rn_f16(s x - hi), s a fixed power of two per operand class
-//     (features 2^6, activations 2^3, weights 2^8; undone exactly by the epilogue's FMA).  |x - (hi + lo)/s| <= max(2^-22 |x|,
-//     2^-25 / s): the 3xTF32 relative error, with an absolute floor far below the fp32 accumulation noise of a K = 128 dot
-//     product.  s |x| must stay below 65504 (activations < 8188, features < 1023, weights < 255): conversions saturate and the
-//     kernel raises a flag in host-mapped memory that the next call reports (G4D_ERR_OVERFLOW).
-//   1 3xTF32: hi = rna_tf32(x), lo = rna_tf32(x - hi), no range limit.
-// Both form the three products lo*hi + hi*lo + hi*hi with fp32 accumulation: fp32-level accuracy (single-pass TF32 or F16 is
-// ~1000x worse than the 1e-4 image tolerance allows).
+// cores with hand-written wgmma PTX (tc_wgmma.cuh), on FP16x2 operands (G4D_OPT_TENSOR_CORES = 2, the default):
+// x = hi + lo with hi = rn_f16(s x), lo = rn_f16(s x - hi), s a fixed power of two per operand class (features 2^6,
+// activations 2^3, weights 2^8; undone exactly by the epilogue's FMA).  |x - (hi + lo)/s| <= max(2^-22 |x|, 2^-25 / s): an
+// absolute floor far below the fp32 accumulation noise of a K = 128 dot product.  The three products lo*hi + hi*lo + hi*hi
+// with fp32 accumulation give fp32-level accuracy (single-pass F16 is ~1000x worse than the 1e-4 image tolerance allows).
+// s |x| must stay below 65504 (activations < 8188, features < 1023, weights < 255): conversions saturate and the kernel
+// raises a flag in host-mapped memory that the next call reports (G4D_ERR_OVERFLOW).  Networks beyond that range run on the
+// FFMA kernels (G4D_OPT_TENSOR_CORES = 0), which have no range limit.
 //
 // Structure: a warpgroup (128 threads) owns 64 Gaussians (the M = 64 of wgmma) and carries them through every layer:
 //   * the A operand of every GEMM lives in registers: the features are loaded straight into fragment layout, and each
@@ -18,8 +17,8 @@
 //   * weights are the B operand in shared memory: packed once per parameter version into the no-swizzle canonical K-major
 //     image (hi | lo), W0 and the SH head's W2 resident, W1 streamed head by head through a two-slot ring with TMA bulk
 //     copies and mbarriers (full: transaction count; empty: one arrival per consumer warp), one load ahead;
-//   * FP16x2 runs three warpgroups per CTA (192 Gaussians per W1 image load) where their shared memory fits, else two
-//     (F = 48 / 64 with the SH head); 3xTF32 runs one (its A fragments take 128 registers);
+//   * three warpgroups per CTA (192 Gaussians per W1 image load) where their shared memory fits, else two (F = 48 / 64
+//     with the SH head);
 //   * layer 2 of the <= 4-wide heads runs in exact fp32 in the epilogue (each lane sums its 32 hidden units, a quad shuffle
 //     completes the row); the SH head's layer 2 (N = 48) is a fourth GEMM;
 //   * the per-Gaussian tail (residual adds, activations, EWA projection, SH colour -- geom_finish.cuh) runs after a hand-over
@@ -31,14 +30,10 @@
 
 namespace g4d {
 
-template <int ARITH> struct TcArith;
-template <> struct TcArith<2> {               // FP16x2
-    static constexpr int KS = 16, ES = 2, EPC = 8, PH = 1;
+// FP16x2 operands: K per wgmma slice, bytes per element, elements per 16-byte core row; scales of features, activations, weights
+struct TcArith {
+    static constexpr int KS = 16, ES = 2, EPC = 8;
     static constexpr float SF = 64.f, SA = 8.f, SW = 256.f;
-};
-template <> struct TcArith<1> {               // 3xTF32
-    static constexpr int KS = 8, ES = 4, EPC = 4, PH = 4;
-    static constexpr float SF = 1.f, SA = 1.f, SW = 1.f;
 };
 constexpr float kF16Max = 65504.f;
 constexpr int kStageCols = 60;
@@ -47,16 +42,16 @@ constexpr int kStageCols = 60;
 constexpr uint32_t kMaxSmemPerBlock = 227u * 1024u;
 constexpr uint32_t kTcStaticSmem = (uint32_t)((sizeof(CameraDev) + 127) & ~(size_t)127);                 // per Gaussian: 11 geometry deltas | 48 SH deltas | pad
 
-struct TcSmem { uint32_t w1, w0, w2, bias, w2s, stage, bars, part_bytes, total; };
+struct TcSmem { uint32_t w1, w0, w2, bias, w2s, stage, bars, slot_bytes, total; };
 
-// part_bytes: one ring slot = one K-range of one head's W1 image, (hi | lo); one stage slab per consumer warpgroup
-inline TcSmem tc_smem_layout(int arith, int nwg, int F, bool sh) {
-    const uint32_t es = arith == 2 ? 2u : 4u, ph = arith == 2 ? 1u : 4u;
+// slot_bytes: one ring slot = one head's W1 image, (hi | lo); one stage slab per consumer warpgroup
+inline TcSmem tc_smem_layout(int nwg, int F, bool sh) {
+    constexpr uint32_t es = TcArith::ES;
     TcSmem s{};
     uint32_t off = 0;
     auto take = [&](uint32_t bytes) { uint32_t o = off; off += (bytes + 127u) & ~127u; return o; };
-    s.part_bytes = 2u * 128u * (128u / ph) * es;
-    s.w1 = take(2u * s.part_bytes);
+    s.slot_bytes = 2u * 128u * 128u * es;
+    s.w1 = take(2u * s.slot_bytes);
     s.w0 = take(2u * 128u * F * es);
     s.w2 = take(sh ? 2u * 48u * 128u * es : 128u);
     s.bias = take((128 + G4D_NUM_HEADS * 128 + 64) * 4);
@@ -67,25 +62,24 @@ inline TcSmem tc_smem_layout(int arith, int nwg, int F, bool sh) {
     return s;
 }
 
-// consumer warpgroups per CTA: FP16x2 the most (3, else 2) whose layout fits a block, 3xTF32 1; 0 when none fits.  More
-// warpgroups share each W1 image load and keep the tensor pipe busy while others run epilogues; every Gaussian's
-// arithmetic is the same at any count.
-inline int tc_warpgroups(int arith, int F, bool sh) {
-    for (int nwg = arith == 2 ? 3 : 1; nwg >= (arith == 2 ? 2 : 1); --nwg)
-        if (tc_smem_layout(arith, nwg, F, sh).total + kTcStaticSmem <= kMaxSmemPerBlock) return nwg;
+// consumer warpgroups per CTA: the most (3, else 2) whose layout fits a block; 0 when none fits.  More warpgroups share
+// each W1 image load and keep the tensor pipe busy while others run epilogues; every Gaussian's arithmetic is the same at
+// any count.
+inline int tc_warpgroups(int F, bool sh) {
+    for (int nwg = 3; nwg >= 2; --nwg)
+        if (tc_smem_layout(nwg, F, sh).total + kTcStaticSmem <= kMaxSmemPerBlock) return nwg;
     return 0;
 }
 
 // ---- weight packing (once per parameter version) --------------------------------------------------------------
-// Every matrix [rows][K] (torch Linear layout) becomes (hi | lo) canonical K-major images, split into `parts` K-ranges
-// (part p = hi | lo of columns [p K/parts, (p+1) K/parts)); `kperm`: TF32 K order of an accumulator-fed A operand.
+// Every matrix [rows][K] (torch Linear layout) becomes a (hi | lo) pair of canonical K-major images of scaled f16 words.
 struct TcPackDesc {
     const float* src[1 + G4D_NUM_HEADS + 1];
     uint8_t* dst[1 + G4D_NUM_HEADS + 1];
-    int rows[1 + G4D_NUM_HEADS + 1], K[1 + G4D_NUM_HEADS + 1], parts[1 + G4D_NUM_HEADS + 1], kperm[1 + G4D_NUM_HEADS + 1];
+    int rows[1 + G4D_NUM_HEADS + 1], K[1 + G4D_NUM_HEADS + 1];
     int start[2 + G4D_NUM_HEADS + 1];
-    int count, arith;
-    uint32_t* status;                 // FP16x2: set to 1 when a scaled weight leaves the f16 range (TcWeights::status)
+    int count;
+    uint32_t* status;                 // set to 1 when a scaled weight leaves the f16 range (TcWeights::status)
 };
 
 __global__ void tc_pack_weights_kernel(TcPackDesc p) {
@@ -95,23 +89,13 @@ __global__ void tc_pack_weights_kernel(TcPackDesc p) {
     while (i >= p.start[m + 1]) ++m;
     const int e = i - p.start[m];
     const uint32_t K = (uint32_t)p.K[m], n = (uint32_t)e / K, k = (uint32_t)e % K, rows = (uint32_t)p.rows[m];
-    const uint32_t kd = p.kperm[m] ? wg::tf32_kperm(k) : k;
-    const uint32_t KP = K / (uint32_t)p.parts[m], part = kd / KP, kk = kd % KP;
     const float v = __ldg(p.src[m] + e);
-    if (p.arith == 2) {
-        uint32_t hi, lo;
-        if (fabsf(v * TcArith<2>::SW) >= kF16Max && p.status) *reinterpret_cast<volatile uint32_t*>(p.status) = 1u;   // saturates
-        wg::f16_split2(v * TcArith<2>::SW, 0.f, hi, lo);
-        uint8_t* base = p.dst[m] + (size_t)part * 2u * rows * KP * 2u + wg::img16_off(n, kk, KP);
-        *reinterpret_cast<uint16_t*>(base) = (uint16_t)hi;
-        *reinterpret_cast<uint16_t*>(base + rows * KP * 2u) = (uint16_t)lo;
-    } else {
-        uint32_t hi, lo;
-        wg::tf32_split(v, hi, lo);
-        uint8_t* base = p.dst[m] + (size_t)part * 2u * rows * KP * 4u + wg::img32_off(n, kk, KP);
-        *reinterpret_cast<uint32_t*>(base) = hi;
-        *reinterpret_cast<uint32_t*>(base + rows * KP * 4u) = lo;
-    }
+    uint32_t hi, lo;
+    if (fabsf(v * TcArith::SW) >= kF16Max && p.status) *reinterpret_cast<volatile uint32_t*>(p.status) = 1u;   // saturates
+    wg::f16_split2(v * TcArith::SW, 0.f, hi, lo);
+    uint8_t* base = p.dst[m] + wg::img16_off(n, k, K);
+    *reinterpret_cast<uint16_t*>(base) = (uint16_t)hi;
+    *reinterpret_cast<uint16_t*>(base + rows * K * 2u) = (uint16_t)lo;
 }
 
 size_t tc_packed_floats(const G4DDeformParams& prm) {
@@ -121,29 +105,27 @@ size_t tc_packed_floats(const G4DDeformParams& prm) {
     return f + 64;
 }
 
-cudaError_t launch_tc_pack_weights(const G4DDeformParams& prm, int arith, float* blob, TcWeights* out, cudaStream_t st) {
+cudaError_t launch_tc_pack_weights(const G4DDeformParams& prm, float* blob, TcWeights* out, cudaStream_t st) {
     TcPackDesc p{};
-    p.arith = arith;
     p.status = out->status;
     const int F = prm.levels * prm.channels;
-    const size_t es = arith == 2 ? 2 : 4;
     int m = 0, total = 0;
     uint8_t* q = reinterpret_cast<uint8_t*>(blob);
-    auto add = [&](const float* src, int rows, int K, int parts, int kperm) {
-        p.src[m] = src; p.dst[m] = q; p.rows[m] = rows; p.K[m] = K; p.parts[m] = parts; p.kperm[m] = kperm && arith == 1;
+    auto add = [&](const float* src, int rows, int K) {
+        p.src[m] = src; p.dst[m] = q; p.rows[m] = rows; p.K[m] = K;
         p.start[m] = total;
         total += rows * K;
         uint8_t* r = q;
-        q += 2 * (size_t)rows * K * es;
+        q += 2 * (size_t)rows * K * TcArith::ES;
         ++m;
         return reinterpret_cast<const float*>(r);
     };
-    out->w0 = add(prm.w0, 128, F, 1, 0);
+    out->w0 = add(prm.w0, 128, F);
     for (int h = 0; h < G4D_NUM_HEADS; ++h) {
         out->w1[h] = nullptr; out->w2[h] = nullptr;
         if (!(prm.head_mask & (1 << h))) continue;
-        out->w1[h] = add(prm.w1[h], 128, 128, arith == 2 ? TcArith<2>::PH : TcArith<1>::PH, 1);
-        if (h == 4) out->w2[h] = add(prm.w2[h], 48, 128, 1, 1);   // the small heads' layer 2 runs in fp32 from the caller's tensors
+        out->w1[h] = add(prm.w1[h], 128, 128);
+        if (h == 4) out->w2[h] = add(prm.w2[h], 48, 128);   // the small heads' layer 2 runs in fp32 from the caller's tensors
     }
     p.start[m] = total; p.count = m;
     tc_pack_weights_kernel<<<(total + 255) / 256, 256, 0, st>>>(p);
@@ -155,37 +137,26 @@ using wg::Frags;
 
 // two values of row g (x0, x1 = columns c, c + 1) and the same columns of row g + 8 (y0, y1), in accumulator block j,
 // -> the A fragment slots they occupy
-template <int ARITH, int NS>
+template <int NS>
 __device__ __forceinline__ void put_block(Frags<NS>& a, int j, float x0, float x1, float y0, float y1) {
-    if constexpr (ARITH == 2) {
-        const int s = j >> 1, o = (j & 1) * 2;
-        wg::f16_split2(x0, x1, a.hi[s][o], a.lo[s][o]);
-        wg::f16_split2(y0, y1, a.hi[s][o + 1], a.lo[s][o + 1]);
-    } else {
-        wg::tf32_split(x0, a.hi[j][0], a.lo[j][0]);
-        wg::tf32_split(y0, a.hi[j][1], a.lo[j][1]);
-        wg::tf32_split(x1, a.hi[j][2], a.lo[j][2]);
-        wg::tf32_split(y1, a.hi[j][3], a.lo[j][3]);
-    }
+    const int s = j >> 1, o = (j & 1) * 2;
+    wg::f16_split2(x0, x1, a.hi[s][o], a.lo[s][o]);
+    wg::f16_split2(y0, y1, a.hi[s][o + 1], a.lo[s][o + 1]);
 }
 
-// D[64 x N] = A * B^T, three products; B = (hi | lo) K-major image with `bcols` columns, K-slices [s0, s0 + NSP) of A
-// against the image's slices [0, NSP)
-template <int ARITH, int N, int NS, int NSP>
-__device__ __forceinline__ void gemm3(float (&d)[N / 2], const Frags<NS>& a, int s0, uint32_t b_hi, uint32_t b_lo, uint32_t bcols,
-                                      bool accumulate) {
-    using A = TcArith<ARITH>;
-    const uint64_t dh = wg::desc_kmajor(b_hi, bcols, A::EPC), dl = wg::desc_kmajor(b_lo, bcols, A::EPC);
+// D[64 x N] = A * B^T, three products; B = (hi | lo) K-major image with `bcols` columns
+template <int N, int NS>
+__device__ __forceinline__ void gemm3(float (&d)[N / 2], const Frags<NS>& a, uint32_t b_hi, uint32_t b_lo, uint32_t bcols) {
+    const uint64_t dh = wg::desc_kmajor(b_hi, bcols, TcArith::EPC), dl = wg::desc_kmajor(b_lo, bcols, TcArith::EPC);
     wg::fence_regs(d);
     wg::fence();
 #pragma unroll
     for (int p = 0; p < 3; ++p) {
 #pragma unroll
-        for (int s = 0; s < NSP; ++s) {
+        for (int s = 0; s < NS; ++s) {
             const uint64_t bd = ((p == 1) ? dl : dh) + (uint64_t)(16 * s);      // + 256 bytes per slice
-            const uint32_t acc = (accumulate || p > 0 || s > 0) ? 1u : 0u;
-            if constexpr (ARITH == 2) wg::mma_f16_rs<N, 0>(d, p == 0 ? a.lo[s0 + s] : a.hi[s0 + s], bd, acc);
-            else wg::mma_tf32_rs<N>(d, p == 0 ? a.lo[s0 + s] : a.hi[s0 + s], bd, acc);
+            const uint32_t acc = (p > 0 || s > 0) ? 1u : 0u;
+            wg::mma_f16_rs<N, 0>(d, p == 0 ? a.lo[s] : a.hi[s], bd, acc);
         }
     }
     wg::commit();
@@ -195,8 +166,7 @@ __device__ __forceinline__ void gemm3(float (&d)[N / 2], const Frags<NS>& a, int
 
 // bias + ReLU of a 64 x 128 accumulator -> next A operand; sign bits of rows g / g + 8 (4 words each, complete for every lane
 // of the quad); running maximum of the converted values
-template <int ARITH>
-__device__ __forceinline__ void relu_to_frags(const float (&d)[64], float inv, const float* __restrict__ bias, int t, Frags<128 / TcArith<ARITH>::KS>& a,
+__device__ __forceinline__ void relu_to_frags(const float (&d)[64], float inv, const float* __restrict__ bias, int t, Frags<128 / TcArith::KS>& a,
                                               uint32_t (&b0)[4], uint32_t (&b1)[4], float& mx) {
 #pragma unroll
     for (int w = 0; w < 4; ++w) { b0[w] = 0u; b1[w] = 0u; }
@@ -211,7 +181,7 @@ __device__ __forceinline__ void relu_to_frags(const float (&d)[64], float inv, c
         b1[j >> 2] |= ((y0 > 0.f ? 1u : 0u) | (y1 > 0.f ? 2u : 0u)) << sh;
         const float r0 = fmaxf(x0, 0.f), r1 = fmaxf(x1, 0.f), r2 = fmaxf(y0, 0.f), r3 = fmaxf(y1, 0.f);
         mx = fmaxf(mx, fmaxf(fmaxf(r0, r1), fmaxf(r2, r3)));
-        put_block<ARITH>(a, j, r0, r1, r2, r3);
+        put_block(a, j, r0, r1, r2, r3);
     }
 #pragma unroll
     for (int w = 0; w < 4; ++w) {
@@ -235,12 +205,13 @@ __device__ __forceinline__ void mbar_arrive(void* bar) {
 __device__ __forceinline__ void bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 
 // MODE as deform_kernel's (g4d_geom.cu): 0 deform only, 1 fused with M = 16 SH coefficients, 2 fused with M < 16
-// NWG consumer warpgroups of 64 Gaussians each (tc_warpgroups)
-template <int ARITH, int NWG, int MODE, int C, int L, bool SAVE>
+// NWG consumer warpgroups of 64 Gaussians each (tc_warpgroups).  tw is __grid_constant__: the W1 ring indexes tw.w1[] at run
+// time, and nvcc would otherwise copy a parameter struct of 128 bytes or less to local memory to do so.
+template <int NWG, int MODE, int C, int L, bool SAVE>
 __global__ void __launch_bounds__(NWG * 128, 1)
-deform_tc_kernel(DeformDesc d, TcWeights tw, TcSmem Ls, const CameraDev* __restrict__ camp, int64_t n, DeformIO io) {
-    using A = TcArith<ARITH>;
-    constexpr int F = C * L, NS0 = F / A::KS, NS1 = 128 / A::KS, NSP = NS1 / A::PH, TM = 64 * NWG, NT = 128 * NWG;
+deform_tc_kernel(DeformDesc d, const __grid_constant__ TcWeights tw, TcSmem Ls, const CameraDev* __restrict__ camp, int64_t n, DeformIO io) {
+    using A = TcArith;
+    constexpr int F = C * L, NS0 = F / A::KS, NS1 = 128 / A::KS, TM = 64 * NWG, NT = 128 * NWG;
     static_assert(F % 16 == 0 && F <= 64, "feature width must be 32, 48 or 64");
     constexpr float kInvL0 = A::SA / (A::SF * A::SW), kInvH = 1.f / (A::SA * A::SW), kInvHS = 1.f / A::SW;
     extern __shared__ __align__(128) uint8_t smem[];   // (every operand image and barrier is placed at a multiple of 128 B)
@@ -290,15 +261,14 @@ deform_tc_kernel(DeformDesc d, TcWeights tw, TcSmem Ls, const CameraDev* __restr
     }
     const int64_t ntiles = (n + TM - 1) / TM;
     const int64_t my_tiles = (int64_t)blockIdx.x < ntiles ? (ntiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
-    const uint32_t per_tile = (uint32_t)(m_heads * A::PH), total_items = (uint32_t)my_tiles * per_tile;
-    // W1 ring: item u = (tile, head position, K-part) in consumption order, slot u & 1; thread 0 loads one item ahead
+    const uint32_t per_tile = (uint32_t)m_heads, total_items = (uint32_t)my_tiles * per_tile;
+    // W1 ring: item u = (tile, head position) in consumption order, slot u & 1; thread 0 loads one item ahead
     auto issue = [&](uint32_t u) {
-        const uint32_t s = u & 1u, r = u % per_tile;
+        const uint32_t s = u & 1u;
         if (u >= 2) mbar_wait(bar_empty + s, ((u >> 1) - 1u) & 1u);
-        const int h = (int)((hseq >> (3 * (r / A::PH))) & 7u);
-        mbar_expect_tx(bar_full + s, Ls.part_bytes);
-        tma_bulk_g2s(smem + Ls.w1 + s * Ls.part_bytes, reinterpret_cast<const uint8_t*>(tw.w1[h]) + (r % A::PH) * Ls.part_bytes,
-                     Ls.part_bytes, bar_full + s);
+        const int h = (int)((hseq >> (3 * (u % per_tile))) & 7u);
+        mbar_expect_tx(bar_full + s, Ls.slot_bytes);
+        tma_bulk_g2s(smem + Ls.w1 + s * Ls.slot_bytes, tw.w1[h], Ls.slot_bytes, bar_full + s);
     };
     if (tid == 0) {
         const uint32_t w0b = 2u * 128u * F * A::ES, w2b = hsh ? 2u * 48u * 128u * A::ES : 0u;
@@ -331,37 +301,25 @@ deform_tc_kernel(DeformDesc d, TcWeights tw, TcSmem Ls, const CameraDev* __restr
                 float v[8];   // (row g: c, c + 1 | row g + 8: c, c + 1) for the two column pairs of the slice
 #pragma unroll
                 for (int hlf = 0; hlf < 2; ++hlf) {
-                    const int c = ARITH == 2 ? 16 * s + 8 * hlf + 2 * t : 8 * s + 4 * hlf + t;
-                    if (ARITH == 2) {
-                        const float2 p0 = g0 < n ? __ldg(reinterpret_cast<const float2*>(f0 + c)) : make_float2(0.f, 0.f);
-                        const float2 p1 = g1 < n ? __ldg(reinterpret_cast<const float2*>(f1 + c)) : make_float2(0.f, 0.f);
-                        v[4 * hlf] = p0.x * A::SF; v[4 * hlf + 1] = p0.y * A::SF; v[4 * hlf + 2] = p1.x * A::SF; v[4 * hlf + 3] = p1.y * A::SF;
-                    } else {
-                        v[4 * hlf] = g0 < n ? __ldg(f0 + c) : 0.f;
-                        v[4 * hlf + 2] = g1 < n ? __ldg(f1 + c) : 0.f;
-                    }
+                    const int c = 16 * s + 8 * hlf + 2 * t;
+                    const float2 p0 = g0 < n ? __ldg(reinterpret_cast<const float2*>(f0 + c)) : make_float2(0.f, 0.f);
+                    const float2 p1 = g1 < n ? __ldg(reinterpret_cast<const float2*>(f1 + c)) : make_float2(0.f, 0.f);
+                    v[4 * hlf] = p0.x * A::SF; v[4 * hlf + 1] = p0.y * A::SF; v[4 * hlf + 2] = p1.x * A::SF; v[4 * hlf + 3] = p1.y * A::SF;
                 }
-                if (ARITH == 2) {
 #pragma unroll
-                    for (int e = 0; e < 8; ++e) mx = fmaxf(mx, fabsf(v[e]));
-                    wg::f16_split2(v[0], v[1], x.hi[s][0], x.lo[s][0]);
-                    wg::f16_split2(v[2], v[3], x.hi[s][1], x.lo[s][1]);
-                    wg::f16_split2(v[4], v[5], x.hi[s][2], x.lo[s][2]);
-                    wg::f16_split2(v[6], v[7], x.hi[s][3], x.lo[s][3]);
-                } else {
-                    wg::tf32_split(v[0], x.hi[s][0], x.lo[s][0]);
-                    wg::tf32_split(v[2], x.hi[s][1], x.lo[s][1]);
-                    wg::tf32_split(v[4], x.hi[s][2], x.lo[s][2]);
-                    wg::tf32_split(v[6], x.hi[s][3], x.lo[s][3]);
-                }
+                for (int e = 0; e < 8; ++e) mx = fmaxf(mx, fabsf(v[e]));
+                wg::f16_split2(v[0], v[1], x.hi[s][0], x.lo[s][0]);
+                wg::f16_split2(v[2], v[3], x.hi[s][1], x.lo[s][1]);
+                wg::f16_split2(v[4], v[5], x.hi[s][2], x.lo[s][2]);
+                wg::f16_split2(v[6], v[7], x.hi[s][3], x.lo[s][3]);
             }
-            gemm3<ARITH, 128, NS0, NS0>(acc, x, 0, sW0, sW0 + 128u * F * A::ES, F, false);
+            gemm3<128, NS0>(acc, x, sW0, sW0 + 128u * F * A::ES, F);
         }
         // ---- epilogue 0: a1 = relu(D / s + b0) -> A fragments (pre-scaled by SA); sign bits for the backward
         Frags<NS1> a1;
         {
             uint32_t bw0[4], bw1[4];
-            relu_to_frags<ARITH>(acc, kInvL0, sBias, t, a1, bw0, bw1, mx);
+            relu_to_frags(acc, kInvL0, sBias, t, a1, bw0, bw1, mx);
             if (SAVE) store_bits(tw.relu_bits, 0, n, g0, g1, t, bw0, bw1);
         }
         if (t == 0) {
@@ -371,25 +329,18 @@ deform_tc_kernel(DeformDesc d, TcWeights tw, TcSmem Ls, const CameraDev* __restr
 #pragma unroll 1
         for (int k = 0; k < m_heads; ++k) {
             const int h = (int)((hseq >> (3 * k)) & 7u);
-            // ---- layer 1: D = a1 W1^T, K-part by K-part out of the ring
-#pragma unroll 1
-            for (int p = 0; p < A::PH; ++p, ++u) {
+            // ---- layer 1: D = a1 W1^T, W1 out of the ring
+            {
                 if (tid == 0 && u + 1 < total_items) issue(u + 1);
                 __syncwarp();
                 const uint32_t s = u & 1u;
                 const long long t0 = dbg ? clock64() : 0;
                 mbar_wait(bar_full + s, (u >> 1) & 1u);
                 if (dbg) t_wait += clock64() - t0;
-                const uint32_t b = sW1 + s * Ls.part_bytes;
-                if constexpr (A::PH == 1) {
-                    gemm3<ARITH, 128, NS1, NSP>(acc, a1, 0, b, b + Ls.part_bytes / 2, 128 / A::PH, false);
-                } else {
-                    // (runtime part index into a register array: unrolled over the parts)
-#pragma unroll
-                    for (int pp = 0; pp < A::PH; ++pp)
-                        if (pp == p) gemm3<ARITH, 128, NS1, NSP>(acc, a1, pp * NSP, b, b + Ls.part_bytes / 2, 128 / A::PH, pp != 0);
-                }
+                const uint32_t b = sW1 + s * Ls.slot_bytes;
+                gemm3<128, NS1>(acc, a1, b, b + Ls.slot_bytes / 2, 128);
                 if (lane == 0) mbar_arrive(bar_empty + s);      // this warp's MMAs have retired: the slot may be refilled
+                ++u;
             }
             uint32_t bw0[4], bw1[4];
             if (h < 4) {
@@ -439,9 +390,9 @@ deform_tc_kernel(DeformDesc d, TcWeights tw, TcSmem Ls, const CameraDev* __restr
             } else {
                 // ---- SH head (always last: a1 is dead once its layer-1 GEMM has retired): hidden layer -> A fragments,
                 //      layer 2 as a GEMM with N = 48, SH deltas to the stage
-                relu_to_frags<ARITH>(acc, kInvHS, sBias + 128 + 4 * 128, t, a1, bw0, bw1, mx);
+                relu_to_frags(acc, kInvHS, sBias + 128 + 4 * 128, t, a1, bw0, bw1, mx);
                 float acc2[24];
-                gemm3<ARITH, 48, NS1, NS1>(acc2, a1, 0, sW2, sW2 + 48u * 128u * A::ES, 128, false);
+                gemm3<48, NS1>(acc2, a1, sW2, sW2 + 48u * 128u * A::ES, 128);
                 const float* b2sh = b2s + 16;
 #pragma unroll
                 for (int j = 0; j < 6; ++j) {
@@ -500,7 +451,7 @@ deform_tc_kernel(DeformDesc d, TcWeights tw, TcSmem Ls, const CameraDev* __restr
         bar_sync(1 + wgi, 128);   // the stage is read before the next tile's deltas overwrite it
     }
     // range check of everything that went through an f16 conversion (already in operand units)
-    if (ARITH == 2 && mx >= kF16Max && tw.status) *reinterpret_cast<volatile uint32_t*>(tw.status) = 1u;
+    if (mx >= kF16Max && tw.status) *reinterpret_cast<volatile uint32_t*>(tw.status) = 1u;
     if (dbg) { tw.dbg[blockIdx.x * 12] = clock64() - t_start; tw.dbg[blockIdx.x * 12 + 1] = t_wait; tw.dbg[blockIdx.x * 12 + 2] = NWG; }
 }
 
@@ -623,51 +574,48 @@ cudaError_t launch_deform_features(const DeformDesc& d, int64_t n, const float* 
     return cudaErrorInvalidValue;
 }
 
-bool tc_deform_supported(const G4DDeformParams& prm, int arith) {
+bool tc_deform_supported(const G4DDeformParams& prm) {
     const int C = prm.channels, L = prm.levels;
     if (prm.net_width != 128 || prm.depth > 1) return false;   // no trunk layers (deep trunks: the FFMA kernels)
     if (!((C == 16 && (L == 2 || L == 3)) || (C == 32 && L == 2))) return false;
-    return tc_warpgroups(arith, C * L, (prm.head_mask & G4D_HEAD_SHS) != 0) != 0;
+    return tc_warpgroups(C * L, (prm.head_mask & G4D_HEAD_SHS) != 0) != 0;
 }
 
-template <int ARITH, int NWG, int MODE, int C, int L>
+template <int NWG, int MODE, int C, int L>
 static cudaError_t launch_deform_tc_t(const DeformDesc& d, const TcWeights& tw, const CameraDev* cam, int64_t n, const DeformIO& io,
                                       int sm_count, cudaStream_t st) {
-    const TcSmem Ls = tc_smem_layout(ARITH, NWG, d.F, (d.head_mask & G4D_HEAD_SHS) != 0);
+    const TcSmem Ls = tc_smem_layout(NWG, d.F, (d.head_mask & G4D_HEAD_SHS) != 0);
     const size_t bytes = Ls.total;
     const int64_t ntiles = (n + 64 * NWG - 1) / (64 * NWG);
     const int grid = (int)(ntiles < sm_count ? ntiles : sm_count);
     cudaError_t e;
     if (tw.relu_bits) {
-        e = cudaFuncSetAttribute(deform_tc_kernel<ARITH, NWG, MODE, C, L, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+        e = cudaFuncSetAttribute(deform_tc_kernel<NWG, MODE, C, L, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
         if (e != cudaSuccess) return e;
-        return launch_k(deform_tc_kernel<ARITH, NWG, MODE, C, L, true>, dim3(grid), dim3(NWG * 128), bytes, st, true, d, tw, Ls, cam, n, io);
+        return launch_k(deform_tc_kernel<NWG, MODE, C, L, true>, dim3(grid), dim3(NWG * 128), bytes, st, true, d, tw, Ls, cam, n, io);
     }
-    e = cudaFuncSetAttribute(deform_tc_kernel<ARITH, NWG, MODE, C, L, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    e = cudaFuncSetAttribute(deform_tc_kernel<NWG, MODE, C, L, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
     if (e != cudaSuccess) return e;
-    return launch_k(deform_tc_kernel<ARITH, NWG, MODE, C, L, false>, dim3(grid), dim3(NWG * 128), bytes, st, true, d, tw, Ls, cam, n, io);
+    return launch_k(deform_tc_kernel<NWG, MODE, C, L, false>, dim3(grid), dim3(NWG * 128), bytes, st, true, d, tw, Ls, cam, n, io);
 }
 
 cudaError_t launch_deform_tc(const DeformDesc& d, const TcWeights& tw, int mode, const CameraDev* cam, int64_t n,
                              const DeformIO& io, int sm_count, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
     if (!tw.feat) return cudaErrorInvalidValue;
-    const int nwg = tc_warpgroups(tw.arith, d.F, (d.head_mask & G4D_HEAD_SHS) != 0);
-    // the (C, L, warpgroups) that tc_warpgroups can choose: F = 32 always fits three FP16x2 warpgroups, F = 48 / 64 fit
-    // three without the SH head and two with it
-#define G4D_TC_CASE(AR, NW, CC, LL)                                                                                          \
-    if (tw.arith == AR && nwg == NW && d.C == CC && d.levels == LL)                                                          \
-        return mode == 0                   ? launch_deform_tc_t<AR, NW, 0, CC, LL>(d, tw, cam, n, io, sm_count, st)         \
-               : io.sh.m == kShCoeffs ? launch_deform_tc_t<AR, NW, 1, CC, LL>(d, tw, cam, n, io, sm_count, st)         \
-                                      : launch_deform_tc_t<AR, NW, 2, CC, LL>(d, tw, cam, n, io, sm_count, st);
-    G4D_TC_CASE(2, 3, 16, 2)
-    G4D_TC_CASE(2, 3, 16, 3)
-    G4D_TC_CASE(2, 2, 16, 3)
-    G4D_TC_CASE(2, 3, 32, 2)
-    G4D_TC_CASE(2, 2, 32, 2)
-    G4D_TC_CASE(1, 1, 16, 2)
-    G4D_TC_CASE(1, 1, 16, 3)
-    G4D_TC_CASE(1, 1, 32, 2)
+    const int nwg = tc_warpgroups(d.F, (d.head_mask & G4D_HEAD_SHS) != 0);
+    // the (C, L, warpgroups) that tc_warpgroups can choose: F = 32 always fits three warpgroups, F = 48 / 64 fit three
+    // without the SH head and two with it
+#define G4D_TC_CASE(NW, CC, LL)                                                                                              \
+    if (nwg == NW && d.C == CC && d.levels == LL)                                                                            \
+        return mode == 0                   ? launch_deform_tc_t<NW, 0, CC, LL>(d, tw, cam, n, io, sm_count, st)             \
+               : io.sh.m == kShCoeffs ? launch_deform_tc_t<NW, 1, CC, LL>(d, tw, cam, n, io, sm_count, st)             \
+                                      : launch_deform_tc_t<NW, 2, CC, LL>(d, tw, cam, n, io, sm_count, st);
+    G4D_TC_CASE(3, 16, 2)
+    G4D_TC_CASE(3, 16, 3)
+    G4D_TC_CASE(2, 16, 3)
+    G4D_TC_CASE(3, 32, 2)
+    G4D_TC_CASE(2, 32, 2)
 #undef G4D_TC_CASE
     return cudaErrorInvalidValue;
 }

@@ -213,23 +213,22 @@ constexpr uint32_t kReluBitsTag = 0x5A5A5A5Au;
 constexpr int kReluBitsTagByte = 0x5A;
 static_assert(kReluBitsTag == 0x01010101u * (uint32_t)kReluBitsTagByte, "the tag is one byte repeated");
 
-// tensor-core weight images (g4d_deform_tc.cu): (hi | lo) parts in the canonical K-major shared-memory layout (tc_wgmma.cuh),
-// FP16x2 (scaled f16) or 3xTF32 words
+// tensor-core weight images (g4d_deform_tc.cu): (hi | lo) pairs of scaled f16 words in the canonical K-major shared-memory
+// layout (tc_wgmma.cuh)
 struct TcWeights {
     const float* w0;                   // packed (hi | lo), [128][F]
-    const float* w1[G4D_NUM_HEADS];    // packed (hi | lo) K-parts, [128][128]
+    const float* w1[G4D_NUM_HEADS];    // packed (hi | lo), [128][128]
     const float* w2[G4D_NUM_HEADS];    // SH head only: packed (hi | lo), [48][128]
     long long* dbg;                    // optional [grid][12] per-phase cycle counters (debug)
     float* feat;                       // the HexPlane features [N][F] and the walk order that gathered them (launch_deform's
     const uint32_t* order;             // DeformGather)
     uint32_t* relu_bits;             // optional [6][N][4]: ReLU sign bits saved for the backward (G4D_RELU_BITS_WORDS)
-    int arith;                         // 1: 3xTF32, 2: FP16x2 (G4D_OPT_TENSOR_CORES)
     uint32_t* status;                  // host-mapped word: set to 1 by the FP16x2 kernel when a value left the f16 operand range
 };
 
 size_t tc_packed_floats(const G4DDeformParams& prm);
-cudaError_t launch_tc_pack_weights(const G4DDeformParams& prm, int arith, float* blob, TcWeights* out, cudaStream_t st);
-bool tc_deform_supported(const G4DDeformParams& prm, int arith);
+cudaError_t launch_tc_pack_weights(const G4DDeformParams& prm, float* blob, TcWeights* out, cudaStream_t st);
+bool tc_deform_supported(const G4DDeformParams& prm);
 // HexPlane gather xyz -> feat [N][F] fp32, Gaussians visited in `order` (NULL: index order; feat[g] stays at row g either
 // way); pdl: launched dependent on the previous kernel of the forward chain (DESIGN.md §4.6)
 cudaError_t launch_deform_features(const DeformDesc& d, int64_t n, const float* xyz, const uint32_t* order, float* feat, bool pdl,

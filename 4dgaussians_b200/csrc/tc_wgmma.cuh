@@ -1,6 +1,6 @@
 // tc_wgmma.cuh -- hand-written Hopper tensor-core building blocks (inline PTX, sm_90a): warpgroup MMAs (wgmma.mma_async)
 // with the A operand in registers (RS) or shared memory (SS) and the B operand in shared memory, the shared-memory matrix
-// descriptor, and the operand splits that keep fp32-level accuracy with 16-bit / TF32 multiplies (x = hi + lo, three
+// descriptor, and the operand splits that keep fp32-level accuracy with 16-bit multiplies (x = hi + lo, three
 // products lo*hi + hi*lo + hi*hi, fp32 accumulation): the reference MLP is plain fp32 (scene/deformation.py:80-142).
 //
 // Fragments (one warpgroup = 4 warps computes a 64 x N tile; warp w owns rows 16w..16w+15, lane = 4 g + t):
@@ -8,17 +8,14 @@
 //                          d[4j + 2, 3] = row g + 8, same columns
 //   A, 16-bit, K = 16:     a[0] = (g, 2t | 2t+1)  a[1] = (g+8, 2t | 2t+1)  a[2] = (g, 2t+8 | 2t+9)  a[3] = (g+8, 2t+8 | 2t+9)
 //                          (low half = even column), i.e. accumulator columns 16s..16s+15 ARE the A fragment of K-slice s
-//   A, TF32, K = 8:        a[0] = (g, t)  a[1] = (g+8, t)  a[2] = (g, t+4)  a[3] = (g+8, t+4); an accumulator block
-//                          j maps onto K-slice j as (d0, d2, d1, d3), i.e. with the K order of the slice permuted
-//                          (tf32_kperm): the B operand of such a GEMM is packed in that order.
 //
 // Shared-memory operands use the no-swizzle ("interleave") canonical layout: core matrices of 8 rows x 16 bytes stored
 // as 128 contiguous bytes.  An image [rows][cols] (cols contiguous in the source) is stored
-//     off(row, col) = (row / 8) * (cols / E) * 128 + (col / E) * 128 + (row % 8) * 16 + (col % E) * S
-// with E elements of S bytes per 16-byte core row (E = 8 for 16-bit types, 4 for TF32).
+//     off(row, col) = (row / 8) * (cols / 8) * 128 + (col / 8) * 128 + (row % 8) * 16 + (col % 8) * 2
+// (8 elements of 2 bytes per 16-byte core row: img16_off).
 //   * read K-major (rows = M or N, cols = K):   LBO = 128 (K-adjacent cores), SBO = (cols / E) * 128; one K step of
 //     two cores advances the start address by 256 bytes;
-//   * read MN-major (rows = K, cols = M or N; 16-bit types only, transpose flag set): LBO = (cols / 8) * 128 (K-adjacent
+//   * read MN-major (rows = K, cols = M or N, transpose flag set): LBO = (cols / 8) * 128 (K-adjacent
 //     cores), SBO = 128 (MN-adjacent cores); one K = 16 step advances the start address by 2 * LBO.
 #pragma once
 #include <cuda_runtime.h>
@@ -42,11 +39,6 @@ __device__ __forceinline__ uint64_t desc_mnmajor(uint32_t saddr, uint32_t cols) 
 __host__ __device__ constexpr uint32_t img16_off(uint32_t row, uint32_t col, uint32_t ncols) {
     return (row >> 3) * ((ncols >> 3) * 128u) + (col >> 3) * 128u + (row & 7u) * 16u + (col & 7u) * 2u;
 }
-__host__ __device__ constexpr uint32_t img32_off(uint32_t row, uint32_t col, uint32_t ncols) {
-    return (row >> 3) * ((ncols >> 2) * 128u) + (col >> 2) * 128u + (row & 7u) * 16u + (col & 3u) * 4u;
-}
-// K position inside an 8-wide TF32 slice that holds hidden unit `c` when the A fragment comes from an accumulator
-__host__ __device__ constexpr uint32_t tf32_kperm(uint32_t c) { return (c & ~7u) | ((c & 1u) ? 4u + ((c & 7u) >> 1) : ((c & 7u) >> 1)); }
 
 // ---- ordering ----------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
@@ -67,15 +59,6 @@ __device__ __forceinline__ void fence_regs(uint32_t (&d)[M]) {
 }
 
 // ---- operand splits ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t tf32_rna(float x) {
-    uint32_t r;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-    return r;
-}
-__device__ __forceinline__ void tf32_split(float x, uint32_t& hi, uint32_t& lo) {
-    hi = tf32_rna(x);
-    lo = tf32_rna(x - __uint_as_float(hi));
-}
 __device__ __forceinline__ uint16_t bf16_rn(float x) {
     uint16_t r;
     asm("cvt.rn.bf16.f32 %0, %1;" : "=h"(r) : "f"(x));
@@ -103,49 +86,8 @@ __device__ __forceinline__ void f16_split2(float a, float b, uint32_t& hi, uint3
 template <int NS>
 struct Frags { uint32_t hi[NS][4], lo[NS][4]; };
 
-// ---- one wgmma each: D[64 x N] (+)= A[64 x K] * B, K = 8 (TF32) or 16 (F16 / BF16); acc = 0 overwrites D ---------------
-//   *_rs: A = fragment registers;  *_ss: A = descriptor.  TA / TB = 1: that operand is MN-major (16-bit types only).
-
-__device__ __forceinline__ void mma_tf32_rs_n16(float (&d)[8], const uint32_t (&a)[4], uint64_t b, uint32_t acc) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %13, 0;\n"
-        "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1;\n}\n"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
-}
-
-__device__ __forceinline__ void mma_tf32_rs_n48(float (&d)[24], const uint32_t (&a)[4], uint64_t b, uint32_t acc) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %29, 0;\n"
-        "wgmma.mma_async.sync.aligned.m64n48k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, {%24, %25, %26, %27}, %28, p, 1, 1;\n}\n"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
-}
-
-__device__ __forceinline__ void mma_tf32_rs_n128(float (&d)[64], const uint32_t (&a)[4], uint64_t b, uint32_t acc) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %69, 0;\n"
-        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1;\n}\n"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
-}
-
-template <int N>
-__device__ __forceinline__ void mma_tf32_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t b, uint32_t acc) {
-    static_assert(N == 16 || N == 48 || N == 128, "unsupported N");
-    if constexpr (N == 16) mma_tf32_rs_n16(d, a, b, acc);
-    else if constexpr (N == 48) mma_tf32_rs_n48(d, a, b, acc);
-    else if constexpr (N == 128) mma_tf32_rs_n128(d, a, b, acc);
-}
+// ---- one wgmma each: D[64 x N] (+)= A[64 x K] * B, K = 16 (F16 / BF16); acc = 0 overwrites D -------------------------
+//   *_rs: A = fragment registers;  *_ss: A = descriptor.  TA / TB = 1: that operand is MN-major.
 
 template <int TB>
 __device__ __forceinline__ void mma_f16_rs_n16(float (&d)[8], const uint32_t (&a)[4], uint64_t b, uint32_t acc) {

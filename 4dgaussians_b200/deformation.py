@@ -207,7 +207,7 @@ class deform_network(nn.Module):
                 p.data = p.data.float().contiguous()
 
     def param_version(self, fresh: bool = False) -> int:
-        """Key of the library's packed weight images (transposes / TF32 / BF16 operand images of the MLP weights).
+        """Key of the library's packed weight images (transposes / FP16 / BF16 operand images of the MLP weights).
 
         It changes whenever a parameter tensor was replaced or modified through an op that bumps ``Tensor._version``
         (``load_state_dict``, ``copy_``, foreach / plain optimizers), whenever the head mask changes, after

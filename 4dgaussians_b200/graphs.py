@@ -216,5 +216,5 @@ class GraphedRender:
                                 "min_capacity)" % (ERR_OVERFLOW, s.overflows, s.max_instances))
         if s.f16_range:
             raise _lib.G4DError("graphed render failed (code %d): an FP16x2 tensor-core launch met a value outside the f16 "
-                                "operand range; its results were saturated (G4D_OPT_TENSOR_CORES = 1 avoids the limit)"
+                                "operand range; its results were saturated (G4D_OPT_TENSOR_CORES = 0, the FFMA kernels, has no range limit)"
                                 % ERR_OVERFLOW)

@@ -48,7 +48,8 @@ enum {
     G4D_ERR_NOMEM = -3,     /* device allocation failed */
     G4D_ERR_STATE = -4,     /* backward without a matching forward, ... */
     G4D_ERR_OVERFLOW = -5   /* tile-instance buffer overflowed in no-sync mode (re-run with sync), or an FP16x2 tensor-core
-                             * launch met a value outside the f16 operand range (G4D_OPT_TENSOR_CORES) */
+                             * launch met a value outside the f16 operand range (G4D_OPT_TENSOR_CORES = 2; 0 has no
+                             * range limit) */
 };
 
 enum { /* bits of G4DDeformParams.head_mask: a set bit means the head is ACTIVE (not no_dx etc.) */
@@ -282,8 +283,9 @@ enum { G4D_OPT_SYNC_MODE = 1,  /* 1 (default): size the instance buffer exactly 
        G4D_OPT_TENSOR_CORES = 5, /* the deformation MLP's forward when the configuration allows tensor cores (net_width 128,
                                    C in {16,32}, F <= 64, and no trunk layers): 2 (default) wgmma with FP16x2 operands (hi + lo halves, 3 products,
                                    fp32-accurate; operands must stay below 65504 after scaling -- activations < 8188, features
-                                   < 1023, weights < 255 -- else the NEXT call returns G4D_ERR_OVERFLOW); 1: wgmma 3xTF32 (no
-                                   range limit); 0: FP32 FFMA kernels.  The tensor-core kernels take the network with
+                                   < 1023, weights < 255 -- else the NEXT call returns G4D_ERR_OVERFLOW); 0: FP32 FFMA
+                                   kernels (no range limit).  1 (3xTF32, removed) returns G4D_ERR_ARG and changes nothing;
+                                   any other value selects 2.  The tensor-core kernels take the network with
                                    no trunk layers (depth <= 1); a deeper one runs on the FFMA kernels whatever the value */
        G4D_OPT_TC_DEBUG = 6,     /* 1: the tensor-core forward records counters per CTA (g4d_debug_tc_cycles: [0] cycles of the
                                    whole kernel, [1] cycles waiting for W1 images, [2] the CTA's consumer warpgroups, [3..11]

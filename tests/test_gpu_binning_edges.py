@@ -108,7 +108,7 @@ def test_depth_range_extremes_preprocess_kernel(n):
         _assert_extremes(ref, near, far)
 
 
-FUSED_PATHS = {"ffma": dict(net="small64", tc=0), "fp16x2": dict(net="small128", tc=2), "tf32x3": dict(net="small128", tc=1),
+FUSED_PATHS = {"ffma": dict(net="small64", tc=0), "fp16x2": dict(net="small128", tc=2),
                "coarse": dict(net="small128", tc=2, stage="coarse"), "cameras3": dict(net="small128", tc=2, cameras=3)}
 _MODULES = {}
 
@@ -123,7 +123,7 @@ def _module(net):
 @pytest.mark.parametrize("path", list(FUSED_PATHS))
 @pytest.mark.parametrize("n", ub.EXTREME_NS)
 def test_depth_range_extremes_fused_paths(path, n):
-    """render() fine stage on the FFMA and both tensor-core kernels, the coarse stage, and render_cameras' extra cameras
+    """render() fine stage on the FFMA and the tensor-core kernels, the coarse stage, and render_cameras' extra cameras
     (project_cameras_kernel): the oracle runs on the GPU's own deformed tensors"""
     p = FUSED_PATHS[path]
     stage = p.get("stage", "fine")

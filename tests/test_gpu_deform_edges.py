@@ -3,8 +3,8 @@ outside the AABB and at NaN / inf, the time-row collapse and distribution at the
 zero, negative or span 1e-6 .. 1e2, one texel hit by 65536 Gaussians, the FP16x2 operand range on both sides of its limits,
 tile tails of every engine, partial upstream gradients, and gradient sinks the scatter cannot take.
 
-Engines: forward FFMA (G4D_OPT_TENSOR_CORES = 0) at net_width 64 and 128, 3xTF32 (1) and FP16x2 (2); backward FFMA and BF16x2
-(the tensor-core backward, after either tensor-core forward).  The scenes' cells are exact in fp32 and fp64, so only rows near a
+Engines: forward FFMA (G4D_OPT_TENSOR_CORES = 0) at net_width 64 and 128 and FP16x2 (2); backward FFMA and BF16x2
+(the tensor-core backward, after the tensor-core forward).  The scenes' cells are exact in fp32 and fp64, so only rows near a
 ReLU kink are masked (util_deep_network.kink_rows with the texel-line test off)."""
 import ctypes as C
 import importlib
@@ -32,7 +32,7 @@ F16_LIMIT = "f16 operand range"
 # a half-tile FFMA configuration (L = 3, C = 20, all heads) and a D = 2 trunk
 TC_NETS = [ue.Net("small128", ue.RES[0]), ue.Net("small128", ue.RES[1], (1, 2, 4)), ue.Net("c32w128sh", ue.RES[2])]
 FFMA_NETS = [ue.Net("small64", ue.RES[1]), ue.Net("c20w128sh", ue.RES[0], (1, 2, 4)), ue.Net("deep64", ue.RES[2], depth=2)]
-ENGINES = [(n, 0) for n in TC_NETS + FFMA_NETS] + [(n, tc) for n in TC_NETS for tc in (1, 2)]
+ENGINES = [(n, 0) for n in TC_NETS + FFMA_NETS] + [(n, 2) for n in TC_NETS]
 SEEN = {}                          # worst row error per case group (printed with -s; DESIGN.md §4.4 quotes one run)
 
 
@@ -178,7 +178,7 @@ def _check_vs_oracle(mod, ins, probes, t, tc, group, backward=True, conditioned=
 def test_faces_and_plane_values_vs_oracle(net, tc, kind):
     """faces, one ulp inside them, outside, edges, corners, the last texel, res = 2 axes: forward and backward per Gaussian
     against fp64.  A face row takes no coordinate gradient from the planes: d(xyz) there is the residual's alone, bit for
-    bit.  (wide planes leave the FP16x2 range: they run on the 3xTF32 and FFMA forwards.)"""
+    bit.  (wide planes leave the FP16x2 range: they run on the FFMA forward.)"""
     if kind == "wide" and tc == 2:
         pytest.skip("features up to 1e12 are outside the FP16x2 operand range by design")
     mod = ue.make_edge_module(net, seed=3)
@@ -460,10 +460,10 @@ def test_fp16x2_tiny_features_within_the_absolute_floor():
 
 
 # --------------------------------------------------------------------------------------------------- tiles
-# (net, engine, tile sizes in Gaussians): the tensor-core forwards (FP16x2: 128 per CTA pass as two warpgroups of 64; 3xTF32:
-# 64) and the BF16x2 backward (128) at W = 128; the FFMA kernels at W = 64 (128 per tile) and in half tiles (C = 20, L = 3,
-# every head, D = 2: 32 per tile)
-TILE_CASES = [(ue.Net("small128", ue.RES[0]), 1, (64, 128)), (ue.Net("small128", ue.RES[0]), 2, (64, 128)),
+# (net, engine, tile sizes in Gaussians): the tensor-core forward (FP16x2: 128 per CTA pass as two warpgroups of 64) and the
+# BF16x2 backward (128) at W = 128; the FFMA kernels at W = 64 (128 per tile) and in half tiles (C = 20, L = 3, every head,
+# D = 2: 32 per tile)
+TILE_CASES = [(ue.Net("small128", ue.RES[0]), 2, (64, 128)),
               (ue.Net("small64", ue.RES[1]), 0, (128,)), (ue.Net("c20w128sh", ue.RES[0], (1, 2, 4), depth=2), 0, (32,))]
 
 

@@ -464,7 +464,7 @@ def test_batched_views_single_backward_matches_per_view_backward():
 @pytest.mark.parametrize("fused_opt", [True, False])
 def test_optimizer_updates_are_seen_by_the_next_forward(net, fused_opt):
     """torch.optim.Adam(fused=True) updates the MLP weights WITHOUT bumping Tensor._version: the library's packed weight
-    images (TF32 / BF16 operand images, FFMA transposes) must still follow -- training forwards rebuild them.  After a few
+    images (FP16 / BF16 operand images, FFMA transposes) must still follow -- training forwards rebuild them.  After a few
     optimizer steps the module must render exactly like a fresh module that loaded its state_dict."""
     c = dict(FUSED_CASES[2]); c["net"] = net
     scene, mod, pc, cam = _fused_setup(c)
@@ -579,14 +579,14 @@ def test_full_size_binning_properties():
 
 
 # --------------------------------------------------------------------------------------------------- tensor cores
-def test_wgmma_building_blocks_selftest():
+def test_wgmma_fp16x2_bf16x2_building_blocks_selftest():
     """D[128,N] = A[128,K] B[N,K]^T through the wgmma building blocks in every operand arrangement the kernels use (register or
-    shared-memory A, K-major or MN-major operands) with the hi / lo split and three products: fp32-level accuracy for 3xTF32 and
-    FP16x2, ~16 bits for BF16x2."""
+    shared-memory A, K-major or MN-major operands) with the hi / lo split and three products: fp32-level accuracy for FP16x2,
+    ~16 bits for BF16x2.  Mode 0, the removed 3xTF32 arrangement, is refused."""
     import ctypes as C
     lib = g4d._lib.load_selftest()      # own tiny library: the self test is not part of the product libg4d.so
-    tol = {0: 2e-6, 1: 2e-6, 2: 3e-5, 3: 3e-5, 4: 3e-5}
-    for mode in range(5):
+    tol = {1: 2e-6, 2: 3e-5, 3: 3e-5, 4: 3e-5}
+    for mode in tol:
         for (N, K) in ((128, 128), (128, 32), (48, 64), (16, 64), (48, 48)):
             gen = torch.Generator().manual_seed(N + K + mode)
             A = torch.randn(128, K, generator=gen).cuda(); B = torch.randn(N, K, generator=gen).cuda()
@@ -597,13 +597,15 @@ def test_wgmma_building_blocks_selftest():
             ref = A.double() @ B.double().t()
             err = float((D.double() - ref).abs().max() / ref.abs().max())
             assert err <= tol[mode], (mode, N, K, err)
+    cfg = (C.c_int * 3)(N, K, 0)                                        # mode 0 (3xTF32) was removed: refused
+    assert lib.g4d_selftest_wgmma(cfg, A.data_ptr(), B.data_ptr(), D.data_ptr(), 0) == -1
 
 
-@pytest.mark.parametrize("tcmode", [2, 1])
+@pytest.mark.parametrize("tcmode", [2])
 @pytest.mark.parametrize("net,n", [("small128", 1000), ("dynerf", 5000), ("hypernerf", 3000), ("dynerf", 40000)])
 def test_tensor_core_mlp_matches_ffma_path(net, n, tcmode):
-    """The wgmma MLPs (2: FP16x2 operands -- the default; 1: 3xTF32) and the FP32 FFMA MLP are implementations of the same
-    function.  40000 Gaussians = 313 tiles of 128 (FP16x2) / 625 of 64 (3xTF32): persistent CTAs with two to five tiles."""
+    """The wgmma MLP (FP16x2 operands, the default) and the FP32 FFMA MLP are implementations of the same function.  40000
+    Gaussians: persistent CTAs with several tiles each."""
     mod = make_module(net, seed=7)
     ins, _ = _deform_inputs(n, 9)
     ws = g4d._lib.Workspace.get(0)
@@ -647,10 +649,11 @@ def test_tensor_core_paths_corner_cases_vs_oracle(net, n):
         assert e <= 3 * GRAD_TOL, (k, e)
 
 
-def test_fp16x2_range_violation_is_reported_and_tf32_path_has_no_limit():
+def test_fp16x2_range_violation_is_reported_and_ffma_path_has_no_limit():
     """The FP16x2 forward converts (scaled) activations to f16: a hidden activation above 65504 / 8 saturates.  The kernel raises
-    a flag in host-mapped memory and the NEXT tensor-core call returns G4D_ERR_OVERFLOW; the 3xTF32 kernel (option 1) and the
-    FFMA kernels compute the same network without a range limit."""
+    a flag in host-mapped memory and the NEXT tensor-core call returns G4D_ERR_OVERFLOW; the FFMA kernels (option 0) compute
+    the same network without a range limit.  Option 1 (the removed 3xTF32 forward) is refused and leaves the workspace on
+    FP16x2."""
     mod = make_module("small128", seed=11)
     n = 600
     ins, _ = _deform_inputs(n, 4)
@@ -660,14 +663,16 @@ def test_fp16x2_range_violation_is_reported_and_tf32_path_has_no_limit():
         mod.deformation_net.feature_out[0].bias.fill_(2.0e4)           # hidden activations ~2e4 >> 8188
     try:
         with torch.no_grad():
-            ws.set_option(g4d._lib.OPT_TENSOR_CORES, 1)
-            a = [o.clone() for o in mod(*ins, t)]
             ws.set_option(g4d._lib.OPT_TENSOR_CORES, 0)
             b = [o.clone() for o in mod(*ins, t)]
-            for x, y in zip(a, b):
-                assert float((x - y).abs().max()) <= 1e-5 * max(1.0, float(y.abs().max()))
+            cfg, prm = oracle_params_from_module(mod)
+            want = dr.deform_forward(cfg, prm, *[x.cpu() for x in ins], 0.3)
+            for x, y in zip(b, want):
+                assert float((x.cpu() - y).abs().max()) <= 1e-5 * max(1.0, float(y.abs().max()))
             ws.set_option(g4d._lib.OPT_TENSOR_CORES, 2)
-            mod(*ins, t)                                                # saturates; flagged
+            with pytest.raises(g4d._lib.G4DError, match="3xTF32"):
+                ws.set_option(g4d._lib.OPT_TENSOR_CORES, 1)
+            mod(*ins, t)                                                # still FP16x2: saturates; flagged
             torch.cuda.synchronize()
             with pytest.raises(g4d._lib.G4DError, match="f16 operand range"):
                 mod(*ins, t)
@@ -742,7 +747,7 @@ def test_no_grad_render_skips_saved_tensors_unless_asked():
     assert torch.equal(img0, img1)
 
 
-@pytest.mark.parametrize("tcmode", [2, 1])
+@pytest.mark.parametrize("tcmode", [2])
 @pytest.mark.parametrize("net,n", [("small128", 700), ("dynerf", 21000), ("hypernerf", 40000)])
 def test_tensor_core_backward_matches_ffma_path(net, n, tcmode):
     """BF16x2 wgmma backward (dgrad + wgrad kernels) against the FP32 FFMA backward: same gradients for every input

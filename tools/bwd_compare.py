@@ -25,14 +25,14 @@ for net, n in [("small128", 700), ("dynerf", 21000), ("hypernerf", 40000)]:
     ws = g4d._lib.Workspace.get(0)
     t = torch.tensor(0.27).repeat(n, 1).cuda()
     res = []
-    for tc in (1, 0, 1):
+    for tc in (2, 0, 2):
         ws.set_option(g4d._lib.OPT_TENSOR_CORES, tc)
         mod.zero_grad(set_to_none=True)
         dev_in = [x.clone().requires_grad_(True) for x in ins]
         outs = mod(*dev_in, t)
         sum((o * p.cuda()).sum() for o, p in zip(outs, probes)).backward()
         res.append(([x.grad.clone() for x in dev_in], {k: p.grad.clone() for k, p in mod.named_parameters() if p.grad is not None}))
-    ws.set_option(g4d._lib.OPT_TENSOR_CORES, 1)
+    ws.set_option(g4d._lib.OPT_TENSOR_CORES, 2)
     print("====", net, n)
     for nm, a, b, c in zip(("xyz", "scales", "rot", "opacity", "shs"), res[0][0], res[1][0], res[2][0]):
         print("  in  %-10s tc-vs-ffma bulk/max %.2e %.2e   tc-vs-tc %.2e" % ((nm,) + rel_err_bulk(a.cpu().numpy(), b.cpu().numpy())
