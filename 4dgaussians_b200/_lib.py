@@ -41,7 +41,7 @@ ABI_SYMBOLS = [
     "g4d_context_stage_times", "g4d_debug_tc_cycles", "g4d_l1_loss", "g4d_l1_loss_backward", "g4d_ssim", "g4d_ssim_backward",
     "g4d_plane_regulation", "g4d_dist2_knn3", "g4d_adam_step", "g4d_render_forward_cameras", "g4d_render_backward_cameras",
     "g4d_context_set_time_source", "g4d_workspace_freeze", "g4d_workspace_graph_status", "g4d_adam_scalars",
-    "g4d_adam_step_device",
+    "g4d_adam_step_device", "g4d_deform_forward_times", "g4d_deform_backward_times",
 ]
 
 fp = C.c_void_p   # device pointers travel as integers
@@ -143,6 +143,9 @@ def load():
             [fp] * 6 + [C.c_void_p]
         lib.g4d_deform_backward.argtypes = [C.c_void_p, C.POINTER(DeformParams), C.POINTER(DeformGrads), C.c_int64, fp,
                                             C.c_float] + [fp] * 11 + [C.c_void_p]
+        lib.g4d_deform_forward_times.argtypes = [C.c_void_p, C.POINTER(DeformParams), C.c_int64] + [fp] * 12 + [C.c_void_p]
+        lib.g4d_deform_backward_times.argtypes = [C.c_void_p, C.POINTER(DeformParams), C.POINTER(DeformGrads), C.c_int64] + \
+            [fp] * 14 + [C.c_void_p]
         lib.g4d_rasterize_forward.argtypes = [C.c_void_p, C.POINTER(Camera), C.c_int64] + [fp] * 8 + [C.c_void_p]
         lib.g4d_rasterize_backward.argtypes = [C.c_void_p, C.POINTER(Camera), C.c_int64] + [fp] * 12 + [C.c_void_p]
         lib.g4d_render_forward.argtypes = [C.c_void_p, C.POINTER(Camera), C.POINTER(DeformParams), C.POINTER(Gaussians),

@@ -36,6 +36,8 @@ struct DeformDesc {
     int ntrunk;                               // trunk layers behind W0: max(defor_depth, 1) - 1
     const float* wtt[G4D_MAX_DEPTH - 1];      // packed [WD][WD]: W_j^T of trunk layer j = 1 .. ntrunk
     const float* bt[G4D_MAX_DEPTH - 1];       // [WD]
+    const float* times;                       // [N] one time per Gaussian (the per-row gather and scatter; trow unused),
+                                              // or NULL: every Gaussian at the time of the collapsed rows trow
 };
 
 // shared-memory carve-up (offsets in floats), computed on the host by deform_smem_layout()

@@ -438,20 +438,23 @@ int collapse_time_rows(DevBuf& rows, float* (*trow)[3], const G4DDeformParams* p
 
 // Pick the forward's path from the params, bring the gather's walk order over xyz [n] up to date, collapse the time rows and
 // bring the weight images the path reads up to date.  The desc is built after that refresh, which may move
-// the transposes it embeds.
+// the transposes it embeds.  times (device [n], one time per Gaussian): no time rows; the gather samples each Gaussian at its
+// own time, and `time` is not used.
 int setup_deform(G4DWorkspace* ws, const G4DDeformParams* p, const float* xyz, int64_t n, DevBuf& rows, float* (*trow)[3],
-                 TimeArg time, cudaStream_t st, DeformSetup* out) {
+                 TimeArg time, const float* times, cudaStream_t st, DeformSetup* out) {
     int rc;
     out->tc = ws->tensor_cores != 0 && tc_deform_supported(*p);
     if ((rc = gather_order(ws, p->aabb, xyz, n, st, &out->gather.order)) != G4D_OK) return rc;
-    if ((rc = collapse_time_rows(rows, trow, p, time, st)) != G4D_OK) return rc;
+    if (!times && (rc = collapse_time_rows(rows, trow, p, time, st)) != G4D_OK) return rc;
     if (!out->tc) {
         if ((rc = refresh_packed(ws, p, st)) != G4D_OK) return rc;
         out->d = make_desc(p, trow, &ws->packed.img);
+        out->d.times = times;
         return G4D_OK;
     }
     if ((rc = refresh_tc(ws, p, st)) != G4D_OK) return rc;
     out->d = make_desc(p, trow, nullptr);
+    out->d.times = times;
     out->tw = ws->tc.img;
     if (ws->tc_debug) {   // per-CTA phase cycle counters (g4d_debug_tc_cycles)
         G4D_CUDA(ws->tc_dbg.ensure((size_t)ws->sm_count * 12 * 8));
@@ -475,11 +478,13 @@ int attach_forward_buffers(G4DWorkspace* ws, DeformSetup& s, float* feat, uint32
     return G4D_OK;
 }
 
-// backward of the deformation network with the time rows trow: picks the engine -- tensor-core when the configuration allows,
-// FFMA otherwise -- and brings its weight images up to date; the desc is built after that refresh
+// backward of the deformation network with the time rows trow -- or, times set, at the per-Gaussian times [n] with dL/d(times)
+// into g_times (may be NULL) -- picks the engine -- tensor-core when the configuration allows, FFMA otherwise -- and brings its
+// weight images up to date; the desc is built after that refresh
 int deform_backward_dispatch(G4DWorkspace* ws, const G4DDeformParams* prm, float* const (*trow)[3], const G4DDeformGrads* grads,
-                             TimeArg time, int64_t n, const float* xyz, const float* const go[G4D_NUM_HEADS],
-                             float* const gi[G4D_NUM_HEADS], const uint32_t* relu_bits, const float* saved_feat, cudaStream_t st) {
+                             TimeArg time, const float* times, float* g_times, int64_t n, const float* xyz,
+                             const float* const go[G4D_NUM_HEADS], float* const gi[G4D_NUM_HEADS], const uint32_t* relu_bits,
+                             const float* saved_feat, cudaStream_t st) {
     int rc;
     const bool tc = ws->tensor_cores && tc_backward_supported(*prm);
     if (tc) {
@@ -488,11 +493,12 @@ int deform_backward_dispatch(G4DWorkspace* ws, const G4DDeformParams* prm, float
     } else if ((rc = refresh_packed(ws, prm, st)) != G4D_OK) {
         return rc;
     }
-    const DeformDesc d = make_desc(prm, trow, tc ? nullptr : &ws->packed.img);
+    DeformDesc d = make_desc(prm, trow, tc ? nullptr : &ws->packed.img);
+    d.times = times;
     const uint32_t* order = nullptr;   // the walk order of the backward's own gather (none when the forward's features are kept)
     if (!saved_feat && (rc = gather_order(ws, prm->aabb, xyz, n, st, &order)) != G4D_OK) return rc;
     G4D_CUDA(ws->scratch.ensure(deform_backward_scratch_bytes(d, n, tc)));
-    G4D_CUDA(launch_deform_backward(d, *prm, *grads, tc ? &ws->tc_bwd.img : nullptr, time, n, xyz, go, gi, relu_bits, saved_feat,
+    G4D_CUDA(launch_deform_backward(d, *prm, *grads, tc ? &ws->tc_bwd.img : nullptr, time, n, xyz, go, gi, g_times, relu_bits, saved_feat,
                                     order, ws->scratch.p, ws->sm_count, st));
     return G4D_OK;
 }
@@ -752,26 +758,62 @@ int g4d_context_stats(G4DContext* c, G4DStats* out) {
 }
 
 // ------------------------------------------------------------------------------------------------------
-int g4d_deform_forward(G4DWorkspace* ws, const G4DDeformParams* prm, int64_t n, const float* xyz, const float* scaling,
-                       const float* rotation, const float* opacity, const float* shs, float time, float* out_xyz,
-                       float* out_scaling, float* out_rotation, float* out_opacity, float* out_shs, uint32_t* relu_bits, void* stream) {
-    if (!ws) return fail(G4D_ERR_ARG, "workspace is NULL");
-    int rc = check_params(prm);
-    if (rc != G4D_OK) return rc;
-    if (n < 0 || (n > 0 && (!xyz || !out_xyz))) return fail(G4D_ERR_ARG, "xyz / out_xyz required");
-    if ((prm->head_mask & G4D_HEAD_SHS) && n > 0 && (!shs || !out_shs)) return fail(G4D_ERR_ARG, "shs / out_shs required when the SHS head is active");
+}  // extern "C"
+
+namespace {
+
+// g4d_deform_forward (times NULL: every Gaussian at `time`) and g4d_deform_forward_times (times [n], `time` unused)
+int deform_forward(G4DWorkspace* ws, const G4DDeformParams* prm, int64_t n, const float* xyz, const float* scaling,
+                   const float* rotation, const float* opacity, const float* shs, float time, const float* times, float* out_xyz,
+                   float* out_scaling, float* out_rotation, float* out_opacity, float* out_shs, uint32_t* relu_bits, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     G4D_CUDA(cudaSetDevice(ws->device));
     CallScope scope(ws, st);
     if (scope.rc != G4D_OK) return scope.rc;
+    int rc;
     float* trow[G4D_MAX_LEVELS][3] = {};
     DeformSetup s{};
-    if ((rc = setup_deform(ws, prm, xyz, n, ws->trow, trow, TimeArg{time, nullptr}, st, &s)) != G4D_OK) return rc;
+    if ((rc = setup_deform(ws, prm, xyz, n, ws->trow, trow, TimeArg{time, nullptr}, times, st, &s)) != G4D_OK) return rc;
     if ((rc = attach_forward_buffers(ws, s, nullptr, relu_bits, n, st)) != G4D_OK) return rc;
     const DeformIO io{xyz, scaling, rotation, opacity, caller_sh<ShIn>(kShCoeffs, false, shs), out_xyz, out_scaling, out_rotation, out_opacity,
                       out_shs, GeomBuffers{}, FusedOutputs{}, nullptr};
     G4D_CUDA(launch_deform(s.d, 0, nullptr, n, io, s.gather, ws->sm_count, st, s.tc ? &s.tw : nullptr));
     return G4D_OK;
+}
+
+// the argument checks of g4d_deform_forward / _forward_times
+int check_deform_forward_args(G4DWorkspace* ws, const G4DDeformParams* prm, int64_t n, const float* xyz, const float* shs,
+                              float* out_xyz, float* out_shs) {
+    if (!ws) return fail(G4D_ERR_ARG, "workspace is NULL");
+    int rc = check_params(prm);
+    if (rc != G4D_OK) return rc;
+    if (n < 0 || (n > 0 && (!xyz || !out_xyz))) return fail(G4D_ERR_ARG, "xyz / out_xyz required");
+    if ((prm->head_mask & G4D_HEAD_SHS) && n > 0 && (!shs || !out_shs)) return fail(G4D_ERR_ARG, "shs / out_shs required when the SHS head is active");
+    return G4D_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int g4d_deform_forward(G4DWorkspace* ws, const G4DDeformParams* prm, int64_t n, const float* xyz, const float* scaling,
+                       const float* rotation, const float* opacity, const float* shs, float time, float* out_xyz,
+                       float* out_scaling, float* out_rotation, float* out_opacity, float* out_shs, uint32_t* relu_bits, void* stream) {
+    const int rc = check_deform_forward_args(ws, prm, n, xyz, shs, out_xyz, out_shs);
+    if (rc != G4D_OK) return rc;
+    return deform_forward(ws, prm, n, xyz, scaling, rotation, opacity, shs, time, nullptr, out_xyz, out_scaling, out_rotation,
+                          out_opacity, out_shs, relu_bits, stream);
+}
+
+int g4d_deform_forward_times(G4DWorkspace* ws, const G4DDeformParams* prm, int64_t n, const float* xyz, const float* scaling,
+                             const float* rotation, const float* opacity, const float* shs, const float* d_times, float* out_xyz,
+                             float* out_scaling, float* out_rotation, float* out_opacity, float* out_shs, uint32_t* relu_bits,
+                             void* stream) {
+    const int rc = check_deform_forward_args(ws, prm, n, xyz, shs, out_xyz, out_shs);
+    if (rc != G4D_OK) return rc;
+    if (!d_times) return fail(G4D_ERR_ARG, "d_times is NULL");
+    return deform_forward(ws, prm, n, xyz, scaling, rotation, opacity, shs, 0.f, d_times, out_xyz, out_scaling, out_rotation,
+                          out_opacity, out_shs, relu_bits, stream);
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -933,25 +975,61 @@ int64_t g4d_context_read(G4DContext* c, int which, void* host_dst, int64_t bytes
 }
 
 // ------------------------------------------------------------------------------------------------------
-int g4d_deform_backward(G4DWorkspace* ws, const G4DDeformParams* prm, G4DDeformGrads* grads, int64_t n, const float* xyz,
-                        float time, const float* g_out_xyz, const float* g_out_scaling, const float* g_out_rotation,
-                        const float* g_out_opacity, const float* g_out_shs, float* g_in_xyz, float* g_in_scaling,
-                        float* g_in_rotation, float* g_in_opacity, float* g_in_shs, const uint32_t* relu_bits, void* stream) {
+}  // extern "C"
+
+namespace {
+
+// the argument checks of g4d_deform_backward / _backward_times
+int check_deform_backward_args(G4DWorkspace* ws, const G4DDeformParams* prm, const G4DDeformGrads* grads, int64_t n, const float* xyz) {
     if (!ws) return fail(G4D_ERR_ARG, "workspace is NULL");
     int rc = check_params(prm);
     if (rc != G4D_OK) return rc;
     if (!grads) return fail(G4D_ERR_ARG, "grads is NULL");
     if ((rc = check_plane_grads(prm, grads)) != G4D_OK) return rc;
     if (n < 0 || (n > 0 && !xyz)) return fail(G4D_ERR_ARG, "xyz required");
+    return G4D_OK;
+}
+
+// g4d_deform_backward (times NULL: the time rows at `time`) and g4d_deform_backward_times (times [n], dL/d(times) into g_times)
+int deform_backward(G4DWorkspace* ws, const G4DDeformParams* prm, G4DDeformGrads* grads, int64_t n, const float* xyz, float time,
+                    const float* times, const float* const go[G4D_NUM_HEADS], float* const gi[G4D_NUM_HEADS], float* g_times,
+                    const uint32_t* relu_bits, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     G4D_CUDA(cudaSetDevice(ws->device));
     CallScope scope(ws, st);
     if (scope.rc != G4D_OK) return scope.rc;
+    int rc;
     float* trow[G4D_MAX_LEVELS][3] = {};
-    if ((rc = collapse_time_rows(ws->trow, trow, prm, TimeArg{time, nullptr}, st)) != G4D_OK) return rc;
+    if (!times && (rc = collapse_time_rows(ws->trow, trow, prm, TimeArg{time, nullptr}, st)) != G4D_OK) return rc;
+    return deform_backward_dispatch(ws, prm, trow, grads, TimeArg{time, nullptr}, times, g_times, n, xyz, go, gi, relu_bits, nullptr, st);
+}
+
+}  // namespace
+
+extern "C" {
+
+int g4d_deform_backward(G4DWorkspace* ws, const G4DDeformParams* prm, G4DDeformGrads* grads, int64_t n, const float* xyz,
+                        float time, const float* g_out_xyz, const float* g_out_scaling, const float* g_out_rotation,
+                        const float* g_out_opacity, const float* g_out_shs, float* g_in_xyz, float* g_in_scaling,
+                        float* g_in_rotation, float* g_in_opacity, float* g_in_shs, const uint32_t* relu_bits, void* stream) {
+    const int rc = check_deform_backward_args(ws, prm, grads, n, xyz);
+    if (rc != G4D_OK) return rc;
     const float* go[G4D_NUM_HEADS] = {g_out_xyz, g_out_scaling, g_out_rotation, g_out_opacity, g_out_shs};
     float* gi[G4D_NUM_HEADS] = {g_in_xyz, g_in_scaling, g_in_rotation, g_in_opacity, g_in_shs};
-    return deform_backward_dispatch(ws, prm, trow, grads, TimeArg{time, nullptr}, n, xyz, go, gi, relu_bits, nullptr, st);
+    return deform_backward(ws, prm, grads, n, xyz, time, nullptr, go, gi, nullptr, relu_bits, stream);
+}
+
+int g4d_deform_backward_times(G4DWorkspace* ws, const G4DDeformParams* prm, G4DDeformGrads* grads, int64_t n, const float* xyz,
+                              const float* d_times, const float* g_out_xyz, const float* g_out_scaling, const float* g_out_rotation,
+                              const float* g_out_opacity, const float* g_out_shs, float* g_in_xyz, float* g_in_scaling,
+                              float* g_in_rotation, float* g_in_opacity, float* g_in_shs, float* g_times, const uint32_t* relu_bits,
+                              void* stream) {
+    const int rc = check_deform_backward_args(ws, prm, grads, n, xyz);
+    if (rc != G4D_OK) return rc;
+    if (!d_times) return fail(G4D_ERR_ARG, "d_times is NULL");
+    const float* go[G4D_NUM_HEADS] = {g_out_xyz, g_out_scaling, g_out_rotation, g_out_opacity, g_out_shs};
+    float* gi[G4D_NUM_HEADS] = {g_in_xyz, g_in_scaling, g_in_rotation, g_in_opacity, g_in_shs};
+    return deform_backward(ws, prm, grads, n, xyz, 0.f, d_times, go, gi, g_times, relu_bits, stream);
 }
 
 }  // extern "C"
@@ -994,7 +1072,7 @@ int fused_forward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* pr
     CameraDev* dcam = c->cam.as<CameraDev>();
     DeformSetup s{};
     auto prep = [&] {
-        return prm ? setup_deform(ws, prm, g->xyz, n, c->trow, c->trow_ptr, TimeArg{cam->time, c->time_src}, st, &s) : G4D_OK;
+        return prm ? setup_deform(ws, prm, g->xyz, n, c->trow, c->trow_ptr, TimeArg{cam->time, c->time_src}, nullptr, st, &s) : G4D_OK;
     };
     if ((rc = setup_view(c, cam, c->time_src, n, st, prep)) != G4D_OK) return rc;
     {
@@ -1070,7 +1148,7 @@ int fused_backward_tail(G4DContext* c, const G4DCamera* cam, const G4DDeformPara
     const bool saved = c->fwd.feat_cols != 0;
     {
         StageTimer tm(c, G4D_STAGE_DEFORM_BWD, st);
-        if ((rc = deform_backward_dispatch(c->ws, prm, c->trow_ptr, pgrads, TimeArg{cam->time, c->time_src}, n, g->xyz, go, gi,
+        if ((rc = deform_backward_dispatch(c->ws, prm, c->trow_ptr, pgrads, TimeArg{cam->time, c->time_src}, nullptr, nullptr, n, g->xyz, go, gi,
                                            saved ? c->relu.as<uint32_t>() : nullptr, saved ? c->feat.as<float>() : nullptr,
                                            st)) != G4D_OK) return rc;
     }

@@ -689,9 +689,11 @@ struct BwdScatterDesc {
     float* trow_grad[G4D_MAX_LEVELS][3];
     const float* go[G4D_NUM_HEADS];
     float* gi[G4D_NUM_HEADS];
+    float* g_times;                         // [N] dL/d(times) of the per-row mode (OVERWRITTEN), or NULL
 };
 
-template <int C4>
+// PER_ROW: Gaussian g at its own time d.times[g]; the time planes' gradients go straight to the planes and dL/dt to g_times
+template <int C4, bool PER_ROW>
 __global__ void __launch_bounds__(256, 2) bwd_scatter_kernel(BwdScatterDesc sd, int64_t n, const float* __restrict__ xyz) {
     const DeformDesc& d = sd.d;
     constexpr int LPG = scatter_lanes(C4);
@@ -707,35 +709,44 @@ __global__ void __launch_bounds__(256, 2) bwd_scatter_kernel(BwdScatterDesc sd, 
         for (int64_t i = lo + threadIdx.x; i < hi; i += 256) sd.gi[hh][i] = sd.go[hh] ? sd.go[hh][i] : 0.f;
     }
     float gpix[3] = {0.f, 0.f, 0.f};
+    float gt = 0.f;   // dL/d(times[g]) (PER_ROW): t enters the time planes unnormalised, so d(t_pix)/dt is the tap's gmul
     const AabbNorm nrm(d.aabb);
     if (g < n && (LPG == C4 || v < C4)) {
         float pcs[3];
 #pragma unroll
         for (int a = 0; a < 3; ++a) pcs[a] = nrm(a, xyz[3 * g + a]);
+        const float tg = PER_ROW ? __ldg(d.times + g) : 0.f;
         for (int l = 0; l < d.levels; ++l) {
-            Tap1D tx[3];
+            Tap1D tx[PER_ROW ? 4 : 3];
 #pragma unroll
             for (int a = 0; a < 3; ++a) tx[a] = make_tap(pcs[a], d.res[l][a]);
+            if (PER_ROW) tx[PER_ROW ? 3 : 0] = make_tap(tg, d.res[l][3]);
             const float4 df = __ldg(reinterpret_cast<const float4*>(sd.dfeat + g * d.F + l * d.C + 4 * v));
-            scatter_vector(d.planes[l], d.trow[l], d.res[l], sd.g_planes[l], sd.trow_grad[l], tx, v, C4, df, gpix);
+            scatter_vector<PER_ROW>(d.planes[l], d.trow[l], d.res[l], sd.g_planes[l], sd.trow_grad[l], tx, v, C4, df, gpix, gt);
         }
     }
     // the LPG lanes of a Gaussian are adjacent
 #pragma unroll
     for (int a = 0; a < 3; ++a)
         for (int o = 1; o < LPG; o <<= 1) gpix[a] += __shfl_xor_sync(0xffffffffu, gpix[a], o);
+    if (PER_ROW)
+        for (int o = 1; o < LPG; o <<= 1) gt += __shfl_xor_sync(0xffffffffu, gt, o);
     if (g < n && v == 0 && sd.gi[0]) {
 #pragma unroll
         for (int a = 0; a < 3; ++a) sd.gi[0][g * 3 + a] = (sd.go[0] ? sd.go[0][g * 3 + a] : 0.f) + gpix[a] * nrm.scale[a];
     }
+    if (PER_ROW && g < n && v == 0 && sd.g_times) sd.g_times[g] = gt;
 }
 
 static cudaError_t launch_bwd_scatter(const BwdScatterDesc& sd, int64_t n, const float* xyz, cudaStream_t st) {
     const int C4 = sd.d.C / 4;
     const unsigned grid = (unsigned)((n * scatter_lanes(C4) + 255) / 256);
     switch (C4) {   // every channel width the C-ABI takes: C = 4 .. 32
-#define G4D_SCATTER_CASE(K) \
-        case K: bwd_scatter_kernel<K><<<grid, 256, 0, st>>>(sd, n, xyz); break;
+#define G4D_SCATTER_CASE(K)                                                     \
+        case K:                                                                 \
+            if (sd.d.times) bwd_scatter_kernel<K, true><<<grid, 256, 0, st>>>(sd, n, xyz); \
+            else bwd_scatter_kernel<K, false><<<grid, 256, 0, st>>>(sd, n, xyz);          \
+            break;
         G4D_SCATTER_CASE(1) G4D_SCATTER_CASE(2) G4D_SCATTER_CASE(3) G4D_SCATTER_CASE(4)
         G4D_SCATTER_CASE(5) G4D_SCATTER_CASE(6) G4D_SCATTER_CASE(7) G4D_SCATTER_CASE(8)
 #undef G4D_SCATTER_CASE
@@ -803,6 +814,7 @@ static DeformBwdBuffers carve_backward_scratch(Carve& m, const DeformDesc& d, in
     const size_t rows128 = (N + 127) / 128 * 128;   // whole tiles of the tensor-core kernels
     b.feat = *gathered = m.take<float>(rows128 * d.F);
     b.dfeat = m.take<float>(rows128 * d.F);
+    if (d.times) return b;   // per-row: the time planes' gradients go straight to the planes
     float* rows = m.take<float>(tr.total());
     if (rows) tr.place(rows, b.trow_grad);
     return b;
@@ -878,8 +890,8 @@ static cudaError_t launch_ffma_engine(const DeformBwdDesc& bd, int64_t n, const 
 
 cudaError_t launch_deform_backward(const DeformDesc& d, const G4DDeformParams& prm, const G4DDeformGrads& grads, const TcBwdWeights* tc,
                                    TimeArg time, int64_t n, const float* xyz, const float* const go[G4D_NUM_HEADS],
-                                   float* const gi[G4D_NUM_HEADS], const uint32_t* relu_bits, const float* saved_feat,
-                                   const uint32_t* order, void* scratch, int sm_count, cudaStream_t st) {
+                                   float* const gi[G4D_NUM_HEADS], float* g_times, const uint32_t* relu_bits,
+                                   const float* saved_feat, const uint32_t* order, void* scratch, int sm_count, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
     const TimeRows tr(d.levels, d.res, d.C);
     Carve m(scratch);
@@ -901,7 +913,8 @@ cudaError_t launch_deform_backward(const DeformDesc& d, const G4DDeformParams& p
         for (int a = 0; a < 3; ++a) sc.trow_grad[l][a] = buf.trow_grad[l][a];
     }
     for (int h = 0; h < G4D_NUM_HEADS; ++h) { sc.go[h] = go[h]; sc.gi[h] = gi[h]; }
-    cudaError_t e = cudaMemsetAsync(buf.trow_grad[0][0], 0, tr.total() * 4, st);
+    sc.g_times = g_times;
+    cudaError_t e = d.times ? cudaSuccess : cudaMemsetAsync(buf.trow_grad[0][0], 0, tr.total() * 4, st);
     if (e != cudaSuccess) return e;
     if (!saved_feat && (e = launch_deform_features(d, n, xyz, order, gathered, false, st)) != cudaSuccess) return e;
     // the engine: d(feat) -> DFEAT and the weight gradients (the tensor-core wgrad kernel after the scatter)
@@ -912,7 +925,7 @@ cudaError_t launch_deform_backward(const DeformDesc& d, const G4DDeformParams& p
     if (e != cudaSuccess) return e;
     if ((e = launch_bwd_scatter(sc, n, xyz, st)) != cudaSuccess) return e;
     if (tc && (e = launch_tc_bwd_wgrad(d, grads, n, buf.images, sm_count, st)) != cudaSuccess) return e;
-    return launch_distribute_time_grad(d, buf.trow_grad, bd.g_planes, time, st);
+    return d.times ? cudaSuccess : launch_distribute_time_grad(d, buf.trow_grad, bd.g_planes, time, st);
 }
 
 // ------------------------------------------------------------------------------------------------------

@@ -533,11 +533,12 @@ cudaError_t launch_gather_order(const float* aabb, int64_t n, const float* xyz, 
 
 // ---- HexPlane gather at full occupancy: C/4 threads per Gaussian, one channel vector each -> feat [N][F] fp32 -----------
 // The gather of every path (FFMA and tensor-core network, forward and backward): the forward launches it dependent on
-// collapse_time_rows, the backward as an ordinary launch.  Thread
+// collapse_time_rows, the backward as an ordinary launch.  PER_ROW: Gaussian g is sampled at its own time d.times[g] (no
+// collapsed rows).  Thread
 // group j gathers Gaussian order[j] (j itself when order is NULL): in spatial order the 8 Gaussians of a warp, and the warps
-// of an SM, tap neighbouring plane texels and share them in L1.  feat[g] depends on xyz[g] alone, so any order gives the
-// same bits.
-template <int C4>
+// of an SM, tap neighbouring plane texels and share them in L1.  feat[g] depends on xyz[g] (and times[g]) alone, so any order
+// gives the same bits.
+template <int C4, bool PER_ROW>
 __global__ void __launch_bounds__(256) deform_features_kernel(DeformDesc d, int64_t n, const float* __restrict__ xyz,
                                                               const uint32_t* __restrict__ order, float* __restrict__ feat) {
     pdl_wait();         // the collapsed time rows come from the previous kernel of the stream
@@ -551,11 +552,13 @@ __global__ void __launch_bounds__(256) deform_features_kernel(DeformDesc d, int6
     float pcs[3];
 #pragma unroll
     for (int a = 0; a < 3; ++a) pcs[a] = nrm(a, xyz[3 * g + a]);
+    const float tg = PER_ROW ? __ldg(d.times + g) : 0.f;
     for (int l = 0; l < d.levels; ++l) {
-        Tap1D tx[3];
+        Tap1D tx[PER_ROW ? 4 : 3];
 #pragma unroll
         for (int a = 0; a < 3; ++a) tx[a] = make_tap(pcs[a], d.res[l][a]);
-        *reinterpret_cast<float4*>(feat + g * d.F + l * d.C + 4 * v) = sample_vector(d.planes[l], d.trow[l], d.res[l], tx, v, C4);
+        if (PER_ROW) tx[PER_ROW ? 3 : 0] = make_tap(tg, d.res[l][3]);
+        *reinterpret_cast<float4*>(feat + g * d.F + l * d.C + 4 * v) = sample_vector<PER_ROW>(d.planes[l], d.trow[l], d.res[l], tx, v, C4);
     }
 }
 
@@ -565,8 +568,9 @@ cudaError_t launch_deform_features(const DeformDesc& d, int64_t n, const float* 
     const int C4 = d.C / 4;
     const unsigned grid = (unsigned)((n * C4 + 255) / 256);
     switch (C4) {   // every channel width the C-ABI takes: C = 4 .. 32
-#define G4D_GATHER_CASE(K) \
-        case K: return launch_k(deform_features_kernel<K>, dim3(grid), dim3(256), 0, st, pdl, d, n, xyz, order, feat);
+#define G4D_GATHER_CASE(K)                                                                                                  \
+        case K: return d.times ? launch_k(deform_features_kernel<K, true>, dim3(grid), dim3(256), 0, st, pdl, d, n, xyz, order, feat) \
+                               : launch_k(deform_features_kernel<K, false>, dim3(grid), dim3(256), 0, st, pdl, d, n, xyz, order, feat);
         G4D_GATHER_CASE(1) G4D_GATHER_CASE(2) G4D_GATHER_CASE(3) G4D_GATHER_CASE(4)
         G4D_GATHER_CASE(5) G4D_GATHER_CASE(6) G4D_GATHER_CASE(7) G4D_GATHER_CASE(8)
 #undef G4D_GATHER_CASE

@@ -302,11 +302,12 @@ cudaError_t launch_preprocess_backward(const CameraDev* cam, int64_t n, const Ra
 // the forward gathered; order: its walk order), an engine -- the tensor-core kernels with the images tc, or the FFMA kernels
 // (tc NULL) -- the scatter and the time-row gradients.  go[h] / gi[h]: gradient w.r.t. the outputs / inputs of head h's
 // residual tensor (xyz, scaling, rotation, opacity, shs).  relu_bits: the signs a tensor-core forward saved, or NULL.
+// d.times set (per-row times; `time` unused): no time rows, and dL/d(times) into g_times [N] when it is not NULL.
 size_t deform_backward_scratch_bytes(const DeformDesc& d, int64_t n, bool tc);   // size of launch_deform_backward's scratch
 cudaError_t launch_deform_backward(const DeformDesc& d, const G4DDeformParams& prm, const G4DDeformGrads& grads, const TcBwdWeights* tc,
                                    TimeArg time, int64_t n, const float* xyz, const float* const go[G4D_NUM_HEADS],
-                                   float* const gi[G4D_NUM_HEADS], const uint32_t* relu_bits, const float* saved_feat,
-                                   const uint32_t* order, void* scratch, int sm_count, cudaStream_t st);
+                                   float* const gi[G4D_NUM_HEADS], float* g_times, const uint32_t* relu_bits,
+                                   const float* saved_feat, const uint32_t* order, void* scratch, int sm_count, cudaStream_t st);
 // ---- several cameras at one timestamp (g4d_render_forward_cameras / _backward_cameras) -----------------------------
 constexpr int kMaxExtraCameras = G4D_MAX_CAMERAS - 1;
 // cameras 1..k-1 of a multi-camera forward: camera c reads cam[c] and writes its own context's records g[c] and out_radii[c]

@@ -1,9 +1,11 @@
 // hexplane.cuh -- the HexPlane field (scene/hexplane.py:19-20,73-106,160-183) for every deformation kernel, forward and backward,
 // FFMA and tensor-core: coordinate normalisation, border-clamped taps, the forward sample of one channel vector and its backward.
 //
-// Planes are channel-last [H][W][C], so one bilinear tap of a channel vector (4 channels) is one float4; the three time planes
-// are collapsed once per view into 1-D rows (every Gaussian of a view shares t).  The functions take one level's entries of
-// DeformDesc (planes[l], trow[l], res[l]) and the taps of the normalised (x, y, z) at that level.  The normalisation and the
+// Planes are channel-last [H][W][C], so one bilinear tap of a channel vector (4 channels) is one float4.  When every Gaussian
+// shares t, the three time planes are collapsed once per call into 1-D rows; in the per-row mode (PER_ROW, one time per
+// Gaussian) each Gaussian forms the two texels of those rows it needs on the fly, with the same arithmetic, so both modes give
+// the same bits at equal times.  The functions take one level's entries of DeformDesc (planes[l], trow[l], res[l]) and the
+// taps of the normalised (x, y, z) at that level, and in the per-row mode the tap of the row's t as tx[3].  The normalisation and the
 // forward sample are explicit roundings (__fmul_rn / __fadd_rn, fmaf()) and single multiplies only: they round the same in the
 // -fmad=false translation units as in the others, so a backward taps the very cells its forward sampled.
 #pragma once
@@ -40,17 +42,41 @@ G4D_D Tap1D make_tap(float u, int size) {
     return t;
 }
 
+// The collapsed time row's texel from the plane's two time rows a (at ty.i0) and b (at ty.i1): the arithmetic of
+// collapse_time_rows_kernel
+G4D_D float4 time_lerp(float4 a, float4 b, const Tap1D& ty) {
+    return make_float4(fmaf(b.x, ty.w1, a.x * ty.w0), fmaf(b.y, ty.w1, a.y * ty.w0), fmaf(b.z, ty.w1, a.z * ty.w0),
+                       fmaf(b.w, ty.w1, a.w * ty.w0));
+}
+
+// The two texels r0 / r1 of the collapsed time row of plane k at the c0 taps X; PER_ROW: formed from the plane at the time
+// tap ty, also handing back the four plane texels (nw, ne at ty.i0; sw, se at ty.i1) for the backward
+template <bool PER_ROW>
+G4D_D void time_row_texels(const float* plane, const float* trow, int W, const Tap1D& X, const Tap1D& ty, int v, int C4,
+                           float4& r0, float4& r1, float4 (&q)[4]) {
+    if (PER_ROW) {
+        const float4* pl = reinterpret_cast<const float4*>(plane);
+        q[0] = __ldg(pl + (ty.i0 * W + X.i0) * C4 + v); q[1] = __ldg(pl + (ty.i0 * W + X.i1) * C4 + v);
+        q[2] = __ldg(pl + (ty.i1 * W + X.i0) * C4 + v); q[3] = __ldg(pl + (ty.i1 * W + X.i1) * C4 + v);
+        r0 = time_lerp(q[0], q[2], ty); r1 = time_lerp(q[1], q[3], ty);
+    } else {
+        const float4* row = reinterpret_cast<const float4*>(trow);
+        r0 = __ldg(row + X.i0 * C4 + v); r1 = __ldg(row + X.i1 * C4 + v);
+    }
+}
+
 // One channel vector v (channels 4v .. 4v+3) of one level: the product over the 6 planes of the bilinear samples.
-G4D_D float4 sample_vector(const float* const planes[6], const float* const trow[3], const int res[4], const Tap1D (&tx)[3], int v,
-                           int C4) {
+template <bool PER_ROW>
+G4D_D float4 sample_vector(const float* const planes[6], const float* const trow[3], const int res[4],
+                           const Tap1D (&tx)[PER_ROW ? 4 : 3], int v, int C4) {
     float4 prod = make_float4(1.f, 1.f, 1.f, 1.f);
 #pragma unroll
     for (int k = 0; k < 6; ++k) {
         const int c0 = plane_axis0(k), c1 = plane_axis1(k);
         float4 s;
-        if (c1 == 3) {   // collapsed time row: 1-D lerp along c0
-            const float4* row = reinterpret_cast<const float4*>(trow[c0]);
-            const float4 r0 = __ldg(row + tx[c0].i0 * C4 + v), r1 = __ldg(row + tx[c0].i1 * C4 + v);
+        if (c1 == 3) {   // time plane: 1-D lerp along c0 of the collapsed row
+            float4 r0, r1, q[4];
+            time_row_texels<PER_ROW>(planes[k], trow[c0], res[c0], tx[c0], tx[PER_ROW ? 3 : 0], v, C4, r0, r1, q);
             const float w0 = tx[c0].w0, w1 = tx[c0].w1;
             s.x = fmaf(r1.x, w1, r0.x * w0); s.y = fmaf(r1.y, w1, r0.y * w0);
             s.z = fmaf(r1.z, w1, r0.z * w0); s.w = fmaf(r1.w, w1, r0.w * w0);
@@ -76,21 +102,29 @@ G4D_D void red_add_v4(float* addr, float4 v) {
 }
 
 // Backward of sample_vector (autograd of F.grid_sample and the plane product): scatter df = dL/d(feat[l*C + 4v .. +3]) into
-// the 4 / 2 taps of every plane (vector RED; the time planes through the collapsed rows' gradient trow_grad) and accumulate
-// dL/d(normalised coordinate) into gpix.
+// the taps of every plane (vector RED) and accumulate dL/d(normalised coordinate) into gpix.  A time plane's gradient goes to
+// the collapsed rows' gradient trow_grad (2 taps), or PER_ROW straight to the plane's 2 x 2 texels of (c0 tap, time tap), and
+// then dL/d(t) is accumulated into gt.
+template <bool PER_ROW>
 G4D_D void scatter_vector(const float* const planes[6], const float* const trow[3], const int res[4], float* const g_planes[6],
-                          float* const trow_grad[3], const Tap1D (&tx)[3], int v, int C4, float4 df, float gpix[3]) {
-    float4 s[6], dsx[6], dsy[6];   // sample, d(sample)/d(x_pix of c0), d/d(y_pix of c1)
+                          float* const trow_grad[3], const Tap1D (&tx)[PER_ROW ? 4 : 3], int v, int C4, float4 df, float gpix[3],
+                          float& gt) {
+    float4 s[6], dsx[6], dsy[6];   // sample, d(sample)/d(x_pix of c0), d/d(y_pix of c1) (PER_ROW time planes: of t_pix)
 #pragma unroll
     for (int k = 0; k < 6; ++k) {
         const int c0 = plane_axis0(k), c1 = plane_axis1(k);
         if (c1 == 3) {
-            const float4* row = reinterpret_cast<const float4*>(trow[c0]);
-            const float4 r0 = __ldg(row + tx[c0].i0 * C4 + v), r1 = __ldg(row + tx[c0].i1 * C4 + v);
+            float4 r0, r1, q[4];
+            time_row_texels<PER_ROW>(planes[k], trow[c0], res[c0], tx[c0], tx[PER_ROW ? 3 : 0], v, C4, r0, r1, q);
             const float w0 = tx[c0].w0, w1 = tx[c0].w1;
             s[k] = make_float4(fmaf(r1.x, w1, r0.x * w0), fmaf(r1.y, w1, r0.y * w0), fmaf(r1.z, w1, r0.z * w0), fmaf(r1.w, w1, r0.w * w0));
             dsx[k] = make_float4(r1.x - r0.x, r1.y - r0.y, r1.z - r0.z, r1.w - r0.w);
-            dsy[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (PER_ROW) {   // q = nw, ne, sw, se of the (c0, t) plane
+                dsy[k] = make_float4((q[2].x - q[0].x) * w0 + (q[3].x - q[1].x) * w1, (q[2].y - q[0].y) * w0 + (q[3].y - q[1].y) * w1,
+                                     (q[2].z - q[0].z) * w0 + (q[3].z - q[1].z) * w1, (q[2].w - q[0].w) * w0 + (q[3].w - q[1].w) * w1);
+            } else {
+                dsy[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+            }
         } else {
             const int W = res[c0];
             const float4* pl = reinterpret_cast<const float4*>(planes[k]);
@@ -120,13 +154,15 @@ G4D_D void scatter_vector(const float* const planes[6], const float* const trow[
         const int c0 = plane_axis0(k), c1 = plane_axis1(k);
         const float4 gs = make_float4(df.x * pre[k].x * suf[k].x, df.y * pre[k].y * suf[k].y, df.z * pre[k].z * suf[k].z, df.w * pre[k].w * suf[k].w);
         gpix[c0] += (gs.x * dsx[k].x + gs.y * dsx[k].y + gs.z * dsx[k].z + gs.w * dsx[k].w) * tx[c0].gmul;
-        if (c1 == 3) {
+        if (c1 == 3 && !PER_ROW) {
             float* row = trow_grad[c0];
             const float w0 = tx[c0].w0, w1 = tx[c0].w1;
             red_add_v4(row + (tx[c0].i0 * C4 + v) * 4, make_float4(gs.x * w0, gs.y * w0, gs.z * w0, gs.w * w0));
             red_add_v4(row + (tx[c0].i1 * C4 + v) * 4, make_float4(gs.x * w1, gs.y * w1, gs.z * w1, gs.w * w1));
         } else {
-            gpix[c1] += (gs.x * dsy[k].x + gs.y * dsy[k].y + gs.z * dsy[k].z + gs.w * dsy[k].w) * tx[c1].gmul;
+            const float gy = (gs.x * dsy[k].x + gs.y * dsy[k].y + gs.z * dsy[k].z + gs.w * dsy[k].w) * tx[c1].gmul;
+            if (c1 == 3) gt += gy;
+            else gpix[c1] += gy;
             const int W = res[c0];
             float* pl = g_planes[k];
             const Tap1D &X = tx[c0], &Y = tx[c1];

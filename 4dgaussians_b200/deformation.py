@@ -156,9 +156,9 @@ class deform_network(nn.Module):
         return self.forward_dynamic(point, scales, rotations, opacity, shs, times_sel)
 
     def forward_dynamic(self, point, scales=None, rotations=None, opacity=None, shs=None, times_sel=None):
-        t = scalar_time(times_sel)
+        t, times = classify_times(times_sel, point.shape[0])
         flat = self.flat_parameters()
-        outs = _DeformFunction.apply(self, t, torch.is_grad_enabled(), point, scales, rotations, opacity, shs, *flat)
+        outs = _DeformFunction.apply(self, t, times, torch.is_grad_enabled(), point, scales, rotations, opacity, shs, *flat)
         pts, sc, rot, op, sh = outs
         a = self.args
         # inactive heads hand the input tensor back, exactly like the reference (deformation.py:106-145)
@@ -376,8 +376,9 @@ class deform_network(nn.Module):
 
 
 def scalar_time(times_sel) -> float:
-    """The reference builds an [N,1] tensor whose rows are identical (gaussian_renderer/__init__.py:52);
-    python floats, 0-d tensors and the int 0 all occur (SURVEY.md §8b 'Input quirks')."""
+    """The time of row 0 of ``times_sel``: the one timestamp of a camera.  The renderer builds an [N,1] tensor whose rows are
+    identical (gaussian_renderer/__init__.py:52); python floats, 0-d tensors and the int 0 all occur (SURVEY.md §8b 'Input
+    quirks').  ``deform_network.forward`` takes rows that differ too (``classify_times``)."""
     if times_sel is None:
         raise RuntimeError("times_sel is required (forward_static is a dead path in the reference)")
     if torch.is_tensor(times_sel):
@@ -387,9 +388,33 @@ def scalar_time(times_sel) -> float:
     return float(times_sel)
 
 
+def classify_times(times_sel, n: int):
+    """(t, None): every one of the n rows at the time t -- a Python number, a one-element tensor, or a tensor whose elements
+    are all equal and that does not require grad (one host sync, as ``scalar_time``'s).  Such a tensor takes this path
+    whatever its element count, an empty one included (t = 0), exactly as before per-row times existed, so no caller of the
+    one-time path sees a new error.  (None, times_sel): one time per row -- any other tensor with n elements ([n] or [n, 1],
+    any real dtype and device), which receives dL/dt when it requires grad.  Any other tensor -- elements that differ, or
+    that require grad, in a count that is neither 1 nor n -- raises ValueError."""
+    if not torch.is_tensor(times_sel) or times_sel.numel() == 1:
+        return scalar_time(times_sel), None
+    if not times_sel.requires_grad:
+        if times_sel.numel() == 0:
+            return scalar_time(times_sel), None
+        lo, hi = torch.aminmax(times_sel.detach().reshape(-1))
+        lo, hi = torch.stack([lo, hi]).tolist()
+        if lo == hi:
+            return float(lo), None
+    if times_sel.numel() != n:
+        raise ValueError("times_sel must hold one time or one per row: %d elements for %d rows" % (times_sel.numel(), n))
+    return None, times_sel
+
+
 class _DeformFunction(torch.autograd.Function):
+    """t: the time of every row, or times (a tensor of N elements, t None): one time per row"""
+
     @staticmethod
-    def forward(ctx, module: deform_network, t: float, grad_mode: bool, xyz, scales, rotations, opacity, shs, *params):
+    def forward(ctx, module: deform_network, t: Optional[float], times, grad_mode: bool, xyz, scales, rotations, opacity, shs,
+                *params):
         lib = _lib.load()
         dev = xyz.device
         n = xyz.shape[0]
@@ -409,14 +434,25 @@ class _DeformFunction(torch.autograd.Function):
         ptr = lambda v: v.data_ptr() if v is not None else None
         # what autograd would save for the ReLU backward: one sign bit per hidden unit (only when a backward can follow)
         relu_bits = torch.empty(_lib.relu_bits_words(n), device=dev, dtype=torch.int32) if needs_bwd else None
+        # per-row times as a contiguous fp32 device copy (N = 0: nothing to sample, the one-time call does it)
+        tt = times.detach().reshape(-1).to(device=dev, dtype=torch.float32).contiguous() if times is not None and n else None
         with torch.cuda.device(dev):
             ws = _lib.workspace_of(dev)
-            _lib.check(lib.g4d_deform_forward(ws.handle, C.byref(prm), n, ptr(x), ptr(s), ptr(r), ptr(o), ptr(sh), float(t),
-                                              ptr(ox), ptr(os_), ptr(orr), ptr(oo), ptr(osh), ptr(relu_bits),
-                                              _lib.stream_of(dev)), "g4d_deform_forward")
-        ctx.module, ctx.t, ctx.n = module, float(t), n
+            if tt is None:
+                _lib.check(lib.g4d_deform_forward(ws.handle, C.byref(prm), n, ptr(x), ptr(s), ptr(r), ptr(o), ptr(sh),
+                                                  float(t or 0.0), ptr(ox), ptr(os_), ptr(orr), ptr(oo), ptr(osh), ptr(relu_bits),
+                                                  _lib.stream_of(dev)), "g4d_deform_forward")
+            else:
+                _lib.check(lib.g4d_deform_forward_times(ws.handle, C.byref(prm), n, ptr(x), ptr(s), ptr(r), ptr(o), ptr(sh),
+                                                        ptr(tt), ptr(ox), ptr(os_), ptr(orr), ptr(oo), ptr(osh), ptr(relu_bits),
+                                                        _lib.stream_of(dev)), "g4d_deform_forward_times")
+        ctx.module, ctx.t, ctx.n = module, float(t or 0.0), n
+        ctx.per_row = times is not None
+        ctx.times_meta = (times.shape, times.dtype, times.device) if times is not None else None
         ctx.relu_bits = relu_bits
-        ctx.save_for_backward(x)
+        # the times are saved like xyz: every backward of the graph reads them, and autograd's version check refuses a
+        # backward after either was changed in place
+        ctx.save_for_backward(x, tt)
         ctx.has = (s is not None, r is not None, o is not None, sh is not None)
         outs = (ox, os_ if os_ is not None else x.new_zeros(0), orr if orr is not None else x.new_zeros(0),
                 oo if oo is not None else x.new_zeros(0), osh if osh is not None else x.new_zeros(0))
@@ -426,7 +462,7 @@ class _DeformFunction(torch.autograd.Function):
     def backward(ctx, g_xyz, g_sc, g_rot, g_op, g_sh):
         lib = _lib.load()
         module, t, n = ctx.module, ctx.t, ctx.n
-        (x,) = ctx.saved_tensors
+        x, tt = ctx.saved_tensors
         dev = x.device
         keep = []
         prm = module.c_params(keep, fresh=True)      # (keeps the "an optimizer step may follow" mark, see param_version)
@@ -447,10 +483,22 @@ class _DeformFunction(torch.autograd.Function):
         gi_o = torch.empty(n, 1, device=dev) if has_o else None
         gi_sh = torch.empty(n, 16, 3, device=dev) if (has_sh and (hm & _lib.HEAD_SHS)) else None
         ptr = lambda v: v.data_ptr() if v is not None else None
+        per_row = ctx.per_row and n > 0      # (N = 0: the forward made the one-time call, which launches nothing per row)
+        g_t = torch.empty(n, device=dev) if ctx.needs_input_grad[2] else None
         with torch.cuda.device(dev):
             ws = _lib.workspace_of(dev)
-            _lib.check(lib.g4d_deform_backward(ws.handle, C.byref(prm), C.byref(cg), n, ptr(x), float(t), ptr(go_x), ptr(go_s),
-                                               ptr(go_r), ptr(go_o), ptr(go_sh), ptr(gi_x), ptr(gi_s), ptr(gi_r), ptr(gi_o),
-                                               ptr(gi_sh), ptr(ctx.relu_bits), _lib.stream_of(dev)), "g4d_deform_backward")
-        ctx.relu_bits = None
-        return (None, None, None, gi_x, gi_s, gi_r, gi_o, gi_sh) + tuple(pgrads)
+            if not per_row:
+                _lib.check(lib.g4d_deform_backward(ws.handle, C.byref(prm), C.byref(cg), n, ptr(x), float(t), ptr(go_x),
+                                                   ptr(go_s), ptr(go_r), ptr(go_o), ptr(go_sh), ptr(gi_x), ptr(gi_s), ptr(gi_r),
+                                                   ptr(gi_o), ptr(gi_sh), ptr(ctx.relu_bits), _lib.stream_of(dev)),
+                           "g4d_deform_backward")
+            else:
+                _lib.check(lib.g4d_deform_backward_times(ws.handle, C.byref(prm), C.byref(cg), n, ptr(x), ptr(tt), ptr(go_x),
+                                                         ptr(go_s), ptr(go_r), ptr(go_o), ptr(go_sh), ptr(gi_x), ptr(gi_s),
+                                                         ptr(gi_r), ptr(gi_o), ptr(gi_sh), ptr(g_t), ptr(ctx.relu_bits),
+                                                         _lib.stream_of(dev)), "g4d_deform_backward_times")
+        ctx.relu_bits = None      # a second backward through the graph derives the ReLU signs itself, as the C-ABI allows
+        if g_t is not None:   # dL/dt in the shape, dtype and device of times_sel
+            times = ctx.times_meta
+            g_t = g_t.reshape(times[0]).to(device=times[2], dtype=times[1])
+        return (None, None, g_t, None, gi_x, gi_s, gi_r, gi_o, gi_sh) + tuple(pgrads)

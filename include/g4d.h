@@ -12,7 +12,7 @@
  *       <- diff_gaussian_rasterization.GaussianRasterizer.forward / autograd backward, called at
  *          gaussian_renderer/__init__.py:120-128 with the settings built at :38-51
  *          (upstream: _C.rasterize_gaussians / _C.rasterize_gaussians_backward, SURVEY.md App. A.5)
- *   g4d_deform_forward / _backward
+ *   g4d_deform_forward / _backward (and _times: one time per row)
  *       <- scene/deformation.py:185-212 deform_network.forward (HexPlane scene/hexplane.py:73-106 +
  *          MLP scene/deformation.py:67-148) and its autograd backward
  *   g4d_render_forward / _backward
@@ -170,6 +170,21 @@ int g4d_deform_backward(G4DWorkspace *ws, const G4DDeformParams *prm, G4DDeformG
                         float *g_in_xyz, float *g_in_scaling, float *g_in_rotation, float *g_in_opacity,
                         float *g_in_shs, const uint32_t *relu_bits, void *stream);
 #define G4D_RELU_BITS_WORDS(n) ((size_t)24 * (size_t)(n) + 4) /* [6 layers][n][4 words] + validity tag */
+/* The same network with one time per Gaussian (the reference's times_sel [N,1] with rows that differ): d_times is device [n]
+ * fp32, row g deformed at d_times[g] -- the trajectory of every Gaussian over several frames in one call, per-Gaussian time
+ * offsets.  Otherwise as g4d_deform_forward / _backward: the same checks, engine and relu_bits.  At equal times the results
+ * are those of the entry points above, bit for bit (the weight and plane gradients up to the order of their atomic sums).
+ * d_times NULL: G4D_ERR_ARG before any launch.  g_times (optional, device [n], OVERWRITTEN): dL/d(times), 0 on a row whose
+ * time lies outside [-1, 1] (grid_sample's border clamp). */
+int g4d_deform_forward_times(G4DWorkspace *ws, const G4DDeformParams *prm, int64_t n, const float *xyz,
+                             const float *scaling, const float *rotation, const float *opacity, const float *shs,
+                             const float *d_times, float *out_xyz, float *out_scaling, float *out_rotation,
+                             float *out_opacity, float *out_shs, uint32_t *relu_bits, void *stream);
+int g4d_deform_backward_times(G4DWorkspace *ws, const G4DDeformParams *prm, G4DDeformGrads *grads, int64_t n,
+                              const float *xyz, const float *d_times, const float *g_out_xyz, const float *g_out_scaling,
+                              const float *g_out_rotation, const float *g_out_opacity, const float *g_out_shs,
+                              float *g_in_xyz, float *g_in_scaling, float *g_in_rotation, float *g_in_opacity,
+                              float *g_in_shs, float *g_times, const uint32_t *relu_bits, void *stream);
 
 /* ---- rasterizer (drop-in for GaussianRasterizer) ------------------------------------------------
  * Inputs are POST-activation (scales = exp, rotations normalised, opacities = sigmoid), shs [N,M,3] (M: cam->sh_coeffs).
