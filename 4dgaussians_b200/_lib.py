@@ -6,10 +6,11 @@ workspaces need a CUDA device.
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import os
 import threading
-from typing import Dict, Optional
+from typing import Dict, Optional, Sequence
 
 import torch
 
@@ -238,9 +239,31 @@ def check_sh_degree(m: int, active: int, head_mask: int = 0):
                          "max_sh_degree 3, the model has %d" % SH_COEFFS.index(m))
 
 
+_routed: Dict[int, "Workspace"] = {}
+
+
 def workspace_of(device: torch.device) -> "Workspace":
-    """The shared workspace of a CUDA device (no index: the current device)."""
-    return Workspace.get(device.index if device.index is not None else torch.cuda.current_device())
+    """The shared workspace of a CUDA device (no index: the current device), or the one ``routed`` names for it."""
+    index = device.index if device.index is not None else torch.cuda.current_device()
+    ws = _routed.get(index)
+    return ws if ws is not None else Workspace.get(index)
+
+
+@contextlib.contextmanager
+def routed(ws: "Workspace", contexts: Sequence["Context"]):
+    """Inside the block every library call on ws's device (``workspace_of``) runs on ws, and its context leases are
+    ``contexts``, handed out in order and never returned to a pool: a CUDA graph captured inside sees the buffers of a
+    workspace it owns and the same context per view at every replay.  The routing is process-wide (an autograd backward
+    runs on another thread), so it is meant for blocks that issue all of the device's library work."""
+    if ws.device in _routed:
+        raise G4DError("a routed workspace is already active on device %d" % ws.device)
+    ws._fixed, ws._next = list(contexts), 0
+    _routed[ws.device] = ws
+    try:
+        yield ws
+    finally:
+        del _routed[ws.device]
+        ws._fixed = None
 
 
 def stream_of(device: torch.device) -> int:
@@ -261,6 +284,8 @@ class Workspace:
         if not self.handle:
             raise G4DError("g4d_workspace_create(%d): %s" % (device, lib.g4d_last_error().decode()))
         self._free_contexts = []
+        self._fixed = None           # the contexts ``routed`` hands out, in order
+        self._live = set()           # handles of this workspace's contexts not destroyed yet
 
     @classmethod
     def get(cls, device: int) -> "Workspace":
@@ -283,8 +308,11 @@ class Workspace:
     def __del__(self):
         try:
             if self.handle and _lib is not None and self._by_device.get(self.device) is not self:
-                for ctx in self._free_contexts:     # (a cycle: the pool's contexts may be collected after their workspace)
-                    ctx.__del__()
+                # (a garbage cycle may finalise the workspace before its contexts: a context is destroyed while its
+                #  workspace exists)
+                for h in self._live:
+                    _lib.g4d_context_destroy(h)
+                self._live.clear()
                 self._free_contexts = []
                 _lib.g4d_workspace_destroy(self.handle)
                 self.handle = None
@@ -295,6 +323,11 @@ class Workspace:
         check(load().g4d_workspace_set_option(self.handle, option, int(value)), "g4d_workspace_set_option")
 
     def acquire_context(self) -> "Context":
+        if self._fixed is not None:
+            if self._next >= len(self._fixed):
+                raise G4DError("more forwards inside the routed block than its %d contexts" % len(self._fixed))
+            self._next += 1
+            return self._fixed[self._next - 1]
         while self._free_contexts:
             ctx = self._free_contexts.pop()
             if ctx.handle:
@@ -302,6 +335,8 @@ class Workspace:
         return Context(self)
 
     def release_context(self, ctx: "Context"):
+        if self._fixed is not None and ctx in self._fixed:
+            return
         if ctx.handle:      # (a context finalised in the same GC pass as its lease must not be resurrected into the pool)
             self._free_contexts.append(ctx)
 
@@ -314,6 +349,7 @@ class Context:
         self.handle = load().g4d_context_create(ws.handle)
         if not self.handle:
             raise G4DError("g4d_context_create: %s" % load().g4d_last_error().decode())
+        ws._live.add(self.handle)
 
     def set_time_source(self, d_time: Optional[int]):
         """Read the timestamp of every forward / backward on this context from the device float at d_time (None: the camera's)."""
@@ -355,8 +391,9 @@ class Context:
 
     def __del__(self):
         try:
-            if self.handle and _lib is not None:
+            if self.handle and _lib is not None and self.handle in self.ws._live:
+                self.ws._live.discard(self.handle)
                 _lib.g4d_context_destroy(self.handle)
-                self.handle = None
+            self.handle = None
         except Exception:
             pass

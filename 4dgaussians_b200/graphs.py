@@ -25,8 +25,111 @@ from .deformation import deform_network, scalar_time
 from .rasterizer import camera_from_settings
 from .renderer import _stage_module, _time_bits, _zero_points, settings_from_camera
 
-_VIEW_FLOATS = 36        # per view in the staging block: view matrix [16], projection matrix [16], camera centre [3], pad
+_VIEW_FLOATS = 36        # per view in the staging block: view matrix [16], projection matrix [16], camera centre [3], time
 ERR_OVERFLOW = -5        # G4D_ERR_OVERFLOW
+
+
+class ViewBlock:
+    """The device block captured kernels read a call's views from -- per view its view matrix [16], projection matrix [16],
+    camera centre [3] and time [1], then ``extra`` floats -- and its pinned host twin: ``stage`` writes host values into the
+    twin, copies it over in one host-to-device copy, and copies device tensors device to device behind it."""
+
+    def __init__(self, dev: torch.device, k: int, extra: int = 0):
+        self.k, self.extra_at = k, k * _VIEW_FLOATS
+        self.block = torch.zeros(k * _VIEW_FLOATS + extra, device=dev, dtype=torch.float32)
+        self._staging = torch.zeros(k * _VIEW_FLOATS + extra, dtype=torch.float32, pin_memory=True)
+        self._staging_np = self._staging.numpy()
+        self._staged = torch.cuda.Event()
+
+    def view(self, i: int):
+        """view i's (view matrix [4,4], projection matrix [4,4], camera centre [3]): views of the block"""
+        o = i * _VIEW_FLOATS
+        b = self.block
+        return b[o:o + 16].view(4, 4), b[o + 16:o + 32].view(4, 4), b[o + 32:o + 35]
+
+    def time_ptr(self, i: int) -> int:
+        return self.block.data_ptr() + 4 * (i * _VIEW_FLOATS + 35)
+
+    def stage(self, views: Sequence, extra: Sequence = ()) -> List[float]:
+        """Views and ``extra`` ((offset past the views, tensor or numpy array), ...) into the block; returns the views' times."""
+        times = []
+        dev_copies = []
+        self._staged.synchronize()          # the previous call's copy has read the staging block
+        st = self._staging_np
+        for i, v in enumerate(views):
+            if isinstance(v, dict):
+                raise NotImplementedError("PanopticSports cameras are not supported by a CUDA graph")
+            times.append(scalar_time(v.time))
+            o = i * _VIEW_FLOATS
+            for j, (t, w) in enumerate(((v.world_view_transform, 16), (v.full_proj_transform, 16), (v.camera_center, 3))):
+                t = t if torch.is_tensor(t) else torch.as_tensor(t, dtype=torch.float32)
+                if t.numel() != w:
+                    raise RuntimeError("camera matrix has %d elements, expected %d" % (t.numel(), w))
+                if t.is_cuda:
+                    dev_copies.append((o + 16 * j, w, t))
+                else:
+                    st[o + 16 * j:o + 16 * j + w] = t.detach().reshape(-1).float().numpy()
+            st[o + 35] = times[-1]
+        for off, t in extra:
+            o = self.extra_at + off
+            if torch.is_tensor(t) and t.is_cuda:
+                dev_copies.append((o, t.numel(), t))
+            else:
+                t = t.detach().reshape(-1).float().numpy() if torch.is_tensor(t) else t.reshape(-1)
+                st[o:o + t.size] = t
+        stream = torch.cuda.current_stream(self.block.device)
+        self.block.copy_(self._staging, non_blocking=True)
+        self._staged.record(stream)
+        for o, w, t in dev_copies:
+            self.block[o:o + w].copy_(t.detach().reshape(-1))
+        return times
+
+
+def status_error(s: _lib.GraphStatus):
+    """The G4DError a graph status reports (None: nothing to report)."""
+    if s.overflows:
+        return _lib.G4DError("graphed render failed (code %d): %d replayed view(s) needed up to %d tile instances, more than "
+                             "the capacity learnt at capture; their images are incomplete (build the graph with a larger "
+                             "min_capacity)" % (ERR_OVERFLOW, s.overflows, s.max_instances))
+    if s.f16_range:
+        return _lib.G4DError("graphed render failed (code %d): an FP16x2 tensor-core launch met a value outside the f16 "
+                             "operand range; its results were saturated (G4D_OPT_TENSOR_CORES = 0, the FFMA kernels, has no range limit)"
+                             % ERR_OVERFLOW)
+    return None
+
+
+class GraphWorkspace:
+    """The private workspace of a CUDA graph and one context per view.  It runs in no-sync mode (G4D_OPT_SYNC_MODE = 0):
+    a context's first forward reads its instance count R back once and keeps R + 50 % (at least ``min_capacity``) as its
+    capacity, later forwards -- and every replay -- are bounded by it.  Context i reads its timestamp from the device float
+    at time_ptrs[i].  ``capture`` freezes the workspace, so that no call can move a buffer the graph points at."""
+
+    def __init__(self, dev: torch.device, time_ptrs: Sequence[int], min_capacity: int = 0):
+        self.ws = _lib.Workspace(dev.index)
+        self.ws.set_option(_lib.OPT_SYNC_MODE, 0)
+        if min_capacity:
+            self.ws.set_option(_lib.OPT_INSTANCE_CAPACITY, int(min_capacity))
+        self.ctxs = [_lib.Context(self.ws) for _ in time_ptrs]
+        for c, t in zip(self.ctxs, time_ptrs):
+            c.set_time_source(t)
+
+    def routed(self):
+        """``with gws.routed():`` -- the library calls of the block run on this workspace and its contexts (``_lib.routed``)."""
+        return _lib.routed(self.ws, self.ctxs)
+
+    def capture(self, launch) -> torch.cuda.CUDAGraph:
+        """Record launch() on a private memory pool, then freeze the workspace."""
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            launch()
+        self.ws.freeze(True)
+        self.ws.graph_status(sync=True)   # (clear: nothing has been replayed yet)
+        return graph
+
+    def check(self, sync: bool = True) -> None:
+        err = status_error(self.ws.graph_status(sync))
+        if err is not None:
+            raise err
 
 
 class GraphedRender:
@@ -67,27 +170,16 @@ class GraphedRender:
         _lib.check_sh_degree(m, self.sh_degree, module.head_mask() if module is not None else 0)
         self._bg = _lib.cuda_f32(bg_color, "bg", 3)
 
-        self.ws = _lib.Workspace(dev.index)
-        self.ws.set_option(_lib.OPT_SYNC_MODE, 0)
-        if min_capacity:
-            self.ws.set_option(_lib.OPT_INSTANCE_CAPACITY, int(min_capacity))
-        self.ctxs = [_lib.Context(self.ws) for _ in range(k)]
-        # device block the captured kernels read: k views, then the timestamp; its pinned staging copy
-        self._block = torch.zeros(k * _VIEW_FLOATS + 4, device=dev, dtype=torch.float32)
-        self._staging = torch.zeros(k * _VIEW_FLOATS + 4, dtype=torch.float32, pin_memory=True)
-        self._staging_np = self._staging.numpy()
-        self._staged = torch.cuda.Event()
-        base, fsz = self._block.data_ptr(), 4
-        d_time = base + k * _VIEW_FLOATS * fsz
-        for c in self.ctxs:
-            c.set_time_source(d_time)
-
+        # device block the captured kernels read: k views; every context takes view 0's timestamp
+        self._views = ViewBlock(dev, k)
+        self._gws = GraphWorkspace(dev, [self._views.time_ptr(0)] * k, min_capacity)
+        self.ws, self.ctxs = self._gws.ws, self._gws.ctxs
         self._cams = (_lib.Camera * k)(*[camera_from_settings(rs._replace(bg=self._bg), sh_coeffs=m)
                                           for rs, _ in settings])
         for i, cam in enumerate(self._cams):      # the view matrices and camera centre: read from the staging block's copy
             cam.debug = _lib.CAM_NO_GRAD
-            off = base + i * _VIEW_FLOATS * fsz
-            cam.d_viewmatrix, cam.d_projmatrix, cam.d_campos = off, off + 16 * fsz, off + 32 * fsz
+            view, proj, campos = self._views.view(i)
+            cam.d_viewmatrix, cam.d_projmatrix, cam.d_campos = view.data_ptr(), proj.data_ptr(), campos.data_ptr()
         self._keep: list = []
         # fresh: the capture records the weight repack, so every replay packs the parameters as they are then
         self._prm = module.c_params(self._keep, fresh=True) if module is not None else None
@@ -111,11 +203,7 @@ class GraphedRender:
             self._launch()
             for c in self.ctxs:
                 c.stats()
-            self.graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(self.graph):
-                self._launch()
-            self.ws.freeze(True)
-            self.ws.graph_status(sync=True)   # (clear: nothing has been replayed yet)
+            self.graph = self._gws.capture(self._launch)
 
     @staticmethod
     def _view_key(rs):
@@ -136,33 +224,9 @@ class GraphedRender:
             torch.gt(r, 0, out=v)
 
     def _stage(self, views: Sequence) -> None:
-        """Views and time into the device block: host values through the pinned staging block (one copy), device matrices
-        by device copies behind it."""
-        times = []
-        dev_copies = []
-        self._staged.synchronize()          # the previous call's copy has read the staging block
-        st = self._staging_np
-        for i, v in enumerate(views):
-            if isinstance(v, dict):
-                raise NotImplementedError("PanopticSports cameras are not supported by a graphed render")
-            times.append(scalar_time(v.time))
-            o = i * _VIEW_FLOATS
-            for j, (t, w) in enumerate(((v.world_view_transform, 16), (v.full_proj_transform, 16), (v.camera_center, 3))):
-                t = t if torch.is_tensor(t) else torch.as_tensor(t, dtype=torch.float32)
-                if t.numel() != w:
-                    raise RuntimeError("camera matrix has %d elements, expected %d" % (t.numel(), w))
-                if t.is_cuda:
-                    dev_copies.append((o + 16 * j, w, t))
-                else:
-                    st[o + 16 * j:o + 16 * j + w] = t.detach().reshape(-1).float().numpy()
+        times = self._views.stage(views)
         if any(_time_bits(t) != _time_bits(times[0]) for t in times):
             raise ValueError("a graphed render_cameras renders one timestamp: the cameras' times differ (%s)" % sorted(set(times)))
-        st[self.k * _VIEW_FLOATS] = float(times[0])
-        stream = torch.cuda.current_stream(self.dev)
-        self._block.copy_(self._staging, non_blocking=True)
-        self._staged.record(stream)
-        for o, w, t in dev_copies:
-            self._block[o:o + w].copy_(t.detach().reshape(-1))
 
     def _network_key(self):
         """what the captured G4DDeformParams points at: the module, its head mask, aabb and parameter storage"""
@@ -209,12 +273,4 @@ class GraphedRender:
     def check(self, sync: bool = True) -> None:
         """Raise G4DError when a replay since the last check overflowed its instance capacity (its images are incomplete) or
         met a value outside the FP16x2 operand range.  sync: wait for the replays first."""
-        s = self.ws.graph_status(sync)
-        if s.overflows:
-            raise _lib.G4DError("graphed render failed (code %d): %d replayed view(s) needed up to %d tile instances, more than "
-                                "the capacity learnt at capture; their images are incomplete (build the graph with a larger "
-                                "min_capacity)" % (ERR_OVERFLOW, s.overflows, s.max_instances))
-        if s.f16_range:
-            raise _lib.G4DError("graphed render failed (code %d): an FP16x2 tensor-core launch met a value outside the f16 "
-                                "operand range; its results were saturated (G4D_OPT_TENSOR_CORES = 0, the FFMA kernels, has no range limit)"
-                                % ERR_OVERFLOW)
+        self._gws.check(sync)

@@ -21,14 +21,16 @@ import ctypes as C
 import math
 import os
 from argparse import Namespace
+from types import SimpleNamespace
 from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 import torch
 import torch.nn as nn
 
-from . import _lib, losses
-from .renderer import render
+from . import _lib, graphs, losses
+from .deformation import deform_network
+from .renderer import _time_bits, render
 
 GAUSSIAN_GROUPS = ("xyz", "f_dc", "f_rest", "opacity", "scaling", "rotation")
 
@@ -138,6 +140,20 @@ class FlatState:
         if count_step:
             self.step_count += 1
         b0, e0 = (0, self.numel) if span is None else span
+        segs = self._segments(lrs, only, b0, e0)
+        if not segs:
+            return
+        dev = self.device
+        off = 4 * b0
+        with torch.cuda.device(dev):
+            ws = _lib.workspace_of(dev)
+            _lib.check(_lib.load().g4d_adam_step(ws.handle, self.param.data_ptr() + off, self.grad.data_ptr() + off,
+                                                 self.exp_avg.data_ptr() + off, self.exp_avg_sq.data_ptr() + off, e0 - b0, segs,
+                                                 len(segs), betas[0], betas[1], eps, self.step_count, float(grad_scale),
+                                                 _lib.stream_of(dev)), "g4d_adam_step")
+
+    def _segments(self, lrs: Dict[str, float], only, b0: int, e0: int):
+        """The Adam segments of the groups in ``only`` (None: all) clipped to [b0, e0), relative to b0."""
         clipped = []
         for n, _ in self.groups:
             if only is not None and n not in only:
@@ -145,19 +161,31 @@ class FlatState:
             sb, se = max(self.segments[n][0], b0), min(self.segments[n][1], e0)
             if se > sb:
                 clipped.append((sb - b0, se - b0, float(lrs[n])))
-        if not clipped:
-            return
         segs = (_lib.AdamSegment * len(clipped))()
         for i, (sb, se, lr) in enumerate(clipped):
             segs[i].begin, segs[i].end, segs[i].lr = sb, se, lr
+        return segs
+
+    def adam_scalars(self, lrs: Dict[str, float], span, grad_scale: float, betas=(0.9, 0.999)) -> np.ndarray:
+        """The G4DAdamScalars of ``adam_step_device`` over span at step ``step_count``: the very values adam_step uses."""
+        segs = self._segments(lrs, None, *span)
+        out = _lib.AdamScalars()
+        _lib.check(_lib.load().g4d_adam_scalars(segs, len(segs), betas[0], betas[1], self.step_count, float(grad_scale),
+                                                C.byref(out)), "g4d_adam_scalars")
+        return np.frombuffer(bytes(out), dtype=np.float32)
+
+    def adam_step_device(self, span, d_scalars: int, betas=(0.9, 0.999), eps=1e-15):
+        """adam_step over span = (begin, end) with its learning rates, bias corrections and grad scale read from the device
+        G4DAdamScalars at d_scalars when the kernel runs (``adam_scalars``): a CUDA graph replays it with each step's values."""
+        b0, e0 = span
+        segs = self._segments({n: 0.0 for n, _ in self.groups}, None, b0, e0)
         dev = self.device
         off = 4 * b0
         with torch.cuda.device(dev):
-            ws = _lib.workspace_of(dev)
-            _lib.check(_lib.load().g4d_adam_step(ws.handle, self.param.data_ptr() + off, self.grad.data_ptr() + off,
-                                                 self.exp_avg.data_ptr() + off, self.exp_avg_sq.data_ptr() + off, e0 - b0, segs,
-                                                 len(clipped), betas[0], betas[1], eps, self.step_count, float(grad_scale),
-                                                 _lib.stream_of(dev)), "g4d_adam_step")
+            _lib.check(_lib.load().g4d_adam_step_device(_lib.workspace_of(dev).handle, self.param.data_ptr() + off,
+                                                        self.grad.data_ptr() + off, self.exp_avg.data_ptr() + off,
+                                                        self.exp_avg_sq.data_ptr() + off, e0 - b0, segs, len(segs), betas[0],
+                                                        betas[1], eps, d_scalars, _lib.stream_of(dev)), "g4d_adam_step_device")
 
 
 class GaussianSet:
@@ -217,14 +245,82 @@ class GaussianSet:
         self._opacity, self._scaling, self._rotation = d["opacity"], d["scaling"], d["rotation"]
 
 
+def densifies(iteration: int, opt) -> bool:
+    """Whether step ``iteration`` densifies, prunes or resets opacities (train.py:259-285): host decisions on device values."""
+    o = opt
+    return iteration < o.densify_until_iter and (iteration % o.densification_interval == 0 or iteration % o.pruning_interval == 0
+                                                 or iteration % o.opacity_reset_interval == 0)
+
+
+def graph_action(iteration: int, opt, template_changed: bool, have_graph: bool) -> str:
+    """How ``DPTrainer(cuda_graph=True)`` runs step ``iteration``:
+
+    * "eager": a densify / prune / opacity-reset step, or the first step of a new template (template_changed: it differs from
+      the previous step's), which is the warm-up of that template;
+    * "capture": the template's second step -- or the first capturable one after an eager step replaced the flat buffers,
+      which drops the graph (have_graph False) -- runs eagerly on the graph's own workspace and is recorded;
+    * "replay": every other step."""
+    if densifies(iteration, opt) or template_changed:
+        return "eager"
+    return "replay" if have_graph else "capture"
+
+
+class _StepGraph:
+    """One captured training step and the static storage it reads: the views (ViewBlock: matrices, camera centre, time,
+    then the background and one G4DAdamScalars per all-reduce slice), the ground-truth images, and stand-in cameras whose
+    matrices are views of the block."""
+
+    def __init__(self, key, cameras, spans, dev, min_capacity):
+        k = len(cameras)
+        nsc = C.sizeof(_lib.AdamScalars) // 4
+        self.key, self.spans, self.nsc = key, spans, nsc
+        self.views = graphs.ViewBlock(dev, k, extra=4 + nsc * len(spans))
+        self.gws = graphs.GraphWorkspace(dev, [self.views.time_ptr(i) for i in range(k)], min_capacity)
+        ex = self.views.extra_at
+        self.bg = self.views.block[ex:ex + 3]
+        self.scalar_ptrs = [self.views.block[ex + 4 + nsc * i:].data_ptr() for i in range(len(spans))]
+        self.cams = []
+        for i, c in enumerate(cameras):
+            view, proj, campos = self.views.view(i)
+            self.cams.append(SimpleNamespace(image_height=int(c.image_height), image_width=int(c.image_width), FoVx=c.FoVx,
+                                             FoVy=c.FoVy, world_view_transform=view, full_proj_transform=proj,
+                                             camera_center=campos, time=0.0))
+        self.gts = [torch.zeros(3, int(c.image_height), int(c.image_width), device=dev) for c in cameras]
+        self.graph = None
+
+    def stage(self, cameras, gt_images, background, scalars):
+        extra = [(0, background)] + [(4 + self.nsc * i, a) for i, a in enumerate(scalars)]
+        self.views.stage(cameras, extra)
+        for s, gt in zip(self.gts, gt_images):
+            s.copy_(gt[:3])
+
+
 class DPTrainer:
+    """``cuda_graph=True``: steps between densifications replay one CUDA graph of the whole step (every view's forward and
+    backward, loss, regulariser, densification statistics, all-reduce, Adam); see ``graph_action`` for the schedule.  It
+    takes the NCCL backend or a single process, the g4d deformation network, a pipe without ``debug`` and camera objects
+    (not PanopticSports dicts)."""
+
     def __init__(self, gaussians: GaussianSet, opt: Optional[Namespace] = None, dist=None, world_size: int = 1, rank: int = 0,
-                 spatial_lr_scale: float = 1.0, cameras_extent: float = 1.0, seed: int = 0):
+                 spatial_lr_scale: float = 1.0, cameras_extent: float = 1.0, seed: int = 0, cuda_graph: bool = False):
+        if cuda_graph:
+            if dist is not None and world_size > 1 and dist.get_backend() != "nccl":
+                raise ValueError("cuda_graph=True needs the NCCL backend: a %s process group stages its collectives through "
+                                 "host memory and is waited for on the host" % dist.get_backend())
+            if not isinstance(gaussians._deformation, deform_network):
+                raise NotImplementedError("cuda_graph=True needs the g4d deformation network, not %s"
+                                          % type(gaussians._deformation).__name__)
         self.g, self.opt = gaussians, opt or default_opt()
         self.dist, self.world, self.rank = dist, world_size, rank
         self.spatial_lr_scale, self.extent, self.seed = spatial_lr_scale, cameras_extent, seed
         self.iteration = 0
         self.rebuilds = 0
+        self.cuda_graph = bool(cuda_graph)
+        self.captures = 0              # CUDA graphs recorded (cuda_graph=True)
+        self.last_action = None        # graph_action of the last step (cuda_graph=True)
+        self._graph: Optional[_StepGraph] = None
+        self._last_key = None
+        self._min_capacity = 0
         self.loss_accum = torch.zeros((), device=gaussians._xyz.device)
         self._rebuilt_this_step = False
         self._build_state(None)
@@ -263,44 +359,22 @@ class DPTrainer:
     # ---- one optimisation step (train.py:180-226, 259-292) ----------------------------------------------------------
     def step(self, cameras: Sequence, gt_images: Sequence[torch.Tensor], background: torch.Tensor, pipe, stage: str = "fine"):
         """cameras / gt_images: this rank's B views of the global batch.  Returns the (device) loss of this rank's views."""
+        if self.cuda_graph:
+            return self._graphed_step(cameras, gt_images, background, pipe, stage)
+        return self._eager_step(cameras, gt_images, background, pipe, stage)
+
+    def _eager_step(self, cameras, gt_images, background, pipe, stage):
         g, o = self.g, self.opt
         self.iteration += 1
         it = self.iteration
-        B = len(cameras)
-        self.state.zero_grad()
-        self.loss_accum.zero_()
-        dev = g._xyz.device
-        radii_max = torch.zeros(g._xyz.shape[0], device=dev)
-        vis_any = torch.zeros(g._xyz.shape[0], dtype=torch.bool, device=dev)
-        m2d_grad = torch.zeros(g._xyz.shape[0], 3, device=dev)
-        for cam, gt in zip(cameras, gt_images):
-            out = render(cam, g, pipe, background, stage=stage)
-            loss = losses.l1_loss(out["render"], gt[:3]) / B                       # mean over the concatenated batch (train.py:201)
-            if o.lambda_dssim != 0:
-                loss = loss + o.lambda_dssim * (1.0 - losses.ssim(out["render"], gt[:3])) / B
-            loss.backward()
-            self.loss_accum += loss.detach()
-            radii_max = torch.maximum(radii_max, out["radii"].float())
-            vis_any |= out["visibility_filter"]
-            m2d_grad += out["viewspace_points"].grad
-        if stage == "fine" and o.time_smoothness_weight != 0:
-            # view-independent: computed identically on every rank, scaled so that the 1 / world of the reduction restores it
-            w = float(self.world)
-            losses.accumulate_regulation(g._deformation, o.time_smoothness_weight * w, o.l1_time_planes * w, o.plane_tv_weight * w,
-                                         loss_accum=None)
+        stats = self._views_backward(cameras, gt_images, background, pipe, stage)
         # ---- the step's ONE exchange: the flat gradient buffer, reduced in `comm_chunks` back-to-back slices so that Adam on
         #      slice i overlaps the reduction of slice i + 1 (the collective runs on the backend's own stream)
         works = None
         if self.dist is not None and self.world > 1:
             works = self._launch_allreduce()
         if it < o.densify_until_iter:
-            # train.py:252-255 / gaussian_model.py:636-638 without the boolean-mask indexing (each `x[mask]` is a nonzero() ->
-            # one host synchronisation per statement): the same values, masked arithmetically (radii and the statistics
-            # are >= 0; an invisible Gaussian's screen-space gradient is exactly zero)
-            vis_f = vis_any.unsqueeze(-1).to(g.denom.dtype)
-            torch.maximum(g.max_radii2D, radii_max * vis_f.squeeze(-1), out=g.max_radii2D)
-            g.xyz_gradient_accum.add_(torch.norm(m2d_grad[:, :2], dim=-1, keepdim=True) * vis_f)
-            g.denom.add_(vis_f)
+            self._record_stats(*stats)
             if it % o.densification_interval == 0 or it % o.pruning_interval == 0:
                 if works is not None:                  # a rebuild copies the reduced network gradients: finish the exchange first
                     for _, _, w in works:
@@ -324,6 +398,122 @@ class DPTrainer:
         self._rebuilt_this_step = False
         return self.loss_accum
 
+    def _views_backward(self, cameras, gt_images, background, pipe, stage):
+        """Every view's forward and backward, then the regulariser, into the flat gradient buffer and loss_accum.  Returns
+        what the densification statistics take: the views' largest radii, visibility and screen-space gradients."""
+        g, o = self.g, self.opt
+        B = len(cameras)
+        self.state.zero_grad()
+        self.loss_accum.zero_()
+        dev = g._xyz.device
+        radii_max = torch.zeros(g._xyz.shape[0], device=dev)
+        vis_any = torch.zeros(g._xyz.shape[0], dtype=torch.bool, device=dev)
+        m2d_grad = torch.zeros(g._xyz.shape[0], 3, device=dev)
+        for cam, gt in zip(cameras, gt_images):
+            out = render(cam, g, pipe, background, stage=stage)
+            loss = losses.l1_loss(out["render"], gt[:3]) / B                       # mean over the concatenated batch (train.py:201)
+            if o.lambda_dssim != 0:
+                loss = loss + o.lambda_dssim * (1.0 - losses.ssim(out["render"], gt[:3])) / B
+            loss.backward()
+            self.loss_accum += loss.detach()
+            radii_max = torch.maximum(radii_max, out["radii"].float())
+            vis_any |= out["visibility_filter"]
+            m2d_grad += out["viewspace_points"].grad
+        if stage == "fine" and o.time_smoothness_weight != 0:
+            # view-independent: computed identically on every rank, scaled so that the 1 / world of the reduction restores it
+            w = float(self.world)
+            losses.accumulate_regulation(g._deformation, o.time_smoothness_weight * w, o.l1_time_planes * w, o.plane_tv_weight * w,
+                                         loss_accum=None)
+        return radii_max, vis_any, m2d_grad
+
+    def _record_stats(self, radii_max, vis_any, m2d_grad):
+        # train.py:252-255 / gaussian_model.py:636-638 without the boolean-mask indexing (each `x[mask]` is a nonzero() ->
+        # one host synchronisation per statement): the same values, masked arithmetically (radii and the statistics
+        # are >= 0; an invisible Gaussian's screen-space gradient is exactly zero)
+        g = self.g
+        vis_f = vis_any.unsqueeze(-1).to(g.denom.dtype)
+        torch.maximum(g.max_radii2D, radii_max * vis_f.squeeze(-1), out=g.max_radii2D)
+        g.xyz_gradient_accum.add_(torch.norm(m2d_grad[:, :2], dim=-1, keepdim=True) * vis_f)
+        g.denom.add_(vis_f)
+
+    # ---- the step as a CUDA graph (cuda_graph=True) --------------------------------------------------------------------
+    def _template(self, cameras, stage: str, it: int):
+        """What a captured step fixes: per view the image size and FoV, the SH degree, N, the stage, the network's head
+        mask, the loss and regulariser weights and whether the densification statistics are updated."""
+        g, o = self.g, self.opt
+        views = tuple((int(c.image_height), int(c.image_width), _time_bits(math.tan(c.FoVx * 0.5)),
+                       _time_bits(math.tan(c.FoVy * 0.5))) for c in cameras)
+        return (views, int(g.active_sh_degree), int(g._xyz.shape[0]), stage, g._deformation.head_mask(),
+                it < o.densify_until_iter, float(o.lambda_dssim), float(o.time_smoothness_weight), float(o.l1_time_planes),
+                float(o.plane_tv_weight))
+
+    def _graphed_step(self, cameras, gt_images, background, pipe, stage):
+        if getattr(pipe, "debug", False):
+            raise ValueError("cuda_graph=True cannot run with pipe.debug (it synchronises after every stage)")
+        if any(isinstance(c, dict) for c in cameras):
+            raise NotImplementedError("PanopticSports cameras are not supported by a CUDA graph")
+        if not 1 <= len(cameras) <= _lib.MAX_CAMERAS or len(gt_images) != len(cameras):
+            raise ValueError("a graphed step takes 1..%d cameras and one ground-truth image per camera" % _lib.MAX_CAMERAS)
+        it = self.iteration + 1
+        key = self._template(cameras, stage, it)
+        tg = self._graph if self._graph is not None and self._graph.key == key else None
+        action = graph_action(it, self.opt, key != self._last_key, tg is not None and tg.graph is not None)
+        self._last_key, self.last_action = key, action
+        if action == "eager":
+            self.check()
+            if tg is None:
+                self._graph = None                    # a new template: the old graph's memory goes now
+            rebuilds = self.rebuilds
+            loss = self._eager_step(cameras, gt_images, background, pipe, stage)
+            if self.rebuilds != rebuilds:
+                self._graph = None                    # the graph points at the replaced flat buffers
+            return loss
+        self.iteration = it
+        self.state.step_count += 1
+        lrs = self.learning_rates(it)
+        if tg is None:
+            st = self.state
+            spans = self._spans() if self.dist is not None and self.world > 1 else [(0, st.numel)]
+            tg = self._graph = _StepGraph(key, cameras, spans, self.g._xyz.device, self._min_capacity)
+        scalars = [self.state.adam_scalars(lrs, sp, 1.0 / self.world) for sp in tg.spans]
+        with torch.cuda.device(self.g._xyz.device):
+            tg.stage(cameras, gt_images, background, scalars)
+            if action == "capture":
+                body = lambda: self._captured_body(tg, pipe, stage, it)
+                with tg.gws.routed():
+                    body()                            # this step's work: the contexts learn their capacities
+                with tg.gws.routed():
+                    tg.graph = tg.gws.capture(body)
+                self.captures += 1
+            else:
+                tg.graph.replay()
+        return self.loss_accum
+
+    def _captured_body(self, tg: _StepGraph, pipe, stage, it):
+        stats = self._views_backward(tg.cams, tg.gts, tg.bg, pipe, stage)
+        works = self._launch_allreduce() if self.dist is not None and self.world > 1 else None
+        if it < self.opt.densify_until_iter:
+            self._record_stats(*stats)
+        for i, (span, d_scalars) in enumerate(zip(tg.spans, tg.scalar_ptrs)):
+            if works is not None:
+                self._wait(works[i][2])
+            self.state.adam_step_device(span, d_scalars)
+
+    def check(self, sync: bool = True) -> None:
+        """Raise G4DError when a replayed step since the last check overflowed a view's instance capacity (that step's
+        images, hence its gradients, were incomplete) or met a value outside the FP16x2 operand range.  The graph is then
+        dropped: the next capturable step records a new one, with the capacity raised to the largest view seen.  Eager
+        steps check first.  sync: wait for the replays."""
+        tg = self._graph
+        if tg is None or tg.graph is None:
+            return
+        s = tg.gws.ws.graph_status(sync)
+        err = graphs.status_error(s)
+        if err is not None:
+            self._graph = None
+            self._min_capacity = max(self._min_capacity, s.max_instances + s.max_instances // 2)
+            raise err
+
     comm_chunks = 4
 
     def _host_staged_collectives(self) -> bool:
@@ -344,14 +534,14 @@ class DPTrainer:
         st = self.state
         if self._host_staged_collectives():
             self._sync_device()
+        return [(b, e, self.dist.all_reduce(st.grad[b:e], op=self.dist.ReduceOp.SUM, async_op=True)) for b, e in self._spans()]
+
+    def _spans(self):
+        """the `comm_chunks` slices of the flat buffers, multiples of 4 floats"""
+        n = self.state.numel
         k = max(1, int(self.comm_chunks))
-        step = (st.numel // k + 3) // 4 * 4
-        works, b = [], 0
-        while b < st.numel:
-            e = min(st.numel, b + step)
-            works.append((b, e, self.dist.all_reduce(st.grad[b:e], op=self.dist.ReduceOp.SUM, async_op=True)))
-            b = e
-        return works
+        step = (n // k + 3) // 4 * 4
+        return [(b, min(n, b + step)) for b in range(0, n, step)]
 
     def _global_stats(self):
         """(sum of ||grad means2D||, visible count, max radii) over ALL ranks.  The per-rank accumulators stay local (they
