@@ -41,7 +41,7 @@ ABI_SYMBOLS = [
     "g4d_rasterize_backward", "g4d_render_forward", "g4d_render_backward", "g4d_workspace_set_option", "g4d_context_read",
     "g4d_context_stage_times", "g4d_debug_tc_cycles", "g4d_l1_loss", "g4d_l1_loss_backward", "g4d_ssim", "g4d_ssim_backward",
     "g4d_plane_regulation", "g4d_dist2_knn3", "g4d_adam_step", "g4d_render_forward_cameras", "g4d_render_backward_cameras",
-    "g4d_context_set_time_source", "g4d_workspace_freeze", "g4d_workspace_graph_status", "g4d_adam_scalars",
+    "g4d_context_set_time_source", "g4d_context_set_camera_grad", "g4d_workspace_freeze", "g4d_workspace_graph_status", "g4d_adam_scalars",
     "g4d_adam_step_device", "g4d_deform_forward_times", "g4d_deform_backward_times",
 ]
 
@@ -168,6 +168,7 @@ def load():
                                       C.c_float, C.c_int64, C.c_float, C.c_void_p]
         lib.g4d_dist2_knn3.argtypes = [C.c_void_p, C.c_int64, fp, fp, C.c_void_p]
         lib.g4d_context_set_time_source.argtypes = [C.c_void_p, fp]
+        lib.g4d_context_set_camera_grad.argtypes = [C.c_void_p, fp]
         lib.g4d_workspace_freeze.argtypes = [C.c_void_p, C.c_int]
         lib.g4d_workspace_graph_status.argtypes = [C.c_void_p, C.c_int, C.POINTER(GraphStatus)]
         lib.g4d_adam_scalars.argtypes = [C.POINTER(AdamSegment), C.c_int32, C.c_float, C.c_float, C.c_int64, C.c_float,
@@ -354,6 +355,11 @@ class Context:
     def set_time_source(self, d_time: Optional[int]):
         """Read the timestamp of every forward / backward on this context from the device float at d_time (None: the camera's)."""
         check(load().g4d_context_set_time_source(self.handle, d_time), "g4d_context_set_time_source")
+
+    def set_camera_grad(self, d_out: Optional[int]):
+        """Every backward on this context overwrites the 35 device floats at d_out with dL/d (view[16], proj[16], campos[3])
+        of its camera (None: off)."""
+        check(load().g4d_context_set_camera_grad(self.handle, d_out), "g4d_context_set_camera_grad")
 
     def stats(self) -> Stats:
         s = Stats()

@@ -170,6 +170,7 @@ struct G4DContext {
     int grid_x = 0, grid_y = 0;
     int64_t R = 0, capacity = 0;
     const float* time_src = nullptr;  // g4d_context_set_time_source (device; NULL: G4DCamera.time)
+    float* cam_grad = nullptr;        // g4d_context_set_camera_grad (device, kCamGradFloats; NULL: no camera gradient)
     const void* bin_ctl = nullptr;    // device BinCtl of the last forward
     bool learned = false;             // R of an earlier exact forward is known (no-sync mode needs a learnt capacity)
     GeomBuffers g{};
@@ -626,7 +627,20 @@ template <class Sh, class T> Sh caller_sh(int m, bool split, T* dc, T* rest = nu
     return split ? Sh{nullptr, dc, rest, m} : Sh{dc, nullptr, nullptr, m};
 }
 
-// blend backward + per-Gaussian backward on `in`; opacity gradient lands in g_opacities (zeroed here)
+// The camera-gradient sinks of a backward on ctx[0, k) (g4d_context_set_camera_grad): refused while capturing (a graph would
+// keep writing a sink the context may since have dropped), else zeroed on st; the per-Gaussian backward adds into them, and
+// a camera outside the loss keeps the zeros.  Called before the backward's first launch.
+int zero_camera_grads(G4DContext* const* ctx, int k, cudaStream_t st) {
+    for (int i = 0; i < k; ++i)
+        if (ctx[i]->cam_grad && t_call.capturing)
+            return fail(G4D_ERR_STATE, "cannot capture a backward on a context with a camera gradient set (g4d_context_set_camera_grad)");
+    for (int i = 0; i < k; ++i)
+        if (ctx[i]->cam_grad) G4D_CUDA(cudaMemsetAsync(ctx[i]->cam_grad, 0, kCamGradFloats * sizeof(float), st));
+    return G4D_OK;
+}
+
+// blend backward + per-Gaussian backward on `in`; opacity gradient lands in g_opacities (zeroed here); the camera's
+// gradient is added into c->cam_grad when it is set
 int raster_backward_stages(G4DContext* c, const G4DCamera* cam, int64_t n, const RasterInputs& in, const float* dL_dcolor,
                            float* g_means3D, float* g_means2D, const ShOut& g_sh, float* g_opacities, float* g_scales,
                            float* g_rotations, cudaStream_t st) {
@@ -651,7 +665,7 @@ int raster_backward_stages(G4DContext* c, const G4DCamera* cam, int64_t n, const
     if ((rc = debug_sync(cam, st, "blend_backward")) != G4D_OK) return rc;
     StageTimer tm(c, G4D_STAGE_GEOM_BWD, st);
     G4D_CUDA(launch_preprocess_backward(dcam, n, in, c->g, g_mean2D, g_conic, g_rgb, g_means3D, g_means2D, g_scales,
-                                        g_rotations, g_sh, st));
+                                        g_rotations, g_sh, c->cam_grad, st));
     return debug_sync(cam, st, "preprocess_backward");
 }
 
@@ -864,6 +878,7 @@ int g4d_rasterize_backward(G4DContext* c, const G4DCamera* cam, int64_t n, const
     if (scope.rc != G4D_OK) return scope.rc;
     if ((rc = refuse_capture(c->ws, cam, 1, nullptr)) != G4D_OK) return rc;
     if ((rc = check_pending(c)) != G4D_OK) return rc;
+    if ((rc = zero_camera_grads(&c, 1, st)) != G4D_OK) return rc;
     (void)opacities;
     const int m = sh_coeffs(cam);
     const RasterInputs in{means3D, scales, rotations, opacities, caller_sh<ShIn>(m, false, shs)};
@@ -1247,6 +1262,7 @@ int g4d_render_backward(G4DContext* c, const G4DCamera* cam, const G4DDeformPara
     if (scope.rc != G4D_OK) return scope.rc;
     if ((rc = refuse_capture(c->ws, cam, 1, nullptr)) != G4D_OK) return rc;
     if ((rc = check_pending(c)) != G4D_OK) return rc;
+    if ((rc = zero_camera_grads(&c, 1, st)) != G4D_OK) return rc;
     return fused_backward(c, cam, prm, pgrads, g, dL_dcolor, gg, st);
 }
 
@@ -1335,6 +1351,7 @@ int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCame
     if ((rc = refuse_capture(ws, cams, k, nullptr)) != G4D_OK) return rc;
     for (int i = 0; i < k; ++i)
         if ((rc = check_pending(ctx[i])) != G4D_OK) return rc;
+    if ((rc = zero_camera_grads(ctx, k, st)) != G4D_OK) return rc;
     if (k == 1 && dL_dcolor[0]) {     // one camera: the single-camera backward
         G4DGaussianGrads g1 = *gg;
         g1.means2D = g_means2D ? g_means2D[0] : nullptr;
@@ -1347,6 +1364,8 @@ int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCame
     if ((rc = deformed_grads(c0, n, gg, &d)) != G4D_OK) return rc;
     // blend backward of every camera in the loss, each into its own scratch
     BackwardCameras bc{};
+    CamGradSinks cs{};
+    bool cam_grads = false;
     for (int i = 0; i < k; ++i) {
         G4DContext* c = ctx[i];
         reset_stage_flags(c, G4D_STAGE_BLEND_BWD, G4D_STAGE_DEFORM_BWD);
@@ -1367,11 +1386,13 @@ int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCame
         const int j = bc.count++;
         bc.cam[j] = c->cam.as<CameraDev>(); bc.radii[j] = c->g.radii; bc.clamped[j] = c->g.clamped; bc.grad[j] = gb;
         bc.g_means2D[j] = g_means2D ? g_means2D[i] : nullptr;
+        cs.out[j] = c->cam_grad;
+        cam_grads |= c->cam_grad != nullptr;
     }
     {
         StageTimer tm(c0, G4D_STAGE_GEOM_BWD, st);
         G4D_CUDA(launch_preprocess_backward_cameras(bc, n, deformed_inputs(c0, c0->fwd, g), d.xyz, d.sc, d.rot, d.op,
-                                                    fused_sh_sinks(c0, g, gg, d.sh), st));
+                                                    fused_sh_sinks(c0, g, gg, d.sh), cam_grads ? &cs : nullptr, st));
     }
     if ((rc = debug_sync(&cams[0], st, "preprocess_backward_cameras")) != G4D_OK) return rc;
     // the network's backward, once, on the gradients summed over the cameras
@@ -1496,6 +1517,12 @@ int g4d_dist2_knn3(G4DWorkspace* ws, int64_t n, const float* xyz, float* out_mea
 int g4d_context_set_time_source(G4DContext* c, const float* d_time) {
     if (!c) return fail(G4D_ERR_ARG, "context is NULL");
     c->time_src = d_time;
+    return G4D_OK;
+}
+
+int g4d_context_set_camera_grad(G4DContext* c, float* d_out) {
+    if (!c) return fail(G4D_ERR_ARG, "context is NULL");
+    c->cam_grad = d_out;
     return G4D_OK;
 }
 

@@ -9,13 +9,31 @@
 
 namespace g4d {
 
-// FULL: M = 16 SH coefficients per Gaussian (ShIn), else M = in.sh.m = g_sh.m
-template <bool FULL>
+// Adds the camera terms of the warp's lanes [0, cnt) into acc[kCamGradFloats]: a shuffle tree to lane 0 per element the
+// forward reads, then one atomic per such element.  Called by exactly the lanes [0, cnt) (cnt >= 1).
+G4D_D void cam_grad_flush(const CamGrad& cg, int lane, int cnt, float* __restrict__ acc) {
+    const unsigned mask = cnt == 32 ? 0xffffffffu : (1u << cnt) - 1u;
+#pragma unroll
+    for (int i = 0; i < kCamGradFloats; ++i) {
+        if (!cam_grad_read(i)) continue;
+        float s = cg.g[i];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float t = __shfl_down_sync(mask, s, o);
+            if (lane + o < cnt) s = add_rn(s, t);
+        }
+        if (lane == 0) atomicAdd(acc + i, s);
+    }
+}
+
+// FULL: M = 16 SH coefficients per Gaussian (ShIn), else M = in.sh.m = g_sh.m.  CAM: the camera's gradient is added into
+// g_cam[kCamGradFloats] (zeroed by the caller).
+template <bool FULL, bool CAM>
 __global__ void __launch_bounds__(256)
 preprocess_backward_kernel(const CameraDev* __restrict__ camp, int64_t n, RasterInputs in, GeomBuffers g,
                            const float* __restrict__ g_mean2D, const float* __restrict__ g_conic,
                            const float* __restrict__ g_rgb, float* __restrict__ g_means3D, float* __restrict__ g_means2D_out,
-                           float* __restrict__ g_scales, float* __restrict__ g_rotations, ShOut g_sh) {
+                           float* __restrict__ g_scales, float* __restrict__ g_rotations, ShOut g_sh, float* __restrict__ g_cam) {
     // SH coefficients travel through shared memory: a warp reads / writes the 32 x 48 floats of its Gaussians as contiguous
     // 128-byte lines instead of 48 scalar accesses per thread at a 192-byte stride
     extern __shared__ float sh_smem[];             // [warps][2][32 * kShRow]
@@ -34,6 +52,10 @@ preprocess_backward_kernel(const CameraDev* __restrict__ camp, int64_t n, Raster
     __syncwarp();
     auto sh_store = [&](int k, int ch, float v) { st[lane * kShRow + 3 * k + ch] = v; };
     if (active) {
+        CamGrad cg;
+        if constexpr (CAM)
+#pragma unroll
+            for (int i = 0; i < kCamGradFloats; ++i) cg.g[i] = 0.f;
         if (g_means2D_out) {
             const bool vis = g.radii[gi] > 0;
             g_means2D_out[3 * gi] = vis ? g_mean2D[2 * gi] : 0.f;
@@ -54,11 +76,12 @@ preprocess_backward_kernel(const CameraDev* __restrict__ camp, int64_t n, Raster
             const float gr[3] = {g_rgb[3 * gi], g_rgb[3 * gi + 1], g_rgb[3 * gi + 2]};
             GaussGrad gg;
             const float* row = ld + lane * kShRow;
-            gaussian_backward(cam, p, sc, Quat{q4.x, q4.y, q4.z, q4.w}, (uint32_t)g.clamped[gi], gm2, gc, gr,
-                              [&](int k, int ch) { return row[3 * k + ch]; }, sh_store, gg);
+            gaussian_backward<CAM>(cam, p, sc, Quat{q4.x, q4.y, q4.z, q4.w}, (uint32_t)g.clamped[gi], gm2, gc, gr,
+                                   [&](int k, int ch) { return row[3 * k + ch]; }, sh_store, gg, &cg);
             for (int k = 0; k < 3; ++k) { g_means3D[3 * gi + k] = gg.mean[k]; g_scales[3 * gi + k] = gg.scale[k]; }
             for (int k = 0; k < 4; ++k) g_rotations[4 * gi + k] = gg.rot[k];
         }
+        if constexpr (CAM) cam_grad_flush(cg, lane, cnt, g_cam);
     }
     __syncwarp();
     g_sh.store_warp<FULL>(g0, cnt, lane, st);
@@ -67,30 +90,33 @@ preprocess_backward_kernel(const CameraDev* __restrict__ camp, int64_t n, Raster
 cudaError_t launch_preprocess_backward(const CameraDev* cam, int64_t n, const RasterInputs& in, GeomBuffers g,
                                        const float* g_mean2D, const float* g_conic, const float* g_rgb, float* g_means3D,
                                        float* g_means2D_out, float* g_scales, float* g_rotations, const ShOut& g_sh,
-                                       cudaStream_t st) {
+                                       float* g_cam, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
     constexpr int kThreads = 128;
     const size_t smem = (size_t)(kThreads / 32) * 2 * 32 * kShRow * sizeof(float);   // 50 KB: SH staging (see the kernel)
-    auto kernel = g_sh.m == kShCoeffs ? preprocess_backward_kernel<true> : preprocess_backward_kernel<false>;
+    const bool full = g_sh.m == kShCoeffs;
+    auto kernel = g_cam ? (full ? preprocess_backward_kernel<true, true> : preprocess_backward_kernel<false, true>)
+                        : (full ? preprocess_backward_kernel<true, false> : preprocess_backward_kernel<false, false>);
     {
         cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
     }
     kernel<<<(unsigned)((n + kThreads - 1) / kThreads), kThreads, smem, st>>>(cam, n, in, g, g_mean2D, g_conic, g_rgb,
                                                                                                   g_means3D, g_means2D_out, g_scales,
-                                                                                                  g_rotations, g_sh);
+                                                                                                  g_rotations, g_sh, g_cam);
     return cudaGetLastError();
 }
 
 // Per-Gaussian backward of several cameras at one timestamp (g4d_render_backward_cameras): the deformed state and the SH
 // coefficients are loaded once, gaussian_backward runs for every camera that sees the Gaussian, and the sums -- mean,
 // scale and rotation in registers, SH in the warp's shared-memory rows, opacity from the cameras' blend backward passes --
-// are written once.  Each camera's screen-space gradient goes to its own sink.
-template <bool FULL>
+// are written once.  Each camera's screen-space gradient goes to its own sink.  CAM: camera c's gradient is added into
+// cs.out[c][kCamGradFloats] (zeroed by the caller; NULL: not wanted), reduced over the warp inside the loop over the cameras.
+template <bool FULL, bool CAM>
 __global__ void __launch_bounds__(128)
 preprocess_backward_cameras_kernel(BackwardCameras bc, int64_t n, RasterInputs in, float* __restrict__ g_means3D,
                                    float* __restrict__ g_scales, float* __restrict__ g_rotations, float* __restrict__ g_opacities,
-                                   ShOut g_sh) {
+                                   ShOut g_sh, CamGradSinks cs) {
     extern __shared__ float sh_smem[];             // [warps][2][32 * kShRow]: SH coefficients, SH gradient sums
     __shared__ CameraDev cams[G4D_MAX_CAMERAS];
     stage_cameras(cams, bc.cam, bc.count);
@@ -125,16 +151,23 @@ preprocess_backward_cameras_kernel(BackwardCameras bc, int64_t n, RasterInputs i
                 bc.g_means2D[c][3 * gi + 1] = vis ? gmb[2 * gi + 1] : 0.f;
                 bc.g_means2D[c][3 * gi + 2] = 0.f;
             }
-            if (!vis) continue;
-            const float gm2[2] = {gmb[2 * gi], gmb[2 * gi + 1]};
-            const float gc[3] = {gcb[3 * gi], gcb[3 * gi + 1], gcb[3 * gi + 2]};
-            const float grgb[3] = {grb[3 * gi], grb[3 * gi + 1], grb[3 * gi + 2]};
-            GaussGrad gg;
-            gaussian_backward(cams[c], p, sc, Quat{q4.x, q4.y, q4.z, q4.w}, (uint32_t)bc.clamped[c][gi], gm2, gc, grgb,
-                              [&](int k, int ch) { return row[3 * k + ch]; },
-                              [&](int k, int ch, float v) { srow[3 * k + ch] += v; }, gg);
-            for (int k = 0; k < 3; ++k) { gm[k] += gg.mean[k]; gs[k] += gg.scale[k]; }
-            for (int k = 0; k < 4; ++k) gr[k] += gg.rot[k];
+            CamGrad cg;
+            if constexpr (CAM)
+#pragma unroll
+                for (int i = 0; i < kCamGradFloats; ++i) cg.g[i] = 0.f;
+            if (vis) {
+                const float gm2[2] = {gmb[2 * gi], gmb[2 * gi + 1]};
+                const float gc[3] = {gcb[3 * gi], gcb[3 * gi + 1], gcb[3 * gi + 2]};
+                const float grgb[3] = {grb[3 * gi], grb[3 * gi + 1], grb[3 * gi + 2]};
+                GaussGrad gg;
+                gaussian_backward<CAM>(cams[c], p, sc, Quat{q4.x, q4.y, q4.z, q4.w}, (uint32_t)bc.clamped[c][gi], gm2, gc, grgb,
+                                       [&](int k, int ch) { return row[3 * k + ch]; },
+                                       [&](int k, int ch, float v) { srow[3 * k + ch] += v; }, gg, &cg);
+                for (int k = 0; k < 3; ++k) { gm[k] += gg.mean[k]; gs[k] += gg.scale[k]; }
+                for (int k = 0; k < 4; ++k) gr[k] += gg.rot[k];
+            }
+            if constexpr (CAM)
+                if (cs.out[c]) cam_grad_flush(cg, lane, cnt, cs.out[c]);
         }
         for (int k = 0; k < 3; ++k) { g_means3D[3 * gi + k] = gm[k]; g_scales[3 * gi + k] = gs[k]; }
         for (int k = 0; k < 4; ++k) g_rotations[4 * gi + k] = gr[k];
@@ -146,15 +179,17 @@ preprocess_backward_cameras_kernel(BackwardCameras bc, int64_t n, RasterInputs i
 
 cudaError_t launch_preprocess_backward_cameras(const BackwardCameras& bc, int64_t n, const RasterInputs& in, float* g_means3D,
                                                float* g_scales, float* g_rotations, float* g_opacities, const ShOut& g_sh,
-                                               cudaStream_t st) {
+                                               const CamGradSinks* cs, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
     constexpr int kThreads = 128;
     const size_t smem = (size_t)(kThreads / 32) * 2 * 32 * kShRow * sizeof(float);   // 50 KB: SH staging and sums
-    auto kernel = g_sh.m == kShCoeffs ? preprocess_backward_cameras_kernel<true> : preprocess_backward_cameras_kernel<false>;
+    const bool full = g_sh.m == kShCoeffs;
+    auto kernel = cs ? (full ? preprocess_backward_cameras_kernel<true, true> : preprocess_backward_cameras_kernel<false, true>)
+                     : (full ? preprocess_backward_cameras_kernel<true, false> : preprocess_backward_cameras_kernel<false, false>);
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     kernel<<<(unsigned)((n + kThreads - 1) / kThreads), kThreads, smem, st>>>(
-        bc, n, in, g_means3D, g_scales, g_rotations, g_opacities, g_sh);
+        bc, n, in, g_means3D, g_scales, g_rotations, g_opacities, g_sh, cs ? *cs : CamGradSinks{});
     return cudaGetLastError();
 }
 

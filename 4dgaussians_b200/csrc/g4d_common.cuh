@@ -21,6 +21,7 @@ namespace g4d {
 constexpr int kTile = 16;                 // BLOCK_X = BLOCK_Y (A: 16x16 pixel tiles)
 constexpr int kTilePixels = kTile * kTile;
 constexpr int kShCoeffs = 16;             // coefficient slots per Gaussian ([N,16,3])
+constexpr int kCamGradFloats = 35;        // a camera's gradient: view [16], proj [16], campos [3] (g4d_context_set_camera_grad)
 constexpr float kNearCull = 0.2f;         // A.1 step 2
 constexpr float kWEps = 0.0000001f;       // A.1 step 3
 constexpr float kGuardBand = 1.3f;        // A.1 step 5

@@ -292,11 +292,12 @@ cudaError_t launch_blend_forward(const CameraDev* cam, int grid_x, int grid_y, G
 cudaError_t launch_blend_backward(const CameraDev* cam, int grid_x, int grid_y, GeomBuffers g, BinBuffers b, ImageBuffers im,
                                   const float* dL_dcolor, float* g_mean2D, float* g_conic, float* g_opacity, float* g_rgb,
                                   int warp_cull, cudaStream_t st);
-// per-Gaussian backward
+// per-Gaussian backward; g_cam != NULL: the camera's gradient (view[16], proj[16], campos[3]) is also added into g_cam,
+// which the caller zeroes first
 cudaError_t launch_preprocess_backward(const CameraDev* cam, int64_t n, const RasterInputs& in, GeomBuffers g,
                                        const float* g_mean2D, const float* g_conic, const float* g_rgb, float* g_means3D,
                                        float* g_means2D_out, float* g_scales, float* g_rotations, const ShOut& g_sh,
-                                       cudaStream_t st);
+                                       float* g_cam, cudaStream_t st);
 
 // Backward of the deformation network (g4d_backward.cu): the HexPlane gather (skipped when saved_feat holds the features
 // the forward gathered; order: its walk order), an engine -- the tensor-core kernels with the images tc, or the FFMA kernels
@@ -330,11 +331,17 @@ struct BackwardCameras {
     const float* grad[G4D_MAX_CAMERAS];    // the camera's blend backward, BlendGradLayout
     float* g_means2D[G4D_MAX_CAMERAS];     // [N,3] screen-space gradient of the camera, or NULL
 };
+// the camera-gradient accumulators of those cameras (out[j]: camera j of BackwardCameras, kCamGradFloats floats, zeroed
+// before the launch)
+struct CamGradSinks {
+    float* out[G4D_MAX_CAMERAS];
+};
 // per-Gaussian backward of all those cameras in one pass: the gradients w.r.t. means3D, scales, rotations, opacity and the
-// SH coefficients are summed over the cameras and written once (OVERWRITTEN)
+// SH coefficients are summed over the cameras and written once (OVERWRITTEN); cs != NULL: each camera's gradient is also
+// added into its sink
 cudaError_t launch_preprocess_backward_cameras(const BackwardCameras& bc, int64_t n, const RasterInputs& in, float* g_means3D,
                                                float* g_scales, float* g_rotations, float* g_opacities, const ShOut& g_sh,
-                                               cudaStream_t st);
+                                               const CamGradSinks* cs, cudaStream_t st);
 
 // coarse stage of render(): the fused forward's tail without the deformation network (io as for launch_deform mode 1)
 cudaError_t launch_activate_preprocess(const CameraDev* cam, int64_t n, const DeformIO& io, cudaStream_t st);

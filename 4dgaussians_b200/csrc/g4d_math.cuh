@@ -241,11 +241,36 @@ G4D_HD void sh_dir_grad(int deg, float x, float y, float z, ShLoad sh, const flo
     s = S(15); gdir[0] += G4D_SH3_6 * (3.f * xx - 3.f * yy) * s; gdir[1] += G4D_SH3_6 * -6.f * x * y * s;
 }
 
-// ShLoad as above; ShStore: void operator()(int coeff, int channel, float grad)
-template <class ShLoad, class ShStore>
+// Rounded product and sum that the compiler may neither contract into an FMA nor merge with the contractable arithmetic
+// around them (mul.rn / add.rn): the camera terms of gaussian_backward use only these, so that computing them adds no use
+// to a product of the per-Gaussian gradients and leaves those gradients' own contractions -- and bits -- as they were.
+G4D_HD float mul_rn(float a, float b) {
+#if defined(__CUDA_ARCH__)
+    return __fmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+G4D_HD float add_rn(float a, float b) {
+#if defined(__CUDA_ARCH__)
+    return __fadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+
+// The camera side of one Gaussian's backward: dL/d view [16], proj [16], campos [3], each in the element order of the
+// caller's tensor (cam.view[i] is element i of the flattened world_view_transform).  Elements the forward never reads --
+// view 3, 7, 11, 15 (xform4x3 uses rows 0..2) and proj 2, 6, 10, 14 (the clip-space z row) -- are zero.
+struct CamGrad { float g[kCamGradFloats]; };
+G4D_HD constexpr bool cam_grad_read(int i) { return i < 16 ? (i & 3) != 3 : i < 32 ? (i & 3) != 2 : true; }
+
+// ShLoad as above; ShStore: void operator()(int coeff, int channel, float grad).  CAM: also the camera terms, into *cg
+// (every element written), in mul_rn / add_rn only: the GaussGrad outputs are those of CAM = false bit for bit.
+template <bool CAM = false, class ShLoad, class ShStore>
 G4D_HD void gaussian_backward(const CameraDev& cam, Vec3 p, Vec3 scale, Quat rot, uint32_t clamped_bits,
                               const float g_mean2D[2], const float g_conic[3], const float g_rgb[3], ShLoad sh,
-                              ShStore sh_store, GaussGrad& out) {
+                              ShStore sh_store, GaussGrad& out, CamGrad* cg = nullptr) {
     const float* v = cam.view;
     const float* pm = cam.proj;
     float gm[3] = {0.f, 0.f, 0.f};
@@ -293,6 +318,26 @@ G4D_HD void gaussian_backward(const CameraDev& cam, Vec3 p, Vec3 scale, Quat rot
     gm[0] += Wr[0][0] * gtx + Wr[1][0] * gty + Wr[2][0] * gtz;
     gm[1] += Wr[0][1] * gtx + Wr[1][1] * gty + Wr[2][1] * gtz;
     gm[2] += Wr[0][2] * gtx + Wr[1][2] * gty + Wr[2][2] * gtz;
+    if constexpr (CAM) {
+        // view: p_view = W p + t, so dL/d view[4c + r] = dL/d p_view[r] * [p, 1][c]; and T = J W, so the rows of W get J^T gT
+        // (J: cov2d_project's j00, j02, j11, j12 at the clamped point)
+        float* gv = cg->g;
+        const float gp[3] = {gtx, gty, gtz};
+        const float j00 = mul_rn(fx, itz), j02 = -mul_rn(mul_rn(fx, ax.tx), itz2);
+        const float j11 = mul_rn(fy, itz), j12 = -mul_rn(mul_rn(fy, ax.ty), itz2);
+#pragma unroll
+        for (int r = 0; r < 3; ++r) {
+            gv[r] = mul_rn(gp[r], p.x); gv[4 + r] = mul_rn(gp[r], p.y); gv[8 + r] = mul_rn(gp[r], p.z); gv[12 + r] = gp[r];
+        }
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+            gv[4 * j] = add_rn(gv[4 * j], mul_rn(j00, gT0[j]));
+            gv[4 * j + 1] = add_rn(gv[4 * j + 1], mul_rn(j11, gT1[j]));
+            gv[4 * j + 2] = add_rn(gv[4 * j + 2], add_rn(mul_rn(j02, gT0[j]), mul_rn(j12, gT1[j])));
+            gv[4 * j + 3] = 0.f;
+        }
+        gv[15] = 0.f;
+    }
     // (2) mean2D (NDC units) -> mean3D through the projective divide
     {
         float hx = pm[0] * p.x + pm[4] * p.y + pm[8] * p.z + pm[12];
@@ -304,6 +349,18 @@ G4D_HD void gaussian_backward(const CameraDev& cam, Vec3 p, Vec3 scale, Quat rot
         gm[0] += (pm[0] * mw - pm[3] * mul1) * g0 + (pm[1] * mw - pm[3] * mul2) * g1;
         gm[1] += (pm[4] * mw - pm[7] * mul1) * g0 + (pm[5] * mw - pm[7] * mul2) * g1;
         gm[2] += (pm[8] * mw - pm[11] * mul1) * g0 + (pm[9] * mw - pm[11] * mul2) * g1;
+        if constexpr (CAM) {
+            // ndc = (hx, hy) / (hw + eps) with h = proj [p, 1]: dL/d proj[4c + r] = dL/dh[r] * [p, 1][c], r = x, y, w
+            float* gp = cg->g + 16;
+            const float ghx = mul_rn(g0, mw), ghy = mul_rn(g1, mw), ghw = -add_rn(mul_rn(g0, mul1), mul_rn(g1, mul2));
+            const float ph[3] = {p.x, p.y, p.z};
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                gp[4 * c] = mul_rn(ghx, ph[c]); gp[4 * c + 1] = mul_rn(ghy, ph[c]); gp[4 * c + 2] = 0.f;
+                gp[4 * c + 3] = mul_rn(ghw, ph[c]);
+            }
+            gp[12] = ghx; gp[13] = ghy; gp[14] = 0.f; gp[15] = ghw;
+        }
     }
     // (3) colour -> SH coefficients and view direction
     {
@@ -326,6 +383,11 @@ G4D_HD void gaussian_backward(const CameraDev& cam, Vec3 p, Vec3 scale, Quat rot
         gm[0] += (gdir[0] - x * dot) * ilen;
         gm[1] += (gdir[1] - y * dot) * ilen;
         gm[2] += (gdir[2] - z * dot) * ilen;
+        if constexpr (CAM) {   // the direction is p - campos: campos gets the negated mean term, (dir * dot - gdir) / len
+            cg->g[32] = mul_rn(add_rn(mul_rn(x, dot), -gdir[0]), ilen);
+            cg->g[33] = mul_rn(add_rn(mul_rn(y, dot), -gdir[1]), ilen);
+            cg->g[34] = mul_rn(add_rn(mul_rn(z, dot), -gdir[2]), ilen);
+        }
     }
     out.mean[0] = gm[0]; out.mean[1] = gm[1]; out.mean[2] = gm[2];
     // (4) Sigma -> scale, quaternion

@@ -57,6 +57,55 @@ def camera_from_settings(rs: GaussianRasterizationSettings, time: float = 0.0, k
     return cam
 
 
+# the camera tensors a backward can differentiate: name in the settings, offset in the C-ABI's 35-float camera gradient
+# (g4d_context_set_camera_grad), element count
+_CAM_FIELDS = (("viewmatrix", 0, 16), ("projmatrix", 16, 16), ("campos", 32, 3))
+
+
+def camera_grad_leaves(rss):
+    """The camera tensors of the settings ``rss`` that take a gradient (grad mode on, ``requires_grad``): ``spec``, one
+    (camera, field) pair per tensor, and the tensors.  Both are empty when there is none."""
+    if not torch.is_grad_enabled():
+        return (), ()
+    spec, leaves = [], []
+    for i, rs in enumerate(rss):
+        for f, (name, _, _) in enumerate(_CAM_FIELDS):
+            t = getattr(rs, name)
+            if torch.is_tensor(t) and t.requires_grad:
+                spec.append((i, f))
+                leaves.append(t)
+    return tuple(spec), tuple(leaves)
+
+
+class CameraGradSinks:
+    """One [k, 35] float32 device buffer whose row i the backward on context ``ctxs[i]`` overwrites with its camera's
+    gradient, for the cameras named in ``spec``; the contexts' pointers are cleared again on exit (they return to a pool)."""
+
+    def __init__(self, spec, ctxs, dev):
+        self.cams = sorted({i for i, _ in spec})
+        self.ctxs = ctxs
+        self.buf = torch.empty(len(ctxs), 35, device=dev, dtype=torch.float32) if spec else None
+
+    def __enter__(self):
+        for i in self.cams:
+            self.ctxs[i].set_camera_grad(self.buf[i].data_ptr())
+        return self
+
+    def __exit__(self, *exc):
+        for i in self.cams:
+            self.ctxs[i].set_camera_grad(None)
+        return False
+
+    def grads(self, spec, metas):
+        """The gradient of each camera tensor of ``spec`` in its (shape, dtype, device), ``metas`` (``tensor_meta``)."""
+        return tuple(self.buf[i, off:off + n].reshape(shape).to(device=device, dtype=dtype)
+                     for (i, f), (shape, dtype, device) in zip(spec, metas) for _, off, n in (_CAM_FIELDS[f],))
+
+
+def tensor_meta(tensors):
+    return tuple((t.shape, t.dtype, t.device) for t in tensors)
+
+
 class _ContextLease:
     """Returns the context to the workspace pool when the autograd node dies."""
 
@@ -78,7 +127,7 @@ class _ContextLease:
 
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, raster_settings):
+    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, raster_settings, cam_spec, *cam_leaves):
         lib = _lib.load()
         dev = means3D.device
         n = means3D.shape[0]
@@ -101,6 +150,7 @@ class _RasterizeGaussians(torch.autograd.Function):
                                                  sc.data_ptr(), ro.data_ptr(), color.data_ptr(), depth.data_ptr(),
                                                  radii.data_ptr(), _lib.stream_of(dev)), "g4d_rasterize_forward")
         ctx.raster_settings = raster_settings
+        ctx.cam_spec, ctx.cam_meta = cam_spec, tensor_meta(cam_leaves)
         ctx.lease = lease
         ctx.n, ctx.m = n, m
         ctx.save_for_backward(m3, shc, op, sc, ro)
@@ -126,14 +176,16 @@ class _RasterizeGaussians(torch.autograd.Function):
         lease = ctx.lease
         if lease is None or lease.ctx is None:
             raise RuntimeError("rasterizer backward called twice (context already released)")
-        with torch.cuda.device(dev):
+        sinks = CameraGradSinks(ctx.cam_spec, [lease.ctx], dev)
+        with torch.cuda.device(dev), sinks:
             _lib.check(lib.g4d_rasterize_backward(lease.ctx.handle, C.byref(cam), n, m3.data_ptr(), shc.data_ptr(), op.data_ptr(),
                                                   sc.data_ptr(), ro.data_ptr(), gcol.data_ptr(), g_means3D.data_ptr(),
                                                   g_means2D.data_ptr(), g_sh.data_ptr(), g_op.data_ptr(), g_sc.data_ptr(),
                                                   g_ro.data_ptr(), _lib.stream_of(dev)), "g4d_rasterize_backward")
         lease.release()
         ctx.lease = None
-        return g_means3D, g_means2D, g_sh, g_op, g_sc, g_ro, None
+        cam_grads = sinks.grads(ctx.cam_spec, ctx.cam_meta) if ctx.cam_spec else ()
+        return (g_means3D, g_means2D, g_sh, g_op, g_sc, g_ro, None, None) + cam_grads
 
 
 class GaussianRasterizer(nn.Module):
@@ -155,4 +207,6 @@ class GaussianRasterizer(nn.Module):
         if colors_precomp is not None or cov3D_precomp is not None:
             raise NotImplementedError("colors_precomp / cov3D_precomp are dead paths in the reference "
                                       "(gaussian_renderer/__init__.py:74-78,105-116) and are not provided")
-        return _RasterizeGaussians.apply(means3D, means2D, shs, opacities, scales, rotations, rs)
+        # the settings' viewmatrix / projmatrix / campos that require grad join the autograd graph as extra inputs
+        cam_spec, cam_leaves = camera_grad_leaves((rs,))
+        return _RasterizeGaussians.apply(means3D, means2D, shs, opacities, scales, rotations, rs, cam_spec, *cam_leaves)

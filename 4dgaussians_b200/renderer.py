@@ -22,7 +22,8 @@ import torch
 
 from . import _lib
 from .deformation import deform_network, scalar_time
-from .rasterizer import GaussianRasterizationSettings, GaussianRasterizer, _ContextLease, camera_from_settings
+from .rasterizer import (CameraGradSinks, GaussianRasterizationSettings, GaussianRasterizer, _ContextLease, camera_from_settings,
+                         camera_grad_leaves, tensor_meta)
 
 
 def settings_from_camera(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, cam_type=None):
@@ -88,14 +89,16 @@ def _pointers(tensors):
 
 
 class _FusedRender(torch.autograd.Function):
-    """inputs: xyz, scaling, rotation, opacity, features_dc, features_rest, k x means2D, *deform parameters;
+    """inputs: xyz, scaling, rotation, opacity, features_dc, features_rest, k x means2D, *deform parameters, then the
+    camera tensors that take a gradient (cam_spec: their (camera, field) pairs, rasterizer.camera_grad_leaves);
     outputs: k images, k radii, k depth maps"""
 
     @staticmethod
-    def forward(ctx, module: Optional[deform_network], rss, t, xyz, scaling, rotation, opacity, f_dc, f_rest, *rest):
+    def forward(ctx, module: Optional[deform_network], rss, t, cam_spec, xyz, scaling, rotation, opacity, f_dc, f_rest, *rest):
         colors, radii, depths, leases, cstructs, saved = _fused_forward(module, rss, t, any(ctx.needs_input_grad), xyz, scaling,
                                                                         rotation, opacity, f_dc, f_rest)
         ctx.module, ctx.rss, ctx.n, ctx.leases = module, rss, xyz.shape[0], leases
+        ctx.cam_spec, ctx.cam_meta = cam_spec, tensor_meta(rest[len(rest) - len(cam_spec):])
         ctx.lease = leases[0]        # camera 0's context: what a render() caller reads the forward's buffers through
         # the C-ABI structs (and the tensors whose pointers they carry) are kept for the backward: rebuilding them costs the
         # host ~0.3 ms per view, during which the GPU has nothing queued behind the forward's last kernel
@@ -134,7 +137,8 @@ class _FusedRender(torch.autograd.Function):
         gm2 = [flat[(end + 3 * i) * npad:(end + 3 * i) * npad + 3 * n].view(n, 3) for i in range(k)]
         gg = _lib.GaussianGrads(gx.data_ptr(), gs.data_ptr(), gr.data_ptr(), go.data_ptr(), gdc.data_ptr(), grest.data_ptr(),
                                 gm2[0].data_ptr() if k == 1 else None)
-        with torch.cuda.device(dev):
+        sinks = CameraGradSinks(ctx.cam_spec, [lease.ctx for lease in leases], dev)
+        with torch.cuda.device(dev), sinks:
             if k == 1:
                 if gcols[0] is None:        # the single-camera backward takes an image gradient
                     gcols[0] = torch.zeros(3 * int(rss[0].image_height) * int(rss[0].image_width), device=dev)
@@ -149,7 +153,8 @@ class _FusedRender(torch.autograd.Function):
         for lease in leases:
             lease.release()
         ctx.leases = ctx.lease = None
-        return (None, None, None, gx, gs, gr, go, gdc, grest) + tuple(gm2) + tuple(pgrads)
+        cam_grads = sinks.grads(ctx.cam_spec, ctx.cam_meta) if ctx.cam_spec else ()
+        return (None, None, None, None, gx, gs, gr, go, gdc, grest) + tuple(gm2) + tuple(pgrads) + cam_grads
 
 
 def _time_bits(t) -> bytes:
@@ -214,8 +219,9 @@ def _render(viewpoint_cameras, pc, pipe, bg_color, scaling_modifier, override_co
                 lease.release()
         else:
             params = tuple(module.flat_parameters()) if module is not None else ()
-            outs = _FusedRender.apply(module, rss, t, xyz, pc._scaling, pc._rotation, pc._opacity, pc._features_dc,
-                                      pc._features_rest, *points, *params)
+            cam_spec, cam_leaves = camera_grad_leaves(rss)      # camera tensors that require grad: extra inputs
+            outs = _FusedRender.apply(module, rss, t, cam_spec, xyz, pc._scaling, pc._rotation, pc._opacity, pc._features_dc,
+                                      pc._features_rest, *points, *params, *cam_leaves)
             images, radii, depths = outs[:k], outs[k:2 * k], outs[2 * k:]
     else:
         # a foreign (e.g. the reference's own PyTorch) deformation module: keep its semantics, deform once, then rasterize

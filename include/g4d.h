@@ -388,6 +388,19 @@ typedef struct G4DGraphStatus {
     int32_t reserved;
 } G4DGraphStatus;
 int g4d_context_set_time_source(G4DContext *ctx, const float *d_time);
+
+/* ---- camera gradients ----------------------------------------------------------------------------------------------
+ * g4d_context_set_camera_grad: while d_out (device, 35 floats) is set, every backward on ctx (g4d_rasterize_backward,
+ * g4d_render_backward, and g4d_render_backward_cameras for the camera ctx holds) OVERWRITES it with dL/d of this camera:
+ * view[16], proj[16], campos[3], each in the element order of G4DCamera.viewmatrix / projmatrix / campos.  Elements the
+ * forward does not read (view 3, 7, 11, 15; proj 2, 6, 10, 14) are 0, and so is every element of a camera whose image
+ * gradient is NULL.  The derivative is that of the forward as the kernels compute it: a guard-band-clamped t.x / t.y is a
+ * constant, alpha's 0.99 clamp passes the gradient, a clamped colour channel and the depth image pass none.  NULL turns it
+ * off.  A backward on a stream that is capturing returns G4D_ERR_STATE before any launch while the pointer is set.  The
+ * sink is zeroed on the stream after the backward's argument and state checks and before its first kernel: a backward that
+ * returns an error after that point (a CUDA error, a buffer that cannot grow) leaves it zeroed or partly summed, not as it
+ * was. */
+int g4d_context_set_camera_grad(G4DContext *ctx, float *d_out);
 int g4d_workspace_freeze(G4DWorkspace *ws, int on);
 int g4d_workspace_graph_status(G4DWorkspace *ws, int sync, G4DGraphStatus *out);
 
