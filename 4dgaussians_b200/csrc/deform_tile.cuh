@@ -40,6 +40,13 @@ struct DeformDesc {
                                               // or NULL: every Gaussian at the time of the collapsed rows trow
 };
 
+// Hands out consecutive regions of a shared-memory layout in the order they are taken, as offsets in floats, each region
+// rounded up to 4 floats so that every one starts 16-byte aligned (float4 access).  off ends as the layout's total.
+struct SmemFloats {
+    int off = 0;
+    int take(int n) { const int o = off; off += (n + 3) & ~3; return o; }
+};
+
 // shared-memory carve-up (offsets in floats), computed on the host by deform_smem_layout()
 struct DeformSmem {
     int w0t, b0, w1t, b1, bt, w2, b2, a0, a1, a2, out, in, mbar, total_floats;
@@ -49,25 +56,24 @@ struct DeformSmem {
 
 inline DeformSmem deform_smem_layout(int TG, int F, int WD, int head_mask, int ntrunk) {
     DeformSmem s{};
-    int off = 0;
-    auto take = [&](int n) { int o = off; off += (n + 3) & ~3; return o; };
+    SmemFloats m;
     s.lda0 = F + 4; s.lda1 = WD + 4; s.w2_stride = WD + 4;
-    s.w0t = take(F * WD);
-    s.b0 = take(WD);
-    s.w1t = take(WD * WD);
-    s.b1 = take(G4D_NUM_HEADS * WD);
-    s.bt = take(ntrunk * WD);
+    s.w0t = m.take(F * WD);
+    s.b0 = m.take(WD);
+    s.w1t = m.take(WD * WD);
+    s.b1 = m.take(G4D_NUM_HEADS * WD);
+    s.bt = m.take(ntrunk * WD);
     int rows = 0;
     for (int h = 0; h < G4D_NUM_HEADS; ++h) { s.w2_off[h] = rows; if (head_mask & (1 << h)) rows += head_out(h); }
-    s.w2 = take(rows * s.w2_stride);
-    s.b2 = take(64);
-    s.a0 = take(TG * s.lda0);
-    s.a1 = take(TG * s.lda1);
-    s.a2 = take(TG * s.lda1);
-    s.out = take(TG * 60);
-    s.in = take(TG * 12);
-    s.mbar = take(4);
-    s.total_floats = off;
+    s.w2 = m.take(rows * s.w2_stride);
+    s.b2 = m.take(64);
+    s.a0 = m.take(TG * s.lda0);
+    s.a1 = m.take(TG * s.lda1);
+    s.a2 = m.take(TG * s.lda1);
+    s.out = m.take(TG * 60);
+    s.in = m.take(TG * 12);
+    s.mbar = m.take(4);
+    s.total_floats = m.off;
     return s;
 }
 

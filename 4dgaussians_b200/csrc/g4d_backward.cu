@@ -9,6 +9,16 @@
 
 namespace g4d {
 
+// sets the kernel's dynamic shared memory to `smem` bytes, then launches it
+template <class... KArgs, class... Args>
+static cudaError_t launch_smem(void (*kernel)(KArgs...), unsigned grid, unsigned block, size_t smem, cudaStream_t st,
+                               const Args&... args) {
+    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    kernel<<<grid, block, smem, st>>>(args...);
+    return cudaGetLastError();
+}
+
 // Adds the camera terms of the warp's lanes [0, cnt) into acc[kCamGradFloats]: a shuffle tree to lane 0 per element the
 // forward reads, then one atomic per such element.  Called by exactly the lanes [0, cnt) (cnt >= 1).
 G4D_D void cam_grad_flush(const CamGrad& cg, int lane, int cnt, float* __restrict__ acc) {
@@ -87,24 +97,27 @@ preprocess_backward_kernel(const CameraDev* __restrict__ camp, int64_t n, Raster
     g_sh.store_warp<FULL>(g0, cnt, lane, st);
 }
 
+// Launches instance <FULL, CAM> of a per-Gaussian backward kernel, given as its instances <false, false>, <false, true>,
+// <true, false>, <true, true> (FULL: M = 16; CAM: camera gradients wanted), over n Gaussians, one per thread in blocks of
+// 128, with 50 KB of dynamic shared memory: each warp's [2][32 * kShRow] floats of SH staging.
+template <class K, class... Args>
+static cudaError_t launch_per_gaussian_backward(K ff, K ft, K tf, K tt, bool full, bool cam, int64_t n, cudaStream_t st,
+                                                const Args&... args) {
+    if (n == 0) return cudaSuccess;
+    constexpr int kThreads = 128;
+    const size_t smem = (size_t)(kThreads / 32) * 2 * 32 * kShRow * sizeof(float);
+    return launch_smem(full ? (cam ? tt : tf) : (cam ? ft : ff), (unsigned)((n + kThreads - 1) / kThreads), kThreads, smem, st,
+                       args...);
+}
+
 cudaError_t launch_preprocess_backward(const CameraDev* cam, int64_t n, const RasterInputs& in, GeomBuffers g,
                                        const float* g_mean2D, const float* g_conic, const float* g_rgb, float* g_means3D,
                                        float* g_means2D_out, float* g_scales, float* g_rotations, const ShOut& g_sh,
                                        float* g_cam, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    constexpr int kThreads = 128;
-    const size_t smem = (size_t)(kThreads / 32) * 2 * 32 * kShRow * sizeof(float);   // 50 KB: SH staging (see the kernel)
-    const bool full = g_sh.m == kShCoeffs;
-    auto kernel = g_cam ? (full ? preprocess_backward_kernel<true, true> : preprocess_backward_kernel<false, true>)
-                        : (full ? preprocess_backward_kernel<true, false> : preprocess_backward_kernel<false, false>);
-    {
-        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-    }
-    kernel<<<(unsigned)((n + kThreads - 1) / kThreads), kThreads, smem, st>>>(cam, n, in, g, g_mean2D, g_conic, g_rgb,
-                                                                                                  g_means3D, g_means2D_out, g_scales,
-                                                                                                  g_rotations, g_sh, g_cam);
-    return cudaGetLastError();
+    return launch_per_gaussian_backward(preprocess_backward_kernel<false, false>, preprocess_backward_kernel<false, true>,
+                                        preprocess_backward_kernel<true, false>, preprocess_backward_kernel<true, true>,
+                                        g_sh.m == kShCoeffs, g_cam != nullptr, n, st, cam, n, in, g, g_mean2D, g_conic, g_rgb,
+                                        g_means3D, g_means2D_out, g_scales, g_rotations, g_sh, g_cam);
 }
 
 // Per-Gaussian backward of several cameras at one timestamp (g4d_render_backward_cameras): the deformed state and the SH
@@ -180,17 +193,11 @@ preprocess_backward_cameras_kernel(BackwardCameras bc, int64_t n, RasterInputs i
 cudaError_t launch_preprocess_backward_cameras(const BackwardCameras& bc, int64_t n, const RasterInputs& in, float* g_means3D,
                                                float* g_scales, float* g_rotations, float* g_opacities, const ShOut& g_sh,
                                                const CamGradSinks* cs, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    constexpr int kThreads = 128;
-    const size_t smem = (size_t)(kThreads / 32) * 2 * 32 * kShRow * sizeof(float);   // 50 KB: SH staging and sums
-    const bool full = g_sh.m == kShCoeffs;
-    auto kernel = cs ? (full ? preprocess_backward_cameras_kernel<true, true> : preprocess_backward_cameras_kernel<false, true>)
-                     : (full ? preprocess_backward_cameras_kernel<true, false> : preprocess_backward_cameras_kernel<false, false>);
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    kernel<<<(unsigned)((n + kThreads - 1) / kThreads), kThreads, smem, st>>>(
-        bc, n, in, g_means3D, g_scales, g_rotations, g_opacities, g_sh, cs ? *cs : CamGradSinks{});
-    return cudaGetLastError();
+    return launch_per_gaussian_backward(
+        preprocess_backward_cameras_kernel<false, false>, preprocess_backward_cameras_kernel<false, true>,
+        preprocess_backward_cameras_kernel<true, false>, preprocess_backward_cameras_kernel<true, true>,
+        g_sh.m == kShCoeffs, cs != nullptr, n, st, bc, n, in, g_means3D, g_scales, g_rotations, g_opacities, g_sh,
+        cs ? *cs : CamGradSinks{});
 }
 
 // ======================================================================================================
@@ -231,19 +238,18 @@ struct DeformBwdBuffers {
     uint8_t* images;                  // tensor-core: tc_bwd_images_bytes
 };
 
-// the arguments of a backward (the FFMA kernels read the network's; the scatter the planes' and the residual paths')
-struct DeformBwdDesc {
+// Everything one backward's kernels read and write besides their plain arguments, built once by launch_deform_backward: the
+// FFMA kernels read the network's, the scatter the planes' and the residual paths'.
+struct DeformBwdArgs {
     DeformDesc d;
-    const float* w0;                  // torch layout [WD][F]
-    const float* w1[G4D_NUM_HEADS];   // torch layout [WD][WD]
+    G4DDeformGrads g;                     // the caller's gradient sinks (accumulated into)
+    const float* w0;                      // torch layout [WD][F]
+    const float* w1[G4D_NUM_HEADS];       // torch layout [WD][WD]
     const float* wt[G4D_MAX_DEPTH - 1];   // trunk, torch layout [WD][WD]
-    float* g_wt[G4D_MAX_DEPTH - 1]; float* g_bt[G4D_MAX_DEPTH - 1];
-    float* g_w0; float* g_b0;
-    float* g_w1[G4D_NUM_HEADS]; float* g_b1[G4D_NUM_HEADS];
-    float* g_w2[G4D_NUM_HEADS]; float* g_b2[G4D_NUM_HEADS];
-    float* g_planes[G4D_MAX_LEVELS][6];
     const float* go[G4D_NUM_HEADS];   // dL/d(out) per head: xyz[N,3], scaling[N,3], rotation[N,4], opacity[N,1], shs[N,48] (NULL = 0)
     float* gi[G4D_NUM_HEADS];         // dL/d(in), same shapes (NULL = not wanted)
+    float* g_times;                   // [N] dL/d(times) of the per-row mode (OVERWRITTEN), or NULL
+    DeformBwdBuffers buf;
 };
 
 // acc[r][c] += sum_k A[ty*RM + r][k] * Bt[tx + 16*c][k]       (both operands K-contiguous in shared memory)
@@ -271,24 +277,118 @@ G4D_D void tile_gemm_nt(const float* __restrict__ A, int lda, const float* __res
     }
 }
 
+// ---- building blocks of the FFMA engine's H, T and Q ----------------------------------------------------
+// dst[r][0 .. K) = src[r][0 .. K) for the WD rows of a torch-layout [WD][K] matrix, rows padded to ld floats in dst
+template <int WD>
+G4D_D void stage_rows(float* dst, int ld, const float* src, int K) {
+    const int K4 = K >> 2;
+    for (int i = threadIdx.x; i < WD * K4; i += kDeformThreads) {
+        const int r = i / K4, v = i - r * K4;
+        *reinterpret_cast<float4*>(dst + r * ld + 4 * v) = __ldg(reinterpret_cast<const float4*>(src + r * K + 4 * v));
+    }
+}
+
+// The register tile of a [WD][WD] weight gradient dW that thread (ty, tx) accumulates over all its CTA's tiles:
+// acc[a][c * 4 + b] = dW[ty * JR + a][c * 64 + tx * 4 + b], JR = WD / 16, c < WD / 64
+template <int WD> using WGradTile = float[WD / 16][WD / 16];
+
+template <int WD>
+G4D_D void wgrad_zero(WGradTile<WD>& acc) {
+#pragma unroll
+    for (int a = 0; a < WD / 16; ++a)
+#pragma unroll
+        for (int b = 0; b < WD / 16; ++b) acc[a][b] = 0.f;
+}
+
+// dW[o][i] += sum_g dz[g][o] a[g][i] over the TG rows of a tile: dz and a [TG][WD] in shared memory, rows ld floats apart
+template <int TG, int WD>
+G4D_D void wgrad_accumulate(WGradTile<WD>& acc, const float* dz, const float* a, int ld, int ty, int tx) {
+    constexpr int CG = WD / 64, JR = WD / 16;
+    for (int g = 0; g < TG; ++g) {
+        float dzv[JR];
+#pragma unroll
+        for (int j = 0; j < JR; j += 4) {
+            const float4 t4 = *reinterpret_cast<const float4*>(dz + g * ld + ty * JR + j);
+            dzv[j] = t4.x; dzv[j + 1] = t4.y; dzv[j + 2] = t4.z; dzv[j + 3] = t4.w;
+        }
+        float4 av[CG];
+#pragma unroll
+        for (int c = 0; c < CG; ++c) av[c] = *reinterpret_cast<const float4*>(a + g * ld + c * 64 + tx * 4);
+#pragma unroll
+        for (int j = 0; j < JR; ++j)
+#pragma unroll
+            for (int c = 0; c < CG; ++c) {
+                acc[j][c * 4 + 0] = fmaf(dzv[j], av[c].x, acc[j][c * 4 + 0]);
+                acc[j][c * 4 + 1] = fmaf(dzv[j], av[c].y, acc[j][c * 4 + 1]);
+                acc[j][c * 4 + 2] = fmaf(dzv[j], av[c].z, acc[j][c * 4 + 2]);
+                acc[j][c * 4 + 3] = fmaf(dzv[j], av[c].w, acc[j][c * 4 + 3]);
+            }
+    }
+}
+
+// adds the tile into the sink g [WD][WD]: one atomic per element per CTA
+template <int WD>
+G4D_D void wgrad_flush(const WGradTile<WD>& acc, float* const& g, int ty, int tx) {
+    constexpr int CG = WD / 64, JR = WD / 16;
+#pragma unroll
+    for (int a = 0; a < JR; ++a)
+#pragma unroll
+        for (int c = 0; c < CG; ++c)
+#pragma unroll
+            for (int b = 0; b < 4; ++b) atomicAdd(g + (ty * JR + a) * WD + c * 64 + tx * 4 + b, acc[a][c * 4 + b]);
+}
+
+// out[base + g][0 .. WD) = (dz W)[g] for the tile's rows g < rem: dz [TG][WD] (rows ldz floats apart) and W [WD][WD] (torch
+// layout, rows ldw floats apart) in shared memory.  (out, a float pointer, by reference: the kernel argument is read where it is
+// stored to, not held in registers across the GEMM.)
+template <int TG, int WD, class P>
+G4D_D void store_dz_w(const float* dz, int ldz, const float* W, int ldw, const P& out,
+                      int64_t base, int64_t rem, int ty, int tx) {
+    constexpr int RM = TG / 16, CG = WD / 64;
+    float acc[RM][CG * 4];
+#pragma unroll
+    for (int r = 0; r < RM; ++r)
+#pragma unroll
+        for (int c = 0; c < CG * 4; ++c) acc[r][c] = 0.f;
+    tile_gemm<RM, CG>(dz, ldz, W, ldw, WD, ty, tx, acc);
+#pragma unroll
+    for (int c = 0; c < CG; ++c)
+#pragma unroll
+        for (int r = 0; r < RM; ++r) {
+            const int g = ty * RM + r;
+            if (g < rem)
+                *reinterpret_cast<float4*>(out + (base + g) * WD + c * 64 + tx * 4) =
+                    make_float4(acc[r][c * 4 + 0], acc[r][c * 4 + 1], acc[r][c * 4 + 2], acc[r][c * 4 + 3]);
+        }
+}
+
+// sum over the TG rows of a tile of column col: a bias gradient's share of the tile
+template <int TG>
+G4D_D float column_sum(const float* t, int ld, int col) {
+    float s = 0.f;
+    for (int g = 0; g < TG; ++g) s += t[g * ld + col];
+    return s;
+}
+
 // ---- kernel P ------------------------------------------------------------------------------------------
-inline DeformSmem prepass_smem_layout(int TG, int K, int WD) {
-    DeformSmem s{};
-    int off = 0;
-    auto take = [&](int n) { int o = off; off += (n + 3) & ~3; return o; };
-    s.lda0 = K + 4;
-    s.w0t = take(K * WD);
-    s.b0 = take(WD);
-    s.a0 = take(TG * s.lda0);
-    s.total_floats = off;
+struct PrepassSmem { int wt, bias, in, total_floats, ldin; };
+
+inline PrepassSmem prepass_smem_layout(int TG, int K, int WD) {
+    PrepassSmem s{};
+    SmemFloats m;
+    s.ldin = K + 4;
+    s.wt = m.take(K * WD);
+    s.bias = m.take(WD);
+    s.in = m.take(TG * s.ldin);
+    s.total_floats = m.off;
     return s;
 }
 
 // out = relu(in wt + bias) for one layer: in [N][K] (the features, K = F; or a trunk layer's input a_{j-1}, K = WD), wt the
-// packed transpose [K][WD], staged at L.w0t, the bias at L.b0, the input tile at L.a0 (prepass_smem_layout).
+// packed transpose [K][WD], staged at L.wt, the bias at L.bias, the input tile at L.in (prepass_smem_layout).
 template <int TG, int WD>
 __global__ void __launch_bounds__(kDeformThreads, 1)
-deform_bwd_prepass_kernel(DeformSmem L, int64_t n, int K, const float* __restrict__ in, const float* __restrict__ wt,
+deform_bwd_prepass_kernel(PrepassSmem L, int64_t n, int K, const float* __restrict__ in, const float* __restrict__ wt,
                           const float* __restrict__ bias, float* __restrict__ a1_out) {
     extern __shared__ __align__(16) float smem[];
     constexpr int RM = TG / 16, CG = WD / 64;
@@ -296,21 +396,21 @@ deform_bwd_prepass_kernel(DeformSmem L, int64_t n, int K, const float* __restric
     const int64_t ntiles = (n + TG - 1) / TG;
     const int n0 = K * WD;
     for (int i = tid * 4; i < n0; i += kDeformThreads * 4)
-        *reinterpret_cast<float4*>(smem + L.w0t + i) = __ldg(reinterpret_cast<const float4*>(wt + i));
-    for (int i = tid; i < WD; i += kDeformThreads) smem[L.b0 + i] = __ldg(bias + i);
+        *reinterpret_cast<float4*>(smem + L.wt + i) = __ldg(reinterpret_cast<const float4*>(wt + i));
+    for (int i = tid; i < WD; i += kDeformThreads) smem[L.bias + i] = __ldg(bias + i);
     for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const int64_t base = tile * TG, rem = n - base;
-        load_feature_tile<TG>(in, K, base, rem, smem + L.a0, L.lda0);
+        load_feature_tile<TG>(in, K, base, rem, smem + L.in, L.ldin);
         __syncthreads();
         float acc[RM][CG * 4];
 #pragma unroll
         for (int r = 0; r < RM; ++r)
 #pragma unroll
             for (int c = 0; c < CG * 4; ++c) acc[r][c] = 0.f;
-        tile_gemm<RM, CG>(smem + L.a0, L.lda0, smem + L.w0t, WD, K, ty, tx, acc);
+        tile_gemm<RM, CG>(smem + L.in, L.ldin, smem + L.wt, WD, K, ty, tx, acc);
 #pragma unroll
         for (int c = 0; c < CG; ++c) {
-            const float4 bv = *reinterpret_cast<const float4*>(smem + L.b0 + c * 64 + tx * 4);
+            const float4 bv = *reinterpret_cast<const float4*>(smem + L.bias + c * 64 + tx * 4);
 #pragma unroll
             for (int r = 0; r < RM; ++r) {
                 const int g = ty * RM + r;
@@ -330,32 +430,31 @@ struct HeadSmem { int w1, w2, b1, a1, a2, dz, dout, total_floats, ldw, lda, ldo;
 
 inline HeadSmem head_smem_layout(int TG, int WD) {
     HeadSmem s{};
-    int off = 0;
-    auto take = [&](int n) { int o = off; off += (n + 3) & ~3; return o; };
+    SmemFloats m;
     s.ldw = WD + 4; s.lda = WD + 4; s.ldo = 48;
-    s.w1 = take(WD * s.ldw);
-    s.w2 = take(48 * s.ldw);
-    s.b1 = take(WD);
-    s.a1 = take(TG * s.lda);
-    s.a2 = take(TG * s.lda);
-    s.dz = take(TG * s.lda);
-    s.dout = take(TG * s.ldo);
-    s.total_floats = off;
+    s.w1 = m.take(WD * s.ldw);
+    s.w2 = m.take(48 * s.ldw);
+    s.b1 = m.take(WD);
+    s.a1 = m.take(TG * s.lda);
+    s.a2 = m.take(TG * s.lda);
+    s.dz = m.take(TG * s.lda);
+    s.dout = m.take(TG * s.ldo);
+    s.total_floats = m.off;
     return s;
 }
 
 template <int TG, int WD>
 __global__ void __launch_bounds__(kDeformThreads, 1)
-deform_bwd_heads_kernel(DeformBwdDesc bd, HeadSmem L, int64_t n, int num_active, DeformBwdBuffers buf) {
+deform_bwd_heads_kernel(DeformBwdArgs ba, HeadSmem L, int64_t n, int num_active) {
     extern __shared__ __align__(16) float smem[];
-    constexpr int RM = TG / 16, CG = WD / 64, CN = WD / 16, JR = WD / 16;
+    constexpr int RM = TG / 16, CG = WD / 64, CN = WD / 16;
     constexpr int NG = kDeformThreads / WD;           // thread groups for the dW2 mapping (2 or 4)
     constexpr int MAXO = 48 / NG;                     // dW2 accumulators per thread (24 or 12)
     const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
     // which head does this CTA own?
     int slot = blockIdx.x % num_active, h = -1;
     for (int hh = 0, s = 0; hh < G4D_NUM_HEADS; ++hh)
-        if (bd.d.head_mask & (1 << hh)) { if (s == slot) h = hh; ++s; }
+        if (ba.d.head_mask & (1 << hh)) { if (s == slot) h = hh; ++s; }
     const int cta_in_head = blockIdx.x / num_active;
     const int ctas_for_head = (gridDim.x - slot + num_active - 1) / num_active;
     const int kout = head_out(h), kp = (kout + 3) & ~3;
@@ -363,29 +462,23 @@ deform_bwd_heads_kernel(DeformBwdDesc bd, HeadSmem L, int64_t n, int num_active,
     float* sW1 = smem + L.w1; float* sW2 = smem + L.w2; float* sB1 = smem + L.b1;
     float* sA1 = smem + L.a1; float* sA2 = smem + L.a2; float* sDZ = smem + L.dz; float* sDO = smem + L.dout;
     // persistent weights: W1 [j][i] and W2 [o][j] in torch layout, rows padded to ldw
-    for (int i = tid; i < WD * (WD >> 2); i += kDeformThreads) {
-        const int r = i / (WD >> 2), v = i - r * (WD >> 2);
-        *reinterpret_cast<float4*>(sW1 + r * L.ldw + 4 * v) = __ldg(reinterpret_cast<const float4*>(bd.w1[h] + r * WD + 4 * v));
-    }
+    stage_rows<WD>(sW1, L.ldw, ba.w1[h], WD);
     for (int i = tid; i < 48 * (WD >> 2); i += kDeformThreads) {
         const int r = i / (WD >> 2), v = i - r * (WD >> 2);
         float4 val = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (r < kout) val = __ldg(reinterpret_cast<const float4*>(bd.d.w2[h] + r * WD + 4 * v));
+        if (r < kout) val = __ldg(reinterpret_cast<const float4*>(ba.d.w2[h] + r * WD + 4 * v));
         *reinterpret_cast<float4*>(sW2 + r * L.ldw + 4 * v) = val;
     }
-    for (int i = tid; i < WD; i += kDeformThreads) sB1[i] = __ldg(bd.d.b1[h] + i);
+    for (int i = tid; i < WD; i += kDeformThreads) sB1[i] = __ldg(ba.d.b1[h] + i);
     // register accumulators that live across all tiles of this CTA
-    float gW1[JR][CG * 4];
-#pragma unroll
-    for (int a = 0; a < JR; ++a)
-#pragma unroll
-        for (int b = 0; b < CG * 4; ++b) gW1[a][b] = 0.f;
+    WGradTile<WD> gW1;
+    wgrad_zero<WD>(gW1);
     float gW2[MAXO];
 #pragma unroll
     for (int a = 0; a < MAXO; ++a) gW2[a] = 0.f;
     float gB1 = 0.f, gB2 = 0.f;
     const int w2_j = tid % WD, w2_g = tid / WD;
-    const float* go = bd.go[h];
+    const float* go = ba.go[h];
     const int go_stride = kout;   // [N][kout] contiguous for every head (shs: 48)
     __syncthreads();
 
@@ -394,7 +487,7 @@ deform_bwd_heads_kernel(DeformBwdDesc bd, HeadSmem L, int64_t n, int num_active,
         for (int i = tid; i < TG * (WD >> 2); i += kDeformThreads) {
             const int g = i / (WD >> 2), v = i - g * (WD >> 2);
             float4 val = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (g < rem) val = *reinterpret_cast<const float4*>(buf.a1 + (base + g) * WD + 4 * v);
+            if (g < rem) val = *reinterpret_cast<const float4*>(ba.buf.a1 + (base + g) * WD + 4 * v);
             *reinterpret_cast<float4*>(sA1 + g * L.lda + 4 * v) = val;
         }
         for (int i = tid; i < TG * kp; i += kDeformThreads) {
@@ -443,70 +536,22 @@ deform_bwd_heads_kernel(DeformBwdDesc bd, HeadSmem L, int64_t n, int num_active,
                 if (o < kp) gW2[m] = fmaf(sDO[g * L.ldo + o], a2, gW2[m]);
             }
         }
-        if (tid < WD) {
-            float s = 0.f;
-            for (int g = 0; g < TG; ++g) s += sDZ[g * L.lda + tid];
-            gB1 += s;
-        } else if (tid - WD < kout && tid >= WD) {
-            float s = 0.f;
-            for (int g = 0; g < TG; ++g) s += sDO[g * L.ldo + (tid - WD)];
-            gB2 += s;
-        }
-        {   // dW1[j][i] += sum_g dz[g][j] a1[g][i];  thread (ty, tx): j = ty*JR + a, i = c*64 + tx*4 + b
-            for (int g = 0; g < TG; ++g) {
-                float dzv[JR];
-#pragma unroll
-                for (int a = 0; a < JR; a += 4) {
-                    const float4 t4 = *reinterpret_cast<const float4*>(sDZ + g * L.lda + ty * JR + a);
-                    dzv[a] = t4.x; dzv[a + 1] = t4.y; dzv[a + 2] = t4.z; dzv[a + 3] = t4.w;
-                }
-                float4 av[CG];
-#pragma unroll
-                for (int c = 0; c < CG; ++c) av[c] = *reinterpret_cast<const float4*>(sA1 + g * L.lda + c * 64 + tx * 4);
-#pragma unroll
-                for (int a = 0; a < JR; ++a)
-#pragma unroll
-                    for (int c = 0; c < CG; ++c) {
-                        gW1[a][c * 4 + 0] = fmaf(dzv[a], av[c].x, gW1[a][c * 4 + 0]);
-                        gW1[a][c * 4 + 1] = fmaf(dzv[a], av[c].y, gW1[a][c * 4 + 1]);
-                        gW1[a][c * 4 + 2] = fmaf(dzv[a], av[c].z, gW1[a][c * 4 + 2]);
-                        gW1[a][c * 4 + 3] = fmaf(dzv[a], av[c].w, gW1[a][c * 4 + 3]);
-                    }
-            }
-        }
-        {   // da1_h = dz W1  -> HBM
-            float acc[RM][CG * 4];
-#pragma unroll
-            for (int r = 0; r < RM; ++r)
-#pragma unroll
-                for (int c = 0; c < CG * 4; ++c) acc[r][c] = 0.f;
-            tile_gemm<RM, CG>(sDZ, L.lda, sW1, L.ldw, WD, ty, tx, acc);
-#pragma unroll
-            for (int c = 0; c < CG; ++c)
-#pragma unroll
-                for (int r = 0; r < RM; ++r) {
-                    const int g = ty * RM + r;
-                    if (g < rem)
-                        *reinterpret_cast<float4*>(buf.da1[h] + (base + g) * WD + c * 64 + tx * 4) =
-                            make_float4(acc[r][c * 4 + 0], acc[r][c * 4 + 1], acc[r][c * 4 + 2], acc[r][c * 4 + 3]);
-                }
-        }
+        if (tid < WD) gB1 += column_sum<TG>(sDZ, L.lda, tid);
+        else if (tid - WD < kout && tid >= WD) gB2 += column_sum<TG>(sDO, L.ldo, tid - WD);
+        // dW1[j][i] += sum_g dz[g][j] a1[g][i]
+        wgrad_accumulate<TG, WD>(gW1, sDZ, sA1, L.lda, ty, tx);
+        store_dz_w<TG, WD>(sDZ, L.lda, sW1, L.ldw, ba.buf.da1[h], base, rem, ty, tx);   // da1_h = dz W1 -> HBM
         __syncthreads();
     }
     // flush the register accumulators (one atomic per element per CTA)
-#pragma unroll
-    for (int a = 0; a < JR; ++a)
-#pragma unroll
-        for (int c = 0; c < CG; ++c)
-#pragma unroll
-            for (int b = 0; b < 4; ++b) atomicAdd(bd.g_w1[h] + (ty * JR + a) * WD + c * 64 + tx * 4 + b, gW1[a][c * 4 + b]);
+    wgrad_flush<WD>(gW1, ba.g.w1[h], ty, tx);
 #pragma unroll
     for (int m = 0; m < MAXO; ++m) {
         const int o = w2_g + NG * m;
-        if (o < kout) atomicAdd(bd.g_w2[h] + o * WD + w2_j, gW2[m]);
+        if (o < kout) atomicAdd(ba.g.w2[h] + o * WD + w2_j, gW2[m]);
     }
-    if (tid < WD) atomicAdd(bd.g_b1[h] + tid, gB1);
-    else if (tid - WD < kout) atomicAdd(bd.g_b2[h] + (tid - WD), gB2);
+    if (tid < WD) atomicAdd(ba.g.b1[h] + tid, gB1);
+    else if (tid - WD < kout) atomicAdd(ba.g.b2[h] + (tid - WD), gB2);
 }
 
 // dst[g][0 .. WD) = dA[g] * (act[g] > 0) for the tile's rows g < rem, zero for the rows past n; dA is in [N][WD], or, when
@@ -542,34 +587,25 @@ struct TrunkSmem { int w, a, dz, total_floats, ldw, lda; };
 
 inline TrunkSmem trunk_smem_layout(int TG, int WD) {
     TrunkSmem s{};
-    int off = 0;
-    auto take = [&](int n) { int o = off; off += (n + 3) & ~3; return o; };
+    SmemFloats m;
     s.ldw = WD + 4; s.lda = WD + 4;
-    s.w = take(WD * s.ldw);
-    s.a = take(TG * s.lda);
-    s.dz = take(TG * s.lda);
-    s.total_floats = off;
+    s.w = m.take(WD * s.ldw);
+    s.a = m.take(TG * s.lda);
+    s.dz = m.take(TG * s.lda);
+    s.total_floats = m.off;
     return s;
 }
 
 template <int TG, int WD>
 __global__ void __launch_bounds__(kDeformThreads, 1)
-deform_bwd_trunk_kernel(DeformBwdDesc bd, TrunkSmem L, int64_t n, int j, DeformBwdBuffers buf, const float* __restrict__ din,
-                        float* __restrict__ dout) {
+deform_bwd_trunk_kernel(DeformBwdArgs ba, TrunkSmem L, int64_t n, int j, const float* __restrict__ din, float* __restrict__ dout) {
     extern __shared__ __align__(16) float smem[];
-    constexpr int RM = TG / 16, CG = WD / 64, JR = WD / 16;
     const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
     float* sW = smem + L.w; float* sA = smem + L.a; float* sDZ = smem + L.dz;
-    const float* act_in = buf.act[j - 1];
-    for (int i = tid; i < WD * (WD >> 2); i += kDeformThreads) {   // W_j [o][i] in torch layout, rows padded to ldw
-        const int r = i / (WD >> 2), v = i - r * (WD >> 2);
-        *reinterpret_cast<float4*>(sW + r * L.ldw + 4 * v) = __ldg(reinterpret_cast<const float4*>(bd.wt[j - 1] + r * WD + 4 * v));
-    }
-    float gW[JR][CG * 4];
-#pragma unroll
-    for (int a = 0; a < JR; ++a)
-#pragma unroll
-        for (int b = 0; b < CG * 4; ++b) gW[a][b] = 0.f;
+    const float* act_in = ba.buf.act[j - 1];
+    stage_rows<WD>(sW, L.ldw, ba.wt[j - 1], WD);   // W_j [o][i] in torch layout, rows padded to ldw
+    WGradTile<WD> gW;
+    wgrad_zero<WD>(gW);
     float gB = 0.f;
     const int64_t ntiles = (n + TG - 1) / TG;
     __syncthreads();
@@ -577,60 +613,16 @@ deform_bwd_trunk_kernel(DeformBwdDesc bd, TrunkSmem L, int64_t n, int j, DeformB
     for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const int64_t base = tile * TG, rem = n - base;
         load_feature_tile<TG>(act_in, WD, base, rem, sA, L.lda);
-        load_masked_grad<TG, WD>(bd.d, buf, din, buf.act[j], base, rem, sDZ, L.lda);
+        load_masked_grad<TG, WD>(ba.d, ba.buf, din, ba.buf.act[j], base, rem, sDZ, L.lda);
         __syncthreads();
-        if (tid < WD) {
-            float s = 0.f;
-            for (int g = 0; g < TG; ++g) s += sDZ[g * L.lda + tid];
-            gB += s;
-        }
-        // dW_j[o][i] += sum_g dz[g][o] a_{j-1}[g][i];  thread (ty, tx): o = ty*JR + a, i = c*64 + tx*4 + b
-        for (int g = 0; g < TG; ++g) {
-            float dzv[JR];
-#pragma unroll
-            for (int a = 0; a < JR; a += 4) {
-                const float4 t4 = *reinterpret_cast<const float4*>(sDZ + g * L.lda + ty * JR + a);
-                dzv[a] = t4.x; dzv[a + 1] = t4.y; dzv[a + 2] = t4.z; dzv[a + 3] = t4.w;
-            }
-            float4 av[CG];
-#pragma unroll
-            for (int c = 0; c < CG; ++c) av[c] = *reinterpret_cast<const float4*>(sA + g * L.lda + c * 64 + tx * 4);
-#pragma unroll
-            for (int a = 0; a < JR; ++a)
-#pragma unroll
-                for (int c = 0; c < CG; ++c) {
-                    gW[a][c * 4 + 0] = fmaf(dzv[a], av[c].x, gW[a][c * 4 + 0]);
-                    gW[a][c * 4 + 1] = fmaf(dzv[a], av[c].y, gW[a][c * 4 + 1]);
-                    gW[a][c * 4 + 2] = fmaf(dzv[a], av[c].z, gW[a][c * 4 + 2]);
-                    gW[a][c * 4 + 3] = fmaf(dzv[a], av[c].w, gW[a][c * 4 + 3]);
-                }
-        }
-        {   // dA_{j-1} = dz W_j -> HBM
-            float acc[RM][CG * 4];
-#pragma unroll
-            for (int r = 0; r < RM; ++r)
-#pragma unroll
-                for (int c = 0; c < CG * 4; ++c) acc[r][c] = 0.f;
-            tile_gemm<RM, CG>(sDZ, L.lda, sW, L.ldw, WD, ty, tx, acc);
-#pragma unroll
-            for (int c = 0; c < CG; ++c)
-#pragma unroll
-                for (int r = 0; r < RM; ++r) {
-                    const int g = ty * RM + r;
-                    if (g < rem)
-                        *reinterpret_cast<float4*>(dout + (base + g) * WD + c * 64 + tx * 4) =
-                            make_float4(acc[r][c * 4 + 0], acc[r][c * 4 + 1], acc[r][c * 4 + 2], acc[r][c * 4 + 3]);
-                }
-        }
+        if (tid < WD) gB += column_sum<TG>(sDZ, L.lda, tid);
+        // dW_j[o][i] += sum_g dz[g][o] a_{j-1}[g][i]
+        wgrad_accumulate<TG, WD>(gW, sDZ, sA, L.lda, ty, tx);
+        store_dz_w<TG, WD>(sDZ, L.lda, sW, L.ldw, dout, base, rem, ty, tx);   // dA_{j-1} = dz W_j -> HBM
         __syncthreads();
     }
-#pragma unroll
-    for (int a = 0; a < JR; ++a)
-#pragma unroll
-        for (int c = 0; c < CG; ++c)
-#pragma unroll
-            for (int b = 0; b < 4; ++b) atomicAdd(bd.g_wt[j - 1] + (ty * JR + a) * WD + c * 64 + tx * 4 + b, gW[a][c * 4 + b]);
-    if (tid < WD) atomicAdd(bd.g_bt[j - 1] + tid, gB);
+    wgrad_flush<WD>(gW, ba.g.wt[j - 1], ty, tx);
+    if (tid < WD) atomicAdd(ba.g.bt[j - 1] + tid, gB);
 }
 
 // ---- kernel Q ------------------------------------------------------------------------------------------
@@ -638,31 +630,28 @@ struct FinalSmem { int w0, feat, dh, total_floats, ldw0, ldf, ldh; };
 
 inline FinalSmem final_smem_layout(int TG, int F, int WD) {
     FinalSmem s{};
-    int off = 0;
-    auto take = [&](int n) { int o = off; off += (n + 3) & ~3; return o; };
+    SmemFloats m;
     s.ldw0 = F + 4; s.ldf = F + 4; s.ldh = WD + 4;
-    s.w0 = take(WD * s.ldw0);
-    s.feat = take(TG * s.ldf);
-    s.dh = take(TG * s.ldh);
-    s.total_floats = off;
+    s.w0 = m.take(WD * s.ldw0);
+    s.feat = m.take(TG * s.ldf);
+    s.dh = m.take(TG * s.ldh);
+    s.total_floats = m.off;
     return s;
 }
 
 // din: dA_0 from the last T launch, or NULL (no trunk): the heads' DA1 sum
 template <int TG, int WD, int FM>
 __global__ void __launch_bounds__(kDeformThreads, 1)
-deform_bwd_final_kernel(DeformBwdDesc bd, FinalSmem L, int64_t n, DeformBwdBuffers buf, const float* __restrict__ din) {
+deform_bwd_final_kernel(DeformBwdArgs ba, FinalSmem L, int64_t n, const float* __restrict__ din) {
     extern __shared__ __align__(16) float smem[];
-    const DeformDesc& d = bd.d;
+    const DeformDesc& d = ba.d;
+    const DeformBwdBuffers& buf = ba.buf;
     const int tid = threadIdx.x;
     const int F = d.F, F4 = F >> 2;
     constexpr int NG = kDeformThreads / WD;
     constexpr int MAXF = FM / NG;                   // dW0 accumulators per thread (F <= FM)
     float* sW0 = smem + L.w0; float* sF = smem + L.feat; float* sDH = smem + L.dh;
-    for (int i = tid; i < WD * F4; i += kDeformThreads) {
-        const int r = i / F4, v = i - r * F4;
-        *reinterpret_cast<float4*>(sW0 + r * L.ldw0 + 4 * v) = __ldg(reinterpret_cast<const float4*>(bd.w0 + r * F + 4 * v));
-    }
+    stage_rows<WD>(sW0, L.ldw0, ba.w0, F);
     float gW0[MAXF];
 #pragma unroll
     for (int m = 0; m < MAXF; ++m) gW0[m] = 0.f;
@@ -685,11 +674,7 @@ deform_bwd_final_kernel(DeformBwdDesc bd, FinalSmem L, int64_t n, DeformBwdBuffe
                 if (f < F) gW0[m] = fmaf(dh, sF[g * L.ldf + f], gW0[m]);
             }
         }
-        if (tid < WD) {
-            float s = 0.f;
-            for (int g = 0; g < TG; ++g) s += sDH[g * L.ldh + tid];
-            gB0 += s;
-        }
+        if (tid < WD) gB0 += column_sum<TG>(sDH, L.ldh, tid);
         // dfeat[g][f..f+3] = sum_j dh[g][j] W0[j][f..f+3]  -> DFEAT (the scatter's input)
         for (int i = tid; i < TG * F4; i += kDeformThreads) {
             const int g = i / F4, v = i - g * F4;
@@ -707,9 +692,9 @@ deform_bwd_final_kernel(DeformBwdDesc bd, FinalSmem L, int64_t n, DeformBwdBuffe
 #pragma unroll
     for (int m = 0; m < MAXF; ++m) {
         const int f = w0_g + NG * m;
-        if (f < F) atomicAdd(bd.g_w0 + w0_j * F + f, gW0[m]);
+        if (f < F) atomicAdd(ba.g.w0 + w0_j * F + f, gW0[m]);
     }
-    if (tid < WD) atomicAdd(bd.g_b0 + tid, gB0);
+    if (tid < WD) atomicAdd(ba.g.b0 + tid, gB0);
 }
 
 // ---- HexPlane scatter of every backward at full occupancy: LPG lanes per Gaussian, lane v < C/4 scatters channel vector v --
@@ -717,20 +702,10 @@ deform_bwd_final_kernel(DeformBwdDesc bd, FinalSmem L, int64_t n, DeformBwdBuffe
 // nothing.
 constexpr int scatter_lanes(int C4) { return C4 <= 1 ? 1 : C4 <= 2 ? 2 : C4 <= 4 ? 4 : 8; }
 
-struct BwdScatterDesc {
-    DeformDesc d;
-    const float* dfeat;                     // [N][F]
-    float* g_planes[G4D_MAX_LEVELS][6];
-    float* trow_grad[G4D_MAX_LEVELS][3];
-    const float* go[G4D_NUM_HEADS];
-    float* gi[G4D_NUM_HEADS];
-    float* g_times;                         // [N] dL/d(times) of the per-row mode (OVERWRITTEN), or NULL
-};
-
 // PER_ROW: Gaussian g at its own time d.times[g]; the time planes' gradients go straight to the planes and dL/dt to g_times
 template <int C4, bool PER_ROW>
-__global__ void __launch_bounds__(256, 2) bwd_scatter_kernel(BwdScatterDesc sd, int64_t n, const float* __restrict__ xyz) {
-    const DeformDesc& d = sd.d;
+__global__ void __launch_bounds__(256, 2) bwd_scatter_kernel(DeformBwdArgs ba, int64_t n, const float* __restrict__ xyz) {
+    const DeformDesc& d = ba.d;
     constexpr int LPG = scatter_lanes(C4);
     constexpr int GPB = 256 / LPG;          // Gaussians per block
     const int64_t g0 = (int64_t)blockIdx.x * GPB;
@@ -738,10 +713,10 @@ __global__ void __launch_bounds__(256, 2) bwd_scatter_kernel(BwdScatterDesc sd, 
     const int v = threadIdx.x % LPG;
     // residual path: d(out)/d(in) = identity for scaling / rotation / opacity / shs (contiguous ranges, coalesced)
     for (int hh = 1; hh < G4D_NUM_HEADS; ++hh) {
-        if (!sd.gi[hh]) continue;
+        if (!ba.gi[hh]) continue;
         const int ko = head_out(hh);
         const int64_t lo = g0 * ko, hi = (g0 + GPB < n ? g0 + GPB : n) * ko;
-        for (int64_t i = lo + threadIdx.x; i < hi; i += 256) sd.gi[hh][i] = sd.go[hh] ? sd.go[hh][i] : 0.f;
+        for (int64_t i = lo + threadIdx.x; i < hi; i += 256) ba.gi[hh][i] = ba.go[hh] ? ba.go[hh][i] : 0.f;
     }
     float gpix[3] = {0.f, 0.f, 0.f};
     float gt = 0.f;   // dL/d(times[g]) (PER_ROW): t enters the time planes unnormalised, so d(t_pix)/dt is the tap's gmul
@@ -756,8 +731,8 @@ __global__ void __launch_bounds__(256, 2) bwd_scatter_kernel(BwdScatterDesc sd, 
 #pragma unroll
             for (int a = 0; a < 3; ++a) tx[a] = make_tap(pcs[a], d.res[l][a]);
             if (PER_ROW) tx[PER_ROW ? 3 : 0] = make_tap(tg, d.res[l][3]);
-            const float4 df = __ldg(reinterpret_cast<const float4*>(sd.dfeat + g * d.F + l * d.C + 4 * v));
-            scatter_vector<PER_ROW>(d.planes[l], d.trow[l], d.res[l], sd.g_planes[l], sd.trow_grad[l], tx, v, C4, df, gpix, gt);
+            const float4 df = __ldg(reinterpret_cast<const float4*>(ba.buf.dfeat + g * d.F + l * d.C + 4 * v));
+            scatter_vector<PER_ROW>(d.planes[l], d.trow[l], d.res[l], ba.g.planes[l], ba.buf.trow_grad[l], tx, v, C4, df, gpix, gt);
         }
     }
     // the LPG lanes of a Gaussian are adjacent
@@ -766,21 +741,21 @@ __global__ void __launch_bounds__(256, 2) bwd_scatter_kernel(BwdScatterDesc sd, 
         for (int o = 1; o < LPG; o <<= 1) gpix[a] += __shfl_xor_sync(0xffffffffu, gpix[a], o);
     if (PER_ROW)
         for (int o = 1; o < LPG; o <<= 1) gt += __shfl_xor_sync(0xffffffffu, gt, o);
-    if (g < n && v == 0 && sd.gi[0]) {
+    if (g < n && v == 0 && ba.gi[0]) {
 #pragma unroll
-        for (int a = 0; a < 3; ++a) sd.gi[0][g * 3 + a] = (sd.go[0] ? sd.go[0][g * 3 + a] : 0.f) + gpix[a] * nrm.scale[a];
+        for (int a = 0; a < 3; ++a) ba.gi[0][g * 3 + a] = (ba.go[0] ? ba.go[0][g * 3 + a] : 0.f) + gpix[a] * nrm.scale[a];
     }
-    if (PER_ROW && g < n && v == 0 && sd.g_times) sd.g_times[g] = gt;
+    if (PER_ROW && g < n && v == 0 && ba.g_times) ba.g_times[g] = gt;
 }
 
-static cudaError_t launch_bwd_scatter(const BwdScatterDesc& sd, int64_t n, const float* xyz, cudaStream_t st) {
-    const int C4 = sd.d.C / 4;
+static cudaError_t launch_bwd_scatter(const DeformBwdArgs& ba, int64_t n, const float* xyz, cudaStream_t st) {
+    const int C4 = ba.d.C / 4;
     const unsigned grid = (unsigned)((n * scatter_lanes(C4) + 255) / 256);
     switch (C4) {   // every channel width the C-ABI takes: C = 4 .. 32
 #define G4D_SCATTER_CASE(K)                                                     \
         case K:                                                                 \
-            if (sd.d.times) bwd_scatter_kernel<K, true><<<grid, 256, 0, st>>>(sd, n, xyz); \
-            else bwd_scatter_kernel<K, false><<<grid, 256, 0, st>>>(sd, n, xyz);          \
+            if (ba.d.times) bwd_scatter_kernel<K, true><<<grid, 256, 0, st>>>(ba, n, xyz); \
+            else bwd_scatter_kernel<K, false><<<grid, 256, 0, st>>>(ba, n, xyz);          \
             break;
         G4D_SCATTER_CASE(1) G4D_SCATTER_CASE(2) G4D_SCATTER_CASE(3) G4D_SCATTER_CASE(4)
         G4D_SCATTER_CASE(5) G4D_SCATTER_CASE(6) G4D_SCATTER_CASE(7) G4D_SCATTER_CASE(8)
@@ -791,42 +766,27 @@ static cudaError_t launch_bwd_scatter(const BwdScatterDesc& sd, int64_t n, const
 }
 
 // ---- kernel T: collapsed time-row gradients -> the two time rows of each (axis, t) plane --------------------
-struct TimeGradDesc {
-    int levels, C;
-    int res[G4D_MAX_LEVELS][4];
-    const float* row_grad[G4D_MAX_LEVELS][3];
-    float* plane_grad[G4D_MAX_LEVELS][3];
-    int start[G4D_MAX_LEVELS * 3 + 1];
-};
-
-__global__ void distribute_time_grad_kernel(TimeGradDesc d, TimeArg time) {
+// s.src: the rows' gradients; s.dst: the time planes' gradients
+__global__ void distribute_time_grad_kernel(TimeRowSegs s, TimeArg time) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    const int nseg = d.levels * 3;
-    if (i >= d.start[nseg]) return;
-    int m = 0;
-    while (i >= d.start[m + 1]) ++m;
-    const int l = m / 3, a = m % 3, e = i - d.start[m];
-    const Tap1D ty = make_tap(time.get(), d.res[l][3]);
-    const int rowlen = d.res[l][a] * d.C;
-    const float gv = d.row_grad[l][a][e];
-    atomicAdd(d.plane_grad[l][a] + (size_t)ty.i0 * rowlen + e, gv * ty.w0);
-    atomicAdd(d.plane_grad[l][a] + (size_t)ty.i1 * rowlen + e, gv * ty.w1);
+    if (i >= s.start[3 * s.levels]) return;
+    int l, a, e;
+    s.locate(i, l, a, e);
+    const Tap1D ty = make_tap(time.get(), s.res[l][3]);
+    const int rowlen = s.res[l][a] * s.C;
+    const float gv = s.src[l][a][e];
+    atomicAdd(s.dst[l][a] + (size_t)ty.i0 * rowlen + e, gv * ty.w0);
+    atomicAdd(s.dst[l][a] + (size_t)ty.i1 * rowlen + e, gv * ty.w1);
 }
 
 // ---- host side -------------------------------------------------------------------------------------------
-static cudaError_t launch_distribute_time_grad(const DeformDesc& d, float* const (*trow_grad)[3], float* const (*g_planes)[6],
-                                               TimeArg time, cudaStream_t st) {
-    TimeGradDesc t{};
-    t.levels = d.levels; t.C = d.C;
-    const TimeRows tr(d.levels, d.res, d.C);
-    const int tk[3] = {2, 4, 5};
-    for (int l = 0; l < d.levels; ++l) {
-        for (int a = 0; a < 4; ++a) t.res[l][a] = d.res[l][a];
-        for (int a = 0; a < 3; ++a) { t.row_grad[l][a] = trow_grad[l][a]; t.plane_grad[l][a] = g_planes[l][tk[a]]; }
-    }
-    for (int m = 0; m <= 3 * d.levels; ++m) t.start[m] = tr.start[m];
-    const int total = (int)tr.total();
-    distribute_time_grad_kernel<<<(total + 255) / 256, 256, 0, st>>>(t, time);
+static cudaError_t launch_distribute_time_grad(const DeformBwdArgs& ba, TimeArg time, cudaStream_t st) {
+    const DeformDesc& d = ba.d;
+    TimeRowSegs s(d.levels, d.res, d.C);
+    for (int l = 0; l < d.levels; ++l)
+        for (int a = 0; a < 3; ++a) { s.src[l][a] = ba.buf.trow_grad[l][a]; s.dst[l][a] = ba.g.planes[l][kTimePlane[a]]; }
+    const int total = (int)s.total();
+    distribute_time_grad_kernel<<<(total + 255) / 256, 256, 0, st>>>(s, time);
     return cudaGetLastError();
 }
 
@@ -864,63 +824,47 @@ size_t deform_backward_scratch_bytes(const DeformDesc& d, int64_t n, bool tc) {
 
 // FFMA engine: P (once per layer up to a_{D-1}), H, T (once per trunk layer), Q
 template <int TG, int WD>
-static cudaError_t launch_ffma_engine(const DeformBwdDesc& bd, int64_t n, const DeformBwdBuffers& buf, int sm_count, cudaStream_t st) {
-    const DeformDesc& d = bd.d;
+static cudaError_t launch_ffma_engine(const DeformBwdArgs& ba, int64_t n, int sm_count, cudaStream_t st) {
+    const DeformDesc& d = ba.d;
+    const DeformBwdBuffers& buf = ba.buf;
     int active = 0;
     for (int h = 0; h < G4D_NUM_HEADS; ++h) active += (d.head_mask >> h) & 1;
     const int64_t ntiles = (n + TG - 1) / TG;
-    const int grid = (int)(ntiles < sm_count ? ntiles : sm_count);
+    const unsigned grid = (unsigned)(ntiles < sm_count ? ntiles : sm_count);
     cudaError_t e;
     // P
     for (int j = 0; j <= d.ntrunk; ++j) {
         const int K = j == 0 ? d.F : WD;
-        const DeformSmem L = prepass_smem_layout(TG, K, WD);
-        const size_t bytes = (size_t)L.total_floats * 4;
-        e = cudaFuncSetAttribute(deform_bwd_prepass_kernel<TG, WD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+        const PrepassSmem L = prepass_smem_layout(TG, K, WD);
+        e = j == 0 ? launch_smem(deform_bwd_prepass_kernel<TG, WD>, grid, kDeformThreads, (size_t)L.total_floats * 4, st, L, n, K,
+                                 buf.feat, d.w0t, d.b0, buf.act[0])
+                   : launch_smem(deform_bwd_prepass_kernel<TG, WD>, grid, kDeformThreads, (size_t)L.total_floats * 4, st, L, n, K,
+                                 buf.act[j - 1], d.wtt[j - 1], d.bt[j - 1], buf.act[j]);
         if (e != cudaSuccess) return e;
-        if (j == 0) deform_bwd_prepass_kernel<TG, WD><<<grid, kDeformThreads, bytes, st>>>(L, n, K, buf.feat, d.w0t, d.b0, buf.act[0]);
-        else deform_bwd_prepass_kernel<TG, WD><<<grid, kDeformThreads, bytes, st>>>(L, n, K, buf.act[j - 1], d.wtt[j - 1], d.bt[j - 1], buf.act[j]);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
     }
     // H
     if (active > 0) {
         const HeadSmem L = head_smem_layout(TG, WD);
-        const size_t bytes = (size_t)L.total_floats * 4;
-        e = cudaFuncSetAttribute(deform_bwd_heads_kernel<TG, WD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-        if (e != cudaSuccess) return e;
         int hgrid = sm_count;
         if ((int64_t)hgrid > ntiles * active) hgrid = (int)(ntiles * active);
         if (hgrid < active) hgrid = active;
-        deform_bwd_heads_kernel<TG, WD><<<hgrid, kDeformThreads, bytes, st>>>(bd, L, n, active, buf);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+        e = launch_smem(deform_bwd_heads_kernel<TG, WD>, hgrid, kDeformThreads, (size_t)L.total_floats * 4, st, ba, L, n, active);
+        if (e != cudaSuccess) return e;
     }
     // T: dA_{j-1} from dA_j, j = ntrunk .. 1 (dA_ntrunk: the heads' DA1 sum)
     const float* din = nullptr;
-    if (d.ntrunk > 0) {
-        const TrunkSmem L = trunk_smem_layout(TG, WD);
-        const size_t bytes = (size_t)L.total_floats * 4;
-        e = cudaFuncSetAttribute(deform_bwd_trunk_kernel<TG, WD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    const TrunkSmem LT = trunk_smem_layout(TG, WD);
+    for (int j = d.ntrunk, k = 0; j >= 1; --j, k ^= 1) {
+        e = launch_smem(deform_bwd_trunk_kernel<TG, WD>, grid, kDeformThreads, (size_t)LT.total_floats * 4, st, ba, LT, n, j, din,
+                        buf.dact[k]);
         if (e != cudaSuccess) return e;
-        for (int j = d.ntrunk, k = 0; j >= 1; --j, k ^= 1) {
-            deform_bwd_trunk_kernel<TG, WD><<<grid, kDeformThreads, bytes, st>>>(bd, L, n, j, buf, din, buf.dact[k]);
-            if ((e = cudaGetLastError()) != cudaSuccess) return e;
-            din = buf.dact[k];
-        }
+        din = buf.dact[k];
     }
     // Q
     const FinalSmem L = final_smem_layout(TG, d.F, WD);
-    const size_t bytes = (size_t)L.total_floats * 4;
-#define G4D_LAUNCH_Q(FM)                                                                                                  \
-    do {                                                                                                                  \
-        e = cudaFuncSetAttribute(deform_bwd_final_kernel<TG, WD, FM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes); \
-        if (e != cudaSuccess) return e;                                                                                   \
-        deform_bwd_final_kernel<TG, WD, FM><<<grid, kDeformThreads, bytes, st>>>(bd, L, n, buf, din);                    \
-    } while (0)
-    if (d.F <= 32) G4D_LAUNCH_Q(32);
-    else if (d.F <= 64) G4D_LAUNCH_Q(64);
-    else G4D_LAUNCH_Q(128);
-#undef G4D_LAUNCH_Q
-    return cudaGetLastError();
+    auto final_kernel = d.F <= 32 ? deform_bwd_final_kernel<TG, WD, 32>
+                      : d.F <= 64 ? deform_bwd_final_kernel<TG, WD, 64> : deform_bwd_final_kernel<TG, WD, 128>;
+    return launch_smem(final_kernel, grid, kDeformThreads, (size_t)L.total_floats * 4, st, ba, L, n, din);
 }
 
 cudaError_t launch_deform_backward(const DeformDesc& d, const G4DDeformParams& prm, const G4DDeformGrads& grads, const TcBwdWeights* tc,
@@ -931,36 +875,28 @@ cudaError_t launch_deform_backward(const DeformDesc& d, const G4DDeformParams& p
     const TimeRows tr(d.levels, d.res, d.C);
     Carve m(scratch);
     float* gathered;
-    DeformBwdBuffers buf = carve_backward_scratch(m, d, n, tc != nullptr, &gathered);
-    if (saved_feat) buf.feat = saved_feat;   // the features the forward of this view gathered
-    DeformBwdDesc bd{};
-    bd.d = d;
-    bd.w0 = prm.w0; bd.g_w0 = grads.w0; bd.g_b0 = grads.b0;
-    for (int h = 0; h < G4D_NUM_HEADS; ++h) {
-        bd.w1[h] = prm.w1[h]; bd.g_w1[h] = grads.w1[h]; bd.g_b1[h] = grads.b1[h]; bd.g_w2[h] = grads.w2[h]; bd.g_b2[h] = grads.b2[h];
-        bd.go[h] = go[h]; bd.gi[h] = gi[h];
-    }
-    for (int j = 0; j < d.ntrunk; ++j) { bd.wt[j] = prm.wt[j]; bd.g_wt[j] = grads.wt[j]; bd.g_bt[j] = grads.bt[j]; }
-    BwdScatterDesc sc{};
-    sc.d = d; sc.dfeat = buf.dfeat;
-    for (int l = 0; l < d.levels; ++l) {
-        for (int k = 0; k < 6; ++k) bd.g_planes[l][k] = sc.g_planes[l][k] = grads.planes[l][k];
-        for (int a = 0; a < 3; ++a) sc.trow_grad[l][a] = buf.trow_grad[l][a];
-    }
-    for (int h = 0; h < G4D_NUM_HEADS; ++h) { sc.go[h] = go[h]; sc.gi[h] = gi[h]; }
-    sc.g_times = g_times;
+    DeformBwdArgs ba{};
+    ba.d = d;
+    ba.g = grads;
+    ba.w0 = prm.w0;
+    for (int h = 0; h < G4D_NUM_HEADS; ++h) { ba.w1[h] = prm.w1[h]; ba.go[h] = go[h]; ba.gi[h] = gi[h]; }
+    for (int j = 0; j < d.ntrunk; ++j) ba.wt[j] = prm.wt[j];
+    ba.g_times = g_times;
+    ba.buf = carve_backward_scratch(m, d, n, tc != nullptr, &gathered);
+    if (saved_feat) ba.buf.feat = saved_feat;   // the features the forward of this view gathered
+    const DeformBwdBuffers& buf = ba.buf;
     cudaError_t e = d.times ? cudaSuccess : cudaMemsetAsync(buf.trow_grad[0][0], 0, tr.total() * 4, st);
     if (e != cudaSuccess) return e;
     if (!saved_feat && (e = launch_deform_features(d, n, xyz, order, gathered, false, st)) != cudaSuccess) return e;
     // the engine: d(feat) -> DFEAT and the weight gradients (the tensor-core wgrad kernel after the scatter)
     if (tc) e = launch_tc_bwd_dgrad(d, *tc, n, go, relu_bits, buf.feat, buf.dfeat, buf.images, sm_count, st);
-    else if (d.WD == 128) e = launch_ffma_engine<64, 128>(bd, n, buf, sm_count, st);
-    else if (d.WD == 64) e = launch_ffma_engine<128, 64>(bd, n, buf, sm_count, st);
+    else if (d.WD == 128) e = launch_ffma_engine<64, 128>(ba, n, sm_count, st);
+    else if (d.WD == 64) e = launch_ffma_engine<128, 64>(ba, n, sm_count, st);
     else e = cudaErrorInvalidValue;
     if (e != cudaSuccess) return e;
-    if ((e = launch_bwd_scatter(sc, n, xyz, st)) != cudaSuccess) return e;
+    if ((e = launch_bwd_scatter(ba, n, xyz, st)) != cudaSuccess) return e;
     if (tc && (e = launch_tc_bwd_wgrad(d, grads, n, buf.images, sm_count, st)) != cudaSuccess) return e;
-    return d.times ? cudaSuccess : launch_distribute_time_grad(d, buf.trow_grad, bd.g_planes, time, st);
+    return d.times ? cudaSuccess : launch_distribute_time_grad(ba, time, st);
 }
 
 // ------------------------------------------------------------------------------------------------------

@@ -81,44 +81,29 @@ cudaError_t launch_pack_weights(const G4DDeformParams& prm, float* w0t, float* c
 }
 
 // ------------------------------------------------------------------------------------------------------
-struct CollapseDesc {
-    int levels, C;
-    int res[G4D_MAX_LEVELS][4];
-    const float* plane[G4D_MAX_LEVELS][3];   // planes 2,4,5 = (x,t),(y,t),(z,t): [T][res[a]][C]
-    float* row[G4D_MAX_LEVELS][3];           // [res[a]][C]
-    int start[G4D_MAX_LEVELS * 3 + 1];
-};
-
 // Every Gaussian of a view shares t, so the time-axis interpolation of the three time planes is done once:
 // row[x][c] = plane[y0][x][c]*(y1-y) + plane[y1][x][c]*(y-y0)  with t NOT normalised (hexplane.py:164).
-__global__ void collapse_time_rows_kernel(CollapseDesc d, TimeArg time) {
+// s.src: the time planes [T][res[a]][C]; s.dst: the rows [res[a]][C].
+__global__ void collapse_time_rows_kernel(TimeRowSegs s, TimeArg time) {
     pdl_wait();         // the row buffer is reused: the previous view's kernels read it until they complete
     pdl_trigger();
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    const int nseg = d.levels * 3;
-    if (i >= d.start[nseg]) return;
-    int m = 0;
-    while (i >= d.start[m + 1]) ++m;
-    const int l = m / 3, a = m % 3, e = i - d.start[m];
-    const int T = d.res[l][3];
+    if (i >= s.start[3 * s.levels]) return;
+    int l, a, e;
+    s.locate(i, l, a, e);
+    const int T = s.res[l][3];
     const Tap1D ty = make_tap(time.get(), T);   // (after pdl_wait: a source written by the previous kernel is complete)
-    const int rowlen = d.res[l][a] * d.C;
-    const float v0 = __ldg(d.plane[l][a] + (size_t)ty.i0 * rowlen + e), v1 = __ldg(d.plane[l][a] + (size_t)ty.i1 * rowlen + e);
-    d.row[l][a][e] = fmaf(v1, ty.w1, v0 * ty.w0);
+    const int rowlen = s.res[l][a] * s.C;
+    const float v0 = __ldg(s.src[l][a] + (size_t)ty.i0 * rowlen + e), v1 = __ldg(s.src[l][a] + (size_t)ty.i1 * rowlen + e);
+    s.dst[l][a][e] = fmaf(v1, ty.w1, v0 * ty.w0);
 }
 
 cudaError_t launch_collapse_time_rows(const G4DDeformParams& p, TimeArg time, float* const (*trow)[3], cudaStream_t st) {
-    CollapseDesc d{};
-    d.levels = p.levels; d.C = p.channels;
-    const TimeRows tr(p.levels, p.res, p.channels);
-    const int tk[3] = {2, 4, 5};
-    for (int l = 0; l < p.levels; ++l) {
-        for (int a = 0; a < 4; ++a) d.res[l][a] = p.res[l][a];
-        for (int a = 0; a < 3; ++a) { d.plane[l][a] = p.planes[l][tk[a]]; d.row[l][a] = trow[l][a]; }
-    }
-    for (int m = 0; m <= 3 * p.levels; ++m) d.start[m] = tr.start[m];
-    const int total = (int)tr.total();
-    return launch_k(collapse_time_rows_kernel, dim3((total + 255) / 256), dim3(256), 0, st, true, d, time);
+    TimeRowSegs s(p.levels, p.res, p.channels);
+    for (int l = 0; l < p.levels; ++l)
+        for (int a = 0; a < 3; ++a) { s.src[l][a] = p.planes[l][kTimePlane[a]]; s.dst[l][a] = trow[l][a]; }
+    const int total = (int)s.total();
+    return launch_k(collapse_time_rows_kernel, dim3((total + 255) / 256), dim3(256), 0, st, true, s, time);
 }
 
 // ------------------------------------------------------------------------------------------------------

@@ -37,6 +37,29 @@ struct TimeRows {
     }
 };
 
+// the time planes among a level's six, for time axes a = x, y, z: (x,t), (y,t), (z,t)
+constexpr int kTimePlane[3] = {2, 4, 5};
+
+// A kernel with one thread per float of the collapsed time rows: segment (l, a) is element range [start[3l+a], start[3l+a+1])
+// and moves data from src[l][a] to dst[l][a].  The time-row collapse reads the time planes and writes the rows; the
+// backward reads the rows' gradients and adds into the time planes' gradients.  The caller sets src and dst.
+struct TimeRowSegs : TimeRows {
+    int C;
+    int res[G4D_MAX_LEVELS][4];
+    const float* src[G4D_MAX_LEVELS][3];
+    float* dst[G4D_MAX_LEVELS][3];
+    TimeRowSegs(int levels_, const int32_t (*res_)[4], int C_) : TimeRows(levels_, res_, C_), C(C_), res{}, src{}, dst{} {
+        for (int l = 0; l < levels; ++l)
+            for (int a = 0; a < 4; ++a) res[l][a] = res_[l][a];
+    }
+    // element i < total() is element e of segment (level l, time axis a)
+    G4D_D void locate(int i, int& l, int& a, int& e) const {
+        int m = 0;
+        while (i >= start[m + 1]) ++m;
+        l = m / 3; a = m % 3; e = i - start[m];
+    }
+};
+
 // The timestamp of a forward or backward: read from src (device; g4d_context_set_time_source) when it is set, so that a
 // replayed CUDA graph sees the value of the replay, else `value`.
 struct TimeArg {
