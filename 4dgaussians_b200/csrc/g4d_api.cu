@@ -16,7 +16,7 @@ namespace {
 
 thread_local std::string t_last_error;
 
-// What the entry point running on this thread allows (CallScope): while its stream captures a CUDA graph nothing may run that
+// What the entry point running on this thread allows (CallFrame): while its stream captures a CUDA graph nothing may run that
 // a replay could not repeat, and while its workspace is frozen or its stream captures no buffer may be reallocated (a graph
 // keeps the addresses it captured).
 // growth_refused: set by the DevBuf::ensure that refused, so that its caller reports the refusal and not a CUDA error.
@@ -218,25 +218,6 @@ struct StageTimer {
     }
 };
 void reset_stage_flags(G4DContext* c, int first, int last) { for (int i = first; i <= last; ++i) c->ev_used[i] = false; }
-
-// t_call for one entry point on workspace ws and stream st, restored when it returns; rc != G4D_OK when the capture status
-// of st cannot be read
-struct CallScope {
-    CallState saved;
-    int rc = G4D_OK;
-    CallScope(const G4DWorkspace* ws, cudaStream_t st) : saved(t_call) {
-        cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-        const cudaError_t e = cudaStreamIsCapturing(st, &cs);
-        if (e != cudaSuccess) {
-            (void)cudaGetLastError();
-            rc = fail(G4D_ERR_STATE, "cudaStreamIsCapturing", cudaGetErrorString(e));
-        }
-        t_call.capturing = cs != cudaStreamCaptureStatusNone;
-        t_call.no_growth = ws->frozen || t_call.capturing;
-        t_call.growth_refused = false;
-    }
-    ~CallScope() { t_call = saved; }
-};
 
 // What a capture refuses, checked before any launch: host events (stage timing), host syncs (G4D_CAM_DEBUG) and, for a
 // forward on the contexts fwd[0, k), the exact-mode read-back of R and a capacity that has not been learnt yet.
@@ -639,33 +620,78 @@ int zero_camera_grads(G4DContext* const* ctx, int k, cudaStream_t st) {
     return G4D_OK;
 }
 
+// The frame of an entry point, built behind its argument checks and before its first launch: it makes ws's device current
+// and sets t_call for the stream st (restored when the entry point returns; kRead synchronises the device instead).  Then,
+// on the contexts ctx[0, k) and their cameras cams[0, k): a forward or backward refuses what a capture cannot repeat, every
+// kind but kContextFree resolves the pending read-backs, a forward clears each context's record once its read-backs are
+// resolved and a backward zeroes the camera-gradient sinks.  rc != G4D_OK: the entry point returns it.
+struct CallFrame {
+    enum Kind { kContextFree, kRead, kForward, kBackward };
+    CallState saved;
+    int rc;
+    CallFrame(Kind kind, const G4DWorkspace* ws, cudaStream_t st, G4DContext* const* ctx = nullptr, int k = 0,
+              const G4DCamera* cams = nullptr)
+        : saved(t_call), rc(open(kind, ws, st, ctx, k, cams)) {}
+    ~CallFrame() { t_call = saved; }
+
+  private:
+    static int open(Kind kind, const G4DWorkspace* ws, cudaStream_t st, G4DContext* const* ctx, int k, const G4DCamera* cams) {
+        G4D_CUDA(cudaSetDevice(ws->device));
+        int rc = G4D_OK;
+        if (kind == kRead) {
+            G4D_CUDA(cudaDeviceSynchronize());
+        } else {
+            cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+            const cudaError_t e = cudaStreamIsCapturing(st, &cs);
+            const bool capturing = cs != cudaStreamCaptureStatusNone;
+            t_call = CallState{capturing, ws->frozen || capturing, false};
+            if (e != cudaSuccess) {
+                (void)cudaGetLastError();
+                return fail(G4D_ERR_STATE, "cudaStreamIsCapturing", cudaGetErrorString(e));
+            }
+            if (kind != kContextFree) rc = refuse_capture(ws, cams, k, kind == kForward ? ctx : nullptr);
+        }
+        for (int i = 0; rc == G4D_OK && i < k; ++i)
+            if ((rc = check_pending(ctx[i])) == G4D_OK && kind == kForward) ctx[i]->fwd = ForwardRecord{};
+        return rc == G4D_OK && kind == kBackward ? zero_camera_grads(ctx, k, st) : rc;
+    }
+};
+
+// The blend backward of the forward on c: dL/d(mean2D, conic, rgb, opacity) into c->gscratch (BlendGradLayout, zeroed here),
+// except that the opacity gradient lands in g_opacities (zeroed here) when it is set.  *gb: the scratch.  n = 0 runs nothing.
+int blend_backward(G4DContext* c, const G4DCamera* cam, int64_t n, const float* dL_dcolor, float* g_opacities, float** gb,
+                   cudaStream_t st) {
+    using L = BlendGradLayout;
+    const size_t N = (size_t)(n > 0 ? n : 1);
+    const size_t floats = N * (g_opacities ? L::kOpacity : L::kFloats);
+    G4D_CUDA(c->gscratch.ensure(floats * 4 + 256));
+    float* b = *gb = c->gscratch.as<float>();
+    if (n == 0) return G4D_OK;
+    G4D_CUDA(cudaMemsetAsync(b, 0, floats * 4, st));
+    if (g_opacities) G4D_CUDA(cudaMemsetAsync(g_opacities, 0, N * 4, st));
+    reset_stage_flags(c, G4D_STAGE_BLEND_BWD, G4D_STAGE_DEFORM_BWD);
+    {
+        StageTimer tm(c, G4D_STAGE_BLEND_BWD, st);
+        G4D_CUDA(launch_blend_backward(c->cam.as<CameraDev>(), c->grid_x, c->grid_y, c->g, c->b, c->im, dL_dcolor, b + L::kMean2D * N,
+                                       b + L::kConic * N, g_opacities ? g_opacities : b + L::kOpacity * N, b + L::kRgb * N,
+                                       c->ws->warp_cull, st));
+    }
+    return debug_sync(cam, st, "blend_backward");
+}
+
 // blend backward + per-Gaussian backward on `in`; opacity gradient lands in g_opacities (zeroed here); the camera's
 // gradient is added into c->cam_grad when it is set
 int raster_backward_stages(G4DContext* c, const G4DCamera* cam, int64_t n, const RasterInputs& in, const float* dL_dcolor,
                            float* g_means3D, float* g_means2D, const ShOut& g_sh, float* g_opacities, float* g_scales,
                            float* g_rotations, cudaStream_t st) {
     using L = BlendGradLayout;
-    const CameraDev* dcam = c->cam.as<CameraDev>();
-    const size_t N = (size_t)(n > 0 ? n : 1);
-    G4D_CUDA(c->gscratch.ensure(N * L::kOpacity * 4 + 256));   // (the opacity block is the caller's g_opacities)
-    float* gb = c->gscratch.as<float>();
-    float* g_mean2D = gb + L::kMean2D * N;
-    float* g_conic = gb + L::kConic * N;
-    float* g_rgb = gb + L::kRgb * N;
-    if (n == 0) return G4D_OK;
-    G4D_CUDA(cudaMemsetAsync(gb, 0, N * L::kOpacity * 4, st));
-    G4D_CUDA(cudaMemsetAsync(g_opacities, 0, N * 4, st));
-    reset_stage_flags(c, G4D_STAGE_BLEND_BWD, G4D_STAGE_DEFORM_BWD);
-    {
-        StageTimer tm(c, G4D_STAGE_BLEND_BWD, st);
-        G4D_CUDA(launch_blend_backward(dcam, c->grid_x, c->grid_y, c->g, c->b, c->im, dL_dcolor, g_mean2D, g_conic, g_opacities,
-                                       g_rgb, c->ws->warp_cull, st));
-    }
-    int rc;
-    if ((rc = debug_sync(cam, st, "blend_backward")) != G4D_OK) return rc;
+    const size_t N = (size_t)n;
+    float* gb;
+    const int rc = blend_backward(c, cam, n, dL_dcolor, g_opacities, &gb, st);
+    if (rc != G4D_OK || n == 0) return rc;
     StageTimer tm(c, G4D_STAGE_GEOM_BWD, st);
-    G4D_CUDA(launch_preprocess_backward(dcam, n, in, c->g, g_mean2D, g_conic, g_rgb, g_means3D, g_means2D, g_scales,
-                                        g_rotations, g_sh, c->cam_grad, st));
+    G4D_CUDA(launch_preprocess_backward(c->cam.as<CameraDev>(), n, in, c->g, gb + L::kMean2D * N, gb + L::kConic * N,
+                                        gb + L::kRgb * N, g_means3D, g_means2D, g_scales, g_rotations, g_sh, c->cam_grad, st));
     return debug_sync(cam, st, "preprocess_backward");
 }
 
@@ -759,9 +785,8 @@ int g4d_context_stage_times(G4DContext* c, float* out_ms, int capacity) {
 int g4d_context_stats(G4DContext* c, G4DStats* out) {
     if (!c || !out) return fail(G4D_ERR_ARG, "NULL argument");
     if (c->fwd.kind == ForwardRecord::kNone) return fail(G4D_ERR_STATE, "no forward has run on this context");
-    cudaSetDevice(c->ws->device);
-    G4D_CUDA(cudaDeviceSynchronize());
-    { int rc_ = check_pending(c); if (rc_ != G4D_OK) return rc_; }
+    CallFrame call(CallFrame::kRead, c->ws, nullptr, &c, 1);
+    if (call.rc != G4D_OK) return call.rc;
     out->num_rendered = c->R; out->instance_capacity = c->capacity; out->tiles_x = c->grid_x; out->tiles_y = c->grid_y;
     std::vector<int32_t> radii((size_t)c->fwd.n);
     if (c->fwd.n) G4D_CUDA(cudaMemcpy(radii.data(), c->g.radii, (size_t)c->fwd.n * 4, cudaMemcpyDeviceToHost));
@@ -781,9 +806,8 @@ int deform_forward(G4DWorkspace* ws, const G4DDeformParams* prm, int64_t n, cons
                    const float* rotation, const float* opacity, const float* shs, float time, const float* times, float* out_xyz,
                    float* out_scaling, float* out_rotation, float* out_opacity, float* out_shs, uint32_t* relu_bits, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
-    G4D_CUDA(cudaSetDevice(ws->device));
-    CallScope scope(ws, st);
-    if (scope.rc != G4D_OK) return scope.rc;
+    CallFrame call(CallFrame::kContextFree, ws, st);
+    if (call.rc != G4D_OK) return call.rc;
     int rc;
     float* trow[G4D_MAX_LEVELS][3] = {};
     DeformSetup s{};
@@ -842,12 +866,8 @@ int g4d_rasterize_forward(G4DContext* c, const G4DCamera* cam, int64_t n, const 
         return fail(G4D_ERR_ARG, "Please provide means3D, shs, opacities, scales and rotations");
     if (n >= (1ll << 31)) return fail(G4D_ERR_ARG, "n too large");
     cudaStream_t st = (cudaStream_t)stream;
-    G4D_CUDA(cudaSetDevice(c->ws->device));
-    CallScope scope(c->ws, st);
-    if (scope.rc != G4D_OK) return scope.rc;
-    if ((rc = refuse_capture(c->ws, cam, 1, &c)) != G4D_OK) return rc;
-    if ((rc = check_pending(c)) != G4D_OK) return rc;
-    c->fwd = ForwardRecord{};
+    CallFrame call(CallFrame::kForward, c->ws, st, &c, 1, cam);
+    if (call.rc != G4D_OK) return call.rc;
     if ((rc = setup_view(c, cam, nullptr, n, st, [] { return G4D_OK; })) != G4D_OK) return rc;
     const RasterInputs in{means3D, scales, rotations, opacities, caller_sh<ShIn>(sh_coeffs(cam), false, shs)};
     {
@@ -873,12 +893,8 @@ int g4d_rasterize_backward(G4DContext* c, const G4DCamera* cam, int64_t n, const
     if (!dL_dcolor || (n > 0 && (!g_means3D || !g_means2D || !g_shs || !g_opacities || !g_scales || !g_rotations)))
         return fail(G4D_ERR_ARG, "NULL gradient pointer");
     cudaStream_t st = (cudaStream_t)stream;
-    G4D_CUDA(cudaSetDevice(c->ws->device));
-    CallScope scope(c->ws, st);
-    if (scope.rc != G4D_OK) return scope.rc;
-    if ((rc = refuse_capture(c->ws, cam, 1, nullptr)) != G4D_OK) return rc;
-    if ((rc = check_pending(c)) != G4D_OK) return rc;
-    if ((rc = zero_camera_grads(&c, 1, st)) != G4D_OK) return rc;
+    CallFrame call(CallFrame::kBackward, c->ws, st, &c, 1, cam);
+    if (call.rc != G4D_OK) return call.rc;
     (void)opacities;
     const int m = sh_coeffs(cam);
     const RasterInputs in{means3D, scales, rotations, opacities, caller_sh<ShIn>(m, false, shs)};
@@ -889,9 +905,8 @@ int g4d_rasterize_backward(G4DContext* c, const G4DCamera* cam, int64_t n, const
 // ------------------------------------------------------------------------------------------------------
 int64_t g4d_context_read(G4DContext* c, int which, void* host_dst, int64_t bytes) {
     if (!c || c->fwd.kind == ForwardRecord::kNone) return fail(G4D_ERR_STATE, "no forward has run on this context");
-    cudaSetDevice(c->ws->device);
-    if (cudaDeviceSynchronize() != cudaSuccess) return fail(G4D_ERR_CUDA, "cudaDeviceSynchronize");
-    { int rc_ = check_pending(c); if (rc_ != G4D_OK) return rc_; }
+    CallFrame call(CallFrame::kRead, c->ws, nullptr, &c, 1);
+    if (call.rc != G4D_OK) return call.rc;
     const size_t N = (size_t)c->fwd.n, P = (size_t)c->fwd.H * c->fwd.W, R = (size_t)c->R, Tn = (size_t)c->grid_x * c->grid_y;
     std::vector<char> tmp;
     auto pull = [&](const void* src, size_t nbytes) -> bool {
@@ -1010,9 +1025,8 @@ int deform_backward(G4DWorkspace* ws, const G4DDeformParams* prm, G4DDeformGrads
                     const float* times, const float* const go[G4D_NUM_HEADS], float* const gi[G4D_NUM_HEADS], float* g_times,
                     const uint32_t* relu_bits, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
-    G4D_CUDA(cudaSetDevice(ws->device));
-    CallScope scope(ws, st);
-    if (scope.rc != G4D_OK) return scope.rc;
+    CallFrame call(CallFrame::kContextFree, ws, st);
+    if (call.rc != G4D_OK) return call.rc;
     int rc;
     float* trow[G4D_MAX_LEVELS][3] = {};
     if (!times && (rc = collapse_time_rows(ws->trow, trow, prm, TimeArg{time, nullptr}, st)) != G4D_OK) return rc;
@@ -1212,80 +1226,46 @@ int check_camera_group(G4DContext* const* ctx, int32_t k, const G4DCamera* cams)
     return G4D_OK;
 }
 
-std::atomic<uint64_t> g_group_serial{0};
-
-}  // namespace
-
-extern "C" {
-
-int g4d_render_forward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* prm, const G4DGaussians* g,
-                       float* out_color, float* out_depth, int32_t* out_radii, void* stream) {
-    if (!c) return fail(G4D_ERR_ARG, "context is NULL");
-    int rc = check_render_args(cam, prm, g, out_color, out_depth, out_radii);
-    if (rc != G4D_OK) return rc;
-    const cudaStream_t st = (cudaStream_t)stream;
-    G4D_CUDA(cudaSetDevice(c->ws->device));
-    CallScope scope(c->ws, st);
-    if (scope.rc != G4D_OK) return scope.rc;
-    if ((rc = refuse_capture(c->ws, cam, 1, &c)) != G4D_OK) return rc;
-    if ((rc = check_pending(c)) != G4D_OK) return rc;
-    c->fwd = ForwardRecord{};
-    ForwardRecord rec;
-    if ((rc = fused_forward(c, cam, prm, g, out_color, out_depth, out_radii, false, st, &rec)) != G4D_OK) return rc;
-    c->fwd = rec;
+// The checks g4d_render_backward and g4d_render_backward_cameras share, behind each one's own checks of its arguments and of
+// the records it matches: the forward on ctx[0, k) (saved: it kept what the backward reads; `who` names the entry point)
+// deformed exactly when params are given now, cams[i] has the image size and M of the forward on ctx[i], and the params,
+// their gradient sinks and the Gaussians' gradient sinks are usable.
+int check_fused_backward(const char* who, bool saved, G4DContext* const* ctx, int k, const G4DCamera* cams,
+                         const G4DDeformParams* prm, const G4DDeformGrads* pgrads, const G4DGaussians* g,
+                         const G4DGaussianGrads* gg) {
+    if (!saved) return fail(G4D_ERR_STATE, (std::string(who) + " after a G4D_CAM_NO_GRAD forward: nothing was saved for it").c_str());
+    if ((prm != nullptr) != ctx[0]->fwd.deformed) return fail(G4D_ERR_STATE, "deform params differ from the forward's");
+    int rc;
+    if (prm && (rc = check_params(prm)) != G4D_OK) return rc;
+    if ((rc = check_sh_head(&cams[0], prm)) != G4D_OK) return rc;
+    if (prm && !pgrads) return fail(G4D_ERR_ARG, "pgrads is NULL");
+    if (prm && (rc = check_plane_grads(prm, pgrads)) != G4D_OK) return rc;
+    for (int i = 0; i < k; ++i) {
+        const ForwardRecord& f = ctx[i]->fwd;
+        if (cams[i].image_height != f.H || cams[i].image_width != f.W) return fail(G4D_ERR_STATE, "camera differs from the forward's");
+        if (sh_coeffs(&cams[i]) != f.sh_coeffs) return fail(G4D_ERR_STATE, "sh_coeffs differs from the forward's");
+    }
+    const int64_t n = g->n;
+    if (n > 0 && (!gg->xyz || !gg->scaling || !gg->rotation || !gg->opacity || !gg->features_dc))
+        return fail(G4D_ERR_ARG, "NULL gradient pointer");
+    if (g->features_rest && n > 0 && !gg->features_rest && sh_coeffs(&cams[0]) > 1)     // (M = 1: features_rest holds nothing)
+        return fail(G4D_ERR_ARG, "features_rest gradient sink is NULL");
     return G4D_OK;
 }
 
-int g4d_render_backward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* prm, G4DDeformGrads* pgrads,
-                        const G4DGaussians* g, const float* dL_dcolor, G4DGaussianGrads* gg, void* stream) {
-    if (!c) return fail(G4D_ERR_ARG, "context is NULL");
-    if (c->fwd.kind != ForwardRecord::kFused || !g || c->fwd.n != g->n) return fail(G4D_ERR_STATE, "g4d_render_backward needs the matching g4d_render_forward on this context");
-    if (c->fwd.group) return fail(G4D_ERR_STATE, "the last forward on this context was g4d_render_forward_cameras: use g4d_render_backward_cameras");
-    if (!c->fwd.kept) return fail(G4D_ERR_STATE, "g4d_render_backward after a G4D_CAM_NO_GRAD forward: nothing was saved for it");
-    if ((prm != nullptr) != c->fwd.deformed) return fail(G4D_ERR_STATE, "deform params differ from the forward's");
-    int rc = check_camera(cam);
-    if (rc != G4D_OK) return rc;
-    if (prm && (rc = check_params(prm)) != G4D_OK) return rc;
-    if ((rc = check_sh_head(cam, prm)) != G4D_OK) return rc;
-    if (prm && !pgrads) return fail(G4D_ERR_ARG, "pgrads is NULL");
-    if (prm && (rc = check_plane_grads(prm, pgrads)) != G4D_OK) return rc;
-    if (cam->image_height != c->fwd.H || cam->image_width != c->fwd.W) return fail(G4D_ERR_STATE, "camera differs from the forward's");
-    if (sh_coeffs(cam) != c->fwd.sh_coeffs) return fail(G4D_ERR_STATE, "sh_coeffs differs from the forward's");
-    const int64_t n = g->n;
-    if (!dL_dcolor || !gg || (n > 0 && (!gg->xyz || !gg->scaling || !gg->rotation || !gg->opacity || !gg->features_dc || !gg->means2D)))
-        return fail(G4D_ERR_ARG, "NULL gradient pointer");
-    if (g->features_rest && n > 0 && !gg->features_rest && sh_coeffs(cam) > 1)     // (M = 1: features_rest holds nothing)
-        return fail(G4D_ERR_ARG, "features_rest gradient sink is NULL");
-    const cudaStream_t st = (cudaStream_t)stream;
-    G4D_CUDA(cudaSetDevice(c->ws->device));
-    CallScope scope(c->ws, st);
-    if (scope.rc != G4D_OK) return scope.rc;
-    if ((rc = refuse_capture(c->ws, cam, 1, nullptr)) != G4D_OK) return rc;
-    if ((rc = check_pending(c)) != G4D_OK) return rc;
-    if ((rc = zero_camera_grads(&c, 1, st)) != G4D_OK) return rc;
-    return fused_backward(c, cam, prm, pgrads, g, dL_dcolor, gg, st);
-}
+std::atomic<uint64_t> g_group_serial{0};
 
-// ------------------------------------------------------------------------------------------------------
-int g4d_render_forward_cameras(G4DContext* const* ctx, int32_t k, const G4DCamera* cams, const G4DDeformParams* prm,
-                               const G4DGaussians* g, float* const* out_color, float* const* out_depth,
-                               int32_t* const* out_radii, void* stream) {
-    int rc = check_camera_group(ctx, k, cams);
-    if (rc != G4D_OK) return rc;
-    if (!out_color || !out_depth || !out_radii) return fail(G4D_ERR_ARG, "output arrays are NULL");
-    for (int i = 0; i < k; ++i)
-        if ((rc = check_render_args(&cams[i], prm, g, out_color[i], out_depth[i], out_radii[i])) != G4D_OK) return rc;
-    cudaStream_t st = (cudaStream_t)stream;
+// The fused forward of cams[0, k) on ctx[0, k) (arguments checked by the caller).  group: the call is
+// g4d_render_forward_cameras, whose records name the call, each camera's position in it and whether it kept what the group
+// backward reads; g4d_render_forward's record (k = 1) has group 0.
+int fused_forward_cameras(G4DContext* const* ctx, int k, const G4DCamera* cams, const G4DDeformParams* prm, const G4DGaussians* g,
+                          float* const* out_color, float* const* out_depth, int32_t* const* out_radii, bool group,
+                          cudaStream_t st) {
     G4DContext* c0 = ctx[0];
-    G4D_CUDA(cudaSetDevice(c0->ws->device));
-    CallScope scope(c0->ws, st);
-    if (scope.rc != G4D_OK) return scope.rc;
-    if ((rc = refuse_capture(c0->ws, cams, k, ctx)) != G4D_OK) return rc;
-    for (int i = 0; i < k; ++i) {
-        if ((rc = check_pending(ctx[i])) != G4D_OK) return rc;
-        ctx[i]->fwd = ForwardRecord{};
-    }
-    // camera 0: the fused forward of g4d_render_forward; it keeps the deformed tensors when other cameras read them
+    CallFrame call(CallFrame::kForward, c0->ws, st, ctx, k, cams);
+    if (call.rc != G4D_OK) return call.rc;
+    int rc;
+    // camera 0: the fused forward of one camera; it keeps the deformed tensors when other cameras read them
     ForwardRecord r0;
     if ((rc = fused_forward(c0, &cams[0], prm, g, out_color[0], out_depth[0], out_radii[0], k > 1, st, &r0)) != G4D_OK) return rc;
     const int64_t n = g->n;
@@ -1306,14 +1286,53 @@ int g4d_render_forward_cameras(G4DContext* const* ctx, int32_t k, const G4DCamer
             if ((rc = bin_and_blend(ctx[i], &cams[i], n, out_color[i], out_depth[i], st)) != G4D_OK) return rc;
     }
     // cameras 1..k-1 keep nothing of their own for a backward: the group backward reads camera 0's tensors
-    const uint64_t serial = ++g_group_serial;
+    const uint64_t serial = group ? ++g_group_serial : 0;
     for (int i = 0; i < k; ++i) {
         ForwardRecord r = i == 0 ? r0 : ForwardRecord{ForwardRecord::kFused, n, cams[i].image_height, cams[i].image_width,
                                                       r0.deformed, r0.sh, false, r0.sh_coeffs};
-        r.group = serial; r.group_pos = i; r.group_size = k; r.group_grad = !(cams[0].debug & G4D_CAM_NO_GRAD);
+        if (group) { r.group = serial; r.group_pos = i; r.group_size = k; r.group_grad = !(cams[0].debug & G4D_CAM_NO_GRAD); }
         ctx[i]->fwd = r;
     }
     return G4D_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int g4d_render_forward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* prm, const G4DGaussians* g,
+                       float* out_color, float* out_depth, int32_t* out_radii, void* stream) {
+    if (!c) return fail(G4D_ERR_ARG, "context is NULL");
+    const int rc = check_render_args(cam, prm, g, out_color, out_depth, out_radii);
+    if (rc != G4D_OK) return rc;
+    return fused_forward_cameras(&c, 1, cam, prm, g, &out_color, &out_depth, &out_radii, false, (cudaStream_t)stream);
+}
+
+int g4d_render_backward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* prm, G4DDeformGrads* pgrads,
+                        const G4DGaussians* g, const float* dL_dcolor, G4DGaussianGrads* gg, void* stream) {
+    if (!c) return fail(G4D_ERR_ARG, "context is NULL");
+    if (c->fwd.kind != ForwardRecord::kFused || !g || c->fwd.n != g->n) return fail(G4D_ERR_STATE, "g4d_render_backward needs the matching g4d_render_forward on this context");
+    if (c->fwd.group) return fail(G4D_ERR_STATE, "the last forward on this context was g4d_render_forward_cameras: use g4d_render_backward_cameras");
+    int rc = check_camera(cam);
+    if (rc != G4D_OK) return rc;
+    if (!dL_dcolor || !gg || (g->n > 0 && !gg->means2D)) return fail(G4D_ERR_ARG, "NULL gradient pointer");
+    if ((rc = check_fused_backward("g4d_render_backward", c->fwd.kept, &c, 1, cam, prm, pgrads, g, gg)) != G4D_OK) return rc;
+    const cudaStream_t st = (cudaStream_t)stream;
+    CallFrame call(CallFrame::kBackward, c->ws, st, &c, 1, cam);
+    if (call.rc != G4D_OK) return call.rc;
+    return fused_backward(c, cam, prm, pgrads, g, dL_dcolor, gg, st);
+}
+
+// ------------------------------------------------------------------------------------------------------
+int g4d_render_forward_cameras(G4DContext* const* ctx, int32_t k, const G4DCamera* cams, const G4DDeformParams* prm,
+                               const G4DGaussians* g, float* const* out_color, float* const* out_depth,
+                               int32_t* const* out_radii, void* stream) {
+    int rc = check_camera_group(ctx, k, cams);
+    if (rc != G4D_OK) return rc;
+    if (!out_color || !out_depth || !out_radii) return fail(G4D_ERR_ARG, "output arrays are NULL");
+    for (int i = 0; i < k; ++i)
+        if ((rc = check_render_args(&cams[i], prm, g, out_color[i], out_depth[i], out_radii[i])) != G4D_OK) return rc;
+    return fused_forward_cameras(ctx, k, cams, prm, g, out_color, out_depth, out_radii, true, (cudaStream_t)stream);
 }
 
 int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCamera* cams, const G4DDeformParams* prm,
@@ -1329,37 +1348,19 @@ int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCame
         if (f.kind == ForwardRecord::kNone || !f.group || f.group != c0->fwd.group || f.group_pos != i || f.group_size != k || f.n != g->n)
             return fail(G4D_ERR_STATE, "g4d_render_backward_cameras needs the matching g4d_render_forward_cameras on these contexts, "
                                        "with no other forward on any of them since");
-        if (cams[i].image_height != f.H || cams[i].image_width != f.W) return fail(G4D_ERR_STATE, "camera differs from the forward's");
-        if (sh_coeffs(&cams[i]) != f.sh_coeffs) return fail(G4D_ERR_STATE, "sh_coeffs differs from the forward's");
     }
-    if (!c0->fwd.group_grad || !c0->fwd.kept) return fail(G4D_ERR_STATE, "g4d_render_backward_cameras after a G4D_CAM_NO_GRAD forward: nothing was saved for it");
-    if ((prm != nullptr) != c0->fwd.deformed) return fail(G4D_ERR_STATE, "deform params differ from the forward's");
-    if (prm && (rc = check_params(prm)) != G4D_OK) return rc;
-    if ((rc = check_sh_head(&cams[0], prm)) != G4D_OK) return rc;
-    if (prm && !pgrads) return fail(G4D_ERR_ARG, "pgrads is NULL");
-    if (prm && (rc = check_plane_grads(prm, pgrads)) != G4D_OK) return rc;
-    const int64_t n = g->n;
-    if (n > 0 && (!gg->xyz || !gg->scaling || !gg->rotation || !gg->opacity || !gg->features_dc))
-        return fail(G4D_ERR_ARG, "NULL gradient pointer");
-    if (g->features_rest && n > 0 && !gg->features_rest && sh_coeffs(&cams[0]) > 1)
-        return fail(G4D_ERR_ARG, "features_rest gradient sink is NULL");
+    if ((rc = check_fused_backward("g4d_render_backward_cameras", c0->fwd.group_grad && c0->fwd.kept, ctx, k, cams, prm, pgrads,
+                                   g, gg)) != G4D_OK) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    G4DWorkspace* ws = c0->ws;
-    G4D_CUDA(cudaSetDevice(ws->device));
-    CallScope scope(ws, st);
-    if (scope.rc != G4D_OK) return scope.rc;
-    if ((rc = refuse_capture(ws, cams, k, nullptr)) != G4D_OK) return rc;
-    for (int i = 0; i < k; ++i)
-        if ((rc = check_pending(ctx[i])) != G4D_OK) return rc;
-    if ((rc = zero_camera_grads(ctx, k, st)) != G4D_OK) return rc;
+    CallFrame call(CallFrame::kBackward, c0->ws, st, ctx, k, cams);
+    if (call.rc != G4D_OK) return call.rc;
     if (k == 1 && dL_dcolor[0]) {     // one camera: the single-camera backward
         G4DGaussianGrads g1 = *gg;
         g1.means2D = g_means2D ? g_means2D[0] : nullptr;
         return fused_backward(c0, &cams[0], prm, pgrads, g, dL_dcolor[0], &g1, st);
     }
+    const int64_t n = g->n;
     if (n == 0) return G4D_OK;
-    using L = BlendGradLayout;
-    const size_t N = (size_t)n;
     DeformedGrads d;
     if ((rc = deformed_grads(c0, n, gg, &d)) != G4D_OK) return rc;
     // blend backward of every camera in the loss, each into its own scratch
@@ -1368,21 +1369,13 @@ int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCame
     bool cam_grads = false;
     for (int i = 0; i < k; ++i) {
         G4DContext* c = ctx[i];
-        reset_stage_flags(c, G4D_STAGE_BLEND_BWD, G4D_STAGE_DEFORM_BWD);
         if (!dL_dcolor[i]) {
-            if (g_means2D && g_means2D[i]) G4D_CUDA(cudaMemsetAsync(g_means2D[i], 0, N * 12, st));
+            reset_stage_flags(c, G4D_STAGE_BLEND_BWD, G4D_STAGE_DEFORM_BWD);
+            if (g_means2D && g_means2D[i]) G4D_CUDA(cudaMemsetAsync(g_means2D[i], 0, (size_t)n * 12, st));
             continue;
         }
-        G4D_CUDA(c->gscratch.ensure(N * L::kFloats * 4 + 256));
-        float* gb = c->gscratch.as<float>();
-        G4D_CUDA(cudaMemsetAsync(gb, 0, N * L::kFloats * 4, st));
-        {
-            StageTimer tm(c, G4D_STAGE_BLEND_BWD, st);
-            G4D_CUDA(launch_blend_backward(c->cam.as<CameraDev>(), c->grid_x, c->grid_y, c->g, c->b, c->im, dL_dcolor[i],
-                                           gb + L::kMean2D * N, gb + L::kConic * N, gb + L::kOpacity * N, gb + L::kRgb * N,
-                                           ws->warp_cull, st));
-        }
-        if ((rc = debug_sync(&cams[i], st, "blend_backward")) != G4D_OK) return rc;
+        float* gb;
+        if ((rc = blend_backward(c, &cams[i], n, dL_dcolor[i], nullptr, &gb, st)) != G4D_OK) return rc;
         const int j = bc.count++;
         bc.cam[j] = c->cam.as<CameraDev>(); bc.radii[j] = c->g.radii; bc.clamped[j] = c->g.clamped; bc.grad[j] = gb;
         bc.g_means2D[j] = g_means2D ? g_means2D[i] : nullptr;
@@ -1506,9 +1499,8 @@ int g4d_adam_step_device(G4DWorkspace* ws, float* param, const float* grad, floa
 int g4d_dist2_knn3(G4DWorkspace* ws, int64_t n, const float* xyz, float* out_mean_dist2, void* stream) {
     if (!ws || n < 0 || (n > 0 && (!xyz || !out_mean_dist2))) return fail(G4D_ERR_ARG, "g4d_dist2_knn3: bad argument");
     if (n >= (1ll << 31)) return fail(G4D_ERR_ARG, "n too large");
-    G4D_CUDA(cudaSetDevice(ws->device));
-    CallScope scope(ws, (cudaStream_t)stream);
-    if (scope.rc != G4D_OK) return scope.rc;
+    CallFrame call(CallFrame::kContextFree, ws, (cudaStream_t)stream);
+    if (call.rc != G4D_OK) return call.rc;
     G4D_CUDA(ws->scratch.ensure(knn_scratch_bytes(n)));
     G4D_CUDA(launch_knn_dist2(n, xyz, out_mean_dist2, ws->scratch.p, ws->sm_count, (cudaStream_t)stream));
     return G4D_OK;
