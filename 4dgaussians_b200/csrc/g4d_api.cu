@@ -171,6 +171,7 @@ struct G4DContext {
     int64_t R = 0, capacity = 0;
     const float* time_src = nullptr;  // g4d_context_set_time_source (device; NULL: G4DCamera.time)
     float* cam_grad = nullptr;        // g4d_context_set_camera_grad (device, kCamGradFloats; NULL: no camera gradient)
+    float* time_grad = nullptr;       // g4d_context_set_time_grad (device, 1 float; NULL: no time gradient)
     const void* bin_ctl = nullptr;    // device BinCtl of the last forward
     bool learned = false;             // R of an earlier exact forward is known (no-sync mode needs a learnt capacity)
     GeomBuffers g{};
@@ -460,11 +461,11 @@ int attach_forward_buffers(G4DWorkspace* ws, DeformSetup& s, float* feat, uint32
     return G4D_OK;
 }
 
-// backward of the deformation network with the time rows trow -- or, times set, at the per-Gaussian times [n] with dL/d(times)
-// into g_times (may be NULL) -- picks the engine -- tensor-core when the configuration allows, FFMA otherwise -- and brings its
+// backward of the deformation network with the time rows trow and dL/d(time) added into g_time (may be NULL) -- or, times
+// set, at the per-Gaussian times [n] with dL/d(times) into g_times (may be NULL) -- picks the engine -- tensor-core when the configuration allows, FFMA otherwise -- and brings its
 // weight images up to date; the desc is built after that refresh
 int deform_backward_dispatch(G4DWorkspace* ws, const G4DDeformParams* prm, float* const (*trow)[3], const G4DDeformGrads* grads,
-                             TimeArg time, const float* times, float* g_times, int64_t n, const float* xyz,
+                             TimeArg time, const float* times, float* g_times, float* g_time, int64_t n, const float* xyz,
                              const float* const go[G4D_NUM_HEADS], float* const gi[G4D_NUM_HEADS], const uint32_t* relu_bits,
                              const float* saved_feat, cudaStream_t st) {
     int rc;
@@ -480,7 +481,7 @@ int deform_backward_dispatch(G4DWorkspace* ws, const G4DDeformParams* prm, float
     const uint32_t* order = nullptr;   // the walk order of the backward's own gather (none when the forward's features are kept)
     if (!saved_feat && (rc = gather_order(ws, prm->aabb, xyz, n, st, &order)) != G4D_OK) return rc;
     G4D_CUDA(ws->scratch.ensure(deform_backward_scratch_bytes(d, n, tc)));
-    G4D_CUDA(launch_deform_backward(d, *prm, *grads, tc ? &ws->tc_bwd.img : nullptr, time, n, xyz, go, gi, g_times, relu_bits, saved_feat,
+    G4D_CUDA(launch_deform_backward(d, *prm, *grads, tc ? &ws->tc_bwd.img : nullptr, time, n, xyz, go, gi, g_times, g_time, relu_bits, saved_feat,
                                     order, ws->scratch.p, ws->sm_count, st));
     return G4D_OK;
 }
@@ -608,15 +609,21 @@ template <class Sh, class T> Sh caller_sh(int m, bool split, T* dc, T* rest = nu
     return split ? Sh{nullptr, dc, rest, m} : Sh{dc, nullptr, nullptr, m};
 }
 
-// The camera-gradient sinks of a backward on ctx[0, k) (g4d_context_set_camera_grad): refused while capturing (a graph would
-// keep writing a sink the context may since have dropped), else zeroed on st; the per-Gaussian backward adds into them, and
-// a camera outside the loss keeps the zeros.  Called before the backward's first launch.
-int zero_camera_grads(G4DContext* const* ctx, int k, cudaStream_t st) {
-    for (int i = 0; i < k; ++i)
+// The gradient sinks of a backward on ctx[0, k), camera (g4d_context_set_camera_grad) and time (g4d_context_set_time_grad):
+// refused while capturing (a graph would keep writing a sink the context may since have dropped), else zeroed on st; the
+// backward adds into them, and a sink nothing adds into (a camera outside the loss, a backward without a deformation) keeps
+// the zeros.  Called before the backward's first launch.
+int zero_grad_sinks(G4DContext* const* ctx, int k, cudaStream_t st) {
+    for (int i = 0; i < k; ++i) {
         if (ctx[i]->cam_grad && t_call.capturing)
             return fail(G4D_ERR_STATE, "cannot capture a backward on a context with a camera gradient set (g4d_context_set_camera_grad)");
-    for (int i = 0; i < k; ++i)
+        if (ctx[i]->time_grad && t_call.capturing)
+            return fail(G4D_ERR_STATE, "cannot capture a backward on a context with a time gradient set (g4d_context_set_time_grad)");
+    }
+    for (int i = 0; i < k; ++i) {
         if (ctx[i]->cam_grad) G4D_CUDA(cudaMemsetAsync(ctx[i]->cam_grad, 0, kCamGradFloats * sizeof(float), st));
+        if (ctx[i]->time_grad) G4D_CUDA(cudaMemsetAsync(ctx[i]->time_grad, 0, sizeof(float), st));
+    }
     return G4D_OK;
 }
 
@@ -624,7 +631,7 @@ int zero_camera_grads(G4DContext* const* ctx, int k, cudaStream_t st) {
 // and sets t_call for the stream st (restored when the entry point returns; kRead synchronises the device instead).  Then,
 // on the contexts ctx[0, k) and their cameras cams[0, k): a forward or backward refuses what a capture cannot repeat, every
 // kind but kContextFree resolves the pending read-backs, a forward clears each context's record once its read-backs are
-// resolved and a backward zeroes the camera-gradient sinks.  rc != G4D_OK: the entry point returns it.
+// resolved and a backward zeroes the gradient sinks.  rc != G4D_OK: the entry point returns it.
 struct CallFrame {
     enum Kind { kContextFree, kRead, kForward, kBackward };
     CallState saved;
@@ -653,7 +660,7 @@ struct CallFrame {
         }
         for (int i = 0; rc == G4D_OK && i < k; ++i)
             if ((rc = check_pending(ctx[i])) == G4D_OK && kind == kForward) ctx[i]->fwd = ForwardRecord{};
-        return rc == G4D_OK && kind == kBackward ? zero_camera_grads(ctx, k, st) : rc;
+        return rc == G4D_OK && kind == kBackward ? zero_grad_sinks(ctx, k, st) : rc;
     }
 };
 
@@ -1030,7 +1037,8 @@ int deform_backward(G4DWorkspace* ws, const G4DDeformParams* prm, G4DDeformGrads
     int rc;
     float* trow[G4D_MAX_LEVELS][3] = {};
     if (!times && (rc = collapse_time_rows(ws->trow, trow, prm, TimeArg{time, nullptr}, st)) != G4D_OK) return rc;
-    return deform_backward_dispatch(ws, prm, trow, grads, TimeArg{time, nullptr}, times, g_times, n, xyz, go, gi, relu_bits, nullptr, st);
+    return deform_backward_dispatch(ws, prm, trow, grads, TimeArg{time, nullptr}, times, g_times, nullptr, n, xyz, go, gi, relu_bits,
+                                    nullptr, st);
 }
 
 }  // namespace
@@ -1163,9 +1171,10 @@ ShOut fused_sh_sinks(const G4DContext* c, const G4DGaussians* g, const G4DGaussi
 }
 
 // The tail of the backward of a fused forward on c, after its per-Gaussian backward wrote d: the SH gradient copy, the
-// activation backward and, in the fine stage, the network's backward.  cam: the camera whose time and debug flag it uses.
+// activation backward and, in the fine stage, the network's backward, which adds dL/d(time) into g_time when it is set.
+// cam: the camera whose time and debug flag it uses.
 int fused_backward_tail(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* prm, G4DDeformGrads* pgrads,
-                        const G4DGaussians* g, const G4DGaussianGrads* gg, const DeformedGrads& d, cudaStream_t st) {
+                        const G4DGaussians* g, const G4DGaussianGrads* gg, const DeformedGrads& d, float* g_time, cudaStream_t st) {
     const int64_t n = g->n;
     int rc;
     if (c->fwd.sh && !g->features_rest)
@@ -1177,9 +1186,9 @@ int fused_backward_tail(G4DContext* c, const G4DCamera* cam, const G4DDeformPara
     const bool saved = c->fwd.feat_cols != 0;
     {
         StageTimer tm(c, G4D_STAGE_DEFORM_BWD, st);
-        if ((rc = deform_backward_dispatch(c->ws, prm, c->trow_ptr, pgrads, TimeArg{cam->time, c->time_src}, nullptr, nullptr, n, g->xyz, go, gi,
-                                           saved ? c->relu.as<uint32_t>() : nullptr, saved ? c->feat.as<float>() : nullptr,
-                                           st)) != G4D_OK) return rc;
+        if ((rc = deform_backward_dispatch(c->ws, prm, c->trow_ptr, pgrads, TimeArg{cam->time, c->time_src}, nullptr, nullptr, g_time,
+                                           n, g->xyz, go, gi, saved ? c->relu.as<uint32_t>() : nullptr,
+                                           saved ? c->feat.as<float>() : nullptr, st)) != G4D_OK) return rc;
     }
     return debug_sync(cam, st, "deform_backward");
 }
@@ -1197,7 +1206,7 @@ int fused_backward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* p
     rc = raster_backward_stages(c, cam, n, deformed_inputs(c, c->fwd, g), dL_dcolor, d.xyz, gg->means2D,
                                 fused_sh_sinks(c, g, gg, d.sh), d.op, d.sc, d.rot, st);
     if (rc != G4D_OK) return rc;
-    return fused_backward_tail(c, cam, prm, pgrads, g, gg, d, st);
+    return fused_backward_tail(c, cam, prm, pgrads, g, gg, d, c->time_grad, st);
 }
 
 // k cameras on k contexts: 1 <= k <= G4D_MAX_CAMERAS, one time bit for bit (or, when ctx[0] has a time source, that same
@@ -1388,8 +1397,15 @@ int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCame
                                                     fused_sh_sinks(c0, g, gg, d.sh), cam_grads ? &cs : nullptr, st));
     }
     if ((rc = debug_sync(&cams[0], st, "preprocess_backward_cameras")) != G4D_OK) return rc;
-    // the network's backward, once, on the gradients summed over the cameras
-    return fused_backward_tail(c0, &cams[0], prm, pgrads, g, gg, d, st);
+    // the network's backward, once, on the gradients summed over the cameras; the one dL/d(time) of the group goes to the
+    // first context with a time sink and is copied into the others'
+    float* g_time = nullptr;
+    for (int i = 0; i < k && !g_time; ++i) g_time = ctx[i]->time_grad;
+    if ((rc = fused_backward_tail(c0, &cams[0], prm, pgrads, g, gg, d, g_time, st)) != G4D_OK) return rc;
+    for (int i = 0; i < k; ++i)
+        if (ctx[i]->time_grad && ctx[i]->time_grad != g_time)
+            G4D_CUDA(cudaMemcpyAsync(ctx[i]->time_grad, g_time, sizeof(float), cudaMemcpyDeviceToDevice, st));
+    return G4D_OK;
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -1515,6 +1531,12 @@ int g4d_context_set_time_source(G4DContext* c, const float* d_time) {
 int g4d_context_set_camera_grad(G4DContext* c, float* d_out) {
     if (!c) return fail(G4D_ERR_ARG, "context is NULL");
     c->cam_grad = d_out;
+    return G4D_OK;
+}
+
+int g4d_context_set_time_grad(G4DContext* c, float* d_out) {
+    if (!c) return fail(G4D_ERR_ARG, "context is NULL");
+    c->time_grad = d_out;
     return G4D_OK;
 }
 

@@ -766,27 +766,50 @@ static cudaError_t launch_bwd_scatter(const DeformBwdArgs& ba, int64_t n, const 
 }
 
 // ---- kernel T: collapsed time-row gradients -> the two time rows of each (axis, t) plane --------------------
-// s.src: the rows' gradients; s.dst: the time planes' gradients
-__global__ void distribute_time_grad_kernel(TimeRowSegs s, TimeArg time) {
+// s.src: the rows' gradients; s.dst: the time planes' gradients; s.plane: the time planes.
+// SINK: also dL/dt into *sink (zeroed by the caller; DESIGN.md §4.11).  A row r = w0 P[i0] + w1 P[i1] of the time plane
+// P = s.plane[l][a] has dr/dt = gmul (P[i1] - P[i0]), so element e adds gv gmul (P[i1][e] - P[i0][e]); the block sums its
+// elements and adds the sum into *sink with one atomic.
+// (The plane pointers are a member of the segments, not a parameter of their own: as one, ptxas copies them to the stack.)
+struct TimeGradSegs : TimeRowSegs {
+    const float* plane[G4D_MAX_LEVELS][3];
+    TimeGradSegs(int levels_, const int32_t (*res_)[4], int C_) : TimeRowSegs(levels_, res_, C_), plane{} {}
+};
+template <bool SINK>
+__global__ void distribute_time_grad_kernel(TimeGradSegs s, TimeArg time, float* sink) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= s.start[3 * s.levels]) return;
-    int l, a, e;
-    s.locate(i, l, a, e);
-    const Tap1D ty = make_tap(time.get(), s.res[l][3]);
-    const int rowlen = s.res[l][a] * s.C;
-    const float gv = s.src[l][a][e];
-    atomicAdd(s.dst[l][a] + (size_t)ty.i0 * rowlen + e, gv * ty.w0);
-    atomicAdd(s.dst[l][a] + (size_t)ty.i1 * rowlen + e, gv * ty.w1);
+    float dt = 0.f;
+    if (i < s.start[3 * s.levels]) {
+        int l, a, e;
+        s.locate(i, l, a, e);
+        const Tap1D ty = make_tap(time.get(), s.res[l][3]);
+        const int rowlen = s.res[l][a] * s.C;
+        const float gv = s.src[l][a][e];
+        atomicAdd(s.dst[l][a] + (size_t)ty.i0 * rowlen + e, gv * ty.w0);
+        atomicAdd(s.dst[l][a] + (size_t)ty.i1 * rowlen + e, gv * ty.w1);
+        if (SINK) {
+            const float* p = s.plane[l][a];
+            dt = gv * (__ldg(p + (size_t)ty.i1 * rowlen + e) - __ldg(p + (size_t)ty.i0 * rowlen + e)) * ty.gmul;
+        }
+    }
+    if (SINK) {
+        const float sum = block_sum_f(dt);
+        if (threadIdx.x == 0) atomicAdd(sink, sum);
+    }
 }
 
 // ---- host side -------------------------------------------------------------------------------------------
-static cudaError_t launch_distribute_time_grad(const DeformBwdArgs& ba, TimeArg time, cudaStream_t st) {
+static cudaError_t launch_distribute_time_grad(const DeformBwdArgs& ba, TimeArg time, float* g_time, cudaStream_t st) {
     const DeformDesc& d = ba.d;
-    TimeRowSegs s(d.levels, d.res, d.C);
+    TimeGradSegs s(d.levels, d.res, d.C);
     for (int l = 0; l < d.levels; ++l)
-        for (int a = 0; a < 3; ++a) { s.src[l][a] = ba.buf.trow_grad[l][a]; s.dst[l][a] = ba.g.planes[l][kTimePlane[a]]; }
+        for (int a = 0; a < 3; ++a) {
+            s.src[l][a] = ba.buf.trow_grad[l][a]; s.dst[l][a] = ba.g.planes[l][kTimePlane[a]];
+            s.plane[l][a] = d.planes[l][kTimePlane[a]];
+        }
     const int total = (int)s.total();
-    distribute_time_grad_kernel<<<(total + 255) / 256, 256, 0, st>>>(s, time);
+    if (g_time) distribute_time_grad_kernel<true><<<(total + 255) / 256, 256, 0, st>>>(s, time, g_time);
+    else distribute_time_grad_kernel<false><<<(total + 255) / 256, 256, 0, st>>>(s, time, nullptr);
     return cudaGetLastError();
 }
 
@@ -869,7 +892,7 @@ static cudaError_t launch_ffma_engine(const DeformBwdArgs& ba, int64_t n, int sm
 
 cudaError_t launch_deform_backward(const DeformDesc& d, const G4DDeformParams& prm, const G4DDeformGrads& grads, const TcBwdWeights* tc,
                                    TimeArg time, int64_t n, const float* xyz, const float* const go[G4D_NUM_HEADS],
-                                   float* const gi[G4D_NUM_HEADS], float* g_times, const uint32_t* relu_bits,
+                                   float* const gi[G4D_NUM_HEADS], float* g_times, float* g_time, const uint32_t* relu_bits,
                                    const float* saved_feat, const uint32_t* order, void* scratch, int sm_count, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
     const TimeRows tr(d.levels, d.res, d.C);
@@ -896,7 +919,7 @@ cudaError_t launch_deform_backward(const DeformDesc& d, const G4DDeformParams& p
     if (e != cudaSuccess) return e;
     if ((e = launch_bwd_scatter(ba, n, xyz, st)) != cudaSuccess) return e;
     if (tc && (e = launch_tc_bwd_wgrad(d, grads, n, buf.images, sm_count, st)) != cudaSuccess) return e;
-    return d.times ? cudaSuccess : launch_distribute_time_grad(ba, time, st);
+    return d.times ? cudaSuccess : launch_distribute_time_grad(ba, time, g_time, st);
 }
 
 // ------------------------------------------------------------------------------------------------------

@@ -103,6 +103,28 @@ inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, siz
     cfg.attrs = attr; cfg.numAttrs = (pdl && g_pdl) ? 1 : 0;
     return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
+
+G4D_D float warp_sum_f(float v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
+// block-wide sum (any block size that is a multiple of 32, <= 1024); result valid in thread 0
+G4D_D float block_sum_f(float v) {
+    __shared__ float s_part[32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    v = warp_sum_f(v);
+    __syncthreads();
+    if (lane == 0) s_part[warp] = v;
+    __syncthreads();
+    float r = 0.f;
+    if (warp == 0) {
+        r = lane < (int)(blockDim.x >> 5) ? s_part[lane] : 0.f;
+        r = warp_sum_f(r);
+    }
+    return r;
+}
 #endif
 
 }  // namespace g4d

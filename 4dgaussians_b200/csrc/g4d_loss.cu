@@ -15,28 +15,6 @@ namespace g4d {
 
 namespace {
 
-__device__ __forceinline__ float warp_sum_f(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
-// block-wide sum (any block size that is a multiple of 32, <= 1024); result valid in thread 0
-__device__ __forceinline__ float block_sum_f(float v) {
-    __shared__ float s_part[32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    v = warp_sum_f(v);
-    __syncthreads();
-    if (lane == 0) s_part[warp] = v;
-    __syncthreads();
-    float r = 0.f;
-    if (warp == 0) {
-        r = lane < (int)(blockDim.x >> 5) ? s_part[lane] : 0.f;
-        r = warp_sum_f(r);
-    }
-    return r;
-}
-
 // ---- L1 -----------------------------------------------------------------------------------------------------------
 // kVec: every pointer is 16-byte aligned, float4 loads + a scalar tail in block 0.  Otherwise (a view at an odd storage
 // offset, e.g. batch[1] of a [B,3,H,W] batch with H*W odd) the same sum with scalar loads.

@@ -79,27 +79,39 @@ def camera_grad_leaves(rss):
 
 class CameraGradSinks:
     """One [k, 35] float32 device buffer whose row i the backward on context ``ctxs[i]`` overwrites with its camera's
-    gradient, for the cameras named in ``spec``; the contexts' pointers are cleared again on exit (they return to a pool)."""
+    gradient, for the cameras named in ``spec``; with ``time``, one device float that the backward on ``ctxs[0]``
+    overwrites with dL/d(time) (g4d_context_set_time_grad).  The contexts' pointers are cleared again on exit (they return
+    to a pool)."""
 
-    def __init__(self, spec, ctxs, dev):
+    def __init__(self, spec, ctxs, dev, time=False):
         self.cams = sorted({i for i, _ in spec})
         self.ctxs = ctxs
         self.buf = torch.empty(len(ctxs), 35, device=dev, dtype=torch.float32) if spec else None
+        self.tbuf = torch.empty(1, device=dev, dtype=torch.float32) if time else None
 
     def __enter__(self):
         for i in self.cams:
             self.ctxs[i].set_camera_grad(self.buf[i].data_ptr())
+        if self.tbuf is not None:
+            self.ctxs[0].set_time_grad(self.tbuf.data_ptr())
         return self
 
     def __exit__(self, *exc):
         for i in self.cams:
             self.ctxs[i].set_camera_grad(None)
+        if self.tbuf is not None:
+            self.ctxs[0].set_time_grad(None)
         return False
 
     def grads(self, spec, metas):
         """The gradient of each camera tensor of ``spec`` in its (shape, dtype, device), ``metas`` (``tensor_meta``)."""
         return tuple(self.buf[i, off:off + n].reshape(shape).to(device=device, dtype=dtype)
                      for (i, f), (shape, dtype, device) in zip(spec, metas) for _, off, n in (_CAM_FIELDS[f],))
+
+    def time_grad(self, meta):
+        """dL/d(time) in the time tensor's (shape, dtype, device), ``meta`` (one entry of ``tensor_meta``)."""
+        shape, dtype, device = meta
+        return self.tbuf.reshape(shape).to(device=device, dtype=dtype)
 
 
 def tensor_meta(tensors):

@@ -10,6 +10,10 @@ no ``torch.cat`` of the SH features, no per-call ``.cuda()`` copies of the camer
 ``render_cameras`` renders one timestamp from several cameras (a camera rig at frame t) in one call: the deformation
 network runs once, forward and backward (``g4d_render_forward_cameras`` / ``g4d_render_backward_cameras``).  ``render``
 is its one-camera case, which takes the single-camera entry points.
+
+Both differentiate the camera tensors that require grad (``rasterizer.camera_grad_leaves``) and the camera's time when it
+is a tensor that requires grad (``time_grad_leaf``): dL/dt comes from the network's backward, for learning per-camera time
+offsets.
 """
 from __future__ import annotations
 
@@ -41,6 +45,25 @@ def settings_from_camera(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=
         rs = viewpoint_camera['camera']
         t = scalar_time(viewpoint_camera['time'])
     return rs, t
+
+
+def time_grad_leaf(viewpoint_cameras, cam_type=None):
+    """The cameras' time tensor that takes a gradient (grad mode on, ``requires_grad``), or None.  The cameras of one call
+    share one deformation and so one dL/dt: when one camera's time takes a gradient, every camera must hold that same
+    tensor object (ValueError otherwise, before anything runs)."""
+    if not torch.is_grad_enabled():
+        return None
+    times = [c['time'] if cam_type == "PanopticSports" else c.time for c in viewpoint_cameras]
+    leaves = [t for t in times if torch.is_tensor(t) and t.requires_grad]
+    if not leaves:
+        return None
+    if any(t is not leaves[0] for t in times):
+        raise ValueError("render_cameras deforms once for all cameras, so it has one time gradient: a camera's time requires "
+                         "grad, and then every camera must hold that same time tensor.  Call render() per camera to learn "
+                         "a time per camera")
+    if leaves[0].numel() != 1:
+        raise ValueError("a camera time that requires grad must have one element, got shape %s" % (tuple(leaves[0].shape),))
+    return leaves[0]
 
 
 def _fused_forward(module: Optional[deform_network], rss, t, needs_bwd, xyz, scaling, rotation, opacity, f_dc, f_rest):
@@ -90,15 +113,18 @@ def _pointers(tensors):
 
 class _FusedRender(torch.autograd.Function):
     """inputs: xyz, scaling, rotation, opacity, features_dc, features_rest, k x means2D, *deform parameters, then the
-    camera tensors that take a gradient (cam_spec: their (camera, field) pairs, rasterizer.camera_grad_leaves);
-    outputs: k images, k radii, k depth maps"""
+    camera tensors that take a gradient (cam_spec: their (camera, field) pairs, rasterizer.camera_grad_leaves), then, when
+    ``timed``, the time tensor that takes a gradient (time_grad_leaf); outputs: k images, k radii, k depth maps"""
 
     @staticmethod
-    def forward(ctx, module: Optional[deform_network], rss, t, cam_spec, xyz, scaling, rotation, opacity, f_dc, f_rest, *rest):
+    def forward(ctx, module: Optional[deform_network], rss, t, cam_spec, timed, xyz, scaling, rotation, opacity, f_dc, f_rest,
+                *rest):
         colors, radii, depths, leases, cstructs, saved = _fused_forward(module, rss, t, any(ctx.needs_input_grad), xyz, scaling,
                                                                         rotation, opacity, f_dc, f_rest)
         ctx.module, ctx.rss, ctx.n, ctx.leases = module, rss, xyz.shape[0], leases
-        ctx.cam_spec, ctx.cam_meta = cam_spec, tensor_meta(rest[len(rest) - len(cam_spec):])
+        end = len(rest) - int(timed)
+        ctx.cam_spec, ctx.cam_meta = cam_spec, tensor_meta(rest[end - len(cam_spec):end])
+        ctx.time_meta = tensor_meta(rest[end:])[0] if timed else None
         ctx.lease = leases[0]        # camera 0's context: what a render() caller reads the forward's buffers through
         # the C-ABI structs (and the tensors whose pointers they carry) are kept for the backward: rebuilding them costs the
         # host ~0.3 ms per view, during which the GPU has nothing queued behind the forward's last kernel
@@ -137,7 +163,7 @@ class _FusedRender(torch.autograd.Function):
         gm2 = [flat[(end + 3 * i) * npad:(end + 3 * i) * npad + 3 * n].view(n, 3) for i in range(k)]
         gg = _lib.GaussianGrads(gx.data_ptr(), gs.data_ptr(), gr.data_ptr(), go.data_ptr(), gdc.data_ptr(), grest.data_ptr(),
                                 gm2[0].data_ptr() if k == 1 else None)
-        sinks = CameraGradSinks(ctx.cam_spec, [lease.ctx for lease in leases], dev)
+        sinks = CameraGradSinks(ctx.cam_spec, [lease.ctx for lease in leases], dev, time=ctx.time_meta is not None)
         with torch.cuda.device(dev), sinks:
             if k == 1:
                 if gcols[0] is None:        # the single-camera backward takes an image gradient
@@ -154,7 +180,8 @@ class _FusedRender(torch.autograd.Function):
             lease.release()
         ctx.leases = ctx.lease = None
         cam_grads = sinks.grads(ctx.cam_spec, ctx.cam_meta) if ctx.cam_spec else ()
-        return (None, None, None, None, gx, gs, gr, go, gdc, grest) + tuple(gm2) + tuple(pgrads) + cam_grads
+        time_grad = (sinks.time_grad(ctx.time_meta),) if ctx.time_meta is not None else ()
+        return (None, None, None, None, None, gx, gs, gr, go, gdc, grest) + tuple(gm2) + tuple(pgrads) + cam_grads + time_grad
 
 
 def _time_bits(t) -> bytes:
@@ -195,6 +222,7 @@ def _render(viewpoint_cameras, pc, pipe, bg_color, scaling_modifier, override_co
         raise ValueError("render_cameras needs at least one camera")
     if len(cams) > _lib.MAX_CAMERAS:
         raise ValueError("render_cameras takes at most %d cameras per call, got %d" % (_lib.MAX_CAMERAS, len(cams)))
+    time_leaf = time_grad_leaf(cams, cam_type)
     settings = [settings_from_camera(c, pc, pipe, bg_color, scaling_modifier, cam_type) for c in cams]
     rss = [rs for rs, _ in settings]
     t = settings[0][1]
@@ -220,14 +248,19 @@ def _render(viewpoint_cameras, pc, pipe, bg_color, scaling_modifier, override_co
         else:
             params = tuple(module.flat_parameters()) if module is not None else ()
             cam_spec, cam_leaves = camera_grad_leaves(rss)      # camera tensors that require grad: extra inputs
-            outs = _FusedRender.apply(module, rss, t, cam_spec, xyz, pc._scaling, pc._rotation, pc._opacity, pc._features_dc,
-                                      pc._features_rest, *points, *params, *cam_leaves)
+            time_leaves = () if time_leaf is None else (time_leaf,)
+            outs = _FusedRender.apply(module, rss, t, cam_spec, time_leaf is not None, xyz, pc._scaling, pc._rotation,
+                                      pc._opacity, pc._features_dc, pc._features_rest, *points, *params, *cam_leaves,
+                                      *time_leaves)
             images, radii, depths = outs[:k], outs[k:2 * k], outs[2 * k:]
     else:
         # a foreign (e.g. the reference's own PyTorch) deformation module: keep its semantics, deform once, then rasterize
         # every camera with g4d
         n = xyz.shape[0]
-        time = torch.tensor(t, device=xyz.device, dtype=torch.float32).repeat(n, 1)
+        if time_leaf is None:
+            time = torch.tensor(t, device=xyz.device, dtype=torch.float32).repeat(n, 1)
+        else:       # kept in the graph: the module's own autograd gives dL/dt
+            time = time_leaf.to(device=xyz.device, dtype=torch.float32).reshape(1, 1).repeat(n, 1)
         m3, sc, rot, op, shs = module(xyz, pc._scaling, pc._rotation, pc._opacity, pc.get_features, time)
         opac, scales, rots = pc.opacity_activation(op), pc.scaling_activation(sc), pc.rotation_activation(rot)
         images, radii, depths = [], [], []
@@ -251,5 +284,6 @@ def render_cameras(viewpoint_cameras, pc, pipe, bg_color: torch.Tensor, scaling_
     """Render one timestamp from several cameras: one result dict per camera, each with the keys render() returns and its
     own ``viewspace_points``.  The cameras must share their time (as float32, bit for bit; else ValueError) and there may
     be at most G4D_MAX_CAMERAS (32) of them.  With the g4d deformation network the deformation runs once for all cameras,
-    forward and backward; a foreign deformation module is run once and its output rasterized per camera."""
+    forward and backward; a foreign deformation module is run once and its output rasterized per camera.  A time that
+    requires grad must be one tensor that every camera holds (ValueError otherwise): the group's one dL/dt goes to it."""
     return _render(viewpoint_cameras, pc, pipe, bg_color, scaling_modifier, override_color, stage, cam_type)

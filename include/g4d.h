@@ -401,6 +401,18 @@ int g4d_context_set_time_source(G4DContext *ctx, const float *d_time);
  * returns an error after that point (a CUDA error, a buffer that cannot grow) leaves it zeroed or partly summed, not as it
  * was. */
 int g4d_context_set_camera_grad(G4DContext *ctx, float *d_out);
+
+/* ---- time gradients ------------------------------------------------------------------------------------------------
+ * g4d_context_set_time_grad: while d_out (device, 1 float) is set, every backward on ctx OVERWRITES d_out[0] with dL/d of
+ * the call's time (G4DCamera.time, or the value read through g4d_context_set_time_source).  g4d_render_backward_cameras
+ * writes the one derivative the group shares into every context of the call that has a sink; a camera whose image gradient
+ * is NULL adds nothing to it.  g4d_rasterize_backward, a fused backward without deformation params (the coarse stage) and
+ * n = 0 write 0.  The derivative is that of the forward as the kernels compute it: a time on a texel row of a time plane
+ * takes the row above it, and a time at or past the plane's border (t <= -1 or t >= 1) gives 0.  It is summed with atomics,
+ * so it is not bit-reproducible from run to run.  NULL turns it off.  Capture, zeroing and errors as for
+ * g4d_context_set_camera_grad: a backward on a capturing stream returns G4D_ERR_STATE before any launch while it is set, and
+ * a backward refused by its argument and state checks (e.g. after a G4D_CAM_NO_GRAD forward) leaves the sink untouched. */
+int g4d_context_set_time_grad(G4DContext *ctx, float *d_out);
 int g4d_workspace_freeze(G4DWorkspace *ws, int on);
 int g4d_workspace_graph_status(G4DWorkspace *ws, int sync, G4DGraphStatus *out);
 
