@@ -43,6 +43,7 @@ ABI_SYMBOLS = [
     "g4d_plane_regulation", "g4d_dist2_knn3", "g4d_adam_step", "g4d_render_forward_cameras", "g4d_render_backward_cameras",
     "g4d_context_set_time_source", "g4d_context_set_camera_grad", "g4d_workspace_freeze", "g4d_workspace_graph_status", "g4d_adam_scalars",
     "g4d_adam_step_device", "g4d_deform_forward_times", "g4d_deform_backward_times", "g4d_context_set_time_grad",
+    "g4d_context_set_depth_grad",
 ]
 
 fp = C.c_void_p   # device pointers travel as integers
@@ -170,6 +171,7 @@ def load():
         lib.g4d_context_set_time_source.argtypes = [C.c_void_p, fp]
         lib.g4d_context_set_camera_grad.argtypes = [C.c_void_p, fp]
         lib.g4d_context_set_time_grad.argtypes = [C.c_void_p, fp]
+        lib.g4d_context_set_depth_grad.argtypes = [C.c_void_p, fp]
         lib.g4d_workspace_freeze.argtypes = [C.c_void_p, C.c_int]
         lib.g4d_workspace_graph_status.argtypes = [C.c_void_p, C.c_int, C.POINTER(GraphStatus)]
         lib.g4d_adam_scalars.argtypes = [C.POINTER(AdamSegment), C.c_int32, C.c_float, C.c_float, C.c_int64, C.c_float,
@@ -365,6 +367,11 @@ class Context:
     def set_time_grad(self, d_out: Optional[int]):
         """Every backward on this context overwrites the device float at d_out with dL/d of its time (None: off)."""
         check(load().g4d_context_set_time_grad(self.handle, d_out), "g4d_context_set_time_grad")
+
+    def set_depth_grad(self, d_grad: Optional[int]):
+        """Every backward on this context also takes the gradient of its forward's depth image, the [1,H,W] device floats at
+        d_grad (None: off)."""
+        check(load().g4d_context_set_depth_grad(self.handle, d_grad), "g4d_context_set_depth_grad")
 
     def stats(self) -> Stats:
         s = Stats()

@@ -172,6 +172,7 @@ struct G4DContext {
     const float* time_src = nullptr;  // g4d_context_set_time_source (device; NULL: G4DCamera.time)
     float* cam_grad = nullptr;        // g4d_context_set_camera_grad (device, kCamGradFloats; NULL: no camera gradient)
     float* time_grad = nullptr;       // g4d_context_set_time_grad (device, 1 float; NULL: no time gradient)
+    const float* depth_grad = nullptr;   // g4d_context_set_depth_grad (device, [H,W] dL/d depth image; NULL: none)
     const void* bin_ctl = nullptr;    // device BinCtl of the last forward
     bool learned = false;             // R of an earlier exact forward is known (no-sync mode needs a learnt capacity)
     GeomBuffers g{};
@@ -612,13 +613,16 @@ template <class Sh, class T> Sh caller_sh(int m, bool split, T* dc, T* rest = nu
 // The gradient sinks of a backward on ctx[0, k), camera (g4d_context_set_camera_grad) and time (g4d_context_set_time_grad):
 // refused while capturing (a graph would keep writing a sink the context may since have dropped), else zeroed on st; the
 // backward adds into them, and a sink nothing adds into (a camera outside the loss, a backward without a deformation) keeps
-// the zeros.  Called before the backward's first launch.
+// the zeros.  A depth gradient (g4d_context_set_depth_grad) is refused while capturing for the same reason: a graph would
+// keep reading it.  Called before the backward's first launch.
 int zero_grad_sinks(G4DContext* const* ctx, int k, cudaStream_t st) {
     for (int i = 0; i < k; ++i) {
         if (ctx[i]->cam_grad && t_call.capturing)
             return fail(G4D_ERR_STATE, "cannot capture a backward on a context with a camera gradient set (g4d_context_set_camera_grad)");
         if (ctx[i]->time_grad && t_call.capturing)
             return fail(G4D_ERR_STATE, "cannot capture a backward on a context with a time gradient set (g4d_context_set_time_grad)");
+        if (ctx[i]->depth_grad && t_call.capturing)
+            return fail(G4D_ERR_STATE, "cannot capture a backward on a context with a depth gradient set (g4d_context_set_depth_grad)");
     }
     for (int i = 0; i < k; ++i) {
         if (ctx[i]->cam_grad) G4D_CUDA(cudaMemsetAsync(ctx[i]->cam_grad, 0, kCamGradFloats * sizeof(float), st));
@@ -665,12 +669,14 @@ struct CallFrame {
 };
 
 // The blend backward of the forward on c: dL/d(mean2D, conic, rgb, opacity) into c->gscratch (BlendGradLayout, zeroed here),
-// except that the opacity gradient lands in g_opacities (zeroed here) when it is set.  *gb: the scratch.  n = 0 runs nothing.
-int blend_backward(G4DContext* c, const G4DCamera* cam, int64_t n, const float* dL_dcolor, float* g_opacities, float** gb,
-                   cudaStream_t st) {
+// except that the opacity gradient lands in g_opacities (zeroed here) when it is set.  depth_block: the scratch has the depth
+// block, which takes dL/d(view-space depth) when c has a depth gradient and stays zero otherwise.  dL_dcolor may be NULL when
+// c has a depth gradient.  *gb: the scratch.  n = 0 runs nothing.
+int blend_backward(G4DContext* c, const G4DCamera* cam, int64_t n, const float* dL_dcolor, float* g_opacities, bool depth_block,
+                   float** gb, cudaStream_t st) {
     using L = BlendGradLayout;
     const size_t N = (size_t)(n > 0 ? n : 1);
-    const size_t floats = N * (g_opacities ? L::kOpacity : L::kFloats);
+    const size_t floats = N * (depth_block ? L::kDepthFloats : g_opacities ? L::kOpacity : L::kFloats);
     G4D_CUDA(c->gscratch.ensure(floats * 4 + 256));
     float* b = *gb = c->gscratch.as<float>();
     if (n == 0) return G4D_OK;
@@ -681,24 +687,25 @@ int blend_backward(G4DContext* c, const G4DCamera* cam, int64_t n, const float* 
         StageTimer tm(c, G4D_STAGE_BLEND_BWD, st);
         G4D_CUDA(launch_blend_backward(c->cam.as<CameraDev>(), c->grid_x, c->grid_y, c->g, c->b, c->im, dL_dcolor, b + L::kMean2D * N,
                                        b + L::kConic * N, g_opacities ? g_opacities : b + L::kOpacity * N, b + L::kRgb * N,
-                                       c->ws->warp_cull, st));
+                                       c->ws->warp_cull, c->depth_grad, c->depth_grad ? b + L::kDepth * N : nullptr, st));
     }
     return debug_sync(cam, st, "blend_backward");
 }
 
 // blend backward + per-Gaussian backward on `in`; opacity gradient lands in g_opacities (zeroed here); the camera's
-// gradient is added into c->cam_grad when it is set
+// gradient is added into c->cam_grad when it is set, and the depth image's gradient c->depth_grad is taken when it is set
 int raster_backward_stages(G4DContext* c, const G4DCamera* cam, int64_t n, const RasterInputs& in, const float* dL_dcolor,
                            float* g_means3D, float* g_means2D, const ShOut& g_sh, float* g_opacities, float* g_scales,
                            float* g_rotations, cudaStream_t st) {
     using L = BlendGradLayout;
     const size_t N = (size_t)n;
     float* gb;
-    const int rc = blend_backward(c, cam, n, dL_dcolor, g_opacities, &gb, st);
+    const int rc = blend_backward(c, cam, n, dL_dcolor, g_opacities, c->depth_grad != nullptr, &gb, st);
     if (rc != G4D_OK || n == 0) return rc;
     StageTimer tm(c, G4D_STAGE_GEOM_BWD, st);
     G4D_CUDA(launch_preprocess_backward(c->cam.as<CameraDev>(), n, in, c->g, gb + L::kMean2D * N, gb + L::kConic * N,
-                                        gb + L::kRgb * N, g_means3D, g_means2D, g_scales, g_rotations, g_sh, c->cam_grad, st));
+                                        gb + L::kRgb * N, g_means3D, g_means2D, g_scales, g_rotations, g_sh, c->cam_grad,
+                                        c->depth_grad ? gb + L::kDepth * N : nullptr, st));
     return debug_sync(cam, st, "preprocess_backward");
 }
 
@@ -1372,19 +1379,21 @@ int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCame
     if (n == 0) return G4D_OK;
     DeformedGrads d;
     if ((rc = deformed_grads(c0, n, gg, &d)) != G4D_OK) return rc;
-    // blend backward of every camera in the loss, each into its own scratch
+    // blend backward of every camera in the loss (an image or a depth gradient), each into its own scratch; when any camera
+    // has a depth gradient, every scratch has the depth block
     BackwardCameras bc{};
     CamGradSinks cs{};
-    bool cam_grads = false;
+    bool cam_grads = false, depth = false;
+    for (int i = 0; i < k; ++i) depth |= ctx[i]->depth_grad != nullptr;
     for (int i = 0; i < k; ++i) {
         G4DContext* c = ctx[i];
-        if (!dL_dcolor[i]) {
+        if (!dL_dcolor[i] && !c->depth_grad) {
             reset_stage_flags(c, G4D_STAGE_BLEND_BWD, G4D_STAGE_DEFORM_BWD);
             if (g_means2D && g_means2D[i]) G4D_CUDA(cudaMemsetAsync(g_means2D[i], 0, (size_t)n * 12, st));
             continue;
         }
         float* gb;
-        if ((rc = blend_backward(c, &cams[i], n, dL_dcolor[i], nullptr, &gb, st)) != G4D_OK) return rc;
+        if ((rc = blend_backward(c, &cams[i], n, dL_dcolor[i], nullptr, depth, &gb, st)) != G4D_OK) return rc;
         const int j = bc.count++;
         bc.cam[j] = c->cam.as<CameraDev>(); bc.radii[j] = c->g.radii; bc.clamped[j] = c->g.clamped; bc.grad[j] = gb;
         bc.g_means2D[j] = g_means2D ? g_means2D[i] : nullptr;
@@ -1394,7 +1403,7 @@ int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCame
     {
         StageTimer tm(c0, G4D_STAGE_GEOM_BWD, st);
         G4D_CUDA(launch_preprocess_backward_cameras(bc, n, deformed_inputs(c0, c0->fwd, g), d.xyz, d.sc, d.rot, d.op,
-                                                    fused_sh_sinks(c0, g, gg, d.sh), cam_grads ? &cs : nullptr, st));
+                                                    fused_sh_sinks(c0, g, gg, d.sh), cam_grads ? &cs : nullptr, depth, st));
     }
     if ((rc = debug_sync(&cams[0], st, "preprocess_backward_cameras")) != G4D_OK) return rc;
     // the network's backward, once, on the gradients summed over the cameras; the one dL/d(time) of the group goes to the
@@ -1537,6 +1546,12 @@ int g4d_context_set_camera_grad(G4DContext* c, float* d_out) {
 int g4d_context_set_time_grad(G4DContext* c, float* d_out) {
     if (!c) return fail(G4D_ERR_ARG, "context is NULL");
     c->time_grad = d_out;
+    return G4D_OK;
+}
+
+int g4d_context_set_depth_grad(G4DContext* c, const float* d_dL_ddepth) {
+    if (!c) return fail(G4D_ERR_ARG, "context is NULL");
+    c->depth_grad = d_dL_ddepth;
     return G4D_OK;
 }
 

@@ -305,22 +305,26 @@ cudaError_t launch_deform(const DeformDesc& d, int mode, const CameraDev* cam, i
                           int sm_count, cudaStream_t st, const TcWeights* tw = nullptr);
 
 // The per-Gaussian gradients of one blend backward in one float buffer, as blocks of N floats: d(mean2D) [2N] from block
-// kMean2D, d(conic) [3N] from kConic, d(rgb) [3N] from kRgb, d(opacity) [N] from kOpacity; kFloats blocks in all.
+// kMean2D, d(conic) [3N] from kConic, d(rgb) [3N] from kRgb, d(opacity) [N] from kOpacity; kFloats blocks in all.  A
+// backward with a depth gradient adds the block d(view-space depth) [N] at kDepth: kDepthFloats blocks in all.
 struct BlendGradLayout {
-    static constexpr int kMean2D = 0, kConic = 2, kRgb = 5, kOpacity = 8, kFloats = 9;
+    static constexpr int kMean2D = 0, kConic = 2, kRgb = 5, kOpacity = 8, kFloats = 9, kDepth = 9, kDepthFloats = 10;
 };
 
 cudaError_t launch_blend_forward(const CameraDev* cam, int grid_x, int grid_y, GeomBuffers g, BinBuffers b, ImageBuffers im,
                                  float* out_color, float* out_depth, int warp_cull, cudaStream_t st);
+// dL_ddepth != NULL: the depth image's gradient [H,W] is added too, and dL/d(view-space depth) of every Gaussian is added
+// into g_depth [N] (zeroed by the caller); dL_dcolor may then be NULL (a zero colour gradient)
 cudaError_t launch_blend_backward(const CameraDev* cam, int grid_x, int grid_y, GeomBuffers g, BinBuffers b, ImageBuffers im,
                                   const float* dL_dcolor, float* g_mean2D, float* g_conic, float* g_opacity, float* g_rgb,
-                                  int warp_cull, cudaStream_t st);
+                                  int warp_cull, const float* dL_ddepth, float* g_depth, cudaStream_t st);
 // per-Gaussian backward; g_cam != NULL: the camera's gradient (view[16], proj[16], campos[3]) is also added into g_cam,
-// which the caller zeroes first
+// which the caller zeroes first; g_depth != NULL: dL/d(view-space depth) [N] of the blend backward, carried to the mean
+// (and to the view matrix's depth row)
 cudaError_t launch_preprocess_backward(const CameraDev* cam, int64_t n, const RasterInputs& in, GeomBuffers g,
                                        const float* g_mean2D, const float* g_conic, const float* g_rgb, float* g_means3D,
                                        float* g_means2D_out, float* g_scales, float* g_rotations, const ShOut& g_sh,
-                                       float* g_cam, cudaStream_t st);
+                                       float* g_cam, const float* g_depth, cudaStream_t st);
 
 // Backward of the deformation network (g4d_backward.cu): the HexPlane gather (skipped when saved_feat holds the features
 // the forward gathered; order: its walk order), an engine -- the tensor-core kernels with the images tc, or the FFMA kernels
@@ -352,7 +356,7 @@ struct BackwardCameras {
     const CameraDev* cam[G4D_MAX_CAMERAS];
     const int32_t* radii[G4D_MAX_CAMERAS];
     const uint8_t* clamped[G4D_MAX_CAMERAS];
-    const float* grad[G4D_MAX_CAMERAS];    // the camera's blend backward, BlendGradLayout
+    const float* grad[G4D_MAX_CAMERAS];    // the camera's blend backward, BlendGradLayout (with the depth block when the call has one)
     float* g_means2D[G4D_MAX_CAMERAS];     // [N,3] screen-space gradient of the camera, or NULL
 };
 // the camera-gradient accumulators of those cameras (out[j]: camera j of BackwardCameras, kCamGradFloats floats, zeroed
@@ -362,10 +366,10 @@ struct CamGradSinks {
 };
 // per-Gaussian backward of all those cameras in one pass: the gradients w.r.t. means3D, scales, rotations, opacity and the
 // SH coefficients are summed over the cameras and written once (OVERWRITTEN); cs != NULL: each camera's gradient is also
-// added into its sink
+// added into its sink; depth: every camera's grad[] has the depth block (zeros for a camera without a depth gradient)
 cudaError_t launch_preprocess_backward_cameras(const BackwardCameras& bc, int64_t n, const RasterInputs& in, float* g_means3D,
                                                float* g_scales, float* g_rotations, float* g_opacities, const ShOut& g_sh,
-                                               const CamGradSinks* cs, cudaStream_t st);
+                                               const CamGradSinks* cs, bool depth, cudaStream_t st);
 
 // coarse stage of render(): the fused forward's tail without the deformation network (io as for launch_deform mode 1)
 cudaError_t launch_activate_preprocess(const CameraDev* cam, int64_t n, const DeformIO& io, cudaStream_t st);

@@ -266,11 +266,13 @@ struct CamGrad { float g[kCamGradFloats]; };
 G4D_HD constexpr bool cam_grad_read(int i) { return i < 16 ? (i & 3) != 3 : i < 32 ? (i & 3) != 2 : true; }
 
 // ShLoad as above; ShStore: void operator()(int coeff, int channel, float grad).  CAM: also the camera terms, into *cg
-// (every element written), in mul_rn / add_rn only: the GaussGrad outputs are those of CAM = false bit for bit.
-template <bool CAM = false, class ShLoad, class ShStore>
+// (every element written), in mul_rn / add_rn only: the GaussGrad outputs are those of CAM = false bit for bit.  DEPTH:
+// g_z = dL/d(view-space depth) joins dL/d p_view.z (the depth is row 2 of xform4x3): the mean gets g_z (view[2], view[6],
+// view[10]) and, with CAM, view[2, 6, 10, 14] get g_z (x, y, z, 1).
+template <bool CAM = false, bool DEPTH = false, class ShLoad, class ShStore>
 G4D_HD void gaussian_backward(const CameraDev& cam, Vec3 p, Vec3 scale, Quat rot, uint32_t clamped_bits,
                               const float g_mean2D[2], const float g_conic[3], const float g_rgb[3], ShLoad sh,
-                              ShStore sh_store, GaussGrad& out, CamGrad* cg = nullptr) {
+                              ShStore sh_store, GaussGrad& out, CamGrad* cg = nullptr, float g_z = 0.f) {
     const float* v = cam.view;
     const float* pm = cam.proj;
     float gm[3] = {0.f, 0.f, 0.f};
@@ -315,6 +317,7 @@ G4D_HD void gaussian_backward(const CameraDev& cam, Vec3 p, Vec3 scale, Quat rot
     float gtx = ax.clampx ? 0.f : -fx * itz2 * gJ02;
     float gty = ax.clampy ? 0.f : -fy * itz2 * gJ12;
     float gtz = -fx * itz2 * gJ00 - fy * itz2 * gJ11 + (2.f * fx * ax.tx) * itz3 * gJ02 + (2.f * fy * ax.ty) * itz3 * gJ12;
+    if constexpr (DEPTH) gtz += g_z;
     gm[0] += Wr[0][0] * gtx + Wr[1][0] * gty + Wr[2][0] * gtz;
     gm[1] += Wr[0][1] * gtx + Wr[1][1] * gty + Wr[2][1] * gtz;
     gm[2] += Wr[0][2] * gtx + Wr[1][2] * gty + Wr[2][2] * gtz;

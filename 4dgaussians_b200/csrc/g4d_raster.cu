@@ -1,6 +1,8 @@
 // g4d_raster.cu -- the per-tile front-to-back alpha compositing forward / back-to-front backward.
 // SURVEY.md Appendix A.3-A.4 (binning, A.2, lives in g4d_bin.cu).
 // Reference stage replaced: the CUDA rasterizer behind /root/reference/gaussian_renderer/__init__.py:120-128.
+#include <type_traits>
+
 #include "g4d_internal.h"
 #include "raster_cull.cuh"
 
@@ -139,19 +141,28 @@ G4D_D float warp_sum(float v) {
     return v;
 }
 
+// the colour b of a staged rec2 entry: the colour-only instance stages (b), the depth instance (b, depth)
+G4D_D float staged_b(float v) { return v; }
+G4D_D float staged_b(float2 v) { return v.x; }
+
 // Two pixels per thread as f32x2 lanes, like the forward: the per-pixel gradient arithmetic is one f2_* operation per pixel
 // PAIR, validity is a select instead of a branch, and power / alpha are formed exactly as the forward forms them (same
 // threshold decisions).
+// DEPTH: the depth image D = sum_i w_i z_i takes the gradient dL_ddepth [H,W] too: a depth accumulator beside the colour
+// ones adds (z_i - aD') dL/dD to dL/dalpha, and dL/dz_i = w_i dL/dD is reduced per warp into g_depth [N].  dL_dcolor may
+// then be NULL (a zero colour gradient).  With DEPTH off the two trailing arguments are not read.
+template <bool DEPTH>
 __global__ void __launch_bounds__(kTilePixels / 2)
 blend_backward_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, const uint32_t* __restrict__ ids,
                       const uint2* __restrict__ ranges, const float* __restrict__ final_T,
                       const uint32_t* __restrict__ n_contrib, const float* __restrict__ dL_dcolor,
                       float* __restrict__ g_mean2D, float* __restrict__ g_conic, float* __restrict__ g_opacity,
-                      float* __restrict__ g_rgb, int warp_cull) {
+                      float* __restrict__ g_rgb, int warp_cull, const float* __restrict__ dL_ddepth,
+                      float* __restrict__ g_depth) {
     constexpr int PPT = 2, NT = kTilePixels / PPT;
     __shared__ float4 s0[kTilePixels];
     __shared__ float4 s1[kTilePixels];
-    __shared__ float s2[kTilePixels];
+    __shared__ std::conditional_t<DEPTH, float2, float> s2[kTilePixels];
     __shared__ uint32_t sid[kTilePixels];
     const int H = cam->H, W = cam->W;
     const int tile = blockIdx.y * gridDim.x + blockIdx.x;
@@ -171,9 +182,12 @@ blend_backward_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, const ui
     const float2 Tfin = make_float2(in0 ? final_T[pix0] : 0.f, in1 ? final_T[pix1] : 0.f);
     float2 T = Tfin;
     const int last0 = in0 ? (int)n_contrib[pix0] : 0, last1 = in1 ? (int)n_contrib[pix1] : 0;
-    const float2 dp0 = make_float2(in0 ? dL_dcolor[pix0] : 0.f, in1 ? dL_dcolor[pix1] : 0.f);
-    const float2 dp1 = make_float2(in0 ? dL_dcolor[hw + pix0] : 0.f, in1 ? dL_dcolor[hw + pix1] : 0.f);
-    const float2 dp2 = make_float2(in0 ? dL_dcolor[2 * hw + pix0] : 0.f, in1 ? dL_dcolor[2 * hw + pix1] : 0.f);
+    const bool c0in = in0 && (!DEPTH || dL_dcolor), c1in = in1 && (!DEPTH || dL_dcolor);
+    const float2 dp0 = make_float2(c0in ? dL_dcolor[pix0] : 0.f, c1in ? dL_dcolor[pix1] : 0.f);
+    const float2 dp1 = make_float2(c0in ? dL_dcolor[hw + pix0] : 0.f, c1in ? dL_dcolor[hw + pix1] : 0.f);
+    const float2 dp2 = make_float2(c0in ? dL_dcolor[2 * hw + pix0] : 0.f, c1in ? dL_dcolor[2 * hw + pix1] : 0.f);
+    float2 dpD = make_float2(0.f, 0.f), aD = dpD, lD = dpD;      // DEPTH: dL/dD, depth accumulator, last depth
+    if constexpr (DEPTH) dpD = make_float2(in0 ? dL_ddepth[pix0] : 0.f, in1 ? dL_ddepth[pix1] : 0.f);
     const float2 bgdot = make_float2(cam->bg[0] * dp0.x + cam->bg[1] * dp1.x + cam->bg[2] * dp2.x,
                                      cam->bg[0] * dp0.y + cam->bg[1] * dp1.y + cam->bg[2] * dp2.y);
     const float2 nTfin = make_float2(-Tfin.x, -Tfin.y);
@@ -210,7 +224,8 @@ blend_backward_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, const ui
                 sid[slot] = id;
                 s0[slot] = g.rec0[id];
                 s1[slot] = g.rec1[id];
-                s2[slot] = g.rec2[id].x;
+                if constexpr (DEPTH) s2[slot] = g.rec2[id];
+                else s2[slot] = g.rec2[id].x;
             }
         }
         __syncthreads();
@@ -241,7 +256,7 @@ blend_backward_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, const ui
                 al.x = fminf(kAlphaMax, al.x); al.y = fminf(kAlphaMax, al.y);
                 const bool v0 = lpos < last0 && pw.x <= 0.f && al.x >= kAlphaMin, v1 = lpos < last1 && pw.y <= 0.f && al.y >= kAlphaMin;
                 if (!__any_sync(0xffffffffu, v0 || v1)) continue;
-                const float c0 = b.z, c1 = b.w, c2 = s2[j];
+                const float c0 = b.z, c1 = b.w, c2 = staged_b(s2[j]);
                 const float2 om = f2_add(one2, make_float2(-al.x, -al.y));
                 const float2 ra = make_float2(__fdividef(1.f, om.x), __fdividef(1.f, om.y));   // alpha <= 0.99
                 const float2 Tn = f2_mul(T, ra);
@@ -253,6 +268,13 @@ blend_backward_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, const ui
                 float2 dLa = f2_mul(f2_add(make_float2(c0, c0), make_float2(-a0n.x, -a0n.y)), dp0);
                 dLa = f2_fma(f2_add(make_float2(c1, c1), make_float2(-a1n.x, -a1n.y)), dp1, dLa);
                 dLa = f2_fma(f2_add(make_float2(c2, c2), make_float2(-a2n.x, -a2n.y)), dp2, dLa);
+                float z = 0.f;
+                float2 aDn = aD;
+                if constexpr (DEPTH) {     // no background term: depth has no bgdot analogue
+                    z = s2[j].y;
+                    aDn = f2_fma(la, lD, f2_mul(oml, aD));
+                    dLa = f2_fma(f2_add(make_float2(z, z), make_float2(-aDn.x, -aDn.y)), dpD, dLa);
+                }
                 dLa = f2_mul(dLa, Tn);
                 dLa = f2_fma(f2_mul(nTfin, ra), bgdot, dLa);
                 // commit the per-pixel state of the pixels this instance is valid for; mask the contributions of the others
@@ -264,6 +286,10 @@ blend_backward_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, const ui
                 lc1.x = v0 ? c1 : lc1.x; lc1.y = v1 ? c1 : lc1.y;
                 lc2.x = v0 ? c2 : lc2.x; lc2.y = v1 ? c2 : lc2.y;
                 la.x = v0 ? al.x : la.x; la.y = v1 ? al.y : la.y;
+                if constexpr (DEPTH) {
+                    aD.x = v0 ? aDn.x : aD.x; aD.y = v1 ? aDn.y : aD.y;
+                    lD.x = v0 ? z : lD.x; lD.y = v1 ? z : lD.y;
+                }
                 w.x = v0 ? w.x : 0.f; w.y = v1 ? w.y : 0.f;
                 dLa.x = v0 ? dLa.x : 0.f; dLa.y = v1 ? dLa.y : 0.f;
                 float v[8];
@@ -306,6 +332,11 @@ blend_backward_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, const ui
                     const uint32_t id = sid[j];
                     atomicAdd(red_base + red_stride * id, lane == 1 ? v_op : x);
                 }
+                if constexpr (DEPTH) {     // the tenth value: dL/dz of the instance, added by lane 2
+                    const float2 pz = f2_mul(w, dpD);
+                    const float v_z = warp_sum(pz.x + pz.y);
+                    if (lane == 2) atomicAdd(g_depth + sid[j], v_z);
+                }
             }
         }
     }
@@ -313,10 +344,11 @@ blend_backward_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, const ui
 
 cudaError_t launch_blend_backward(const CameraDev* cam, int grid_x, int grid_y, GeomBuffers g, BinBuffers b, ImageBuffers im,
                                   const float* dL_dcolor, float* g_mean2D, float* g_conic, float* g_opacity, float* g_rgb,
-                                  int warp_cull, cudaStream_t st) {
+                                  int warp_cull, const float* dL_ddepth, float* g_depth, cudaStream_t st) {
     if (grid_x * grid_y == 0) return cudaSuccess;
-    blend_backward_kernel<<<dim3(grid_x, grid_y), kTilePixels / 2, 0, st>>>(cam, g, b.ids_sorted, b.ranges, im.final_T, im.n_contrib,
-                                                                             dL_dcolor, g_mean2D, g_conic, g_opacity, g_rgb, warp_cull);
+    auto kernel = dL_ddepth ? blend_backward_kernel<true> : blend_backward_kernel<false>;
+    kernel<<<dim3(grid_x, grid_y), kTilePixels / 2, 0, st>>>(cam, g, b.ids_sorted, b.ranges, im.final_T, im.n_contrib, dL_dcolor,
+                                                             g_mean2D, g_conic, g_opacity, g_rgb, warp_cull, dL_ddepth, g_depth);
     return cudaGetLastError();
 }
 

@@ -80,20 +80,24 @@ def camera_grad_leaves(rss):
 class CameraGradSinks:
     """One [k, 35] float32 device buffer whose row i the backward on context ``ctxs[i]`` overwrites with its camera's
     gradient, for the cameras named in ``spec``; with ``time``, one device float that the backward on ``ctxs[0]``
-    overwrites with dL/d(time) (g4d_context_set_time_grad).  The contexts' pointers are cleared again on exit (they return
-    to a pool)."""
+    overwrites with dL/d(time) (g4d_context_set_time_grad); ``depths[i]``, when given and not None, the gradient of camera
+    i's depth image (contiguous fp32 CUDA, [H*W]) that the backward on ``ctxs[i]`` takes (g4d_context_set_depth_grad).  The
+    contexts' pointers are cleared again on exit (they return to a pool)."""
 
-    def __init__(self, spec, ctxs, dev, time=False):
+    def __init__(self, spec, ctxs, dev, time=False, depths=()):
         self.cams = sorted({i for i, _ in spec})
         self.ctxs = ctxs
         self.buf = torch.empty(len(ctxs), 35, device=dev, dtype=torch.float32) if spec else None
         self.tbuf = torch.empty(1, device=dev, dtype=torch.float32) if time else None
+        self.depths = [(i, d) for i, d in enumerate(depths) if d is not None]
 
     def __enter__(self):
         for i in self.cams:
             self.ctxs[i].set_camera_grad(self.buf[i].data_ptr())
         if self.tbuf is not None:
             self.ctxs[0].set_time_grad(self.tbuf.data_ptr())
+        for i, d in self.depths:
+            self.ctxs[i].set_depth_grad(d.data_ptr())
         return self
 
     def __exit__(self, *exc):
@@ -101,6 +105,8 @@ class CameraGradSinks:
             self.ctxs[i].set_camera_grad(None)
         if self.tbuf is not None:
             self.ctxs[0].set_time_grad(None)
+        for i, _ in self.depths:
+            self.ctxs[i].set_depth_grad(None)
         return False
 
     def grads(self, spec, metas):
@@ -139,7 +145,8 @@ class _ContextLease:
 
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, raster_settings, cam_spec, *cam_leaves):
+    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, raster_settings, differentiable_depth, cam_spec,
+                *cam_leaves):
         lib = _lib.load()
         dev = means3D.device
         n = means3D.shape[0]
@@ -166,17 +173,22 @@ class _RasterizeGaussians(torch.autograd.Function):
         ctx.lease = lease
         ctx.n, ctx.m = n, m
         ctx.save_for_backward(m3, shc, op, sc, ro)
-        ctx.mark_non_differentiable(radii, depth)
+        ctx.mark_non_differentiable(*((radii,) if differentiable_depth else (radii, depth)))
+        ctx.set_materialize_grads(False)         # a depth image outside the loss arrives as None: no depth gradient is set
         return color, radii, depth
 
     @staticmethod
-    def backward(ctx, grad_color, _grad_radii, _grad_depth):
+    def backward(ctx, grad_color, _grad_radii, grad_depth):
         lib = _lib.load()
         m3, shc, op, sc, ro = ctx.saved_tensors
         dev = m3.device
         n = ctx.n
         rs = ctx.raster_settings
-        gcol = _lib.cuda_f32(grad_color, "grad_out_color", 3 * int(rs.image_height) * int(rs.image_width))
+        hw = int(rs.image_height) * int(rs.image_width)
+        if grad_color is None:      # a depth-only loss: the backward takes an image gradient
+            grad_color = torch.zeros(3 * hw, device=dev)
+        gcol = _lib.cuda_f32(grad_color, "grad_out_color", 3 * hw)
+        gdep = _lib.cuda_f32(grad_depth, "grad_out_depth", hw)
         g_means3D = torch.empty(n, 3, device=dev)
         g_means2D = torch.empty(n, 3, device=dev)
         g_sh = torch.empty(n, ctx.m, 3, device=dev)
@@ -188,7 +200,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         lease = ctx.lease
         if lease is None or lease.ctx is None:
             raise RuntimeError("rasterizer backward called twice (context already released)")
-        sinks = CameraGradSinks(ctx.cam_spec, [lease.ctx], dev)
+        sinks = CameraGradSinks(ctx.cam_spec, [lease.ctx], dev, depths=(gdep,))
         with torch.cuda.device(dev), sinks:
             _lib.check(lib.g4d_rasterize_backward(lease.ctx.handle, C.byref(cam), n, m3.data_ptr(), shc.data_ptr(), op.data_ptr(),
                                                   sc.data_ptr(), ro.data_ptr(), gcol.data_ptr(), g_means3D.data_ptr(),
@@ -197,13 +209,18 @@ class _RasterizeGaussians(torch.autograd.Function):
         lease.release()
         ctx.lease = None
         cam_grads = sinks.grads(ctx.cam_spec, ctx.cam_meta) if ctx.cam_spec else ()
-        return (g_means3D, g_means2D, g_sh, g_op, g_sc, g_ro, None, None) + cam_grads
+        return (g_means3D, g_means2D, g_sh, g_op, g_sc, g_ro, None, None, None) + cam_grads
 
 
 class GaussianRasterizer(nn.Module):
-    def __init__(self, raster_settings: GaussianRasterizationSettings):
+    """differentiable_depth: the depth image it returns takes a gradient too (render() and render_cameras() render theirs
+    so).  Off by default the depth is a tensor without grad, as diff_gaussian_rasterization's callers read it (a tensor
+    that requires grad refuses .numpy())."""
+
+    def __init__(self, raster_settings: GaussianRasterizationSettings, differentiable_depth: bool = False):
         super().__init__()
         self.raster_settings = raster_settings
+        self.differentiable_depth = bool(differentiable_depth)
 
     def markVisible(self, positions):
         raise NotImplementedError("markVisible is not used by 4DGaussians (SURVEY.md §8b) and is not part of the g4d path")
@@ -221,4 +238,5 @@ class GaussianRasterizer(nn.Module):
                                       "(gaussian_renderer/__init__.py:74-78,105-116) and are not provided")
         # the settings' viewmatrix / projmatrix / campos that require grad join the autograd graph as extra inputs
         cam_spec, cam_leaves = camera_grad_leaves((rs,))
-        return _RasterizeGaussians.apply(means3D, means2D, shs, opacities, scales, rotations, rs, cam_spec, *cam_leaves)
+        return _RasterizeGaussians.apply(means3D, means2D, shs, opacities, scales, rotations, rs, self.differentiable_depth,
+                                         cam_spec, *cam_leaves)

@@ -13,7 +13,7 @@ is its one-camera case, which takes the single-camera entry points.
 
 Both differentiate the camera tensors that require grad (``rasterizer.camera_grad_leaves``) and the camera's time when it
 is a tensor that requires grad (``time_grad_leaf``): dL/dt comes from the network's backward, for learning per-camera time
-offsets.
+offsets.  The ``depth`` maps they return are differentiable too, for depth supervision.
 """
 from __future__ import annotations
 
@@ -130,8 +130,9 @@ class _FusedRender(torch.autograd.Function):
         # host ~0.3 ms per view, during which the GPU has nothing queued behind the forward's last kernel
         ctx.cstructs = cstructs
         ctx.save_for_backward(*saved)
-        ctx.mark_non_differentiable(*radii, *depths)
-        ctx.set_materialize_grads(False)         # an image outside the loss arrives as None: its blend backward is skipped
+        ctx.mark_non_differentiable(*radii)
+        # an image or depth map outside the loss arrives as None: a camera with neither has its blend backward skipped
+        ctx.set_materialize_grads(False)
         return tuple(colors) + tuple(radii) + tuple(depths)
 
     @staticmethod
@@ -146,6 +147,8 @@ class _FusedRender(torch.autograd.Function):
                                "render_cameras backward called twice (contexts already released)")
         gcols = [None if gc is None else _lib.cuda_f32(gc, "grad_out_color", 3 * int(rs.image_height) * int(rs.image_width))
                  for gc, rs in zip(grads[:k], rss)]
+        gdeps = [_lib.cuda_f32(gd, "grad_out_depth", int(rs.image_height) * int(rs.image_width))
+                 for gd, rs in zip(grads[2 * k:], rss)]
         cams, prm, g, keep, version, handles = ctx.cstructs
         if module is not None and version != module._param_version:      # another forward ran since: take the current key
             keep = []
@@ -163,7 +166,8 @@ class _FusedRender(torch.autograd.Function):
         gm2 = [flat[(end + 3 * i) * npad:(end + 3 * i) * npad + 3 * n].view(n, 3) for i in range(k)]
         gg = _lib.GaussianGrads(gx.data_ptr(), gs.data_ptr(), gr.data_ptr(), go.data_ptr(), gdc.data_ptr(), grest.data_ptr(),
                                 gm2[0].data_ptr() if k == 1 else None)
-        sinks = CameraGradSinks(ctx.cam_spec, [lease.ctx for lease in leases], dev, time=ctx.time_meta is not None)
+        sinks = CameraGradSinks(ctx.cam_spec, [lease.ctx for lease in leases], dev, time=ctx.time_meta is not None,
+                                depths=gdeps)
         with torch.cuda.device(dev), sinks:
             if k == 1:
                 if gcols[0] is None:        # the single-camera backward takes an image gradient
@@ -265,9 +269,9 @@ def _render(viewpoint_cameras, pc, pipe, bg_color, scaling_modifier, override_co
         opac, scales, rots = pc.opacity_activation(op), pc.scaling_activation(sc), pc.rotation_activation(rot)
         images, radii, depths = [], [], []
         for rs, p in zip(rss, points):
-            img, rad, dep = GaussianRasterizer(raster_settings=rs)(means3D=m3, means2D=p, shs=shs, colors_precomp=None,
-                                                                   opacities=opac, scales=scales, rotations=rots,
-                                                                   cov3D_precomp=None)
+            img, rad, dep = GaussianRasterizer(raster_settings=rs, differentiable_depth=True)(
+                means3D=m3, means2D=p, shs=shs, colors_precomp=None, opacities=opac, scales=scales, rotations=rots,
+                cov3D_precomp=None)
             images.append(img); radii.append(rad); depths.append(dep)
     return [{"render": img, "viewspace_points": p, "visibility_filter": rad > 0, "radii": rad, "depth": dep}
             for img, p, rad, dep in zip(images, points, radii, depths)]

@@ -213,7 +213,8 @@ int g4d_render_backward(G4DContext *ctx, const G4DCamera *cam, const G4DDeformPa
  * runs ONCE: camera 0 runs the g4d_render_forward sequence on ctx[0] (k == 1 is g4d_render_forward), cameras 1..k-1 are
  * projected from ctx[0]'s deformed, activated tensors and binned / blended on their own contexts.  out_color[i] [3,H_i,W_i],
  * out_depth[i] [1,H_i,W_i], out_radii[i] [N].  G4D_CAM_NO_GRAD on cams[0] skips the state only the backward reads.
- * The backward takes the same k contexts: dL_dcolor[i] == NULL leaves camera i out of the loss; gg receives the per-Gaussian
+ * The backward takes the same k contexts: dL_dcolor[i] == NULL leaves camera i out of the loss unless ctx[i] has a depth
+ * gradient (g4d_context_set_depth_grad), which then makes dL_dcolor[i] == NULL a zero image gradient; gg receives the per-Gaussian
  * gradients summed over the cameras (OVERWRITTEN; gg->means2D must be NULL), g_means2D[i] ([N,3], may be NULL) camera i's
  * screen-space gradient; the network's backward runs once, ACCUMULATED into pgrads.  It returns G4D_ERR_STATE when any of
  * the contexts ran another forward since; g4d_render_backward / g4d_rasterize_backward refuse a member context. */
@@ -393,9 +394,10 @@ int g4d_context_set_time_source(G4DContext *ctx, const float *d_time);
  * g4d_context_set_camera_grad: while d_out (device, 35 floats) is set, every backward on ctx (g4d_rasterize_backward,
  * g4d_render_backward, and g4d_render_backward_cameras for the camera ctx holds) OVERWRITES it with dL/d of this camera:
  * view[16], proj[16], campos[3], each in the element order of G4DCamera.viewmatrix / projmatrix / campos.  Elements the
- * forward does not read (view 3, 7, 11, 15; proj 2, 6, 10, 14) are 0, and so is every element of a camera whose image
- * gradient is NULL.  The derivative is that of the forward as the kernels compute it: a guard-band-clamped t.x / t.y is a
- * constant, alpha's 0.99 clamp passes the gradient, a clamped colour channel and the depth image pass none.  NULL turns it
+ * forward does not read (view 3, 7, 11, 15; proj 2, 6, 10, 14) are 0, and so is every element of a camera outside the loss
+ * (image gradient NULL and no depth gradient).  The derivative is that of the forward as the kernels compute it: a
+ * guard-band-clamped t.x / t.y is a constant, alpha's 0.99 clamp passes the gradient, a clamped colour channel passes none,
+ * and the depth image passes its gradient when the context has one (g4d_context_set_depth_grad).  NULL turns it
  * off.  A backward on a stream that is capturing returns G4D_ERR_STATE before any launch while the pointer is set.  The
  * sink is zeroed on the stream after the backward's argument and state checks and before its first kernel: a backward that
  * returns an error after that point (a CUDA error, a buffer that cannot grow) leaves it zeroed or partly summed, not as it
@@ -405,14 +407,26 @@ int g4d_context_set_camera_grad(G4DContext *ctx, float *d_out);
 /* ---- time gradients ------------------------------------------------------------------------------------------------
  * g4d_context_set_time_grad: while d_out (device, 1 float) is set, every backward on ctx OVERWRITES d_out[0] with dL/d of
  * the call's time (G4DCamera.time, or the value read through g4d_context_set_time_source).  g4d_render_backward_cameras
- * writes the one derivative the group shares into every context of the call that has a sink; a camera whose image gradient
- * is NULL adds nothing to it.  g4d_rasterize_backward, a fused backward without deformation params (the coarse stage) and
+ * writes the one derivative the group shares into every context of the call that has a sink; a camera outside the loss (image
+ * gradient NULL and no depth gradient) adds nothing to it.  g4d_rasterize_backward, a fused backward without deformation params (the coarse stage) and
  * n = 0 write 0.  The derivative is that of the forward as the kernels compute it: a time on a texel row of a time plane
  * takes the row above it, and a time at or past the plane's border (t <= -1 or t >= 1) gives 0.  It is summed with atomics,
  * so it is not bit-reproducible from run to run.  NULL turns it off.  Capture, zeroing and errors as for
  * g4d_context_set_camera_grad: a backward on a capturing stream returns G4D_ERR_STATE before any launch while it is set, and
  * a backward refused by its argument and state checks (e.g. after a G4D_CAM_NO_GRAD forward) leaves the sink untouched. */
 int g4d_context_set_time_grad(G4DContext *ctx, float *d_out);
+
+/* ---- depth gradients -----------------------------------------------------------------------------------------------
+ * g4d_context_set_depth_grad: while d_dL_ddepth (device, [1,H,W] floats of the forward's image size) is set, every backward on
+ * ctx (g4d_rasterize_backward, g4d_render_backward, and g4d_render_backward_cameras for the camera ctx holds) adds the
+ * gradient of the forward's depth image out_depth to every gradient it computes, as if the loss had been differentiated
+ * w.r.t. out_depth as well.  The depth image is D = sum_i w_i z_i over the pixel's colour instances (w_i = alpha_i T_i, the
+ * colour weights; z_i the Gaussian's view-space depth; no background term, no normalisation).  The derivative is that of the
+ * forward as the kernels compute it, with the conventions of the colour's (alpha's 0.99 clamp passes the gradient, only
+ * Gaussians with radius > 0 get one).  It is summed with atomics, so it is not bit-reproducible from run to run.  The buffer
+ * is read, never written.  NULL turns it off; with no pointer set a backward runs exactly as it did before this entry point
+ * existed.  A backward on a capturing stream returns G4D_ERR_STATE before any launch while it is set. */
+int g4d_context_set_depth_grad(G4DContext *ctx, const float *d_dL_ddepth);
 int g4d_workspace_freeze(G4DWorkspace *ws, int on);
 int g4d_workspace_graph_status(G4DWorkspace *ws, int sync, G4DGraphStatus *out);
 
