@@ -173,6 +173,8 @@ struct G4DContext {
     float* cam_grad = nullptr;        // g4d_context_set_camera_grad (device, kCamGradFloats; NULL: no camera gradient)
     float* time_grad = nullptr;       // g4d_context_set_time_grad (device, 1 float; NULL: no time gradient)
     const float* depth_grad = nullptr;   // g4d_context_set_depth_grad (device, [H,W] dL/d depth image; NULL: none)
+    float* alpha_out = nullptr;          // g4d_context_set_alpha_out (device, [H,W] alpha image of every forward; NULL: none)
+    const float* alpha_grad = nullptr;   // g4d_context_set_alpha_grad (device, [H,W] dL/d alpha image; NULL: none)
     const void* bin_ctl = nullptr;    // device BinCtl of the last forward
     bool learned = false;             // R of an earlier exact forward is known (no-sync mode needs a learnt capacity)
     GeomBuffers g{};
@@ -590,7 +592,8 @@ int bin_and_blend(G4DContext* c, const G4DCamera* cam, int64_t n, float* out_col
     if ((rc = debug_sync(cam, st, "binning")) != G4D_OK) return rc;
     {
         StageTimer tm(c, G4D_STAGE_BLEND, st);
-        G4D_CUDA(launch_blend_forward(dcam, c->grid_x, c->grid_y, c->g, c->b, c->im, out_color, out_depth, ws->warp_cull, st));
+        G4D_CUDA(launch_blend_forward(dcam, c->grid_x, c->grid_y, c->g, c->b, c->im, out_color, out_depth, ws->warp_cull,
+                                      c->alpha_out, st));
     }
     if (readback && t_call.capturing) {
         G4D_CUDA(launch_record_overflow(static_cast<const BinCtl*>(c->bin_ctl), cap_place, ws->pinned->overflow, st));
@@ -613,8 +616,8 @@ template <class Sh, class T> Sh caller_sh(int m, bool split, T* dc, T* rest = nu
 // The gradient sinks of a backward on ctx[0, k), camera (g4d_context_set_camera_grad) and time (g4d_context_set_time_grad):
 // refused while capturing (a graph would keep writing a sink the context may since have dropped), else zeroed on st; the
 // backward adds into them, and a sink nothing adds into (a camera outside the loss, a backward without a deformation) keeps
-// the zeros.  A depth gradient (g4d_context_set_depth_grad) is refused while capturing for the same reason: a graph would
-// keep reading it.  Called before the backward's first launch.
+// the zeros.  A depth or alpha gradient (g4d_context_set_depth_grad / _alpha_grad) is refused while capturing for the same
+// reason: a graph would keep reading it.  Called before the backward's first launch.
 int zero_grad_sinks(G4DContext* const* ctx, int k, cudaStream_t st) {
     for (int i = 0; i < k; ++i) {
         if (ctx[i]->cam_grad && t_call.capturing)
@@ -623,6 +626,8 @@ int zero_grad_sinks(G4DContext* const* ctx, int k, cudaStream_t st) {
             return fail(G4D_ERR_STATE, "cannot capture a backward on a context with a time gradient set (g4d_context_set_time_grad)");
         if (ctx[i]->depth_grad && t_call.capturing)
             return fail(G4D_ERR_STATE, "cannot capture a backward on a context with a depth gradient set (g4d_context_set_depth_grad)");
+        if (ctx[i]->alpha_grad && t_call.capturing)
+            return fail(G4D_ERR_STATE, "cannot capture a backward on a context with an alpha gradient set (g4d_context_set_alpha_grad)");
     }
     for (int i = 0; i < k; ++i) {
         if (ctx[i]->cam_grad) G4D_CUDA(cudaMemsetAsync(ctx[i]->cam_grad, 0, kCamGradFloats * sizeof(float), st));
@@ -670,8 +675,8 @@ struct CallFrame {
 
 // The blend backward of the forward on c: dL/d(mean2D, conic, rgb, opacity) into c->gscratch (BlendGradLayout, zeroed here),
 // except that the opacity gradient lands in g_opacities (zeroed here) when it is set.  depth_block: the scratch has the depth
-// block, which takes dL/d(view-space depth) when c has a depth gradient and stays zero otherwise.  dL_dcolor may be NULL when
-// c has a depth gradient.  *gb: the scratch.  n = 0 runs nothing.
+// block, which takes dL/d(view-space depth) when c has a depth gradient and stays zero otherwise.  c's alpha gradient, when
+// set, is taken too.  dL_dcolor may be NULL when c has a depth or an alpha gradient.  *gb: the scratch.  n = 0 runs nothing.
 int blend_backward(G4DContext* c, const G4DCamera* cam, int64_t n, const float* dL_dcolor, float* g_opacities, bool depth_block,
                    float** gb, cudaStream_t st) {
     using L = BlendGradLayout;
@@ -687,13 +692,15 @@ int blend_backward(G4DContext* c, const G4DCamera* cam, int64_t n, const float* 
         StageTimer tm(c, G4D_STAGE_BLEND_BWD, st);
         G4D_CUDA(launch_blend_backward(c->cam.as<CameraDev>(), c->grid_x, c->grid_y, c->g, c->b, c->im, dL_dcolor, b + L::kMean2D * N,
                                        b + L::kConic * N, g_opacities ? g_opacities : b + L::kOpacity * N, b + L::kRgb * N,
-                                       c->ws->warp_cull, c->depth_grad, c->depth_grad ? b + L::kDepth * N : nullptr, st));
+                                       c->ws->warp_cull, c->depth_grad, c->depth_grad ? b + L::kDepth * N : nullptr,
+                                       c->alpha_grad, st));
     }
     return debug_sync(cam, st, "blend_backward");
 }
 
 // blend backward + per-Gaussian backward on `in`; opacity gradient lands in g_opacities (zeroed here); the camera's
-// gradient is added into c->cam_grad when it is set, and the depth image's gradient c->depth_grad is taken when it is set
+// gradient is added into c->cam_grad when it is set, and the depth and alpha images' gradients c->depth_grad / c->alpha_grad
+// are taken when they are set
 int raster_backward_stages(G4DContext* c, const G4DCamera* cam, int64_t n, const RasterInputs& in, const float* dL_dcolor,
                            float* g_means3D, float* g_means2D, const ShOut& g_sh, float* g_opacities, float* g_scales,
                            float* g_rotations, cudaStream_t st) {
@@ -1379,7 +1386,7 @@ int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCame
     if (n == 0) return G4D_OK;
     DeformedGrads d;
     if ((rc = deformed_grads(c0, n, gg, &d)) != G4D_OK) return rc;
-    // blend backward of every camera in the loss (an image or a depth gradient), each into its own scratch; when any camera
+    // blend backward of every camera in the loss (an image, a depth or an alpha gradient), each into its own scratch; when any camera
     // has a depth gradient, every scratch has the depth block
     BackwardCameras bc{};
     CamGradSinks cs{};
@@ -1387,7 +1394,7 @@ int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCame
     for (int i = 0; i < k; ++i) depth |= ctx[i]->depth_grad != nullptr;
     for (int i = 0; i < k; ++i) {
         G4DContext* c = ctx[i];
-        if (!dL_dcolor[i] && !c->depth_grad) {
+        if (!dL_dcolor[i] && !c->depth_grad && !c->alpha_grad) {
             reset_stage_flags(c, G4D_STAGE_BLEND_BWD, G4D_STAGE_DEFORM_BWD);
             if (g_means2D && g_means2D[i]) G4D_CUDA(cudaMemsetAsync(g_means2D[i], 0, (size_t)n * 12, st));
             continue;
@@ -1552,6 +1559,18 @@ int g4d_context_set_time_grad(G4DContext* c, float* d_out) {
 int g4d_context_set_depth_grad(G4DContext* c, const float* d_dL_ddepth) {
     if (!c) return fail(G4D_ERR_ARG, "context is NULL");
     c->depth_grad = d_dL_ddepth;
+    return G4D_OK;
+}
+
+int g4d_context_set_alpha_out(G4DContext* c, float* d_out) {
+    if (!c) return fail(G4D_ERR_ARG, "context is NULL");
+    c->alpha_out = d_out;
+    return G4D_OK;
+}
+
+int g4d_context_set_alpha_grad(G4DContext* c, const float* d_dL_dalpha) {
+    if (!c) return fail(G4D_ERR_ARG, "context is NULL");
+    c->alpha_grad = d_dL_dalpha;
     return G4D_OK;
 }
 

@@ -312,12 +312,14 @@ struct BlendGradLayout {
 };
 
 cudaError_t launch_blend_forward(const CameraDev* cam, int grid_x, int grid_y, GeomBuffers g, BinBuffers b, ImageBuffers im,
-                                 float* out_color, float* out_depth, int warp_cull, cudaStream_t st);
+                                 float* out_color, float* out_depth, int warp_cull, float* out_alpha, cudaStream_t st);
 // dL_ddepth != NULL: the depth image's gradient [H,W] is added too, and dL/d(view-space depth) of every Gaussian is added
-// into g_depth [N] (zeroed by the caller); dL_dcolor may then be NULL (a zero colour gradient)
+// into g_depth [N] (zeroed by the caller).  dL_dalpha != NULL: the alpha image's gradient [H,W] is added too.  dL_dcolor
+// may be NULL (a zero colour gradient) when either is set.
 cudaError_t launch_blend_backward(const CameraDev* cam, int grid_x, int grid_y, GeomBuffers g, BinBuffers b, ImageBuffers im,
                                   const float* dL_dcolor, float* g_mean2D, float* g_conic, float* g_opacity, float* g_rgb,
-                                  int warp_cull, const float* dL_ddepth, float* g_depth, cudaStream_t st);
+                                  int warp_cull, const float* dL_ddepth, float* g_depth, const float* dL_dalpha,
+                                  cudaStream_t st);
 // per-Gaussian backward; g_cam != NULL: the camera's gradient (view[16], proj[16], campos[3]) is also added into g_cam,
 // which the caller zeroes first; g_depth != NULL: dL/d(view-space depth) [N] of the blend backward, carried to the mean
 // (and to the view matrix's depth row)

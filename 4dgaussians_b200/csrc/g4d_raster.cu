@@ -21,10 +21,12 @@ G4D_D float2 f2_fma(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn
 // pixels of a thread share their column, so dx, the dx^2 term and the instance record are scalar and computed once per
 // instance, and only what depends on the row is evaluated per lane (f2_add / f2_mul / f2_fma).  The per-pixel decisions are
 // selects, not branches.  power = fma(dy, -(conic.y dx), -0.5 (conic.z dy^2 + conic.x dx^2)) per lane.
+// out_alpha (may be NULL): the accumulated opacity 1 - T of every pixel, T the transmittance final_T holds.
 __global__ void __launch_bounds__(kTilePixels / 2)
 blend_forward_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, const uint32_t* __restrict__ ids,
                      const uint2* __restrict__ ranges, float* __restrict__ final_T, uint32_t* __restrict__ n_contrib,
-                     float* __restrict__ out_color, float* __restrict__ out_depth, int warp_cull) {
+                     float* __restrict__ out_color, float* __restrict__ out_depth, int warp_cull,
+                     float* __restrict__ out_alpha) {
     constexpr int PPT = 2, NT = kTilePixels / PPT;
     __shared__ float4 s0[kTilePixels];
     __shared__ float4 s1[kTilePixels];
@@ -114,6 +116,7 @@ blend_forward_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, const uin
         out_color[pix] = fmaf(T.x, cam->bg[0], C0.x); out_color[hw + pix] = fmaf(T.x, cam->bg[1], C1.x);
         out_color[2 * hw + pix] = fmaf(T.x, cam->bg[2], C2.x);
         out_depth[pix] = D.x;
+        if (out_alpha) out_alpha[pix] = 1.f - T.x;
     }
     if (in1) {
         const size_t pix = (size_t)py1 * W + (size_t)px;
@@ -121,14 +124,15 @@ blend_forward_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, const uin
         out_color[pix] = fmaf(T.y, cam->bg[0], C0.y); out_color[hw + pix] = fmaf(T.y, cam->bg[1], C1.y);
         out_color[2 * hw + pix] = fmaf(T.y, cam->bg[2], C2.y);
         out_depth[pix] = D.y;
+        if (out_alpha) out_alpha[pix] = 1.f - T.y;
     }
 }
 
 cudaError_t launch_blend_forward(const CameraDev* cam, int grid_x, int grid_y, GeomBuffers g, BinBuffers b, ImageBuffers im,
-                                 float* out_color, float* out_depth, int warp_cull, cudaStream_t st) {
+                                 float* out_color, float* out_depth, int warp_cull, float* out_alpha, cudaStream_t st) {
     if (grid_x * grid_y == 0) return cudaSuccess;
     return launch_k(blend_forward_kernel, dim3(grid_x, grid_y), dim3(kTilePixels / 2), 0, st, true, cam, g, b.ids_sorted, b.ranges,
-                    im.final_T, im.n_contrib, out_color, out_depth, warp_cull);
+                    im.final_T, im.n_contrib, out_color, out_depth, warp_cull, out_alpha);
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -150,7 +154,10 @@ G4D_D float staged_b(float2 v) { return v.x; }
 // threshold decisions).
 // DEPTH: the depth image D = sum_i w_i z_i takes the gradient dL_ddepth [H,W] too: a depth accumulator beside the colour
 // ones adds (z_i - aD') dL/dD to dL/dalpha, and dL/dz_i = w_i dL/dD is reduced per warp into g_depth [N].  dL_dcolor may
-// then be NULL (a zero colour gradient).  With DEPTH off the two trailing arguments are not read.
+// then be NULL (a zero colour gradient).  With DEPTH off dL_ddepth and g_depth are not read.
+// dL_dalpha (may be NULL): the gradient [H,W] of the alpha image A = 1 - T_final.  dA/dalpha_i = T_final / (1 - alpha_i) is
+// the background term's derivative with the opposite sign, so dL/dA folds into the per-pixel bgdot (bgdot - dL/dA) and needs
+// no per-Gaussian term.  dL_dcolor may then be NULL too.
 template <bool DEPTH>
 __global__ void __launch_bounds__(kTilePixels / 2)
 blend_backward_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, const uint32_t* __restrict__ ids,
@@ -158,7 +165,7 @@ blend_backward_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, const ui
                       const uint32_t* __restrict__ n_contrib, const float* __restrict__ dL_dcolor,
                       float* __restrict__ g_mean2D, float* __restrict__ g_conic, float* __restrict__ g_opacity,
                       float* __restrict__ g_rgb, int warp_cull, const float* __restrict__ dL_ddepth,
-                      float* __restrict__ g_depth) {
+                      float* __restrict__ g_depth, const float* __restrict__ dL_dalpha) {
     constexpr int PPT = 2, NT = kTilePixels / PPT;
     __shared__ float4 s0[kTilePixels];
     __shared__ float4 s1[kTilePixels];
@@ -182,14 +189,18 @@ blend_backward_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, const ui
     const float2 Tfin = make_float2(in0 ? final_T[pix0] : 0.f, in1 ? final_T[pix1] : 0.f);
     float2 T = Tfin;
     const int last0 = in0 ? (int)n_contrib[pix0] : 0, last1 = in1 ? (int)n_contrib[pix1] : 0;
-    const bool c0in = in0 && (!DEPTH || dL_dcolor), c1in = in1 && (!DEPTH || dL_dcolor);
+    const bool c0in = in0 && dL_dcolor, c1in = in1 && dL_dcolor;
     const float2 dp0 = make_float2(c0in ? dL_dcolor[pix0] : 0.f, c1in ? dL_dcolor[pix1] : 0.f);
     const float2 dp1 = make_float2(c0in ? dL_dcolor[hw + pix0] : 0.f, c1in ? dL_dcolor[hw + pix1] : 0.f);
     const float2 dp2 = make_float2(c0in ? dL_dcolor[2 * hw + pix0] : 0.f, c1in ? dL_dcolor[2 * hw + pix1] : 0.f);
     float2 dpD = make_float2(0.f, 0.f), aD = dpD, lD = dpD;      // DEPTH: dL/dD, depth accumulator, last depth
     if constexpr (DEPTH) dpD = make_float2(in0 ? dL_ddepth[pix0] : 0.f, in1 ? dL_ddepth[pix1] : 0.f);
-    const float2 bgdot = make_float2(cam->bg[0] * dp0.x + cam->bg[1] * dp1.x + cam->bg[2] * dp2.x,
-                                     cam->bg[0] * dp0.y + cam->bg[1] * dp1.y + cam->bg[2] * dp2.y);
+    float2 bgdot = make_float2(cam->bg[0] * dp0.x + cam->bg[1] * dp1.x + cam->bg[2] * dp2.x,
+                               cam->bg[0] * dp0.y + cam->bg[1] * dp1.y + cam->bg[2] * dp2.y);
+    if (dL_dalpha) {
+        if (in0) bgdot.x = __fsub_rn(bgdot.x, dL_dalpha[pix0]);
+        if (in1) bgdot.y = __fsub_rn(bgdot.y, dL_dalpha[pix1]);
+    }
     const float2 nTfin = make_float2(-Tfin.x, -Tfin.y);
     float2 ac0 = make_float2(0.f, 0.f), ac1 = ac0, ac2 = ac0, lc0 = ac0, lc1 = ac0, lc2 = ac0, la = ac0;
     const float ddx = 0.5f * (float)W, ddy = 0.5f * (float)H;
@@ -344,11 +355,13 @@ blend_backward_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, const ui
 
 cudaError_t launch_blend_backward(const CameraDev* cam, int grid_x, int grid_y, GeomBuffers g, BinBuffers b, ImageBuffers im,
                                   const float* dL_dcolor, float* g_mean2D, float* g_conic, float* g_opacity, float* g_rgb,
-                                  int warp_cull, const float* dL_ddepth, float* g_depth, cudaStream_t st) {
+                                  int warp_cull, const float* dL_ddepth, float* g_depth, const float* dL_dalpha,
+                                  cudaStream_t st) {
     if (grid_x * grid_y == 0) return cudaSuccess;
     auto kernel = dL_ddepth ? blend_backward_kernel<true> : blend_backward_kernel<false>;
     kernel<<<dim3(grid_x, grid_y), kTilePixels / 2, 0, st>>>(cam, g, b.ids_sorted, b.ranges, im.final_T, im.n_contrib, dL_dcolor,
-                                                             g_mean2D, g_conic, g_opacity, g_rgb, warp_cull, dL_ddepth, g_depth);
+                                                             g_mean2D, g_conic, g_opacity, g_rgb, warp_cull, dL_ddepth, g_depth,
+                                                             dL_dalpha);
     return cudaGetLastError();
 }
 

@@ -138,10 +138,11 @@ class GraphedRender:
 
     ``__call__`` takes a camera (or a list of cameras) with the template's image sizes and FoVs and returns the result
     dict(s) ``render()`` returns.  Their tensors are the graph's static outputs: the next call overwrites them.
-    ``min_capacity`` raises the instance capacity learnt from the template views (G4D_OPT_INSTANCE_CAPACITY)."""
+    ``min_capacity`` raises the instance capacity learnt from the template views (G4D_OPT_INSTANCE_CAPACITY).
+    ``return_alpha``: the result dicts also hold ``alpha``, as ``render(..., return_alpha=True)`` returns it."""
 
     def __init__(self, pc, pipe, bg_color: torch.Tensor, template, stage: str = "fine", scaling_modifier: float = 1.0,
-                 min_capacity: int = 0):
+                 min_capacity: int = 0, return_alpha: bool = False):
         self.multi = isinstance(template, (list, tuple))
         views = list(template) if self.multi else [template]
         if not views or len(views) > _lib.MAX_CAMERAS:
@@ -188,6 +189,10 @@ class GraphedRender:
         self._g = _lib.Gaussians(n, *self._ptrs)
         self.colors = [torch.zeros(3, int(rs.image_height), int(rs.image_width), device=dev) for rs, _ in settings]
         self.depths = [torch.zeros(1, int(rs.image_height), int(rs.image_width), device=dev) for rs, _ in settings]
+        self.alphas = [torch.zeros(1, int(rs.image_height), int(rs.image_width), device=dev) for rs, _ in settings] \
+            if return_alpha else []
+        for c, a in zip(self.ctxs, self.alphas):     # the private contexts write their alpha maps into the static outputs
+            c.set_alpha_out(a.data_ptr())
         self.radii = [torch.zeros(n, device=dev, dtype=torch.int32) for _ in range(k)]
         self.visible = [torch.zeros(n, device=dev, dtype=torch.bool) for _ in range(k)]
         ptrs = lambda ts: (C.c_void_p * k)(*[t.data_ptr() for t in ts])
@@ -268,6 +273,8 @@ class GraphedRender:
         pts = _zero_points(self.pc.get_xyz)
         out = [{"render": c, "viewspace_points": pts, "visibility_filter": v, "radii": r, "depth": d}
                for c, v, r, d in zip(self.colors, self.visible, self.radii, self.depths)]
+        for o, a in zip(out, self.alphas):
+            o["alpha"] = a
         return out if self.multi else out[0]
 
     def check(self, sync: bool = True) -> None:

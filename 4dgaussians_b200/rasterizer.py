@@ -7,6 +7,7 @@ plumbing here: device memory, the current stream, autograd bookkeeping.
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 from typing import NamedTuple, Optional
 
@@ -81,15 +82,17 @@ class CameraGradSinks:
     """One [k, 35] float32 device buffer whose row i the backward on context ``ctxs[i]`` overwrites with its camera's
     gradient, for the cameras named in ``spec``; with ``time``, one device float that the backward on ``ctxs[0]``
     overwrites with dL/d(time) (g4d_context_set_time_grad); ``depths[i]``, when given and not None, the gradient of camera
-    i's depth image (contiguous fp32 CUDA, [H*W]) that the backward on ``ctxs[i]`` takes (g4d_context_set_depth_grad).  The
-    contexts' pointers are cleared again on exit (they return to a pool)."""
+    i's depth image (contiguous fp32 CUDA, [H*W]) that the backward on ``ctxs[i]`` takes (g4d_context_set_depth_grad);
+    ``alphas[i]`` likewise for camera i's alpha image (g4d_context_set_alpha_grad).  The contexts' pointers are cleared
+    again on exit (they return to a pool)."""
 
-    def __init__(self, spec, ctxs, dev, time=False, depths=()):
+    def __init__(self, spec, ctxs, dev, time=False, depths=(), alphas=()):
         self.cams = sorted({i for i, _ in spec})
         self.ctxs = ctxs
         self.buf = torch.empty(len(ctxs), 35, device=dev, dtype=torch.float32) if spec else None
         self.tbuf = torch.empty(1, device=dev, dtype=torch.float32) if time else None
         self.depths = [(i, d) for i, d in enumerate(depths) if d is not None]
+        self.alphas = [(i, a) for i, a in enumerate(alphas) if a is not None]
 
     def __enter__(self):
         for i in self.cams:
@@ -98,6 +101,8 @@ class CameraGradSinks:
             self.ctxs[0].set_time_grad(self.tbuf.data_ptr())
         for i, d in self.depths:
             self.ctxs[i].set_depth_grad(d.data_ptr())
+        for i, a in self.alphas:
+            self.ctxs[i].set_alpha_grad(a.data_ptr())
         return self
 
     def __exit__(self, *exc):
@@ -107,6 +112,8 @@ class CameraGradSinks:
             self.ctxs[0].set_time_grad(None)
         for i, _ in self.depths:
             self.ctxs[i].set_depth_grad(None)
+        for i, _ in self.alphas:
+            self.ctxs[i].set_alpha_grad(None)
         return False
 
     def grads(self, spec, metas):
@@ -118,6 +125,20 @@ class CameraGradSinks:
         """dL/d(time) in the time tensor's (shape, dtype, device), ``meta`` (one entry of ``tensor_meta``)."""
         shape, dtype, device = meta
         return self.tbuf.reshape(shape).to(device=device, dtype=dtype)
+
+
+@contextlib.contextmanager
+def alpha_outputs(ctxs, alphas):
+    """Inside the block every forward on ``ctxs[i]`` also writes its alpha image into ``alphas[i]`` (contiguous fp32 CUDA,
+    [1,H,W]; g4d_context_set_alpha_out).  The pointers are cleared again on exit: the contexts return to a pool and must
+    not keep writing into a tensor that may be freed."""
+    for c, a in zip(ctxs, alphas):
+        c.set_alpha_out(a.data_ptr())
+    try:
+        yield
+    finally:
+        for c in ctxs:
+            c.set_alpha_out(None)
 
 
 def tensor_meta(tensors):
@@ -145,8 +166,8 @@ class _ContextLease:
 
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, raster_settings, differentiable_depth, cam_spec,
-                *cam_leaves):
+    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, raster_settings, differentiable_depth, return_alpha,
+                cam_spec, *cam_leaves):
         lib = _lib.load()
         dev = means3D.device
         n = means3D.shape[0]
@@ -165,30 +186,35 @@ class _RasterizeGaussians(torch.autograd.Function):
         cam = camera_from_settings(raster_settings, keep=keep, sh_coeffs=m)
         with torch.cuda.device(dev):
             lease = _ContextLease(_lib.workspace_of(dev))
-            _lib.check(lib.g4d_rasterize_forward(lease.ctx.handle, C.byref(cam), n, m3.data_ptr(), shc.data_ptr(), op.data_ptr(),
-                                                 sc.data_ptr(), ro.data_ptr(), color.data_ptr(), depth.data_ptr(),
-                                                 radii.data_ptr(), _lib.stream_of(dev)), "g4d_rasterize_forward")
+            alpha = torch.empty(1, H, W, device=dev, dtype=torch.float32) if return_alpha else None
+            with alpha_outputs([lease.ctx] if return_alpha else [], [alpha]):
+                _lib.check(lib.g4d_rasterize_forward(lease.ctx.handle, C.byref(cam), n, m3.data_ptr(), shc.data_ptr(),
+                                                     op.data_ptr(), sc.data_ptr(), ro.data_ptr(), color.data_ptr(),
+                                                     depth.data_ptr(), radii.data_ptr(), _lib.stream_of(dev)),
+                           "g4d_rasterize_forward")
         ctx.raster_settings = raster_settings
         ctx.cam_spec, ctx.cam_meta = cam_spec, tensor_meta(cam_leaves)
         ctx.lease = lease
         ctx.n, ctx.m = n, m
         ctx.save_for_backward(m3, shc, op, sc, ro)
         ctx.mark_non_differentiable(*((radii,) if differentiable_depth else (radii, depth)))
-        ctx.set_materialize_grads(False)         # a depth image outside the loss arrives as None: no depth gradient is set
-        return color, radii, depth
+        # a depth or alpha image outside the loss arrives as None: no depth or alpha gradient is set
+        ctx.set_materialize_grads(False)
+        return (color, radii, depth, alpha) if return_alpha else (color, radii, depth)
 
     @staticmethod
-    def backward(ctx, grad_color, _grad_radii, grad_depth):
+    def backward(ctx, grad_color, _grad_radii, grad_depth, grad_alpha=None):
         lib = _lib.load()
         m3, shc, op, sc, ro = ctx.saved_tensors
         dev = m3.device
         n = ctx.n
         rs = ctx.raster_settings
         hw = int(rs.image_height) * int(rs.image_width)
-        if grad_color is None:      # a depth-only loss: the backward takes an image gradient
+        if grad_color is None:      # a depth- or alpha-only loss: the backward takes an image gradient
             grad_color = torch.zeros(3 * hw, device=dev)
         gcol = _lib.cuda_f32(grad_color, "grad_out_color", 3 * hw)
         gdep = _lib.cuda_f32(grad_depth, "grad_out_depth", hw)
+        galpha = _lib.cuda_f32(grad_alpha, "grad_out_alpha", hw)
         g_means3D = torch.empty(n, 3, device=dev)
         g_means2D = torch.empty(n, 3, device=dev)
         g_sh = torch.empty(n, ctx.m, 3, device=dev)
@@ -200,7 +226,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         lease = ctx.lease
         if lease is None or lease.ctx is None:
             raise RuntimeError("rasterizer backward called twice (context already released)")
-        sinks = CameraGradSinks(ctx.cam_spec, [lease.ctx], dev, depths=(gdep,))
+        sinks = CameraGradSinks(ctx.cam_spec, [lease.ctx], dev, depths=(gdep,), alphas=(galpha,))
         with torch.cuda.device(dev), sinks:
             _lib.check(lib.g4d_rasterize_backward(lease.ctx.handle, C.byref(cam), n, m3.data_ptr(), shc.data_ptr(), op.data_ptr(),
                                                   sc.data_ptr(), ro.data_ptr(), gcol.data_ptr(), g_means3D.data_ptr(),
@@ -209,18 +235,22 @@ class _RasterizeGaussians(torch.autograd.Function):
         lease.release()
         ctx.lease = None
         cam_grads = sinks.grads(ctx.cam_spec, ctx.cam_meta) if ctx.cam_spec else ()
-        return (g_means3D, g_means2D, g_sh, g_op, g_sc, g_ro, None, None, None) + cam_grads
+        return (g_means3D, g_means2D, g_sh, g_op, g_sc, g_ro, None, None, None, None) + cam_grads
 
 
 class GaussianRasterizer(nn.Module):
     """differentiable_depth: the depth image it returns takes a gradient too (render() and render_cameras() render theirs
     so).  Off by default the depth is a tensor without grad, as diff_gaussian_rasterization's callers read it (a tensor
-    that requires grad refuses .numpy())."""
+    that requires grad refuses .numpy()).
+    return_alpha: return (color, radii, depth, alpha), alpha [1,H,W] the accumulated opacity 1 - T of each pixel, which
+    takes a gradient; off by default the result is diff_gaussian_rasterization's (color, radii, depth)."""
 
-    def __init__(self, raster_settings: GaussianRasterizationSettings, differentiable_depth: bool = False):
+    def __init__(self, raster_settings: GaussianRasterizationSettings, differentiable_depth: bool = False,
+                 return_alpha: bool = False):
         super().__init__()
         self.raster_settings = raster_settings
         self.differentiable_depth = bool(differentiable_depth)
+        self.return_alpha = bool(return_alpha)
 
     def markVisible(self, positions):
         raise NotImplementedError("markVisible is not used by 4DGaussians (SURVEY.md §8b) and is not part of the g4d path")
@@ -239,4 +269,4 @@ class GaussianRasterizer(nn.Module):
         # the settings' viewmatrix / projmatrix / campos that require grad join the autograd graph as extra inputs
         cam_spec, cam_leaves = camera_grad_leaves((rs,))
         return _RasterizeGaussians.apply(means3D, means2D, shs, opacities, scales, rotations, rs, self.differentiable_depth,
-                                         cam_spec, *cam_leaves)
+                                         self.return_alpha, cam_spec, *cam_leaves)

@@ -13,7 +13,9 @@ is its one-camera case, which takes the single-camera entry points.
 
 Both differentiate the camera tensors that require grad (``rasterizer.camera_grad_leaves``) and the camera's time when it
 is a tensor that requires grad (``time_grad_leaf``): dL/dt comes from the network's backward, for learning per-camera time
-offsets.  The ``depth`` maps they return are differentiable too, for depth supervision.
+offsets.  The ``depth`` maps they return are differentiable too, for depth supervision.  With ``return_alpha=True`` each
+result dict also holds ``alpha``, the accumulated opacity 1 - T of each pixel, differentiable as well, for mask supervision
+and compositing.
 """
 from __future__ import annotations
 
@@ -26,8 +28,8 @@ import torch
 
 from . import _lib
 from .deformation import deform_network, scalar_time
-from .rasterizer import (CameraGradSinks, GaussianRasterizationSettings, GaussianRasterizer, _ContextLease, camera_from_settings,
-                         camera_grad_leaves, tensor_meta)
+from .rasterizer import (CameraGradSinks, GaussianRasterizationSettings, GaussianRasterizer, _ContextLease, alpha_outputs,
+                         camera_from_settings, camera_grad_leaves, tensor_meta)
 
 
 def settings_from_camera(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, cam_type=None):
@@ -66,9 +68,11 @@ def time_grad_leaf(viewpoint_cameras, cam_type=None):
     return leaves[0]
 
 
-def _fused_forward(module: Optional[deform_network], rss, t, needs_bwd, xyz, scaling, rotation, opacity, f_dc, f_rest):
+def _fused_forward(module: Optional[deform_network], rss, t, needs_bwd, want_alpha, xyz, scaling, rotation, opacity, f_dc,
+                   f_rest):
     """One fused render call over the cameras' settings rss, one context lease per camera: g4d_render_forward for one
-    camera, g4d_render_forward_cameras for several.  Shared by the autograd Function and by the no-grad fast path."""
+    camera, g4d_render_forward_cameras for several.  Shared by the autograd Function and by the no-grad fast path.
+    want_alpha: the cameras' alpha maps are rendered too (else ``alphas`` is empty)."""
     lib = _lib.load()
     dev = xyz.device
     n, k = xyz.shape[0], len(rss)
@@ -79,6 +83,8 @@ def _fused_forward(module: Optional[deform_network], rss, t, needs_bwd, xyz, sca
     dc, rest = _lib.cuda_f32(f_dc, "features_dc", n * 3), _lib.cuda_f32(f_rest, "features_rest", n * 3 * (m - 1))
     colors = [torch.empty(3, int(rs.image_height), int(rs.image_width), device=dev, dtype=torch.float32) for rs in rss]
     depths = [torch.empty(1, int(rs.image_height), int(rs.image_width), device=dev, dtype=torch.float32) for rs in rss]
+    alphas = [torch.empty(1, int(rs.image_height), int(rs.image_width), device=dev, dtype=torch.float32)
+              for rs in rss] if want_alpha else []
     radii = [torch.empty(n, device=dev, dtype=torch.int32) for _ in rss]
     keep = []
     cams = [camera_from_settings(rs, time=t, keep=keep, sh_coeffs=m) for rs in rss]
@@ -93,18 +99,19 @@ def _fused_forward(module: Optional[deform_network], rss, t, needs_bwd, xyz, sca
     with torch.cuda.device(dev):
         ws = _lib.workspace_of(dev)
         leases = [_ContextLease(ws) for _ in rss]
-        if k == 1:
-            cams, handles = cams[0], None       # one camera: the Camera itself, several: a Camera array
-            _lib.check(lib.g4d_render_forward(leases[0].ctx.handle, C.byref(cams), C.byref(prm) if prm is not None else None,
-                                              C.byref(g), colors[0].data_ptr(), depths[0].data_ptr(), radii[0].data_ptr(),
-                                              _lib.stream_of(dev)), "g4d_render_forward")
-        else:
-            cams, handles = (_lib.Camera * k)(*cams), (C.c_void_p * k)(*[lease.ctx.handle for lease in leases])
-            _lib.check(lib.g4d_render_forward_cameras(handles, k, cams, C.byref(prm) if prm is not None else None,
-                                                      C.byref(g), _pointers(colors), _pointers(depths), _pointers(radii),
-                                                      _lib.stream_of(dev)), "g4d_render_forward_cameras")
+        pm = C.byref(prm) if prm is not None else None
+        with alpha_outputs([lease.ctx for lease in leases] if want_alpha else [], alphas):
+            if k == 1:
+                cams, handles = cams[0], None       # one camera: the Camera itself, several: a Camera array
+                _lib.check(lib.g4d_render_forward(leases[0].ctx.handle, C.byref(cams), pm, C.byref(g), colors[0].data_ptr(),
+                                                  depths[0].data_ptr(), radii[0].data_ptr(), _lib.stream_of(dev)),
+                           "g4d_render_forward")
+            else:
+                cams, handles = (_lib.Camera * k)(*cams), (C.c_void_p * k)(*[lease.ctx.handle for lease in leases])
+                _lib.check(lib.g4d_render_forward_cameras(handles, k, cams, pm, C.byref(g), _pointers(colors), _pointers(depths),
+                                                          _pointers(radii), _lib.stream_of(dev)), "g4d_render_forward_cameras")
     cstructs = (cams, prm, g, keep, int(prm.version) if prm is not None else None, handles)
-    return colors, radii, depths, leases, cstructs, (x, s, r, o, dc, rest)
+    return colors, radii, depths, alphas, leases, cstructs, (x, s, r, o, dc, rest)
 
 
 def _pointers(tensors):
@@ -114,13 +121,15 @@ def _pointers(tensors):
 class _FusedRender(torch.autograd.Function):
     """inputs: xyz, scaling, rotation, opacity, features_dc, features_rest, k x means2D, *deform parameters, then the
     camera tensors that take a gradient (cam_spec: their (camera, field) pairs, rasterizer.camera_grad_leaves), then, when
-    ``timed``, the time tensor that takes a gradient (time_grad_leaf); outputs: k images, k radii, k depth maps"""
+    ``timed``, the time tensor that takes a gradient (time_grad_leaf); outputs: k images, k radii, k depth maps, and with
+    ``want_alpha`` k alpha maps"""
 
     @staticmethod
-    def forward(ctx, module: Optional[deform_network], rss, t, cam_spec, timed, xyz, scaling, rotation, opacity, f_dc, f_rest,
-                *rest):
-        colors, radii, depths, leases, cstructs, saved = _fused_forward(module, rss, t, any(ctx.needs_input_grad), xyz, scaling,
-                                                                        rotation, opacity, f_dc, f_rest)
+    def forward(ctx, module: Optional[deform_network], rss, t, cam_spec, timed, want_alpha, xyz, scaling, rotation, opacity,
+                f_dc, f_rest, *rest):
+        colors, radii, depths, alphas, leases, cstructs, saved = _fused_forward(module, rss, t, any(ctx.needs_input_grad),
+                                                                                want_alpha, xyz, scaling, rotation, opacity,
+                                                                                f_dc, f_rest)
         ctx.module, ctx.rss, ctx.n, ctx.leases = module, rss, xyz.shape[0], leases
         end = len(rest) - int(timed)
         ctx.cam_spec, ctx.cam_meta = cam_spec, tensor_meta(rest[end - len(cam_spec):end])
@@ -131,9 +140,10 @@ class _FusedRender(torch.autograd.Function):
         ctx.cstructs = cstructs
         ctx.save_for_backward(*saved)
         ctx.mark_non_differentiable(*radii)
-        # an image or depth map outside the loss arrives as None: a camera with neither has its blend backward skipped
+        # an image, depth or alpha map outside the loss arrives as None: a camera with none of them in the loss has its blend
+        # backward skipped
         ctx.set_materialize_grads(False)
-        return tuple(colors) + tuple(radii) + tuple(depths)
+        return tuple(colors) + tuple(radii) + tuple(depths) + tuple(alphas)
 
     @staticmethod
     def backward(ctx, *grads):
@@ -148,7 +158,9 @@ class _FusedRender(torch.autograd.Function):
         gcols = [None if gc is None else _lib.cuda_f32(gc, "grad_out_color", 3 * int(rs.image_height) * int(rs.image_width))
                  for gc, rs in zip(grads[:k], rss)]
         gdeps = [_lib.cuda_f32(gd, "grad_out_depth", int(rs.image_height) * int(rs.image_width))
-                 for gd, rs in zip(grads[2 * k:], rss)]
+                 for gd, rs in zip(grads[2 * k:3 * k], rss)]
+        galphas = [_lib.cuda_f32(ga, "grad_out_alpha", int(rs.image_height) * int(rs.image_width))
+                   for ga, rs in zip(grads[3 * k:], rss)]
         cams, prm, g, keep, version, handles = ctx.cstructs
         if module is not None and version != module._param_version:      # another forward ran since: take the current key
             keep = []
@@ -167,7 +179,7 @@ class _FusedRender(torch.autograd.Function):
         gg = _lib.GaussianGrads(gx.data_ptr(), gs.data_ptr(), gr.data_ptr(), go.data_ptr(), gdc.data_ptr(), grest.data_ptr(),
                                 gm2[0].data_ptr() if k == 1 else None)
         sinks = CameraGradSinks(ctx.cam_spec, [lease.ctx for lease in leases], dev, time=ctx.time_meta is not None,
-                                depths=gdeps)
+                                depths=gdeps, alphas=galphas)
         with torch.cuda.device(dev), sinks:
             if k == 1:
                 if gcols[0] is None:        # the single-camera backward takes an image gradient
@@ -185,7 +197,7 @@ class _FusedRender(torch.autograd.Function):
         ctx.leases = ctx.lease = None
         cam_grads = sinks.grads(ctx.cam_spec, ctx.cam_meta) if ctx.cam_spec else ()
         time_grad = (sinks.time_grad(ctx.time_meta),) if ctx.time_meta is not None else ()
-        return (None, None, None, None, None, gx, gs, gr, go, gdc, grest) + tuple(gm2) + tuple(pgrads) + cam_grads + time_grad
+        return (None, None, None, None, None, None, gx, gs, gr, go, gdc, grest) + tuple(gm2) + tuple(pgrads) + cam_grads + time_grad
 
 
 def _time_bits(t) -> bytes:
@@ -216,7 +228,7 @@ def _zero_points(xyz: torch.Tensor) -> torch.Tensor:
     return z
 
 
-def _render(viewpoint_cameras, pc, pipe, bg_color, scaling_modifier, override_color, stage, cam_type):
+def _render(viewpoint_cameras, pc, pipe, bg_color, scaling_modifier, override_color, stage, cam_type, return_alpha):
     """The body of render() and render_cameras(): one result dict per camera."""
     if override_color is not None or getattr(pipe, "convert_SHs_python", False) or getattr(pipe, "compute_cov3D_python", False):
         raise NotImplementedError("override_color / convert_SHs_python / compute_cov3D_python are dead or broken paths in "
@@ -245,18 +257,19 @@ def _render(viewpoint_cameras, pc, pipe, bg_color, scaling_modifier, override_co
     if module is None or isinstance(module, deform_network):
         if not torch.is_grad_enabled():
             # no autograd node to build: skip Function.apply and its per-input bookkeeping (40 inputs with the network's parameters)
-            images, radii, depths, leases, _, _ = _fused_forward(module, rss, t, False, xyz, pc._scaling, pc._rotation, pc._opacity,
-                                                                 pc._features_dc, pc._features_rest)
+            images, radii, depths, alphas, leases, _, _ = _fused_forward(module, rss, t, False, return_alpha, xyz, pc._scaling,
+                                                                         pc._rotation, pc._opacity, pc._features_dc,
+                                                                         pc._features_rest)
             for lease in leases:
                 lease.release()
         else:
             params = tuple(module.flat_parameters()) if module is not None else ()
             cam_spec, cam_leaves = camera_grad_leaves(rss)      # camera tensors that require grad: extra inputs
             time_leaves = () if time_leaf is None else (time_leaf,)
-            outs = _FusedRender.apply(module, rss, t, cam_spec, time_leaf is not None, xyz, pc._scaling, pc._rotation,
-                                      pc._opacity, pc._features_dc, pc._features_rest, *points, *params, *cam_leaves,
+            outs = _FusedRender.apply(module, rss, t, cam_spec, time_leaf is not None, return_alpha, xyz, pc._scaling,
+                                      pc._rotation, pc._opacity, pc._features_dc, pc._features_rest, *points, *params, *cam_leaves,
                                       *time_leaves)
-            images, radii, depths = outs[:k], outs[k:2 * k], outs[2 * k:]
+            images, radii, depths, alphas = outs[:k], outs[k:2 * k], outs[2 * k:3 * k], outs[3 * k:]
     else:
         # a foreign (e.g. the reference's own PyTorch) deformation module: keep its semantics, deform once, then rasterize
         # every camera with g4d
@@ -267,27 +280,34 @@ def _render(viewpoint_cameras, pc, pipe, bg_color, scaling_modifier, override_co
             time = time_leaf.to(device=xyz.device, dtype=torch.float32).reshape(1, 1).repeat(n, 1)
         m3, sc, rot, op, shs = module(xyz, pc._scaling, pc._rotation, pc._opacity, pc.get_features, time)
         opac, scales, rots = pc.opacity_activation(op), pc.scaling_activation(sc), pc.rotation_activation(rot)
-        images, radii, depths = [], [], []
+        images, radii, depths, alphas = [], [], [], []
         for rs, p in zip(rss, points):
-            img, rad, dep = GaussianRasterizer(raster_settings=rs, differentiable_depth=True)(
+            r = GaussianRasterizer(raster_settings=rs, differentiable_depth=True, return_alpha=return_alpha)(
                 means3D=m3, means2D=p, shs=shs, colors_precomp=None, opacities=opac, scales=scales, rotations=rots,
                 cov3D_precomp=None)
-            images.append(img); radii.append(rad); depths.append(dep)
-    return [{"render": img, "viewspace_points": p, "visibility_filter": rad > 0, "radii": rad, "depth": dep}
+            images.append(r[0]); radii.append(r[1]); depths.append(r[2]); alphas.extend(r[3:])
+    outs = [{"render": img, "viewspace_points": p, "visibility_filter": rad > 0, "radii": rad, "depth": dep}
             for img, p, rad, dep in zip(images, points, radii, depths)]
+    for out, alp in zip(outs, alphas):
+        out["alpha"] = alp
+    return outs
 
 
 def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None, stage="fine",
-           cam_type=None):
-    """Render the scene.  Background tensor (bg_color) must be on GPU (as in the reference)."""
-    return _render((viewpoint_camera,), pc, pipe, bg_color, scaling_modifier, override_color, stage, cam_type)[0]
+           cam_type=None, return_alpha=False):
+    """Render the scene.  Background tensor (bg_color) must be on GPU (as in the reference).  return_alpha: the result
+    dict also holds ``alpha`` [1,H,W], the accumulated opacity 1 - T of each pixel (render = C_fg + (1 - alpha) * bg up to
+    fp32 rounding), which takes a gradient in grad mode."""
+    return _render((viewpoint_camera,), pc, pipe, bg_color, scaling_modifier, override_color, stage, cam_type,
+                   return_alpha)[0]
 
 
 def render_cameras(viewpoint_cameras, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None, stage="fine",
-                   cam_type=None):
+                   cam_type=None, return_alpha=False):
     """Render one timestamp from several cameras: one result dict per camera, each with the keys render() returns and its
     own ``viewspace_points``.  The cameras must share their time (as float32, bit for bit; else ValueError) and there may
     be at most G4D_MAX_CAMERAS (32) of them.  With the g4d deformation network the deformation runs once for all cameras,
     forward and backward; a foreign deformation module is run once and its output rasterized per camera.  A time that
-    requires grad must be one tensor that every camera holds (ValueError otherwise): the group's one dL/dt goes to it."""
-    return _render(viewpoint_cameras, pc, pipe, bg_color, scaling_modifier, override_color, stage, cam_type)
+    requires grad must be one tensor that every camera holds (ValueError otherwise): the group's one dL/dt goes to it.
+    return_alpha: as for render(), per camera."""
+    return _render(viewpoint_cameras, pc, pipe, bg_color, scaling_modifier, override_color, stage, cam_type, return_alpha)
