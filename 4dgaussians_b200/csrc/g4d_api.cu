@@ -163,6 +163,29 @@ struct G4DWorkspace {
     PinnedWords* pinned = nullptr;
 };
 
+// What a context's view takes and gives beyond its colour image, one device pointer per g4d_context_set_* entry point
+// (NULL: off).  A capture refuses every term a backward reads or writes: a graph would keep using a pointer the context
+// may since have dropped.
+struct ViewTerms {
+    float* cam_grad = nullptr;           // g4d_context_set_camera_grad (kCamGradFloats)
+    float* time_grad = nullptr;          // g4d_context_set_time_grad (1 float)
+    const float* depth_grad = nullptr;   // g4d_context_set_depth_grad ([H,W] dL/d depth image)
+    float* alpha_out = nullptr;          // g4d_context_set_alpha_out ([H,W] alpha image of every forward)
+    const float* alpha_grad = nullptr;   // g4d_context_set_alpha_grad ([H,W] dL/d alpha image)
+
+    // a backward takes the view into the loss: it has an image (dL_dcolor), a depth or an alpha gradient
+    bool in_loss(const float* dL_dcolor) const { return dL_dcolor || depth_grad || alpha_grad; }
+
+    // the refusal of a backward on a capturing stream, in the order the terms are checked (NULL: nothing to refuse)
+    const char* capture_refusal() const {
+        if (cam_grad) return "cannot capture a backward on a context with a camera gradient set (g4d_context_set_camera_grad)";
+        if (time_grad) return "cannot capture a backward on a context with a time gradient set (g4d_context_set_time_grad)";
+        if (depth_grad) return "cannot capture a backward on a context with a depth gradient set (g4d_context_set_depth_grad)";
+        if (alpha_grad) return "cannot capture a backward on a context with an alpha gradient set (g4d_context_set_alpha_grad)";
+        return nullptr;
+    }
+};
+
 struct G4DContext {
     G4DWorkspace* ws = nullptr;
     DevBuf cam, geom, bin, binaux, img, fused, gscratch, gdeform, trow, relu, feat;
@@ -170,11 +193,7 @@ struct G4DContext {
     int grid_x = 0, grid_y = 0;
     int64_t R = 0, capacity = 0;
     const float* time_src = nullptr;  // g4d_context_set_time_source (device; NULL: G4DCamera.time)
-    float* cam_grad = nullptr;        // g4d_context_set_camera_grad (device, kCamGradFloats; NULL: no camera gradient)
-    float* time_grad = nullptr;       // g4d_context_set_time_grad (device, 1 float; NULL: no time gradient)
-    const float* depth_grad = nullptr;   // g4d_context_set_depth_grad (device, [H,W] dL/d depth image; NULL: none)
-    float* alpha_out = nullptr;          // g4d_context_set_alpha_out (device, [H,W] alpha image of every forward; NULL: none)
-    const float* alpha_grad = nullptr;   // g4d_context_set_alpha_grad (device, [H,W] dL/d alpha image; NULL: none)
+    ViewTerms terms;
     const void* bin_ctl = nullptr;    // device BinCtl of the last forward
     bool learned = false;             // R of an earlier exact forward is known (no-sync mode needs a learnt capacity)
     GeomBuffers g{};
@@ -593,7 +612,7 @@ int bin_and_blend(G4DContext* c, const G4DCamera* cam, int64_t n, float* out_col
     {
         StageTimer tm(c, G4D_STAGE_BLEND, st);
         G4D_CUDA(launch_blend_forward(dcam, c->grid_x, c->grid_y, c->g, c->b, c->im, out_color, out_depth, ws->warp_cull,
-                                      c->alpha_out, st));
+                                      c->terms.alpha_out, st));
     }
     if (readback && t_call.capturing) {
         G4D_CUDA(launch_record_overflow(static_cast<const BinCtl*>(c->bin_ctl), cap_place, ws->pinned->overflow, st));
@@ -613,25 +632,16 @@ template <class Sh, class T> Sh caller_sh(int m, bool split, T* dc, T* rest = nu
     return split ? Sh{nullptr, dc, rest, m} : Sh{dc, nullptr, nullptr, m};
 }
 
-// The gradient sinks of a backward on ctx[0, k), camera (g4d_context_set_camera_grad) and time (g4d_context_set_time_grad):
-// refused while capturing (a graph would keep writing a sink the context may since have dropped), else zeroed on st; the
-// backward adds into them, and a sink nothing adds into (a camera outside the loss, a backward without a deformation) keeps
-// the zeros.  A depth or alpha gradient (g4d_context_set_depth_grad / _alpha_grad) is refused while capturing for the same
-// reason: a graph would keep reading it.  Called before the backward's first launch.
+// The terms of a backward on ctx[0, k): every context's capture refusal (ViewTerms::capture_refusal), then the camera and
+// time gradient sinks zeroed on st; the backward adds into them, and a sink nothing adds into (a camera outside the loss, a
+// backward without a deformation) keeps the zeros.  Called before the backward's first launch.
 int zero_grad_sinks(G4DContext* const* ctx, int k, cudaStream_t st) {
+    for (int i = 0; i < k && t_call.capturing; ++i)
+        if (const char* why = ctx[i]->terms.capture_refusal()) return fail(G4D_ERR_STATE, why);
     for (int i = 0; i < k; ++i) {
-        if (ctx[i]->cam_grad && t_call.capturing)
-            return fail(G4D_ERR_STATE, "cannot capture a backward on a context with a camera gradient set (g4d_context_set_camera_grad)");
-        if (ctx[i]->time_grad && t_call.capturing)
-            return fail(G4D_ERR_STATE, "cannot capture a backward on a context with a time gradient set (g4d_context_set_time_grad)");
-        if (ctx[i]->depth_grad && t_call.capturing)
-            return fail(G4D_ERR_STATE, "cannot capture a backward on a context with a depth gradient set (g4d_context_set_depth_grad)");
-        if (ctx[i]->alpha_grad && t_call.capturing)
-            return fail(G4D_ERR_STATE, "cannot capture a backward on a context with an alpha gradient set (g4d_context_set_alpha_grad)");
-    }
-    for (int i = 0; i < k; ++i) {
-        if (ctx[i]->cam_grad) G4D_CUDA(cudaMemsetAsync(ctx[i]->cam_grad, 0, kCamGradFloats * sizeof(float), st));
-        if (ctx[i]->time_grad) G4D_CUDA(cudaMemsetAsync(ctx[i]->time_grad, 0, sizeof(float), st));
+        const ViewTerms& v = ctx[i]->terms;
+        if (v.cam_grad) G4D_CUDA(cudaMemsetAsync(v.cam_grad, 0, kCamGradFloats * sizeof(float), st));
+        if (v.time_grad) G4D_CUDA(cudaMemsetAsync(v.time_grad, 0, sizeof(float), st));
     }
     return G4D_OK;
 }
@@ -680,6 +690,7 @@ struct CallFrame {
 int blend_backward(G4DContext* c, const G4DCamera* cam, int64_t n, const float* dL_dcolor, float* g_opacities, bool depth_block,
                    float** gb, cudaStream_t st) {
     using L = BlendGradLayout;
+    const ViewTerms& v = c->terms;
     const size_t N = (size_t)(n > 0 ? n : 1);
     const size_t floats = N * (depth_block ? L::kDepthFloats : g_opacities ? L::kOpacity : L::kFloats);
     G4D_CUDA(c->gscratch.ensure(floats * 4 + 256));
@@ -692,27 +703,26 @@ int blend_backward(G4DContext* c, const G4DCamera* cam, int64_t n, const float* 
         StageTimer tm(c, G4D_STAGE_BLEND_BWD, st);
         G4D_CUDA(launch_blend_backward(c->cam.as<CameraDev>(), c->grid_x, c->grid_y, c->g, c->b, c->im, dL_dcolor, b + L::kMean2D * N,
                                        b + L::kConic * N, g_opacities ? g_opacities : b + L::kOpacity * N, b + L::kRgb * N,
-                                       c->ws->warp_cull, c->depth_grad, c->depth_grad ? b + L::kDepth * N : nullptr,
-                                       c->alpha_grad, st));
+                                       c->ws->warp_cull, v.depth_grad, v.depth_grad ? b + L::kDepth * N : nullptr, v.alpha_grad, st));
     }
     return debug_sync(cam, st, "blend_backward");
 }
 
-// blend backward + per-Gaussian backward on `in`; opacity gradient lands in g_opacities (zeroed here); the camera's
-// gradient is added into c->cam_grad when it is set, and the depth and alpha images' gradients c->depth_grad / c->alpha_grad
-// are taken when they are set
+// blend backward + per-Gaussian backward on `in`; opacity gradient lands in g_opacities (zeroed here); the terms of c taken
+// as they are set: the camera's gradient added into its sink, the depth and alpha images' gradients
 int raster_backward_stages(G4DContext* c, const G4DCamera* cam, int64_t n, const RasterInputs& in, const float* dL_dcolor,
                            float* g_means3D, float* g_means2D, const ShOut& g_sh, float* g_opacities, float* g_scales,
                            float* g_rotations, cudaStream_t st) {
     using L = BlendGradLayout;
+    const ViewTerms& v = c->terms;
     const size_t N = (size_t)n;
     float* gb;
-    const int rc = blend_backward(c, cam, n, dL_dcolor, g_opacities, c->depth_grad != nullptr, &gb, st);
+    const int rc = blend_backward(c, cam, n, dL_dcolor, g_opacities, v.depth_grad != nullptr, &gb, st);
     if (rc != G4D_OK || n == 0) return rc;
     StageTimer tm(c, G4D_STAGE_GEOM_BWD, st);
     G4D_CUDA(launch_preprocess_backward(c->cam.as<CameraDev>(), n, in, c->g, gb + L::kMean2D * N, gb + L::kConic * N,
-                                        gb + L::kRgb * N, g_means3D, g_means2D, g_scales, g_rotations, g_sh, c->cam_grad,
-                                        c->depth_grad ? gb + L::kDepth * N : nullptr, st));
+                                        gb + L::kRgb * N, g_means3D, g_means2D, g_scales, g_rotations, g_sh, v.cam_grad,
+                                        v.depth_grad ? gb + L::kDepth * N : nullptr, st));
     return debug_sync(cam, st, "preprocess_backward");
 }
 
@@ -1220,7 +1230,7 @@ int fused_backward(G4DContext* c, const G4DCamera* cam, const G4DDeformParams* p
     rc = raster_backward_stages(c, cam, n, deformed_inputs(c, c->fwd, g), dL_dcolor, d.xyz, gg->means2D,
                                 fused_sh_sinks(c, g, gg, d.sh), d.op, d.sc, d.rot, st);
     if (rc != G4D_OK) return rc;
-    return fused_backward_tail(c, cam, prm, pgrads, g, gg, d, c->time_grad, st);
+    return fused_backward_tail(c, cam, prm, pgrads, g, gg, d, c->terms.time_grad, st);
 }
 
 // k cameras on k contexts: 1 <= k <= G4D_MAX_CAMERAS, one time bit for bit (or, when ctx[0] has a time source, that same
@@ -1386,15 +1396,15 @@ int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCame
     if (n == 0) return G4D_OK;
     DeformedGrads d;
     if ((rc = deformed_grads(c0, n, gg, &d)) != G4D_OK) return rc;
-    // blend backward of every camera in the loss (an image, a depth or an alpha gradient), each into its own scratch; when any camera
-    // has a depth gradient, every scratch has the depth block
+    // blend backward of every camera in the loss, each into its own scratch; when any camera has a depth gradient, every
+    // scratch has the depth block
     BackwardCameras bc{};
     CamGradSinks cs{};
     bool cam_grads = false, depth = false;
-    for (int i = 0; i < k; ++i) depth |= ctx[i]->depth_grad != nullptr;
+    for (int i = 0; i < k; ++i) depth |= ctx[i]->terms.depth_grad != nullptr;
     for (int i = 0; i < k; ++i) {
         G4DContext* c = ctx[i];
-        if (!dL_dcolor[i] && !c->depth_grad && !c->alpha_grad) {
+        if (!c->terms.in_loss(dL_dcolor[i])) {
             reset_stage_flags(c, G4D_STAGE_BLEND_BWD, G4D_STAGE_DEFORM_BWD);
             if (g_means2D && g_means2D[i]) G4D_CUDA(cudaMemsetAsync(g_means2D[i], 0, (size_t)n * 12, st));
             continue;
@@ -1404,8 +1414,8 @@ int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCame
         const int j = bc.count++;
         bc.cam[j] = c->cam.as<CameraDev>(); bc.radii[j] = c->g.radii; bc.clamped[j] = c->g.clamped; bc.grad[j] = gb;
         bc.g_means2D[j] = g_means2D ? g_means2D[i] : nullptr;
-        cs.out[j] = c->cam_grad;
-        cam_grads |= c->cam_grad != nullptr;
+        cs.out[j] = c->terms.cam_grad;
+        cam_grads |= c->terms.cam_grad != nullptr;
     }
     {
         StageTimer tm(c0, G4D_STAGE_GEOM_BWD, st);
@@ -1416,11 +1426,11 @@ int g4d_render_backward_cameras(G4DContext* const* ctx, int32_t k, const G4DCame
     // the network's backward, once, on the gradients summed over the cameras; the one dL/d(time) of the group goes to the
     // first context with a time sink and is copied into the others'
     float* g_time = nullptr;
-    for (int i = 0; i < k && !g_time; ++i) g_time = ctx[i]->time_grad;
+    for (int i = 0; i < k && !g_time; ++i) g_time = ctx[i]->terms.time_grad;
     if ((rc = fused_backward_tail(c0, &cams[0], prm, pgrads, g, gg, d, g_time, st)) != G4D_OK) return rc;
     for (int i = 0; i < k; ++i)
-        if (ctx[i]->time_grad && ctx[i]->time_grad != g_time)
-            G4D_CUDA(cudaMemcpyAsync(ctx[i]->time_grad, g_time, sizeof(float), cudaMemcpyDeviceToDevice, st));
+        if (float* t = ctx[i]->terms.time_grad; t && t != g_time)
+            G4D_CUDA(cudaMemcpyAsync(t, g_time, sizeof(float), cudaMemcpyDeviceToDevice, st));
     return G4D_OK;
 }
 
@@ -1546,31 +1556,31 @@ int g4d_context_set_time_source(G4DContext* c, const float* d_time) {
 
 int g4d_context_set_camera_grad(G4DContext* c, float* d_out) {
     if (!c) return fail(G4D_ERR_ARG, "context is NULL");
-    c->cam_grad = d_out;
+    c->terms.cam_grad = d_out;
     return G4D_OK;
 }
 
 int g4d_context_set_time_grad(G4DContext* c, float* d_out) {
     if (!c) return fail(G4D_ERR_ARG, "context is NULL");
-    c->time_grad = d_out;
+    c->terms.time_grad = d_out;
     return G4D_OK;
 }
 
 int g4d_context_set_depth_grad(G4DContext* c, const float* d_dL_ddepth) {
     if (!c) return fail(G4D_ERR_ARG, "context is NULL");
-    c->depth_grad = d_dL_ddepth;
+    c->terms.depth_grad = d_dL_ddepth;
     return G4D_OK;
 }
 
 int g4d_context_set_alpha_out(G4DContext* c, float* d_out) {
     if (!c) return fail(G4D_ERR_ARG, "context is NULL");
-    c->alpha_out = d_out;
+    c->terms.alpha_out = d_out;
     return G4D_OK;
 }
 
 int g4d_context_set_alpha_grad(G4DContext* c, const float* d_dL_dalpha) {
     if (!c) return fail(G4D_ERR_ARG, "context is NULL");
-    c->alpha_grad = d_dL_dalpha;
+    c->terms.alpha_grad = d_dL_dalpha;
     return G4D_OK;
 }
 

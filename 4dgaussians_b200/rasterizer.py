@@ -78,71 +78,86 @@ def camera_grad_leaves(rss):
     return tuple(spec), tuple(leaves)
 
 
-class CameraGradSinks:
-    """One [k, 35] float32 device buffer whose row i the backward on context ``ctxs[i]`` overwrites with its camera's
-    gradient, for the cameras named in ``spec``; with ``time``, one device float that the backward on ``ctxs[0]``
-    overwrites with dL/d(time) (g4d_context_set_time_grad); ``depths[i]``, when given and not None, the gradient of camera
-    i's depth image (contiguous fp32 CUDA, [H*W]) that the backward on ``ctxs[i]`` takes (g4d_context_set_depth_grad);
-    ``alphas[i]`` likewise for camera i's alpha image (g4d_context_set_alpha_grad).  The contexts' pointers are cleared
-    again on exit (they return to a pool)."""
-
-    def __init__(self, spec, ctxs, dev, time=False, depths=(), alphas=()):
-        self.cams = sorted({i for i, _ in spec})
-        self.ctxs = ctxs
-        self.buf = torch.empty(len(ctxs), 35, device=dev, dtype=torch.float32) if spec else None
-        self.tbuf = torch.empty(1, device=dev, dtype=torch.float32) if time else None
-        self.depths = [(i, d) for i, d in enumerate(depths) if d is not None]
-        self.alphas = [(i, a) for i, a in enumerate(alphas) if a is not None]
-
-    def __enter__(self):
-        for i in self.cams:
-            self.ctxs[i].set_camera_grad(self.buf[i].data_ptr())
-        if self.tbuf is not None:
-            self.ctxs[0].set_time_grad(self.tbuf.data_ptr())
-        for i, d in self.depths:
-            self.ctxs[i].set_depth_grad(d.data_ptr())
-        for i, a in self.alphas:
-            self.ctxs[i].set_alpha_grad(a.data_ptr())
-        return self
-
-    def __exit__(self, *exc):
-        for i in self.cams:
-            self.ctxs[i].set_camera_grad(None)
-        if self.tbuf is not None:
-            self.ctxs[0].set_time_grad(None)
-        for i, _ in self.depths:
-            self.ctxs[i].set_depth_grad(None)
-        for i, _ in self.alphas:
-            self.ctxs[i].set_alpha_grad(None)
-        return False
-
-    def grads(self, spec, metas):
-        """The gradient of each camera tensor of ``spec`` in its (shape, dtype, device), ``metas`` (``tensor_meta``)."""
-        return tuple(self.buf[i, off:off + n].reshape(shape).to(device=device, dtype=dtype)
-                     for (i, f), (shape, dtype, device) in zip(spec, metas) for _, off, n in (_CAM_FIELDS[f],))
-
-    def time_grad(self, meta):
-        """dL/d(time) in the time tensor's (shape, dtype, device), ``meta`` (one entry of ``tensor_meta``)."""
-        shape, dtype, device = meta
-        return self.tbuf.reshape(shape).to(device=device, dtype=dtype)
+def per_view(seq, k):
+    """The outputs of a render of k views, or their incoming gradients, in the order its autograd Function returns them:
+    (colour images, radii, depth images, alpha images), k of each, and no alpha images unless they are rendered."""
+    return seq[:k], seq[k:2 * k], seq[2 * k:3 * k], seq[3 * k:]
 
 
 @contextlib.contextmanager
-def alpha_outputs(ctxs, alphas):
-    """Inside the block every forward on ``ctxs[i]`` also writes its alpha image into ``alphas[i]`` (contiguous fp32 CUDA,
-    [1,H,W]; g4d_context_set_alpha_out).  The pointers are cleared again on exit: the contexts return to a pool and must
-    not keep writing into a tensor that may be freed."""
-    for c, a in zip(ctxs, alphas):
-        c.set_alpha_out(a.data_ptr())
+def _bound(terms):
+    """``terms``: (context, name of its ``set_*`` method, tensor or None).  Inside the block each context points at its
+    tensor; on exit, on an exception too, the pointers are cleared again: the contexts return to a pool and must not keep
+    reading or writing a tensor that may be freed."""
+    done = []
     try:
+        for c, setter, t in terms:
+            if t is not None:
+                getattr(c, setter)(t.data_ptr())
+                done.append((c, setter))
         yield
     finally:
-        for c in ctxs:
-            c.set_alpha_out(None)
+        for c, setter in done:
+            getattr(c, setter)(None)
 
 
-def tensor_meta(tensors):
-    return tuple((t.shape, t.dtype, t.device) for t in tensors)
+class ViewTerms:
+    """What the views of one render call, the settings ``rss``, take and give beyond their colour images, and its binding to
+    the contexts leased for the call, ``ctxs[i]`` for view i, for the one C-ABI call made inside ``forward`` or ``backward``.
+
+    Forward: each view's depth image and, with ``alpha``, its alpha image (g4d_context_set_alpha_out).  Backward: the depth
+    and alpha images' incoming gradients (g4d_context_set_depth_grad / _alpha_grad), the gradient of each camera tensor that
+    takes one (``camera_grad_leaves``; g4d_context_set_camera_grad) and, with ``time_leaf``, dL/d(time), which the backward
+    on ``ctxs[0]`` writes (g4d_context_set_time_grad).  ``leaves``: the camera tensors, then the time, that the caller
+    passes to its autograd Function as inputs."""
+
+    def __init__(self, rss, alpha=False, time_leaf=None):
+        self.rss, self.k, self.alpha, self.timed = rss, len(rss), bool(alpha), time_leaf is not None
+        self.cam_spec, cam_leaves = camera_grad_leaves(rss)
+        self.leaves = cam_leaves + ((time_leaf,) if self.timed else ())
+        self.metas = tuple((t.shape, t.dtype, t.device) for t in self.leaves)
+        self.cam_sink = self.time_sink = None
+
+    def outputs(self, dev, n):
+        """The fp32 images and the int32 radii of n Gaussians of every view, in ``per_view`` order."""
+        def images(c):
+            return [torch.empty(c, int(rs.image_height), int(rs.image_width), device=dev, dtype=torch.float32) for rs in self.rss]
+        return images(3), [torch.empty(n, device=dev, dtype=torch.int32) for _ in self.rss], images(1), \
+            images(1) if self.alpha else []
+
+    def forward(self, ctxs, alphas):
+        """``with``: the forward on ``ctxs[i]`` also writes view i's alpha image into ``alphas[i]``."""
+        return _bound([(c, "set_alpha_out", a) for c, a in zip(ctxs, alphas)])
+
+    def gradients(self, grads, dev):
+        """The incoming gradients ``grads`` (``per_view`` order) as contiguous fp32 CUDA buffers: per view its colour, depth
+        and alpha gradient, None for one outside the loss -- but with one view the colour gradient is zeros then, since the
+        single-camera backward entry points take an image gradient."""
+        gcol, _, gdep, galpha = per_view(grads, self.k)
+        hw = [int(rs.image_height) * int(rs.image_width) for rs in self.rss]
+        gcols = [_lib.cuda_f32(g, "grad_out_color", 3 * p) for g, p in zip(gcol, hw)]
+        if self.k == 1 and gcols[0] is None:
+            gcols[0] = torch.zeros(3 * hw[0], device=dev, dtype=torch.float32)
+        return gcols, [_lib.cuda_f32(g, "grad_out_depth", p) for g, p in zip(gdep, hw)], \
+            [_lib.cuda_f32(g, "grad_out_alpha", p) for g, p in zip(galpha, hw)]
+
+    def backward(self, ctxs, dev, depths=(), alphas=()):
+        """``with``: the backward on ``ctxs[i]`` takes ``depths[i]`` and ``alphas[i]`` (None: outside the loss) and writes the
+        sinks ``leaf_grads`` reads."""
+        cams = sorted({i for i, _ in self.cam_spec})
+        self.cam_sink = torch.empty(len(ctxs), 35, device=dev, dtype=torch.float32) if cams else None
+        self.time_sink = torch.empty(1, device=dev, dtype=torch.float32) if self.timed else None
+        return _bound([(ctxs[i], "set_camera_grad", self.cam_sink[i]) for i in cams] +
+                      [(ctxs[0], "set_time_grad", self.time_sink)] +
+                      [(c, "set_depth_grad", d) for c, d in zip(ctxs, depths)] +
+                      [(c, "set_alpha_grad", a) for c, a in zip(ctxs, alphas)])
+
+    def leaf_grads(self):
+        """The gradient of each tensor of ``leaves`` in its shape, dtype and device, from the last ``backward``'s sinks."""
+        rows = [self.cam_sink[i, off:off + n] for i, f in self.cam_spec for _, off, n in (_CAM_FIELDS[f],)]
+        if self.timed:
+            rows.append(self.time_sink)
+        return tuple(r.reshape(shape).to(device=device, dtype=dtype) for r, (shape, dtype, device) in zip(rows, self.metas))
 
 
 class _ContextLease:
@@ -166,55 +181,43 @@ class _ContextLease:
 
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, raster_settings, differentiable_depth, return_alpha,
-                cam_spec, *cam_leaves):
+    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, terms, differentiable_depth, *cam_leaves):
         lib = _lib.load()
         dev = means3D.device
         n = means3D.shape[0]
+        rs = terms.rss[0]
         m3 = _lib.cuda_f32(means3D, "means3D", n * 3)
         m = _lib.sh_coeffs(sh, n, "shs")
-        _lib.check_sh_degree(m, int(raster_settings.sh_degree))
+        _lib.check_sh_degree(m, int(rs.sh_degree))
         shc = _lib.cuda_f32(sh, "shs", n * 3 * m)
         op = _lib.cuda_f32(opacities, "opacities", n)
         sc = _lib.cuda_f32(scales, "scales", n * 3)
         ro = _lib.cuda_f32(rotations, "rotations", n * 4)
-        H, W = int(raster_settings.image_height), int(raster_settings.image_width)
-        color = torch.empty(3, H, W, device=dev, dtype=torch.float32)
-        depth = torch.empty(1, H, W, device=dev, dtype=torch.float32)
-        radii = torch.empty(n, device=dev, dtype=torch.int32)
+        (color,), (radii,), (depth,), alphas = terms.outputs(dev, n)
         keep = []
-        cam = camera_from_settings(raster_settings, keep=keep, sh_coeffs=m)
+        cam = camera_from_settings(rs, keep=keep, sh_coeffs=m)
         with torch.cuda.device(dev):
             lease = _ContextLease(_lib.workspace_of(dev))
-            alpha = torch.empty(1, H, W, device=dev, dtype=torch.float32) if return_alpha else None
-            with alpha_outputs([lease.ctx] if return_alpha else [], [alpha]):
+            with terms.forward([lease.ctx], alphas):
                 _lib.check(lib.g4d_rasterize_forward(lease.ctx.handle, C.byref(cam), n, m3.data_ptr(), shc.data_ptr(),
                                                      op.data_ptr(), sc.data_ptr(), ro.data_ptr(), color.data_ptr(),
                                                      depth.data_ptr(), radii.data_ptr(), _lib.stream_of(dev)),
                            "g4d_rasterize_forward")
-        ctx.raster_settings = raster_settings
-        ctx.cam_spec, ctx.cam_meta = cam_spec, tensor_meta(cam_leaves)
-        ctx.lease = lease
+        ctx.terms, ctx.lease = terms, lease
         ctx.n, ctx.m = n, m
         ctx.save_for_backward(m3, shc, op, sc, ro)
         ctx.mark_non_differentiable(*((radii,) if differentiable_depth else (radii, depth)))
         # a depth or alpha image outside the loss arrives as None: no depth or alpha gradient is set
         ctx.set_materialize_grads(False)
-        return (color, radii, depth, alpha) if return_alpha else (color, radii, depth)
+        return (color, radii, depth, *alphas)
 
     @staticmethod
-    def backward(ctx, grad_color, _grad_radii, grad_depth, grad_alpha=None):
+    def backward(ctx, *grads):
         lib = _lib.load()
         m3, shc, op, sc, ro = ctx.saved_tensors
         dev = m3.device
-        n = ctx.n
-        rs = ctx.raster_settings
-        hw = int(rs.image_height) * int(rs.image_width)
-        if grad_color is None:      # a depth- or alpha-only loss: the backward takes an image gradient
-            grad_color = torch.zeros(3 * hw, device=dev)
-        gcol = _lib.cuda_f32(grad_color, "grad_out_color", 3 * hw)
-        gdep = _lib.cuda_f32(grad_depth, "grad_out_depth", hw)
-        galpha = _lib.cuda_f32(grad_alpha, "grad_out_alpha", hw)
+        n, terms = ctx.n, ctx.terms
+        gcols, gdeps, galphas = terms.gradients(grads, dev)
         g_means3D = torch.empty(n, 3, device=dev)
         g_means2D = torch.empty(n, 3, device=dev)
         g_sh = torch.empty(n, ctx.m, 3, device=dev)
@@ -222,20 +225,18 @@ class _RasterizeGaussians(torch.autograd.Function):
         g_sc = torch.empty(n, 3, device=dev)
         g_ro = torch.empty(n, 4, device=dev)
         keep = []
-        cam = camera_from_settings(rs, keep=keep, sh_coeffs=ctx.m)
+        cam = camera_from_settings(terms.rss[0], keep=keep, sh_coeffs=ctx.m)
         lease = ctx.lease
         if lease is None or lease.ctx is None:
             raise RuntimeError("rasterizer backward called twice (context already released)")
-        sinks = CameraGradSinks(ctx.cam_spec, [lease.ctx], dev, depths=(gdep,), alphas=(galpha,))
-        with torch.cuda.device(dev), sinks:
+        with torch.cuda.device(dev), terms.backward([lease.ctx], dev, gdeps, galphas):
             _lib.check(lib.g4d_rasterize_backward(lease.ctx.handle, C.byref(cam), n, m3.data_ptr(), shc.data_ptr(), op.data_ptr(),
-                                                  sc.data_ptr(), ro.data_ptr(), gcol.data_ptr(), g_means3D.data_ptr(),
+                                                  sc.data_ptr(), ro.data_ptr(), gcols[0].data_ptr(), g_means3D.data_ptr(),
                                                   g_means2D.data_ptr(), g_sh.data_ptr(), g_op.data_ptr(), g_sc.data_ptr(),
                                                   g_ro.data_ptr(), _lib.stream_of(dev)), "g4d_rasterize_backward")
         lease.release()
         ctx.lease = None
-        cam_grads = sinks.grads(ctx.cam_spec, ctx.cam_meta) if ctx.cam_spec else ()
-        return (g_means3D, g_means2D, g_sh, g_op, g_sc, g_ro, None, None, None, None) + cam_grads
+        return (g_means3D, g_means2D, g_sh, g_op, g_sc, g_ro, None, None) + terms.leaf_grads()
 
 
 class GaussianRasterizer(nn.Module):
@@ -257,7 +258,6 @@ class GaussianRasterizer(nn.Module):
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
                 cov3D_precomp=None):
-        rs = self.raster_settings
         if (shs is None and colors_precomp is None) or (shs is not None and colors_precomp is not None):
             raise Exception('Please provide excatly one of either SHs or precomputed colors!')
         if ((scales is None or rotations is None) and cov3D_precomp is None) or \
@@ -267,6 +267,6 @@ class GaussianRasterizer(nn.Module):
             raise NotImplementedError("colors_precomp / cov3D_precomp are dead paths in the reference "
                                       "(gaussian_renderer/__init__.py:74-78,105-116) and are not provided")
         # the settings' viewmatrix / projmatrix / campos that require grad join the autograd graph as extra inputs
-        cam_spec, cam_leaves = camera_grad_leaves((rs,))
-        return _RasterizeGaussians.apply(means3D, means2D, shs, opacities, scales, rotations, rs, self.differentiable_depth,
-                                         self.return_alpha, cam_spec, *cam_leaves)
+        terms = ViewTerms((self.raster_settings,), self.return_alpha)
+        return _RasterizeGaussians.apply(means3D, means2D, shs, opacities, scales, rotations, terms, self.differentiable_depth,
+                                         *terms.leaves)

@@ -28,8 +28,8 @@ import torch
 
 from . import _lib
 from .deformation import deform_network, scalar_time
-from .rasterizer import (CameraGradSinks, GaussianRasterizationSettings, GaussianRasterizer, _ContextLease, alpha_outputs,
-                         camera_from_settings, camera_grad_leaves, tensor_meta)
+from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, ViewTerms, _ContextLease, camera_from_settings,
+                         per_view)
 
 
 def settings_from_camera(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, cam_type=None):
@@ -68,26 +68,21 @@ def time_grad_leaf(viewpoint_cameras, cam_type=None):
     return leaves[0]
 
 
-def _fused_forward(module: Optional[deform_network], rss, t, needs_bwd, want_alpha, xyz, scaling, rotation, opacity, f_dc,
+def _fused_forward(module: Optional[deform_network], terms: ViewTerms, t, needs_bwd, xyz, scaling, rotation, opacity, f_dc,
                    f_rest):
-    """One fused render call over the cameras' settings rss, one context lease per camera: g4d_render_forward for one
-    camera, g4d_render_forward_cameras for several.  Shared by the autograd Function and by the no-grad fast path.
-    want_alpha: the cameras' alpha maps are rendered too (else ``alphas`` is empty)."""
+    """One fused render call over the views of ``terms``, one context lease per camera: g4d_render_forward for one camera,
+    g4d_render_forward_cameras for several.  Shared by the autograd Function and by the no-grad fast path."""
     lib = _lib.load()
     dev = xyz.device
-    n, k = xyz.shape[0], len(rss)
+    n, k = xyz.shape[0], terms.k
     x, s = _lib.cuda_f32(xyz, "xyz", n * 3), _lib.cuda_f32(scaling, "scaling", n * 3)
     r, o = _lib.cuda_f32(rotation, "rotation", n * 4), _lib.cuda_f32(opacity, "opacity", n)
     m = _lib.sh_coeffs(f_rest, n, "features_rest", skip=1)
-    _lib.check_sh_degree(m, int(rss[0].sh_degree), module.head_mask() if module is not None else 0)
+    _lib.check_sh_degree(m, int(terms.rss[0].sh_degree), module.head_mask() if module is not None else 0)
     dc, rest = _lib.cuda_f32(f_dc, "features_dc", n * 3), _lib.cuda_f32(f_rest, "features_rest", n * 3 * (m - 1))
-    colors = [torch.empty(3, int(rs.image_height), int(rs.image_width), device=dev, dtype=torch.float32) for rs in rss]
-    depths = [torch.empty(1, int(rs.image_height), int(rs.image_width), device=dev, dtype=torch.float32) for rs in rss]
-    alphas = [torch.empty(1, int(rs.image_height), int(rs.image_width), device=dev, dtype=torch.float32)
-              for rs in rss] if want_alpha else []
-    radii = [torch.empty(n, device=dev, dtype=torch.int32) for _ in rss]
+    colors, radii, depths, alphas = terms.outputs(dev, n)
     keep = []
-    cams = [camera_from_settings(rs, time=t, keep=keep, sh_coeffs=m) for rs in rss]
+    cams = [camera_from_settings(rs, time=t, keep=keep, sh_coeffs=m) for rs in terms.rss]
     if not needs_bwd:
         for cam in cams:
             cam.debug |= _lib.CAM_NO_GRAD      # torch.no_grad() rendering: nothing is saved for a backward
@@ -98,9 +93,9 @@ def _fused_forward(module: Optional[deform_network], rss, t, needs_bwd, want_alp
     g = _lib.Gaussians(n, x.data_ptr(), s.data_ptr(), r.data_ptr(), o.data_ptr(), dc.data_ptr(), rest.data_ptr())
     with torch.cuda.device(dev):
         ws = _lib.workspace_of(dev)
-        leases = [_ContextLease(ws) for _ in rss]
+        leases = [_ContextLease(ws) for _ in cams]
         pm = C.byref(prm) if prm is not None else None
-        with alpha_outputs([lease.ctx for lease in leases] if want_alpha else [], alphas):
+        with terms.forward([lease.ctx for lease in leases], alphas):
             if k == 1:
                 cams, handles = cams[0], None       # one camera: the Camera itself, several: a Camera array
                 _lib.check(lib.g4d_render_forward(leases[0].ctx.handle, C.byref(cams), pm, C.byref(g), colors[0].data_ptr(),
@@ -119,21 +114,15 @@ def _pointers(tensors):
 
 
 class _FusedRender(torch.autograd.Function):
-    """inputs: xyz, scaling, rotation, opacity, features_dc, features_rest, k x means2D, *deform parameters, then the
-    camera tensors that take a gradient (cam_spec: their (camera, field) pairs, rasterizer.camera_grad_leaves), then, when
-    ``timed``, the time tensor that takes a gradient (time_grad_leaf); outputs: k images, k radii, k depth maps, and with
-    ``want_alpha`` k alpha maps"""
+    """inputs: xyz, scaling, rotation, opacity, features_dc, features_rest, k x means2D, *deform parameters, then
+    ``terms.leaves`` (the camera and time tensors that take a gradient); outputs (``per_view``): k images, k radii, k depth
+    maps, and with ``terms.alpha`` k alpha maps"""
 
     @staticmethod
-    def forward(ctx, module: Optional[deform_network], rss, t, cam_spec, timed, want_alpha, xyz, scaling, rotation, opacity,
-                f_dc, f_rest, *rest):
-        colors, radii, depths, alphas, leases, cstructs, saved = _fused_forward(module, rss, t, any(ctx.needs_input_grad),
-                                                                                want_alpha, xyz, scaling, rotation, opacity,
-                                                                                f_dc, f_rest)
-        ctx.module, ctx.rss, ctx.n, ctx.leases = module, rss, xyz.shape[0], leases
-        end = len(rest) - int(timed)
-        ctx.cam_spec, ctx.cam_meta = cam_spec, tensor_meta(rest[end - len(cam_spec):end])
-        ctx.time_meta = tensor_meta(rest[end:])[0] if timed else None
+    def forward(ctx, module: Optional[deform_network], terms, t, xyz, scaling, rotation, opacity, f_dc, f_rest, *rest):
+        colors, radii, depths, alphas, leases, cstructs, saved = _fused_forward(module, terms, t, any(ctx.needs_input_grad),
+                                                                                xyz, scaling, rotation, opacity, f_dc, f_rest)
+        ctx.module, ctx.terms, ctx.n, ctx.leases = module, terms, xyz.shape[0], leases
         ctx.lease = leases[0]        # camera 0's context: what a render() caller reads the forward's buffers through
         # the C-ABI structs (and the tensors whose pointers they carry) are kept for the backward: rebuilding them costs the
         # host ~0.3 ms per view, during which the GPU has nothing queued behind the forward's last kernel
@@ -149,18 +138,13 @@ class _FusedRender(torch.autograd.Function):
     def backward(ctx, *grads):
         lib = _lib.load()
         x, s, r, o, dc, rest = ctx.saved_tensors
-        dev, n, rss, module = x.device, ctx.n, ctx.rss, ctx.module
-        k = len(rss)
+        dev, n, terms, module = x.device, ctx.n, ctx.terms, ctx.module
+        k = terms.k
         leases = ctx.leases
         if leases is None:
             raise RuntimeError("render backward called twice (context already released)" if k == 1 else
                                "render_cameras backward called twice (contexts already released)")
-        gcols = [None if gc is None else _lib.cuda_f32(gc, "grad_out_color", 3 * int(rs.image_height) * int(rs.image_width))
-                 for gc, rs in zip(grads[:k], rss)]
-        gdeps = [_lib.cuda_f32(gd, "grad_out_depth", int(rs.image_height) * int(rs.image_width))
-                 for gd, rs in zip(grads[2 * k:3 * k], rss)]
-        galphas = [_lib.cuda_f32(ga, "grad_out_alpha", int(rs.image_height) * int(rs.image_width))
-                   for ga, rs in zip(grads[3 * k:], rss)]
+        gcols, gdeps, galphas = terms.gradients(grads, dev)
         cams, prm, g, keep, version, handles = ctx.cstructs
         if module is not None and version != module._param_version:      # another forward ran since: take the current key
             keep = []
@@ -178,12 +162,8 @@ class _FusedRender(torch.autograd.Function):
         gm2 = [flat[(end + 3 * i) * npad:(end + 3 * i) * npad + 3 * n].view(n, 3) for i in range(k)]
         gg = _lib.GaussianGrads(gx.data_ptr(), gs.data_ptr(), gr.data_ptr(), go.data_ptr(), gdc.data_ptr(), grest.data_ptr(),
                                 gm2[0].data_ptr() if k == 1 else None)
-        sinks = CameraGradSinks(ctx.cam_spec, [lease.ctx for lease in leases], dev, time=ctx.time_meta is not None,
-                                depths=gdeps, alphas=galphas)
-        with torch.cuda.device(dev), sinks:
+        with torch.cuda.device(dev), terms.backward([lease.ctx for lease in leases], dev, gdeps, galphas):
             if k == 1:
-                if gcols[0] is None:        # the single-camera backward takes an image gradient
-                    gcols[0] = torch.zeros(3 * int(rss[0].image_height) * int(rss[0].image_width), device=dev)
                 _lib.check(lib.g4d_render_backward(leases[0].ctx.handle, C.byref(cams), C.byref(prm) if prm is not None else None,
                                                    C.byref(cg) if cg is not None else None, C.byref(g), gcols[0].data_ptr(),
                                                    C.byref(gg), _lib.stream_of(dev)), "g4d_render_backward")
@@ -195,9 +175,7 @@ class _FusedRender(torch.autograd.Function):
         for lease in leases:
             lease.release()
         ctx.leases = ctx.lease = None
-        cam_grads = sinks.grads(ctx.cam_spec, ctx.cam_meta) if ctx.cam_spec else ()
-        time_grad = (sinks.time_grad(ctx.time_meta),) if ctx.time_meta is not None else ()
-        return (None, None, None, None, None, None, gx, gs, gr, go, gdc, grest) + tuple(gm2) + tuple(pgrads) + cam_grads + time_grad
+        return (None, None, None, gx, gs, gr, go, gdc, grest) + tuple(gm2) + tuple(pgrads) + terms.leaf_grads()
 
 
 def _time_bits(t) -> bytes:
@@ -255,21 +233,18 @@ def _render(viewpoint_cameras, pc, pipe, bg_color, scaling_modifier, override_co
     else:       # nothing will ever flow into them: a cached all-zero tensor instead of a memset (+ add) launch per view
         points = [_zero_points(xyz)] * k
     if module is None or isinstance(module, deform_network):
+        terms = ViewTerms(rss, return_alpha, time_leaf)
         if not torch.is_grad_enabled():
             # no autograd node to build: skip Function.apply and its per-input bookkeeping (40 inputs with the network's parameters)
-            images, radii, depths, alphas, leases, _, _ = _fused_forward(module, rss, t, False, return_alpha, xyz, pc._scaling,
-                                                                         pc._rotation, pc._opacity, pc._features_dc,
-                                                                         pc._features_rest)
+            images, radii, depths, alphas, leases, _, _ = _fused_forward(module, terms, t, False, xyz, pc._scaling, pc._rotation,
+                                                                         pc._opacity, pc._features_dc, pc._features_rest)
             for lease in leases:
                 lease.release()
         else:
             params = tuple(module.flat_parameters()) if module is not None else ()
-            cam_spec, cam_leaves = camera_grad_leaves(rss)      # camera tensors that require grad: extra inputs
-            time_leaves = () if time_leaf is None else (time_leaf,)
-            outs = _FusedRender.apply(module, rss, t, cam_spec, time_leaf is not None, return_alpha, xyz, pc._scaling,
-                                      pc._rotation, pc._opacity, pc._features_dc, pc._features_rest, *points, *params, *cam_leaves,
-                                      *time_leaves)
-            images, radii, depths, alphas = outs[:k], outs[k:2 * k], outs[2 * k:3 * k], outs[3 * k:]
+            outs = _FusedRender.apply(module, terms, t, xyz, pc._scaling, pc._rotation, pc._opacity, pc._features_dc,
+                                      pc._features_rest, *points, *params, *terms.leaves)
+            images, radii, depths, alphas = per_view(outs, k)
     else:
         # a foreign (e.g. the reference's own PyTorch) deformation module: keep its semantics, deform once, then rasterize
         # every camera with g4d

@@ -140,34 +140,44 @@ class _FakeContext:
         self.log.append(("out", self.i, p))
 
 
-def test_alpha_gradient_is_set_for_the_call_only():
+def _views(k):
+    rs = rasterizer.GaussianRasterizationSettings(4, 3, 0.5, 0.5, torch.zeros(3), 1.0, torch.eye(4), torch.eye(4), 0,
+                                                  torch.zeros(3), False, False)
+    return [rs] * k
+
+
+def test_view_terms_set_the_alpha_gradient_for_the_call_only():
     log = []
     ctxs = [_FakeContext(log, i) for i in range(3)]
     a2, d0 = torch.zeros(12), torch.zeros(12)
-    with rasterizer.CameraGradSinks((), ctxs, torch.device("cpu"), depths=(d0,), alphas=(None, None, a2)):
+    with rasterizer.ViewTerms(_views(3)).backward(ctxs, torch.device("cpu"), depths=(d0,), alphas=(None, None, a2)):
         assert log == [("depth", 0, d0.data_ptr()), ("alpha", 2, a2.data_ptr())]
     assert log[2:] == [("depth", 0, None), ("alpha", 2, None)]
 
 
-def test_no_alpha_gradient_sets_nothing():
+def test_view_terms_without_an_alpha_gradient_set_nothing():
     log = []
     ctxs = [_FakeContext(log, i) for i in range(2)]
     for alphas in ((), (None, None)):
-        with rasterizer.CameraGradSinks((), ctxs, torch.device("cpu"), alphas=alphas):
+        with rasterizer.ViewTerms(_views(2)).backward(ctxs, torch.device("cpu"), alphas=alphas):
             pass
     assert log == []
 
 
-def test_alpha_output_is_set_for_the_forward_only():
+def test_view_terms_set_the_alpha_output_for_the_forward_only():
     log = []
     ctxs = [_FakeContext(log, i) for i in range(2)]
-    outs = [torch.zeros(4), torch.zeros(4)]
+    terms = rasterizer.ViewTerms(_views(2), alpha=True)
+    outs = terms.outputs(torch.device("cpu"), 5)[3]
+    assert [tuple(a.shape) for a in outs] == [(1, 4, 3), (1, 4, 3)]
     with pytest.raises(RuntimeError):
-        with rasterizer.alpha_outputs(ctxs, outs):
+        with terms.forward(ctxs, outs):
             assert log == [("out", 0, outs[0].data_ptr()), ("out", 1, outs[1].data_ptr())]
             raise RuntimeError("a failed forward")
     assert log[2:] == [("out", 0, None), ("out", 1, None)]
     log.clear()
-    with rasterizer.alpha_outputs([], []):
+    no_alpha = rasterizer.ViewTerms(_views(2))
+    assert no_alpha.outputs(torch.device("cpu"), 5)[3] == []
+    with no_alpha.forward(ctxs, []):
         pass
     assert log == []

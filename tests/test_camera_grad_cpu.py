@@ -111,11 +111,26 @@ def test_camera_grad_leaves():
         assert rasterizer.camera_grad_leaves([_settings(vl, p, cl)]) == ((), ())
 
 
-def test_camera_grads_take_the_callers_layout():
-    sinks = rasterizer.CameraGradSinks(((0, 0), (0, 1), (0, 2)), [None], "cpu")
-    sinks.buf.copy_(torch.arange(35, dtype=torch.float32))
-    metas = rasterizer.tensor_meta((torch.zeros(4, 4, dtype=torch.float64), torch.zeros(16), torch.zeros(1, 3, dtype=torch.float16)))
-    gv, gp, gc = sinks.grads(((0, 0), (0, 1), (0, 2)), metas)
+class _FakeContext:
+    def __init__(self, log, i):
+        self.log, self.i = log, i
+
+    def set_camera_grad(self, p):
+        self.log.append(("camera", self.i, p))
+
+
+def test_view_terms_return_camera_grads_in_the_callers_layout():
+    v, p, c = torch.eye(4), torch.eye(4), torch.zeros(3)
+    leaves = (torch.zeros(4, 4, dtype=torch.float64, requires_grad=True), torch.zeros(16, requires_grad=True),
+              torch.zeros(1, 3, dtype=torch.float16, requires_grad=True))
+    terms = rasterizer.ViewTerms([_settings(v, p, c), _settings(*leaves)])
+    assert terms.cam_spec == ((1, 0), (1, 1), (1, 2)) and all(a is b for a, b in zip(terms.leaves, leaves))
+    log = []
+    with terms.backward([_FakeContext(log, 0), _FakeContext(log, 1)], "cpu"):
+        assert log == [("camera", 1, terms.cam_sink[1].data_ptr())]
+        terms.cam_sink[1].copy_(torch.arange(35, dtype=torch.float32))
+    assert log[1:] == [("camera", 1, None)]
+    gv, gp, gc = terms.leaf_grads()
     assert gv.shape == (4, 4) and gv.dtype == torch.float64 and gv.reshape(-1).tolist() == list(range(16))
     assert gp.shape == (16,) and gp.tolist() == list(range(16, 32))
     assert gc.shape == (1, 3) and gc.dtype == torch.float16 and gc.reshape(-1).tolist() == [32, 33, 34]

@@ -169,19 +169,27 @@ class _FakeContext:
         self.log.append(("depth", self.i, p))
 
 
-def test_depth_gradient_is_set_for_the_call_only():
+def _views(k):
+    rs = rasterizer.GaussianRasterizationSettings(4, 3, 0.5, 0.5, torch.zeros(3), 1.0, torch.eye(4), torch.eye(4), 0,
+                                                  torch.zeros(3), False, False)
+    return [rs] * k
+
+
+def test_view_terms_set_the_depth_gradient_for_the_call_only():
     log = []
     ctxs = [_FakeContext(log, i) for i in range(3)]
     d1 = torch.zeros(12)
-    with rasterizer.CameraGradSinks((), ctxs, torch.device("cpu"), depths=(None, d1, None)):
-        assert log == [("depth", 1, d1.data_ptr())]
+    with pytest.raises(RuntimeError):
+        with rasterizer.ViewTerms(_views(3)).backward(ctxs, torch.device("cpu"), depths=(None, d1, None)):
+            assert log == [("depth", 1, d1.data_ptr())]
+            raise RuntimeError("a failed backward")
     assert log == [("depth", 1, d1.data_ptr()), ("depth", 1, None)]
 
 
-def test_no_depth_gradient_sets_nothing():
+def test_view_terms_without_a_depth_gradient_set_nothing():
     log = []
     ctxs = [_FakeContext(log, i) for i in range(2)]
     for depths in ((), (None, None)):
-        with rasterizer.CameraGradSinks((), ctxs, torch.device("cpu"), depths=depths):
+        with rasterizer.ViewTerms(_views(2)).backward(ctxs, torch.device("cpu"), depths=depths):
             pass
     assert log == []

@@ -167,11 +167,26 @@ def test_render_cameras_refuses_distinct_time_tensors(times):
         renderer.render_cameras([_Cam(a), _Cam(b)], None, _Pipe, None)
 
 
-def test_time_grad_takes_the_callers_layout():
-    sinks = rasterizer.CameraGradSinks((), [None], "cpu", time=True)
-    sinks.tbuf.fill_(2.5)
+class _FakeContext:
+    def __init__(self, log, i):
+        self.log, self.i = log, i
+
+    def set_time_grad(self, p):
+        self.log.append(("time", self.i, p))
+
+
+def test_view_terms_return_the_time_grad_of_camera_0_in_the_callers_layout():
+    rs = rasterizer.GaussianRasterizationSettings(4, 3, 0.5, 0.5, torch.zeros(3), 1.0, torch.eye(4), torch.eye(4), 0,
+                                                  torch.zeros(3), False, False)
     for leaf in (torch.tensor(0.0, dtype=torch.float64), torch.zeros(1, 1, dtype=torch.float16), torch.zeros(1)):
-        g = sinks.time_grad(rasterizer.tensor_meta((leaf,))[0])
+        log = []
+        terms = rasterizer.ViewTerms([rs, rs], time_leaf=leaf)
+        assert terms.leaves[0] is leaf
+        with terms.backward([_FakeContext(log, 0), _FakeContext(log, 1)], "cpu"):
+            assert log == [("time", 0, terms.time_sink.data_ptr())]
+            terms.time_sink.fill_(2.5)
+        assert log[1:] == [("time", 0, None)]
+        (g,) = terms.leaf_grads()
         assert g.shape == leaf.shape and g.dtype == leaf.dtype and float(g.reshape(-1)[0]) == 2.5
 
 
