@@ -30,7 +30,7 @@ UNITS = {
     "g4d_knn.cu": ["-fmad=false"],
     "g4d_optim.cu": [],
     "g4d_backward.cu": [],
-    "g4d_backward_depth.cu": [],
+    "g4d_geom_bwd.cu": [],
     "g4d_api.cu": [],
     "g4d_deform_tc.cu": ["-fmad=false"],
     "g4d_deform_tc_bwd.cu": [],

@@ -1,39 +1,13 @@
-// g4d_backward.cu -- per-Gaussian backward of the projection stage (A.4; kernels in per_gaussian_bwd.cuh, the instances with a
-// depth gradient in g4d_backward_depth.cu) and the backward of the deformation network: the
-// frame every backward runs (HexPlane gather, scatter, time-row distribution) around the FFMA engine here or the tensor-core
-// engine of g4d_deform_tc_bwd.cu.  Compiled with the default FMA contraction: the coordinate normalisation of the scatter
+// g4d_backward.cu -- backward of the deformation network: the frame every backward runs (HexPlane gather, scatter, time-row
+// distribution) around the FFMA engine here or the tensor-core engine of g4d_deform_tc_bwd.cu, and the chain rule through
+// the activations.  Compiled with the default FMA contraction: the coordinate normalisation of the scatter
 // rounds explicitly, as the forward's gather does (hexplane.cuh).
 // Reference autograd path replaced: loss.backward() at /root/reference/train.py:219 through
 // _RasterizeGaussians.backward, F.normalize/exp/sigmoid, nn.Linear, F.grid_sample.
 #include "g4d_internal.h"
 #include "g4d_math.cuh"
-#include "per_gaussian_bwd.cuh"
 
 namespace g4d {
-
-cudaError_t launch_preprocess_backward(const CameraDev* cam, int64_t n, const RasterInputs& in, GeomBuffers g,
-                                       const float* g_mean2D, const float* g_conic, const float* g_rgb, float* g_means3D,
-                                       float* g_means2D_out, float* g_scales, float* g_rotations, const ShOut& g_sh,
-                                       float* g_cam, const float* g_depth, cudaStream_t st) {
-    if (g_depth)
-        return launch_preprocess_backward_depth(cam, n, in, g, g_mean2D, g_conic, g_rgb, g_means3D, g_means2D_out, g_scales,
-                                                g_rotations, g_sh, g_cam, g_depth, st);
-    return launch_per_gaussian_backward(preprocess_backward_kernel<false, false, false>, preprocess_backward_kernel<false, true, false>,
-                                        preprocess_backward_kernel<true, false, false>, preprocess_backward_kernel<true, true, false>,
-                                        g_sh.m == kShCoeffs, g_cam != nullptr, n, st, cam, n, in, g, g_mean2D, g_conic, g_rgb,
-                                        g_means3D, g_means2D_out, g_scales, g_rotations, g_sh, g_cam, g_depth);
-}
-
-cudaError_t launch_preprocess_backward_cameras(const BackwardCameras& bc, int64_t n, const RasterInputs& in, float* g_means3D,
-                                               float* g_scales, float* g_rotations, float* g_opacities, const ShOut& g_sh,
-                                               const CamGradSinks* cs, bool depth, cudaStream_t st) {
-    if (depth) return launch_preprocess_backward_cameras_depth(bc, n, in, g_means3D, g_scales, g_rotations, g_opacities, g_sh, cs, st);
-    return launch_per_gaussian_backward(
-        preprocess_backward_cameras_kernel<false, false, false>, preprocess_backward_cameras_kernel<false, true, false>,
-        preprocess_backward_cameras_kernel<true, false, false>, preprocess_backward_cameras_kernel<true, true, false>,
-        g_sh.m == kShCoeffs, cs != nullptr, n, st, bc, n, in, g_means3D, g_scales, g_rotations, g_opacities, g_sh,
-        cs ? *cs : CamGradSinks{});
-}
 
 // ======================================================================================================
 // Backward of the deformation network (DESIGN.md §4): one frame (launch_deform_backward) around one of two engines.
@@ -589,15 +563,13 @@ static cudaError_t launch_bwd_scatter(const DeformBwdArgs& ba, int64_t n, const 
     switch (C4) {   // every channel width the C-ABI takes: C = 4 .. 32
 #define G4D_SCATTER_CASE(K)                                                     \
         case K:                                                                 \
-            if (ba.d.times) bwd_scatter_kernel<K, true><<<grid, 256, 0, st>>>(ba, n, xyz); \
-            else bwd_scatter_kernel<K, false><<<grid, 256, 0, st>>>(ba, n, xyz);          \
-            break;
+            return launch_k(ba.d.times ? bwd_scatter_kernel<K, true> : bwd_scatter_kernel<K, false>, grid, 256, 0, st, kOrdinary, \
+                            ba, n, xyz);
         G4D_SCATTER_CASE(1) G4D_SCATTER_CASE(2) G4D_SCATTER_CASE(3) G4D_SCATTER_CASE(4)
         G4D_SCATTER_CASE(5) G4D_SCATTER_CASE(6) G4D_SCATTER_CASE(7) G4D_SCATTER_CASE(8)
 #undef G4D_SCATTER_CASE
-        default: return cudaErrorInvalidValue;
     }
-    return cudaGetLastError();
+    return cudaErrorInvalidValue;
 }
 
 // ---- kernel T: collapsed time-row gradients -> the two time rows of each (axis, t) plane --------------------
@@ -643,9 +615,8 @@ static cudaError_t launch_distribute_time_grad(const DeformBwdArgs& ba, TimeArg 
             s.plane[l][a] = d.planes[l][kTimePlane[a]];
         }
     const int total = (int)s.total();
-    if (g_time) distribute_time_grad_kernel<true><<<(total + 255) / 256, 256, 0, st>>>(s, time, g_time);
-    else distribute_time_grad_kernel<false><<<(total + 255) / 256, 256, 0, st>>>(s, time, nullptr);
-    return cudaGetLastError();
+    return launch_k(g_time ? distribute_time_grad_kernel<true> : distribute_time_grad_kernel<false>, (total + 255) / 256, 256, 0, st,
+                    kOrdinary, s, time, g_time);
 }
 
 // carves the scratch; *gathered: where the gather writes the features (buf.feat until the forward's replace them)
@@ -694,10 +665,10 @@ static cudaError_t launch_ffma_engine(const DeformBwdArgs& ba, int64_t n, int sm
     for (int j = 0; j <= d.ntrunk; ++j) {
         const int K = j == 0 ? d.F : WD;
         const PrepassSmem L = prepass_smem_layout(TG, K, WD);
-        e = j == 0 ? launch_smem(deform_bwd_prepass_kernel<TG, WD>, grid, kDeformThreads, (size_t)L.total_floats * 4, st, L, n, K,
-                                 buf.feat, d.w0t, d.b0, buf.act[0])
-                   : launch_smem(deform_bwd_prepass_kernel<TG, WD>, grid, kDeformThreads, (size_t)L.total_floats * 4, st, L, n, K,
-                                 buf.act[j - 1], d.wtt[j - 1], d.bt[j - 1], buf.act[j]);
+        e = j == 0 ? launch_k(deform_bwd_prepass_kernel<TG, WD>, grid, kDeformThreads, (size_t)L.total_floats * 4, st, kOrdinary, L, n,
+                              K, buf.feat, d.w0t, d.b0, buf.act[0])
+                   : launch_k(deform_bwd_prepass_kernel<TG, WD>, grid, kDeformThreads, (size_t)L.total_floats * 4, st, kOrdinary, L, n,
+                              K, buf.act[j - 1], d.wtt[j - 1], d.bt[j - 1], buf.act[j]);
         if (e != cudaSuccess) return e;
     }
     // H
@@ -706,15 +677,16 @@ static cudaError_t launch_ffma_engine(const DeformBwdArgs& ba, int64_t n, int sm
         int hgrid = sm_count;
         if ((int64_t)hgrid > ntiles * active) hgrid = (int)(ntiles * active);
         if (hgrid < active) hgrid = active;
-        e = launch_smem(deform_bwd_heads_kernel<TG, WD>, hgrid, kDeformThreads, (size_t)L.total_floats * 4, st, ba, L, n, active);
+        e = launch_k(deform_bwd_heads_kernel<TG, WD>, hgrid, kDeformThreads, (size_t)L.total_floats * 4, st, kOrdinary, ba, L, n,
+                     active);
         if (e != cudaSuccess) return e;
     }
     // T: dA_{j-1} from dA_j, j = ntrunk .. 1 (dA_ntrunk: the heads' DA1 sum)
     const float* din = nullptr;
     const TrunkSmem LT = trunk_smem_layout(TG, WD);
     for (int j = d.ntrunk, k = 0; j >= 1; --j, k ^= 1) {
-        e = launch_smem(deform_bwd_trunk_kernel<TG, WD>, grid, kDeformThreads, (size_t)LT.total_floats * 4, st, ba, LT, n, j, din,
-                        buf.dact[k]);
+        e = launch_k(deform_bwd_trunk_kernel<TG, WD>, grid, kDeformThreads, (size_t)LT.total_floats * 4, st, kOrdinary, ba, LT, n, j,
+                     din, buf.dact[k]);
         if (e != cudaSuccess) return e;
         din = buf.dact[k];
     }
@@ -722,7 +694,7 @@ static cudaError_t launch_ffma_engine(const DeformBwdArgs& ba, int64_t n, int sm
     const FinalSmem L = final_smem_layout(TG, d.F, WD);
     auto final_kernel = d.F <= 32 ? deform_bwd_final_kernel<TG, WD, 32>
                       : d.F <= 64 ? deform_bwd_final_kernel<TG, WD, 64> : deform_bwd_final_kernel<TG, WD, 128>;
-    return launch_smem(final_kernel, grid, kDeformThreads, (size_t)L.total_floats * 4, st, ba, L, n, din);
+    return launch_k(final_kernel, grid, kDeformThreads, (size_t)L.total_floats * 4, st, kOrdinary, ba, L, n, din);
 }
 
 cudaError_t launch_deform_backward(const DeformDesc& d, const G4DDeformParams& prm, const G4DDeformGrads& grads, const TcBwdWeights* tc,
@@ -780,8 +752,8 @@ activation_backward_kernel(int64_t n, FusedOutputs fo, float* __restrict__ g_sca
 cudaError_t launch_activation_backward(int64_t n, const FusedOutputs& fo, float* g_scales, float* g_rotations,
                                        float* g_opacities, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
-    activation_backward_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, fo, g_scales, g_rotations, g_opacities);
-    return cudaGetLastError();
+    return launch_k(activation_backward_kernel, (unsigned)((n + 255) / 256), 256, 0, st, kOrdinary, n, fo, g_scales, g_rotations,
+                    g_opacities);
 }
 
 }  // namespace g4d

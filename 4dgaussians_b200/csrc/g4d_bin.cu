@@ -73,7 +73,7 @@ __device__ __forceinline__ uint32_t block_scan_incl(uint32_t v, uint32_t* s_w, u
     return x + s_w[warp];
 }
 
-// Grid-wide barrier of the cooperative bin_sort_kernel (all CTAs co-resident: cudaLaunchCooperativeKernel).  A monotonic arrival
+// Grid-wide barrier of the cooperative bin_sort_kernel (all CTAs co-resident: a kCooperative launch).  A monotonic arrival
 // counter, one release-arrive and an acquire-spin by thread 0 of every CTA, lighter than cooperative_groups' grid.sync() (nine
 // of them are on the critical path of one forward).
 struct GridBar {
@@ -647,10 +647,7 @@ cudaError_t launch_bin_sort(int64_t n, int grid_x, int grid_y, const GeomBuffers
     if (smem < kSortSmemBytes) smem = kSortSmemBytes;
     out->chunk_start = a.chunk_start; out->M = a.M; out->tile_total = a.tile_total; out->tile_start = tile_start; out->ctl = a.ctl;
     out->chunks = sm_count;
-    cudaError_t e = cudaFuncSetAttribute(bin_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    void* args[] = {&a};
-    return cudaLaunchCooperativeKernel((const void*)bin_sort_kernel, dim3((unsigned)sm_count), dim3(kBinThreads), args, smem, st);
+    return launch_k(bin_sort_kernel, dim3((unsigned)sm_count), dim3(kBinThreads), smem, st, kCooperative, a);
 }
 
 cudaError_t launch_bin_place(int grid_x, int grid_y, const GeomBuffers& g, const BinLayout& lay, uint32_t* ids, uint2* kbuf,
@@ -664,11 +661,10 @@ cudaError_t launch_bin_place(int grid_x, int grid_y, const GeomBuffers& g, const
     if (a.band_rows < 1) return cudaErrorInvalidValue;
     if (a.band_rows > grid_y) a.band_rows = grid_y;
     const size_t smem = 4 * (size_t)a.band_rows * grid_x;
-    cudaError_t e = cudaFuncSetAttribute(bin_place_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    const cudaError_t e = launch_k(bin_place_kernel, dim3(lay.chunks), dim3(kBinThreads), smem, st, kPdl, a);
     if (e != cudaSuccess) return e;
-    if ((e = launch_k(bin_place_kernel, dim3(lay.chunks), dim3(kBinThreads), smem, st, true, a)) != cudaSuccess) return e;
     const int rounds = (lay.chunks + 31) / 32;
-    return launch_k(bin_fix_kernel, dim3((num_tiles * rounds + 7) / 8), dim3(256), 0, st, true, a, lay.chunks);
+    return launch_k(bin_fix_kernel, dim3((num_tiles * rounds + 7) / 8), dim3(256), 0, st, kPdl, a, lay.chunks);
 }
 
 // One thread, ordinary launch (after the blend: no programmatic edge to break).  The forwards of a stream run one after the
@@ -681,8 +677,7 @@ __global__ void record_overflow_kernel(const BinCtl* ctl, uint32_t capacity, vol
 }
 
 cudaError_t launch_record_overflow(const BinCtl* ctl, uint32_t capacity, uint32_t* words, cudaStream_t st) {
-    record_overflow_kernel<<<1, 1, 0, st>>>(ctl, capacity, words);
-    return cudaGetLastError();
+    return launch_k(record_overflow_kernel, 1, 1, 0, st, kOrdinary, ctl, capacity, words);
 }
 
 }  // namespace g4d

@@ -92,15 +92,34 @@ G4D_D void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: 
 
 extern int g_pdl;   // process-wide switch (G4D_OPT_PDL / env G4D_PDL; g4d_api.cu)
 
-// <<<grid, block, smem, st>>> with the programmatic-stream-serialization attribute when `pdl` is set
+// how a launch follows the kernels before it in its stream
+enum LaunchDep {
+    kOrdinary,      // once the previous kernel has completed
+    kPdl,           // with the programmatic-stream-serialization attribute when g_pdl is set (above)
+    kCooperative,   // as kOrdinary, with all CTAs resident at once: the kernel has grid-wide barriers
+};
+
+// The one way libg4d.so launches a kernel: <<<grid, block, smem, st>>> as `dep` says.  The default dynamic shared memory
+// limit is 48 KiB less the kernel's static shared memory, so a launch that asks for any dynamic shared memory first sets
+// the limit to `smem`.  Returns the error of this launch (or of setting the limit).
 template <class... KArgs, class... Args>
-inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl, Args&&... args) {
+inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, LaunchDep dep,
+                            Args&&... args) {
+    if (smem > 0) {
+        const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+    }
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = (pdl && g_pdl) ? 1 : 0;
+    cudaLaunchAttribute attr{};
+    if (dep == kCooperative) {
+        attr.id = cudaLaunchAttributeCooperative;
+        attr.val.cooperative = 1;
+    } else {
+        attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attr.val.programmaticStreamSerializationAllowed = 1;
+    }
+    cfg.attrs = &attr; cfg.numAttrs = dep == kCooperative || (dep == kPdl && g_pdl) ? 1 : 0;
     return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 

@@ -128,8 +128,7 @@ cudaError_t launch_tc_pack_weights(const G4DDeformParams& prm, float* blob, TcWe
         if (h == 4) out->w2[h] = add(prm.w2[h], 48, 128);   // the small heads' layer 2 runs in fp32 from the caller's tensors
     }
     p.start[m] = total; p.count = m;
-    tc_pack_weights_kernel<<<(total + 255) / 256, 256, 0, st>>>(p);
-    return cudaGetLastError();
+    return launch_k(tc_pack_weights_kernel, (total + 255) / 256, 256, 0, st, kOrdinary, p);
 }
 
 // ---- fragments ----------------------------------------------------------------------------------------------------------
@@ -525,10 +524,9 @@ cudaError_t launch_gather_order(const float* aabb, int64_t n, const float* xyz, 
     cudaError_t e = cudaMemsetAsync(b.cell_start, 0, (size_t)kOrderCells * 4, st);
     if (e != cudaSuccess) return e;
     const unsigned grid = (unsigned)((n + 255) / 256);
-    order_count_kernel<<<grid, 256, 0, st>>>(aabb, n, xyz, b);
-    order_scan_kernel<<<kOrderCells / 1024, 256, 0, st>>>(b);
-    order_scatter_kernel<<<grid, 256, 0, st>>>(n, b);
-    return cudaGetLastError();
+    if ((e = launch_k(order_count_kernel, grid, 256, 0, st, kOrdinary, aabb, n, xyz, b)) != cudaSuccess) return e;
+    if ((e = launch_k(order_scan_kernel, kOrderCells / 1024, 256, 0, st, kOrdinary, b)) != cudaSuccess) return e;
+    return launch_k(order_scatter_kernel, grid, 256, 0, st, kOrdinary, n, b);
 }
 
 // ---- HexPlane gather at full occupancy: C/4 threads per Gaussian, one channel vector each -> feat [N][F] fp32 -----------
@@ -569,8 +567,8 @@ cudaError_t launch_deform_features(const DeformDesc& d, int64_t n, const float* 
     const unsigned grid = (unsigned)((n * C4 + 255) / 256);
     switch (C4) {   // every channel width the C-ABI takes: C = 4 .. 32
 #define G4D_GATHER_CASE(K)                                                                                                  \
-        case K: return d.times ? launch_k(deform_features_kernel<K, true>, dim3(grid), dim3(256), 0, st, pdl, d, n, xyz, order, feat) \
-                               : launch_k(deform_features_kernel<K, false>, dim3(grid), dim3(256), 0, st, pdl, d, n, xyz, order, feat);
+        case K: return launch_k(d.times ? deform_features_kernel<K, true> : deform_features_kernel<K, false>, grid, 256, 0, st,   \
+                                pdl ? kPdl : kOrdinary, d, n, xyz, order, feat);
         G4D_GATHER_CASE(1) G4D_GATHER_CASE(2) G4D_GATHER_CASE(3) G4D_GATHER_CASE(4)
         G4D_GATHER_CASE(5) G4D_GATHER_CASE(6) G4D_GATHER_CASE(7) G4D_GATHER_CASE(8)
 #undef G4D_GATHER_CASE
@@ -592,15 +590,8 @@ static cudaError_t launch_deform_tc_t(const DeformDesc& d, const TcWeights& tw, 
     const size_t bytes = Ls.total;
     const int64_t ntiles = (n + 64 * NWG - 1) / (64 * NWG);
     const int grid = (int)(ntiles < sm_count ? ntiles : sm_count);
-    cudaError_t e;
-    if (tw.relu_bits) {
-        e = cudaFuncSetAttribute(deform_tc_kernel<NWG, MODE, C, L, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-        if (e != cudaSuccess) return e;
-        return launch_k(deform_tc_kernel<NWG, MODE, C, L, true>, dim3(grid), dim3(NWG * 128), bytes, st, true, d, tw, Ls, cam, n, io);
-    }
-    e = cudaFuncSetAttribute(deform_tc_kernel<NWG, MODE, C, L, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-    if (e != cudaSuccess) return e;
-    return launch_k(deform_tc_kernel<NWG, MODE, C, L, false>, dim3(grid), dim3(NWG * 128), bytes, st, true, d, tw, Ls, cam, n, io);
+    return launch_k(tw.relu_bits ? deform_tc_kernel<NWG, MODE, C, L, true> : deform_tc_kernel<NWG, MODE, C, L, false>, grid, NWG * 128,
+                    bytes, st, kPdl, d, tw, Ls, cam, n, io);
 }
 
 cudaError_t launch_deform_tc(const DeformDesc& d, const TcWeights& tw, int mode, const CameraDev* cam, int64_t n,

@@ -164,8 +164,7 @@ cudaError_t launch_tc_bwd_pack_weights(const G4DDeformParams& prm, uint8_t* blob
     }
     if (prm.head_mask & G4D_HEAD_SHS) out->w2sh = add(prm.w2[4], 48, 128, 1);
     p.start[m] = total; p.count = m;
-    bwd_pack_weights_kernel<<<(total + 255) / 256, 256, 0, st>>>(p);
-    return cudaGetLastError();
+    return launch_k(bwd_pack_weights_kernel, (total + 255) / 256, 256, 0, st, kOrdinary, p);
 }
 
 bool tc_backward_supported(const G4DDeformParams& prm) {
@@ -618,12 +617,9 @@ template <int C, int L>
 static cudaError_t launch_a(const BwdADesc& bd, int64_t n, int sm_count, cudaStream_t st) {
     const BwdSmemA Ls = bwd_smem_a(C * L, bd.d.head_mask & G4D_HEAD_SHS);
     const size_t bytes = Ls.total + 1024;
-    cudaError_t e = cudaFuncSetAttribute(deform_tc_bwd_dgrad_kernel<C, L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-    if (e != cudaSuccess) return e;
     const int64_t ntiles = (n + 127) / 128;
     const int grid = (int)(ntiles < sm_count ? ntiles : sm_count);
-    deform_tc_bwd_dgrad_kernel<C, L><<<grid, 256, bytes, st>>>(bd, Ls, n);
-    return cudaGetLastError();
+    return launch_k(deform_tc_bwd_dgrad_kernel<C, L>, grid, 256, bytes, st, kOrdinary, bd, Ls, n);
 }
 
 cudaError_t launch_tc_bwd_dgrad(const DeformDesc& d, const TcBwdWeights& w, int64_t n, const float* const go[G4D_NUM_HEADS],
@@ -662,10 +658,7 @@ cudaError_t launch_tc_bwd_wgrad(const DeformDesc& d, const G4DDeformGrads& grads
     b.g_w0 = grads.w0; b.g_b0 = grads.b0;
     for (int h = 0; h < G4D_NUM_HEADS; ++h) { b.g_w1[h] = grads.w1[h]; b.g_b1[h] = grads.b1[h]; b.g_w2[h] = grads.w2[h]; b.g_b2[h] = grads.b2[h]; }
     const size_t smem_b = (size_t)2 * kStage + kOnes + 1024;   // two half-tile stages + the all-ones operand
-    cudaError_t e = cudaFuncSetAttribute(deform_tc_bwd_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_b);
-    if (e != cudaSuccess) return e;
-    deform_tc_bwd_wgrad_kernel<<<b.nheads * b.chunks_head + b.chunks_l0, 256, smem_b, st>>>(b);
-    return cudaGetLastError();
+    return launch_k(deform_tc_bwd_wgrad_kernel, b.nheads * b.chunks_head + b.chunks_l0, 256, smem_b, st, kOrdinary, b);
 }
 
 }  // namespace g4d

@@ -38,8 +38,7 @@ __global__ void pack_camera_kernel(G4DCamera c, const float* d_time, CameraDev* 
 }
 
 cudaError_t launch_pack_camera(const G4DCamera& cam, const float* d_time, CameraDev* dst, cudaStream_t st) {
-    pack_camera_kernel<<<1, 32, 0, st>>>(cam, d_time, dst);
-    return cudaGetLastError();
+    return launch_k(pack_camera_kernel, 1, 32, 0, st, kOrdinary, cam, d_time, dst);
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -76,8 +75,7 @@ cudaError_t launch_pack_weights(const G4DDeformParams& prm, float* w0t, float* c
         p.src[m] = prm.wt[j - 1]; p.dst[m] = wtt[j - 1]; p.rows[m] = WD; p.cols[m] = WD; p.start[m] = total; total += WD * WD; ++m;
     }
     p.start[m] = total; p.count = m;
-    pack_weights_kernel<<<(total + 255) / 256, 256, 0, st>>>(p);
-    return cudaGetLastError();
+    return launch_k(pack_weights_kernel, (total + 255) / 256, 256, 0, st, kOrdinary, p);
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -103,7 +101,7 @@ cudaError_t launch_collapse_time_rows(const G4DDeformParams& p, TimeArg time, fl
     for (int l = 0; l < p.levels; ++l)
         for (int a = 0; a < 3; ++a) { s.src[l][a] = p.planes[l][kTimePlane[a]]; s.dst[l][a] = trow[l][a]; }
     const int total = (int)s.total();
-    return launch_k(collapse_time_rows_kernel, dim3((total + 255) / 256), dim3(256), 0, st, true, s, time);
+    return launch_k(collapse_time_rows_kernel, dim3((total + 255) / 256), dim3(256), 0, st, kPdl, s, time);
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -131,9 +129,8 @@ cudaError_t launch_preprocess(const CameraDev* cam, int64_t n, const RasterInput
                               cudaStream_t st) {
     if (n == 0) return cudaSuccess;
     const unsigned blocks = (unsigned)((n + 255) / 256);
-    if (in.sh.m == kShCoeffs) preprocess_kernel<true><<<blocks, 256, 0, st>>>(cam, n, in, g, out_radii);
-    else preprocess_kernel<false><<<blocks, 256, 0, st>>>(cam, n, in, g, out_radii);
-    return cudaGetLastError();
+    return launch_k(in.sh.m == kShCoeffs ? preprocess_kernel<true> : preprocess_kernel<false>, blocks, 256, 0, st, kOrdinary, cam, n,
+                    in, g, out_radii);
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -179,9 +176,7 @@ cudaError_t launch_project_cameras(const ExtraCameras& ec, int64_t n, const Rast
     constexpr int kThreads = 256;
     const size_t smem = (size_t)(kThreads / 32) * 32 * kShRow * sizeof(float);   // 49 KB: SH staging
     auto kernel = in.sh.m == kShCoeffs ? project_cameras_kernel<true> : project_cameras_kernel<false>;
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    return launch_k(kernel, dim3((unsigned)((n + kThreads - 1) / kThreads)), dim3(kThreads), smem, st, true, ec, n, in);
+    return launch_k(kernel, dim3((unsigned)((n + kThreads - 1) / kThreads)), dim3(kThreads), smem, st, kPdl, ec, n, in);
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -280,12 +275,9 @@ cudaError_t launch_deform_tc(const DeformDesc& d, const TcWeights& tw, int mode,
 template <int TG, int WD, int MODE>
 static cudaError_t launch_deform_t(const DeformDesc& d, const DeformSmem& L, size_t bytes, const CameraDev* cam, int64_t n,
                                    const float* feat, const DeformIO& io, int sm_count, cudaStream_t st) {
-    cudaError_t e = cudaFuncSetAttribute(deform_kernel<TG, WD, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-    if (e != cudaSuccess) return e;
     const int64_t ntiles = (n + TG - 1) / TG;
     const int grid = (int)(ntiles < sm_count ? ntiles : sm_count);
-    deform_kernel<TG, WD, MODE><<<grid, kDeformThreads, bytes, st>>>(d, L, cam, n, feat, io);
-    return cudaGetLastError();
+    return launch_k(deform_kernel<TG, WD, MODE>, grid, kDeformThreads, bytes, st, kOrdinary, d, L, cam, n, feat, io);
 }
 
 // The FFMA network runs tiles of TG Gaussians when their shared memory (dynamic and static) fits in an SM, and of TG / 2
@@ -352,9 +344,8 @@ __global__ void __launch_bounds__(256) activate_preprocess_kernel(const CameraDe
 cudaError_t launch_activate_preprocess(const CameraDev* cam, int64_t n, const DeformIO& io, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
     const unsigned blocks = (unsigned)((n + 255) / 256);
-    if (io.sh.m == kShCoeffs) activate_preprocess_kernel<true><<<blocks, 256, 0, st>>>(cam, n, io);
-    else activate_preprocess_kernel<false><<<blocks, 256, 0, st>>>(cam, n, io);
-    return cudaGetLastError();
+    return launch_k(io.sh.m == kShCoeffs ? activate_preprocess_kernel<true> : activate_preprocess_kernel<false>, blocks, 256, 0, st,
+                    kOrdinary, cam, n, io);
 }
 
 }  // namespace g4d

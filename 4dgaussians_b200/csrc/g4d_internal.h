@@ -286,7 +286,7 @@ cudaError_t launch_tc_bwd_dgrad(const DeformDesc& d, const TcBwdWeights& w, int6
 cudaError_t launch_tc_bwd_wgrad(const DeformDesc& d, const G4DDeformGrads& grads, int64_t n, uint8_t* images, int sm_count,
                                 cudaStream_t st);
 
-// ---- launchers (defined in g4d_geom.cu / g4d_raster.cu / g4d_backward.cu) -----------------------------
+// ---- launchers (defined in g4d_geom.cu / g4d_raster.cu / g4d_geom_bwd.cu / g4d_backward.cu) -------------
 // d_time: the camera's timestamp from device memory (NULL: cam.time)
 cudaError_t launch_pack_camera(const G4DCamera& cam, const float* d_time, CameraDev* dst, cudaStream_t st);
 cudaError_t launch_pack_weights(const G4DDeformParams& p, float* w0t, float* const* w1t, float* const* wtt, cudaStream_t st);

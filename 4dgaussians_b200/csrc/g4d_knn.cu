@@ -201,13 +201,14 @@ cudaError_t launch_knn_dist2(int64_t n, const float* xyz, float* out, void* scra
     if ((e = cudaMemcpyAsync(s.mm, init, sizeof(init), cudaMemcpyHostToDevice, st)) != cudaSuccess) return e;
     if ((e = cudaMemsetAsync(s.cnt, 0, kCells * 4, st)) != cudaSuccess) return e;
     int blocks = (int)((n + 255) / 256);
-    knn_bbox_kernel<<<blocks < sm_count * 8 ? blocks : sm_count * 8, 256, 0, st>>>(xyz, n, s.mm);
-    knn_setup_kernel<<<1, 1, 0, st>>>(s.mm, n, s.grid);
-    knn_count_kernel<<<blocks, 256, 0, st>>>(xyz, s.grid, s.cnt, s.cell_of);
-    knn_scan_kernel<<<1, 1024, 0, st>>>(s.grid, s.cnt, s.start);
-    knn_scatter_kernel<<<blocks, 256, 0, st>>>(s.grid, s.cell_of, s.start, s.cnt, s.sorted);
-    knn_search_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(xyz, s.grid, s.start, s.sorted, out);
-    return cudaGetLastError();
+    if ((e = launch_k(knn_bbox_kernel, blocks < sm_count * 8 ? blocks : sm_count * 8, 256, 0, st, kOrdinary, xyz, n, s.mm)) != cudaSuccess)
+        return e;
+    if ((e = launch_k(knn_setup_kernel, 1, 1, 0, st, kOrdinary, s.mm, n, s.grid)) != cudaSuccess) return e;
+    if ((e = launch_k(knn_count_kernel, blocks, 256, 0, st, kOrdinary, xyz, s.grid, s.cnt, s.cell_of)) != cudaSuccess) return e;
+    if ((e = launch_k(knn_scan_kernel, 1, 1024, 0, st, kOrdinary, s.grid, s.cnt, s.start)) != cudaSuccess) return e;
+    if ((e = launch_k(knn_scatter_kernel, blocks, 256, 0, st, kOrdinary, s.grid, s.cell_of, s.start, s.cnt, s.sorted)) != cudaSuccess)
+        return e;
+    return launch_k(knn_search_kernel, (unsigned)((n + 127) / 128), 128, 0, st, kOrdinary, xyz, s.grid, s.start, s.sorted, out);
 }
 
 }  // namespace g4d

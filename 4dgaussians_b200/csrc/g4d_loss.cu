@@ -227,19 +227,15 @@ int grid_for(int64_t work, int sm_count) {
 cudaError_t launch_l1_loss(const float* a, const float* b, int64_t n, float scale, float* loss, int sm_count, cudaStream_t st) {
     if (n <= 0) return cudaSuccess;
     if (aligned16(a) && aligned16(b))
-        l1_loss_kernel<true><<<grid_for(n / 4, sm_count), 256, 0, st>>>(a, b, n, scale, loss);
-    else
-        l1_loss_kernel<false><<<grid_for(n, sm_count), 256, 0, st>>>(a, b, n, scale, loss);
-    return cudaGetLastError();
+        return launch_k(l1_loss_kernel<true>, grid_for(n / 4, sm_count), 256, 0, st, kOrdinary, a, b, n, scale, loss);
+    return launch_k(l1_loss_kernel<false>, grid_for(n, sm_count), 256, 0, st, kOrdinary, a, b, n, scale, loss);
 }
 cudaError_t launch_l1_grad(const float* a, const float* b, int64_t n, float scale, const float* upstream, float* grad, int sm_count,
                            cudaStream_t st) {
     if (n <= 0) return cudaSuccess;
     if (aligned16(a) && aligned16(b) && aligned16(grad))
-        l1_grad_kernel<true><<<grid_for(n / 4, sm_count), 256, 0, st>>>(a, b, n, scale, upstream, grad);
-    else
-        l1_grad_kernel<false><<<grid_for(n, sm_count), 256, 0, st>>>(a, b, n, scale, upstream, grad);
-    return cudaGetLastError();
+        return launch_k(l1_grad_kernel<true>, grid_for(n / 4, sm_count), 256, 0, st, kOrdinary, a, b, n, scale, upstream, grad);
+    return launch_k(l1_grad_kernel<false>, grid_for(n, sm_count), 256, 0, st, kOrdinary, a, b, n, scale, upstream, grad);
 }
 
 cudaError_t launch_plane_regulation(const G4DDeformParams& prm, const G4DDeformGrads* grads, float w_plane_tv, float w_time_smooth,
@@ -260,23 +256,22 @@ cudaError_t launch_plane_regulation(const G4DDeformParams& prm, const G4DDeformG
         }
     d.total = total;
     if (total == 0) return cudaSuccess;
-    plane_regulation_kernel<<<grid_for(total, sm_count), 256, 0, st>>>(d, loss, upstream);
-    return cudaGetLastError();
+    return launch_k(plane_regulation_kernel, grid_for(total, sm_count), 256, 0, st, kOrdinary, d, loss, upstream);
 }
 
 cudaError_t launch_ssim_forward(const float* x, const float* y, int C, int H, int W, float scale, float* loss, float* dmu, float* dxx,
                                 float* dxy, cudaStream_t st) {
     if ((int64_t)C * H * W == 0) return cudaSuccess;
     const dim3 grid((W + kSsimT - 1) / kSsimT, (H + kSsimT - 1) / kSsimT, C);
-    ssim_forward_kernel<<<grid, kSsimT * kSsimT, 0, st>>>(make_ssim_window(), x, y, H, W, scale, loss, dmu, dxx, dxy);
-    return cudaGetLastError();
+    return launch_k(ssim_forward_kernel, grid, kSsimT * kSsimT, 0, st, kOrdinary, make_ssim_window(), x, y, H, W, scale, loss, dmu,
+                    dxx, dxy);
 }
 cudaError_t launch_ssim_backward(const float* x, const float* y, int C, int H, int W, float scale, const float* upstream,
                                  const float* dmu, const float* dxx, const float* dxy, float* grad, cudaStream_t st) {
     if ((int64_t)C * H * W == 0) return cudaSuccess;
     const dim3 grid((W + kSsimT - 1) / kSsimT, (H + kSsimT - 1) / kSsimT, C);
-    ssim_backward_kernel<<<grid, kSsimT * kSsimT, 0, st>>>(make_ssim_window(), x, y, H, W, scale, upstream, dmu, dxx, dxy, grad);
-    return cudaGetLastError();
+    return launch_k(ssim_backward_kernel, grid, kSsimT * kSsimT, 0, st, kOrdinary, make_ssim_window(), x, y, H, W, scale, upstream,
+                    dmu, dxx, dxy, grad);
 }
 
 }  // namespace g4d

@@ -56,9 +56,8 @@ cudaError_t launch_adam(float* p, const float* g, float* m, float* v, int64_t nu
     const int64_t n4 = numel / 4;
     int64_t blocks = (n4 + 255) / 256;
     if (blocks > (int64_t)sm_count * 16) blocks = (int64_t)sm_count * 16;
-    adam_flat_kernel<kDevice><<<(unsigned)blocks, 256, 0, st>>>(p, g, m, v, n4, s, b1, b2, eps, hs.inv_bc1, hs.inv_sqrt_bc2,
-                                                                hs.grad_scale, ds);
-    return cudaGetLastError();
+    return launch_k(adam_flat_kernel<kDevice>, (unsigned)blocks, 256, 0, st, kOrdinary, p, g, m, v, n4, s, b1, b2, eps, hs.inv_bc1,
+                    hs.inv_sqrt_bc2, hs.grad_scale, ds);
 }
 }  // namespace
 

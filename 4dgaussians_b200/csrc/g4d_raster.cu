@@ -131,7 +131,7 @@ blend_forward_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, const uin
 cudaError_t launch_blend_forward(const CameraDev* cam, int grid_x, int grid_y, GeomBuffers g, BinBuffers b, ImageBuffers im,
                                  float* out_color, float* out_depth, int warp_cull, float* out_alpha, cudaStream_t st) {
     if (grid_x * grid_y == 0) return cudaSuccess;
-    return launch_k(blend_forward_kernel, dim3(grid_x, grid_y), dim3(kTilePixels / 2), 0, st, true, cam, g, b.ids_sorted, b.ranges,
+    return launch_k(blend_forward_kernel, dim3(grid_x, grid_y), dim3(kTilePixels / 2), 0, st, kPdl, cam, g, b.ids_sorted, b.ranges,
                     im.final_T, im.n_contrib, out_color, out_depth, warp_cull, out_alpha);
 }
 
@@ -139,12 +139,6 @@ cudaError_t launch_blend_forward(const CameraDev* cam, int grid_x, int grid_y, G
 // A.4 blend backward: same tiling, instances traversed back to front.  Per instance the 9 partial gradients
 // of a warp's 32 pixels are reduced with shuffles (only when some lane contributes) and lane 0 issues the
 // atomics, so global RED traffic is <= 8 x 9 per (tile, instance) instead of 256 x 9.
-G4D_D float warp_sum(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
 // the colour b of a staged rec2 entry: the colour-only instance stages (b), the depth instance (b, depth)
 G4D_D float staged_b(float v) { return v; }
 G4D_D float staged_b(float2 v) { return v.x; }
@@ -338,14 +332,14 @@ blend_backward_kernel(const CameraDev* __restrict__ cam, GeomBuffers g, const ui
                 float x = (hi4 ? x2[1] : x2[0]) + __shfl_xor_sync(0xffffffffu, hi4 ? x2[0] : x2[1], 4);
                 x += __shfl_xor_sync(0xffffffffu, x, 2);
                 x += __shfl_xor_sync(0xffffffffu, x, 1);
-                v_op = warp_sum(v_op);
+                v_op = warp_sum_f(v_op);
                 if (red_lane) {
                     const uint32_t id = sid[j];
                     atomicAdd(red_base + red_stride * id, lane == 1 ? v_op : x);
                 }
                 if constexpr (DEPTH) {     // the tenth value: dL/dz of the instance, added by lane 2
                     const float2 pz = f2_mul(w, dpD);
-                    const float v_z = warp_sum(pz.x + pz.y);
+                    const float v_z = warp_sum_f(pz.x + pz.y);
                     if (lane == 2) atomicAdd(g_depth + sid[j], v_z);
                 }
             }
@@ -358,11 +352,9 @@ cudaError_t launch_blend_backward(const CameraDev* cam, int grid_x, int grid_y, 
                                   int warp_cull, const float* dL_ddepth, float* g_depth, const float* dL_dalpha,
                                   cudaStream_t st) {
     if (grid_x * grid_y == 0) return cudaSuccess;
-    auto kernel = dL_ddepth ? blend_backward_kernel<true> : blend_backward_kernel<false>;
-    kernel<<<dim3(grid_x, grid_y), kTilePixels / 2, 0, st>>>(cam, g, b.ids_sorted, b.ranges, im.final_T, im.n_contrib, dL_dcolor,
-                                                             g_mean2D, g_conic, g_opacity, g_rgb, warp_cull, dL_ddepth, g_depth,
-                                                             dL_dalpha);
-    return cudaGetLastError();
+    return launch_k(dL_ddepth ? blend_backward_kernel<true> : blend_backward_kernel<false>, dim3(grid_x, grid_y), kTilePixels / 2, 0,
+                    st, kOrdinary, cam, g, b.ids_sorted, b.ranges, im.final_T, im.n_contrib, dL_dcolor, g_mean2D, g_conic, g_opacity,
+                    g_rgb, warp_cull, dL_ddepth, g_depth, dL_dalpha);
 }
 
 }  // namespace g4d
